@@ -6,16 +6,21 @@ iterations (minIterations = maxIterations = ITERS, so no instance stops early) o
 FK sweep -> residual/Jacobian -> JtJ/Jtr -> damped Cholesky -> update.
 
 Default workload "cfg3-shard": the per-GPU shard of BASELINE.json configs[2] — the configuration the
-metric/target is quoted on ("72-joint / 128-residual batch at 8xB200") — 8192 x humanoid72 with 24
+metric/target is quoted on ("72-joint / 128-residual batch at 8 GPUs") — 8192 x humanoid72 with 24
 Position + 6 Orientation constraints (m = 126 -> 128 rows, n = 220), constant damping 0.05, weak
 scaling (8 GPUs = 65536 instances = cfg3 exactly). ``--workload cfg2`` / ``cfg4`` select the other
 single-GPU configs.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (solved parameters, per-instance error, iteration
+count and status) as DIR/<name>.npy, at most 64 MB (beyond that a fixed seeded sample of instances); the inputs are seeded, so two
+builds run with the same arguments can be compared output for output.
 
     value   : whole-job GN iterations/s with parameters and targets resident in HBM
     e2e     : same metric through mb2_solver_solve with HOST (pinned) buffers: H2D of targets and initial
               parameters and D2H of solved parameters + per-instance results inside the timed region
     roofline: the JtJ kernel (the kernel BASELINE's metric names), algorithmic m*n*(n+1) FLOP per
-              instance-iteration over its CUDA-event time, against the measured tensor peak
+              instance-iteration over its CUDA-event time, against the tensor peak (MEASURED_PEAKS.json if present, else the
+              H100 SXM data sheet)
     cpu_baseline / --impl reference: the oracle restatement of the reference's CPU solver (one solver per
               instance over all host threads, as tensor_ik.cpp:127), bounded sample
 """
@@ -55,23 +60,14 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm_gbs=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
-
-
-def measured_traffic(workload, batch):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full captures (profiles/ncu_traffic.json);
-    only valid for the exact workload / batch they were captured on."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if not os.path.exists(p):
-        return {}
-    d = json.load(open(p))
-    return d.get(f"{workload}:{batch}", {}).get("dram_bytes_per_launch", {})
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16; never reached, a card at a lower power limit gets less
+    return dict(hbm_gbs=3350.0, bf16=989.0, bf16_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """SM clock / clock-event reasons sampled DURING the timed regions (B200_PROFILING.md recipe). NVML is polled in-process
-    (the timed regions of the default run are ~45 ms each, shorter than one nvidia-smi start-up) every 25 ms; the two queries take
-    microseconds (scripts/nvml_cost.py: median 3 us), --clock-poll-ms changes the period."""
+    """SM clock / clock-event reasons sampled DURING the timed regions. NVML is polled in-process (a timed region of the default
+    run is shorter than one nvidia-smi start-up) every 25 ms; the two queries take microseconds (scripts/nvml_cost.py measures
+    them), --clock-poll-ms changes the period."""
 
     REASONS = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap", 0x80: "hw_power_brake_slowdown"}
 
@@ -182,9 +178,49 @@ def run_reference(args, rank, world):
     print(json.dumps(line))
 
 
-def measure_workload(ms, torch, workload, B, rank, local_rank, args, steps, warmup, min_it=ITERS, max_it=ITERS, e2e=True, profile=True, flush=None, barrier=None):
+DUMP_LIMIT_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(directory, per_instance, rank, world, extra=None):
+    """Writes the outputs of a timed step as <directory>/<name>.npy (float32 stays float32, everything else becomes float64).
+    per_instance: name -> array indexed by instance, or a list of per-instance arrays (mixed rigs: written flat, with <name>_offsets).
+    When they exceed DUMP_LIMIT_BYTES in all, a fixed seeded sample of instances is written and its indices go to sample_index.npy.
+    extra: small arrays written as they are. One file set per rank."""
+    def conv(a):
+        a = np.asarray(a)
+        return a.astype(np.float32 if a.dtype == np.float32 else np.float64)
+
+    per_instance = {k: [conv(x) for x in v] if isinstance(v, list) else conv(v) for k, v in per_instance.items()}
+    extra = {k: conv(v) for k, v in (extra or {}).items()}
+    B = len(next(iter(per_instance.values())))
+    row_bytes = np.zeros(B)
+    for v in per_instance.values():
+        row_bytes += [x.nbytes for x in v] if isinstance(v, list) else v.nbytes / max(B, 1)
+    budget = DUMP_LIMIT_BYTES - sum(v.nbytes for v in extra.values()) - 8 * B  # room for the sample indices
+    index = None
+    if row_bytes.sum() > budget:
+        order = np.random.default_rng(20240607).permutation(B)  # fixed: the same sample in every run and every build
+        k = int(np.searchsorted(np.cumsum(row_bytes[order]), budget, side="right"))
+        index = np.sort(order[:k])
+        per_instance = {n: [v[i] for i in index] if isinstance(v, list) else v[index] for n, v in per_instance.items()}
+        extra["sample_index"] = index.astype(np.float64)
+    out = dict(extra)
+    for n, v in per_instance.items():
+        if isinstance(v, list):
+            out[n] = np.concatenate(v) if v else np.zeros(0, np.float32)
+            out[n + "_offsets"] = np.cumsum([0] + [len(x) for x in v]).astype(np.float64)
+        else:
+            out[n] = v
+    os.makedirs(directory, exist_ok=True)
+    for n, a in out.items():
+        np.save(os.path.join(directory, (f"{n}_rank{rank}" if world > 1 else n) + ".npy"), a)
+
+
+def measure_workload(ms, torch, workload, B, rank, local_rank, args, steps, warmup, min_it=ITERS, max_it=ITERS, e2e=True, profile=True, flush=None, barrier=None,
+                     dump_dir=None, world=1):
     """Device-resident timing (CUDA events on the launching stream, L2 flushed between steps), the end-to-end leg through mb2_set_targets +
-    mb2_solver_solve with pinned host buffers, and one profiling solve (events around every launch + in-kernel phase cycles)."""
+    mb2_solver_solve with pinned host buffers, and one profiling solve (events around every launch + in-kernel phase cycles).
+    dump_dir: write the last timed step's outputs there (dump_outputs)."""
     ch, efs, theta0, _ = make_problem(workload, B, seed_offset=1000 * rank)  # each rank owns a different shard
     n = ch.num_params
     fn = ms.SkeletonSolverFunction(ch, B, efs, device=local_rank)
@@ -215,6 +251,8 @@ def measure_workload(ms, torch, workload, B, rank, local_rank, args, steps, warm
         total_ms += ev0.elapsed_time(ev1)
     barrier()
     res = solver.get_results()
+    if dump_dir:
+        dump_outputs(dump_dir, {"params": theta_dev.cpu().numpy(), "errors": res["errors"], "iterations": res["iterations"], "status": res["status"]}, rank, world)
     out = {"ch": ch, "efs": efs, "n": n, "B": B, "solver": solver, "fn": fn, "total_ms": total_ms, "its_per_step": int(res["iterations"].sum()),
            "err_sum": float(res["errors"].sum()), "launches": solver.get_counters()[1], "status_bad": int((res["status"] != 0).sum())}
     if profile:
@@ -232,10 +270,9 @@ def measure_workload(ms, torch, workload, B, rank, local_rank, args, steps, warm
     if e2e:
         theta0_pin = torch.from_numpy(theta0.astype(np.float32)).pin_memory()
         # Two long-lived pinned staging buffers used alternately, as a streaming caller keeps them: mb2_solver_solve uploads the buffer's
-        # parameters, solves in place and downloads the result into the same buffer. (Measured alternatives: a FRESH pinned buffer per step
-        # makes the 7.2 MB transfers 0.7 - 1.1 ms slower - the DMA path is slow on host pages it has not seen recently: 9.3 - 9.8 instead of
-        # 8.66 ms per step; refilling the idle buffer from the host while the device works costs more than it hides - the host memcpy fights
-        # the D2H for memory bandwidth and torch's copy threads stall for tens of ms now and then.) From its second use on a buffer holds the
+        # parameters, solves in place and downloads the result into the same buffer, so the host pages the DMA touches stay the same
+        # from step to step; refilling the idle buffer from the host while the device works would make the host memcpy compete with
+        # the D2H for memory bandwidth. From its second use on a buffer holds the
         # previous result of that buffer: with minIterations = maxIterations the work of a step does not depend on the starting point.
         theta_pins = [theta0_pin.clone().pin_memory() for _ in range(2)]
         target_pins = [torch.from_numpy(np.ascontiguousarray(e.targets, np.float32)).pin_memory() for e in efs]
@@ -248,7 +285,7 @@ def measure_workload(ms, torch, workload, B, rank, local_rank, args, steps, warm
                 fn._check(fn._L.mb2_set_targets(fn._h, idx, ms.C.cast(tp.data_ptr(), ms._fp)))
             return solver.solve_host_pointer(buf.data_ptr(), results=True)  # mb2_solver_solve: parameters in / out + per-instance results
 
-        for _ in range(max(2, warmup // 2)):  # (the first call allocates the staging buffers: 20 - 30 ms)
+        for _ in range(max(2, warmup // 2)):  # (the first call allocates the staging buffers)
             e2e_step()
         barrier()
         step_s = []
@@ -269,19 +306,18 @@ def kernel_report(m, peaks, workload):
     """Per-kernel roofline entries from the profiling solve. ALGORITHMIC bytes / flops per instance and launch (DESIGN.md section 4)."""
     solver, n, B, efs = m["solver"], m["n"], m["B"], m["efs"]
     st = solver.get_plan_stats()
-    tf32_peak = 0.5 * peaks["bf16"]  # TF32 dense = half the bf16 rate (B200_PROFILING.md table); bf16 figure is the measured cuBLAS burst
+    tf32_peak = 0.5 * peaks["bf16"]  # TF32 dense = half the bf16 rate (H100 data sheet: 495 vs 989 TFLOP/s)
     hbm_peak = peaks["hbm_gbs"]
     pm, pl = m["phase_ms"], m["phase_launches"]
     sweep_ms = pm[0] / max(1, pl[0]); jtj_ms = pm[1] / max(1, pl[1]); chol_ms = pm[2] / max(1, pl[2])
     m_rows = WORKLOADS[workload]["rows_m"]
     target_floats = sum(int(np.prod(np.asarray(e.targets).shape[1:])) for e in efs)
-    traffic = measured_traffic(workload, B)
     jtj_flops = float(m_rows) * n * (n + 1)  # SURVEY 8(d): the JtJ credit, whatever the kernel executes
 
     def hbm_entry(name, key, bytes_per_instance, ms_):
         ach = bytes_per_instance * B / (ms_ * 1e-3) / 1e9 if ms_ > 0 else 0.0
         return {"kernel": name, "bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "peak_source": f"{peaks['src']} copy bandwidth",
-                "traffic": traffic.get(key), "ms_per_launch": ms_, "algorithmic_bytes_per_instance": bytes_per_instance}
+                "ms_per_launch": ms_, "algorithmic_bytes_per_instance": bytes_per_instance}
 
     k1_bytes = 4.0 * (n + target_floats + st["jacobian_nonzeros"] + m_rows) + 8.0
     kernels = [hbm_entry("sweepKernel<true> (three-pass FK + residual + Jacobian strips)", "fk_residual_jacobian", k1_bytes, sweep_ms)]
@@ -291,10 +327,10 @@ def kernel_report(m, peaks, workload):
     jtj_phase = None
     if fused["fused"] == 2:  # Gram + Cholesky in one launch: strips in, theta / delta / bookkeeping out; tiles never leave the SM
         gc_bytes = 4.0 * (st["strip_floats"] + 4 * st["normal_parameters"]) + 32.0
-        e = hbm_entry("gramCholeskyKernel (tile-sparse J^T J on mma.sync 3xTF32 -> TMEM -> tiles in shared memory -> tile Cholesky + update)", "gram_cholesky", gc_bytes, chol_ms)
+        e = hbm_entry("gramCholeskyKernel (tile-sparse J^T J on mma.sync 3xTF32 -> tiles in shared memory -> tile Cholesky + update)", "gram_cholesky", gc_bytes, chol_ms)
         cyc = fused["phase_cycles"]
         tot = float(sum(cyc.values())) or 1.0
-        share = (cyc["gram"] + cyc["tiles_from_tmem"]) / tot
+        share = (cyc["gram"] + cyc["parked_tiles"]) / tot
         gram_ms = chol_ms * share
         jtj_phase = {"where": "Gram phase of gramCholeskyKernel (in-kernel cycle share x the kernel's event time)", "share_of_kernel": share, "ms": gram_ms}
         e["phase_cycle_shares"] = {k: v / tot for k, v in cyc.items() if v}
@@ -310,8 +346,8 @@ def kernel_report(m, peaks, workload):
         k2_bytes = 4.0 * (m_rows * (st["jacobian_columns"] + 1) + (st["normal_parameters"] + 1) * (st["normal_parameters"] + 2) / 2)
         ach = jtj_flops * B / (jtj_ms * 1e-3) / 1e12 if jtj_ms > 0 else 0.0
         dense = st["jacobian_columns"] + 1 <= 512
-        kernels.append({"kernel": "jtjTensorKernel (JtJ/Jtr, tcgen05 3xTF32)" if dense else "jtjSimtKernel", "bound": "tensor", "achieved": ach, "peak": tf32_peak, "unit": "TFLOP/s",
-                        "frac": ach / tf32_peak, "peak_source": f"0.5 x {peaks['src']} bf16 cuBLAS burst ({peaks['bf16']} TF/s) = TF32 dense", "traffic": traffic.get("jtj_jtr"),
+        kernels.append({"kernel": "jtjTensorKernel (JtJ/Jtr, wgmma 3xTF32)" if dense else "jtjSimtKernel", "bound": "tensor", "achieved": ach, "peak": tf32_peak, "unit": "TFLOP/s",
+                        "frac": ach / tf32_peak, "peak_source": f"0.5 x {peaks['src']} bf16 ({peaks['bf16']} TF/s) = TF32 dense",
                         "ms_per_launch": jtj_ms, "algorithmic_flops_per_instance": jtj_flops, "algorithmic_bytes_per_instance": k2_bytes})
         k3_entries = ntiles * 256 if ntiles else st["normal_parameters"] * (st["normal_parameters"] + 1) / 2
         kernels.append(hbm_entry("choleskyScheduledKernel (damped LLT + solves + update)" if ntiles else "choleskyKernel (dense LLT + solves + update)", "cholesky_update",
@@ -324,7 +360,7 @@ def kernel_report(m, peaks, workload):
                           "executed_flops_per_instance": gram_flops, "executed_tflops": executed, "executed_frac_of_tf32_peak": executed / tf32_peak,
                           "credited_tflops_end_to_end": jtj_flops * B / (step_ms * 1e-3) / 1e12 if step_ms > 0 else 0.0,
                           "tf32_peak": tf32_peak, "note": "credit = m n (n + 1) per instance-iteration (SURVEY 8d); executed = the multiply-adds of the non-zero 4x16 strips only; "
-                                                         "mma.sync (HMMA) path, not tcgen05: see profiles/sass_r02.txt"})
+                                                         "mma.sync (HMMA) path: the 4-row strips are too narrow for wgmma"})
     return kernels, jtj_phase, {"fk_residual_jacobian": sweep_ms, "jtj_jtr": jtj_ms, "cholesky_update": chol_ms}, st
 
 
@@ -369,8 +405,9 @@ def extra_workloads(ms, torch, args, rank, local_rank, flush, barrier, peaks):
     return ex
 
 
-def measure_mixed(ms, torch, args, local_rank, N, rank, steps=2):
-    """cfg5 per-GPU shard through mb2_mixed_batch_solve: host buffers in, host buffers out (an end-to-end figure by construction)."""
+def measure_mixed(ms, torch, args, local_rank, N, rank, steps=2, dump_dir=None, world=1):
+    """cfg5 per-GPU shard through mb2_mixed_batch_solve: host buffers in, host buffers out (an end-to-end figure by construction).
+    dump_dir: write the last timed solve's outputs there (dump_outputs)."""
     from momentum_b200.problems import mixed_problem
 
     rigs, inst = mixed_problem(N, seed=12351 + 1000 * rank)
@@ -392,6 +429,8 @@ def measure_mixed(ms, torch, args, local_rank, N, rank, steps=2):
         for i, x in enumerate(inst):
             mb.set_parameters(i, x["theta0"])
     dt = time.perf_counter() - t0
+    if dump_dir:
+        dump_outputs(dump_dir, {"params": out["params"], "errors": out["errors"], "iterations": out["iterations"], "status": out["status"]}, rank, world)
     per_rig = {}
     for b in range(st["buckets"]):
         info = mb.bucket_info(b)
@@ -404,7 +443,8 @@ def measure_mixed(ms, torch, args, local_rank, N, rank, steps=2):
 
 def measure_sharded(ms, torch, args, B):
     """Single-process multi-GPU (mb2_sharded_solver_*, ik_sharded.cpp): B instances per device, one host thread per shard, host buffers in
-    and out (pinned), aggregate on the host. Wall clock around mb2_sharded_solver_solve."""
+    and out (pinned), aggregate on the host. Wall clock around mb2_sharded_solver_solve. --dump-outputs: the solved parameters of the
+    last timed step (its buffer) and the aggregate."""
     N = args.sharded
     ch, efs, theta0, _ = make_problem(args.workload, B * N)
     proto = ms.SkeletonSolverFunction(ch, 1, efs, device=0)  # the definition only: targets go to the shards
@@ -422,6 +462,9 @@ def measure_sharded(ms, torch, args, B):
         step_ms.append(round(1e3 * (time.perf_counter() - t1), 3))
     dt = time.perf_counter() - t0
     agg = sh.get_aggregate()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"params": pins[(args.steps - 1) % 2].numpy()}, 0, 1,
+                     extra={"aggregate": [agg["error_sum"], agg["iterations"], agg["instances_ok"]]})
     value = agg["iterations"] * args.steps / dt
     return {"metric": "GN iterations/sec (batched 72-joint IK)", "value": value, "unit": "GN it/s", "n_gpus": N, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": 1e3 * dt / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
@@ -446,6 +489,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--clock-poll-ms", type=float, default=25.0, help="NVML clock / throttle-reason sampling period during the timed regions")
     ap.add_argument("--no-extras", action="store_true", help="skip the other workloads measured in the same run (cfg2, cfg4, cfg5, convergence mode)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (params, errors, iterations, status; --sharded: params and the aggregate) as "
+                         "DIR/<name>.npy, at most 64 MB (a fixed seeded sample of instances beyond that)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -459,7 +505,7 @@ def main():
 
     from momentum_b200 import solver as ms
 
-    assert torch.cuda.is_available(), "bench.py needs a B200 (no CPU fallback)"
+    assert torch.cuda.is_available(), "bench.py needs an H100 (no CPU fallback)"
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
@@ -469,7 +515,7 @@ def main():
     B = args.batch_per_gpu or WORKLOADS[args.workload]["batch"]
     work_stream = torch.cuda.Stream()  # a real (non-NULL) stream: NULL means "the handle's own stream" in the C-ABI
     torch.cuda.set_stream(work_stream)
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")  # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -482,7 +528,7 @@ def main():
         print(json.dumps(measure_sharded(ms, torch, args, B)))
         return
     if args.workload == "cfg5":
-        r = measure_mixed(ms, torch, args, local_rank, B, rank, steps=args.steps)
+        r = measure_mixed(ms, torch, args, local_rank, B, rank, steps=args.steps, dump_dir=args.dump_outputs, world=world)
         from momentum_b200.distributed import aggregate_solve_stats
 
         its_total, _, _ = aggregate_solve_stats(float(r["value"]), 0.0, 0.0, device="cuda")
@@ -497,7 +543,8 @@ def main():
 
     sampler = ClockSampler(local_rank, args.clock_poll_ms * 1e-3)
     sampler.start()
-    m = measure_workload(ms, torch, args.workload, B, rank, local_rank, args, args.steps, args.warmup, flush=flush, barrier=barrier)
+    m = measure_workload(ms, torch, args.workload, B, rank, local_rank, args, args.steps, args.warmup, flush=flush, barrier=barrier,
+                         dump_dir=args.dump_outputs, world=world)
     clocks = sampler.stop()  # sampled across the device-resident and the end-to-end timed regions
     # the one collective of the path: aggregate iterations / residual norm (SUM) and elapsed device time (MAX over ranks)
     from momentum_b200.distributed import aggregate_solve_stats

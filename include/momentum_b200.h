@@ -1,5 +1,5 @@
 /*
- * momentum_b200 — C-ABI of the B200-native batched Gauss-Newton IK path.
+ * momentum_b200 — C-ABI of the H100-native (sm_90a) batched Gauss-Newton IK path.
  *
  * This is the drop-in boundary for ONE hot path of facebookresearch/momentum: the per-iteration
  * FK sweep -> residual/Jacobian (Position / Orientation / State / Limit) -> JtJ, Jtr -> damped
@@ -19,7 +19,7 @@
  *    thread, tensor_ik.cpp:127-162; mutable scratch in skeleton_solver_function.h:89).
  *  - quaternions are (x, y, z, w) like Eigen::Quaternion::coeffs().
  *  - batched arrays are instance-major: [B][...].
- *  - there is no CPU fallback: every compute entry point fails with MB2_ERR_CUDA when no sm_100
+ *  - there is no CPU fallback: every compute entry point fails with MB2_ERR_CUDA when no sm_90
  *    device is usable.
  */
 #ifndef MOMENTUM_B200_H_
@@ -84,10 +84,10 @@ typedef enum mb2_rotation_error_type {
 
 /* How JtJ is formed on the device (extension; the reference always uses Eigen fp32/fp64 GEMM). */
 typedef enum mb2_jtj_mode {
-  MB2_JTJ_AUTO = 0,      /* tile-sparse Gram (mma.sync, three-term TF32 split: fp32-class, not bit-exact fp32) with the tile-scheduled Cholesky; else tcgen05 3xTF32 where the shape allows, else FP32 SIMT */
+  MB2_JTJ_AUTO = 0,      /* tile-sparse Gram (mma.sync, three-term TF32 split: fp32-class, not bit-exact fp32) with the tile-scheduled Cholesky; else wgmma 3xTF32 where the shape allows, else FP32 SIMT */
   MB2_JTJ_FP32_SIMT = 1, /* CUDA-core fp32 (validation path) */
-  MB2_JTJ_TF32X3 = 2,    /* tcgen05 kind::tf32, 3-term split, fp32 accumulate in TMEM (fp32-class accuracy); up to 511 Jacobian columns */
-  MB2_JTJ_TF32 = 3,      /* tcgen05 kind::tf32 single pass (~1e-3 relative; changes the GN path, not the fixed point) */
+  MB2_JTJ_TF32X3 = 2,    /* wgmma tf32, 3-term split, fp32 accumulate in registers (fp32-class accuracy); up to 511 Jacobian columns */
+  MB2_JTJ_TF32 = 3,      /* wgmma tf32 single pass (~1e-3 relative; changes the GN path, not the fixed point) */
   MB2_JTJ_SPARSE_TILES = 4 /* tensor cores (mma.sync m16n8k8, hi*hi + hi*lo + lo*hi TF32 split, the lo*lo term is dropped: ~2^-21 relative) over the non-zero
                               strips of J only, straight into the Cholesky tile layout (tile-scheduled Cholesky only) */
 } mb2_jtj_mode;
@@ -107,14 +107,13 @@ typedef enum mb2_cholesky_mode {
 /* Which kernels run one Gauss-Newton iteration on the tile path (extension; every mode solves the same system with the same device
  * functions, results agree to float rounding).
  *   GRAM_CHOLESKY  two launches per iteration: FK / residual / Jacobian strips, then ONE kernel that forms the stored tiles of
- *                  J^T J + lambda I from the strips on the tensor cores, parks them in TMEM, writes them over the dead strips in shared
- *                  memory and runs the tile Cholesky + update on them: the normal equations never exist in HBM.
+ *                  J^T J + lambda I from the strips on the tensor cores (a tile that would overwrite strips still being read waits in
+ *                  thread-local memory), writes them over the dead strips in shared memory and runs the tile Cholesky + update on them.
  *   OFF            three launches per iteration (sweep, tile-sparse Gram to HBM, tile Cholesky).
  *   PERSISTENT     ONE launch per solve: groups of 256 threads keep an instance in shared memory for all of its iterations (FK sweep
  *                  included) and stop it on the device; no host round trip, no HBM traffic beyond theta / targets / results. Needs no
- *                  line search and a plan whose tiles fit in shared memory next to the staged tables. Measured slower than GRAM_CHOLESKY
- *                  at thousands of instances (three instances per SM cannot hide the sweep's dependent chains; profiles/), so AUTO does
- *                  not pick it. */
+ *                  line search and a plan whose tiles fit in shared memory next to the staged tables. At most three instances per SM
+ *                  are in flight, so AUTO takes it only for a batch of one wave of instance groups. */
 typedef enum mb2_fused_mode {
   MB2_FUSED_AUTO = 0,          /* PERSISTENT when the batch is a single wave of instance groups (<= 3 per SM), else GRAM_CHOLESKY when strips / tiles fit in
                                   shared memory, else OFF */
@@ -161,7 +160,7 @@ typedef struct mb2_solver_function mb2_solver_function; /* batch of B SkeletonSo
 typedef struct mb2_solver mb2_solver;                   /* batch of B GaussNewtonSolverT<float> */
 
 const char* mb2_last_error(void);
-/* number of usable sm_100 devices (0 => every compute call fails with MB2_ERR_CUDA) */
+/* number of usable sm_90 devices (0 => every compute call fails with MB2_ERR_CUDA) */
 int mb2_device_count(void);
 void mb2_default_gauss_newton_options(mb2_gauss_newton_options* opt);
 
@@ -292,7 +291,7 @@ int mb2_solver_get_plan_stats(mb2_solver* s, int64_t stats[12]);
 /* Which fused kernel the last solve ran (fused: 0 none, 1 persistent whole-solve kernel, 2 Gram + Cholesky per iteration) and, after
  * mb2_solver_set_profiling(s, 1), its device time and the per-phase SM cycles of one instance group (persistent kernel: over its whole
  * share of the batch; Gram + Cholesky: CTA 0 summed over the iterations, [0] = prologue, [1..4] unused): [0] work fetch + theta load, [1] ParameterTransform
- * + strip zero fill, [2] FK sweep, [3] residual/units, [4] Jacobian cells, [5] Gram (J^T J, J^T r), [6] tiles out of TMEM,
+ * + strip zero fill, [2] FK sweep, [3] residual/units, [4] Jacobian cells, [5] Gram (J^T J, J^T r), [6] parked tiles written over the strips,
  * [7] Cholesky diagonal tiles, [8] panel tiles, [9] updates, [10] backward substitution, [11] update + bookkeeping + write-back.
  * groups = instance groups per CTA of the persistent kernel. Any output pointer may be NULL. No reference counterpart. */
 int mb2_solver_get_fused_profile(mb2_solver* s, int32_t* fused, int32_t* groups, double* kernel_ms, uint64_t phase_cycles[12]);

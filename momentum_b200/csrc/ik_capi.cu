@@ -1,6 +1,6 @@
 // C-ABI of momentum_b200 (include/momentum_b200.h): handle management, host<->device plumbing and
 // the batched SolverT::solve driver. No CPU fallback: every compute entry fails with MB2_ERR_CUDA
-// when no sm_100 device is usable.
+// when no sm_90 device is usable.
 #include "../../include/momentum_b200.h"
 
 #include <cuda_runtime.h>
@@ -86,7 +86,7 @@ struct DeviceGuard {
   DeviceGuard& operator=(const DeviceGuard&) = delete;
 };
 #define MB2_DEVICE_GUARD(device)                                                                                      \
-  if (usableDevices() <= 0) return fail(MB2_ERR_CUDA, "no usable sm_100 CUDA device: momentum_b200 has no CPU fallback"); \
+  if (usableDevices() <= 0) return fail(MB2_ERR_CUDA, "no usable sm_90 CUDA device: momentum_b200 has no CPU fallback"); \
   DeviceGuard _guard(device);                                                                                         \
   MB2_CUDA(_guard.err)
 
@@ -243,7 +243,7 @@ int usableDevices() {
     int ok = 0;
     for (int d = 0; d < n; ++d) {
       int major = 0;
-      if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, d) == cudaSuccess && major == 10) ++ok;
+      if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, d) == cudaSuccess && major == 9) ++ok;
     }
     g_usableDevices = ok;
     g_deviceChecked = true;
@@ -252,7 +252,7 @@ int usableDevices() {
 }
 
 int requireDevice(int device) {
-  if (usableDevices() <= 0) return fail(MB2_ERR_CUDA, "no usable sm_100 CUDA device: momentum_b200 has no CPU fallback");
+  if (usableDevices() <= 0) return fail(MB2_ERR_CUDA, "no usable sm_90 CUDA device: momentum_b200 has no CPU fallback");
   MB2_CUDA(cudaSetDevice(device));
   MB2_CUDA(initKernelAttributes());
   return MB2_OK;
@@ -1100,8 +1100,9 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
     if (o.fused_mode == MB2_FUSED_PERSISTENT && !eligible)
       return fail(MB2_ERR_UNSUPPORTED, "the fused kernel needs the tile-sparse Gram + tile-scheduled Cholesky path, no line search, and a plan that fits in shared memory");
     // AUTO takes the persistent kernel when the whole batch is one wave of instance groups: a single launch with no host round trip
-    // beats ~2 launches per iteration there (measured 0.60 vs 0.89 ms at 256 x humanoid72 x 10 iterations); at thousands of instances
-    // the per-iteration kernels hide latency better (three instances per SM cannot) and AUTO keeps them
+    // saves ~2 launches per iteration there (H100 80GB HBM3 at 400 W, 256 x humanoid72 x 10 iterations: 0.68 - 0.71 vs 0.83 ms); at
+    // thousands of instances the per-iteration kernels keep more instances in flight per SM (the persistent kernel holds at most three)
+    // and AUTO keeps them (8192 instances: 13.0 vs 9.8 - 9.9 ms)
     int smCount = 0;
     if (eligible && o.fused_mode == MB2_FUSED_AUTO) {
       int dev0 = 0;
@@ -1174,8 +1175,8 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   if (useGram && useSchedule) {
     const DeviceSchedule& ds = *f->sched;
     const int rounds = std::max(int(ds.gram.tileOrder.size()) / kGramWarps, 1);
-    const bool fits = gramCholeskySmemBytes(size_t(ds.gram.stride), ds.gBlobInts, ns, ds.host.nPad, ds.host.numTiles, ds.dev.blobInts) <= size_t(200 * 1024) && 16 * rounds <= 128;
-    if (o.fused_mode == MB2_FUSED_GRAM_CHOLESKY && !fits) return fail(MB2_ERR_UNSUPPORTED, "Gram + Cholesky fusion: strips / tiles of this plan do not fit in shared memory or TMEM");
+    const bool fits = gramCholeskySmemBytes(size_t(ds.gram.stride), ds.gBlobInts, ns, ds.host.nPad, ds.host.numTiles, ds.dev.blobInts) <= size_t(200 * 1024) && rounds <= kGramCholMaxRounds;
+    if (o.fused_mode == MB2_FUSED_GRAM_CHOLESKY && !fits) return fail(MB2_ERR_UNSUPPORTED, "Gram + Cholesky fusion: strips / tiles of this plan do not fit in shared memory, or too many tiles per warp");
     useGramChol = fits && (o.fused_mode == MB2_FUSED_AUTO || o.fused_mode == MB2_FUSED_GRAM_CHOLESKY);
   } else if (o.fused_mode == MB2_FUSED_GRAM_CHOLESKY) {
     return fail(MB2_ERR_UNSUPPORTED, "Gram + Cholesky fusion needs the tile-sparse Gram + tile-scheduled Cholesky path");
@@ -1532,7 +1533,7 @@ int mb2_solver_get_fused_profile(mb2_solver* s, int32_t* fused, int32_t* groups,
       MB2_CUDA(cudaMemcpy(h, s->dPhaseCycles.p, sizeof(h), cudaMemcpyDeviceToHost));
       if (s->lastFused) {
         for (int k = 0; k < 12; ++k) phaseCycles[k] = h[k];
-      } else { // gramCholeskyKernel (block 0, summed over the iterations): prologue, gram, tiles from TMEM, diag, panel, update, backward, finish
+      } else { // gramCholeskyKernel (block 0, summed over the iterations): prologue, gram, parked tiles, diag, panel, update, backward, finish
         phaseCycles[0] = h[0];
         for (int k = 1; k < 8; ++k) phaseCycles[4 + k] = h[k];
       }

@@ -285,9 +285,8 @@ MB2_HD void tileStoreRow(float* tile, int r, const float* a) {
 // execute the same instruction:   v[j] -= (v[k] / d_k) * c_j  for j > k
 //   row hl of A:     a[j] -= U[hl][k] * A[k][j]             (A[k][j] = A[j][k] = c_j: the trailing block stays symmetric)
 //   column hl of E:  E[j][hl] -= U[j][k] * E[k][hl] = c_j * (E[k][hl] / d_k)
-// so a step costs one column broadcast and 15 - k FMAs for the whole tile. (A warp is limited by its own issue rate, about one instruction
-// per three cycles: the first version, a half-warp per tile with separate a / e loops and 33 shuffles per step, ran ~100 instructions per
-// step and took 4800 cycles per tile on an idle SM; measured with scripts/microbench.cu.)
+// so a step costs one column broadcast and 15 - k FMAs for the whole tile: a warp is limited by its own issue rate, and a half-warp per
+// tile with separate a / e loops and 33 shuffles per step would issue several times the instructions.
 // The tile is symmetric (the Gram / update products compute both triangles; K-major boxes are mirrored by cholConvertBox) and only
 // entries A[r][c], c <= r, are ever consumed.
 MB2_HD void cholDiagTile(float* tile, float* y16, int lane, float fallback, int* fail) {
@@ -299,9 +298,8 @@ MB2_HD void cholDiagTile(float* tile, float* y16, int lane, float fallback, int*
   for (int k = 0; k < 16; ++k) v[k] = isE ? (k == hl ? 1.f : 0.f) : tile[tileIdx(k, hl)];
   float z = isE ? 0.f : y16[hl], rdSelf = 0.f;
   // Column k of A (c_j = lane j's element k) reaches every lane through shared memory: the row lanes store their element k with ONE
-  // instruction and everyone reads the column back as broadcast LDS.128 - a chain of (17 - k) shuffles per step kept the warp at one
-  // shuffle / FMA pair per 13 cycles (3800 cycles per tile). The tile's own storage is the buffer (its contents live in registers until
-  // W is written at the end): two blocks of [16 column entries | 16 right-hand-side entries], alternating by step parity so that one
+  // instruction and everyone reads the column back as broadcast LDS.128 instead of a chain of (17 - k) dependent shuffles per step.
+  // The tile's own storage is the buffer (its contents live in registers until W is written at the end): two blocks of [16 column entries | 16 right-hand-side entries], alternating by step parity so that one
   // __syncwarp per step orders everything.
   __syncwarp(); // every lane has read its column before the buffer blocks are written
 #pragma unroll
@@ -439,9 +437,9 @@ MB2_HD void cholVectorTask(const float* tiles, float* y, const CholSchedDev& S, 
 // ---- backward substitution for one tile column K: y_K <- L(K,K)^-T (y_K - sum_I L(I,K)^T y_I); ONE WARP per column ----
 // Both parts are "column sums of a tile against a vector": sum_r X(r, c) v[r]. A lane reads its own fragment of the tile (two
 // conflict-free LDS.128: rows g, g + 8 x columns 2t, 2t + 1, 8 + 2t, 9 + 2t), multiplies by v[g], v[g + 8] and keeps four partial
-// column sums over all panel tiles of the column; ONE butterfly over the eight lanes that share t finishes them. (The first version,
-// a half-warp per column with lane c reading X(r, c) scalar by scalar, made 18 % of the fused kernel's shared-memory wavefronts, most
-// of them bank-conflict replays: a row of the fragment layout is not a conflict-free 4-byte access.)
+// column sums over all panel tiles of the column; ONE butterfly over the eight lanes that share t finishes them. (A half-warp per
+// column with lane c reading X(r, c) scalar by scalar would replay on bank conflicts: a row of the fragment layout is not a
+// conflict-free 4-byte access.)
 MB2_HD void cholBackwardColumn(const float* tiles, float* y, const CholSchedDev& S, int K, int lane) {
 #if defined(__CUDA_ARCH__)
   const int g = lane >> 2, t = lane & 3, so = tileSlotOffset(lane);

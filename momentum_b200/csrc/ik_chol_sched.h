@@ -72,6 +72,10 @@ inline int cholSchedLdH(int n) { return (n + 1 + 15) / 16 * 16; }
 // exists only where a unit with rows in q has a cell in tile column K. Tile (I,J) = sum over quads touching both I and J
 // of strip(q,I)^T strip(q,J); block K of J^T r = sum over its strips of strip^T r[4q..4q+3].
 constexpr int kGramWarps = 8; // warps that share the tiles of one instance (gramTilesKernel, gramCholeskyKernel, a group of the fused kernel)
+// gramCholeskyKernel writes the tiles over the strips they are computed from: a finished tile that would land on strips still being
+// read waits in its warp's registers' spill space (thread-local memory, served by L1 / L2) until every warp is done with the strips.
+// Rounds of the tile-order table that one warp can hold that way.
+constexpr int kGramCholMaxRounds = 8;
 struct GramPlan {
   int32_t numStrips{0}, numTiles{0}, numTileCols{0};
   std::vector<int32_t> stripCoord;    // [numStrips][2] {first row 4q, first device column gi0(K)}; strips are ordered by (quad, tile column)

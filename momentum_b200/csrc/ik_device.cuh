@@ -1,8 +1,8 @@
 // Per-lane building blocks of the FK / residual / Jacobian sweep. Every function is
 // __host__ __device__ so the same code is exercised by the CPU lane-emulation test
-// (tests/emu) before it runs in the sm_100a kernels of ik_kernels.cu.
+// (tests/emu) before it runs in the sm_90a kernels of ik_kernels.cu.
 //
-// Reference math (file:line relative to /root/reference/momentum):
+// Reference math (file:line relative to the momentum/ directory of the momentum repository):
 //   character/joint_state.cpp:22-82, character/skeleton_state.cpp:87-121,
 //   character/parameter_transform.cpp:110-123, math/transform.h:124-129,165-167,193-195,
 //   character_solver/joint_error_function-inl.h:179-297, position_/orientation_/state_/limit_error_function.cpp,

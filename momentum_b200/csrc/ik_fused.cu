@@ -33,10 +33,9 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
   uint8_t* base = fusedSmem + ((128u - (smemAddr(fusedSmem) & 127u)) & 127u);
   int32_t* tab = reinterpret_cast<int32_t*>(base);
   unsigned long long* bar = reinterpret_cast<unsigned long long*>(tab + a.L.words);
-  uint32_t* tmemSlot = reinterpret_cast<uint32_t*>(bar + 1);
   float* groupBase = reinterpret_cast<float*>(bar + 2) + size_t(group) * a.groupFloats;
 
-  // ---- once per CTA: every table by bulk copies on one mbarrier; TMEM for the whole CTA ----
+  // ---- once per CTA: every table by bulk copies on one mbarrier ----
   const uint32_t barAddr = smemAddr(bar);
   if (tid == 0) {
     mbarInit(barAddr, 1);
@@ -46,14 +45,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
     const char* src = reinterpret_cast<const char*>(a.blob);
     for (uint32_t off = 0; off < total; off += 32768u) bulkLoad(smemAddr(tab) + off, src + off, total - off < 32768u ? total - off : 32768u, barAddr);
   }
-  if (tid < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smemAddr(tmemSlot)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmemBase = *reinterpret_cast<volatile uint32_t*>(tmemSlot);
   mbarWaitRelaxed(barAddr, 0);
 
   // table views on the staged copy (every pointer derived from the shared-memory base: see rebaseSchedule)
@@ -97,7 +89,8 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
 
   auto groupSync = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(1 + group), "r"(kFusedGroupThreads) : "memory"); };
   const int numJointParams = T.numJoints * kParametersPerJoint;
-  const uint32_t tmemWarp = tmemBase + (uint32_t(((tid >> 5) & 3) * 32) << 16) + uint32_t((tid >> 7) * a.tmemColsPerWarp); // lane quarter, column slot
+  const size_t sweepStripFloats = size_t(a.stripStride) + 64; // strips | residual | zero strip: what the Gram phase reads
+  float parked[kFusedMaxRounds][8]; // Gram tiles that would overwrite live strips, indexed by the round: thread-local memory
 
   unsigned long long pc[kPhases];
   long long pt = 0;
@@ -150,7 +143,8 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
       }
       groupSync();
       MB2_PH(kPhCells)
-      // ---- tile-sparse Gram: a warp owns a tile at a time; finished accumulators wait in TMEM because the tiles will overwrite the strips ----
+      // ---- tile-sparse Gram: a warp owns a tile at a time; a finished tile beyond the strips is stored at once, one that would
+      //      overwrite strips still being read waits in thread-local memory ----
       {
         int slot = 0;
         for (int ti = warp; ti < a.numOrder; ti += kFusedGroupThreads / 32, ++slot) {
@@ -162,11 +156,14 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
 #pragma unroll
             for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
           gramTileAccumulate(strips, quads, tileQuadStart[t], tileQuadStart[t + 1], lane, acc);
-          tmemPark8(tmemWarp + 8u * slot, &acc[0][0]);
+          if (size_t(t) * 256 >= sweepStripFloats) gramTileStore(tiles + size_t(t) * 256, acc, tileInfo[t], a.regularization, lane);
+          else {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) parked[slot][i] = acc[i >> 2][i & 3];
+          }
         }
         for (int K = hw; K < S.numTileCols; K += kFusedGroupThreads / 16)
           y[16 * K + hl] = gramVectorEntry(strips, resid, colStrip, stripRow, colStripStart[K], colStripStart[K + 1], hl);
-        tmemParkWait();
       }
       groupSync();
       MB2_PH(kPhGram)
@@ -174,9 +171,10 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
         int slot = 0;
         for (int ti = warp; ti < a.numOrder; ti += kFusedGroupThreads / 32, ++slot) {
           const int t = tileOrder[ti];
-          if (t < 0) continue;
+          if (t < 0 || size_t(t) * 256 >= sweepStripFloats) continue;
           float acc[2][4];
-          tmemFetch8(tmemWarp + 8u * slot, &acc[0][0]);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) acc[i >> 2][i & 3] = parked[slot][i];
           gramTileStore(tiles + size_t(t) * 256, acc, tileInfo[t], a.regularization, lane);
         }
         for (int s = gt; s < S.nPad; s += kFusedGroupThreads) {
@@ -252,9 +250,6 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
     if (profiler && a.phaseCycles != nullptr)
       for (int k = 0; k < kPhases; ++k) a.phaseCycles[k] = pc[k];
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (tid < 32) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmemBase), "r"(512u) : "memory");
 }
 
 } // namespace
@@ -265,11 +260,11 @@ FusedConfig fusedConfigure(const FunctionTables& T, const FusedBlobLayout& L, co
   const int sweep = stripStride + 64 + ((T.numJoints * kJointStateStride + 3) & ~3) + ((T.numJoints * kParametersPerJoint + 3) & ~3) + ((T.recStride + 3) & ~3);
   c.unionFloats = (std::max(S.numTiles * 256, sweep) + 3) & ~3;
   c.groupFloats = c.unionFloats + S.nPad + 2 * nc4 + np4 + 32; // + 10 doubles and 4 ints of per-instance state
-  c.tmemColsPerWarp = 8 * std::max(orderRounds, 1);
+  if (orderRounds > kFusedMaxRounds) return c; // more parked tiles per warp than the kernel holds
   const size_t fixed = 128 + size_t(L.words) * 4 + 16;
   for (int g = kFusedMaxGroups; g >= 1; --g) {
     const size_t need = fixed + size_t(g) * c.groupFloats * sizeof(float);
-    if (need <= size_t(maxSmemOptin) && 2 * g * c.tmemColsPerWarp <= 512) { // two warps of every group share a TMEM lane quarter
+    if (need <= size_t(maxSmemOptin)) {
       c.groups = g;
       c.smemBytes = need;
       break;
@@ -284,7 +279,6 @@ cudaError_t launchFusedSolve(const FusedArgs& a0, const FusedConfig& cfg, int nu
   a.groups = cfg.groups;
   a.groupFloats = cfg.groupFloats;
   a.unionFloats = cfg.unionFloats;
-  a.tmemColsPerWarp = cfg.tmemColsPerWarp;
   int grid = (a.batch + cfg.groups - 1) / cfg.groups;
   if (grid > numSms) grid = numSms;
   if (grid < 1) grid = 1;

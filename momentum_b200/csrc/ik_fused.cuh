@@ -5,8 +5,8 @@
 // in shared memory for ALL of its iterations:
 //
 //   theta --ParameterTransform / FK sweep--> joint frames --units/cells--> Jacobian strips (shared memory)
-//         --tile-sparse Gram (mma.sync 3xTF32)--> accumulators parked in TMEM while the strips are still being read
-//         --tcgen05.ld--> 16x16 tiles of J^T J + lambda I written over the (now dead) strips
+//         --tile-sparse Gram (mma.sync 3xTF32)--> 16x16 tiles of J^T J + lambda I; a tile that would overwrite strips still being
+//           read is parked in thread-local memory and written over them once they are dead
 //         --level-scheduled Cholesky + both substitutions--> delta --> theta -= delta, convergence test (solver.cpp:98-113)
 //
 // so per solve an instance moves theta, its targets and three result words through HBM and nothing else: no Jacobian, no normal
@@ -23,6 +23,7 @@ namespace mb2 {
 
 constexpr int kFusedGroupThreads = 256;
 constexpr int kFusedMaxGroups = 3;
+constexpr int kFusedMaxRounds = 32; // rounds of the Gram tile-order table a warp can park (fusedConfigure refuses larger plans)
 
 // word (4-byte) offsets of the tables inside the plan blob (every table starts on a 16-byte boundary)
 struct FusedBlobLayout {
@@ -58,12 +59,11 @@ struct FusedArgs {
   int32_t groups;              // instance groups per CTA (1..3)
   int32_t groupFloats;         // shared-memory floats per group
   int32_t unionFloats;         // ... of which the strips / tiles union region
-  int32_t tmemColsPerWarp;     // 8 * tiles per warp
 };
 
 struct FusedConfig {
   int groups{0};
-  int groupFloats{0}, unionFloats{0}, tmemColsPerWarp{0};
+  int groupFloats{0}, unionFloats{0};
   size_t smemBytes{0};
 };
 // how many groups fit next to the staged tables (0: the fused kernel cannot run this plan)

@@ -1,36 +1,34 @@
-// K2 on the 5th-generation tensor cores: per-instance [J r]^T [J r] (lower triangle) with
-// tcgen05.mma kind::tf32, fp32 accumulators in TMEM, operands staged global -> shared by TMA.
+// K2 on the Hopper tensor cores: per-instance [J r]^T [J r] (upper triangle) with wgmma (tf32 inputs, fp32 accumulators in
+// registers), operands staged global -> shared by TMA.
 //
 //   reference computation: jtj.selfadjointView<Lower>().rankUpdate(J^T); jtr += J^T r
 //   (momentum/solver/solver_function.cpp:113-116, gauss_newton_solver.cpp:215-216)
 //
 // Data layout. The device Jacobian of an instance is R = numCols + 1 "column vectors" of ldJ floats
 // (column c of J at J + c*ldJ, the residual r as vector numCols): a K-major [R x K] operand, which is
-// exactly what both UMMA operands want for D = X X^T with X = [J r]^T. D's last row is J^T r, so Jtr
-// costs nothing extra. One TMA box (boxRows x 32 floats, SWIZZLE_128B) per 32-row K block lands the
-// whole K slab of an instance; out-of-range rows are zero-filled by TMA.
+// exactly what both wgmma operands want for D = X X^T with X = [J r]^T (tf32 wgmma takes K-major operands only). D's last row is
+// J^T r, so Jtr costs nothing extra. One TMA box (boxRows x 32 floats, SWIZZLE_128B) per 32-row K block lands the whole K slab of
+// an instance; out-of-range rows are zero-filled by TMA.
 //
-// Precision. kind::tf32 keeps 10 mantissa bits, so a single pass gives ~1e-3 relative error, which
-// would change the Gauss-Newton path of the under-determined IK problems (m < n). The default is the
-// 3xTF32 split: x = hi + lo with hi = tf32(x), lo = tf32(x - hi); D += hi*hi + hi*lo + lo*hi. A group of
-// converter warps derives hi (in place) and lo (second buffer, same swizzled positions) from the raw
-// fp32 slab that TMA delivered.
+// Precision. tf32 keeps 10 mantissa bits, so a single pass gives ~1e-3 relative error, which would change the Gauss-Newton path
+// of the under-determined IK problems (m < n). The default is the 3xTF32 split: x = hi + lo with hi = tf32(x), lo = tf32(x - hi);
+// D += hi*hi + hi*lo + lo*hi. The consumer threads derive hi (in place) and lo (second buffer, same swizzled positions) from the
+// raw fp32 slab that TMA delivered.
 //
-// Work items. The result is cut into row tiles of 128 (UMMA M = 128); row tile t needs the columns 128 t .. only (consumers read the
-// upper triangle). An item is (row tile t, a chunk of at most 256 of those columns) = one accumulator of at most 256 TMEM columns:
+// Work items. The result is cut into row tiles of 128 (two warpgroups of M = 64); row tile t needs the columns 128 t .. only (the
+// upper triangle). An item is (row tile t, a chunk of at most 256 of those columns) = one register accumulator of N = 128 or 256
+// columns per warpgroup:
 //   * diagonal item: columns 128 t .. 128 t + 255 - ONE box of up to 256 operand rows, whose first 128 rows are also the A operand;
 //   * far item (only when numCols + 1 > 128 t + 256): the remaining columns - a B box of those rows plus a separate 128-row A box.
-// numCols + 1 <= 256 gives the two diagonal items of the first version of this kernel; up to 512 (bodyhands300: 425) there are at most
-// four row tiles and at most one far item per tile. Two TMEM slots of 256 columns alternate between consecutive items, so the epilogue
-// of one item drains while the MMAs of the next run.
+// Up to numCols + 1 = 512 (bodyhands300: 425) there are at most four row tiles and at most one far item per tile. Columns of an
+// accumulator beyond the item's width multiply rows that TMA zero-filled and are not stored.
 //
-// Roles in one persistent CTA (1 CTA / SM, 448 threads):
-//   warp 0        TMA producer (one elected lane)
-//   warp 1        TMEM allocator + MMA issuer (one elected lane)
-//   warps 2..9    hi/lo converters
-//   warps 10..13  epilogue: TMEM -> registers -> shared (32x32 transpose stage) -> global rows (upper triangle) of the symmetric matrix,
-//                 every store instruction covering four full 128-byte lines
-// Pipelines: smem ring full -> converted -> (MMA) -> empty; TMEM full/empty between MMA and epilogue.
+// Roles in one persistent CTA (1 CTA / SM, 288 threads):
+//   warps 0..7  two consumer warpgroups: hi/lo conversion of a landed stage (all 256 threads), then each warpgroup issues the
+//               wgmmas of its 64 rows; the conversion of stage s + 1 overlaps the wgmmas of stage s. After an item's last K
+//               block the accumulators go straight from registers to the rows (upper triangle) of the symmetric matrix.
+//   warp 8      TMA producer (one elected lane)
+// Pipeline: smem ring full (TMA) -> empty (both warpgroups' wgmmas of the stage have completed).
 #include "ik_jtj_tc.cuh"
 #include "ik_ptx.cuh"
 
@@ -39,27 +37,23 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
-#include <map>
-#include <mutex>
-#include <tuple>
 
 namespace mb2 {
 
 namespace {
 
-constexpr int kTcThreads = 448;      // warp 0 TMA, warp 1 MMA, warps 2-9 converters, warps 10-13 epilogue
-constexpr int kConvThreads = 256;
-constexpr int kStageRowFloats = 36;  // epilogue staging row: 32 floats + 4 pad (16-byte aligned, conflict-free float4 rows)
+constexpr int kConsumerThreads = 256; // two warpgroups
+constexpr int kTcThreads = kConsumerThreads + 32;
 constexpr int kKBlock = 32;         // floats per K block = one 128-byte swizzle row
 constexpr int kRowBytes = 128;
-constexpr int kUmmaK = 8;           // tf32: 32 bytes of K per instruction
+constexpr int kWgmmaK = 8;          // tf32: 32 bytes of K per instruction
 
 constexpr int kMaxItems = 8;
 struct TcItem {
   int aRow0;    // first operand row of the A box = first row of the row tile (128 t)
   int bRow0;    // first operand row of the B box = first column of the chunk
-  int n;        // UMMA N: columns of the chunk, a multiple of 16, <= 256
-  int bBoxRows; // 256 or 128: which tensor map loads the B box
+  int n;        // columns of the chunk, a multiple of 16, <= 256
+  int bBoxRows; // 256 or 128: which tensor map loads the B box (also the wgmma N)
   int sepA;     // far item: the A rows are not in the B box, a second (128-row) box is loaded behind the B region
 };
 struct TcParams {
@@ -73,299 +67,187 @@ struct TcParams {
   TcItem items[kMaxItems];
   int bRegionRows; // operand rows reserved for the B box in a stage (256, or 128 when every item fits a 128-row box)
   int planeRows;   // bRegionRows (+ 128 when some item needs a separate A box): rows of one hi (or lo) plane of a stage
-  int tmemCols;    // 2 slots x 256 (or the power of two that holds 2 x the widest item)
-  int slotCols;
   int stages;
   size_t hStride;
   float* G;       // optional [batch][ldG]: J^T r as a contiguous vector (the scheduled Cholesky bulk-copies it)
   int ldG;
-  int profile;    // MB2_TC_PROFILE=1: block 0 prints per-role wait/busy cycles (debug aid, off by default)
 };
 
-__device__ __forceinline__ void ummaTf32(uint32_t tmemD, uint64_t descA, uint64_t descB, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmmaTf32N128(float (&d)[64], uint64_t descA, uint64_t descB, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmemD),
-      "l"(descA), "l"(descB), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(descA), "l"(descB), "r"(accumulate)
       : "memory");
 }
-__device__ __forceinline__ void ummaCommit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void wgmmaTf32N256(float (&d)[128], uint64_t descA, uint64_t descB, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(descA), "l"(descB), "r"(accumulate)
+      : "memory");
 }
-__device__ __forceinline__ void tcFenceBefore() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcFenceAfter() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+
 __device__ __forceinline__ uint32_t toTf32(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return r;
 }
-__device__ __forceinline__ void tmemLoad16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
 
-__device__ __forceinline__ void tmemLoad32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
-      "%23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-// start>>4 [0,14) | LBO>>4 [16,30) (=1, unused for swizzled K-major) | SBO>>4 [32,46) (8 rows * 128 B)
-// | version=1 [46,48) | layout_type=2 (SWIZZLE_128B) [61,64)
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (the stage buffers are 1024-byte aligned, base offset 0):
+// start>>4 [0,14) | LBO>>4 [16,30) (=1, unused for swizzled K-major) | SBO>>4 [32,46) (8 rows * 128 B) | layout 1 = SWIZZLE_128B [62,64)
 __device__ __forceinline__ uint64_t makeSmemDesc(uint32_t addr) {
-  return (uint64_t)((addr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((addr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// cute::UMMA::InstrDescriptor: c_format F32 (1) [4,6) | a_format TF32 (2) [7,10) | b_format TF32 (2) [10,13)
-// | a_major K (0) [15] | b_major K (0) [16] | N>>3 [17,23) | M>>4 [24,29)
-__device__ __forceinline__ uint32_t makeInstrDesc(int m, int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+
+struct TcSmem {
+  uint32_t base;      // shared-window address of the 1024-aligned stage ring
+  uint8_t* gen;       // generic pointer to the same byte
+  uint32_t slabBytes, stageBytes, aRegionOff, barBase;
+  int stages;
+  __device__ uint32_t fullBar(int s) const { return barBase + 8u * s; }
+  __device__ uint32_t emptyBar(int s) const { return barBase + 8u * (stages + s); }
+};
+
+// One work item of instance b for both consumer warpgroups: the K loop (convert, wgmma) and the store of the accumulators.
+// N = the item's B box rows = the wgmma N.
+template <int N>
+__device__ __forceinline__ void consumeItem(const TcParams& p, const TcSmem& m, const TcItem& I, int b, int& s, uint32_t& ph) {
+  constexpr int kRegs = N / 2;
+  float d[kRegs];
+#pragma unroll
+  for (int i = 0; i < kRegs; ++i) d[i] = 0.f;
+  const int ct = threadIdx.x, wg = ct >> 7, t = ct & 127;
+  // two segments of a plane: the B box, and (far items) the A box behind the B region
+  const int vecsB = I.bBoxRows * kRowBytes / 16, vecsA = I.sepA ? 128 * kRowBytes / 16 : 0, offA = int(m.aRegionOff / 16u);
+  const uint32_t aOff = (I.sepA ? m.aRegionOff : 0u) + uint32_t(wg * 64 * kRowBytes); // this warpgroup's 64 rows of the A operand
+  int prev = -1;
+  for (int kb = 0; kb < p.kBlocks; ++kb) {
+    mbarWaitSilent<false>(m.fullBar(s), ph);
+    float4* hi = reinterpret_cast<float4*>(m.gen + m.stageBytes * s);
+    float4* lo = reinterpret_cast<float4*>(m.gen + m.stageBytes * s + m.slabBytes);
+#pragma unroll 4
+    for (int j = ct; j < vecsB + vecsA; j += kConsumerThreads) {
+      const int i = j < vecsB ? j : offA + (j - vecsB);
+      const float4 x = hi[i];
+      uint4 h;
+      h.x = toTf32(x.x); h.y = toTf32(x.y); h.z = toTf32(x.z); h.w = toTf32(x.w);
+      reinterpret_cast<uint4*>(hi)[i] = h;
+      if (p.passes == 3) {
+        uint4 l;
+        l.x = toTf32(x.x - __uint_as_float(h.x)); l.y = toTf32(x.y - __uint_as_float(h.y));
+        l.z = toTf32(x.z - __uint_as_float(h.z)); l.w = toTf32(x.w - __uint_as_float(h.w));
+        reinterpret_cast<uint4*>(lo)[i] = l;
+      }
+    }
+    fenceProxyAsync(); // generic-proxy stores -> visible to the tensor core (async proxy)
+    asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+    const uint32_t hiA = m.base + m.stageBytes * s, loA = hiA + m.slabBytes;
+    for (int pass = 0; pass < p.passes; ++pass) {
+      const uint32_t aBase = (pass == 2 ? loA : hiA) + aOff; // hi*hi, hi*lo, lo*hi
+      const uint32_t bBase = pass == 1 ? loA : hiA;
+#pragma unroll
+      for (int k4 = 0; k4 < kKBlock / kWgmmaK; ++k4) {
+        const uint32_t acc = (kb == 0 && pass == 0 && k4 == 0) ? 0u : 1u;
+        if constexpr (N == 256) wgmmaTf32N256(d, makeSmemDesc(aBase + k4 * 32u), makeSmemDesc(bBase + k4 * 32u), acc);
+        else wgmmaTf32N128(d, makeSmemDesc(aBase + k4 * 32u), makeSmemDesc(bBase + k4 * 32u), acc);
+      }
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); // the previous stage's wgmmas are done: release it
+    if (prev >= 0 && t == 0) mbarArrive(m.emptyBar(prev));
+    prev = s;
+    if (++s == p.stages) { s = 0; ph ^= 1u; }
+  }
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+  if (t == 0) mbarArrive(m.emptyBar(prev));
+
+  // accumulator fragment: d[4j + 2h + e] = D(16 warp + lane / 4 + 8 h, 8 j + 2 (lane % 4) + e) of this warpgroup's 64 rows
+  float* H = p.H + (size_t)b * p.hStride;
+  const int warp = t >> 5, lane = t & 31;
+  const int colEnd = I.bRow0 + I.n;
+  const bool solverPath = p.ns == p.numCols;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = I.aRow0 + wg * 64 + warp * 16 + (lane >> 2) + 8 * h;
+    const int i = row < p.ns ? row : (row == p.numCols ? p.ns : -1); // row of the (ns+1) system; -1: not wanted
+    if (i < 0) continue;
+    float* Hrow = H + (size_t)i * p.ldH;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const int c = I.bRow0 + 8 * j + 2 * (lane & 3);
+      const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+      if (solverPath) {
+        // full rows, upper triangle (col >= row) only: everything downstream reads H(min, max)
+        if (c + 1 < colEnd && c + 1 < p.ldH && c >= i) *reinterpret_cast<float2*>(Hrow + c) = make_float2(v0, v1);
+        else {
+          if (c < colEnd && c < p.ldH && c >= i) Hrow[c] = v0;
+          if (c + 1 < colEnd && c + 1 < p.ldH && c + 1 >= i) Hrow[c + 1] = v1;
+        }
+        if (p.G != nullptr && i < p.ns) { // column numCols = J^T r
+          if (c == p.numCols) p.G[(size_t)b * p.ldG + i] = v0;
+          if (c + 1 == p.numCols) p.G[(size_t)b * p.ldG + i] = v1;
+        }
+      } else {
+        // leading-block request (ns < numCols, getJtJR parity entry): columns ns.. are skipped except the residual column
+        if (c < p.ns) Hrow[c] = v0; else if (c == p.numCols) Hrow[p.ns] = v0;
+        if (c + 1 < p.ns) Hrow[c + 1] = v1; else if (c + 1 == p.numCols) Hrow[p.ns] = v1;
+      }
+    }
+  }
 }
 
 __global__ void __launch_bounds__(kTcThreads, 1) jtjTensorKernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmapHalf, const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smemRaw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t base = (smemAddr(smemRaw) + 1023u) & ~1023u;
-  const uint32_t slabBytes = (uint32_t)p.planeRows * kRowBytes;        // one K block of every operand row of an item: [B box | A box of far items]
-  const uint32_t stageBytes = slabBytes * (p.passes == 3 ? 2u : 1u);   // hi [+ lo]
-  const uint32_t aRegionOff = (uint32_t)p.bRegionRows * kRowBytes;     // where a far item's A box sits inside a plane
-  const uint32_t barBase = base + stageBytes * p.stages;
-  auto fullBar = [&](int s) { return barBase + 8u * s; };
-  auto convBar = [&](int s) { return barBase + 8u * (p.stages + s); };
-  auto emptyBar = [&](int s) { return barBase + 8u * (2 * p.stages + s); };
-  // Two TMEM slots with their own full / empty barriers alternate between consecutive work items (file header)
-  auto tmemFullBar = [&](int t) { return barBase + 8u * (3 * p.stages + t); };
-  auto tmemEmptyBar = [&](int t) { return barBase + 8u * (3 * p.stages + 2 + t); };
-  const uint32_t tmemSlot = barBase + 8u * (3 * p.stages + 4);
-  const uint32_t stageOff = ((tmemSlot + 16u - base) + 15u) & ~15u; // epilogue transpose stages: 4 warps x 32 rows x 36 floats
-  uint8_t* gen = smemRaw + (base - smemAddr(smemRaw)); // generic pointer to the aligned base
+  TcSmem m;
+  m.base = (smemAddr(smemRaw) + 1023u) & ~1023u;
+  m.gen = smemRaw + (m.base - smemAddr(smemRaw));
+  m.slabBytes = (uint32_t)p.planeRows * kRowBytes;                // one K block of every operand row of an item: [B box | A box of far items]
+  m.stageBytes = m.slabBytes * (p.passes == 3 ? 2u : 1u);          // hi [+ lo]
+  m.aRegionOff = (uint32_t)p.bRegionRows * kRowBytes;              // where a far item's A box sits inside a plane
+  m.barBase = m.base + m.stageBytes * p.stages;
+  m.stages = p.stages;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbarInit(fullBar(s), 1); mbarInit(convBar(s), kConvThreads); mbarInit(emptyBar(s), 1); }
-    for (int t = 0; t < 2; ++t) { mbarInit(tmemFullBar(t), 1); mbarInit(tmemEmptyBar(t), 128); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int s = 0; s < p.stages; ++s) { mbarInit(m.fullBar(s), 1); mbarInit(m.emptyBar(s), 2); } // empty: one arrival per consumer warpgroup
+    fenceBarrierInit();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmemSlot), "r"((uint32_t)p.tmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcFenceBefore();
   __syncthreads();
-  tcFenceAfter();
-  const uint32_t tmemBase = *reinterpret_cast<volatile uint32_t*>(gen + (tmemSlot - base));
 
-  if (warp == 0) {
+  int s = 0;
+  uint32_t ph = 0;
+  if (warp == kConsumerThreads / 32) {
     // ---------------- TMA producer ----------------
     if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      long long wEmpty = 0, tStart = clock64();
       for (int b = blockIdx.x; b < p.batch; b += gridDim.x) {
         if (p.active != nullptr && p.active[b] == 0) continue;
         for (int it = 0; it < p.numItems; ++it) {
           const TcItem I = p.items[it];
           const uint32_t bBytes = (uint32_t)I.bBoxRows * kRowBytes;
           for (int kb = 0; kb < p.kBlocks; ++kb) {
-            long long t0 = clock64();
-            mbarWaitRelaxed(emptyBar(s), ph ^ 1u);
-            wEmpty += clock64() - t0;
-            mbarExpectTx(fullBar(s), bBytes + (I.sepA ? 128u * kRowBytes : 0u));
-            tmaLoad3d(base + stageBytes * s, I.bBoxRows == 128 ? &tmapHalf : &tmap, kb * kKBlock, I.bRow0, b, fullBar(s));
-            if (I.sepA) tmaLoad3d(base + stageBytes * s + aRegionOff, &tmapHalf, kb * kKBlock, I.aRow0, b, fullBar(s));
+            mbarWaitSilent<true>(m.emptyBar(s), ph ^ 1u);
+            mbarExpectTx(m.fullBar(s), bBytes + (I.sepA ? 128u * kRowBytes : 0u));
+            tmaLoad3d(m.base + m.stageBytes * s, I.bBoxRows == 128 ? &tmapHalf : &tmap, kb * kKBlock, I.bRow0, b, m.fullBar(s));
+            if (I.sepA) tmaLoad3d(m.base + m.stageBytes * s + m.aRegionOff, &tmapHalf, kb * kKBlock, I.aRow0, b, m.fullBar(s));
             if (++s == p.stages) { s = 0; ph ^= 1u; }
           }
         }
       }
-      if ((p.profile & 1) && blockIdx.x == 0) printf("tc-profile producer: total %lld waitEmpty %lld\n", clock64() - tStart, wEmpty);
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer ----------------
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0, tph[2] = {0, 0}, count = 0;
-      long long wTmem = 0, wConv = 0, tStart = clock64();
-      for (int b = blockIdx.x; b < p.batch; b += gridDim.x) {
-        if (p.active != nullptr && p.active[b] == 0) continue;
-        for (int it = 0; it < p.numItems; ++it, ++count) {
-          const TcItem I = p.items[it];
-          const int slot = int(count & 1u);
-          long long t0 = clock64();
-          mbarWait(tmemEmptyBar(slot), tph[slot] ^ 1u); // the epilogue has drained the item that used this slot before
-          wTmem += clock64() - t0;
-          tcFenceAfter();
-          const uint32_t dcol = tmemBase + uint32_t(slot * p.slotCols);
-          const uint32_t idesc = makeInstrDesc(128, I.n);
-          const uint32_t aOff = I.sepA ? aRegionOff : 0u; // diagonal item: the A rows are the first 128 rows of the B box
-          for (int kb = 0; kb < p.kBlocks; ++kb) {
-            t0 = clock64();
-            mbarWait(convBar(s), ph);
-            wConv += clock64() - t0;
-            tcFenceAfter();
-            const uint32_t hi = base + stageBytes * s, lo = hi + slabBytes;
-            for (int pass = 0; pass < p.passes; ++pass) {
-              const uint32_t aBase = (pass == 2 ? lo : hi) + aOff; // hi*hi, hi*lo, lo*hi
-              const uint32_t bBase = pass == 1 ? lo : hi;
-#pragma unroll
-              for (int k4 = 0; k4 < kKBlock / kUmmaK; ++k4) {
-                const uint32_t acc = (kb == 0 && pass == 0 && k4 == 0) ? 0u : 1u;
-                ummaTf32(dcol, makeSmemDesc(aBase + k4 * 32u), makeSmemDesc(bBase + k4 * 32u), idesc, acc);
-              }
-            }
-            ummaCommit(emptyBar(s)); // smem slab reusable once these MMAs have read it
-            if (kb == p.kBlocks - 1) ummaCommit(tmemFullBar(slot));
-            if (++s == p.stages) { s = 0; ph ^= 1u; }
-          }
-          tph[slot] ^= 1u;
-        }
-      }
-      if ((p.profile & 1) && blockIdx.x == 0) printf("tc-profile mma: total %lld waitTmemEmpty %lld waitConverted %lld\n", clock64() - tStart, wTmem, wConv);
-    }
-  } else if (warp < 10) {
-    // ---------------- converters: raw fp32 -> tf32 hi (in place) and lo ----------------
-    const int ct = threadIdx.x - 64; // 0..255
-    int s = 0;
-    uint32_t ph = 0;
-    long long wFull = 0, tStart = clock64();
+  } else {
+    // ---------------- consumer warpgroups ----------------
     for (int b = blockIdx.x; b < p.batch; b += gridDim.x) {
       if (p.active != nullptr && p.active[b] == 0) continue;
       for (int it = 0; it < p.numItems; ++it) {
         const TcItem I = p.items[it];
-        // two segments of the plane: the B box, and (far items) the A box behind the B region
-        const int vecsB = I.bBoxRows * kRowBytes / 16, vecsA = I.sepA ? 128 * kRowBytes / 16 : 0, offA = int(aRegionOff / 16u);
-        for (int kb = 0; kb < p.kBlocks; ++kb) {
-          long long t0 = clock64();
-          mbarWaitRelaxed(fullBar(s), ph);
-          wFull += clock64() - t0;
-          float4* hi = reinterpret_cast<float4*>(gen + stageBytes * s);
-          float4* lo = reinterpret_cast<float4*>(gen + stageBytes * s + slabBytes);
-#pragma unroll 4
-          for (int j = ct; j < vecsB + vecsA; j += kConvThreads) {
-            const int i = j < vecsB ? j : offA + (j - vecsB);
-            const float4 x = hi[i];
-            uint4 h;
-            h.x = toTf32(x.x); h.y = toTf32(x.y); h.z = toTf32(x.z); h.w = toTf32(x.w);
-            reinterpret_cast<uint4*>(hi)[i] = h;
-            if (p.passes == 3) {
-              uint4 l;
-              l.x = toTf32(x.x - __uint_as_float(h.x)); l.y = toTf32(x.y - __uint_as_float(h.y));
-              l.z = toTf32(x.z - __uint_as_float(h.z)); l.w = toTf32(x.w - __uint_as_float(h.w));
-              reinterpret_cast<uint4*>(lo)[i] = l;
-            }
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy stores -> visible to the tensor core (async proxy)
-          mbarArrive(convBar(s));
-          if (++s == p.stages) { s = 0; ph ^= 1u; }
-        }
+        if (I.bBoxRows == 128) consumeItem<128>(p, m, I, b, s, ph);
+        else consumeItem<256>(p, m, I, b, s, ph);
       }
     }
-    if ((p.profile & 1) && blockIdx.x == 0 && ct == 0) printf("tc-profile converter: total %lld waitFull %lld\n", clock64() - tStart, wFull);
-  } else {
-    // ---------------- epilogue: TMEM -> global, column-major lower triangle of [JtJ; Jtr] ----------------
-    const int q = warp & 3; // TMEM lane quarter this warp may access
-    float* stage = reinterpret_cast<float*>(gen + stageOff) + (warp - 10) * 32 * kStageRowFloats;
-    uint32_t eph[2] = {0, 0}, count = 0;
-    long long wFullT = 0, tStart = clock64(), tLd = 0, nChunks = 0, tSts = 0, tStg = 0;
-    for (int b = blockIdx.x; b < p.batch; b += gridDim.x) {
-      if (p.active != nullptr && p.active[b] == 0) continue;
-      float* H = p.H + (size_t)b * p.hStride;
-      for (int it = 0; it < p.numItems; ++it, ++count) {
-        const TcItem I = p.items[it];
-        const int slot = int(count & 1u);
-        long long t0 = clock64();
-        mbarWaitRelaxed(tmemFullBar(slot), eph[slot]);
-        wFullT += clock64() - t0;
-        tcFenceAfter();
-        const int rowBase = I.aRow0 + q * 32;                     // first of this warp's 32 rows of [J r]^T [J r]
-        const int cb = I.bRow0;                                   // first matrix column of the item's accumulator
-        const int row = rowBase + lane;
-        const int i = row < p.ns ? row : (row == p.numCols ? p.ns : -1); // row of the (ns+1) system; -1: not wanted
-        if (__reduce_max_sync(0xffffffffu, i) < 0) { tcFenceBefore(); mbarArrive(tmemEmptyBar(slot)); eph[slot] ^= 1u; continue; } // warp-uniform: nothing to write
-        const int nT = I.n;
-        const uint32_t colBase = tmemBase + ((uint32_t)(q * 32) << 16) + uint32_t(slot * p.slotCols);
-        if (p.ns == p.numCols) {
-          // solver path: full rows. 32x32 blocks go TMEM -> registers -> shared (row = TMEM lane) -> global, re-mapped so
-          // that one store instruction writes four rows x 128 contiguous bytes.
-          // the four rows x 128 bytes this lane stores per instruction are the same for every chunk of the tile
-          float* rowPtr[8];
-          int rowIo[8];
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const int rowAbs = rowBase + 4 * k + (lane >> 3);
-            rowIo[k] = rowAbs < p.ns ? rowAbs : (rowAbs == p.numCols ? p.ns : (1 << 30)); // 1 << 30: never stored (col + 3 >= row fails)
-            rowPtr[k] = H + (size_t)(rowIo[k] < (1 << 30) ? rowIo[k] : 0) * p.ldH + 4 * (lane & 7);
-          }
-          for (int c0 = 0; c0 < nT; c0 += 32) {
-            if (cb + c0 + 32 <= rowBase && !(cb + c0 <= p.numCols && p.numCols < cb + c0 + 32)) continue; // entirely left of the diagonal
-            float v[32];
-            const long long tl0 = p.profile ? clock64() : 0;
-            if (c0 + 32 <= nT) tmemLoad32(colBase + (uint32_t)c0, v);
-            else { tmemLoad16(colBase + (uint32_t)c0, v); for (int k = 16; k < 32; ++k) v[k] = 0.f; }
-            if (p.profile) { tLd += clock64() - tl0; ++nChunks; }
-#pragma unroll
-            for (int g4 = 0; g4 < 8; ++g4)
-              *reinterpret_cast<float4*>(stage + lane * kStageRowFloats + 4 * g4) = make_float4(v[4 * g4], v[4 * g4 + 1], v[4 * g4 + 2], v[4 * g4 + 3]);
-            __syncwarp();
-            if (p.profile) { tSts += clock64() - tl0; }
-            if (p.G != nullptr && cb + c0 <= p.numCols && p.numCols < cb + c0 + 32 && i >= 0 && i < p.ns) // column numCols = J^T r
-              p.G[(size_t)b * p.ldG + i] = stage[lane * kStageRowFloats + (p.numCols - cb - c0)];
-            const int c = cb + c0 + 4 * (lane & 7); // matrix column of this lane's float4
-            float4 vals[8]; // all shared-memory reads first: the compiler cannot move them across the global stores itself (possible aliasing)
-#pragma unroll
-            for (int k = 0; k < 8; ++k) vals[k] = *reinterpret_cast<const float4*>(stage + (4 * k + (lane >> 3)) * kStageRowFloats + 4 * (lane & 7));
-            if (!(p.profile & 2) && c < p.ldH) {
-#pragma unroll
-              for (int k = 0; k < 8; ++k)
-                if (c + 3 >= rowIo[k]) *reinterpret_cast<float4*>(rowPtr[k] + (cb + c0)) = vals[k]; // upper triangle (col >= row) only: everything downstream reads H(min, max)
-            }
-            __syncwarp();
-            if (p.profile) { tStg += clock64() - tl0; }
-          }
-        } else {
-          // leading-block request (ns < numCols, getJtJR parity entry): columns ns.. are skipped except the residual column
-          float* Hrow = H + (size_t)(i < 0 ? 0 : i) * p.ldH;
-          for (int c0 = 0; c0 < nT; c0 += 16) {
-            float v[16];
-            tmemLoad16(colBase + (uint32_t)c0, v);
-            if (i < 0) continue;
-#pragma unroll
-            for (int cc = 0; cc < 16; ++cc) {
-              const int c = cb + c0 + cc;
-              if (c < p.ns) Hrow[c] = v[cc];
-              else if (c == p.numCols) Hrow[p.ns] = v[cc];
-            }
-          }
-        }
-        tcFenceBefore();
-        mbarArrive(tmemEmptyBar(slot));
-        eph[slot] ^= 1u;
-      }
-    }
-    if ((p.profile & 1) && blockIdx.x == 0 && lane == 0)
-      printf("tc-profile epilogue q%d: total %lld waitTmemFull %lld chunks %lld | cumulative per chunk: tmemLoad %lld +sts %lld +stg %lld\n", q, clock64() - tStart, wFullT, nChunks,
-             tLd / (nChunks ? nChunks : 1), tSts / (nChunks ? nChunks : 1), tStg / (nChunks ? nChunks : 1));
-  }
-  tcFenceBefore();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmemBase), "r"((uint32_t)p.tmemCols) : "memory");
   }
 }
 
@@ -388,7 +270,7 @@ EncodeTiledFn encodeTiled() {
 int roundUpI(int v, int m) { return (v + m - 1) / m * m; }
 
 struct Shape {
-  int rows, r16, numItems, bRegionRows, planeRows, maxN;
+  int rows, r16, numItems, bRegionRows, planeRows;
   bool anySepA;
   TcItem items[kMaxItems];
 };
@@ -409,7 +291,7 @@ Shape shapeFor(int numCols) {
       s.anySepA = true;
     }
   }
-  for (int i = 0; i < s.numItems; ++i) { s.bRegionRows = s.bRegionRows > s.items[i].bBoxRows ? s.bRegionRows : s.items[i].bBoxRows; s.maxN = s.maxN > s.items[i].n ? s.maxN : s.items[i].n; }
+  for (int i = 0; i < s.numItems; ++i) s.bRegionRows = s.bRegionRows > s.items[i].bBoxRows ? s.bRegionRows : s.items[i].bBoxRows;
   s.planeRows = s.bRegionRows + (s.anySepA ? 128 : 0);
   return s;
 }
@@ -462,19 +344,16 @@ cudaError_t launchJtJTensor(const JtJArgs& a, int passes, cudaStream_t stream) {
   for (int i = 0; i < sh.numItems; ++i) p.items[i] = sh.items[i];
   p.bRegionRows = sh.bRegionRows;
   p.planeRows = sh.planeRows;
-  p.slotCols = 32;
-  while (p.slotCols < sh.maxN) p.slotCols <<= 1;
-  p.tmemCols = 2 * p.slotCols; // a power of two >= 64
   p.hStride = a.hStride;
   p.G = a.g;
   p.ldG = a.ldG;
-  p.profile = getenv("MB2_TC_PROFILE") != nullptr ? atoi(getenv("MB2_TC_PROFILE")) : 0;
+  // stage ring within 196 KB of the 227 KB a block may have: 3 stages of the humanoid's 3xTF32 slab (2 x 32 KB), 2 of bodyhands' (2 x 48 KB)
   const size_t stageBytes = size_t(sh.planeRows) * kRowBytes * (p.passes == 3 ? 2 : 1);
   int stages = int((196 * 1024) / stageBytes);
   if (stages > 6) stages = 6;
   if (stages < 2) return cudaErrorInvalidConfiguration;
   p.stages = stages;
-  const size_t smem = stageBytes * stages + 1024 /*alignment slack*/ + 8 * (3 * stages + 4) + 48 + 4 * 32 * kStageRowFloats * sizeof(float);
+  const size_t smem = stageBytes * stages + 1024 /*alignment slack*/ + 8 * 2 * stages;
   cudaError_t e = cudaFuncSetAttribute(jtjTensorKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
   if (e != cudaSuccess) return e;
   int dev = 0, sms = 0;

@@ -1,4 +1,4 @@
-// Tensor-core JtJ (tcgen05.mma kind::tf32, accumulators in TMEM, operands staged by TMA).
+// Tensor-core JtJ (wgmma tf32, accumulators in registers, operands staged by TMA).
 #pragma once
 
 #include <cuda.h>
@@ -8,7 +8,7 @@
 
 namespace mb2 {
 
-// true when the tcgen05 kernel handles this (subset size, Jacobian row stride)
+// true when the wgmma kernel handles this (subset size, Jacobian row stride)
 bool jtjTensorSupported(int ns, int numCols, int ldJ);
 // passes: 3 = 3xTF32 split (fp32-class accuracy), 1 = single TF32 pass
 cudaError_t launchJtJTensor(const JtJArgs& a, int passes, cudaStream_t stream);

@@ -1,4 +1,4 @@
-// sm_100a kernels for one Gauss-Newton iteration over a batch of IK instances.
+// sm_90a kernels for one Gauss-Newton iteration over a batch of IK instances.
 //
 //   K1  sweepKernel<true, W>      FK sweep + residual + Jacobian cells (strip layout or K-major matrix)  (skeleton_solver_function.cpp:200-261)
 //   K4  sweepKernel<false, W>     FK sweep + error only (line search)                                    (skeleton_solver_function.cpp:64-83)
@@ -8,7 +8,7 @@
 //   K3' choleskyKernel<NB>        dense blocked LLT with Eigen's block structure and early exit (gauss_newton_solver.cpp:248-259, solver.cpp:89-122)
 //   small kernels                 line search, bookkeeping, target scatter / quaternion normalisation
 //
-// The dense tensor-core JtJ (tcgen05, TMEM accumulators, TMA-fed) lives in ik_jtj_tc.cu; PTX wrappers in ik_ptx.cuh.
+// The dense tensor-core JtJ (wgmma, register accumulators, TMA-fed) lives in ik_jtj_tc.cu; PTX wrappers in ik_ptx.cuh.
 #include "ik_kernels.cuh"
 
 #include <algorithm>
@@ -81,8 +81,8 @@ __device__ __forceinline__ void stageTable(const E*& table, size_t count, uint32
 // kStage (1 all tables, 2 all but cells / contributions, 0 none): the tables live in shared memory for the whole kernel. A template parameter rather than a run-time branch so that every
 // table pointer is PROVABLY a shared-memory address: with `if (a.stageTables)` the pointers could be either and all 273 table loads
 // of the kernel were generic LD instructions (address-space check on every hop of the dependent chains cell -> unit -> record ->
-// contributions; 43 % of the warp-state samples were long-scoreboard waits on them, profiles/r02k).
-constexpr int kSweepMaxWarps = 24; // up to 24 warps per CTA (85 registers per thread)
+// contributions).
+constexpr int kSweepMaxWarps = 24; // up to 24 warps per CTA (80 registers per thread on sm_90a)
 template <bool kJacobian, int W, int kStage>
 __global__ void __launch_bounds__(32 * kSweepMaxWarps) sweepKernel(const SweepArgs a) {
   extern __shared__ __align__(16) float smem[];
@@ -189,10 +189,9 @@ cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream)
   const int groupsOneWarp = int((budget - tableBytes) / sweepSmemPerInstance(a.T, 1)); // (no joint-parameter array)
   int W = 1;
   if (groupsOneWarp >= 16) {
-    // The instances of an SM are dealt to its warps round by round, and from about a dozen warps on the kernel is throughput bound
-    // (measured on the cfg3 shard: 0.049 / 0.059 / 0.095 ms per round with 16 / 19 / 28 warps): the time is rounds x warps, i.e. the
-    // padded instance count. Pick the warp count that wastes the fewest slots (8192 instances on 148 SMs: 19 warps x 3 rounds = 8436
-    // slots; 4096 instances: 14 warps x 2 rounds = 4144); a 28-warp variant (73 registers) spilled and lost more than its two rounds won.
+    // The instances of an SM are dealt to its warps round by round, and from about a dozen warps on the kernel is throughput bound:
+    // the time is rounds x warps, i.e. the padded instance count. Pick the warp count that wastes the fewest slots over the SMs of
+    // this device (rounds x warps x SMs closest above the batch); more warps than kSweepMaxWarps spill registers.
     const int sms = std::max(g_numSms, 1);
     const int maxG = std::min(groupsOneWarp, kSweepMaxWarps), minG = std::min(12, maxG);
     long best = -1;
@@ -712,9 +711,9 @@ cudaError_t launchCholeskyScheduled(const CholArgs& a, const CholSchedDev& sched
 // ------------------------------------------------------------------------------------------------
 // K2s + K3 fused (default on the tile path): one CTA per instance, three CTAs per SM.
 //   prologue   strips + residual of the instance, the Gram plan and the Cholesky schedule arrive as bulk copies on one mbarrier
-//   Gram       a warp owns a tile at a time (longest-first assignment); finished accumulators are parked in TMEM
-//              (tcgen05.st) because the tiles are about to overwrite the strips they are computed from
-//   restore    tcgen05.ld -> 16x16 tiles of J^T J + lambda I in the Cholesky layout, over the dead strips
+//   Gram       a warp owns a tile at a time (longest-first assignment); a finished tile that lies beyond the strips is stored at
+//              once, one that would overwrite strips still being read is parked in thread-local memory (L1 / L2)
+//   restore    parked accumulators -> 16x16 tiles of J^T J + lambda I in the Cholesky layout, over the dead strips
 //   Cholesky   level-scheduled tile factorisation, both substitutions, theta -= delta, SolverT bookkeeping (cholFinish)
 // The stored tiles (0.45 GB per iteration on the cfg3 shard) never exist in HBM and the second launch is gone.
 // ------------------------------------------------------------------------------------------------
@@ -725,11 +724,11 @@ size_t gramCholeskySmemBytes(size_t stripStride, int gramBlobInts, int n, int nP
 }
 
 // Shared memory holds only what is per instance: the strip / tile union, the right-hand side in slot order and J^T r per device column
-// (cfg3: 56.4 KB), so that FOUR CTAs fit on an SM (57 KB each, 64 registers per thread); the Gram plan and the Cholesky schedule
+// (cfg3: 54.9 KB), so that FOUR CTAs fit on an SM (with the 1 KB reserved per block, 64 registers per thread); the Gram plan and the Cholesky schedule
 // (10 KB, identical for every CTA) are read from global memory through L1 by the same device functions. The per-instance critical
 // path is a chain of dependent phases no wider than a few warps: instances in flight per SM are what buys throughput.
 template <bool kProfile>
-__global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const GramCholArgs a, const CholSchedDev S, const int tmemColumns) {
+__global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const GramCholArgs a, const CholSchedDev S) {
   extern __shared__ __align__(16) float gcSmem[];
   const GramArgs& g = a.g;
   const CholArgs& c = a.c;
@@ -747,7 +746,6 @@ __global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const Gram
   float* y = U + uni;
   float* gsub = y + S.nPad;
   int* flags = reinterpret_cast<int*>(gsub + ((n + 3) & ~3));
-  uint32_t* tmemSlot = reinterpret_cast<uint32_t*>(flags + 2);
   unsigned long long* bar = reinterpret_cast<unsigned long long*>(flags + 4);
   long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, pt = 0;
   if constexpr (kProfile) pt = clock64();
@@ -762,19 +760,15 @@ __global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const Gram
     const char* src = reinterpret_cast<const char*>(g.strips + size_t(b) * g.stripStride);
     for (uint32_t off = 0; off < stripBytes; off += 16384u) bulkLoad(smemAddr(strips) + off, src + off, stripBytes - off < 16384u ? stripBytes - off : 16384u, barAddr);
   }
-  if (warp == 1) tmemAlloc(smemAddr(tmemSlot), uint32_t(tmemColumns));
   if (tid >= 64 && tid < 128) strips[g.stripStride + (tid - 64)] = 0.f; // the all-zero strip that pads odd pair lists
-  tcgenFenceBeforeSync();
   __syncthreads();
-  tcgenFenceAfterSync();
-  const uint32_t tmemBase = *reinterpret_cast<volatile uint32_t*>(tmemSlot);
-  const uint32_t tmemWarp = tmemBase + (uint32_t((warp & 3) * 32) << 16) + uint32_t((warp >> 2) * (tmemColumns / 2)); // lane quarter; two warps share one
   mbarWaitRelaxed(barAddr, 0);
   MB2_GC(0)
   const int32_t* __restrict__ gtab = g.blob;
   const int32_t* tileOrder = gtab + g.offTileOrder, *tileQuadStart = gtab + g.offTilePairStart, *quads = gtab + g.offPairA;
   const int32_t* colStripStart = gtab + g.offColStripStart, *colStrip = gtab + g.offColStrip, *stripRow = gtab + g.offStripRow, *tileInfo = gtab + g.offTileInfo;
   // ---- Gram ----
+  float parked[kGramCholMaxRounds][8]; // indexed by the round: thread-local memory
   {
     int slot = 0;
     for (int ti = warp; ti < g.numOrder; ti += kGramThreads / 32, ++slot) {
@@ -786,11 +780,14 @@ __global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const Gram
 #pragma unroll
         for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
       gramTileAccumulate(strips, quads, tileQuadStart[t], tileQuadStart[t + 1], lane, acc);
-      tmemPark8(tmemWarp + 8u * slot, &acc[0][0]);
+      if (size_t(t) * 256 >= sweepFloats) gramTileStore(tiles + size_t(t) * 256, acc, tileInfo[t], g.regularization, lane);
+      else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) parked[slot][i] = acc[i >> 2][i & 3];
+      }
     }
     for (int K = hw; K < S.numTileCols; K += kGramThreads / 16)
       y[16 * K + hl] = gramVectorEntry(strips, resid, colStrip, stripRow, colStripStart[K], colStripStart[K + 1], hl);
-    tmemParkWait();
   }
   __syncthreads();
   MB2_GC(1)
@@ -798,9 +795,10 @@ __global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const Gram
     int slot = 0;
     for (int ti = warp; ti < g.numOrder; ti += kGramThreads / 32, ++slot) {
       const int t = tileOrder[ti];
-      if (t < 0) continue;
+      if (t < 0 || size_t(t) * 256 >= sweepFloats) continue;
       float acc[2][4];
-      tmemFetch8(tmemWarp + 8u * slot, &acc[0][0]);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i >> 2][i & 3] = parked[slot][i];
       gramTileStore(tiles + size_t(t) * 256, acc, tileInfo[t], g.regularization, lane);
     }
     for (int s2 = tid; s2 < S.nPad; s2 += kGramThreads) {
@@ -845,28 +843,20 @@ __global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const Gram
       for (int k = 0; k < 8; ++k) a.phaseCycles[k] += (unsigned long long)pc[k];
   }
 #undef MB2_GC
-  tcgenFenceBeforeSync();
-  __syncthreads();
-  if (warp == 1) tmemFree(tmemBase, uint32_t(tmemColumns));
 }
 
 cudaError_t launchGramCholesky(const GramCholArgs& a, const CholSchedDev& sched, bool profile, cudaStream_t stream) {
   const size_t smem = gramCholeskySmemBytes(a.g.stripStride, a.g.blobInts, a.c.ns, sched.nPad, sched.numTiles, sched.blobInts);
   if (smem > size_t(g_maxSmemOptin) || (a.g.stripStride & 3) != 0) return cudaErrorInvalidConfiguration;
-  // TMEM: two warps share a lane quarter, each parks up to `rounds` tiles of 8 columns; allocations are powers of two >= 32,
-  // and the (up to four) CTAs of an SM must fit in its 512 columns together
-  const int rounds = std::max(a.g.numOrder / (kGramThreads / 32), 1);
-  int columns = 32;
-  while (columns < 2 * 8 * rounds) columns <<= 1;
-  if (columns > 128) return cudaErrorInvalidConfiguration;
+  if (a.g.numOrder > kGramCholMaxRounds * (kGramThreads / 32)) return cudaErrorInvalidConfiguration; // parked tiles per warp
   cudaError_t e = profile ? cudaFuncSetAttribute(gramCholeskyKernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem))
                           : cudaFuncSetAttribute(gramCholeskyKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
   if (e != cudaSuccess) return e;
   e = profile ? cudaFuncSetAttribute(gramCholeskyKernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared))
               : cudaFuncSetAttribute(gramCholeskyKernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared));
   if (e != cudaSuccess) return e;
-  if (profile) gramCholeskyKernel<true><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched, columns);
-  else gramCholeskyKernel<false><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched, columns);
+  if (profile) gramCholeskyKernel<true><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched);
+  else gramCholeskyKernel<false><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched);
   return cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-// sm_100a kernels of the batched Gauss-Newton iteration (declarations + launch parameter structs).
+// sm_90a kernels of the batched Gauss-Newton iteration (declarations + launch parameter structs).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -85,12 +85,12 @@ struct GramArgs {            // K2s: stored tiles of J^T J + lambda I and J^T r 
 cudaError_t launchGramTiles(const GramArgs& a, cudaStream_t stream);
 size_t gramTilesSmemBytes(size_t stripStride, int blobInts);
 
-// K2s + K3 in one launch: strips in (bulk copy), Gram accumulators parked in TMEM, tiles written over the strips, tile Cholesky,
-// update. No tile round trip through HBM and no second launch; `g.out` is unused.
+// K2s + K3 in one launch: strips in (bulk copy), tiles beyond the strips stored at once, the others parked in thread-local memory
+// and written over the strips once they are dead, tile Cholesky, update. No second launch; `g.out` is unused.
 struct GramCholArgs {
   GramArgs g;
   CholArgs c;
-  unsigned long long* phaseCycles; // optional [8], profiling instantiation: prologue, gram, tiles from TMEM, diag, panel, update, backward, finish (block 0)
+  unsigned long long* phaseCycles; // optional [8], profiling instantiation: prologue, gram, parked tiles, diag, panel, update, backward, finish (block 0)
 };
 size_t gramCholeskySmemBytes(size_t stripStride, int gramBlobInts, int n, int nPad, int numTiles, int schedBlobInts);
 cudaError_t launchGramCholesky(const GramCholArgs& a, const CholSchedDev& sched, bool profile, cudaStream_t stream);

@@ -1,4 +1,4 @@
-// PTX wrappers shared by the sm_100a kernels: mbarrier, TMA (tensor and 1-D bulk copies into shared memory).
+// PTX wrappers shared by the sm_90a kernels: mbarrier, TMA (tensor and 1-D bulk copies into shared memory).
 #pragma once
 
 #include <cuda.h>
@@ -39,6 +39,25 @@ __device__ __forceinline__ void mbarWait(uint32_t bar, uint32_t parity) {
     }
   }
 }
+// same, without the diagnostic print: for kernels that issue wgmma, where any function call (printf) makes the compiler serialise
+// the wgmma pipeline. kSleep: sleep between polls (waiters with slack)
+template <bool kSleep>
+__device__ __forceinline__ void mbarWaitSilent(uint32_t bar, uint32_t parity) {
+  uint32_t done = 0;
+  const long long t0 = clock64();
+  while (true) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done)
+        : "r"(bar), "r"(parity)
+        : "memory");
+    if (done) break;
+    if constexpr (kSleep) __nanosleep(32);
+    if ((uint64_t)(clock64() - t0) > kSpinLimit) __trap();
+  }
+}
 // same, for waiters with slack (producer / converter / epilogue roles): sleeps between polls so that the spinning warp does not
 // take issue slots from the warps doing the work
 __device__ __forceinline__ void mbarWaitRelaxed(uint32_t bar, uint32_t parity) {
@@ -73,37 +92,5 @@ __device__ __forceinline__ void bulkLoad(uint32_t dst, const void* src, uint32_t
 // makes mbarrier.init visible to the async proxy before the first TMA completes on it
 __device__ __forceinline__ void fenceBarrierInit() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fenceProxyAsync() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// ---- TMEM as a parking lot for the Gram accumulators (tcgen05.st / tcgen05.ld, shape 32x32b: lane i of the warp owns TMEM lane
-// 32 * (warp % 4) + i, eight consecutive columns per tile). Only the warp that parked a tile reads it back, so the only ordering
-// needed is tcgen05.wait::st before the group barrier and tcgen05.wait::ld before the registers are used.
-__device__ __forceinline__ void tmemPark8(uint32_t taddr, const float v[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(__float_as_uint(v[0])),
-               "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-               "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-               : "memory");
-}
-__device__ __forceinline__ void tmemParkWait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmemFetch8(uint32_t taddr, float v[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// TMEM allocation for one CTA (columns: power of two >= 32); the allocating warp also frees it
-__device__ __forceinline__ void tmemAlloc(uint32_t slotAddr, uint32_t columns) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slotAddr), "r"(columns) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmemFree(uint32_t tmemBase, uint32_t columns) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmemBase), "r"(columns) : "memory");
-}
-__device__ __forceinline__ void tcgenFenceBeforeSync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgenFenceAfterSync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 } // namespace mb2

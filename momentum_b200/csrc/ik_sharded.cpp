@@ -75,7 +75,7 @@ int mb2_sharded_solver_create(const mb2_solver_function* prototype, int32_t tota
   const int available = mb2_device_count();
   for (int k = 0; k < numDevices; ++k)
     if (devices[k] < 0 || devices[k] >= available)
-      return shardedFail(MB2_ERR_CUDA, "device " + std::to_string(devices[k]) + " is not a usable sm_100 device (" + std::to_string(available) + " found)");
+      return shardedFail(MB2_ERR_CUDA, "device " + std::to_string(devices[k]) + " is not a usable sm_90 device (" + std::to_string(available) + " found)");
   auto s = std::make_unique<mb2_sharded_solver>();
   s->totalBatch = totalBatch;
   s->numParams = mb2_solver_function_num_parameters(prototype);

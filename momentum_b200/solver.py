@@ -1,12 +1,12 @@
-"""Host-side mirror of the reference's solver interface for the batched B200 path.
+"""Host-side mirror of the reference's solver interface for the batched H100 path.
 
 Class and option names follow momentum (``SolverOptions`` / ``GaussNewtonSolverOptions`` —
 solver/solver.h:19-34, solver/gauss_newton_solver.h:17-59; ``SkeletonSolverFunction`` —
 character_solver/skeleton_solver_function.h:21-95; ``GaussNewtonSolver`` —
 solver/gauss_newton_solver.h:67-137) with a leading batch dimension on parameters and results.
 Everything here is a thin ctypes veneer over the C-ABI in include/momentum_b200.h; the compute is
-in momentum_b200/lib/libmomentum_b200.so (hand-written sm_100a kernels). There is no CPU fallback:
-if the library or a B200 is missing, construction raises.
+in momentum_b200/lib/libmomentum_b200.so (hand-written sm_90a kernels). There is no CPU fallback:
+if the library or an H100 (sm_90) is missing, construction raises.
 """
 from __future__ import annotations
 
@@ -485,7 +485,7 @@ class GaussNewtonSolver(_Base):
                 "strip_floats", "gram_macs", "gram_pairs", "fused_groups"]
         return dict(zip(keys, (int(v) for v in st)))
 
-    FUSED_PHASES = ["fetch", "joint_parameters", "fk", "units", "cells", "gram", "tiles_from_tmem", "chol_diag", "chol_panel", "chol_update",
+    FUSED_PHASES = ["fetch", "joint_parameters", "fk", "units", "cells", "gram", "parked_tiles", "chol_diag", "chol_panel", "chol_update",
                     "chol_backward", "update_bookkeeping"]
 
     def get_fused_profile(self):

@@ -5,16 +5,18 @@ The product package momentum_b200 never does.
 """
 from __future__ import annotations
 
+import atexit
 import ctypes as C
 import os
+import shutil
 import subprocess
+import tempfile
 from typing import Optional, Sequence
 
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "liboracle.so")
-_NATIVE_PATH = os.path.join(_HERE, "liboracle_native.so")  # timing arm only, built on the machine that runs it (oracle/Makefile)
 _lib = None
 _native = None
 
@@ -31,12 +33,16 @@ def build(force: bool = False) -> str:
 
 def native_lib():
     """The -march=native / fast-math build for bench.py's CPU arm. Always rebuilt by the process that times it (a copy built on
-    another host may use instructions this one lacks); falls back to the portable checker build if the compile fails."""
+    another host may use instructions this one lacks) into a temporary directory, never into the source tree; falls back to the
+    portable checker build if the compile fails."""
     global _native
     if _native is None:
         try:
-            subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "native"])
-            _native = _bind(C.CDLL(_NATIVE_PATH))
+            tmp = tempfile.mkdtemp(prefix="oracle_native_")
+            atexit.register(shutil.rmtree, tmp, ignore_errors=True)  # the library stays loaded until exit; the directory goes with it
+            path = os.path.join(tmp, "liboracle_native.so")
+            subprocess.check_call(["make", "-C", _HERE, "-s", "-B", f"NATIVE_OUT={path}", "native"])
+            _native = _bind(C.CDLL(path))
             _native.is_native = True
         except Exception as e:  # noqa: BLE001
             print(f"[oracle] native build unavailable ({e}); timing the portable build", flush=True)

@@ -10,7 +10,7 @@
 // be compiled in this image (Eigen 5, ms-gsl, fmt, spdlog, dispenso absent), so Eigen's small-matrix
 // and quaternion formulas are restated below (each tagged "Eigen:").
 //
-// Every function cites the reference file:line it follows (paths relative to /root/reference/momentum).
+// Every function cites the reference file:line it follows (paths relative to the momentum/ directory of the momentum repository).
 #pragma once
 
 #include <algorithm>

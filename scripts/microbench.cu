@@ -1,5 +1,5 @@
 // Latency / throughput probes of the instructions the per-instance kernels are built from (one CTA, clock64 around unrolled loops).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -I momentum_b200/csrc -o scratch/microbench scripts/microbench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I momentum_b200/csrc -o scratch/microbench scripts/microbench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "ik_chol_sched.cuh"

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Per-kernel SASS census of the shipped library: `cuobjdump -sass` of momentum_b200/lib/libmomentum_b200.so reduced to the mnemonics
-that say which hardware path a kernel uses (HMMA = mma.sync tensor cores, UTC*MMA / LDTM / STTM = tcgen05 + TMEM, UTMALDG / UBLKCP = TMA
+that say which hardware path a kernel uses (HMMA = mma.sync tensor cores, HGMMA = wgmma, UTMALDG / UBLKCP = TMA
 tensor / bulk copies, STL / LDL = local-memory spills) plus registers and instruction count. Runs without a GPU.
 
-    python scripts/sass_census.py > profiles/sass_r02.txt
+    python scripts/sass_census.py
 """
 import collections
 import os
@@ -13,7 +13,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "momentum_b200", "lib", "libmomentum_b200.so")
-WATCH = ["HMMA", "UTCHMMA", "UTCQMMA", "UTCIMMA", "UTCOMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "FFMA", "FMUL", "FADD", "MUFU", "LOP3", "IADD3", "IMAD", "SHFL", "LDS", "STS",
+WATCH = ["HMMA", "HGMMA", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "FFMA", "FMUL", "FADD", "MUFU", "LOP3", "IADD3", "IMAD", "SHFL", "LDS", "STS",
          "LDG", "STG", "LDL", "STL", "BAR", "LDSM", "REDUX", "ATOM", "RED", "DFMA", "DADD", "DMUL", "F2F", "F2FP"]
 
 
@@ -50,8 +50,8 @@ def main():
             kernels[cur][m.group(1)] += 1
             kernels[cur]["_total"] += 1
     names = demangle(list(kernels))
-    print(f"SASS census of {os.path.relpath(LIB, ROOT)} (cuobjdump -sass; sm_100a). Static instruction counts per kernel.")
-    print("HMMA = mma.sync (legacy tensor path); UTC*MMA + LDTM/STTM = tcgen05 + TMEM; UTMALDG = TMA tensor copy; UBLKCP = cp.async.bulk; STL/LDL = spills.\n")
+    print(f"SASS census of {os.path.relpath(LIB, ROOT)} (cuobjdump -sass; sm_90a). Static instruction counts per kernel.")
+    print("HMMA = mma.sync; HGMMA = wgmma (warpgroup tensor path); UTMALDG = TMA tensor copy; UBLKCP = cp.async.bulk; STL/LDL = spills.\n")
     for k, c in kernels.items():
         short = re.sub(r"\(anonymous namespace\)::", "", names[k])
         short = re.sub(r"\(.*", "", short)

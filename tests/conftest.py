@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on a B200)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on an H100)")
 
 
 def _usable_devices():
@@ -24,11 +24,11 @@ def _usable_devices():
 
 
 def pytest_collection_modifyitems(config, items):
-    """A plain `pytest tests` on a box without an sm_100 device skips the gpu tests instead of failing them; `-m gpu` on a GPU
+    """A plain `pytest tests` on a box without an sm_90 device skips the gpu tests instead of failing them; `-m gpu` on a GPU
     box runs them (and fails loudly if the extension is missing there: the skip only applies when no device is usable)."""
     gpu_items = [it for it in items if it.get_closest_marker("gpu") is not None]
     if not gpu_items or _usable_devices() > 0:
         return
-    skip = pytest.mark.skip(reason="no usable sm_100 CUDA device (momentum_b200 has no CPU fallback)")
+    skip = pytest.mark.skip(reason="no usable sm_90 CUDA device (momentum_b200 has no CPU fallback)")
     for it in gpu_items:
         it.add_marker(skip)

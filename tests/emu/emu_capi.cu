@@ -3,7 +3,7 @@
 // It exports the subset of include/momentum_b200.h that the parity tests use, but runs the
 // __host__ __device__ building blocks of momentum_b200/csrc (ik_device.cuh, ik_chol.cuh) and the real
 // planner (ik_plan.cpp) lane by lane on the CPU. Purpose: catch planner / indexing / semantics bugs
-// in this GPU-less container before spending B200 time. It is not part of the product library and
+// in this GPU-less container before spending GPU time. It is not part of the product library and
 // nothing in momentum_b200/ loads it.
 #include <cfloat>
 #include <cmath>

@@ -28,7 +28,7 @@ def test_header_symbols_exported(lib):
 
 
 def test_no_cpu_fallback_without_device(lib):
-    """Without a usable sm_100 device every compute entry point must fail loudly (no CPU path)."""
+    """Without a usable sm_90 device every compute entry point must fail loudly (no CPU path)."""
     import numpy as np
     import torch
 
@@ -38,7 +38,7 @@ def test_no_cpu_fallback_without_device(lib):
 
     lib.mb2_device_count.restype = ctypes.c_int
     assert lib.mb2_device_count() == 0
-    with pytest.raises(ms.MomentumB200Error, match="no usable sm_100 CUDA device|cuda"):
+    with pytest.raises(ms.MomentumB200Error, match="no usable sm_90 CUDA device|cuda"):
         ms.DeviceCharacter(mc.create_test_character(3))
 
 

@@ -51,7 +51,7 @@ def test_humanoid_single_iteration():
 @pytest.mark.parametrize("mode,rtol", [(ms.JTJ_TF32X3, 2e-5), (ms.JTJ_TF32, 5e-3)])
 @pytest.mark.parametrize("case", ["humanoid", "chain22", "chain_all_families", "subset", "bodyhands", "bodyhands_subset"])
 def test_jtj_tensor_core_modes(case, mode, rtol):
-    """tcgen05 JtJ (3xTF32 split: fp32-class; single TF32: ~1e-3) vs the float oracle's getJtJR."""
+    """wgmma JtJ (3xTF32 split: fp32-class; single TF32: ~1e-3) vs the float oracle's getJtJR."""
     enabled = None
     if case.startswith("bodyhands"):  # cfg4 shape: 425 operand rows -> four row tiles, six work items (two with a separate A box), m = 600
         ch, efs, theta0, theta_star = bodyhands_problem(5)
@@ -80,15 +80,15 @@ def test_solve_with_tensor_core_jtj_matches_oracle():
     print("max rel param diff (3xTF32 JtJ)", worst)
 
 
-def test_cfg4_solve_on_the_dense_tcgen05_jtj():
-    """BASELINE configs[3] "full JtJ tensor-core path": bodyhands300 (n = 424) with the dense tcgen05 JtJ (3xTF32) feeding the
+def test_cfg4_solve_on_the_dense_wgmma_jtj():
+    """BASELINE configs[3] "full JtJ tensor-core path": bodyhands300 (n = 424) with the dense wgmma JtJ (3xTF32) feeding the
     tile-scheduled Cholesky, against the oracle and against the default tile-sparse path."""
     ch, efs, theta0, _ = bodyhands_problem(8)
     opts = ms.GaussNewtonSolverOptions(min_iterations=10, max_iterations=10, threshold=1.0, regularization=0.05, jtj_mode=ms.JTJ_TF32X3)
     out, worst = parity.check_solve(ch, efs, theta0, opts, instances=range(0, 8, 3), param_tol=2e-4)
     ref = ms.GaussNewtonSolver(ms.GaussNewtonSolverOptions(min_iterations=10, max_iterations=10, threshold=1.0, regularization=0.05), parity.build_function(ch, efs, 8)).solve(theta0)
     assert np.all(out["status"] == 0) and np.max(np.abs(out["params"] - ref["params"])) <= 2e-3
-    print("cfg4 on the dense tcgen05 JtJ: max rel param diff vs oracle", worst)
+    print("cfg4 on the dense wgmma JtJ: max rel param diff vs oracle", worst)
 
 
 def test_plane_and_model_parameters_error_functions():
@@ -268,8 +268,8 @@ def test_cfg2_cfg3_humanoid_converged_parameters(orientation):
     # cfg2 (24 Position, m=72) / cfg3 (+6 Orientation, m=126) at a size the oracle finishes in seconds
     # Every one of the 96 instances is compared at the stated 1e-4 against the FLOAT oracle. These under-determined problems (m < n)
     # are still creeping along their weakly constrained directions after 50 damped iterations, and on a few of them float rounding
-    # alone moves the reference by ~1e-4 (scripts/parity_survey.py, profiles/r02s_parity_survey.txt): such an instance must be as close to
-    # the DOUBLE oracle as the reference's float build is, and at most 8 of the 96 may need that second look (measured: 2 / 6).
+    # alone moves the reference by ~1e-4 (scripts/parity_survey.py): such an instance must be as close to
+    # the DOUBLE oracle as the reference's float build is, and at most 8 of the 96 may need that second look.
     B = 96
     ch, efs, theta0, _ = humanoid_problem(B, orientation=orientation)
     opts = ms.GaussNewtonSolverOptions(min_iterations=1, max_iterations=50, threshold=1.0, regularization=0.05)
@@ -316,7 +316,7 @@ def test_cfg5_mixed_rigs_on_concurrent_streams():
 @pytest.mark.parametrize("case", ["cfg3", "cfg2_odd_batch", "chain_all_families", "subset"])
 def test_fused_kernels_match_the_three_kernel_path(case):
     """Gram + Cholesky in one launch (the default on the tile path) and the persistent whole-solve kernel run the same device functions
-    as the three-kernel path. Gram + Cholesky is bit-identical to it (same code, only the tile hand-off differs: TMEM instead of HBM);
+    as the three-kernel path. Gram + Cholesky is bit-identical to it (same code, only the tile hand-off differs: shared memory instead of HBM);
     the persistent kernel agrees to float rounding (its sweep is compiled in another context: different FMA contraction)."""
     enabled, kw = None, dict(min_iterations=6, max_iterations=6)
     if case == "cfg3":

@@ -57,9 +57,8 @@ def test_mixed_batch_matches_the_oracle_instance_by_instance():
     assert np.all(out["status"] == 0) and np.all(out["iterations"] == 8)
     # Every instance is judged against the reference's float AND double builds on the same inputs: a 22-joint chain that starts far from
     # its targets amplifies rounding several hundred times per iteration, so on this mix the reference's own float result is more than
-    # 1e-4 away from its double result on about a third of the instances (scripts/mixed_survey.py on a B200: reference float-vs-double
-    # median 6.7e-5 / p90 7.4e-4, CUDA-vs-double median 3.3e-5 / p90 7.0e-4; the op-for-op fp32 SIMT + Eigen-structured LLT path misses
-    # 1e-4 against the float oracle on 15 of 64 as well). The rule: an instance either agrees with the float oracle to 2e-4 / 1e-3 in the
+    # 1e-4 away from its double result on about a third of the instances (scripts/mixed_survey.py
+    # measures both the reference's float-vs-double gap and the CUDA-vs-double distance on this mix). The rule: an instance either agrees with the float oracle to 2e-4 / 1e-3 in the
     # objective, or (second look) it stays within 4x the reference's own reproducibility on that instance - its float-vs-double gap and
     # its spread under 2^-21 relative perturbations of the targets (the size of the 3xTF32 rounding, include/momentum_b200.h) - and, over
     # the batch, the CUDA results are not farther from the exact (double) answers than the reference's float build is.
