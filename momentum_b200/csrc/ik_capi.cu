@@ -109,11 +109,8 @@ struct mb2_character {
 struct DeviceSchedule {
   CholSchedule host;
   CholSchedDev dev{};
-  bool valid{false};
-  bool dense{false};
   DeviceBuffer<int32_t> blob;
-  GramPlan gram;          // tile-sparse Gram tables of the same plan (rows aligned to quads)
-  bool gramValid{false};
+  GramPlan gram;          // tile-sparse Gram tables of the same plan (rows aligned to quads), when the plan has strips
   DeviceBuffer<int32_t> gBlob;
   int32_t gBlobInts{0}, gOffsets[8]{};
   // fused persistent kernel (ik_fused.cuh): every table of the plan as one blob + how many instance groups fit beside it
@@ -126,10 +123,7 @@ struct mb2_solver_function {
   const mb2_character* ch{nullptr};
   int B{0};
   cudaStream_t stream{nullptr};
-  std::vector<HostErrorFunction> efs;
-  std::vector<uint8_t> enabled;
-  int targetStride{0}, numWeights{0};
-  bool weightsPerInstance{false};
+  HostFunction host;
   bool planDirty{true};
   int planMode{0};        // 0 full columns (API parity), 1 solver: enabled columns in natural order, 2 solver: elimination order + tile schedule
   bool planSchedDense{false};
@@ -147,7 +141,6 @@ struct mb2_solver_function {
   // device data
   DeviceBuffer<float> dTargets, dWeights, dJ, dTheta, dState, dH, dTargetStage;
   DeviceBuffer<double> dErrors;
-  std::vector<float> hWeights; // shared weights mirror
   std::unique_ptr<DeviceSchedule> sched; // Cholesky schedule of the current (compact) plan
   FunctionTables tables() const;
 };
@@ -213,17 +206,17 @@ FunctionTables mb2_solver_function::tables() const {
   T.cells = dCells.p;
   T.contribs = dContribs.p;
   T.limitData = dLimitData.p;
-  T.targetStride = targetStride;
+  T.targetStride = host.targetStride;
   T.recStride = plan.recStride;
   T.numRows = plan.numRows;
   T.ldJ = ldJ;
   T.numCols = plan.numCols;
-  T.weightsPerInstance = weightsPerInstance ? 1 : 0;
-  T.numWeights = numWeights;
+  T.weightsPerInstance = host.weightsPerInstance ? 1 : 0;
+  T.numWeights = host.numWeights;
   T.ptNnz = int(h.ptInner.size());
   T.numContribs = int(plan.contribs.size());
   T.numLimitData = int(plan.limitData.size());
-  const bool strips = planMode == 2 && planAlignRows && sched && sched->gramValid;
+  const bool strips = planMode == 2 && planAlignRows && sched;
   T.stripMode = strips ? 1 : 0;
   T.residOff = strips ? sched->gram.residOff : 0;
   T.jacobianStride = strips ? size_t(sched->gram.stride) : size_t(plan.numCols + 1) * ldJ;
@@ -259,7 +252,7 @@ int requireDevice(int device) {
 }
 
 int ensureTargets(mb2_solver_function* f) {
-  const size_t need = size_t(f->B) * std::max(f->targetStride, 1);
+  const size_t need = size_t(f->B) * std::max(f->host.targetStride, 1);
   if (f->dTargets.n < need) {
     DeviceBuffer<float> old;
     std::swap(old.p, f->dTargets.p);
@@ -274,33 +267,11 @@ int ensureTargets(mb2_solver_function* f) {
 }
 
 int uploadWeights(mb2_solver_function* f) {
-  if (!f->weightsPerInstance) {
-    std::vector<float> w = f->hWeights;
+  if (!f->host.weightsPerInstance) {
+    std::vector<float> w = f->host.weights;
     if (w.empty()) w.push_back(0.f);
     MB2_CUDA(f->dWeights.upload(w, f->stream));
   }
-  return MB2_OK;
-}
-
-// depth (in the joint tree) of the deepest joint each enabled parameter drives: tie-break priority of the elimination order
-static std::vector<int> columnDepthPriority(const HostCharacter& h, const std::vector<int32_t>& enabledList) {
-  std::vector<int> jointDepth(h.numJoints, 0);
-  for (int j = 0; j < h.numJoints; ++j) { int d = 0; for (int a = h.parent[j]; a >= 0; a = h.parent[a]) ++d; jointDepth[j] = d; }
-  std::vector<int> paramDepth(h.numParams, 0);
-  for (int r = 0; r < kParametersPerJoint * h.numJoints; ++r)
-    for (int k = h.ptOuter[r]; k < h.ptOuter[r + 1]; ++k) paramDepth[h.ptInner[k]] = std::max(paramDepth[h.ptInner[k]], jointDepth[r / kParametersPerJoint]);
-  std::vector<int> prio(enabledList.size());
-  for (size_t a = 0; a < enabledList.size(); ++a) prio[a] = paramDepth[enabledList[a]];
-  return prio;
-}
-
-int uploadSchedule(mb2_solver_function* f, std::unique_ptr<DeviceSchedule>& ds) {
-  std::vector<int32_t> blob;
-  CholSchedDev hostView;
-  makeScheduleBlob(ds->host, blob, hostView);
-  MB2_CUDA(ds->blob.upload(blob, f->stream));
-  ds->dev = rebaseSchedule(hostView, ds->blob.p);
-  ds->valid = true;
   return MB2_OK;
 }
 
@@ -348,7 +319,7 @@ int buildFusedBlob(mb2_solver_function* f, DeviceSchedule& ds, const std::vector
 // Modes 0 and 1 coincide when every parameter is enabled.
 int ensurePlan(mb2_solver_function* f, int mode, bool schedDense = false, bool alignRows = false) {
   bool allEnabled = true;
-  for (uint8_t e : f->enabled) allEnabled = allEnabled && e;
+  for (uint8_t e : f->host.enabled) allEnabled = allEnabled && e;
   if (allEnabled && mode == 1) mode = 0;
   if (mode != 2) alignRows = false;
   if (!f->planDirty && f->planLimitsVersion == f->ch->limitsVersion && f->planMode == mode && (mode != 2 || (f->planSchedDense == schedDense && f->planAlignRows == alignRows)))
@@ -356,44 +327,26 @@ int ensurePlan(mb2_solver_function* f, int mode, bool schedDense = false, bool a
   MB2_DEVICE_GUARD(f->ch->device);
   cudaStream_t s = f->stream;
   f->sched.reset();
-  std::string err = buildPlan(f->ch->host, f->efs, f->enabled, mode != 0, f->plan);
-  if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
+  std::unique_ptr<DeviceSchedule> ds;
+  std::string err;
   if (mode == 2) {
-    auto ds = std::make_unique<DeviceSchedule>();
-    const int ns = f->plan.numCols;
-    std::vector<std::vector<int>> cliques(f->plan.units.size());
-    for (const CellDesc& c : f->plan.cells) cliques[c.unit].push_back(int(c.col));
-    const std::vector<int> prio = columnDepthPriority(f->ch->host, f->plan.enabledList);
-    err = buildCholSchedule(ns, cliques, schedDense, ds->host, &prio);
-    if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
-    // re-plan with the device columns in elimination order (tile starts aligned to 4 columns), the schedule expressed in them
-    std::vector<int32_t> colOrder;
-    layoutDeviceColumns(ds->host, colOrder);
-    for (int32_t& c : colOrder) if (c >= 0) c = f->plan.enabledList[c];
-    err = buildPlan(f->ch->host, f->efs, f->enabled, true, f->plan, &colOrder, alignRows);
-    if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
+    ds = std::make_unique<DeviceSchedule>();
+    err = planSolverPath(f->ch->host, f->host.efs, f->host.enabled, schedDense, alignRows, f->plan, ds->host, ds->gram);
+  } else {
+    err = buildPlan(f->ch->host, f->host.efs, f->host.enabled, mode != 0, f->plan);
+  }
+  if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
+  if (ds) {
+    std::vector<int32_t> sblob, gblob;
+    CholSchedDev hostView;
+    makeScheduleBlob(ds->host, sblob, hostView);
+    MB2_CUDA(ds->blob.upload(sblob, s));
+    ds->dev = rebaseSchedule(hostView, ds->blob.p);
     if (alignRows) {
-      std::vector<int32_t> cr0, crn, cc;
-      for (const CellDesc& c : f->plan.cells) { cr0.push_back(f->plan.units[c.unit].row0); crn.push_back(f->plan.units[c.unit].numRows); cc.push_back(int32_t(c.col)); }
-      err = buildGramPlan(ds->host, cr0, crn, cc, f->plan.numRows, ds->gram);
-      if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
-      for (size_t i = 0; i < f->plan.cells.size(); ++i) { f->plan.cells[i].stripOff = ds->gram.cellStripOff[i]; f->plan.cells[i].quadStride = ds->gram.cellQuadStride[i]; }
-      std::vector<int32_t> gblob;
       makeGramBlob(ds->gram, ds->host, gblob, ds->gOffsets);
       ds->gBlobInts = int32_t(gblob.size());
       MB2_CUDA(ds->gBlob.upload(gblob, s));
-      ds->gramValid = true;
-    }
-    ds->dense = schedDense;
-    int rc = uploadSchedule(f, ds);
-    if (rc != MB2_OK) return rc;
-    if (alignRows) {
-      std::vector<int32_t> gblob2, sblob;
-      int32_t goff[8];
-      makeGramBlob(ds->gram, ds->host, gblob2, goff);
-      CholSchedDev hostView;
-      makeScheduleBlob(ds->host, sblob, hostView);
-      rc = buildFusedBlob(f, *ds, gblob2, sblob, s);
+      const int rc = buildFusedBlob(f, *ds, gblob, sblob, s);
       if (rc != MB2_OK) return rc;
     }
     f->sched = std::move(ds);
@@ -424,12 +377,10 @@ int ensurePlan(mb2_solver_function* f, int mode, bool schedDense = false, bool a
   if (rc != MB2_OK) return rc;
   rc = uploadWeights(f);
   if (rc != MB2_OK) return rc;
-  if (stripLayout && f->sched) {
+  if (stripLayout) {
     int dev = 0, optin = 0;
     MB2_CUDA(cudaGetDevice(&dev));
     MB2_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    f->planMode = mode; // tables() reads the mode
-    f->planAlignRows = alignRows;
     f->sched->fConfig = fusedConfigure(f->tables(), f->sched->fLayout, f->sched->dev, f->sched->gram.stride, int(f->sched->gram.tileOrder.size()) / kGramWarps, optin);
   }
   // Plan tables, schedule / Gram blobs, weights and the Jacobian zero fill were issued on the handle's stream; the solve may run on a
@@ -455,19 +406,12 @@ SweepArgs sweepArgs(mb2_solver_function* f, const float* theta, const int32_t* a
   return a;
 }
 
-int addBlock(mb2_solver_function* f, HostErrorFunction& ef, int32_t* outIndex) {
-  const bool hasWeights = ef.kind <= 2 || ef.kind == 5;
-  if (hasWeights && f->weightsPerInstance) return fail(MB2_ERR_UNSUPPORTED, "add all error functions before setting per-instance constraint weights");
-  ef.targetOff = f->targetStride;
-  ef.weightOff = f->numWeights;
-  f->targetStride += ef.targetSize;
-  if (hasWeights) {
-    f->numWeights += ef.numConstraints();
-    f->hWeights.insert(f->hWeights.end(), ef.weights.begin(), ef.weights.end());
-  }
-  f->efs.push_back(ef);
+// buildError: what the block's constructor said about the C-ABI arguments ef was built from
+int addBlock(mb2_solver_function* f, const std::string& buildError, const HostErrorFunction& ef, int32_t* outIndex) {
+  if (!buildError.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, buildError);
+  const std::string err = f->host.add(ef, outIndex);
+  if (!err.empty()) return fail(MB2_ERR_UNSUPPORTED, err);
   f->planDirty = true;
-  if (outIndex) *outIndex = int32_t(f->efs.size()) - 1;
   return MB2_OK;
 }
 
@@ -576,24 +520,11 @@ void mb2_default_gauss_newton_options(mb2_gauss_newton_options* o) {
 
 int mb2_character_create(int device, int32_t J, const int32_t* parents, const float* offsets, const float* prerot, int32_t n,
                          const int32_t* outer, const int32_t* inner, const float* vals, const float* ptoffsets, mb2_character** out) {
-  MB2_CHECK(out != nullptr && parents && offsets && prerot && outer && ptoffsets, "null argument");
-  MB2_CHECK(J > 0 && n > 0, "numJoints and numModelParameters must be positive");
+  MB2_CHECK(out != nullptr, "null argument");
   auto c = std::make_unique<mb2_character>();
   HostCharacter& h = c->host;
-  h.numJoints = J;
-  h.numParams = n;
-  h.parent.assign(parents, parents + J);
-  h.offset.assign(offsets, offsets + 3 * J);
-  h.prerot.assign(prerot, prerot + 4 * J);
-  h.ptOuter.assign(outer, outer + 7 * J + 1);
-  const int nnz = outer[7 * J];
-  MB2_CHECK(nnz >= 0 && (nnz == 0 || (inner && vals)), "parameter transform nnz invalid");
-  h.ptInner.assign(inner, inner + nnz);
-  h.ptVals.assign(vals, vals + nnz);
-  h.ptOffsets.assign(ptoffsets, ptoffsets + 7 * J);
-  const std::string err = h.validate();
+  const std::string err = makeCharacter(J, parents, offsets, prerot, n, outer, inner, vals, ptoffsets, h);
   if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
-  h.buildLevels();
   MB2_DEVICE_GUARD(device);
   int rc = requireDevice(device);
   if (rc != MB2_OK) return rc;
@@ -613,17 +544,9 @@ int mb2_character_create(int device, int32_t J, const int32_t* parents, const fl
 }
 
 int mb2_character_set_parameter_limits(mb2_character* c, int32_t count, const mb2_parameter_limit* limits) {
-  MB2_CHECK(c != nullptr && count >= 0 && (count == 0 || limits), "invalid limits");
-  c->host.limits.clear();
-  for (int i = 0; i < count; ++i) {
-    HostLimit l;
-    l.type = limits[i].type;
-    l.weight = limits[i].weight;
-    std::memcpy(l.i, limits[i].i, sizeof(l.i));
-    std::memcpy(l.f, limits[i].f, sizeof(l.f));
-    MB2_CHECK(l.type >= 0 && l.type <= 6, "Unknown parameter type for joint limit");
-    c->host.limits.push_back(l);
-  }
+  MB2_CHECK(c != nullptr, "invalid limits");
+  const std::string err = setParameterLimits(c->host, count, limits);
+  if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
   c->limitsVersion++;
   return MB2_OK;
 }
@@ -639,7 +562,7 @@ int mb2_solver_function_create(const mb2_character* c, int32_t batch, mb2_solver
   auto f = std::make_unique<mb2_solver_function>();
   f->ch = c;
   f->B = batch;
-  f->enabled.assign(c->host.numParams, 1); // all parameters enabled by default (skeleton_error_function.h:27)
+  f->host.enabled.assign(c->host.numParams, 1); // all parameters enabled by default (skeleton_error_function.h:27)
   MB2_CUDA(cudaStreamCreateWithFlags(&f->stream, cudaStreamNonBlocking));
   *out = f.release();
   return MB2_OK;
@@ -671,171 +594,85 @@ int mb2_character_clone(const mb2_character* c, int device, mb2_character** out)
 int mb2_solver_function_clone(const mb2_solver_function* f, const mb2_character* c, int32_t batch, mb2_solver_function** out) {
   MB2_CHECK(f != nullptr && c != nullptr && out != nullptr, "null argument");
   MB2_CHECK(c->host.numJoints == f->ch->host.numJoints && c->host.numParams == f->ch->host.numParams, "clone target character has a different shape");
-  MB2_CHECK(!f->weightsPerInstance, "a function with per-instance constraint weights cannot be cloned (set them on the clone)");
+  MB2_CHECK(!f->host.weightsPerInstance, "a function with per-instance constraint weights cannot be cloned (set them on the clone)");
   mb2_solver_function* g = nullptr;
   int rc = mb2_solver_function_create(c, batch, &g);
   if (rc != MB2_OK) return rc;
-  g->efs = f->efs;
-  g->enabled = f->enabled;
-  g->targetStride = f->targetStride;
-  g->numWeights = f->numWeights;
-  g->hWeights = f->hWeights;
+  g->host = f->host;
   g->planDirty = true;
   *out = g;
   return MB2_OK;
 }
 int mb2_character_device(const mb2_character* c) { return c ? c->device : -1; }
 const mb2_character* mb2_solver_function_character(const mb2_solver_function* f) { return f ? f->ch : nullptr; }
-int32_t mb2_solver_function_num_error_functions(const mb2_solver_function* f) { return f ? int32_t(f->efs.size()) : 0; }
+int32_t mb2_solver_function_num_error_functions(const mb2_solver_function* f) { return f ? int32_t(f->host.efs.size()) : 0; }
 int32_t mb2_solver_function_target_size(const mb2_solver_function* f, int32_t index) {
-  return (f && index >= 0 && index < int32_t(f->efs.size())) ? f->efs[index].targetSize : -1;
+  return (f && index >= 0 && index < int32_t(f->host.efs.size())) ? f->host.efs[index].targetSize : -1;
 }
 
 int32_t mb2_solver_function_num_parameters(const mb2_solver_function* f) { return f ? f->ch->host.numParams : 0; }
 int32_t mb2_solver_function_batch(const mb2_solver_function* f) { return f ? f->B : 0; }
-int32_t mb2_solver_function_actual_parameters(const mb2_solver_function* f) {
-  if (!f) return 0;
-  int ap = 0;
-  for (int i = 0; i < f->ch->host.numParams; ++i) if (f->enabled[i]) ap = i + 1;
-  return ap;
-}
-int32_t mb2_solver_function_jacobian_rows(const mb2_solver_function* f) {
-  if (!f) return 0;
-  int total = 0;
-  for (const auto& ef : f->efs) if (ef.weight > 0.f) total += jacobianBlockSize(f->ch->host, ef);
-  return roundUp(total, 8); // padToSimdAlignment (solver_function.h:27-29)
-}
-int32_t mb2_solver_function_jacobian_stride(const mb2_solver_function* f) {
-  if (!f) return 0;
-  int total = 0;
-  for (const auto& ef : f->efs) if (ef.weight > 0.f) total += jacobianBlockSize(f->ch->host, ef);
-  return std::max(32, roundUp(total, 32));
-}
+int32_t mb2_solver_function_actual_parameters(const mb2_solver_function* f) { return f ? f->host.actualParameters() : 0; }
+int32_t mb2_solver_function_jacobian_rows(const mb2_solver_function* f) { return f ? f->host.jacobianRows(f->ch->host) : 0; }
+int32_t mb2_solver_function_jacobian_stride(const mb2_solver_function* f) { return f ? f->host.jacobianStride(f->ch->host) : 0; }
 
 int mb2_add_position_error_function(mb2_solver_function* f, float weight, float alpha, float c, int32_t nc, const int32_t* parents,
                                     const float* offsets, const float* weights, int32_t* outIndex) {
-  MB2_CHECK(f != nullptr && nc >= 0 && (nc == 0 || (parents && offsets && weights)), "invalid position constraints");
-  MB2_CHECK(c > 0.f, "Parameter c should be positive"); // generalized_loss.cpp:83
+  MB2_CHECK(f != nullptr, "null solver function");
   HostErrorFunction ef;
-  ef.kind = 0;
-  ef.weight = weight;
-  ef.lossAlpha = alpha;
-  ef.lossC = c;
-  ef.parents.assign(parents, parents + nc);
-  for (int p : ef.parents) MB2_CHECK(p >= 0 && p < f->ch->host.numJoints, "constraint parent joint out of range");
-  ef.offsets.assign(offsets, offsets + 3 * size_t(nc));
-  ef.weights.assign(weights, weights + nc);
-  ef.targetSize = 3 * nc;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, positionErrorFunction(f->ch->host, weight, alpha, c, nc, parents, offsets, weights, ef), ef, outIndex);
 }
 
 int mb2_add_position_error_function_instanced(mb2_solver_function* f, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* weights,
                                               int32_t* outIndex) {
-  MB2_CHECK(f != nullptr && nc >= 0 && (nc == 0 || (parents && weights)), "invalid position constraints");
-  MB2_CHECK(c > 0.f, "Parameter c should be positive");
+  MB2_CHECK(f != nullptr, "null solver function");
   HostErrorFunction ef;
-  ef.kind = 0;
-  ef.weight = weight;
-  ef.lossAlpha = alpha;
-  ef.lossC = c;
-  ef.instanceOffsets = true;
-  ef.parents.assign(parents, parents + nc);
-  for (int p : ef.parents) MB2_CHECK(p >= 0 && p < f->ch->host.numJoints, "constraint parent joint out of range");
-  ef.offsets.assign(3 * size_t(nc), 0.f);
-  ef.weights.assign(weights, weights + nc);
-  ef.targetSize = 6 * nc;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, instancedPositionErrorFunction(f->ch->host, weight, alpha, c, nc, parents, weights, ef), ef, outIndex);
 }
 
 int mb2_add_plane_error_function(mb2_solver_function* f, float weight, float alpha, float c, int32_t above, int32_t nc, const int32_t* parents,
                                  const float* offsets, const float* weights, int32_t* outIndex) {
-  MB2_CHECK(f != nullptr && nc >= 0 && (nc == 0 || (parents && offsets && weights)), "invalid plane constraints");
-  MB2_CHECK(c > 0.f, "Parameter c should be positive");
+  MB2_CHECK(f != nullptr, "null solver function");
   HostErrorFunction ef;
-  ef.kind = 5;
-  ef.weight = weight;
-  ef.lossAlpha = alpha;
-  ef.lossC = c;
-  ef.halfPlane = above != 0;
-  ef.parents.assign(parents, parents + nc);
-  for (int p : ef.parents) MB2_CHECK(p >= 0 && p < f->ch->host.numJoints, "constraint parent joint out of range");
-  ef.offsets.assign(offsets, offsets + 3 * size_t(nc));
-  ef.weights.assign(weights, weights + nc);
-  ef.targetSize = 4 * nc;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, planeErrorFunction(f->ch->host, weight, alpha, c, above, nc, parents, offsets, weights, ef), ef, outIndex);
 }
 
 int mb2_add_model_parameters_error_function(mb2_solver_function* f, float weight, const float* targetWeights, int32_t* outIndex) {
-  MB2_CHECK(f != nullptr && targetWeights != nullptr, "invalid model-parameter weights");
+  MB2_CHECK(f != nullptr, "null solver function");
   HostErrorFunction ef;
-  ef.kind = 6;
-  ef.weight = weight;
-  ef.paramWeights.assign(targetWeights, targetWeights + f->ch->host.numParams);
-  ef.targetSize = f->ch->host.numParams;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, modelParametersErrorFunction(f->ch->host, weight, targetWeights, ef), ef, outIndex);
 }
 
 int mb2_add_orientation_error_function(mb2_solver_function* f, float weight, float alpha, float c, int32_t rotDiff, int32_t nc,
                                        const int32_t* parents, const float* offsets, const float* weights, int32_t* outIndex) {
-  MB2_CHECK(f != nullptr && nc >= 0 && (nc == 0 || (parents && offsets && weights)), "invalid orientation constraints");
-  MB2_CHECK(c > 0.f, "Parameter c should be positive");
+  MB2_CHECK(f != nullptr, "null solver function");
   HostErrorFunction ef;
-  ef.kind = rotDiff ? 2 : 1;
-  ef.weight = weight;
-  ef.lossAlpha = alpha;
-  ef.lossC = c;
-  ef.parents.assign(parents, parents + nc);
-  for (int p : ef.parents) MB2_CHECK(p >= 0 && p < f->ch->host.numJoints, "constraint parent joint out of range");
-  ef.offsets.assign(offsets, offsets + 4 * size_t(nc));
-  for (int i = 0; i < nc; ++i) { // OrientationDataT ctor: offset(inOffset.normalized()) (orientation_error_function.h:33-35)
-    float* q = &ef.offsets[4 * size_t(i)];
-    const float nrm = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    for (int k = 0; k < 4; ++k) q[k] /= nrm;
-  }
-  ef.weights.assign(weights, weights + nc);
-  ef.targetSize = 4 * nc;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, orientationErrorFunction(f->ch->host, weight, alpha, c, rotDiff, nc, parents, offsets, weights, ef), ef, outIndex);
 }
 
 int mb2_add_state_error_function(mb2_solver_function* f, float weight, int32_t rotationErrorType, float posWgt, float rotWgt,
                                  const float* posW, const float* rotW, int32_t* outIndex) {
-  MB2_CHECK(f != nullptr && posW && rotW, "invalid state error function");
-  MB2_CHECK(rotationErrorType == 0 || rotationErrorType == 1, "unknown rotation error type");
+  MB2_CHECK(f != nullptr, "null solver function");
   HostErrorFunction ef;
-  ef.kind = 3;
-  ef.weight = weight;
-  ef.rotationErrorType = rotationErrorType;
-  ef.posWgt = posWgt;
-  ef.rotWgt = rotWgt;
-  const int J = f->ch->host.numJoints;
-  ef.posW.assign(posW, posW + J);
-  ef.rotW.assign(rotW, rotW + J);
-  ef.targetSize = 8 * J;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, stateErrorFunction(f->ch->host, weight, rotationErrorType, posWgt, rotWgt, posW, rotW, ef), ef, outIndex);
 }
 
 int mb2_add_limit_error_function(mb2_solver_function* f, float weight, float alpha, float c, int32_t* outIndex) {
   MB2_CHECK(f != nullptr, "null solver function");
-  MB2_CHECK(c > 0.f, "Parameter c should be positive");
   HostErrorFunction ef;
-  ef.kind = 4;
-  ef.weight = weight;
-  ef.lossAlpha = alpha;
-  ef.lossC = c;
-  ef.targetSize = 0;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, limitErrorFunction(weight, alpha, c, ef), ef, outIndex);
 }
 
 int mb2_set_error_function_weight(mb2_solver_function* f, int32_t index, float weight) {
-  MB2_CHECK(f != nullptr && index >= 0 && index < int(f->efs.size()), "error function index out of range");
-  f->efs[index].weight = weight;
+  MB2_CHECK(f != nullptr && index >= 0 && index < int(f->host.efs.size()), "error function index out of range");
+  f->host.efs[index].weight = weight;
   f->planDirty = true;
   return MB2_OK;
 }
 
 static int setTargetsImpl(mb2_solver_function* f, int32_t index, const float* targets, bool deviceSrc, cudaStream_t st) {
-  MB2_CHECK(f != nullptr && index >= 0 && index < int(f->efs.size()) && targets, "invalid targets");
-  const HostErrorFunction& ef = f->efs[index];
+  MB2_CHECK(f != nullptr && index >= 0 && index < int(f->host.efs.size()) && targets, "invalid targets");
+  const HostErrorFunction& ef = f->host.efs[index];
   if (ef.targetSize == 0 && ef.kind != 4) return MB2_OK; // a block without constraints: nothing to send (setConstraints({}) in the reference)
   MB2_CHECK(ef.targetSize > 0, "this error function has no per-instance targets");
   MB2_DEVICE_GUARD(f->ch->device);
@@ -848,8 +685,8 @@ static int setTargetsImpl(mb2_solver_function* f, int32_t index, const float* ta
     MB2_CUDA(cudaMemcpyAsync(f->dTargetStage.p, targets, size_t(f->B) * ef.targetSize * sizeof(float), cudaMemcpyHostToDevice, st));
     packed = f->dTargetStage.p;
   }
-  MB2_CUDA(launchScatterTargets(packed, dst, ef.targetSize, f->targetStride, f->B, st));
-  if (ef.kind == 1 || ef.kind == 2) MB2_CUDA(launchNormalizeQuats(dst, 0, f->targetStride, ef.numConstraints(), f->B, st));
+  MB2_CUDA(launchScatterTargets(packed, dst, ef.targetSize, f->host.targetStride, f->B, st));
+  if (ef.kind == 1 || ef.kind == 2) MB2_CUDA(launchNormalizeQuats(dst, 0, f->host.targetStride, ef.numConstraints(), f->B, st));
   return MB2_OK;
 }
 int mb2_set_targets(mb2_solver_function* f, int32_t index, const float* targets) {
@@ -865,25 +702,25 @@ int mb2_set_targets_device(mb2_solver_function* f, int32_t index, const float* t
 }
 
 int mb2_set_constraint_weights(mb2_solver_function* f, int32_t index, const float* weights, int32_t perInstance) {
-  MB2_CHECK(f != nullptr && index >= 0 && index < int(f->efs.size()) && weights, "invalid constraint weights");
-  HostErrorFunction& ef = f->efs[index];
+  MB2_CHECK(f != nullptr && index >= 0 && index < int(f->host.efs.size()) && weights, "invalid constraint weights");
+  HostErrorFunction& ef = f->host.efs[index];
   MB2_CHECK(ef.kind <= 2 || ef.kind == 5, "constraint weights apply to Position/Orientation/Plane error functions");
   MB2_DEVICE_GUARD(f->ch->device);
   const int nc = ef.numConstraints();
   if (!perInstance) {
-    MB2_CHECK(!f->weightsPerInstance, "solver function already uses per-instance constraint weights");
+    MB2_CHECK(!f->host.weightsPerInstance, "solver function already uses per-instance constraint weights");
     ef.weights.assign(weights, weights + nc);
-    std::copy(weights, weights + nc, f->hWeights.begin() + ef.weightOff);
+    std::copy(weights, weights + nc, f->host.weights.begin() + ef.weightOff);
     return uploadWeights(f);
   }
-  if (!f->weightsPerInstance) { // expand the shared array to [B][numWeights]
-    std::vector<float> all(size_t(f->B) * f->numWeights);
-    for (int b = 0; b < f->B; ++b) std::copy(f->hWeights.begin(), f->hWeights.end(), all.begin() + size_t(b) * f->numWeights);
+  if (!f->host.weightsPerInstance) { // expand the shared array to [B][numWeights]
+    std::vector<float> all(size_t(f->B) * f->host.numWeights);
+    for (int b = 0; b < f->B; ++b) std::copy(f->host.weights.begin(), f->host.weights.end(), all.begin() + size_t(b) * f->host.numWeights);
     f->dWeights.release();
     MB2_CUDA(f->dWeights.upload(all, f->stream));
-    f->weightsPerInstance = true;
+    f->host.weightsPerInstance = true;
   }
-  MB2_CUDA(cudaMemcpy2DAsync(f->dWeights.p + ef.weightOff, size_t(f->numWeights) * sizeof(float), weights, size_t(nc) * sizeof(float),
+  MB2_CUDA(cudaMemcpy2DAsync(f->dWeights.p + ef.weightOff, size_t(f->host.numWeights) * sizeof(float), weights, size_t(nc) * sizeof(float),
                              size_t(nc) * sizeof(float), f->B, cudaMemcpyHostToDevice, f->stream));
   MB2_CUDA(cudaStreamSynchronize(f->stream));
   return MB2_OK;
@@ -891,30 +728,30 @@ int mb2_set_constraint_weights(mb2_solver_function* f, int32_t index, const floa
 
 // per-instance weights of one block from DEVICE memory [B][nc] (the torch binding's path: no host round trip)
 int mb2_set_constraint_weights_device(mb2_solver_function* f, int32_t index, const float* weights_device, void* stream) {
-  MB2_CHECK(f != nullptr && index >= 0 && index < int(f->efs.size()) && weights_device, "invalid constraint weights");
-  HostErrorFunction& ef = f->efs[index];
+  MB2_CHECK(f != nullptr && index >= 0 && index < int(f->host.efs.size()) && weights_device, "invalid constraint weights");
+  HostErrorFunction& ef = f->host.efs[index];
   MB2_CHECK(ef.kind <= 2 || ef.kind == 5, "constraint weights apply to Position/Orientation/Plane error functions");
   MB2_DEVICE_GUARD(f->ch->device);
   const int nc = ef.numConstraints();
-  if (!f->weightsPerInstance) { // expand the shared array to [B][numWeights]
-    std::vector<float> all(size_t(f->B) * f->numWeights);
-    for (int b = 0; b < f->B; ++b) std::copy(f->hWeights.begin(), f->hWeights.end(), all.begin() + size_t(b) * f->numWeights);
+  if (!f->host.weightsPerInstance) { // expand the shared array to [B][numWeights]
+    std::vector<float> all(size_t(f->B) * f->host.numWeights);
+    for (int b = 0; b < f->B; ++b) std::copy(f->host.weights.begin(), f->host.weights.end(), all.begin() + size_t(b) * f->host.numWeights);
     f->dWeights.release();
     MB2_CUDA(f->dWeights.upload(all, f->stream));
     MB2_CUDA(cudaStreamSynchronize(f->stream));
-    f->weightsPerInstance = true;
+    f->host.weightsPerInstance = true;
     f->planDirty = true; // tables() carries the per-instance flag
   }
   cudaStream_t st = stream ? (cudaStream_t)stream : f->stream;
   if (nc > 0)
-    MB2_CUDA(cudaMemcpy2DAsync(f->dWeights.p + ef.weightOff, size_t(f->numWeights) * sizeof(float), weights_device, size_t(nc) * sizeof(float), size_t(nc) * sizeof(float), f->B,
+    MB2_CUDA(cudaMemcpy2DAsync(f->dWeights.p + ef.weightOff, size_t(f->host.numWeights) * sizeof(float), weights_device, size_t(nc) * sizeof(float), size_t(nc) * sizeof(float), f->B,
                                cudaMemcpyDeviceToDevice, st));
   return MB2_OK;
 }
 
 int mb2_solver_function_set_enabled_parameters(mb2_solver_function* f, const uint64_t* bits) {
   MB2_CHECK(f != nullptr && bits != nullptr, "null argument");
-  bitsToEnabled(bits, f->ch->host.numParams, f->enabled);
+  bitsToEnabled(bits, f->ch->host.numParams, f->host.enabled);
   f->planDirty = true;
   return MB2_OK;
 }
@@ -1055,10 +892,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   NvtxRange nvtxSolve("mb2::SolverT::solve");
   const mb2_gauss_newton_options& o = s->opt;
   // Cholesky path: 0 auto, 1 dense Eigen-structured kernel, 2 tile schedule on the dense pattern, 3 tile schedule on the sparse pattern
-  int numEnabled = 0;
-  for (uint8_t e : f->enabled) numEnabled += e ? 1 : 0;
-  int cholMode = o.cholesky_mode;
-  if (cholMode == 0) cholMode = numEnabled >= 48 ? 3 : 1;
+  int cholMode = resolveCholeskyMode(o.cholesky_mode, f->host.enabled);
   // GaussNewtonSolverQRT's step: Householder QR of the K-major Jacobian (ik_qr.cuh); TrustRegionQRT's iteration builds on the same fold (ik_tr_qr.cuh)
   const bool useTr = o.linear_solver == MB2_LINEAR_SOLVER_TRUST_REGION_QR;
   const bool useQr = o.linear_solver == MB2_LINEAR_SOLVER_QR || useTr;
@@ -1203,7 +1037,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
     }
     std::vector<int32_t> starts{0};
     int r0 = 0, widest = 0;
-    for (const auto& ef : f->efs) {
+    for (const auto& ef : f->host.efs) {
       if (!(ef.weight > 0.f)) continue;
       const int size = jacobianBlockSize(f->ch->host, ef);
       for (int done = 0; done < size; done += qrMaxRows) { const int p = std::min(qrMaxRows, size - done); starts.push_back(r0 + done + p); widest = std::max(widest, p); }
@@ -1503,7 +1337,7 @@ int mb2_solver_get_plan_stats(mb2_solver* s, int64_t stats[12]) {
   const mb2_solver_function* f = s->fn;
   int64_t nnz = 0;
   for (const CellDesc& c : f->plan.cells) nnz += f->plan.units[c.unit].numRows;
-  const bool tiles = f->planMode == 2 && f->sched && f->sched->valid;
+  const bool tiles = f->planMode == 2 && f->sched;
   stats[0] = nnz;
   stats[1] = f->plan.numCols;
   stats[2] = f->ldJ;
@@ -1512,7 +1346,7 @@ int mb2_solver_get_plan_stats(mb2_solver* s, int64_t stats[12]) {
   stats[5] = tiles ? f->sched->host.tileOps : 0;
   stats[6] = tiles ? f->sched->host.numLevels : 0;
   stats[7] = f->plan.numRows;
-  const bool gram = tiles && f->planAlignRows && f->sched->gramValid;
+  const bool gram = tiles && f->planAlignRows;
   stats[8] = gram ? f->sched->gram.stride : 0;
   stats[9] = gram ? f->sched->gram.macs : 0;
   stats[10] = gram ? int64_t(f->sched->gram.pairA.size()) : 0;

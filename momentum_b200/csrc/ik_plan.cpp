@@ -3,6 +3,7 @@
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <cstring>
 #include <map>
 
 namespace mb2 {
@@ -75,6 +76,164 @@ int32_t jacobianBlockSize(const HostCharacter& ch, const HostErrorFunction& ef) 
   }
   return 0;
 }
+
+std::string makeCharacter(int32_t numJoints, const int32_t* parents, const float* offsets, const float* prerot, int32_t numParams, const int32_t* outer,
+                          const int32_t* inner, const float* vals, const float* ptOffsets, HostCharacter& out) {
+  if (!(parents && offsets && prerot && outer && ptOffsets)) return "null argument";
+  if (!(numJoints > 0 && numParams > 0)) return "numJoints and numModelParameters must be positive";
+  const int J = numJoints;
+  out = HostCharacter();
+  out.numJoints = J;
+  out.numParams = numParams;
+  out.parent.assign(parents, parents + J);
+  out.offset.assign(offsets, offsets + 3 * J);
+  out.prerot.assign(prerot, prerot + 4 * J);
+  out.ptOuter.assign(outer, outer + 7 * J + 1);
+  const int nnz = outer[7 * J];
+  if (!(nnz >= 0 && (nnz == 0 || (inner && vals)))) return "parameter transform nnz invalid";
+  out.ptInner.assign(inner, inner + nnz);
+  out.ptVals.assign(vals, vals + nnz);
+  out.ptOffsets.assign(ptOffsets, ptOffsets + 7 * J);
+  const std::string err = out.validate();
+  if (!err.empty()) return err;
+  out.buildLevels();
+  return "";
+}
+
+std::string setParameterLimits(HostCharacter& ch, int32_t count, const mb2_parameter_limit* limits) {
+  if (!(count >= 0 && (count == 0 || limits))) return "invalid limits";
+  ch.limits.clear();
+  for (int i = 0; i < count; ++i) {
+    HostLimit l;
+    l.type = limits[i].type;
+    l.weight = limits[i].weight;
+    std::memcpy(l.i, limits[i].i, sizeof(l.i));
+    std::memcpy(l.f, limits[i].f, sizeof(l.f));
+    if (!(l.type >= 0 && l.type <= 6)) return "Unknown parameter type for joint limit";
+    ch.limits.push_back(l);
+  }
+  return "";
+}
+
+// What Position, Plane and Orientation blocks share: the generalized loss, and the parent joint and weight of each constraint.
+static std::string jointConstraints(const HostCharacter& ch, int32_t kind, float weight, float alpha, float c, int32_t nc, const int32_t* parents,
+                                    const float* weights, HostErrorFunction& ef) {
+  if (!(c > 0.f)) return "Parameter c should be positive"; // generalized_loss.cpp:83
+  ef.kind = kind;
+  ef.weight = weight;
+  ef.lossAlpha = alpha;
+  ef.lossC = c;
+  ef.parents.assign(parents, parents + nc);
+  for (int p : ef.parents)
+    if (p < 0 || p >= ch.numJoints) return "constraint parent joint out of range";
+  ef.weights.assign(weights, weights + nc);
+  return "";
+}
+
+std::string positionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* offsets,
+                                  const float* weights, HostErrorFunction& ef) {
+  if (!(nc >= 0 && (nc == 0 || (parents && offsets && weights)))) return "invalid position constraints";
+  ef.offsets.assign(offsets, offsets + 3 * size_t(nc));
+  ef.targetSize = 3 * nc;
+  return jointConstraints(ch, 0, weight, alpha, c, nc, parents, weights, ef);
+}
+
+std::string instancedPositionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* weights,
+                                           HostErrorFunction& ef) {
+  if (!(nc >= 0 && (nc == 0 || (parents && weights)))) return "invalid position constraints";
+  ef.instanceOffsets = true;
+  ef.offsets.assign(3 * size_t(nc), 0.f);
+  ef.targetSize = 6 * nc;
+  return jointConstraints(ch, 0, weight, alpha, c, nc, parents, weights, ef);
+}
+
+std::string planeErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t above, int32_t nc, const int32_t* parents, const float* offsets,
+                               const float* weights, HostErrorFunction& ef) {
+  if (!(nc >= 0 && (nc == 0 || (parents && offsets && weights)))) return "invalid plane constraints";
+  ef.halfPlane = above != 0;
+  ef.offsets.assign(offsets, offsets + 3 * size_t(nc));
+  ef.targetSize = 4 * nc;
+  return jointConstraints(ch, 5, weight, alpha, c, nc, parents, weights, ef);
+}
+
+std::string modelParametersErrorFunction(const HostCharacter& ch, float weight, const float* targetWeights, HostErrorFunction& ef) {
+  if (targetWeights == nullptr) return "invalid model-parameter weights";
+  ef.kind = 6;
+  ef.weight = weight;
+  ef.paramWeights.assign(targetWeights, targetWeights + ch.numParams);
+  ef.targetSize = ch.numParams;
+  return "";
+}
+
+std::string orientationErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t rotDiff, int32_t nc, const int32_t* parents,
+                                     const float* offsets, const float* weights, HostErrorFunction& ef) {
+  if (!(nc >= 0 && (nc == 0 || (parents && offsets && weights)))) return "invalid orientation constraints";
+  ef.offsets.assign(offsets, offsets + 4 * size_t(nc));
+  for (int i = 0; i < nc; ++i) { // OrientationDataT ctor: offset(inOffset.normalized()) (orientation_error_function.h:33-35)
+    float* q = &ef.offsets[4 * size_t(i)];
+    const float nrm = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+    for (int k = 0; k < 4; ++k) q[k] /= nrm;
+  }
+  ef.targetSize = 4 * nc;
+  return jointConstraints(ch, rotDiff ? 2 : 1, weight, alpha, c, nc, parents, weights, ef);
+}
+
+std::string stateErrorFunction(const HostCharacter& ch, float weight, int32_t rotationErrorType, float posWgt, float rotWgt, const float* posW, const float* rotW,
+                               HostErrorFunction& ef) {
+  if (!(posW && rotW)) return "invalid state error function";
+  if (!(rotationErrorType == 0 || rotationErrorType == 1)) return "unknown rotation error type";
+  ef.kind = 3;
+  ef.weight = weight;
+  ef.rotationErrorType = rotationErrorType;
+  ef.posWgt = posWgt;
+  ef.rotWgt = rotWgt;
+  ef.posW.assign(posW, posW + ch.numJoints);
+  ef.rotW.assign(rotW, rotW + ch.numJoints);
+  ef.targetSize = 8 * ch.numJoints;
+  return "";
+}
+
+std::string limitErrorFunction(float weight, float alpha, float c, HostErrorFunction& ef) {
+  if (!(c > 0.f)) return "Parameter c should be positive";
+  ef.kind = 4;
+  ef.weight = weight;
+  ef.lossAlpha = alpha;
+  ef.lossC = c;
+  ef.targetSize = 0;
+  return "";
+}
+
+std::string HostFunction::add(const HostErrorFunction& block, int32_t* index) {
+  const bool hasWeights = block.kind <= 2 || block.kind == 5;
+  if (hasWeights && weightsPerInstance) return "add all error functions before setting per-instance constraint weights";
+  HostErrorFunction ef = block;
+  ef.targetOff = targetStride;
+  ef.weightOff = numWeights;
+  targetStride += ef.targetSize;
+  if (hasWeights) {
+    numWeights += ef.numConstraints();
+    weights.insert(weights.end(), ef.weights.begin(), ef.weights.end());
+  }
+  efs.push_back(std::move(ef));
+  if (index) *index = int32_t(efs.size()) - 1;
+  return "";
+}
+
+int32_t HostFunction::actualParameters() const {
+  int32_t ap = 0;
+  for (size_t i = 0; i < enabled.size(); ++i)
+    if (enabled[i]) ap = int32_t(i) + 1;
+  return ap;
+}
+
+static int32_t unpaddedRows(const HostCharacter& ch, const std::vector<HostErrorFunction>& efs) {
+  int32_t total = 0;
+  for (const auto& ef : efs)
+    if (ef.weight > 0.f) total += jacobianBlockSize(ch, ef);
+  return total;
+}
+int32_t HostFunction::jacobianRows(const HostCharacter& ch) const { return (unpaddedRows(ch, efs) + 7) / 8 * 8; }
+int32_t HostFunction::jacobianStride(const HostCharacter& ch) const { return std::max(32, (unpaddedRows(ch, efs) + 31) / 32 * 32); }
 
 static EfDesc makeEfDesc(const HostErrorFunction& ef) {
   EfDesc d{};
@@ -444,6 +603,49 @@ std::string buildPlan(const HostCharacter& ch, const std::vector<HostErrorFuncti
     if (a.col != b.col) return a.col < b.col;
     return a.unit < b.unit;
   });
+  return "";
+}
+
+int resolveCholeskyMode(int requested, const std::vector<uint8_t>& enabled) {
+  if (requested != MB2_CHOLESKY_AUTO) return requested;
+  int numEnabled = 0;
+  for (uint8_t e : enabled) numEnabled += e ? 1 : 0;
+  return numEnabled >= 48 ? MB2_CHOLESKY_TILES_SPARSE : MB2_CHOLESKY_DENSE_EIGEN;
+}
+
+// depth (in the joint tree) of the deepest joint each enabled parameter drives: tie-break priority of the elimination order
+static std::vector<int> columnDepthPriority(const HostCharacter& h, const std::vector<int32_t>& enabledList) {
+  std::vector<int> jointDepth(h.numJoints, 0);
+  for (int j = 0; j < h.numJoints; ++j) { int d = 0; for (int a = h.parent[j]; a >= 0; a = h.parent[a]) ++d; jointDepth[j] = d; }
+  std::vector<int> paramDepth(h.numParams, 0);
+  for (int r = 0; r < kParametersPerJoint * h.numJoints; ++r)
+    for (int k = h.ptOuter[r]; k < h.ptOuter[r + 1]; ++k) paramDepth[h.ptInner[k]] = std::max(paramDepth[h.ptInner[k]], jointDepth[r / kParametersPerJoint]);
+  std::vector<int> prio(enabledList.size());
+  for (size_t a = 0; a < enabledList.size(); ++a) prio[a] = paramDepth[enabledList[a]];
+  return prio;
+}
+
+std::string planSolverPath(const HostCharacter& ch, const std::vector<HostErrorFunction>& efs, const std::vector<uint8_t>& enabled, bool densePattern, bool strips,
+                           Plan& plan, CholSchedule& sched, GramPlan& gram) {
+  gram = GramPlan();
+  std::string err = buildPlan(ch, efs, enabled, true, plan);
+  if (!err.empty()) return err;
+  std::vector<std::vector<int>> cliques(plan.units.size());
+  for (const CellDesc& c : plan.cells) cliques[c.unit].push_back(int(c.col));
+  const std::vector<int> prio = columnDepthPriority(ch, plan.enabledList);
+  err = buildCholSchedule(plan.numCols, cliques, densePattern, sched, &prio);
+  if (!err.empty()) return err;
+  // re-plan with the device columns in elimination order (tile starts aligned to 4 columns), the schedule expressed in them
+  std::vector<int32_t> colOrder;
+  layoutDeviceColumns(sched, colOrder);
+  for (int32_t& c : colOrder) if (c >= 0) c = plan.enabledList[c];
+  err = buildPlan(ch, efs, enabled, true, plan, &colOrder, strips);
+  if (!err.empty() || !strips) return err;
+  std::vector<int32_t> cr0, crn, cc;
+  for (const CellDesc& c : plan.cells) { cr0.push_back(plan.units[c.unit].row0); crn.push_back(plan.units[c.unit].numRows); cc.push_back(int32_t(c.col)); }
+  err = buildGramPlan(sched, cr0, crn, cc, plan.numRows, gram);
+  if (!err.empty()) return err;
+  for (size_t i = 0; i < plan.cells.size(); ++i) { plan.cells[i].stripOff = gram.cellStripOff[i]; plan.cells[i].quadStride = gram.cellQuadStride[i]; }
   return "";
 }
 

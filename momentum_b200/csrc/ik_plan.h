@@ -11,6 +11,8 @@
 #include <string>
 #include <vector>
 
+#include "../../include/momentum_b200.h"
+#include "ik_chol_sched.h"
 #include "ik_types.h"
 
 namespace mb2 {
@@ -56,6 +58,41 @@ struct HostErrorFunction {
   int32_t numConstraints() const { return int32_t(parents.size()); }
 };
 
+// The host description of a solver function: its blocks, the per-instance layout of their targets and constraint weights, and the
+// enabled parameters.
+struct HostFunction {
+  std::vector<HostErrorFunction> efs;
+  std::vector<uint8_t> enabled;     // [numParams]
+  int32_t targetStride{0};          // target floats per instance
+  int32_t numWeights{0};            // constraint weights per instance
+  std::vector<float> weights;       // the shared constraint weights [numWeights]
+  bool weightsPerInstance{false};
+  // Appends a block and assigns its target and weight offsets; *index = its position. A block with constraint weights cannot follow
+  // per-instance weights (their [B][numWeights] layout is fixed).
+  std::string add(const HostErrorFunction& ef, int32_t* index);
+  int32_t actualParameters() const;                       // last enabled parameter + 1 (skeleton_solver_function.cpp:45-52)
+  int32_t jacobianRows(const HostCharacter& ch) const;    // getJacobianBlockSize of the blocks with weight > 0, padded to 8 (solver_function.cpp:33-38)
+  int32_t jacobianStride(const HostCharacter& ch) const;  // leading dimension of a K-major device Jacobian column
+};
+
+// ---- Characters and error-function blocks from the C-ABI arrays (mb2_character_*, mb2_add_*_error_function) ----
+// Each returns an empty string when the arguments are accepted, else the message of the first rejected one.
+std::string makeCharacter(int32_t numJoints, const int32_t* parents, const float* offsets, const float* prerot, int32_t numParams, const int32_t* outer,
+                          const int32_t* inner, const float* vals, const float* ptOffsets, HostCharacter& out); // validated, tree levels built
+std::string setParameterLimits(HostCharacter& ch, int32_t count, const mb2_parameter_limit* limits);
+std::string positionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* offsets,
+                                  const float* weights, HostErrorFunction& out);
+std::string instancedPositionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* weights,
+                                           HostErrorFunction& out);
+std::string planeErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t above, int32_t nc, const int32_t* parents, const float* offsets,
+                               const float* weights, HostErrorFunction& out);
+std::string modelParametersErrorFunction(const HostCharacter& ch, float weight, const float* targetWeights, HostErrorFunction& out);
+std::string orientationErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t rotDiff, int32_t nc, const int32_t* parents,
+                                     const float* offsets, const float* weights, HostErrorFunction& out);
+std::string stateErrorFunction(const HostCharacter& ch, float weight, int32_t rotationErrorType, float posWgt, float rotWgt, const float* posW, const float* rotW,
+                               HostErrorFunction& out);
+std::string limitErrorFunction(float weight, float alpha, float c, HostErrorFunction& out);
+
 struct Plan {
   std::vector<EfDesc> efs;
   std::vector<UnitDesc> units;
@@ -85,5 +122,16 @@ std::string buildPlan(const HostCharacter& ch, const std::vector<HostErrorFuncti
 // getJacobianSize() of a block (joint_error_function-inl.h:300-302, state_error_function.cpp:394-404,
 // limit_error_function.cpp:1138-1161)
 int32_t jacobianBlockSize(const HostCharacter& ch, const HostErrorFunction& ef);
+
+// MB2_CHOLESKY_AUTO: the tile schedule on the sparse pattern from 48 enabled parameters up, the dense Eigen-structured kernel below.
+int resolveCholeskyMode(int requested, const std::vector<uint8_t>& enabled);
+
+// Planning of the tile-scheduled solver path, which fixes the data layout every tile kernel reads:
+//   1. the compact plan in natural column order; 2. the elimination order (ties broken by joint depth) and the tile schedule over it
+//   (densePattern: every tile present); 3. the device columns in elimination order (layoutDeviceColumns); 4. the plan re-built on those
+//   columns, with multi-row units on row quads when `strips`; 5. with strips, the Gram plan, and each cell's strip offset and quad stride
+//   patched into the plan. `gram` stays empty without strips.
+std::string planSolverPath(const HostCharacter& ch, const std::vector<HostErrorFunction>& efs, const std::vector<uint8_t>& enabled, bool densePattern, bool strips,
+                           Plan& plan, CholSchedule& sched, GramPlan& gram);
 
 } // namespace mb2

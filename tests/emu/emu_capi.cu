@@ -1,10 +1,9 @@
 // TEST HARNESS ONLY — CPU lane-emulation of the device code, built into tests/emu/libmb2_emu.so.
 //
-// It exports the subset of include/momentum_b200.h that the parity tests use, but runs the
-// __host__ __device__ building blocks of momentum_b200/csrc (ik_device.cuh, ik_chol.cuh) and the real
-// planner (ik_plan.cpp) lane by lane on the CPU. Purpose: catch planner / indexing / semantics bugs
-// in this GPU-less container before spending GPU time. It is not part of the product library and
-// nothing in momentum_b200/ loads it.
+// It exports the subset of include/momentum_b200.h that the parity tests use. Character and block setup and the solver-path planning
+// are the library's own (ik_plan.cpp, ik_chol_sched.cpp); only the kernels' lane loops over the __host__ __device__ building blocks of
+// momentum_b200/csrc (ik_device.cuh, ik_chol.cuh) run here, lane by lane on the CPU. Purpose: catch planner / indexing / semantics bugs
+// without a GPU. It is not part of the product library and nothing in momentum_b200/ loads it.
 #include <cfloat>
 #include <cmath>
 #include <cstdio>
@@ -30,18 +29,15 @@ struct mb2_character { HostCharacter host; };
 struct mb2_solver_function {
   const mb2_character* ch;
   int B;
-  std::vector<HostErrorFunction> efs;
-  std::vector<uint8_t> enabled;
-  int targetStride{0}, numWeights{0};
-  bool weightsPerInstance{false};
-  std::vector<float> weights, targets;
+  HostFunction host;
+  std::vector<float> targets;         // [B][targetStride]
+  std::vector<float> instanceWeights; // [B][numWeights] once the constraint weights are per instance
   Plan plan;
   int ldJ{32};
   std::vector<float> J;
   bool planCompact{false};
   bool stripMode{false};   // Jacobian buffer in strip layout (GramPlan) instead of the K-major matrix
   int residOff{0}, stripStride{0};
-  std::vector<double> errors;
 };
 struct mb2_solver {
   mb2_solver_function* fn;
@@ -53,29 +49,30 @@ struct mb2_solver {
 
 static int roundUp(int v, int m) { return (v + m - 1) / m * m; }
 
+// Jacobian storage of f->plan: the strips of a Gram plan, or the K-major matrix
+static void layoutJacobian(mb2_solver_function* f, const GramPlan* strips) {
+  f->stripMode = strips != nullptr;
+  f->residOff = strips ? strips->residOff : 0;
+  f->stripStride = strips ? strips->stride : 0;
+  f->ldJ = std::max(32, roundUp(f->plan.numRows, 32));
+  f->J.assign(strips ? size_t(f->B) * strips->stride : size_t(f->B) * (f->plan.numCols + 1) * f->ldJ, 0.f);
+}
+
 static std::string plan(mb2_solver_function* f, bool compact) {
-  std::string e = buildPlan(f->ch->host, f->efs, f->enabled, compact, f->plan);
+  const std::string e = buildPlan(f->ch->host, f->host.efs, f->host.enabled, compact, f->plan);
   if (!e.empty()) return e;
   f->planCompact = compact;
-  f->stripMode = false;
-  f->ldJ = std::max(32, roundUp(f->plan.numRows, 32));
-  f->J.assign(size_t(f->B) * (f->plan.numCols + 1) * f->ldJ, 0.f);
-  f->errors.assign(f->B, 0.0);
-  f->targets.resize(size_t(f->B) * std::max(f->targetStride, 1), 0.f);
-  if (f->weights.empty()) f->weights.push_back(0.f);
+  layoutJacobian(f, nullptr);
   return "";
 }
 
-// depth (in the joint tree) of the deepest joint each enabled parameter drives: tie-break priority of the elimination order
-static std::vector<int> columnDepthPriority(const HostCharacter& h, const std::vector<int32_t>& enabledList) {
-  std::vector<int> jointDepth(h.numJoints, 0);
-  for (int j = 0; j < h.numJoints; ++j) { int d = 0; for (int a = h.parent[j]; a >= 0; a = h.parent[a]) ++d; jointDepth[j] = d; }
-  std::vector<int> paramDepth(h.numParams, 0);
-  for (int r = 0; r < kParametersPerJoint * h.numJoints; ++r)
-    for (int k = h.ptOuter[r]; k < h.ptOuter[r + 1]; ++k) paramDepth[h.ptInner[k]] = std::max(paramDepth[h.ptInner[k]], jointDepth[r / kParametersPerJoint]);
-  std::vector<int> prio(enabledList.size());
-  for (size_t a = 0; a < enabledList.size(); ++a) prio[a] = paramDepth[enabledList[a]];
-  return prio;
+// the plan of the tile-scheduled solver path (cholMode 2: dense pattern, 3: sparse pattern), as the library plans it
+static std::string planTiles(mb2_solver_function* f, int cholMode, bool strips, CholSchedule& s, GramPlan& g) {
+  const std::string e = planSolverPath(f->ch->host, f->host.efs, f->host.enabled, cholMode == MB2_CHOLESKY_TILES_DENSE, strips, f->plan, s, g);
+  if (!e.empty()) return e;
+  f->planCompact = true;
+  layoutJacobian(f, strips ? &g : nullptr);
+  return "";
 }
 
 static FunctionTables tables(const mb2_solver_function* f) {
@@ -88,8 +85,8 @@ static FunctionTables tables(const mb2_solver_function* f) {
   T.numEf = int(f->plan.efs.size()); T.numUnits = int(f->plan.units.size()); T.numCells = int(f->plan.cells.size());
   T.efs = f->plan.efs.data(); T.units = f->plan.units.data(); T.cells = f->plan.cells.data(); T.contribs = f->plan.contribs.data();
   T.limitData = f->plan.limitData.data();
-  T.targetStride = f->targetStride; T.recStride = f->plan.recStride; T.numRows = f->plan.numRows; T.ldJ = f->ldJ; T.numCols = f->plan.numCols;
-  T.weightsPerInstance = f->weightsPerInstance; T.numWeights = f->numWeights;
+  T.targetStride = f->host.targetStride; T.recStride = f->plan.recStride; T.numRows = f->plan.numRows; T.ldJ = f->ldJ; T.numCols = f->plan.numCols;
+  T.weightsPerInstance = f->host.weightsPerInstance; T.numWeights = f->host.numWeights;
   T.stripMode = f->stripMode ? 1 : 0; T.residOff = f->residOff;
   T.jacobianStride = f->stripMode ? size_t(f->stripStride) : size_t(f->plan.numCols + 1) * f->ldJ;
   return T;
@@ -100,25 +97,16 @@ template <bool kJacobian>
 static void sweepOne(mb2_solver_function* f, const FunctionTables& T, int b, const float* theta, double* errOut, float* stateOut) {
   std::vector<float> jp(size_t(T.numJoints) * 7), js(size_t(T.numJoints) * kJointStateStride), rec(T.recStride + 4);
   for (int row = 0; row < T.numJoints * 7; ++row) jp[row] = jointParameterRow(T, row, theta);
-  // the kernels' three passes (fkJoint, the statement-by-statement form, is checked against them below)
+  // the kernels' three passes
   for (int j = 0; j < T.numJoints; ++j) fkLocalFromTheta<kJacobian>(T, j, theta, js.data()); // as sweepKernel: joint parameters straight from theta
   for (int lvl = 1; lvl < T.numLevels; ++lvl)
     for (int k = T.levelStart[lvl]; k < T.levelStart[lvl + 1]; ++k) fkCompose(T, T.levelJoints[k], js.data());
   if (kJacobian)
     for (int i = 0; i < 3 * T.numJoints; ++i) fkAxis(T, i / 3, i % 3, js.data());
-  if (kJacobian && getenv("MB2_EMU_CHECK_FK") != nullptr) { // both forms of JointStateT::set agree to rounding
-    std::vector<float> ref(js.size());
-    for (int lvl = 0; lvl < T.numLevels; ++lvl)
-      for (int k = T.levelStart[lvl]; k < T.levelStart[lvl + 1]; ++k) fkJoint<true>(T, T.levelJoints[k], jp.data(), ref.data());
-    for (size_t i = 0; i < js.size(); ++i) {
-      const float scale = std::max(1.f, std::fabs(ref[i]));
-      if (std::fabs(js[i] - ref[i]) > 2e-5f * scale) { std::fprintf(stderr, "emu: three-pass FK differs from fkJoint at %zu: %g vs %g\n", i, js[i], ref[i]); std::abort(); }
-    }
-  }
   if (stateOut)
     for (int i = 0; i < T.numJoints * 8; ++i) stateOut[i] = js[(i >> 3) * kJointStateStride + (i & 7)];
   const float* tg = f->targets.data() + size_t(b) * T.targetStride;
-  const float* cw = f->weights.data() + (T.weightsPerInstance ? size_t(b) * T.numWeights : 0);
+  const float* cw = T.weightsPerInstance ? f->instanceWeights.data() + size_t(b) * T.numWeights : f->host.weights.data();
   float* Jb = f->J.data() + size_t(b) * T.jacobianStride;
   float* res = kJacobian ? Jb + (T.stripMode ? size_t(T.residOff) : size_t(T.numCols) * T.ldJ) : nullptr;
   // lanes accumulate in double, then a butterfly reduction: emulate the same association
@@ -286,136 +274,77 @@ void mb2_default_gauss_newton_options(mb2_gauss_newton_options* o) {
 int mb2_character_create(int, int32_t J, const int32_t* parents, const float* offsets, const float* prerot, int32_t n, const int32_t* outer,
                          const int32_t* inner, const float* vals, const float* ptoffsets, mb2_character** out) {
   auto c = std::make_unique<mb2_character>();
-  HostCharacter& h = c->host;
-  h.numJoints = J; h.numParams = n;
-  h.parent.assign(parents, parents + J);
-  h.offset.assign(offsets, offsets + 3 * J);
-  h.prerot.assign(prerot, prerot + 4 * J);
-  h.ptOuter.assign(outer, outer + 7 * J + 1);
-  const int nnz = outer[7 * J];
-  h.ptInner.assign(inner, inner + nnz);
-  h.ptVals.assign(vals, vals + nnz);
-  h.ptOffsets.assign(ptoffsets, ptoffsets + 7 * J);
-  const std::string e = h.validate();
+  const std::string e = makeCharacter(J, parents, offsets, prerot, n, outer, inner, vals, ptoffsets, c->host);
   if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  h.buildLevels();
   *out = c.release();
   return MB2_OK;
 }
 int mb2_character_set_parameter_limits(mb2_character* c, int32_t count, const mb2_parameter_limit* limits) {
-  c->host.limits.clear();
-  for (int i = 0; i < count; ++i) {
-    HostLimit l;
-    l.type = limits[i].type; l.weight = limits[i].weight;
-    std::memcpy(l.i, limits[i].i, sizeof(l.i)); std::memcpy(l.f, limits[i].f, sizeof(l.f));
-    c->host.limits.push_back(l);
-  }
-  return MB2_OK;
+  const std::string e = setParameterLimits(c->host, count, limits);
+  return e.empty() ? MB2_OK : fail(MB2_ERR_INVALID_ARGUMENT, e);
 }
 void mb2_character_destroy(mb2_character* c) { delete c; }
 
 int mb2_solver_function_create(const mb2_character* c, int32_t batch, mb2_solver_function** out) {
   auto f = std::make_unique<mb2_solver_function>();
   f->ch = c; f->B = batch;
-  f->enabled.assign(c->host.numParams, 1);
+  f->host.enabled.assign(c->host.numParams, 1);
+  f->targets.assign(size_t(batch), 0.f);
   *out = f.release();
   return MB2_OK;
 }
 void mb2_solver_function_destroy(mb2_solver_function* f) { delete f; }
 int32_t mb2_solver_function_num_parameters(const mb2_solver_function* f) { return f->ch->host.numParams; }
 int32_t mb2_solver_function_batch(const mb2_solver_function* f) { return f->B; }
-int32_t mb2_solver_function_actual_parameters(const mb2_solver_function* f) {
-  int ap = 0;
-  for (int i = 0; i < f->ch->host.numParams; ++i) if (f->enabled[i]) ap = i + 1;
-  return ap;
-}
-int32_t mb2_solver_function_jacobian_rows(const mb2_solver_function* f) {
-  int total = 0;
-  for (const auto& ef : f->efs) if (ef.weight > 0.f) total += jacobianBlockSize(f->ch->host, ef);
-  return roundUp(total, 8);
-}
-int32_t mb2_solver_function_jacobian_stride(const mb2_solver_function* f) {
-  int total = 0;
-  for (const auto& ef : f->efs) if (ef.weight > 0.f) total += jacobianBlockSize(f->ch->host, ef);
-  return std::max(32, roundUp(total, 32));
-}
+int32_t mb2_solver_function_actual_parameters(const mb2_solver_function* f) { return f->host.actualParameters(); }
+int32_t mb2_solver_function_jacobian_rows(const mb2_solver_function* f) { return f->host.jacobianRows(f->ch->host); }
+int32_t mb2_solver_function_jacobian_stride(const mb2_solver_function* f) { return f->host.jacobianStride(f->ch->host); }
 
-static int addBlock(mb2_solver_function* f, HostErrorFunction& ef, int32_t* outIndex) {
-  ef.targetOff = f->targetStride; ef.weightOff = f->numWeights;
-  f->targetStride += ef.targetSize;
-  if (ef.kind <= 2 || ef.kind == 5) { f->numWeights += ef.numConstraints(); f->weights.insert(f->weights.end(), ef.weights.begin(), ef.weights.end()); }
-  f->efs.push_back(ef);
-  // re-layout targets (tests add all blocks before setting targets)
-  f->targets.assign(size_t(f->B) * std::max(f->targetStride, 1), 0.f);
-  if (outIndex) *outIndex = int32_t(f->efs.size()) - 1;
+static int addBlock(mb2_solver_function* f, const std::string& buildError, const HostErrorFunction& ef, int32_t* outIndex) {
+  if (!buildError.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, buildError);
+  const std::string e = f->host.add(ef, outIndex);
+  if (!e.empty()) return fail(MB2_ERR_UNSUPPORTED, e);
+  f->targets.assign(size_t(f->B) * std::max(f->host.targetStride, 1), 0.f); // re-layout targets (tests add all blocks before setting targets)
   return MB2_OK;
 }
 int mb2_add_position_error_function(mb2_solver_function* f, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* offsets,
                                     const float* weights, int32_t* outIndex) {
   HostErrorFunction ef;
-  ef.kind = 0; ef.weight = weight; ef.lossAlpha = alpha; ef.lossC = c;
-  ef.parents.assign(parents, parents + nc); ef.offsets.assign(offsets, offsets + 3 * size_t(nc)); ef.weights.assign(weights, weights + nc);
-  ef.targetSize = 3 * nc;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, positionErrorFunction(f->ch->host, weight, alpha, c, nc, parents, offsets, weights, ef), ef, outIndex);
 }
 int mb2_add_position_error_function_instanced(mb2_solver_function* f, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* weights,
                                               int32_t* outIndex) {
   HostErrorFunction ef;
-  ef.kind = 0; ef.weight = weight; ef.lossAlpha = alpha; ef.lossC = c; ef.instanceOffsets = true;
-  ef.parents.assign(parents, parents + nc);
-  ef.offsets.assign(3 * size_t(nc), 0.f);
-  ef.weights.assign(weights, weights + nc);
-  ef.targetSize = 6 * nc;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, instancedPositionErrorFunction(f->ch->host, weight, alpha, c, nc, parents, weights, ef), ef, outIndex);
 }
 int mb2_add_plane_error_function(mb2_solver_function* f, float weight, float alpha, float c, int32_t above, int32_t nc, const int32_t* parents,
                                  const float* offsets, const float* weights, int32_t* outIndex) {
   HostErrorFunction ef;
-  ef.kind = 5; ef.weight = weight; ef.lossAlpha = alpha; ef.lossC = c; ef.halfPlane = above != 0;
-  ef.parents.assign(parents, parents + nc); ef.offsets.assign(offsets, offsets + 3 * size_t(nc)); ef.weights.assign(weights, weights + nc);
-  ef.targetSize = 4 * nc;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, planeErrorFunction(f->ch->host, weight, alpha, c, above, nc, parents, offsets, weights, ef), ef, outIndex);
 }
 int mb2_add_model_parameters_error_function(mb2_solver_function* f, float weight, const float* targetWeights, int32_t* outIndex) {
   HostErrorFunction ef;
-  ef.kind = 6; ef.weight = weight;
-  ef.paramWeights.assign(targetWeights, targetWeights + f->ch->host.numParams);
-  ef.targetSize = f->ch->host.numParams;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, modelParametersErrorFunction(f->ch->host, weight, targetWeights, ef), ef, outIndex);
 }
 int mb2_add_orientation_error_function(mb2_solver_function* f, float weight, float alpha, float c, int32_t rotDiff, int32_t nc, const int32_t* parents,
                                        const float* offsets, const float* weights, int32_t* outIndex) {
   HostErrorFunction ef;
-  ef.kind = rotDiff ? 2 : 1; ef.weight = weight; ef.lossAlpha = alpha; ef.lossC = c;
-  ef.parents.assign(parents, parents + nc); ef.offsets.assign(offsets, offsets + 4 * size_t(nc));
-  for (int i = 0; i < nc; ++i) {
-    float* q = &ef.offsets[4 * size_t(i)];
-    const float nrm = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    for (int k = 0; k < 4; ++k) q[k] /= nrm;
-  }
-  ef.weights.assign(weights, weights + nc);
-  ef.targetSize = 4 * nc;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, orientationErrorFunction(f->ch->host, weight, alpha, c, rotDiff, nc, parents, offsets, weights, ef), ef, outIndex);
 }
 int mb2_add_state_error_function(mb2_solver_function* f, float weight, int32_t rotationErrorType, float posWgt, float rotWgt, const float* posW,
                                  const float* rotW, int32_t* outIndex) {
   HostErrorFunction ef;
-  ef.kind = 3; ef.weight = weight; ef.rotationErrorType = rotationErrorType; ef.posWgt = posWgt; ef.rotWgt = rotWgt;
-  const int J = f->ch->host.numJoints;
-  ef.posW.assign(posW, posW + J); ef.rotW.assign(rotW, rotW + J);
-  ef.targetSize = 8 * J;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, stateErrorFunction(f->ch->host, weight, rotationErrorType, posWgt, rotWgt, posW, rotW, ef), ef, outIndex);
 }
 int mb2_add_limit_error_function(mb2_solver_function* f, float weight, float alpha, float c, int32_t* outIndex) {
   HostErrorFunction ef;
-  ef.kind = 4; ef.weight = weight; ef.lossAlpha = alpha; ef.lossC = c; ef.targetSize = 0;
-  return addBlock(f, ef, outIndex);
+  return addBlock(f, limitErrorFunction(weight, alpha, c, ef), ef, outIndex);
 }
-int mb2_set_error_function_weight(mb2_solver_function* f, int32_t index, float weight) { f->efs[index].weight = weight; return MB2_OK; }
+int mb2_set_error_function_weight(mb2_solver_function* f, int32_t index, float weight) { f->host.efs[index].weight = weight; return MB2_OK; }
 int mb2_set_targets(mb2_solver_function* f, int32_t index, const float* targets) {
-  const HostErrorFunction& ef = f->efs[index];
+  const HostErrorFunction& ef = f->host.efs[index];
   for (int b = 0; b < f->B; ++b) {
-    float* dst = f->targets.data() + size_t(b) * f->targetStride + ef.targetOff;
+    float* dst = f->targets.data() + size_t(b) * f->host.targetStride + ef.targetOff;
     std::memcpy(dst, targets + size_t(b) * ef.targetSize, size_t(ef.targetSize) * sizeof(float));
     if (ef.kind == 1 || ef.kind == 2)
       for (int q = 0; q < ef.numConstraints(); ++q) {
@@ -427,20 +356,20 @@ int mb2_set_targets(mb2_solver_function* f, int32_t index, const float* targets)
   return MB2_OK;
 }
 int mb2_set_constraint_weights(mb2_solver_function* f, int32_t index, const float* weights, int32_t perInstance) {
-  HostErrorFunction& ef = f->efs[index];
+  HostFunction& h = f->host;
+  const HostErrorFunction& ef = h.efs[index];
   const int nc = ef.numConstraints();
-  if (!perInstance) { std::copy(weights, weights + nc, f->weights.begin() + ef.weightOff); return MB2_OK; }
-  if (!f->weightsPerInstance) {
-    std::vector<float> all(size_t(f->B) * f->numWeights);
-    for (int b = 0; b < f->B; ++b) std::copy(f->weights.begin(), f->weights.begin() + f->numWeights, all.begin() + size_t(b) * f->numWeights);
-    f->weights = all;
-    f->weightsPerInstance = true;
+  if (!perInstance) { std::copy(weights, weights + nc, h.weights.begin() + ef.weightOff); return MB2_OK; }
+  if (!h.weightsPerInstance) {
+    f->instanceWeights.resize(size_t(f->B) * h.numWeights);
+    for (int b = 0; b < f->B; ++b) std::copy(h.weights.begin(), h.weights.end(), f->instanceWeights.begin() + size_t(b) * h.numWeights);
+    h.weightsPerInstance = true;
   }
-  for (int b = 0; b < f->B; ++b) std::copy(weights + size_t(b) * nc, weights + size_t(b + 1) * nc, f->weights.begin() + size_t(b) * f->numWeights + ef.weightOff);
+  for (int b = 0; b < f->B; ++b) std::copy(weights + size_t(b) * nc, weights + size_t(b + 1) * nc, f->instanceWeights.begin() + size_t(b) * h.numWeights + ef.weightOff);
   return MB2_OK;
 }
 int mb2_solver_function_set_enabled_parameters(mb2_solver_function* f, const uint64_t* bits) {
-  for (int i = 0; i < f->ch->host.numParams; ++i) f->enabled[i] = (bits[i >> 6] >> (i & 63)) & 1ull ? 1 : 0;
+  for (int i = 0; i < f->ch->host.numParams; ++i) f->host.enabled[i] = (bits[i >> 6] >> (i & 63)) & 1ull ? 1 : 0;
   return MB2_OK;
 }
 
@@ -509,38 +438,12 @@ int mb2_solver_set_enabled_parameters(mb2_solver* s, const uint64_t* bits) { ret
 int mb2_solver_solve(mb2_solver* s, float* params, double* errors, int32_t* iterations, int32_t* status) {
   mb2_solver_function* f = s->fn;
   const auto& o = s->opt;
-  int numEnabled = 0;
-  for (uint8_t e : f->enabled) numEnabled += e ? 1 : 0;
-  int cholMode = o.cholesky_mode;
-  if (cholMode == 0) cholMode = numEnabled >= 48 ? 3 : 1;
-  std::string e = plan(f, true);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
+  const int cholMode = resolveCholeskyMode(o.cholesky_mode, f->host.enabled);
+  const bool useGram = cholMode >= 2 && (o.jtj_mode == MB2_JTJ_AUTO || o.jtj_mode == MB2_JTJ_SPARSE_TILES);
   CholSchedule sched;
   GramPlan gram;
-  const bool useGram = cholMode >= 2 && (o.jtj_mode == MB2_JTJ_AUTO || o.jtj_mode == MB2_JTJ_SPARSE_TILES);
-  if (cholMode >= 2) { // same two-pass planning as ensurePlan(mode 2) in ik_capi.cu
-    const int ns0 = f->plan.numCols;
-    std::vector<std::vector<int>> cliques(f->plan.units.size());
-    for (const CellDesc& c : f->plan.cells) cliques[c.unit].push_back(int(c.col));
-    const std::vector<int> prio = columnDepthPriority(f->ch->host, f->plan.enabledList);
-    e = buildCholSchedule(ns0, cliques, cholMode == 2, sched, &prio);
-    if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-    std::vector<int32_t> colOrder;
-    layoutDeviceColumns(sched, colOrder);
-    for (int32_t& c : colOrder) if (c >= 0) c = f->plan.enabledList[c];
-    e = buildPlan(f->ch->host, f->efs, f->enabled, true, f->plan, &colOrder, useGram);
-    if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-    if (useGram) {
-      std::vector<int32_t> cr0, crn, cc;
-      for (const CellDesc& c : f->plan.cells) { cr0.push_back(f->plan.units[c.unit].row0); crn.push_back(f->plan.units[c.unit].numRows); cc.push_back(int32_t(c.col)); }
-      e = buildGramPlan(sched, cr0, crn, cc, f->plan.numRows, gram);
-      if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-      for (size_t i = 0; i < f->plan.cells.size(); ++i) { f->plan.cells[i].stripOff = gram.cellStripOff[i]; f->plan.cells[i].quadStride = gram.cellQuadStride[i]; }
-    }
-    f->stripMode = useGram; f->residOff = gram.residOff; f->stripStride = gram.stride;
-    f->ldJ = std::max(32, roundUp(f->plan.numRows, 32));
-    f->J.assign(useGram ? size_t(f->B) * gram.stride : size_t(f->B) * (f->plan.numCols + 1) * f->ldJ, 0.f);
-  }
+  const std::string e = cholMode >= 2 ? planTiles(f, cholMode, useGram, sched, gram) : plan(f, true);
+  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
   std::vector<int32_t> blob;
   CholSchedDev S{};
   if (cholMode >= 2) makeScheduleBlob(sched, blob, S);
@@ -559,15 +462,14 @@ int mb2_solver_solve(mb2_solver* s, float* params, double* errors, int32_t* iter
       sweepOne<true>(f, T, b, theta, &error, nullptr);
       float gdd = 0.f;
       int failed;
-      std::fill(H.begin(), H.end(), std::nanf("")); // entries the device never writes (lower triangle) are garbage there: poison them here
-      jtjOne(f, b, ns, H.data(), ldH);
-      if (cholMode >= 2 && useGram) {
+      if (useGram) { // the strips hold no K-major matrix: the normal equations come from the Gram tiles only
         gramOne(f, b, gram, S, o.regularization, gramOut.data());
         failed = cholScheduledOne(S, nullptr, ldH, ns, o.regularization, delta.data(), &gdd, gramOut.data());
-      } else if (cholMode >= 2) {
-        failed = cholScheduledOne(S, H.data(), ldH, ns, o.regularization, delta.data(), &gdd);
       } else {
-        failed = cholDispatch(H.data(), ns, ldH, o.regularization, delta.data(), &gdd);
+        std::fill(H.begin(), H.end(), std::nanf("")); // entries the device never writes (lower triangle) are garbage there: poison them here
+        jtjOne(f, b, ns, H.data(), ldH);
+        failed = cholMode >= 2 ? cholScheduledOne(S, H.data(), ldH, ns, o.regularization, delta.data(), &gdd)
+                               : cholDispatch(H.data(), ns, ldH, o.regularization, delta.data(), &gdd);
       }
       if (failed && s->status[b] == 0) s->status[b] = MB2_INSTANCE_CHOLESKY_BREAKDOWN;
       if (!o.do_line_search) {
@@ -615,153 +517,21 @@ int mb2_solver_get_counters(mb2_solver* s, uint64_t* totalIterations, uint64_t* 
 
 } // extern "C"
 
-// ---- scheduler statistics (test/debug helper) ----
-#include "../../momentum_b200/csrc/ik_chol_sched.h"
-extern "C" int emu_chol_schedule_stats(int n, int numCliques, const int* cliqueStart, const int* cliqueCols, int forceDense, long long* stats) {
-  std::vector<std::vector<int>> cl(numCliques);
-  for (int c = 0; c < numCliques; ++c) cl[c].assign(cliqueCols + cliqueStart[c], cliqueCols + cliqueStart[c + 1]);
-  CholSchedule s;
-  const std::string e = buildCholSchedule(n, cl, forceDense != 0, s);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  stats[0] = s.numTileCols; stats[1] = s.numTiles; stats[2] = s.numLevels; stats[3] = s.tileOps; stats[4] = s.denseTileOps;
-  stats[5] = (long long)s.taskDst.size(); stats[6] = (long long)s.panelTile.size();
-  return MB2_OK;
-}
-
-extern "C" int emu_chol_schedule_dump(int n, int numCliques, const int* cliqueStart, const int* cliqueCols, int forceDense) {
-  std::vector<std::vector<int>> cl(numCliques);
-  for (int c = 0; c < numCliques; ++c) cl[c].assign(cliqueCols + cliqueStart[c], cliqueCols + cliqueStart[c + 1]);
-  CholSchedule s;
-  const std::string e = buildCholSchedule(n, cl, forceDense != 0, s);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  std::printf("n %d nPad %d tilecols %d tiles %d levels %d\n", s.n, s.nPad, s.numTileCols, s.numTiles, s.numLevels);
-  for (int L = 0; L < s.numLevels; ++L) {
-    int maxPairs = 0, totPairs = 0;
-    for (int t = s.levelTaskStart[L]; t < s.levelTaskStart[L + 1]; ++t) { const int p = s.taskPairStart[t + 1] - s.taskPairStart[t]; maxPairs = std::max(maxPairs, p); totPairs += p; }
-    std::printf(" level %d: cols %d panels %d tasks %d pairs %d maxPairsPerTask %d vtasks %d | cols:", L, s.levelColStart[L + 1] - s.levelColStart[L],
-                s.levelPanelStart[L + 1] - s.levelPanelStart[L], s.levelTaskStart[L + 1] - s.levelTaskStart[L], totPairs, maxPairs,
-                s.levelVTaskStart[L + 1] - s.levelVTaskStart[L]);
-    for (int c = s.levelColStart[L]; c < s.levelColStart[L + 1]; ++c) {
-      int valid = 0;
-      for (int r = 0; r < 16; ++r) valid += s.perm[16 * s.levelCols[c] + r] >= 0;
-      std::printf(" %d(%d)", s.levelCols[c], valid);
-    }
-    std::printf("\n");
-  }
-  return MB2_OK;
-}
-
-extern "C" int emu_chol_chunk_stats(int n, int numCliques, const int* cliqueStart, const int* cliqueCols) {
-  std::vector<std::vector<int>> cl(numCliques);
-  for (int c = 0; c < numCliques; ++c) cl[c].assign(cliqueCols + cliqueStart[c], cliqueCols + cliqueStart[c + 1]);
-  CholSchedule s;
-  const std::string e = buildCholSchedule(n, cl, false, s);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  std::vector<int32_t> order;
-  layoutDeviceColumns(s, order);
-  const int nd = s.n + 1; // + residual column
-  const int nb = (nd + 31) / 32;
-  std::vector<int> need(nb * nb, 0);
-  auto validOf = [&](int K) { int v = 0; while (v < 16 && s.perm[16 * K + v] >= 0) ++v; return v; };
-  for (int t = 0; t < s.numTiles; ++t) {
-    const int I = s.tileRow[t], J = s.tileCol[t];
-    const int vI = validOf(I), vJ = validOf(J), gi0 = s.perm[16 * I], gj0 = s.perm[16 * J];
-    for (int r = gj0; r < gj0 + vJ; ++r) for (int c = gi0; c < gi0 + vI; ++c) if (c >= r) need[(r / 32) * nb + c / 32] = 1;
-  }
-  int total = 0, needed = 0;
-  for (int a = 0; a < nb; ++a) for (int b2 = a; b2 < nb; ++b2) { ++total; needed += need[a * nb + b2] || b2 == (nd - 1) / 32; }
-  std::printf("device columns %d (+1), 32x32 chunks in the upper triangle %d, needed %d\n", s.n, total, needed);
-  for (int a = 0; a < nb; ++a) { for (int b2 = 0; b2 < nb; ++b2) std::printf("%c", b2 < a ? ' ' : (need[a * nb + b2] ? '#' : (b2 == (nd - 1) / 32 ? 'g' : '.'))); std::printf("\n"); }
-  return MB2_OK;
-}
-
-extern "C" int emu_gram_stats(mb2_solver_function* f) {
-  std::string e = plan(f, true);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  CholSchedule sched;
-  std::vector<std::vector<int>> cliques(f->plan.units.size());
-  for (const CellDesc& c : f->plan.cells) cliques[c.unit].push_back(int(c.col));
-  const std::vector<int> prio = columnDepthPriority(f->ch->host, f->plan.enabledList);
-  e = buildCholSchedule(f->plan.numCols, cliques, false, sched, &prio);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  std::vector<int32_t> colOrder;
-  layoutDeviceColumns(sched, colOrder);
-  for (int32_t& c : colOrder) if (c >= 0) c = f->plan.enabledList[c];
-  e = buildPlan(f->ch->host, f->efs, f->enabled, true, f->plan, &colOrder, true);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  std::vector<int32_t> cr0, crn, cc;
-  for (const CellDesc& c : f->plan.cells) { cr0.push_back(f->plan.units[c.unit].row0); crn.push_back(f->plan.units[c.unit].numRows); cc.push_back(int32_t(c.col)); }
-  GramPlan g;
-  e = buildGramPlan(sched, cr0, crn, cc, f->plan.numRows, g);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  int maxPairs = 0;
-  for (int t = 0; t < g.numTiles; ++t) maxPairs = std::max(maxPairs, g.tilePairStart[t + 1] - g.tilePairStart[t]);
-  std::printf("rows %d (aligned), device columns %d, strips %d (%d KB), tiles %d, pairs %zu (max per tile %d), MACs %lld\n", f->plan.numRows, f->plan.numCols, g.numStrips,
-              g.numStrips / 4, g.numTiles, g.pairA.size(), maxPairs, (long long)g.macs);
-  std::printf("pairs per tile in order:");
-  for (size_t ti = 0; ti < g.tileOrder.size(); ++ti) { const int t = g.tileOrder[ti]; if (t >= 0) std::printf(" %d", g.tilePairStart[t + 1] - g.tilePairStart[t]); else std::printf(" -"); }
-  std::printf("\n");
-  return MB2_OK;
-}
-
-extern "C" int emu_sched_structure(mb2_solver_function* f) {
-  std::string e = plan(f, true);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  CholSchedule s;
-  std::vector<std::vector<int>> cliques(f->plan.units.size());
-  for (const CellDesc& c : f->plan.cells) cliques[c.unit].push_back(int(c.col));
-  const std::vector<int> prio = columnDepthPriority(f->ch->host, f->plan.enabledList);
-  e = buildCholSchedule(f->plan.numCols, cliques, false, s, &prio);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  std::printf("levels %d tiles %d\n", s.numLevels, s.numTiles);
-  for (int L = 0; L < s.numLevels; ++L) { std::printf(" level %d:", L); for (int c = s.levelColStart[L]; c < s.levelColStart[L + 1]; ++c) std::printf(" %d", s.levelCols[c]); std::printf("\n"); }
-  const int T = s.numTileCols;
-  const HostCharacter& h = f->ch->host;
-  // parameter -> a joint it drives (first one)
-  std::vector<int> jointOf(h.numParams, -1);
-  for (int r = 0; r < 7 * h.numJoints; ++r)
-    for (int k = h.ptOuter[r]; k < h.ptOuter[r + 1]; ++k) if (jointOf[h.ptInner[k]] < 0) jointOf[h.ptInner[k]] = r / 7;
-  for (int K = 0; K < T; ++K) {
-    std::printf("tile col %2d: joints {", K);
-    int last = -2;
-    for (int j = 0; j < 16; ++j) { const int p = s.perm[16 * K + j]; if (p < 0) continue; const int jt = jointOf[f->plan.enabledList[p]]; if (jt != last) std::printf(" %d", jt); last = jt; }
-    std::printf(" }  rows below:");
-    for (int I = K + 1; I < T; ++I) if (s.tileIdTable[size_t(I) * T + K] >= 0) std::printf(" %d", I);
-    std::printf("\n");
-  }
-  std::printf("parents:");
-  for (int j = 0; j < h.numJoints; ++j) std::printf(" %d:%d", j, h.parent[j]);
-  std::printf("\n");
-  return MB2_OK;
-}
-
-// schedule / Gram-plan figures of the solver plan (mode 2 planning of ik_capi.cu): out = {levels, tiles, tile columns, nPad, device
+// schedule / Gram-plan figures of the solver plan (cholesky_mode 3 with strips): out = {levels, tiles, tile columns, nPad, device
 // columns, strips, pairs, misaligned tile starts, odd pair lists, cells outside their strip}
 extern "C" int emu_plan_figures(mb2_solver_function* f, int64_t out[10]) {
-  std::string e = plan(f, true);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
   CholSchedule s;
-  std::vector<std::vector<int>> cliques(f->plan.units.size());
-  for (const CellDesc& c : f->plan.cells) cliques[c.unit].push_back(int(c.col));
-  const std::vector<int> prio = columnDepthPriority(f->ch->host, f->plan.enabledList);
-  e = buildCholSchedule(f->plan.numCols, cliques, false, s, &prio);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  std::vector<int32_t> colOrder;
-  layoutDeviceColumns(s, colOrder);
-  for (int32_t& c : colOrder) if (c >= 0) c = f->plan.enabledList[c];
-  e = buildPlan(f->ch->host, f->efs, f->enabled, true, f->plan, &colOrder, true);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  std::vector<int32_t> cr0, crn, cc;
-  for (const CellDesc& c : f->plan.cells) { cr0.push_back(f->plan.units[c.unit].row0); crn.push_back(f->plan.units[c.unit].numRows); cc.push_back(int32_t(c.col)); }
   GramPlan g;
-  e = buildGramPlan(s, cr0, crn, cc, f->plan.numRows, g);
+  const std::string e = planTiles(f, MB2_CHOLESKY_TILES_SPARSE, true, s, g);
   if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
+  const Plan& p = f->plan;
   int64_t misaligned = 0, odd = 0, outside = 0;
   for (int K = 0; K < s.numTileCols; ++K) misaligned += (s.perm[16 * K] < 0 || (s.perm[16 * K] & 3) != 0) ? 1 : 0;
   for (int t = 0; t < s.numTiles; ++t) odd += (g.tilePairStart[t + 1] - g.tilePairStart[t]) & 1;
-  for (size_t i = 0; i < cc.size(); ++i) {
+  for (size_t i = 0; i < p.cells.size(); ++i) {
+    const int row0 = p.units[p.cells[i].unit].row0, col = p.cells[i].col;
     const int strip = int(g.cellStripOff[i] / 64), colInStrip = int(g.cellStripOff[i] % 64) / 4;
-    if (strip >= g.numStrips || g.stripCoord[2 * strip] != (cr0[i] & ~3) || g.stripCoord[2 * strip + 1] + colInStrip != cc[i]) ++outside;
+    if (strip >= g.numStrips || g.stripCoord[2 * strip] != (row0 & ~3) || g.stripCoord[2 * strip + 1] + colInStrip != col) ++outside;
   }
   out[0] = s.numLevels; out[1] = s.numTiles; out[2] = s.numTileCols; out[3] = s.nPad; out[4] = s.n; out[5] = g.numStrips; out[6] = int64_t(g.pairA.size());
   out[7] = misaligned; out[8] = odd; out[9] = outside;
@@ -774,8 +544,10 @@ extern "C" int emu_plan_figures(mb2_solver_function* f, int64_t out[10]) {
 // out: [0] units starting off a quad boundary, [1] units whose padding rows overlap another unit, [2] cells at unaligned strip offsets,
 //      [3] cells out of (kind, unit, column) order, [4] multi-row units, [5] cells
 extern "C" int emu_store_invariants(mb2_solver_function* f, int64_t out[6]) {
-  int64_t fig[10];
-  if (emu_plan_figures(f, fig) != MB2_OK) return MB2_ERR_INVALID_ARGUMENT; // leaves f->plan in the solver layout (aligned row groups)
+  CholSchedule s;
+  GramPlan g;
+  const std::string e = planTiles(f, MB2_CHOLESKY_TILES_SPARSE, true, s, g);
+  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
   const Plan& p = f->plan;
   std::vector<int> owner(size_t(p.numRows) + 8, -1);
   int64_t offQuad = 0, overlap = 0, multi = 0;
@@ -785,28 +557,6 @@ extern "C" int emu_store_invariants(mb2_solver_function* f, int64_t out[6]) {
     if (joint) { ++multi; if ((d.row0 & 3) != 0) ++offQuad; }
     const int end = joint ? ((d.row0 + d.numRows + 3) & ~3) : d.row0 + d.numRows; // a joint unit claims its padding rows too
     for (int r = d.row0; r < end; ++r) { if (owner[size_t(r)] >= 0) ++overlap; owner[size_t(r)] = int(u); }
-  }
-  // strip offsets of the cells: the Gram plan of the same layout (as emu_plan_figures builds it)
-  CholSchedule s;
-  std::vector<std::vector<int>> cliques(p.units.size());
-  for (const CellDesc& c : p.cells) cliques[c.unit].push_back(int(c.col));
-  std::vector<int32_t> cr0, crn, cc;
-  for (const CellDesc& c : p.cells) { cr0.push_back(p.units[c.unit].row0); crn.push_back(p.units[c.unit].numRows); cc.push_back(int32_t(c.col)); }
-  GramPlan g;
-  {
-    // the schedule must be the one the plan's device columns were laid out for: rebuild it from the natural-order plan
-    mb2_solver_function tmp = *f; // (plain copy of the host description; device-free harness)
-    std::string e = plan(&tmp, true);
-    if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-    std::vector<std::vector<int>> cl(tmp.plan.units.size());
-    for (const CellDesc& c : tmp.plan.cells) cl[c.unit].push_back(int(c.col));
-    const std::vector<int> prio = columnDepthPriority(f->ch->host, tmp.plan.enabledList);
-    e = buildCholSchedule(tmp.plan.numCols, cl, false, s, &prio);
-    if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-    std::vector<int32_t> colOrder;
-    layoutDeviceColumns(s, colOrder);
-    e = buildGramPlan(s, cr0, crn, cc, p.numRows, g);
-    if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
   }
   int64_t unaligned = 0, disorder = 0;
   for (size_t i = 0; i < p.cells.size(); ++i) {
@@ -820,47 +570,5 @@ extern "C" int emu_store_invariants(mb2_solver_function* f, int64_t out[6]) {
     }
   }
   out[0] = offQuad; out[1] = overlap; out[2] = unaligned; out[3] = disorder; out[4] = multi; out[5] = int64_t(p.cells.size());
-  return MB2_OK;
-}
-
-// table sizes of the solver plan (bytes): what a kernel that stages every table in shared memory has to hold
-extern "C" int emu_table_sizes(mb2_solver_function* f, int64_t out[12]) {
-  int64_t fig[10];
-  if (emu_plan_figures(f, fig) != MB2_OK) return MB2_ERR_INVALID_ARGUMENT; // leaves f->plan in the solver layout
-  const HostCharacter& h = f->ch->host;
-  out[0] = int64_t(f->plan.units.size());
-  out[1] = int64_t(f->plan.cells.size());
-  out[2] = int64_t(f->plan.contribs.size());
-  out[3] = int64_t(h.ptInner.size());
-  out[4] = int64_t(f->plan.limitData.size());
-  out[5] = f->plan.recStride;
-  out[6] = f->targetStride;
-  out[7] = int64_t(sizeof(UnitDesc));
-  out[8] = int64_t(sizeof(CellDesc));
-  out[9] = int64_t(sizeof(ContribDesc));
-  out[10] = int64_t(h.levelStart.size()) - 1;
-  int maxContrib = 0;
-  for (const CellDesc& c : f->plan.cells) maxContrib = std::max<int>(maxContrib, c.contribCount);
-  out[11] = maxContrib;
-  return MB2_OK;
-}
-
-// per-level update-task pair counts of the solver plan's schedule (balance analysis)
-extern "C" int emu_task_loads(mb2_solver_function* f) {
-  std::string e = plan(f, true);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  CholSchedule s;
-  std::vector<std::vector<int>> cliques(f->plan.units.size());
-  for (const CellDesc& c : f->plan.cells) cliques[c.unit].push_back(int(c.col));
-  const std::vector<int> prio = columnDepthPriority(f->ch->host, f->plan.enabledList);
-  e = buildCholSchedule(f->plan.numCols, cliques, false, s, &prio);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  for (int L = 0; L < s.numLevels; ++L) {
-    std::printf("level %d: diag %d panels %d tasks:", L, s.levelColStart[L + 1] - s.levelColStart[L], s.levelPanelStart[L + 1] - s.levelPanelStart[L]);
-    for (int t = s.levelTaskStart[L]; t < s.levelTaskStart[L + 1]; ++t) std::printf(" %d", s.taskPairStart[t + 1] - s.taskPairStart[t]);
-    std::printf(" | vtasks:");
-    for (int t = s.levelVTaskStart[L]; t < s.levelVTaskStart[L + 1]; ++t) std::printf(" %d", s.vtaskSrcStart[t + 1] - s.vtaskSrcStart[t]);
-    std::printf("\n");
-  }
   return MB2_OK;
 }
