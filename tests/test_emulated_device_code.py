@@ -187,6 +187,51 @@ def test_chain22_cfg1():
     parity.check_solve(ch, efs, theta0, opts, EMU_LIB, param_tol=2e-4)
 
 
+@pytest.mark.parametrize("n", [1, 8, 9, 16, 17, 31, 32, 127, 128, 231, 232, 255, 256])
+def test_dense_cholesky_backward_error(n):
+    """One Gauss-Newton step through the dense Eigen-structured Cholesky at every block size (tests/f64ref.py: normwise backward error
+    against the float64 normal equations of the emulator's own float Jacobian). The emulator factors on the host, so the kernel's
+    shared / global memory branch and the TF32 JtJ modes are GPU-only (tests/test_gpu_kernel_bounds.py). No path is asserted here: the
+    emulator has no plan statistics and no fallback, so the explicit cholesky_mode alone decides what it runs."""
+    from tests import f64ref as R
+
+    if n < 10:
+        ch, efs, _ = R.chain_case(10, positions=3, seed=n)
+        en = np.zeros(10, bool); en[:n] = True
+    else:
+        ch, efs, _ = R.chain_case(n, positions=min(n - 7, 12), seed=n)
+        en = None
+    opts = ms.GaussNewtonSolverOptions(min_iterations=1, max_iterations=1, regularization=0.05, cholesky_mode=ms.CHOLESKY_DENSE_EIGEN)
+    _, out, J, r, cols, delta, lam = R.one_step(ch, efs, np.zeros((1, ch.num_params)), opts, EMU_LIB, en, rel_damping=1e-5)
+    assert np.all(out["status"] == 0) and len(cols) == n
+    be = R.backward_error(J[0], r[0], cols, delta[0], lam)
+    assert be <= R.solve_limit(n), (n, be, R.solve_limit(n))
+
+
+@pytest.mark.parametrize("chol", [ms.CHOLESKY_TILES_DENSE, ms.CHOLESKY_TILES_SPARSE])
+@pytest.mark.parametrize("jtj", [ms.JTJ_SPARSE_TILES, ms.JTJ_FP32_SIMT])
+@pytest.mark.parametrize("rig", ["humanoid", "humanoid_subset", "chain330"])
+def test_tile_cholesky_backward_error(rig, jtj, chol):
+    """The level-scheduled tile Cholesky fed by the tile-sparse Gram and by the K-major JtJ, same bound as the dense kernel. The
+    emulator has no shared-memory budget: the 330-parameter chain, whose dense schedule sends CHOLESKY_AUTO to the dense kernel on the
+    device, runs the tile schedule here; the fused kernels, the 256 / 512-thread variants and the QR step are GPU-only. As above, the
+    explicit modes decide the path and none is asserted."""
+    from tests import f64ref as R
+
+    en = None
+    if rig == "chain330":
+        ch, efs, _ = R.chain_case(330, positions=12, seed=330)
+    else:
+        ch, efs, _, _ = humanoid_problem(1, orientation=True)
+        if rig == "humanoid_subset":
+            en = np.ones(ch.num_params, bool); en[[0, 5, 6, 40, 41, 42, 100, 219]] = False
+    opts = ms.GaussNewtonSolverOptions(min_iterations=1, max_iterations=1, regularization=0.05, cholesky_mode=chol, jtj_mode=jtj)
+    _, out, J, r, cols, delta, lam = R.one_step(ch, efs, np.zeros((1, ch.num_params)), opts, EMU_LIB, en, rel_damping=1e-5)
+    assert np.all(out["status"] == 0)
+    be = R.backward_error(J[0], r[0], cols, delta[0], lam)
+    assert be <= R.solve_limit(len(cols), "tiles"), (be, R.solve_limit(len(cols), "tiles"))
+
+
 def test_solver_plan_figures_humanoid_and_bodyhands():
     """Host planning of the solver path: elimination order + tile schedule + device-column layout + Gram plan. Guards the
     structural invariants the kernels rely on and the schedule quality reached in round 1 (levels / tiles of humanoid72)."""
