@@ -113,6 +113,11 @@ struct DeviceSchedule {
   GramPlan gram;          // tile-sparse Gram tables of the same plan (rows aligned to quads), when the plan has strips
   DeviceBuffer<int32_t> gBlob;
   int32_t gBlobInts{0}, gOffsets[8]{};
+  // gramCholeskyKernel's flattened tables: in its parameter block when they fit (gcParams), else in global memory (gcTab)
+  GramCholTables gc;
+  bool gcValid{false};
+  std::unique_ptr<GramCholParamTables> gcParams;
+  DeviceBuffer<uint16_t> gcTab;
   // fused persistent kernel (ik_fused.cuh): every table of the plan as one blob + how many instance groups fit beside it
   DeviceBuffer<int32_t> fBlob;
   FusedBlobLayout fLayout{};
@@ -157,6 +162,8 @@ struct mb2_solver {
   DeviceBuffer<double> dLastErrors, dTrialErrors, dHistory;
   DeviceBuffer<int32_t> dActive, dIterations, dStatus, dSearching, dActiveCount, dWorkCounter, dQrChunks;
   DeviceBuffer<unsigned long long> dPhaseCycles;
+  DeviceBuffer<float> dPark;          // gramCholeskyKernel: parked Gram tiles, one slot per resident CTA
+  DeviceBuffer<uint32_t> dParkSlots;  // its slot bitmap (zero between launches)
   bool lastFused{false}, lastGramChol{false};
   int lastFusedGroups{0};
   cudaEvent_t fusedStart{nullptr}, fusedStop{nullptr};
@@ -346,6 +353,14 @@ int ensurePlan(mb2_solver_function* f, int mode, bool schedDense = false, bool a
       makeGramBlob(ds->gram, ds->host, gblob, ds->gOffsets);
       ds->gBlobInts = int32_t(gblob.size());
       MB2_CUDA(ds->gBlob.upload(gblob, s));
+      ds->gcValid = makeGramCholTables(ds->gram, ds->host, ds->gc).empty(); // else the three-kernel path
+      if (ds->gcValid && ds->gc.tab.size() <= size_t(kGramCholParamEntries)) {
+        ds->gcParams = std::make_unique<GramCholParamTables>();
+        ds->gcParams->L = ds->gc.L;
+        std::copy(ds->gc.tab.begin(), ds->gc.tab.end(), ds->gcParams->tab);
+      } else if (ds->gcValid) {
+        MB2_CUDA(ds->gcTab.upload(ds->gc.tab, s));
+      }
       const int rc = buildFusedBlob(f, *ds, gblob, sblob, s);
       if (rc != MB2_OK) return rc;
     }
@@ -1009,7 +1024,8 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   if (useGram && useSchedule) {
     const DeviceSchedule& ds = *f->sched;
     const int rounds = std::max(int(ds.gram.tileOrder.size()) / kGramWarps, 1);
-    const bool fits = gramCholeskySmemBytes(size_t(ds.gram.stride), ds.gBlobInts, ns, ds.host.nPad, ds.host.numTiles, ds.dev.blobInts) <= size_t(200 * 1024) && rounds <= kGramCholMaxRounds;
+    const bool fits = gramCholeskySmemBytes(size_t(ds.gram.stride), ds.gBlobInts, ns, ds.host.nPad, ds.host.numTiles, ds.dev.blobInts) <= size_t(200 * 1024) && rounds <= kGramCholMaxRounds &&
+                      ds.gcValid;
     if (o.fused_mode == MB2_FUSED_GRAM_CHOLESKY && !fits) return fail(MB2_ERR_UNSUPPORTED, "Gram + Cholesky fusion: strips / tiles of this plan do not fit in shared memory, or too many tiles per warp");
     useGramChol = fits && (o.fused_mode == MB2_FUSED_AUTO || o.fused_mode == MB2_FUSED_GRAM_CHOLESKY);
   } else if (o.fused_mode == MB2_FUSED_GRAM_CHOLESKY) {
@@ -1184,7 +1200,24 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
       gc.c = c;
       gc.c.tilesIn = nullptr;
       gc.phaseCycles = s->inKernelProfile ? s->dPhaseCycles.p : nullptr;
-      MB2_CUDA(launchGramCholesky(gc, f->sched->dev, s->inKernelProfile, st));
+      const DeviceSchedule& ds = *f->sched;
+      gc.parkTiles = ds.gc.parkTiles;
+      if (gc.parkTiles > 0) {
+        const int slots = gramCholeskyParkSlots(gc, ds.dev, ds.gcParams != nullptr);
+        if (slots < 1) return fail(MB2_ERR_CUDA, "Gram + Cholesky fusion: no resident CTA");
+        if (s->dParkSlots.n < size_t(slots / 32)) { // grown only here, and every launch leaves it all zero
+          MB2_CUDA(s->dParkSlots.resize(size_t(slots / 32)));
+          MB2_CUDA(cudaMemsetAsync(s->dParkSlots.p, 0, s->dParkSlots.n * sizeof(uint32_t), st));
+        }
+        MB2_CUDA(s->dPark.resize(size_t(slots) * size_t(gc.parkTiles) * 256));
+        gc.park = s->dPark.p;
+        gc.parkSlots = s->dParkSlots.p;
+        gc.parkSlotWords = int32_t(slots / 32);
+      }
+      GramCholGlobalTables gt{};
+      gt.L = ds.gc.L;
+      gt.tab = ds.gcTab.p;
+      MB2_CUDA(launchGramCholesky(gc, ds.dev, ds.gcParams.get(), gt, s->inKernelProfile, st));
     } else if (useSchedule) MB2_CUDA(launchCholeskyScheduled(c, f->sched->dev, st));
     else MB2_CUDA(launchCholesky(c, st));
     recordPhaseStop(s, st);

@@ -411,6 +411,53 @@ void makeGramBlob(const GramPlan& g, const CholSchedule& s, std::vector<int32_t>
   if (blob.empty()) blob.push_back(0);
 }
 
+std::string makeGramCholTables(const GramPlan& g, const CholSchedule& s, GramCholTables& out) {
+  out = GramCholTables();
+  std::vector<uint16_t>& t = out.tab;
+  bool fits = true;
+  auto put = [&](int64_t v) { fits = fits && v >= 0 && v <= 0xFFFF; t.push_back(uint16_t(v)); };
+  auto section = [&]() { while (t.size() % 4) t.push_back(0); return int32_t(t.size()); };
+  auto validOf = [&](int K) { int v = 0; while (v < kCholTile && s.perm[16 * K + v] >= 0) ++v; return v; };
+  out.L.gram = section();
+  for (int32_t tile : g.tileOrder) {
+    if (tile < 0) { put(0xFFFF); put(0); put(0); put(0); continue; }
+    fits = fits && tile < 0xFFFF;
+    put(tile);
+    put(validOf(s.tileRow[tile]) | (validOf(s.tileCol[tile]) << 8) | ((s.tileRow[tile] == s.tileCol[tile] ? 1 : 0) << 15));
+    put(g.tileQuadStart[tile]); put(g.tileQuadStart[tile + 1]);
+  }
+  out.L.quad = section();
+  for (int32_t v : g.quad) put(v);
+  out.L.col = section();
+  for (int32_t v : g.colStripStart) put(v);
+  out.L.colEnt = section();
+  for (int32_t sidx : g.colStrip) { put(int64_t(sidx) * 64); put(g.stripCoord[2 * sidx]); }
+  out.L.level = section();
+  for (int L = 0; L <= s.numLevels; ++L) { put(s.levelColStart[L]); put(s.levelPanelStart[L]); put(s.levelOrderStart8[L]); put(s.levelVTaskStart[L]); }
+  out.L.diag = section();
+  for (int32_t K : s.levelCols) { put(K); put(s.diagTile[K]); put(s.colPanelStart[K]); put(s.colPanelStart[K + 1]); }
+  out.L.panel = section();
+  for (size_t pi = 0; pi < s.panelTile.size(); ++pi) { put(s.panelTile[pi]); put(s.panelDiag[pi]); }
+  out.L.order = section();
+  for (int32_t ti : s.taskOrder8) {
+    if (ti < 0) { put(0xFFFF); put(0); put(0); put(0); continue; }
+    fits = fits && s.taskDst[ti] < 0xFFFF;
+    put(s.taskDst[ti]); put(s.taskPairStart[ti]); put(s.taskPairStart[ti + 1]); put(0);
+  }
+  out.L.pair = section();
+  for (size_t p = 0; p < s.pairA.size(); ++p) { put(s.pairA[p]); put(s.pairB[p]); }
+  out.L.vtask = section();
+  for (size_t vi = 0; vi < s.vtaskRow.size(); ++vi) { put(s.vtaskRow[vi]); put(s.vtaskSrcStart[vi]); put(s.vtaskSrcStart[vi + 1]); put(0); }
+  out.L.vsrc = section();
+  for (size_t p = 0; p < s.vsrcTile.size(); ++p) { put(s.vsrcTile[p]); put(s.vsrcCol[p]); }
+  out.L.colPanel = section();
+  for (size_t p = 0; p < s.colPanelTile.size(); ++p) { put(s.colPanelTile[p]); put(s.colPanelRow[p]); }
+  section();
+  const int64_t onStrips = (int64_t(g.stride) + 64 + 255) / 256;
+  out.parkTiles = int32_t(std::min<int64_t>(s.numTiles, onStrips));
+  return fits ? "" : "Gram + Cholesky tables: an entry does not fit in 16 bits";
+}
+
 void layoutDeviceColumns(CholSchedule& s, std::vector<int32_t>& deviceColumnOrder) {
   deviceColumnOrder.clear();
   s.nParams = s.n;

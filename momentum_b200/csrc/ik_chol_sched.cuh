@@ -210,16 +210,43 @@ MB2_HD void gramTilePairs(const float* strips, int oa0, int ob0, int oa1, int ob
     }
 #endif
 }
-// quads: {A0, B0, A1, B1} float offsets per step (GramPlan::quad, pair lists padded to even length), staged in shared memory
-MB2_HD void gramTileAccumulate(const float* strips, const int32_t* quads, int q0, int q1, int lane, float d[2][4]) {
+// Four consecutive table entries (16-byte aligned int32 or 8-byte aligned uint16 records) as ONE warp-uniform read
+MB2_HD int4 tableRecord4(const int32_t* p) {
+#if defined(__CUDA_ARCH__)
+  return *reinterpret_cast<const int4*>(p);
+#else
+  int4 r; r.x = p[0]; r.y = p[1]; r.z = p[2]; r.w = p[3];
+  return r;
+#endif
+}
+MB2_HD int4 tableRecord4(const uint16_t* p) {
+  int4 r;
+#if defined(__CUDA_ARCH__)
+  const uint2 v = *reinterpret_cast<const uint2*>(p);
+  r.x = int(v.x & 0xFFFFu); r.y = int(v.x >> 16); r.z = int(v.y & 0xFFFFu); r.w = int(v.y >> 16);
+#else
+  r.x = p[0]; r.y = p[1]; r.z = p[2]; r.w = p[3];
+#endif
+  return r;
+}
+MB2_HD int2 tableRecord2(const uint16_t* p) {
+  int2 r;
+#if defined(__CUDA_ARCH__)
+  const uint32_t v = *reinterpret_cast<const uint32_t*>(p);
+  r.x = int(v & 0xFFFFu); r.y = int(v >> 16);
+#else
+  r.x = p[0]; r.y = p[1];
+#endif
+  return r;
+}
+// quads: {A0, B0, A1, B1} float offsets per step (GramPlan::quad, pair lists padded to even length): the int32 blob staged in shared
+// memory, or the 16-bit copy of gramCholeskyKernel's parameter block
+template <class Q>
+MB2_HD void gramTileAccumulate(const float* strips, const Q* quads, int q0, int q1, int lane, float d[2][4]) {
   float small[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
   for (int q = q0; q < q1; ++q) {
-#if defined(__CUDA_ARCH__)
-    const int4 o = *reinterpret_cast<const int4*>(quads + 4 * q); // one broadcast read
+    const int4 o = tableRecord4(quads + 4 * q); // one broadcast read
     gramTilePairs(strips, o.x, o.y, o.z, o.w, lane, d, small);
-#else
-    gramTilePairs(strips, quads[4 * q], quads[4 * q + 1], quads[4 * q + 2], quads[4 * q + 3], lane, d, small);
-#endif
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h)
@@ -242,14 +269,26 @@ MB2_HD void gramTileStore(float* tile, const float d[2][4], int info, float lamb
   tileStoreFrag(tile, lane, v);
 }
 // entry hl of block K of J^T r: sum over the strips of tile column K of strip[hl][0..3] . r[4q..4q+3]
+MB2_HD void gramVectorTerm(const float* strip, const float* r4, int hl, float& g0, float& g1) {
+  const float4 sv = *reinterpret_cast<const float4*>(strip + 4 * hl);
+  const float4 rv = *reinterpret_cast<const float4*>(r4);
+  g0 += sv.x * rv.x + sv.y * rv.y;
+  g1 += sv.z * rv.z + sv.w * rv.w;
+}
 MB2_HD float gramVectorEntry(const float* strips, const float* resid, const int32_t* colStrip, const int32_t* stripRow, int s0, int s1, int hl) {
   float g0 = 0.f, g1 = 0.f;
   for (int k = s0; k < s1; ++k) {
     const int sidx = colStrip[k];
-    const float4 sv = *reinterpret_cast<const float4*>(strips + size_t(sidx) * 64 + 4 * hl);
-    const float4 rv = *reinterpret_cast<const float4*>(resid + stripRow[sidx]);
-    g0 += sv.x * rv.x + sv.y * rv.y;
-    g1 += sv.z * rv.z + sv.w * rv.w;
+    gramVectorTerm(strips + size_t(sidx) * 64, resid + stripRow[sidx], hl, g0, g1);
+  }
+  return g0 + g1;
+}
+// the same sum over pre-resolved {strip float offset, first row} records (GramCholTables::colEnt)
+MB2_HD float gramVectorEntry(const float* strips, const float* resid, const uint16_t* colEnt, int s0, int s1, int hl) {
+  float g0 = 0.f, g1 = 0.f;
+  for (int k = s0; k < s1; ++k) {
+    const int2 e = tableRecord2(colEnt + 2 * k);
+    gramVectorTerm(strips + e.x, resid + e.y, hl, g0, g1);
   }
   return g0 + g1;
 }
@@ -403,15 +442,18 @@ MB2_HD void cholPanelProduct(const float* tile, const float* diagW, int lane, fl
 MB2_HD void cholPanelStore(float* tile, int lane, const float out[2][4]) { tileStoreFrag(tile, lane, out); }
 
 // ---- phase C: one update task, D(I,J) -= sum_K L(I,K) L(J,K)^T; a warp per destination tile ----
-MB2_HD void cholUpdateTask(float* tiles, const CholSchedDev& S, int task, int lane) {
+// pairs p0 .. p1 - 1 of the task: source tiles pairA[p * stride], pairB[p * stride] (the schedule's two arrays, or the {A, B} records
+// of GramCholTables with stride 2); dst = destination tile
+template <class I>
+MB2_HD void cholUpdateTile(float* tiles, const I* pairA, const I* pairB, int stride, int p0, int p1, int dst, int lane) {
   float d[2][4], small[2][4];
 #pragma unroll
   for (int h = 0; h < 2; ++h)
 #pragma unroll
     for (int e = 0; e < 4; ++e) { d[h][e] = 0.f; small[h][e] = 0.f; }
-  for (int p = S.taskPairStart[task]; p < S.taskPairStart[task + 1]; ++p)
-    tileProduct(tiles + size_t(S.pairA[p]) * 256, tiles + size_t(S.pairB[p]) * 256, lane, d, small);
-  float* D = tiles + size_t(S.taskDst[task]) * 256;
+  for (int p = p0; p < p1; ++p)
+    tileProduct(tiles + size_t(pairA[p * stride]) * 256, tiles + size_t(pairB[p * stride]) * 256, lane, d, small);
+  float* D = tiles + size_t(dst) * 256;
   float v[2][4];
   tileLoadFrag(D, lane, v);
 #pragma unroll
@@ -420,18 +462,26 @@ MB2_HD void cholUpdateTask(float* tiles, const CholSchedDev& S, int task, int la
     for (int e = 0; e < 4; ++e) v[h][e] -= d[h][e] + small[h][e];
   tileStoreFrag(D, lane, v);
 }
+MB2_HD void cholUpdateTask(float* tiles, const CholSchedDev& S, int task, int lane) {
+  cholUpdateTile(tiles, S.pairA, S.pairB, 1, S.taskPairStart[task], S.taskPairStart[task + 1], S.taskDst[task], lane);
+}
 
 // ---- phase C (vector part): y_I -= sum L(I,K) y_K over this level's columns; lane hl = row ----
-MB2_HD void cholVectorTask(const float* tiles, float* y, const CholSchedDev& S, int vtask, int hl) {
+// sources p0 .. p1 - 1: tile srcTile[p * stride] times block srcCol[p * stride] of y; row = the block of y it updates
+template <class I>
+MB2_HD void cholVectorRows(const float* tiles, float* y, const I* srcTile, const I* srcCol, int stride, int p0, int p1, int row, int hl) {
   float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f; // four partial sums: the dependent chain is 4 deep instead of 16 per source tile
-  for (int p = S.vtaskSrcStart[vtask]; p < S.vtaskSrcStart[vtask + 1]; ++p) {
+  for (int p = p0; p < p1; ++p) {
     float t[16];
-    tileLoadRow(tiles + size_t(S.vsrcTile[p]) * 256, hl, t);
-    const float* yk = y + S.vsrcCol[p] * 16;
+    tileLoadRow(tiles + size_t(srcTile[p * stride]) * 256, hl, t);
+    const float* yk = y + srcCol[p * stride] * 16;
 #pragma unroll
     for (int c = 0; c < 16; c += 4) { s0 += t[c] * yk[c]; s1 += t[c + 1] * yk[c + 1]; s2 += t[c + 2] * yk[c + 2]; s3 += t[c + 3] * yk[c + 3]; }
   }
-  y[S.vtaskRow[vtask] * 16 + hl] -= (s0 + s1) + (s2 + s3);
+  y[row * 16 + hl] -= (s0 + s1) + (s2 + s3);
+}
+MB2_HD void cholVectorTask(const float* tiles, float* y, const CholSchedDev& S, int vtask, int hl) {
+  cholVectorRows(tiles, y, S.vsrcTile, S.vsrcCol, 1, S.vtaskSrcStart[vtask], S.vtaskSrcStart[vtask + 1], S.vtaskRow[vtask], hl);
 }
 
 // ---- backward substitution for one tile column K: y_K <- L(K,K)^-T (y_K - sum_I L(I,K)^T y_I); ONE WARP per column ----
@@ -440,13 +490,15 @@ MB2_HD void cholVectorTask(const float* tiles, float* y, const CholSchedDev& S, 
 // column sums over all panel tiles of the column; ONE butterfly over the eight lanes that share t finishes them. (A half-warp per
 // column with lane c reading X(r, c) scalar by scalar would replay on bank conflicts: a row of the fragment layout is not a
 // conflict-free 4-byte access.)
-MB2_HD void cholBackwardColumn(const float* tiles, float* y, const CholSchedDev& S, int K, int lane) {
+// panels p0 .. p1 - 1 of column K: tile panelTile[p * stride] in block row panelRow[p * stride]; diag = the diagonal tile of K (holds W)
+template <class I>
+MB2_HD void cholBackwardPanels(const float* tiles, float* y, const I* panelTile, const I* panelRow, int stride, int p0, int p1, int K, int diag, int lane) {
 #if defined(__CUDA_ARCH__)
   const int g = lane >> 2, t = lane & 3, so = tileSlotOffset(lane);
   float c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f;
-  for (int p = S.colPanelStart[K]; p < S.colPanelStart[K + 1]; ++p) {
-    const float* T = tiles + size_t(S.colPanelTile[p]) * 256;
-    const float* yi = y + S.colPanelRow[p] * 16;
+  for (int p = p0; p < p1; ++p) {
+    const float* T = tiles + size_t(panelTile[p * stride]) * 256;
+    const float* yi = y + panelRow[p * stride] * 16;
     const float4 v0 = *reinterpret_cast<const float4*>(T + so), v1 = *reinterpret_cast<const float4*>(T + 128 + so);
     const float ya = yi[g], yb = yi[g + 8];
     c0 = fmaf(v0.x, ya, fmaf(v0.z, yb, c0)); c1 = fmaf(v0.y, ya, fmaf(v0.w, yb, c1));
@@ -461,7 +513,7 @@ MB2_HD void cholBackwardColumn(const float* tiles, float* y, const CholSchedDev&
   if (g == 0) { yk[2 * t] -= c0; yk[2 * t + 1] -= c1; yk[8 + 2 * t] -= c2; yk[9 + 2 * t] -= c3; } // s = y_K - sums
   __syncwarp();
   // x_K = W^T s with W = L(K,K)^-1 stored by phase A
-  const float* W = tiles + size_t(S.diagTile[K]) * 256;
+  const float* W = tiles + size_t(diag) * 256;
   const float4 w0 = *reinterpret_cast<const float4*>(W + so), w1 = *reinterpret_cast<const float4*>(W + 128 + so);
   const float sa = yk[g], sb = yk[g + 8];
   float x0 = fmaf(w0.x, sa, w0.z * sb), x1 = fmaf(w0.y, sa, w0.w * sb), x2 = fmaf(w1.x, sa, w1.z * sb), x3 = fmaf(w1.y, sa, w1.w * sb);
@@ -476,20 +528,23 @@ MB2_HD void cholBackwardColumn(const float* tiles, float* y, const CholSchedDev&
   if (lane != 0) return; // host emulation: one caller plays the warp
   float s[16];
   for (int c = 0; c < 16; ++c) s[c] = 0.f;
-  for (int p = S.colPanelStart[K]; p < S.colPanelStart[K + 1]; ++p) {
-    const float* T = tiles + size_t(S.colPanelTile[p]) * 256;
-    const float* yi = y + S.colPanelRow[p] * 16;
+  for (int p = p0; p < p1; ++p) {
+    const float* T = tiles + size_t(panelTile[p * stride]) * 256;
+    const float* yi = y + panelRow[p * stride] * 16;
     for (int c = 0; c < 16; ++c) for (int r = 0; r < 16; ++r) s[c] += T[tileIdx(r, c)] * yi[r];
   }
   float* yk = y + K * 16;
   for (int c = 0; c < 16; ++c) s[c] = yk[c] - s[c];
-  const float* W = tiles + size_t(S.diagTile[K]) * 256;
+  const float* W = tiles + size_t(diag) * 256;
   for (int c = 0; c < 16; ++c) {
     float x = 0.f;
     for (int r = 0; r < 16; ++r) x += W[tileIdx(r, c)] * s[r];
     yk[c] = x;
   }
 #endif
+}
+MB2_HD void cholBackwardColumn(const float* tiles, float* y, const CholSchedDev& S, int K, int lane) {
+  cholBackwardPanels(tiles, y, S.colPanelTile, S.colPanelRow, 1, S.colPanelStart[K], S.colPanelStart[K + 1], K, S.diagTile[K], lane);
 }
 
 } // namespace mb2

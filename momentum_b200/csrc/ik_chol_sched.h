@@ -73,8 +73,8 @@ inline int cholSchedLdH(int n) { return (n + 1 + 15) / 16 * 16; }
 // of strip(q,I)^T strip(q,J); block K of J^T r = sum over its strips of strip^T r[4q..4q+3].
 constexpr int kGramWarps = 8; // warps that share the tiles of one instance (gramTilesKernel, gramCholeskyKernel, a group of the fused kernel)
 // gramCholeskyKernel writes the tiles over the strips they are computed from: a finished tile that would land on strips still being
-// read waits in its warp's registers' spill space (thread-local memory, served by L1 / L2) until every warp is done with the strips.
-// Rounds of the tile-order table that one warp can hold that way.
+// read is parked in an L2 scratch slot until every warp is done with the strips. Rounds of the tile-order table per warp up to which
+// the solver takes that kernel (the limit it had when the parked tiles lived in a fixed per-thread array).
 constexpr int kGramCholMaxRounds = 8;
 struct GramPlan {
   int32_t numStrips{0}, numTiles{0}, numTileCols{0};
@@ -103,5 +103,30 @@ void makeGramBlob(const GramPlan& g, const CholSchedule& s, std::vector<int32_t>
 struct CholSchedDev;
 // Concatenates every table into one int32 blob; `dev` gets pointers into blob.data() (rebase them after uploading).
 void makeScheduleBlob(const CholSchedule& s, std::vector<int32_t>& blob, CholSchedDev& dev);
+
+// The tables gramCholeskyKernel walks, flattened so that every item of every phase is ONE read of pre-resolved 16-bit entries (no
+// tile -> range -> entry chains), small enough to travel in the kernel's parameter block (constant cache: the parked tiles and the
+// strips that go through L1 cannot evict it). Offsets of the sections below, in entries of `tab`; every record is 4 or 2 entries
+// and every section starts on a multiple of 4 entries (8 bytes):
+//   gram     [numOrder][4]     per (round, warp) of GramPlan::tileOrder: {tile (0xFFFF = idle), validI | validJ << 8 | diag << 15, q0, q1}
+//   quad     [numQuads][4]     GramPlan::quad (float offsets of the four strips of a step)
+//   col      [numTileCols + 1] GramPlan::colStripStart;   colEnt [..][2] {float offset of the strip, first row of its quad}
+//   level    [numLevels + 1][4] {first diagonal item, first panel, first update-order entry (8 warps), first vector task}
+//   diag     [..][4]           per entry of levelCols: {K, diagonal tile, first and end panel of column K (backward substitution)}
+//   panel    [..][2]           {panel tile, diagonal tile of its column}
+//   order    [..][4]           per entry of taskOrder8: {destination tile (0xFFFF = idle), first pair, end pair, 0}
+//   pair     [..][2]           {pairA, pairB}
+//   vtask    [..][4]           {row block, first source, end source, 0};   vsrc [..][2] {vsrcTile, vsrcCol}
+//   colPanel [..][2]           {colPanelTile, colPanelRow}
+struct GramCholLayout {
+  int32_t gram, quad, col, colEnt, level, diag, panel, order, pair, vtask, vsrc, colPanel;
+};
+struct GramCholTables {
+  GramCholLayout L{};
+  std::vector<uint16_t> tab;
+  int32_t parkTiles{0}; // tiles 0 .. parkTiles - 1 lie on the strips (tile * 256 < stride + 64): they are parked until the strips are dead
+};
+// Fails (non-empty message) when a value does not fit in 16 bits.
+std::string makeGramCholTables(const GramPlan& g, const CholSchedule& s, GramCholTables& out);
 
 } // namespace mb2

@@ -709,26 +709,45 @@ cudaError_t launchCholeskyScheduled(const CholArgs& a, const CholSchedDev& sched
 }
 
 // ------------------------------------------------------------------------------------------------
-// K2s + K3 fused (default on the tile path): one CTA per instance, three CTAs per SM.
-//   prologue   strips + residual of the instance, the Gram plan and the Cholesky schedule arrive as bulk copies on one mbarrier
+// K2s + K3 fused (default on the tile path): one CTA per instance, four CTAs per SM.
+//   prologue   strips + residual of the instance arrive as bulk copies on one mbarrier; the CTA takes a parking slot
 //   Gram       a warp owns a tile at a time (longest-first assignment); a finished tile that lies beyond the strips is stored at
-//              once, one that would overwrite strips still being read is parked in thread-local memory (L1 / L2)
-//   restore    parked accumulators -> 16x16 tiles of J^T J + lambda I in the Cholesky layout, over the dead strips
+//              once, one that would overwrite strips still being read is parked in the CTA's scratch slot (L2-only stores)
+//   restore    parked accumulators -> 16x16 tiles of J^T J + lambda I in the Cholesky layout, over the dead strips; slot released
 //   Cholesky   level-scheduled tile factorisation, both substitutions, theta -= delta, SolverT bookkeeping (cholFinish)
 // The stored tiles (0.45 GB per iteration on the cfg3 shard) never exist in HBM and the second launch is gone.
 // ------------------------------------------------------------------------------------------------
 size_t gramCholeskySmemBytes(size_t stripStride, int gramBlobInts, int n, int nPad, int numTiles, int schedBlobInts) {
-  (void)gramBlobInts; (void)schedBlobInts; // the plan tables stay in global memory (L1): see the kernel
+  (void)gramBlobInts; (void)schedBlobInts; // the plan tables are not staged in shared memory: see the kernel
   const size_t uni = std::max<size_t>(size_t(numTiles) * 256, stripStride + 64);
   return 128 + sizeof(float) * (((uni + 3) & ~size_t(3)) + size_t(nPad) + size_t((n + 3) & ~3)) + 32;
 }
 
+// A free parking slot (see GramCholArgs): the search starts at a word that depends on the instance so that the CTAs of a wave do not
+// all contend for the first word.
+__device__ int acquireParkSlot(uint32_t* words, int numWords, int start) {
+  for (int w = start % numWords;; w = (w + 1 == numWords) ? 0 : w + 1) {
+    uint32_t freeBits = ~__ldcg(words + w);
+    while (freeBits != 0u) {
+      const int bit = __ffs(freeBits) - 1;
+      if ((atomicOr(words + w, 1u << bit) & (1u << bit)) == 0u) return 32 * w + bit;
+      freeBits &= freeBits - 1u;
+    }
+  }
+}
+
 // Shared memory holds only what is per instance: the strip / tile union, the right-hand side in slot order and J^T r per device column
-// (cfg3: 54.9 KB), so that FOUR CTAs fit on an SM (with the 1 KB reserved per block, 64 registers per thread); the Gram plan and the Cholesky schedule
-// (10 KB, identical for every CTA) are read from global memory through L1 by the same device functions. The per-instance critical
-// path is a chain of dependent phases no wider than a few warps: instances in flight per SM are what buys throughput.
-template <bool kProfile>
-__global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const GramCholArgs a, const CholSchedDev S) {
+// (cfg3: 54.9 KB), so that FOUR CTAs fit on an SM (with the 1 KB reserved per block, 64 registers per thread). That leaves ~28 KB of
+// L1 per SM, so neither the plan nor the parked tiles go through it:
+//   * the plan (GramCholTables: about 2 k entries on cfg3) is read from the kernel's parameter block through the constant cache (Tables =
+//     GramCholParamTables), or from global memory when it does not fit there (GramCholGlobalTables). Every item of every phase is
+//     one warp-uniform read of a pre-resolved record, where the schedule blob took a chain of two or three dependent reads;
+//   * a parked tile goes to the CTA's scratch slot with L2-only stores and comes back with L2-only loads: no stack frame, and
+//     the slots of the resident CTAs (cfg3: 544 x 30 KB) stay in L2.
+// The per-instance critical path is a chain of dependent phases no wider than a few warps: instances in flight per SM are what
+// buys throughput. The per-tile arithmetic is that of gramTilesKernel + choleskyScheduledKernel (the same device functions).
+template <bool kProfile, class Tables>
+__global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const GramCholArgs a, const CholSchedDev S, const __grid_constant__ Tables P) {
   extern __shared__ __align__(16) float gcSmem[];
   const GramArgs& g = a.g;
   const CholArgs& c = a.c;
@@ -736,7 +755,7 @@ __global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const Gram
   if (c.active[b] == 0) return;
   const int n = c.ns, tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31, hw = tid >> 4, hl = tid & 15;
-  const unsigned hmask = 0xFFFFu << (16 * ((tid >> 4) & 1));
+  constexpr int kWarps = kGramThreads / 32;
   float* U = gcSmem + (((128u - (smemAddr(gcSmem) & 127u)) & 127u) >> 2); // strips | residual | zero strip, later the tiles
   const size_t tileFloats = size_t(S.numTiles) * 256, sweepFloats = g.stripStride + 64;
   const size_t uni = ((tileFloats > sweepFloats ? tileFloats : sweepFloats) + 3) & ~size_t(3);
@@ -745,8 +764,10 @@ __global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const Gram
   float* tiles = U;
   float* y = U + uni;
   float* gsub = y + S.nPad;
-  int* flags = reinterpret_cast<int*>(gsub + ((n + 3) & ~3));
+  int* flags = reinterpret_cast<int*>(gsub + ((n + 3) & ~3)); // [0] breakdown, [1] parking slot
   unsigned long long* bar = reinterpret_cast<unsigned long long*>(flags + 4);
+  const uint16_t* tab = P.tab;
+  const GramCholLayout& L = P.L;
   long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, pt = 0;
   if constexpr (kProfile) pt = clock64();
 #define MB2_GC(k) if constexpr (kProfile) { const long long now = clock64(); pc[k] += now - pt; pt = now; }
@@ -759,78 +780,87 @@ __global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const Gram
     mbarExpectTx(barAddr, stripBytes);
     const char* src = reinterpret_cast<const char*>(g.strips + size_t(b) * g.stripStride);
     for (uint32_t off = 0; off < stripBytes; off += 16384u) bulkLoad(smemAddr(strips) + off, src + off, stripBytes - off < 16384u ? stripBytes - off : 16384u, barAddr);
+    flags[1] = a.parkTiles > 0 ? acquireParkSlot(a.parkSlots, a.parkSlotWords, b) : 0; // (overlaps the copy)
   }
   if (tid >= 64 && tid < 128) strips[g.stripStride + (tid - 64)] = 0.f; // the all-zero strip that pads odd pair lists
   __syncthreads();
   mbarWaitRelaxed(barAddr, 0);
   MB2_GC(0)
-  const int32_t* __restrict__ gtab = g.blob;
-  const int32_t* tileOrder = gtab + g.offTileOrder, *tileQuadStart = gtab + g.offTilePairStart, *quads = gtab + g.offPairA;
-  const int32_t* colStripStart = gtab + g.offColStripStart, *colStrip = gtab + g.offColStrip, *stripRow = gtab + g.offStripRow, *tileInfo = gtab + g.offTileInfo;
+  // this CTA's parked tile t, lane's two float4: park + t * 256 + {4 lane, 128 + 4 lane} (coalesced 512-byte warp accesses)
+  float* park = a.park + size_t(flags[1]) * size_t(a.parkTiles) * 256 + 4 * lane;
+  const int rounds = g.numOrder / kWarps;
+  auto tileInfoOf = [](int packed) { return (packed & 0x7FFF) | ((packed >> 15) << 16); }; // GramCholTables::gram -> tileInfo
   // ---- Gram ----
-  float parked[kGramCholMaxRounds][8]; // indexed by the round: thread-local memory
-  {
-    int slot = 0;
-    for (int ti = warp; ti < g.numOrder; ti += kGramThreads / 32, ++slot) {
-      const int t = tileOrder[ti];
-      if (t < 0) continue;
-      float acc[2][4];
+  for (int r = 0; r < rounds; ++r) {
+    const int4 rec = tableRecord4(tab + L.gram + 4 * (r * kWarps + warp)); // {tile, packed info, q0, q1}
+    if (rec.x == 0xFFFF) continue;
+    float acc[2][4];
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
+    for (int i = 0; i < 2; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-      gramTileAccumulate(strips, quads, tileQuadStart[t], tileQuadStart[t + 1], lane, acc);
-      if (size_t(t) * 256 >= sweepFloats) gramTileStore(tiles + size_t(t) * 256, acc, tileInfo[t], g.regularization, lane);
-      else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) parked[slot][i] = acc[i >> 2][i & 3];
-      }
+      for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    gramTileAccumulate(strips, tab + L.quad, rec.z, rec.w, lane, acc);
+    if (rec.x >= a.parkTiles) gramTileStore(tiles + size_t(rec.x) * 256, acc, tileInfoOf(rec.y), g.regularization, lane);
+    else {
+      __stcg(reinterpret_cast<float4*>(park + size_t(rec.x) * 256), make_float4(acc[0][0], acc[0][1], acc[0][2], acc[0][3]));
+      __stcg(reinterpret_cast<float4*>(park + size_t(rec.x) * 256 + 128), make_float4(acc[1][0], acc[1][1], acc[1][2], acc[1][3]));
     }
-    for (int K = hw; K < S.numTileCols; K += kGramThreads / 16)
-      y[16 * K + hl] = gramVectorEntry(strips, resid, colStrip, stripRow, colStripStart[K], colStripStart[K + 1], hl);
   }
+  for (int K = hw; K < S.numTileCols; K += kGramThreads / 16)
+    y[16 * K + hl] = gramVectorEntry(strips, resid, tab + L.colEnt, int(tab[L.col + K]), int(tab[L.col + K + 1]), hl);
   __syncthreads();
   MB2_GC(1)
-  {
-    int slot = 0;
-    for (int ti = warp; ti < g.numOrder; ti += kGramThreads / 32, ++slot) {
-      const int t = tileOrder[ti];
-      if (t < 0 || size_t(t) * 256 >= sweepFloats) continue;
-      float acc[2][4];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) acc[i >> 2][i & 3] = parked[slot][i];
-      gramTileStore(tiles + size_t(t) * 256, acc, tileInfo[t], g.regularization, lane);
-    }
-    for (int s2 = tid; s2 < S.nPad; s2 += kGramThreads) {
-      const int p = S.perm[s2];
-      if (p >= 0) gsub[p] = y[s2];
-    }
+  for (int r = 0; r < rounds; ++r) {
+    const int4 rec = tableRecord4(tab + L.gram + 4 * (r * kWarps + warp));
+    if (rec.x == 0xFFFF || rec.x >= a.parkTiles) continue;
+    const float4 v0 = __ldcg(reinterpret_cast<const float4*>(park + size_t(rec.x) * 256));
+    const float4 v1 = __ldcg(reinterpret_cast<const float4*>(park + size_t(rec.x) * 256 + 128));
+    const float acc[2][4] = {{v0.x, v0.y, v0.z, v0.w}, {v1.x, v1.y, v1.z, v1.w}};
+    gramTileStore(tiles + size_t(rec.x) * 256, acc, tileInfoOf(rec.y), g.regularization, lane);
+  }
+  for (int s2 = tid; s2 < S.nPad; s2 += kGramThreads) {
+    const int p = S.perm[s2];
+    if (p >= 0) gsub[p] = y[s2];
   }
   __syncthreads();
+  // every parked value has been read (it sits in the tiles now): the slot is free for the next CTA
+  if (tid == 0 && a.parkTiles > 0) atomicAnd(a.parkSlots + (flags[1] >> 5), ~(1u << (flags[1] & 31)));
   MB2_GC(2)
   // ---- level-scheduled Cholesky (same phases as choleskyScheduledKernel) ----
-  for (int L = 0; L < S.numLevels; ++L) {
-    for (int ci = S.levelColStart[L] + warp; ci < S.levelColStart[L + 1]; ci += kGramThreads / 32) {
-      const int K = S.levelCols[ci];
-      cholDiagTile(tiles + size_t(S.diagTile[K]) * 256, y + 16 * K, lane, c.regularization, flags);
+  for (int Lv = 0; Lv < S.numLevels; ++Lv) {
+    const int4 l0 = tableRecord4(tab + L.level + 4 * Lv), l1 = tableRecord4(tab + L.level + 4 * (Lv + 1)); // {diag, panel, order, vtask}
+    for (int ci = l0.x + warp; ci < l1.x; ci += kWarps) {
+      const int4 d = tableRecord4(tab + L.diag + 4 * ci); // {K, diagonal tile, ...}
+      cholDiagTile(tiles + size_t(d.y) * 256, y + 16 * d.x, lane, c.regularization, flags);
     }
     __syncthreads();
     MB2_GC(3)
-    for (int pi = S.levelPanelStart[L] + warp; pi < S.levelPanelStart[L + 1]; pi += kGramThreads / 32) {
-      float* ptile = tiles + size_t(S.panelTile[pi]) * 256;
+    for (int pi = l0.y + warp; pi < l1.y; pi += kWarps) {
+      const int2 pe = tableRecord2(tab + L.panel + 2 * pi);
+      float* ptile = tiles + size_t(pe.x) * 256;
       float x[2][4];
-      cholPanelProduct(ptile, tiles + size_t(S.panelDiag[pi]) * 256, lane, x);
+      cholPanelProduct(ptile, tiles + size_t(pe.y) * 256, lane, x);
       cholPanelStore(ptile, lane, x);
     }
     __syncthreads();
     MB2_GC(4)
-    for (int oi = S.levelOrderStart8[L] + warp; oi < S.levelOrderStart8[L + 1]; oi += kGramThreads / 32) { const int ti = S.taskOrder8[oi]; if (ti >= 0) cholUpdateTask(tiles, S, ti, lane); }
-    for (int vi = S.levelVTaskStart[L] + hw; vi < S.levelVTaskStart[L + 1]; vi += kGramThreads / 16) cholVectorTask(tiles, y, S, vi, hl);
+    for (int oi = l0.z + warp; oi < l1.z; oi += kWarps) {
+      const int4 o = tableRecord4(tab + L.order + 4 * oi); // {destination, first pair, end pair}
+      if (o.x != 0xFFFF) cholUpdateTile(tiles, tab + L.pair, tab + L.pair + 1, 2, o.y, o.z, o.x, lane);
+    }
+    for (int vi = l0.w + hw; vi < l1.w; vi += kGramThreads / 16) {
+      const int4 v = tableRecord4(tab + L.vtask + 4 * vi); // {row block, first source, end source}
+      cholVectorRows(tiles, y, tab + L.vsrc, tab + L.vsrc + 1, 2, v.y, v.z, v.x, hl);
+    }
     __syncthreads();
     MB2_GC(5)
   }
-  for (int L = S.numLevels - 1; L >= 0; --L) {
-    for (int ci = S.levelColStart[L] + warp; ci < S.levelColStart[L + 1]; ci += kGramThreads / 32) cholBackwardColumn(tiles, y, S, S.levelCols[ci], lane);
+  for (int Lv = S.numLevels - 1; Lv >= 0; --Lv) {
+    const int c0 = tab[L.level + 4 * Lv], c1 = tab[L.level + 4 * (Lv + 1)];
+    for (int ci = c0 + warp; ci < c1; ci += kWarps) {
+      const int4 d = tableRecord4(tab + L.diag + 4 * ci); // {K, diagonal tile, first panel, end panel}
+      cholBackwardPanels(tiles, y, tab + L.colPanel, tab + L.colPanel + 1, 2, d.z, d.w, d.x, d.y, lane);
+    }
     __syncthreads();
   }
   MB2_GC(6)
@@ -845,18 +875,41 @@ __global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const Gram
 #undef MB2_GC
 }
 
-cudaError_t launchGramCholesky(const GramCholArgs& a, const CholSchedDev& sched, bool profile, cudaStream_t stream) {
+template <bool kProfile, class Tables>
+static cudaError_t prepareGramCholesky(size_t smem) {
+  cudaError_t e = cudaFuncSetAttribute(gramCholeskyKernel<kProfile, Tables>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(gramCholeskyKernel<kProfile, Tables>, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared));
+}
+
+int gramCholeskyParkSlots(const GramCholArgs& a, const CholSchedDev& sched, bool paramTables) {
+  const size_t smem = gramCholeskySmemBytes(a.g.stripStride, a.g.blobInts, a.c.ns, sched.nPad, sched.numTiles, sched.blobInts);
+  // the profiling instantiations carry more registers: never more resident CTAs than the production ones
+  cudaError_t e = paramTables ? prepareGramCholesky<false, GramCholParamTables>(smem) : prepareGramCholesky<false, GramCholGlobalTables>(smem);
+  int perSm = 0;
+  if (e == cudaSuccess)
+    e = paramTables ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, gramCholeskyKernel<false, GramCholParamTables>, kGramThreads, smem)
+                    : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, gramCholeskyKernel<false, GramCholGlobalTables>, kGramThreads, smem);
+  if (e != cudaSuccess || perSm < 1) return -1;
+  return (g_numSms * perSm + 31) / 32 * 32;
+}
+
+cudaError_t launchGramCholesky(const GramCholArgs& a, const CholSchedDev& sched, const GramCholParamTables* inParams, const GramCholGlobalTables& inGlobal, bool profile,
+                               cudaStream_t stream) {
   const size_t smem = gramCholeskySmemBytes(a.g.stripStride, a.g.blobInts, a.c.ns, sched.nPad, sched.numTiles, sched.blobInts);
   if (smem > size_t(g_maxSmemOptin) || (a.g.stripStride & 3) != 0) return cudaErrorInvalidConfiguration;
-  if (a.g.numOrder > kGramCholMaxRounds * (kGramThreads / 32)) return cudaErrorInvalidConfiguration; // parked tiles per warp
-  cudaError_t e = profile ? cudaFuncSetAttribute(gramCholeskyKernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem))
-                          : cudaFuncSetAttribute(gramCholeskyKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (a.parkTiles > 0 && (a.park == nullptr || a.parkSlots == nullptr || a.parkSlotWords < 1)) return cudaErrorInvalidValue;
+  cudaError_t e;
+  if (inParams != nullptr) e = profile ? prepareGramCholesky<true, GramCholParamTables>(smem) : prepareGramCholesky<false, GramCholParamTables>(smem);
+  else e = profile ? prepareGramCholesky<true, GramCholGlobalTables>(smem) : prepareGramCholesky<false, GramCholGlobalTables>(smem);
   if (e != cudaSuccess) return e;
-  e = profile ? cudaFuncSetAttribute(gramCholeskyKernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared))
-              : cudaFuncSetAttribute(gramCholeskyKernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, int(cudaSharedmemCarveoutMaxShared));
-  if (e != cudaSuccess) return e;
-  if (profile) gramCholeskyKernel<true><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched);
-  else gramCholeskyKernel<false><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched);
+  if (inParams != nullptr) {
+    if (profile) gramCholeskyKernel<true, GramCholParamTables><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched, *inParams);
+    else gramCholeskyKernel<false, GramCholParamTables><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched, *inParams);
+  } else {
+    if (profile) gramCholeskyKernel<true, GramCholGlobalTables><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched, inGlobal);
+    else gramCholeskyKernel<false, GramCholGlobalTables><<<a.c.batch, kGramThreads, smem, stream>>>(a, sched, inGlobal);
+  }
   return cudaGetLastError();
 }
 

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include "ik_chol_sched.cuh"
+#include "ik_chol_sched.h"
 #include "ik_types.h"
 
 namespace mb2 {
@@ -85,15 +86,36 @@ struct GramArgs {            // K2s: stored tiles of J^T J + lambda I and J^T r 
 cudaError_t launchGramTiles(const GramArgs& a, cudaStream_t stream);
 size_t gramTilesSmemBytes(size_t stripStride, int blobInts);
 
-// K2s + K3 in one launch: strips in (bulk copy), tiles beyond the strips stored at once, the others parked in thread-local memory
-// and written over the strips once they are dead, tile Cholesky, update. No second launch; `g.out` is unused.
+// K2s + K3 in one launch: strips in (bulk copy), tiles beyond the strips stored at once, the others parked in an L2-resident scratch
+// slot and written over the strips once they are dead, tile Cholesky, update. No second launch; `g.out` is unused.
 struct GramCholArgs {
   GramArgs g;
   CholArgs c;
   unsigned long long* phaseCycles; // optional [8], profiling instantiation: prologue, gram, parked tiles, diag, panel, update, backward, finish (block 0)
+  // Parked tiles: a CTA takes one of 32 * parkSlotWords slots (a set bit of parkSlots = taken; all zero between launches) for the
+  // Gram phase, and holds its tiles 0 .. parkTiles - 1 at park + (slot * parkTiles + tile) * 256 floats. At least as many slots as
+  // CTAs can be resident (gramCholeskyParkSlots), so a free one always exists.
+  float* park;
+  uint32_t* parkSlots;
+  int32_t parkSlotWords, parkTiles;
+};
+// gramCholeskyKernel's flattened tables (GramCholTables): in the kernel's parameter block (read through the constant cache) when
+// they fit, else in global memory
+constexpr int kGramCholParamEntries = 8192;
+struct alignas(16) GramCholParamTables {
+  GramCholLayout L;
+  uint16_t tab[kGramCholParamEntries];
+};
+struct GramCholGlobalTables {
+  GramCholLayout L;
+  const uint16_t* tab;
 };
 size_t gramCholeskySmemBytes(size_t stripStride, int gramBlobInts, int n, int nPad, int numTiles, int schedBlobInts);
-cudaError_t launchGramCholesky(const GramCholArgs& a, const CholSchedDev& sched, bool profile, cudaStream_t stream);
+// scratch slots for the parked tiles: resident CTAs of the launch on this device, rounded up to whole 32-bit words of parkSlots
+int gramCholeskyParkSlots(const GramCholArgs& a, const CholSchedDev& sched, bool paramTables);
+// tables: exactly one of inParams (non-null) or inGlobal is used
+cudaError_t launchGramCholesky(const GramCholArgs& a, const CholSchedDev& sched, const GramCholParamTables* inParams, const GramCholGlobalTables& inGlobal, bool profile,
+                               cudaStream_t stream);
 
 // QR-accurate linear step (ik_qr.cu): Householder sweeps of the K-major Jacobian into a shared-memory R, replaces JtJ + Cholesky
 struct QrArgs {
