@@ -248,6 +248,17 @@ int mb2_solver_function_get_jtjr(mb2_solver_function* f, const float* parameters
 /* Skeleton state after initializeJacobianComputation (skeleton_state.cpp:87-121): [B][J][8] (t,q,s) */
 int mb2_solver_function_get_skeleton_state(mb2_solver_function* f, const float* parameters, float* state);
 
+/* Differentiable forward kinematics on the character alone, device memory in and out, on `cuda_stream` (NULL = the legacy default
+ * stream), asynchronous. batch == 0 is a no-op. A null pointer (batch > 0), batch < 0, or a pointer that is not device memory on the
+ * character's device is MB2_ERR_INVALID_ARGUMENT.
+ * pymomentum model_parameters_to_skeleton_state (tensor_skeleton_state.cpp:500-502, :213-270): [B][n] -> [B][J][8] (t, q xyzw, s) */
+int mb2_character_skeleton_state_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                        float* skeleton_state_device, void* cuda_stream);
+/* its backward (computeSkelStateBackward, :62-134, then the ParameterTransform transposed): dLoss/dtheta [B][n], overwritten */
+int mb2_character_skeleton_state_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                 const float* grad_skeleton_state_device, float* grad_model_parameters_device,
+                                                 void* cuda_stream);
+
 /* ---- GaussNewtonSolverT<float> x B (solver/gauss_newton_solver.h:67-137, solver/solver.h:36-100) ---- */
 int mb2_solver_create(mb2_solver_function* f, const mb2_gauss_newton_options* opt, mb2_solver** out);
 void mb2_solver_destroy(mb2_solver* s);

@@ -103,6 +103,8 @@ struct mb2_character {
   HostCharacter host;
   DeviceBuffer<int32_t> parent, ptOuter, ptInner, levelStart, levelJoints;
   DeviceBuffer<float> offset, prerot, ptVals, ptOffsets;
+  DeviceBuffer<int32_t> childStart, children, ptColStart, ptColRows; // skeleton-state backward (HostCharacter::buildBackwardTables)
+  DeviceBuffer<float> ptColVals;
   uint64_t limitsVersion{0};
 };
 
@@ -553,6 +555,11 @@ int mb2_character_create(int device, int32_t J, const int32_t* parents, const fl
   MB2_CUDA(c->ptOffsets.upload(h.ptOffsets, nullptr));
   MB2_CUDA(c->levelStart.upload(h.levelStart, nullptr));
   MB2_CUDA(c->levelJoints.upload(h.levelJoints, nullptr));
+  MB2_CUDA(c->childStart.upload(h.childStart, nullptr));
+  MB2_CUDA(c->children.upload(h.children, nullptr));
+  MB2_CUDA(c->ptColStart.upload(h.ptColStart, nullptr));
+  MB2_CUDA(c->ptColRows.upload(h.ptColRows, nullptr));
+  MB2_CUDA(c->ptColVals.upload(h.ptColVals, nullptr));
   MB2_CUDA(cudaStreamSynchronize(nullptr));
   *out = c.release();
   return MB2_OK;
@@ -868,6 +875,62 @@ int mb2_solver_function_get_skeleton_state(mb2_solver_function* f, const float* 
   MB2_CUDA(cudaMemcpyAsync(state, f->dState.p, sz * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
   MB2_CUDA(cudaStreamSynchronize(f->stream));
   return MB2_OK;
+}
+
+namespace {
+bool isDeviceMemoryOn(const void* p, int device) {
+  cudaPointerAttributes attr{};
+  if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) { cudaGetLastError(); return false; }
+  return attr.type == cudaMemoryTypeDevice && attr.device == device;
+}
+
+// both directions of mb2_character_skeleton_state*_device (gradState is read by the backward only)
+int skeletonStateDevice(const mb2_character* c, int32_t batch, const float* theta, const float* gradState, float* out, void* stream, bool backward) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(batch >= 0, "batch must not be negative");
+  if (batch == 0) return MB2_OK;
+  MB2_CHECK(theta != nullptr && out != nullptr && (!backward || gradState != nullptr), "null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(isDeviceMemoryOn(theta, c->device) && isDeviceMemoryOn(out, c->device) && (!backward || isDeviceMemoryOn(gradState, c->device)),
+            "skeleton state: every array must be device memory on the character's device");
+  NvtxRange range(backward ? "skeletonStateBackward" : "skeletonState");
+  const HostCharacter& h = c->host;
+  SkeletonStateArgs a{};
+  a.T.numJoints = h.numJoints;
+  a.T.numParams = h.numParams;
+  a.T.parent = c->parent.p;
+  a.T.offset = c->offset.p;
+  a.T.prerot = c->prerot.p;
+  a.T.ptOuter = c->ptOuter.p;
+  a.T.ptInner = c->ptInner.p;
+  a.T.ptVals = c->ptVals.p;
+  a.T.ptOffsets = c->ptOffsets.p;
+  a.T.numLevels = int(h.levelStart.size()) - 1;
+  a.T.levelStart = c->levelStart.p;
+  a.T.levelJoints = c->levelJoints.p;
+  a.T.ptNnz = int(h.ptInner.size());
+  a.S.childStart = c->childStart.p;
+  a.S.children = c->children.p;
+  a.S.ptColStart = c->ptColStart.p;
+  a.S.ptColRows = c->ptColRows.p;
+  a.S.ptColVals = c->ptColVals.p;
+  a.numChildren = int(h.children.size());
+  a.batch = batch;
+  a.theta = theta;
+  a.gradState = gradState;
+  a.out = out;
+  MB2_CUDA(launchSkeletonState(a, backward, (cudaStream_t)stream));
+  return MB2_OK;
+}
+} // namespace
+
+int mb2_character_skeleton_state_device(const mb2_character* c, int32_t batch, const float* model_parameters_device, float* skeleton_state_device,
+                                        void* cuda_stream) {
+  return skeletonStateDevice(c, batch, model_parameters_device, nullptr, skeleton_state_device, cuda_stream, false);
+}
+int mb2_character_skeleton_state_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                 const float* grad_skeleton_state_device, float* grad_model_parameters_device, void* cuda_stream) {
+  return skeletonStateDevice(c, batch, model_parameters_device, grad_skeleton_state_device, grad_model_parameters_device, cuda_stream, true);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -224,6 +224,66 @@ MB2_HD F3 pointDerivative(const FunctionTables& T, const float* js, int a, int d
   return off * kLn2;
 }
 
+// ---- Backward of the skeleton state (t, q = (v, w), s) of every joint with respect to the model parameters ----
+// Each joint-parameter DOF of joint a moves the joints of its subtree sub(a) rigidly (the same derivatives pointDerivative uses):
+//   translation k:  dt_i = B_a e_k                      (B_a = translationAxisCol)
+//   rotation k:     dt_i = w x (t_i - t_a), dq_i = 1/2 (w, 0) (x) q_i   (w = rotationAxisCol k)
+//   scale:          dt_i = ln2 (t_i - t_a), ds_i = ln2 s_i
+// so with the upstream gradient G_i = (g_t, g_v, g_w, g_s) every joint needs 11 subtree sums, accumulated once from the leaves up
+// (O(J) instead of one ancestor walk per joint and DOF):
+//   [0..2] S_g = sum g_t    [3..5] R = sum (t_i - t_a) x g_t    [6] D = sum (t_i - t_a) . g_t
+//   [7..9] S_c = sum 1/2 (w_i g_v + v_i x g_v - g_w v_i)        [10] S_s = sum s_i g_s
+// R and D are kept relative to the joint's own origin and shifted once per child edge: the form sum t_i x g - t_a x sum g cancels
+// catastrophically for a rig far from the origin.
+constexpr int kSkelAccStride = 11; // odd: conflict-free with lanes = joints
+
+// the joint's own term (its subtree before any child is folded in); g: the joint's 8 upstream gradient floats
+MB2_HD void skelGradSeed(const float* js, int i, const float* g, float* acc) {
+  const float* ps = js + i * kJointStateStride;
+  const F3 v = ld3(ps + 3), gv = ld3(g + 3);
+  const float w = ps[6], gw = g[6];
+  const F3 sc = 0.5f * (w * gv + cross(v, gv) - gw * v);
+  float* a = acc + i * kSkelAccStride;
+  a[0] = g[0]; a[1] = g[1]; a[2] = g[2];
+  a[3] = 0.f; a[4] = 0.f; a[5] = 0.f; a[6] = 0.f;
+  a[7] = sc.x; a[8] = sc.y; a[9] = sc.z;
+  a[10] = ps[7] * g[7];
+}
+// adds the children's finished subtree sums to joint a, children in ascending index order (deterministic)
+MB2_HD void skelGradFold(const SkeletonTables& S, const float* js, int a, float* acc) {
+  float* A = acc + a * kSkelAccStride;
+  const F3 ta = ld3(js + a * kJointStateStride);
+  F3 sg = ld3(A), r = ld3(A + 3), sc = ld3(A + 7);
+  float d = A[6], ss = A[10];
+  for (int k = S.childStart[a]; k < S.childStart[a + 1]; ++k) {
+    const int c = S.children[k];
+    const float* C = acc + c * kSkelAccStride;
+    const F3 off = ld3(js + c * kJointStateStride) - ta, sgc = ld3(C);
+    r = r + (ld3(C + 3) + cross(off, sgc));
+    d = d + (C[6] + dot(off, sgc));
+    sg = sg + sgc;
+    sc = sc + ld3(C + 7);
+    ss = ss + C[10];
+  }
+  A[0] = sg.x; A[1] = sg.y; A[2] = sg.z;
+  A[3] = r.x; A[4] = r.y; A[5] = r.z; A[6] = d;
+  A[7] = sc.x; A[8] = sc.y; A[9] = sc.z; A[10] = ss;
+}
+// dLoss / d joint parameter `row` (= 7 a + k) from the finished sums of joint a; js holds the world state and DOF axes (fkAxis)
+MB2_HD float skelGradJointParameter(const FunctionTables& T, const float* js, const float* acc, int row) {
+  const int a = row / kParametersPerJoint, k = row - a * kParametersPerJoint;
+  const float* A = acc + a * kSkelAccStride;
+  if (k < 3) return dot(translationAxisCol(T, js, a, k), ld3(A));
+  if (k < 6) return dot(rotationAxisCol(js, a, k - 3), ld3(A + 3) + ld3(A + 7));
+  return kLn2 * (A[6] + A[10]);
+}
+// dLoss / d model parameter p = column p of the ParameterTransform against the joint-parameter gradient, rows ascending
+MB2_HD float skelGradModelParameter(const SkeletonTables& S, const float* gjp, int p) {
+  float s = 0.f;
+  for (int k = S.ptColStart[p]; k < S.ptColStart[p + 1]; ++k) s += S.ptColVals[k] * gjp[S.ptColRows[k]];
+  return s;
+}
+
 // ---- quaternion log map (math/utility.cpp:72-180) ----
 MB2_HD F3 quaternionLogMap(Q4 q) {
   const Q4 qn = qnormalized(q);

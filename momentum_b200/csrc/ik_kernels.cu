@@ -242,6 +242,144 @@ cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream)
   return jacobian ? pickStage(std::true_type{}) : pickStage(std::false_type{});
 }
 
+// ------------------------------------------------------------------------------------------------
+// Skeleton state of a batch of model parameters, and its backward (ik_device.cuh skelGrad*): a persistent grid, one group of W warps
+// per instance, the character tables staged in shared memory once per CTA.
+//   forward:   lanes = joints (local part from theta), level by level compose, [J][8] out
+//   backward:  the same FK with the DOF axes, then lanes = joints seed their 11 subtree sums from G, levels from the deepest up fold
+//              in their children, lanes = joint-parameter rows, lanes = model parameters over the CSC ParameterTransform.
+// Every output element is written by one lane in a fixed order: no atomics, the result does not depend on the launch shape.
+// ------------------------------------------------------------------------------------------------
+constexpr int kSkelMaxWarps = 16;
+MB2_HD size_t skelAligned(size_t floats) { return (floats + 3) & ~size_t(3); } // 16-byte aligned regions
+
+// per instance: theta [n], joint states [J][17], backward: subtree sums [J][11] and the joint-parameter gradient [7 J]
+MB2_HD size_t skeletonStateSmemPerInstanceFloats(int J, int n, bool backward) {
+  size_t f = skelAligned(size_t(n)) + skelAligned(size_t(J) * kJointStateStride);
+  if (backward) f += skelAligned(size_t(J) * kSkelAccStride) + skelAligned(size_t(J) * kParametersPerJoint);
+  return f;
+}
+size_t skeletonStateSmemPerInstance(const FunctionTables& T, bool backward) {
+  return sizeof(float) * skeletonStateSmemPerInstanceFloats(T.numJoints, T.numParams, backward);
+}
+
+size_t skeletonStateTableBytes(const SkeletonStateArgs& a, bool backward) {
+  const FunctionTables& T = a.T;
+  const size_t J = T.numJoints;
+  size_t w = tableWords(J, 4) + tableWords(3 * J, 4) + tableWords(4 * J, 4);                   // parent, offset, prerot
+  w += tableWords(7 * J + 1, 4) + tableWords(T.ptNnz, 4) * 2 + tableWords(7 * J, 4);          // ptOuter, ptInner, ptVals, ptOffsets
+  w += tableWords(T.numLevels + 1, 4) + tableWords(J, 4);                                     // levelStart, levelJoints
+  if (backward) w += tableWords(J + 1, 4) + tableWords(a.numChildren, 4) + tableWords(T.numParams + 1, 4) + tableWords(T.ptNnz, 4) * 2;
+  return w * 4;
+}
+
+template <bool kBackward, int W>
+__global__ void __launch_bounds__(32 * kSkelMaxWarps) skeletonStateKernel(const SkeletonStateArgs a) {
+  extern __shared__ __align__(16) float smem[];
+  FunctionTables T = a.T;
+  SkeletonTables S = a.S;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int group = warp / W, gl = (warp % W) * 32 + lane;
+  constexpr int gs = 32 * W;
+  const int groupsPerCta = (blockDim.x >> 5) / W;
+  const int J = T.numJoints, n = T.numParams;
+  const int thF = int(skelAligned(n)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
+  const int accF = kBackward ? int(skelAligned(size_t(J) * kSkelAccStride)) : 0;
+  const int perGroup = int(skeletonStateSmemPerInstanceFloats(J, n, kBackward));
+  float* th = smem + size_t(group) * perGroup;
+  float* js = th + thF;
+  float* acc = js + jsF;
+  float* gjp = acc + accF;
+  auto groupSync = [&]() {
+    if (W == 1) __syncwarp();
+    else asm volatile("bar.sync %0, %1;" ::"r"(1 + group), "r"(gs) : "memory");
+  };
+  {
+    uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
+    const size_t Jz = J;
+    stageTable(T.parent, Jz, cursor); stageTable(T.offset, 3 * Jz, cursor); stageTable(T.prerot, 4 * Jz, cursor);
+    stageTable(T.ptOuter, 7 * Jz + 1, cursor); stageTable(T.ptInner, T.ptNnz, cursor); stageTable(T.ptVals, T.ptNnz, cursor);
+    stageTable(T.ptOffsets, 7 * Jz, cursor);
+    stageTable(T.levelStart, T.numLevels + 1, cursor); stageTable(T.levelJoints, Jz, cursor);
+    if constexpr (kBackward) {
+      stageTable(S.childStart, Jz + 1, cursor); stageTable(S.children, a.numChildren, cursor);
+      stageTable(S.ptColStart, n + 1, cursor); stageTable(S.ptColRows, T.ptNnz, cursor); stageTable(S.ptColVals, T.ptNnz, cursor);
+    }
+    __syncthreads();
+  }
+  for (int b = blockIdx.x * groupsPerCta + group; b < a.batch; b += gridDim.x * groupsPerCta) {
+    const float* theta = a.theta + size_t(b) * n;
+    for (int i = gl; i < n; i += gs) th[i] = theta[i];
+    groupSync();
+    for (int j = gl; j < J; j += gs) fkLocalFromTheta<kBackward>(T, j, th, js);
+    groupSync();
+    for (int lvl = 1; lvl < T.numLevels; ++lvl) { // level 0 = roots: world = local
+      const int end = T.levelStart[lvl + 1];
+      for (int k = T.levelStart[lvl] + gl; k < end; k += gs) fkCompose(T, T.levelJoints[k], js);
+      groupSync();
+    }
+    if constexpr (!kBackward) {
+      float* so = a.out + size_t(b) * J * 8;
+      for (int i = gl; i < J * 8; i += gs) so[i] = js[(i >> 3) * kJointStateStride + (i & 7)];
+    } else {
+      // fkAxis writes only the axes and skelGradSeed reads only (t, q, s): one barrier for both
+      for (int i = gl; i < 3 * J; i += gs) fkAxis(T, i / 3, i % 3, js);
+      const float* G = a.gradState + size_t(b) * J * 8;
+      for (int i = gl; i < J; i += gs) skelGradSeed(js, i, G + 8 * i, acc);
+      groupSync();
+      for (int lvl = T.numLevels - 2; lvl >= 0; --lvl) { // the deepest level has no children
+        const int end = T.levelStart[lvl + 1];
+        for (int k = T.levelStart[lvl] + gl; k < end; k += gs) skelGradFold(S, js, T.levelJoints[k], acc);
+        groupSync();
+      }
+      for (int row = gl; row < J * kParametersPerJoint; row += gs) gjp[row] = skelGradJointParameter(T, js, acc, row);
+      groupSync();
+      float* go = a.out + size_t(b) * n;
+      for (int p = gl; p < n; p += gs) go[p] = skelGradModelParameter(S, gjp, p);
+    }
+    groupSync(); // the next instance overwrites th / js / gjp
+  }
+}
+
+cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream) {
+  if (a.batch <= 0) return cudaSuccess;
+  // As many instances per CTA as shared memory holds next to the tables, one warp each up to kSkelMaxWarps. When fewer than eight fit
+  // (large rigs), several warps share an instance. A batch smaller than one instance group per SM is spread over the SMs.
+  const size_t budget = size_t(g_maxSmemOptin);
+  const size_t tableBytes = skeletonStateTableBytes(a, backward) + 16;
+  const size_t per = skeletonStateSmemPerInstance(a.T, backward);
+  if (tableBytes + per > budget) return cudaErrorInvalidConfiguration;
+  const int fit = int((budget - tableBytes) / per);
+  int W = 1, groups = std::min(fit, kSkelMaxWarps);
+  if (fit < 8)
+    while (W < 8 && groups * W * 2 <= kSkelMaxWarps) W *= 2; // named barriers 1..groups
+  const int sms = std::max(g_numSms, 1);
+  if (a.batch < sms * groups) groups = std::max(1, (a.batch + sms - 1) / sms);
+  const size_t smem = per * groups + tableBytes;
+  const int threads = groups * W * 32;
+  auto launch = [&](auto kernel) -> cudaError_t {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e != cudaSuccess) return e;
+    int perSm = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kernel, threads, smem);
+    if (e != cudaSuccess) return e;
+    const long needed = (long(a.batch) + groups - 1) / groups;
+    const int grid = int(std::max(1L, std::min(long(sms) * std::max(perSm, 1), needed)));
+    kernel<<<grid, threads, smem, stream>>>(a);
+    return cudaGetLastError();
+  };
+  auto pick = [&](auto bwd) -> cudaError_t {
+    constexpr bool kB = decltype(bwd)::value;
+    switch (W) {
+      case 1: return launch(skeletonStateKernel<kB, 1>);
+      case 2: return launch(skeletonStateKernel<kB, 2>);
+      case 4: return launch(skeletonStateKernel<kB, 4>);
+      default: return launch(skeletonStateKernel<kB, 8>);
+    }
+  };
+  return backward ? pick(std::true_type{}) : pick(std::false_type{});
+}
+
 
 // ------------------------------------------------------------------------------------------------
 // K2 (SIMT validation path): H[i][j] = sum_k J[k][cols[i]] J[k][cols[j]] for i >= j; g = J^T r.

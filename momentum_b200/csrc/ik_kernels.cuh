@@ -141,6 +141,18 @@ cudaError_t launchTrustRegionQr(const TrQrArgs& a, cudaStream_t stream);
 size_t qrSmemFloats(int n, int maxChunkRows);
 int qrMaxChunkRows(int n, size_t smemBytes); // rows of Jacobian that fit beside R (0: the system is too large for this kernel)
 cudaError_t launchQrSolve(const QrArgs& a, int maxChunkRows, cudaStream_t stream);
+// skeletonStateKernel<kBackward>: pymomentum's model_parameters_to_skeleton_state for a batch on the character alone (no solver
+// function), and its backward
+struct SkeletonStateArgs {
+  FunctionTables T;          // character part only (parent .. levelJoints, numParams, ptNnz)
+  SkeletonTables S;          // backward only
+  int32_t numChildren;       // entries of S.children
+  int32_t batch;
+  const float* theta;        // [B][n]
+  const float* gradState;    // backward: [B][J][8] dLoss / d state
+  float* out;                // forward: [B][J][8] (t, q xyzw, s); backward: [B][n] dLoss / d theta, overwritten
+};
+cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream);
 cudaError_t launchSweep(const SweepArgs& a, bool jacobian, cudaStream_t stream);
 size_t sweepSmemPerInstance(const FunctionTables& T, int warpsPerInstance);
 cudaError_t launchJtJSimt(const JtJArgs& a, cudaStream_t stream);

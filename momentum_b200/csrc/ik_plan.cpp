@@ -41,6 +41,30 @@ void HostCharacter::buildLevels() {
   for (int j = 0; j < numJoints; ++j) levelJoints[cursor[depth[j]]++] = j;
 }
 
+void HostCharacter::buildBackwardTables() {
+  childStart.assign(numJoints + 1, 0);
+  for (int j = 0; j < numJoints; ++j)
+    if (parent[j] >= 0) childStart[parent[j] + 1]++;
+  for (int j = 0; j < numJoints; ++j) childStart[j + 1] += childStart[j];
+  children.resize(childStart[numJoints]);
+  std::vector<int32_t> cursor(childStart.begin(), childStart.end() - 1);
+  for (int j = 0; j < numJoints; ++j) // ascending j: each joint's children in increasing index order
+    if (parent[j] >= 0) children[cursor[parent[j]]++] = j;
+  const int rows = numJoints * kParametersPerJoint;
+  ptColStart.assign(numParams + 1, 0);
+  for (int c : ptInner) ptColStart[c + 1]++;
+  for (int p = 0; p < numParams; ++p) ptColStart[p + 1] += ptColStart[p];
+  ptColRows.resize(ptInner.size());
+  ptColVals.resize(ptInner.size());
+  cursor.assign(ptColStart.begin(), ptColStart.end() - 1);
+  for (int r = 0; r < rows; ++r) // ascending rows: each column's rows in increasing order
+    for (int k = ptOuter[r]; k < ptOuter[r + 1]; ++k) {
+      const int at = cursor[ptInner[k]]++;
+      ptColRows[at] = r;
+      ptColVals[at] = ptVals[k];
+    }
+}
+
 std::vector<uint8_t> HostCharacter::computeActiveJointParams(const std::vector<uint8_t>& enabled) const {
   std::vector<uint8_t> r(size_t(numJoints) * kParametersPerJoint, 0);
   for (int row = 0; row < numJoints * kParametersPerJoint; ++row)
@@ -97,6 +121,7 @@ std::string makeCharacter(int32_t numJoints, const int32_t* parents, const float
   const std::string err = out.validate();
   if (!err.empty()) return err;
   out.buildLevels();
+  out.buildBackwardTables();
   return "";
 }
 

@@ -33,8 +33,14 @@ struct HostCharacter {
   std::vector<HostLimit> limits;
   // derived
   std::vector<int32_t> levelStart, levelJoints;
+  // the reverse sweep of the skeleton-state backward: children of each joint (CSR, ascending), and the ParameterTransform by model
+  // parameter (CSC, rows ascending within a column)
+  std::vector<int32_t> childStart, children;
+  std::vector<int32_t> ptColStart, ptColRows;
+  std::vector<float> ptColVals;
   std::string validate() const; // empty when fine (MT_CHECK-style message otherwise)
   void buildLevels();
+  void buildBackwardTables();
   // ParameterTransformT::computeActiveJointParams (parameter_transform.cpp:97-107)
   std::vector<uint8_t> computeActiveJointParams(const std::vector<uint8_t>& enabled) const;
 };

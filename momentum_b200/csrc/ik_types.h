@@ -122,4 +122,13 @@ struct FunctionTables {
   size_t jacobianStride;     // floats per instance in the Jacobian buffer
 };
 
+// What the skeleton-state backward walks besides the character part of FunctionTables (HostCharacter::buildBackwardTables)
+struct SkeletonTables {
+  const int32_t* childStart; // [J+1]
+  const int32_t* children;   // [J - roots], ascending within a joint
+  const int32_t* ptColStart; // [n+1] ParameterTransform as CSC
+  const int32_t* ptColRows;  // [nnz] ascending within a column
+  const float* ptColVals;    // [nnz]
+};
+
 } // namespace mb2

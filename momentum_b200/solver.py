@@ -73,6 +73,7 @@ CABI_SYMBOLS = [
     "mb2_character_clone", "mb2_solver_function_clone", "mb2_character_device", "mb2_solver_function_character", "mb2_solver_function_num_error_functions",
     "mb2_solver_function_target_size", "mb2_sharded_last_error", "mb2_sharded_solver_create", "mb2_sharded_solver_destroy", "mb2_sharded_solver_num_shards",
     "mb2_sharded_solver_shard_info", "mb2_sharded_solver_set_options", "mb2_sharded_solver_set_targets", "mb2_sharded_solver_solve", "mb2_sharded_solver_get_aggregate",
+    "mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device",
 ]
 
 _libs = {}
@@ -166,6 +167,9 @@ def load_library(path: Optional[str] = None):
         L.mb2_sharded_solver_set_targets.argtypes = [vp, C.c_int32, _fp]
         L.mb2_sharded_solver_solve.argtypes = [vp, vp, _dp, _ip, _ip]
         L.mb2_sharded_solver_get_aggregate.argtypes = [vp, _dp]
+    if hasattr(L, "mb2_character_skeleton_state_device"):
+        L.mb2_character_skeleton_state_device.argtypes = [vp, C.c_int32, vp, vp, vp]
+        L.mb2_character_skeleton_state_backward_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
     _libs[path] = L
     return L
 
@@ -254,6 +258,17 @@ class DeviceCharacter(_Base):
                 for j in range(27):
                     arr[k].f[j] = float(ff[j])
             self._check(self._L.mb2_character_set_parameter_limits(self._h, len(character.limits), arr))
+
+    def skeleton_state_device(self, batch: int, params_device_ptr: int, state_device_ptr: int, stream: int = 0):
+        """Skeleton state [B][J][8] (t, q xyzw, s) of model parameters [B][n], float32 device memory on this character's device, enqueued
+        on ``stream`` (0: the legacy default stream)."""
+        self._check(self._L.mb2_character_skeleton_state_device(self._h, int(batch), C.c_void_p(params_device_ptr), C.c_void_p(state_device_ptr),
+                                                                C.c_void_p(stream)))
+
+    def skeleton_state_backward_device(self, batch: int, params_device_ptr: int, grad_state_device_ptr: int, grad_params_device_ptr: int, stream: int = 0):
+        """dLoss/d model parameters [B][n] (overwritten) from dLoss/d skeleton state [B][J][8], float32 device memory, on ``stream``."""
+        self._check(self._L.mb2_character_skeleton_state_backward_device(self._h, int(batch), C.c_void_p(params_device_ptr), C.c_void_p(grad_state_device_ptr),
+                                                                         C.c_void_p(grad_params_device_ptr), C.c_void_p(stream)))
 
     def __del__(self):
         if getattr(self, "_h", None):
