@@ -196,6 +196,10 @@ int mb2_add_position_error_function(mb2_solver_function* f, float weight, float 
  * sparsity pattern and stay shared). Per-instance record (mb2_set_targets): [B][nc*6] = target xyz, offset xyz per constraint. */
 int mb2_add_position_error_function_instanced(mb2_solver_function* f, float weight, float loss_alpha, float loss_c, int32_t num_constraints,
                                               const int32_t* parents, const float* weights /*[nc]*/, int32_t* out_index);
+/* Orientation (matrix difference, rot_diff = 0, or rot-diff) with the constraint OFFSETS per instance, like the Position one above.
+ * Per-instance record (mb2_set_targets[_device]): [B][nc*8] = target xyzw, offset xyzw per constraint; both are normalised on upload. */
+int mb2_add_orientation_error_function_instanced(mb2_solver_function* f, float weight, float loss_alpha, float loss_c, int32_t rot_diff,
+                                                 int32_t num_constraints, const int32_t* parents, const float* weights /*[nc]*/, int32_t* out_index);
 /* addErrorFunction(PlaneErrorFunctionT) — plane_error_function.h:20-101, .cpp:49-70: signed distance of T_parent * offset to the plane
  * (normal, d), one residual row per constraint; above != 0 is the half-plane mode (only val < 0 is penalised). Per-instance targets
  * (mb2_set_targets): [B][nc*4] = normal xyz (normalised as in PlaneDataT's ctor), d. kLegacyWeight = 1e-4 (.h:83). */
@@ -258,6 +262,20 @@ int mb2_character_skeleton_state_device(const mb2_character* c, int32_t batch, c
 int mb2_character_skeleton_state_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
                                                  const float* grad_skeleton_state_device, float* grad_model_parameters_device,
                                                  void* cuda_stream);
+
+/* Input contraction of the implicit-function backward of solve_ik (diff_ik d_gradient_d_input_dot): for block `index` and every
+ * instance b, the derivatives of grad_theta E_index(theta_b) . v_b with respect to the block's inputs, at the targets, constraint weights
+ * and offsets the handle currently holds:
+ *   grad_weights [B][nc]        w.r.t. the (per-instance) constraint weights
+ *   grad_offsets [B][nc][3|4]   w.r.t. the offsets (orientation: the normalised quaternions the handle stores)
+ *   grad_targets [B][nc][3|4]   w.r.t. the targets (idem)
+ * for a Position block (shared or instanced) or an Orientation block (matrix difference, shared or instanced) with the L2 loss.
+ * Entries of v for disabled parameters are ignored. Device memory in and out, asynchronous on `cuda_stream` (NULL = the legacy default
+ * stream); a null output is skipped. Any other block kind or loss, an index out of range, a null parameters / direction pointer
+ * (batch > 0) or memory that is not device memory on the function's device is MB2_ERR_INVALID_ARGUMENT. */
+int mb2_solver_function_input_gradients_device(mb2_solver_function* f, int32_t index, const float* parameters_device /*[B][n]*/,
+                                               const float* direction_device /*[B][n]*/, float* grad_weights_device, float* grad_offsets_device,
+                                               float* grad_targets_device, void* cuda_stream);
 
 /* ---- GaussNewtonSolverT<float> x B (solver/gauss_newton_solver.h:67-137, solver/solver.h:36-100) ---- */
 int mb2_solver_create(mb2_solver_function* f, const mb2_gauss_newton_options* opt, mb2_solver** out);

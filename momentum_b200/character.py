@@ -329,6 +329,7 @@ class OrientationErrorFunction:
     loss_alpha: float = LOSS_L2
     loss_c: float = 1.0
     rot_diff: bool = False
+    instance_offsets: Optional[np.ndarray] = None  # [B,nc,4]: offsets per batch element (the instanced block)
     kLegacyWeight = 1e-1  # orientation_error_function.h:63
 
     @property

@@ -672,6 +672,13 @@ int mb2_add_orientation_error_function(mb2_solver_function* f, float weight, flo
   return addBlock(f, orientationErrorFunction(f->ch->host, weight, alpha, c, rotDiff, nc, parents, offsets, weights, ef), ef, outIndex);
 }
 
+int mb2_add_orientation_error_function_instanced(mb2_solver_function* f, float weight, float alpha, float c, int32_t rotDiff, int32_t nc,
+                                                 const int32_t* parents, const float* weights, int32_t* outIndex) {
+  MB2_CHECK(f != nullptr, "null solver function");
+  HostErrorFunction ef;
+  return addBlock(f, instancedOrientationErrorFunction(f->ch->host, weight, alpha, c, rotDiff, nc, parents, weights, ef), ef, outIndex);
+}
+
 int mb2_add_state_error_function(mb2_solver_function* f, float weight, int32_t rotationErrorType, float posWgt, float rotWgt,
                                  const float* posW, const float* rotW, int32_t* outIndex) {
   MB2_CHECK(f != nullptr, "null solver function");
@@ -708,7 +715,8 @@ static int setTargetsImpl(mb2_solver_function* f, int32_t index, const float* ta
     packed = f->dTargetStage.p;
   }
   MB2_CUDA(launchScatterTargets(packed, dst, ef.targetSize, f->host.targetStride, f->B, st));
-  if (ef.kind == 1 || ef.kind == 2) MB2_CUDA(launchNormalizeQuats(dst, 0, f->host.targetStride, ef.numConstraints(), f->B, st));
+  if (ef.kind == 1 || ef.kind == 2) // targets (and the offsets of an instanced block, interleaved with them) are unit quaternions
+    MB2_CUDA(launchNormalizeQuats(dst, 0, f->host.targetStride, (ef.instanceOffsets ? 2 : 1) * ef.numConstraints(), f->B, st));
   return MB2_OK;
 }
 int mb2_set_targets(mb2_solver_function* f, int32_t index, const float* targets) {
@@ -931,6 +939,54 @@ int mb2_character_skeleton_state_device(const mb2_character* c, int32_t batch, c
 int mb2_character_skeleton_state_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
                                                  const float* grad_skeleton_state_device, float* grad_model_parameters_device, void* cuda_stream) {
   return skeletonStateDevice(c, batch, model_parameters_device, grad_skeleton_state_device, grad_model_parameters_device, cuda_stream, true);
+}
+
+int mb2_solver_function_input_gradients_device(mb2_solver_function* f, int32_t index, const float* parameters_device, const float* direction_device,
+                                               float* grad_weights_device, float* grad_offsets_device, float* grad_targets_device, void* cuda_stream) {
+  MB2_CHECK(f != nullptr, "null solver function");
+  MB2_CHECK(index >= 0 && index < int(f->host.efs.size()), "error function index out of range");
+  const HostErrorFunction& ef = f->host.efs[index];
+  MB2_CHECK(ef.kind == 0 || ef.kind == 1, "input gradients: only Position and Orientation (matrix difference) blocks are supported");
+  const float kEps = 1e-9f; // the L2 snapping of GeneralizedLossT (makeEfDesc)
+  MB2_CHECK(ef.lossAlpha >= 2.f - kEps && ef.lossAlpha <= 2.f + kEps, "input gradients: only the L2 loss is supported");
+  MB2_CHECK(parameters_device != nullptr && direction_device != nullptr, "null parameters or direction");
+  MB2_DEVICE_GUARD(f->ch->device);
+  float* outs[3] = {grad_weights_device, grad_offsets_device, grad_targets_device};
+  bool onDevice = isDeviceMemoryOn(parameters_device, f->ch->device) && isDeviceMemoryOn(direction_device, f->ch->device);
+  for (float* o : outs) onDevice = onDevice && (o == nullptr || isDeviceMemoryOn(o, f->ch->device));
+  MB2_CHECK(onDevice, "input gradients: every array must be device memory on the function's device");
+  int rc = ensurePlan(f, f->planMode, f->planSchedDense, f->planAlignRows);
+  if (rc != MB2_OK) return rc;
+  NvtxRange range("inputGradients");
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  const int nc = ef.numConstraints(), per = ef.kind == 0 ? 3 : 4;
+  int unitBegin = -1;
+  for (size_t u = 0; u < f->plan.units.size() && unitBegin < 0; ++u)
+    if (f->plan.units[u].ef == index) unitBegin = int(u);
+  if (nc == 0) return MB2_OK;
+  if (unitBegin < 0) { // a block with weight 0 has no rows: its gradient contribution is zero
+    const size_t sizes[3] = {size_t(nc), size_t(nc) * per, size_t(nc) * per};
+    for (int k = 0; k < 3; ++k)
+      if (outs[k]) MB2_CUDA(cudaMemsetAsync(outs[k], 0, size_t(f->B) * sizes[k] * sizeof(float), st));
+    return MB2_OK;
+  }
+  InputGradientArgs a{};
+  a.T = f->tables();
+  a.unitBegin = unitBegin;
+  a.numConstraints = nc;
+  a.kind = ef.kind == 0 ? kUnitPosition : kUnitOrientation;
+  a.batch = f->B;
+  a.theta = parameters_device;
+  a.direction = direction_device;
+  a.enabledList = f->dEnabledList.p;
+  a.numEnabled = int(f->plan.enabledList.size());
+  a.targets = f->dTargets.p;
+  a.cweights = f->dWeights.p;
+  a.gradWeights = grad_weights_device;
+  a.gradOffsets = grad_offsets_device;
+  a.gradTargets = grad_targets_device;
+  MB2_CUDA(launchInputGradients(a, st));
+  return MB2_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -284,6 +284,112 @@ MB2_HD float skelGradModelParameter(const SkeletonTables& S, const float* gjp, i
   return s;
 }
 
+// ---- Input contractions of the implicit-function backward of solve_ik: d/d input [grad_theta E_c . v] ----
+// Under the parameter direction v every joint moves rigidly: angular velocity w, log-scale rate sigma, origin velocity tdot. With the
+// joint-parameter velocity u = P v (linear part of the ParameterTransform; its offsets do not move) and pi = parent(j):
+//   w_j = w_pi + sum_k u[7j+3+k] A_jk,   sigma_j = sigma_pi + ln2 u[7j+6],
+//   tdot_j = tdot_pi + w_pi x (t_j - t_pi) + sigma_pi (t_j - t_pi) + sum_k u[7j+k] B_jk
+// (A = rotationAxisCol, B = translationAxisCol; zero motion above a root). A point p attached to j moves at
+// pdot = tdot_j + w_j x (p - t_j) + sigma_j (p - t_j) = J_c v. t_j - t_pi stays relative (no cancellation for a rig far from the origin).
+constexpr int kTangentStride = 7; // w(3) sigma tdot(3); odd: conflict-free with lanes = joints
+
+// u[row] = (P v)[row] without ptOffsets (jointParameterRow adds them)
+MB2_HD float tangentJointParameter(const FunctionTables& T, int row, const float* v) {
+  float s = 0.f;
+  for (int k = T.ptOuter[row]; k < T.ptOuter[row + 1]; ++k) s += T.ptVals[k] * v[T.ptInner[k]];
+  return s;
+}
+// the joint's own share of its motion (all joints at once; js holds the world state and DOF axes, fkAxis)
+MB2_HD void tangentLocal(const FunctionTables& T, const float* js, int j, const float* v, float* tan) {
+  const int r0 = j * kParametersPerJoint;
+  F3 w = f3(0.f, 0.f, 0.f), td = f3(0.f, 0.f, 0.f);
+  for (int k = 0; k < 3; ++k) {
+    td = td + translationAxisCol(T, js, j, k) * tangentJointParameter(T, r0 + k, v);
+    w = w + rotationAxisCol(js, j, k) * tangentJointParameter(T, r0 + 3 + k, v);
+  }
+  float* o = tan + j * kTangentStride;
+  o[0] = w.x; o[1] = w.y; o[2] = w.z;
+  o[3] = kLn2 * tangentJointParameter(T, r0 + 6, v);
+  o[4] = td.x; o[5] = td.y; o[6] = td.z;
+}
+// level by level from the roots: adds the (finished) parent's motion to the joint's own share
+MB2_HD void tangentCompose(const FunctionTables& T, const float* js, int j, float* tan) {
+  const int par = T.parent[j];
+  if (par < 0) return;
+  const float* P = tan + par * kTangentStride;
+  float* o = tan + j * kTangentStride;
+  const F3 wp = ld3(P), off = ld3(js + j * kJointStateStride) - ld3(js + par * kJointStateStride);
+  const float sp = P[3];
+  const F3 w = wp + ld3(o);
+  const F3 td = ld3(P + 4) + cross(wp, off) + sp * off + ld3(o + 4);
+  o[0] = w.x; o[1] = w.y; o[2] = w.z;
+  o[3] = sp + o[3];
+  o[4] = td.x; o[5] = td.y; o[6] = td.z;
+}
+
+// Position constraint (L2), p = t_j + s_j R_j o, d = p - t, W = e.weight w_c / c^2, g = 2 W d . pdot:
+//   dg/dw_c = 2 e.weight / c^2 d . pdot,   dg/dt = -2 W pdot,   dg/do = 2 W s_j R_j^T (pdot - w_j x d + sigma_j d)
+// tg: the constraint's target record (xyz, then the offset for an instanced block). Null outputs are skipped.
+MB2_HD void positionInputGradient(const UnitDesc& u, const EfDesc& e, const float* js, const float* tan, const float* tg, float cw, float* gW,
+                                  float* gO, float* gT) {
+  const float* ps = js + u.joint * kJointStateStride;
+  const float* tj = tan + u.joint * kTangentStride;
+  const Q4 q = ld4(ps + 3);
+  const float s = ps[7];
+  const F3 off = u.pad[2] != 0 ? f3(tg[3], tg[4], tg[5]) : f3(u.f[0], u.f[1], u.f[2]);
+  const F3 rel = qrot(q, s * off); // p - t_j
+  const F3 d = ld3(ps) + rel - ld3(tg);
+  const F3 w = ld3(tj);
+  const float sg = tj[3];
+  const F3 pdot = ld3(tj + 4) + cross(w, rel) + sg * rel;
+  const float ew = e.weight * e.invC2, W = ew * cw;
+  if (gW) gW[0] = 2.f * ew * dot(d, pdot);
+  if (gT) { const F3 g = pdot * (-2.f * W); gT[0] = g.x; gT[1] = g.y; gT[2] = g.z; }
+  if (gO) {
+    const F3 g = qrot(qconj(q), pdot - cross(w, d) + sg * d) * (2.f * W * s);
+    gO[0] = g.x; gO[1] = g.y; gO[2] = g.z;
+  }
+}
+
+// <dR(q)/dq_k, X> for k = x, y, z, w (qmat's quadratic form, X column-major m[3*col + row])
+MB2_HD void qmatDerivativeDot(Q4 q, const float* X, float* out) {
+  const float x01 = X[3] + X[1], x02 = X[6] + X[2], x12 = X[7] + X[5];
+  const float a01 = X[1] - X[3], a02 = X[6] - X[2], a21 = X[5] - X[7]; // X10 - X01, X02 - X20, X21 - X12
+  out[0] = 2.f * (q.y * x01 + q.z * x02 + q.w * a21) - 4.f * q.x * (X[4] + X[8]);
+  out[1] = 2.f * (q.x * x01 + q.w * a02 + q.z * x12) - 4.f * q.y * (X[0] + X[8]);
+  out[2] = 2.f * (q.w * a01 + q.x * x02 + q.y * x12) - 4.f * q.z * (X[0] + X[4]);
+  out[3] = 2.f * (q.z * a01 + q.y * a02 + q.x * a21);
+}
+
+// Orientation constraint (matrix difference, L2), R_c = R_j R(q_o), F = R_c - R(q_t), dR_c = [w_j]x R_c, g = 2 W <F, [w_j]x R_c>:
+//   dg/dw_c = 2 e.weight / c^2 <F, [w_j]x R_c>,   dg/dq_t,k = -2 W <dR/dq_k(q_t), [w_j]x R_c>,
+//   dg/dq_o,k = 2 W <R_j dR/dq_k(q_o), [w_j]x R(q_t)>   (R_c - F = R(q_t))
+// at the normalised quaternions the record holds (target xyzw, then the offset for an instanced block).
+MB2_HD void orientationInputGradient(const UnitDesc& u, const EfDesc& e, const float* js, const float* tan, const float* tg, float cw, float* gW,
+                                     float* gO, float* gT) {
+  const Q4 q = ld4(js + u.joint * kJointStateStride + 3);
+  const F3 w = ld3(tan + u.joint * kTangentStride);
+  const Q4 qo = u.pad[2] != 0 ? ld4(tg + 4) : q4(u.f[0], u.f[1], u.f[2], u.f[3]);
+  const Q4 qt = ld4(tg);
+  float ro[9], rt[9], xt[9], xo[9];
+  qmat(qo, ro);
+  qmat(qt, rt);
+  float fx = 0.f;
+  for (int k = 0; k < 3; ++k) {
+    const F3 rc = qrot(q, f3(ro[3 * k], ro[3 * k + 1], ro[3 * k + 2])); // column k of R_c, as evalUnit forms it
+    const F3 rtk = f3(rt[3 * k], rt[3 * k + 1], rt[3 * k + 2]);
+    const F3 a = cross(w, rc), b = qrot(qconj(q), cross(w, rtk)); // [w]x R_c and R_j^T [w]x R_t, column k
+    fx += dot(rc - rtk, a);
+    xt[3 * k] = a.x; xt[3 * k + 1] = a.y; xt[3 * k + 2] = a.z;
+    xo[3 * k] = b.x; xo[3 * k + 1] = b.y; xo[3 * k + 2] = b.z;
+  }
+  const float ew = e.weight * e.invC2, W = ew * cw;
+  if (gW) gW[0] = 2.f * ew * fx;
+  float d[4];
+  if (gT) { qmatDerivativeDot(qt, xt, d); for (int k = 0; k < 4; ++k) gT[k] = -2.f * W * d[k]; }
+  if (gO) { qmatDerivativeDot(qo, xo, d); for (int k = 0; k < 4; ++k) gO[k] = 2.f * W * d[k]; }
+}
+
 // ---- quaternion log map (math/utility.cpp:72-180) ----
 MB2_HD F3 quaternionLogMap(Q4 q) {
   const Q4 qn = qnormalized(q);
@@ -417,7 +523,10 @@ MB2_HD float evalUnit(const FunctionTables& T, int ui, const float* theta, const
       }
       const Q4 q = ld4(js + u.joint * kJointStateStride + 3);
       float ro[9], rt[9], f[9], v[9];
-      qmat(q4(u.f[0], u.f[1], u.f[2], u.f[3]), ro);
+      // the offset is shared by the batch (u.f) or, for an instanced block, follows the target quaternion in the instance's record
+      Q4 qo = q4(u.f[0], u.f[1], u.f[2], u.f[3]);
+      if (u.pad[2] != 0) qo = ld4(targets + u.targetOff + 4);
+      qmat(qo, ro);
       qmat(ld4(targets + u.targetOff), rt);
       for (int k = 0; k < 3; ++k) {
         const F3 vk = qrot(q, f3(ro[3 * k], ro[3 * k + 1], ro[3 * k + 2]));

@@ -380,6 +380,129 @@ cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaS
   return backward ? pick(std::true_type{}) : pick(std::false_type{});
 }
 
+// ------------------------------------------------------------------------------------------------
+// Input gradients of one Position / Orientation block, d/d input [grad_theta E . v] (ik_device.cuh tangent* / *InputGradient): laid out
+// like skeletonStateKernel, a persistent grid with one group of W warps per instance and the character tables in shared memory.
+//   lanes = parameters: theta, and v gated by the enabled set;  lanes = joints: FK with the DOF axes;  lanes = joints: each joint's own
+//   motion;  level by level: the parent's motion added;  lanes = constraints of the block.
+// Every output element is written by one lane: no atomics, the result does not depend on the launch shape.
+// ------------------------------------------------------------------------------------------------
+// per instance: theta [n], v [n], joint states [J][17], joint motions [J][7]
+MB2_HD size_t inputGradientSmemPerInstanceFloats(int J, int n) {
+  return 2 * skelAligned(size_t(n)) + skelAligned(size_t(J) * kJointStateStride) + skelAligned(size_t(J) * kTangentStride);
+}
+
+size_t inputGradientTableBytes(const FunctionTables& T) {
+  const size_t J = T.numJoints;
+  size_t w = tableWords(J, 4) + tableWords(3 * J, 4) + tableWords(4 * J, 4);
+  w += tableWords(7 * J + 1, 4) + tableWords(T.ptNnz, 4) * 2 + tableWords(7 * J, 4);
+  w += tableWords(T.numLevels + 1, 4) + tableWords(J, 4);
+  return w * 4;
+}
+
+template <int W>
+__global__ void __launch_bounds__(32 * kSkelMaxWarps) inputGradientKernel(const InputGradientArgs a) {
+  extern __shared__ __align__(16) float smem[];
+  FunctionTables T = a.T;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int group = warp / W, gl = (warp % W) * 32 + lane;
+  constexpr int gs = 32 * W;
+  const int groupsPerCta = (blockDim.x >> 5) / W;
+  const int J = T.numJoints, n = T.numParams, nc = a.numConstraints;
+  const int thF = int(skelAligned(n)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
+  const int perGroup = int(inputGradientSmemPerInstanceFloats(J, n));
+  float* th = smem + size_t(group) * perGroup;
+  float* vs = th + thF;
+  float* js = vs + thF;
+  float* tan = js + jsF;
+  auto groupSync = [&]() {
+    if (W == 1) __syncwarp();
+    else asm volatile("bar.sync %0, %1;" ::"r"(1 + group), "r"(gs) : "memory");
+  };
+  {
+    uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
+    const size_t Jz = J;
+    stageTable(T.parent, Jz, cursor); stageTable(T.offset, 3 * Jz, cursor); stageTable(T.prerot, 4 * Jz, cursor);
+    stageTable(T.ptOuter, 7 * Jz + 1, cursor); stageTable(T.ptInner, T.ptNnz, cursor); stageTable(T.ptVals, T.ptNnz, cursor);
+    stageTable(T.ptOffsets, 7 * Jz, cursor);
+    stageTable(T.levelStart, T.numLevels + 1, cursor); stageTable(T.levelJoints, Jz, cursor);
+    __syncthreads();
+  }
+  const EfDesc e = T.efs[T.units[a.unitBegin].ef];
+  const bool position = a.kind == kUnitPosition;
+  const int per = position ? 3 : 4;
+  for (int b = blockIdx.x * groupsPerCta + group; b < a.batch; b += gridDim.x * groupsPerCta) {
+    const float* theta = a.theta + size_t(b) * n;
+    const float* dir = a.direction + size_t(b) * n;
+    for (int i = gl; i < n; i += gs) { th[i] = theta[i]; vs[i] = 0.f; }
+    groupSync();
+    for (int k = gl; k < a.numEnabled; k += gs) { const int p = a.enabledList[k]; vs[p] = dir[p]; }
+    for (int j = gl; j < J; j += gs) fkLocalFromTheta<true>(T, j, th, js);
+    groupSync();
+    for (int lvl = 1; lvl < T.numLevels; ++lvl) {
+      const int end = T.levelStart[lvl + 1];
+      for (int k = T.levelStart[lvl] + gl; k < end; k += gs) fkCompose(T, T.levelJoints[k], js);
+      groupSync();
+    }
+    for (int i = gl; i < 3 * J; i += gs) fkAxis(T, i / 3, i % 3, js);
+    groupSync();
+    for (int j = gl; j < J; j += gs) tangentLocal(T, js, j, vs, tan);
+    groupSync();
+    for (int lvl = 1; lvl < T.numLevels; ++lvl) {
+      const int end = T.levelStart[lvl + 1];
+      for (int k = T.levelStart[lvl] + gl; k < end; k += gs) tangentCompose(T, js, T.levelJoints[k], tan);
+      groupSync();
+    }
+    const float* targets = a.targets + size_t(b) * T.targetStride;
+    const float* cweights = a.cweights + (T.weightsPerInstance ? size_t(b) * T.numWeights : 0);
+    for (int c = gl; c < nc; c += gs) {
+      const UnitDesc& u = T.units[a.unitBegin + c];
+      const size_t o = size_t(b) * nc + c;
+      float* gW = a.gradWeights ? a.gradWeights + o : nullptr;
+      float* gO = a.gradOffsets ? a.gradOffsets + o * per : nullptr;
+      float* gT = a.gradTargets ? a.gradTargets + o * per : nullptr;
+      if (position) positionInputGradient(u, e, js, tan, targets + u.targetOff, cweights[u.weightIdx], gW, gO, gT);
+      else orientationInputGradient(u, e, js, tan, targets + u.targetOff, cweights[u.weightIdx], gW, gO, gT);
+    }
+    groupSync(); // the next instance overwrites th / vs / js / tan
+  }
+}
+
+cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream) {
+  if (a.batch <= 0) return cudaSuccess;
+  // the sizing rule of launchSkeletonState: as many instances per CTA as shared memory holds beside the tables, several warps per
+  // instance for large rigs, a small batch spread over the SMs
+  const size_t budget = size_t(g_maxSmemOptin);
+  const size_t tableBytes = inputGradientTableBytes(a.T) + 16;
+  const size_t per = sizeof(float) * inputGradientSmemPerInstanceFloats(a.T.numJoints, a.T.numParams);
+  if (tableBytes + per > budget) return cudaErrorInvalidConfiguration;
+  const int fit = int((budget - tableBytes) / per);
+  int W = 1, groups = std::min(fit, kSkelMaxWarps);
+  if (fit < 8)
+    while (W < 8 && groups * W * 2 <= kSkelMaxWarps) W *= 2;
+  const int sms = std::max(g_numSms, 1);
+  if (a.batch < sms * groups) groups = std::max(1, (a.batch + sms - 1) / sms);
+  const size_t smem = per * groups + tableBytes;
+  const int threads = groups * W * 32;
+  auto launch = [&](auto kernel) -> cudaError_t {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e != cudaSuccess) return e;
+    int perSm = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kernel, threads, smem);
+    if (e != cudaSuccess) return e;
+    const long needed = (long(a.batch) + groups - 1) / groups;
+    const int grid = int(std::max(1L, std::min(long(sms) * std::max(perSm, 1), needed)));
+    kernel<<<grid, threads, smem, stream>>>(a);
+    return cudaGetLastError();
+  };
+  switch (W) {
+    case 1: return launch(inputGradientKernel<1>);
+    case 2: return launch(inputGradientKernel<2>);
+    case 4: return launch(inputGradientKernel<4>);
+    default: return launch(inputGradientKernel<8>);
+  }
+}
+
 
 // ------------------------------------------------------------------------------------------------
 // K2 (SIMT validation path): H[i][j] = sum_k J[k][cols[i]] J[k][cols[j]] for i >= j; g = J^T r.

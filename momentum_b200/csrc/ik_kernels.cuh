@@ -153,6 +153,25 @@ struct SkeletonStateArgs {
   float* out;                // forward: [B][J][8] (t, q xyzw, s); backward: [B][n] dLoss / d theta, overwritten
 };
 cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream);
+// inputGradientKernel: d/d input [grad_theta E . v] of one Position or Orientation (matrix difference) block with the L2 loss, per
+// instance: the input contraction of solve_ik's implicit-function backward
+struct InputGradientArgs {
+  FunctionTables T;          // character part, units / efs, targetStride, weightsPerInstance, numWeights
+  int32_t unitBegin;         // first unit of the block (its constraints are units unitBegin .. + numConstraints - 1)
+  int32_t numConstraints;
+  int32_t kind;              // kUnitPosition or kUnitOrientation
+  int32_t batch;
+  const float* theta;        // [B][n]
+  const float* direction;    // [B][n] v; entries of disabled parameters are ignored
+  const int32_t* enabledList; // [numEnabled]
+  int32_t numEnabled;
+  const float* targets;      // the handle's per-instance records [B][targetStride]
+  const float* cweights;     // constraint weights [numWeights] or [B][numWeights]
+  float* gradWeights;        // [B][nc] or null
+  float* gradOffsets;        // [B][nc][3|4] or null
+  float* gradTargets;        // [B][nc][3|4] or null
+};
+cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream);
 cudaError_t launchSweep(const SweepArgs& a, bool jacobian, cudaStream_t stream);
 size_t sweepSmemPerInstance(const FunctionTables& T, int warpsPerInstance);
 cudaError_t launchJtJSimt(const JtJArgs& a, cudaStream_t stream);

@@ -203,6 +203,15 @@ std::string orientationErrorFunction(const HostCharacter& ch, float weight, floa
   return jointConstraints(ch, rotDiff ? 2 : 1, weight, alpha, c, nc, parents, weights, ef);
 }
 
+std::string instancedOrientationErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t rotDiff, int32_t nc, const int32_t* parents,
+                                              const float* weights, HostErrorFunction& ef) {
+  if (!(nc >= 0 && (nc == 0 || (parents && weights)))) return "invalid orientation constraints";
+  ef.instanceOffsets = true;
+  ef.offsets.assign(4 * size_t(nc), 0.f);
+  ef.targetSize = 8 * nc;
+  return jointConstraints(ch, rotDiff ? 2 : 1, weight, alpha, c, nc, parents, weights, ef);
+}
+
 std::string stateErrorFunction(const HostCharacter& ch, float weight, int32_t rotationErrorType, float posWgt, float rotWgt, const float* posW, const float* rotW,
                                HostErrorFunction& ef) {
   if (!(posW && rotW)) return "invalid state error function";
@@ -369,8 +378,8 @@ std::string buildPlan(const HostCharacter& ch, const std::vector<HostErrorFuncti
         if (alignRowGroups) row = (row + 3) & ~3;
         u.row0 = row;
         u.numRows = isPos ? 3 : 9;
-        const bool instanced = isPos && ef.instanceOffsets;
-        u.targetOff = ef.targetOff + (instanced ? 6 : per) * c;
+        const bool instanced = ef.instanceOffsets; // record per constraint: target, then its offset
+        u.targetOff = ef.targetOff + (instanced ? 2 * per : per) * c;
         u.weightIdx = ef.weightOff + c;
         u.recOff = rec;
         u.extra = -1;

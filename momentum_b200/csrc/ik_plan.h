@@ -56,7 +56,7 @@ struct HostErrorFunction {
   float posWgt{1.f}, rotWgt{1.f};
   std::vector<float> posW, rotW;
   bool halfPlane{false};            // plane: PlaneErrorFunctionT(above)
-  bool instanceOffsets{false};      // position: offsets are per instance (record = target xyz, offset xyz per constraint)
+  bool instanceOffsets{false};      // position / orientation: offsets are per instance (record per constraint = target, then offset)
   std::vector<float> paramWeights; // model parameters: targetWeights_ [numParams]
   // layout (assigned when added)
   int32_t targetOff{0}, targetSize{0}; // floats per instance
@@ -95,6 +95,9 @@ std::string planeErrorFunction(const HostCharacter& ch, float weight, float alph
 std::string modelParametersErrorFunction(const HostCharacter& ch, float weight, const float* targetWeights, HostErrorFunction& out);
 std::string orientationErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t rotDiff, int32_t nc, const int32_t* parents,
                                      const float* offsets, const float* weights, HostErrorFunction& out);
+// record per constraint = target xyzw, offset xyzw (both normalised when uploaded)
+std::string instancedOrientationErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t rotDiff, int32_t nc, const int32_t* parents,
+                                              const float* weights, HostErrorFunction& out);
 std::string stateErrorFunction(const HostCharacter& ch, float weight, int32_t rotationErrorType, float posWgt, float rotWgt, const float* posW, const float* rotW,
                                HostErrorFunction& out);
 std::string limitErrorFunction(float weight, float alpha, float c, HostErrorFunction& out);

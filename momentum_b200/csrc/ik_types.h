@@ -64,7 +64,7 @@ struct UnitDesc {
   int32_t i[4];      // limit indices (model parameter / joint-parameter rows), ellipsoidParent in i[0]
   float f[8];        // offset (3 or 4) | posW, rotW | limit floats f0..f3
   int32_t extra;     // float offset into limitData (ellipsoid matrices), -1 none
-  int32_t pad[3];     // [0] limit gated off by the enabled set (zero rows); [1] error-only unit (ModelParameters with a negative target weight); [2] Position: per-instance offset stored after the target
+  int32_t pad[3];     // [0] limit gated off by the enabled set (zero rows); [1] error-only unit (ModelParameters with a negative target weight); [2] Position / Orientation: per-instance offset stored after the target
 };
 
 // One Jacobian cell: rows [unit.row0, +numRows) x column `col`

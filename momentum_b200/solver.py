@@ -74,6 +74,7 @@ CABI_SYMBOLS = [
     "mb2_solver_function_target_size", "mb2_sharded_last_error", "mb2_sharded_solver_create", "mb2_sharded_solver_destroy", "mb2_sharded_solver_num_shards",
     "mb2_sharded_solver_shard_info", "mb2_sharded_solver_set_options", "mb2_sharded_solver_set_targets", "mb2_sharded_solver_solve", "mb2_sharded_solver_get_aggregate",
     "mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device",
+    "mb2_add_orientation_error_function_instanced", "mb2_solver_function_input_gradients_device",
 ]
 
 _libs = {}
@@ -170,6 +171,9 @@ def load_library(path: Optional[str] = None):
     if hasattr(L, "mb2_character_skeleton_state_device"):
         L.mb2_character_skeleton_state_device.argtypes = [vp, C.c_int32, vp, vp, vp]
         L.mb2_character_skeleton_state_backward_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
+    if hasattr(L, "mb2_solver_function_input_gradients_device"):
+        L.mb2_add_orientation_error_function_instanced.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_int32, C.c_int32, _ip, _fp, _ip]
+        L.mb2_solver_function_input_gradients_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
     _libs[path] = L
     return L
 
@@ -305,6 +309,10 @@ class SkeletonSolverFunction(_Base):
         elif ef.kind == mc.KIND_POSITION:
             pa, pp = _i32(ef.parents); of, op = _f32(ef.offsets); w, wp = _f32(ef.weights)
             self._check(self._L.mb2_add_position_error_function(self._h, ef.weight, alpha, ef.loss_c, len(pa), pp, op, wp, C.byref(idx)))
+        elif ef.kind in (mc.KIND_ORIENTATION, mc.KIND_ORIENTATION_ROTDIFF) and getattr(ef, "instance_offsets", None) is not None:
+            pa, pp = _i32(ef.parents); w, wp = _f32(ef.weights)
+            self._check(self._L.mb2_add_orientation_error_function_instanced(self._h, ef.weight, alpha, ef.loss_c, int(ef.rot_diff), len(pa), pp, wp,
+                                                                             C.byref(idx)))
         elif ef.kind in (mc.KIND_ORIENTATION, mc.KIND_ORIENTATION_ROTDIFF):
             pa, pp = _i32(ef.parents); of, op = _f32(ef.offsets); w, wp = _f32(ef.weights)
             self._check(self._L.mb2_add_orientation_error_function(self._h, ef.weight, alpha, ef.loss_c, int(ef.rot_diff), len(pa), pp, op, wp,
@@ -331,7 +339,7 @@ class SkeletonSolverFunction(_Base):
         """(Re)send every block's per-instance targets from the spec objects."""
         for idx, ef in enumerate(self.error_functions):
             if getattr(ef, "targets", None) is not None and ef.kind != mc.KIND_LIMIT:
-                if ef.kind == mc.KIND_POSITION and getattr(ef, "instance_offsets", None) is not None:  # record = target xyz, offset xyz
+                if getattr(ef, "instance_offsets", None) is not None:  # record = target, then offset (xyz or xyzw)
                     self.set_targets(idx, np.concatenate([np.asarray(ef.targets, np.float32), np.asarray(ef.instance_offsets, np.float32)], -1))
                 else:
                     self.set_targets(idx, ef.targets)
@@ -356,6 +364,15 @@ class SkeletonSolverFunction(_Base):
         ptr = C.c_void_p(); ld = C.c_int32(0)
         self._check(self._L.mb2_solver_function_get_jacobian_device(self._h, C.c_void_p(params_device_ptr), C.byref(ptr), C.byref(ld), C.c_void_p(stream)))
         return ptr.value, ld.value
+
+    def input_gradients_device(self, index: int, params_device_ptr: int, direction_device_ptr: int, grad_weights_ptr: int = 0,
+                               grad_offsets_ptr: int = 0, grad_targets_ptr: int = 0, stream: int = 0):
+        """d/d input [grad_theta E_index . v] per instance for a Position or Orientation (matrix difference, L2) block: constraint weights
+        [B][nc], offsets and targets [B][nc][3|4] (0 = skip that output), from parameters and directions [B][n]; float32 device memory,
+        enqueued on ``stream``."""
+        self._check(self._L.mb2_solver_function_input_gradients_device(self._h, int(index), C.c_void_p(params_device_ptr), C.c_void_p(direction_device_ptr),
+                                                                       C.c_void_p(grad_weights_ptr or None), C.c_void_p(grad_offsets_ptr or None),
+                                                                       C.c_void_p(grad_targets_ptr or None), C.c_void_p(stream)))
 
     def set_error_function_weight(self, index: int, weight: float):
         self._check(self._L.mb2_set_error_function_weight(self._h, index, weight))

@@ -12,7 +12,11 @@ Jacobian restricted to the active parameters (singular values with s^2 < 1e-5 dr
     dLoss/d weight_k       = -(grad_theta E_k / weight_k) . v
     dLoss/d input          = d/d input [ grad_theta E_k . (-v) ]
 and no gradient for an element whose gradient RMS exceeds 0.01 (the solve did not converge, tensor_ik.cpp:254). The Jacobian comes
-from the device (``mb2_solver_function_get_jacobian_device``); the small dense algebra is torch on the same device.
+from the device (``mb2_solver_function_get_jacobian_device``); the small dense algebra is torch on the same device. The input
+contractions of the Position offsets and of every Orientation input need the motion of each constraint's parent frame under v, one
+sweep over the joint tree per element: a CUDA kernel computes them (``mb2_solver_function_input_gradients_device``). Position targets
+and weights come from the Jacobian rows, Motion targets and weights are elementwise. Before it reads the handle, the backward sends it
+this forward's targets, weights and offsets again, so another solve on the same cached handle in between does not change the result.
 torch is plumbing here (tensors, streams, autograd bookkeeping): every kernel on the forward path is this repo's.
 """
 from __future__ import annotations
@@ -69,10 +73,15 @@ def _f32c(t, device):
 
 
 def _build(character: mc.Character, B, device_index, pos_parents, pos_offsets, ori_parents, ori_offsets, motion_weights, use_limit, active):
-    """One cached solver function per (character, batch, constraint topology): the plan is built once."""
-    key = (id(character), B, device_index, None if pos_parents is None else pos_parents.tobytes(), None if pos_offsets is None else pos_offsets.tobytes(),
-           None if ori_parents is None else ori_parents.tobytes(), None if ori_offsets is None else ori_offsets.tobytes(),
-           None if motion_weights is None else motion_weights.tobytes(), use_limit, active.tobytes())
+    """One cached solver function per (character, batch, constraint topology): the plan is built once. ``pos_offsets`` /
+    ``ori_offsets`` None with parents given select the instanced block (offsets per element, in the target records): the key then
+    holds the parents only, so new offset values reuse the handle."""
+    def key_of(a):
+        return None if a is None else a.tobytes()
+
+    key = (id(character), B, device_index, key_of(pos_parents), "instanced" if pos_parents is not None and pos_offsets is None else key_of(pos_offsets),
+           key_of(ori_parents), "instanced" if ori_parents is not None and ori_offsets is None else key_of(ori_offsets),
+           key_of(motion_weights), use_limit, active.tobytes())
     if key in _handles:
         return _handles[key]
     fn = ms.SkeletonSolverFunction(character, B, device=device_index)
@@ -80,10 +89,17 @@ def _build(character: mc.Character, B, device_index, pos_parents, pos_offsets, o
     n = character.num_params
     if pos_parents is not None:
         nc = len(pos_parents)
-        blocks["position"] = fn.add_error_function(mc.PositionErrorFunction(pos_parents, pos_offsets, np.ones(nc, np.float32), np.zeros((B, nc, 3), np.float32), weight=1.0))
+        inst = None if pos_offsets is not None else np.zeros((B, nc, 3), np.float32)
+        offs = pos_offsets if pos_offsets is not None else np.zeros((nc, 3), np.float32)
+        blocks["position"] = fn.add_error_function(mc.PositionErrorFunction(pos_parents, offs, np.ones(nc, np.float32), np.zeros((B, nc, 3), np.float32), weight=1.0,
+                                                                            instance_offsets=inst))
     if ori_parents is not None:
         nc = len(ori_parents)
-        blocks["orientation"] = fn.add_error_function(mc.OrientationErrorFunction(ori_parents, ori_offsets, np.ones(nc, np.float32), np.zeros((B, nc, 4), np.float32), weight=1.0))
+        identity = np.tile(np.array([0, 0, 0, 1], np.float32), (nc, 1))
+        inst = None if ori_offsets is not None else np.broadcast_to(identity, (B, nc, 4)).copy()
+        offs = ori_offsets if ori_offsets is not None else identity
+        blocks["orientation"] = fn.add_error_function(mc.OrientationErrorFunction(ori_parents, offs, np.ones(nc, np.float32), np.zeros((B, nc, 4), np.float32), weight=1.0,
+                                                                                  instance_offsets=inst))
     if use_limit:
         blocks["limit"] = fn.add_error_function(mc.LimitErrorFunction(weight=1.0))
     if motion_weights is not None:
@@ -93,59 +109,91 @@ def _build(character: mc.Character, B, device_index, pos_parents, pos_offsets, o
     return _handles[key]
 
 
+def _normalization_backward(g, q):
+    """Gradient w.r.t. a raw quaternion q from the gradient g w.r.t. its normalisation q / |q|: (I - q^ q^T) g / |q|."""
+    nrm = torch.linalg.vector_norm(q, dim=-1, keepdim=True)
+    qh = q / nrm
+    return (g - qh * (qh * g).sum(dim=-1, keepdim=True)) / nrm
+
+
+def _reduce_to(g, like):
+    """A per-element gradient [B, ...] for an input shared by the batch ([...]): the sum over the batch."""
+    return g.sum(dim=0) if like.dim() == g.dim() - 1 else g
+
+
 class _SolveIK(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, cfg, theta0, efw, pos_targets, pos_weights, ori_targets, ori_weights, motion_targets):
+    def forward(ctx, cfg, theta0, efw, pos_targets, pos_weights, pos_offsets, ori_targets, ori_weights, ori_offsets, motion_targets, motion_weights):
         fn, blocks, opts, kinds = cfg["fn"], cfg["blocks"], cfg["options"], cfg["kinds"]
         dev = theta0.device
-        stream = torch.cuda.current_stream(dev).cuda_stream
         B = theta0.shape[0]
         efw32 = _f32c(efw, dev)
-        keep = []  # device buffers the asynchronous calls read
+        saved = {}  # device copies of everything the handle was given: the backward sends them again before it reads the handle
         # per-element error-function weights (buildMomentumErrorFunctions, tensor_ik_utility.cpp:149-181): folded into the per-instance
         # constraint weights for Position / Orientation; Limit and Motion carry one weight for the whole batch on the device
-        for name, tgt, w in (("position", pos_targets, pos_weights), ("orientation", ori_targets, ori_weights)):
+        for name, tgt, w, off in (("position", pos_targets, pos_weights, pos_offsets), ("orientation", ori_targets, ori_weights, ori_offsets)):
             if name not in blocks:
                 continue
             k = kinds.index(ErrorFunctionType.Position if name == "position" else ErrorFunctionType.Orientation)
-            t32 = _f32c(tgt, dev)
-            w32 = (_f32c(w, dev) * efw32[:, k:k + 1]).contiguous()
-            fn.set_targets_device(blocks[name], t32.data_ptr(), stream)
-            fn.set_constraint_weights_device(blocks[name], w32.data_ptr(), stream)
-            keep += [t32, w32]
+            rec = _f32c(tgt, dev)
+            if off is not None:  # instanced block: the record is target, then offset, per constraint
+                rec = torch.cat([rec, _f32c(off, dev).expand(rec.shape)], dim=-1).contiguous()
+            saved[name + "_record"] = rec
+            saved[name + "_weights"] = (_f32c(w, dev) * efw32[:, k:k + 1]).contiguous()
+        if "motion" in blocks:
+            saved["motion_targets"] = _f32c(motion_targets, dev)
         for name, kind in (("limit", ErrorFunctionType.Limit), ("motion", ErrorFunctionType.Motion)):
             if name not in blocks:
                 continue
             col = efw32[:, kinds.index(kind)]
-            w0 = float(col[0])
             if not bool(torch.all(col == col[0])):
                 raise ValueError(f"{name} error-function weights must be the same for every batch element on the device path")
-            fn.set_error_function_weight(blocks[name], w0)
-        if "motion" in blocks:
-            m32 = _f32c(motion_targets, dev)
-            fn.set_targets_device(blocks["motion"], m32.data_ptr(), stream)
-            keep.append(m32)
+        _SolveIK._send(cfg, efw32, saved, torch.cuda.current_stream(dev).cuda_stream)
         solver = ms.GaussNewtonSolver(opts, fn)
         theta = _f32c(theta0, dev).clone()
-        solver.solve_device(theta.data_ptr(), stream)
+        solver.solve_device(theta.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
         res = solver.get_results()  # synchronises; the NaN / Inf guard (tensor_ik.cpp:168-173) already ran on the device
         ctx.cfg = cfg
         ctx.status = res["status"]
-        ctx.save_for_backward(theta, efw32, *(keep))
-        ctx.keep_names = [n for n in ("position", "orientation") if n in blocks]
-        ctx.in_dtypes = (efw.dtype, None if pos_targets is None else pos_targets.dtype, None if pos_weights is None else pos_weights.dtype)
+        ctx.names = list(saved)
+        raw = [t.detach() if t is not None else None for t in (ori_targets, ori_offsets, pos_offsets, motion_weights)]
+        ctx.raw_present = [t is not None for t in raw]
+        ctx.save_for_backward(theta, efw32, *saved.values(), *[t for t in raw if t is not None])
+        ctx.in_dtypes = {k: (None if t is None else t.dtype) for k, t in (("efw", efw), ("pos_targets", pos_targets), ("pos_weights", pos_weights),
+                                                                           ("pos_offsets", pos_offsets), ("ori_targets", ori_targets), ("ori_weights", ori_weights),
+                                                                           ("ori_offsets", ori_offsets), ("motion_targets", motion_targets),
+                                                                           ("motion_weights", motion_weights))}
         cfg["last_results"] = res
         return theta.to(theta0.dtype)
+
+    @staticmethod
+    def _send(cfg, efw32, saved, stream):
+        """Targets, constraint weights, offsets and block weights into the cached handle (device to device, on ``stream``)."""
+        fn, blocks, kinds = cfg["fn"], cfg["blocks"], cfg["kinds"]
+        for name in ("position", "orientation"):
+            if name in blocks:
+                fn.set_targets_device(blocks[name], saved[name + "_record"].data_ptr(), stream)
+                fn.set_constraint_weights_device(blocks[name], saved[name + "_weights"].data_ptr(), stream)
+        for name, kind in (("limit", ErrorFunctionType.Limit), ("motion", ErrorFunctionType.Motion)):
+            if name in blocks:
+                fn.set_error_function_weight(blocks[name], float(efw32[0, kinds.index(kind)]))
+        if "motion" in blocks:
+            fn.set_targets_device(blocks["motion"], saved["motion_targets"].data_ptr(), stream)
 
     @staticmethod
     def backward(ctx, grad_theta):
         cfg = ctx.cfg
         fn, blocks, kinds, active = cfg["fn"], cfg["blocks"], cfg["kinds"], cfg["active"]
-        saved = ctx.saved_tensors
-        theta, efw32 = saved[0], saved[1]
+        tensors = ctx.saved_tensors
+        theta, efw32 = tensors[0], tensors[1]
+        saved = dict(zip(ctx.names, tensors[2:2 + len(ctx.names)]))
+        rest = iter(tensors[2 + len(ctx.names):])
+        ori_targets_raw, ori_offsets_raw, pos_offsets_raw, motion_weights_raw = [next(rest) if p else None for p in ctx.raw_present]
         dev = theta.device
         B, n = theta.shape
         stream = torch.cuda.current_stream(dev).cuda_stream
+        # another solve on the same cached handle may have run since this forward: give it this forward's inputs again
+        _SolveIK._send(cfg, efw32, saved, stream)
         ptr, ld = fn.get_jacobian_device(theta.data_ptr(), stream)
         rows = sum(cfg["block_rows"].values())
         torch.cuda.current_stream(dev).synchronize()
@@ -166,12 +214,14 @@ class _SolveIK(torch.autograd.Function):
         v = torch.zeros(B, n, dtype=torch.float64, device=dev)
         v[:, act] = va
         Jv = torch.einsum("brn,bn->br", J, v) * ok          # [B, rows], zero for unconverged elements
+        v_ok32 = (v * ok).float().contiguous()               # the direction the input contractions use (zero for unconverged elements)
         # rows of each block in the API-parity layout: blocks in the order they were added
         grad_efw = torch.zeros(B, len(kinds), dtype=torch.float64, device=dev)
-        grads = {"pos_targets": None, "pos_weights": None}
+        grads = {}
+        need = dict(zip(("pos_targets", "pos_weights", "pos_offsets", "ori_targets", "ori_weights", "ori_offsets", "motion_targets", "motion_weights"),
+                        ctx.needs_input_grad[3:]))
         row = 0
         sizes = cfg["block_rows"]
-        idx = 2
         for name in cfg["block_order"]:
             nr = sizes[name]
             rk, Jvk = r[:, row:row + nr], Jv[:, row:row + nr]
@@ -182,7 +232,7 @@ class _SolveIK(torch.autograd.Function):
             grad_efw[:, k] = torch.where(wk != 0, -2.0 * (rk * Jvk).sum(dim=1) / wk.clamp_min(1e-30) * (wk != 0), torch.zeros_like(wk))
             if name == "position":
                 nc = nr // 3
-                w_eff = saved[idx + 1].double()             # [B, nc] = constraint weight x error-function weight
+                w_eff = saved["position_weights"].double()   # [B, nc] = constraint weight x error-function weight
                 sq = torch.sqrt(w_eff)[:, :, None]
                 Jv3, r3 = Jvk.reshape(B, nc, 3), rk.reshape(B, nc, 3)
                 # rows = sqrt(w) (p - t): d/dt [grad E . (-v)] = 2 sqrt(w) (J_dev v)
@@ -190,15 +240,45 @@ class _SolveIK(torch.autograd.Function):
                 # d/d(constraint weight): grad E_c = 2 w J_c^T f_c -> -(2 J_c^T f_c) . v * efw = -(2 r_c . Jv_c) / w_eff * efw
                 cwg = -2.0 * (r3 * Jv3).sum(dim=2) / w_eff.clamp_min(1e-30) * (w_eff != 0)
                 grads["pos_weights"] = cwg * wk[:, None]
-                idx += 2
+                if need["pos_offsets"] and pos_offsets_raw is not None:
+                    go = torch.empty(B, nc, 3, device=dev)
+                    fn.input_gradients_device(blocks["position"], theta.data_ptr(), v_ok32.data_ptr(), grad_offsets_ptr=go.data_ptr(), stream=stream)
+                    grads["pos_offsets"] = _reduce_to(-go.double(), pos_offsets_raw)
             elif name == "orientation":
-                idx += 2
+                nc = nr // 9
+                if not (need["ori_targets"] or need["ori_weights"] or need["ori_offsets"]):
+                    row += nr
+                    continue
+                gw = torch.empty(B, nc, device=dev)
+                gt = torch.empty(B, nc, 4, device=dev)
+                go = torch.empty(B, nc, 4, device=dev) if ori_offsets_raw is not None else None
+                fn.input_gradients_device(blocks["orientation"], theta.data_ptr(), v_ok32.data_ptr(), gw.data_ptr(), 0 if go is None else go.data_ptr(),
+                                          gt.data_ptr(), stream)
+                grads["ori_weights"] = -gw.double() * wk[:, None]   # the device weight is constraint weight x error-function weight
+                grads["ori_targets"] = _normalization_backward(-gt.double(), ori_targets_raw.to(dev).double())
+                if go is not None:
+                    off = ori_offsets_raw.to(dev).double().expand(B, nc, 4)
+                    grads["ori_offsets"] = _reduce_to(_normalization_backward(-go.double(), off), ori_offsets_raw)
+            elif name == "motion":
+                # E = efw 0.1 sum_i w_i^2 (theta_i - t_i)^2 over the enabled parameters with w_i > 0 (model_parameters_error_function.cpp,
+                # kMotionWeight = 0.1): d/dt_i [grad E . v] = -2 s w_i^2 v_i,  d/dw_i = 4 s w_i (theta_i - t_i) v_i
+                mw = torch.as_tensor(cfg["motion_weights"], device=dev, dtype=torch.float64)
+                on = torch.as_tensor(active[:n] & (cfg["motion_weights"] > 0), device=dev)
+                sc = 0.1 * wk[:, None]
+                vv = (v * ok) * on
+                grads["motion_targets"] = 2.0 * sc * mw * mw * vv
+                gmw = -4.0 * sc * mw * (theta.double() - saved["motion_targets"].double()) * vv
+                if motion_weights_raw is not None:  # the device block holds the first row of [B, n] weights for the whole batch
+                    grads["motion_weights"] = gmw.sum(dim=0) if motion_weights_raw.dim() == 1 else torch.cat([gmw.sum(dim=0, keepdim=True), torch.zeros_like(gmw[1:])])
             row += nr
-        in_dt = ctx.in_dtypes
-        g_efw = grad_efw.to(in_dt[0])
-        g_pt = None if grads["pos_targets"] is None or in_dt[1] is None else grads["pos_targets"].to(in_dt[1])
-        g_pw = None if grads["pos_weights"] is None or in_dt[2] is None else grads["pos_weights"].to(in_dt[2])
-        return None, None, g_efw, g_pt, g_pw, None, None, None
+        dt = ctx.in_dtypes
+
+        def out(name):
+            t = grads.get(name)
+            return None if t is None or dt[name] is None or not need[name] else t.to(dt[name])
+
+        return (None, None, grad_efw.to(dt["efw"]), out("pos_targets"), out("pos_weights"), out("pos_offsets"), out("ori_targets"), out("ori_weights"),
+                out("ori_offsets"), out("motion_targets"), out("motion_weights"))
 
 
 def _device_view(ptr: int, shape, device):
@@ -218,8 +298,12 @@ def solve_ik(character: mc.Character, active_parameters, model_parameters_init: 
              orientation_cons_parents=None, orientation_cons_offsets=None, orientation_cons_weights=None, orientation_cons_targets=None,
              motion_targets=None, motion_weights=None) -> torch.Tensor:
     """Batched IK on the GPU; arguments as pymomentum.solver.solve_ik. ``model_parameters_init`` [B, n] must live on a CUDA device;
-    constraint parents / offsets are shared by the batch ([nc] / [nc, 3] / [nc, 4]), targets and weights are per element.
-    Differentiable w.r.t. ``error_function_weights``, ``position_cons_targets`` and ``position_cons_weights``."""
+    constraint parents are shared by the batch ([nc]); offsets are shared ([nc, 3] / [nc, 4]) or per element ([B, nc, 3] / [B, nc, 4]),
+    as tensors or arrays; targets and weights are per element.
+
+    Differentiable w.r.t. ``error_function_weights``, the position targets, weights and offsets, the orientation targets, weights and
+    offsets, and the motion targets and weights. Offsets that are batched or require grad use the instanced device block (offsets in
+    the per-element records), whose cached handle does not depend on the offset values; other offsets keep the shared block."""
     if not model_parameters_init.is_cuda:
         raise ValueError("momentum_b200.torch_ik.solve_ik runs on CUDA tensors (there is no CPU fallback)")
     options = options or SolverOptions()
@@ -234,13 +318,23 @@ def solve_ik(character: mc.Character, active_parameters, model_parameters_init: 
     def np_or_none(x, dt):
         return None if x is None else np.ascontiguousarray(x.detach().cpu().numpy() if torch.is_tensor(x) else x, dt)
 
+    def offsets(x, use, count, default):
+        """(shared offsets for the cache key, or None for the instanced block; the offsets as a tensor for the instanced block)"""
+        if not use:
+            return None, None
+        if x is None:
+            return np.tile(np.asarray(default, np.float32), (count, 1)), None
+        if (torch.is_tensor(x) and x.requires_grad) or np.ndim(x) == 3:
+            return None, x if torch.is_tensor(x) else torch.as_tensor(np.asarray(x, np.float32))
+        return np_or_none(x, np.float32), None
+
     use_pos = ErrorFunctionType.Position in kinds and position_cons_parents is not None
     use_ori = ErrorFunctionType.Orientation in kinds and orientation_cons_parents is not None
     use_motion = ErrorFunctionType.Motion in kinds and motion_targets is not None
     pp = np_or_none(position_cons_parents, np.int32) if use_pos else None
-    po = (np_or_none(position_cons_offsets, np.float32) if position_cons_offsets is not None else np.zeros((len(pp), 3), np.float32)) if use_pos else None
     op = np_or_none(orientation_cons_parents, np.int32) if use_ori else None
-    oo = (np_or_none(orientation_cons_offsets, np.float32) if orientation_cons_offsets is not None else np.tile(np.array([0, 0, 0, 1], np.float32), (len(op), 1))) if use_ori else None
+    po, po_t = offsets(position_cons_offsets, use_pos, 0 if pp is None else len(pp), [0, 0, 0])
+    oo, oo_t = offsets(orientation_cons_offsets, use_ori, 0 if op is None else len(op), [0, 0, 0, 1])
     mw = None
     if use_motion:
         mwt = motion_weights if motion_weights is not None else torch.ones(n)
@@ -258,11 +352,12 @@ def solve_ik(character: mc.Character, active_parameters, model_parameters_init: 
     # (tensor_ik.cpp:149-152): iterations / threshold only, radius 1.
     opts = ms.GaussNewtonSolverOptions(min_iterations=options.min_iter, max_iterations=options.max_iter, threshold=options.threshold, regularization=options.levmar_lambda,
                                        do_line_search=options.line_search, subset_line_search=True, linear_solver=linear)
-    cfg = {"fn": fn, "blocks": blocks, "options": opts, "kinds": kinds, "active": active, "block_order": order, "block_rows": block_rows}
+    cfg = {"fn": fn, "blocks": blocks, "options": opts, "kinds": kinds, "active": active, "block_order": order, "block_rows": block_rows, "motion_weights": mw}
     ones = lambda nc: torch.ones(B, nc, device=dev)
     pw = position_cons_weights if position_cons_weights is not None else (ones(len(pp)) if use_pos else None)
     ow = orientation_cons_weights if orientation_cons_weights is not None else (ones(len(op)) if use_ori else None)
-    out = _SolveIK.apply(cfg, model_parameters_init, efw, position_cons_targets if use_pos else None, pw if use_pos else None,
-                         orientation_cons_targets if use_ori else None, ow if use_ori else None, motion_targets if use_motion else None)
+    mwt = motion_weights if (use_motion and torch.is_tensor(motion_weights)) else None
+    out = _SolveIK.apply(cfg, model_parameters_init, efw, position_cons_targets if use_pos else None, pw if use_pos else None, po_t,
+                         orientation_cons_targets if use_ori else None, ow if use_ori else None, oo_t, motion_targets if use_motion else None, mwt)
     solve_ik.last_results = cfg.get("last_results")
     return out
