@@ -277,6 +277,27 @@ int mb2_solver_function_input_gradients_device(mb2_solver_function* f, int32_t i
                                                const float* direction_device /*[B][n]*/, float* grad_weights_device, float* grad_offsets_device,
                                                float* grad_targets_device, void* cuda_stream);
 
+/* Direction of the implicit-function backward of solve_ik: the reference's hessianInverseTimes
+ * (diff_ik/fully_differentiable_body_ik.cpp:74-109) with the quantities d_modelParams_d_inputs (:112-238) needs beside it. For every
+ * instance b, with E the enabled parameters, J_E the rows x |E| slice of the Jacobian at theta_b (the matrix
+ * mb2_solver_function_get_jacobian_device writes; rows = the unpadded residual rows), r the residual and g = grad_parameters[b]
+ * restricted to E:
+ *   direction [B][n]                v_E = (2 J_E^T J_E)^+ g = 1/2 V diag(1 / s^2 if s^2 >= 1e-5, else 0) V^T g  (J_E = U S V^T, s^2
+ *                                   compared in double); 0 on disabled parameters, and everywhere when E is empty
+ *   jacobian_direction [B][rows8]   J v
+ *   residual [B][rows8]             r
+ *   gradient_rms [B]                sqrt(mean over E of (2 J_E^T r)^2), the RMS d_modelParams_d_inputs reports (0 when E is empty)
+ * rows8 = mb2_solver_function_jacobian_rows (rows padded to 8; the padding rows are written 0). v then feeds
+ * mb2_solver_function_input_gradients_device, and the per-block weight and target contractions follow from r and J v. The Jacobian
+ * sweep and the solve (float64 Gram matrix on the smaller side of J_E, cyclic Jacobi eigen-solve) run on the device; device memory in
+ * and out, asynchronous on `cuda_stream` (NULL = the legacy default stream), no host synchronisation. A null jacobian_direction,
+ * residual or gradient_rms is skipped. A null parameters, gradient or direction pointer, or memory that is not device memory on the
+ * function's device, is MB2_ERR_INVALID_ARGUMENT. The call uses the handle's Jacobian buffer: calls on the same handle must not overlap. */
+int mb2_solver_function_implicit_direction_device(mb2_solver_function* f, const float* parameters_device /*[B][n]*/,
+                                                  const float* grad_parameters_device /*[B][n]*/, float* direction_device /*[B][n]*/,
+                                                  float* jacobian_direction_device /*[B][rows8]*/, float* residual_device /*[B][rows8]*/,
+                                                  float* gradient_rms_device /*[B]*/, void* cuda_stream);
+
 /* ---- GaussNewtonSolverT<float> x B (solver/gauss_newton_solver.h:67-137, solver/solver.h:36-100) ---- */
 int mb2_solver_create(mb2_solver_function* f, const mb2_gauss_newton_options* opt, mb2_solver** out);
 void mb2_solver_destroy(mb2_solver* s);

@@ -148,6 +148,7 @@ struct mb2_solver_function {
   // device data
   DeviceBuffer<float> dTargets, dWeights, dJ, dTheta, dState, dH, dTargetStage;
   DeviceBuffer<double> dErrors;
+  DeviceBuffer<double> dJacobi;          // implicit direction: per-CTA rotation logs (and Gram matrices too large for shared memory)
   std::unique_ptr<DeviceSchedule> sched; // Cholesky schedule of the current (compact) plan
   FunctionTables tables() const;
 };
@@ -986,6 +987,48 @@ int mb2_solver_function_input_gradients_device(mb2_solver_function* f, int32_t i
   a.gradOffsets = grad_offsets_device;
   a.gradTargets = grad_targets_device;
   MB2_CUDA(launchInputGradients(a, st));
+  return MB2_OK;
+}
+
+int mb2_solver_function_implicit_direction_device(mb2_solver_function* f, const float* parameters_device, const float* grad_parameters_device,
+                                                  float* direction_device, float* jacobian_direction_device, float* residual_device,
+                                                  float* gradient_rms_device, void* cuda_stream) {
+  MB2_CHECK(f != nullptr, "null solver function");
+  MB2_CHECK(parameters_device != nullptr && grad_parameters_device != nullptr, "null parameters or gradient");
+  MB2_CHECK(direction_device != nullptr, "null direction");
+  MB2_DEVICE_GUARD(f->ch->device);
+  const float* ins[2] = {parameters_device, grad_parameters_device};
+  float* outs[4] = {direction_device, jacobian_direction_device, residual_device, gradient_rms_device};
+  bool onDevice = true;
+  for (const float* p : ins) onDevice = onDevice && isDeviceMemoryOn(p, f->ch->device);
+  for (float* o : outs) onDevice = onDevice && (o == nullptr || isDeviceMemoryOn(o, f->ch->device));
+  MB2_CHECK(onDevice, "implicit direction: every array must be device memory on the function's device");
+  int rc = ensurePlan(f, 0); // the API-order Jacobian: column c = model parameter c
+  if (rc != MB2_OK) return rc;
+  NvtxRange range("implicitDirection");
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  MB2_CUDA(launchSweep(sweepArgs(f, parameters_device, nullptr), true, st));
+  ImplicitDirectionArgs a{};
+  a.batch = f->B;
+  a.numParams = f->ch->host.numParams;
+  a.rows = f->plan.numRows;
+  a.rowStride = mb2_solver_function_jacobian_rows(f);
+  a.ldJ = f->ldJ;
+  a.jacobian = f->dJ.p;
+  a.enabledList = f->dEnabledList.p;
+  a.numEnabled = int(f->plan.enabledList.size());
+  a.gradParameters = grad_parameters_device;
+  a.direction = direction_device;
+  a.jacobianDirection = jacobian_direction_device;
+  a.residual = residual_device;
+  a.gradientRms = gradient_rms_device;
+  ImplicitDirectionConfig cfg;
+  MB2_CUDA(implicitDirectionConfigure(a, cfg));
+  MB2_CUDA(f->dJacobi.resize(std::max<size_t>(1, size_t(cfg.grid) * cfg.slotDoubles)));
+  a.scratch = f->dJacobi.p;
+  a.slotDoubles = cfg.slotDoubles;
+  a.gramInShared = cfg.gramInShared ? 1 : 0;
+  MB2_CUDA(launchImplicitDirection(a, cfg, st));
   return MB2_OK;
 }
 

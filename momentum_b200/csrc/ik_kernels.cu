@@ -20,6 +20,7 @@
 #include "ik_jtj_tc.cuh"
 #include "ik_ptx.cuh"
 #include "ik_device.cuh"
+#include "ik_jacobi.cuh"
 
 namespace mb2 {
 
@@ -501,6 +502,154 @@ cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream
     case 4: return launch(inputGradientKernel<4>);
     default: return launch(inputGradientKernel<8>);
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Implicit-function direction of solve_ik's backward (ik_jacobi.cuh): per instance v = (2 J_E^T J_E)^+ g, J v, the residual and the
+// gradient RMS, from the K-major Jacobian the sweep wrote. A persistent grid with one CTA per instance in flight:
+//   lanes = E: g, the gradient terms;  lanes = the triangle's columns, row by row: the float64 Gram K;  lanes = k: y
+//   per sweep, per round-robin step: lanes = pairs: rotations, diagonal blocks, Q^T y, the log;  lanes = off-diagonal 2 x 2 blocks
+//   lanes = k: the truncated inverse eigenvalues;  the log backwards, lanes = pairs;  lanes = E: v;  lanes = rows: J v
+// K sits in shared memory when it fits, else in the CTA's global scratch slot (slot = blockIdx.x), which also holds the rotation log.
+// Every sum is one lane's loop in a fixed order and there are no atomics: a result depends neither on the batch nor on the launch shape.
+// ------------------------------------------------------------------------------------------------
+constexpr int kJacobiThreads = 256;
+constexpr size_t kJacobiScratchBudget = size_t(2) << 30; // the persistent grid is trimmed so that its scratch slots stay below 2 GiB
+
+// shared memory besides K: y [k], g [n_E], v_E [n_E], c / s [h] (doubles), p / q [h] (ints)
+static size_t implicitDirectionExtraBytes(int k, int nE) {
+  const size_t h = size_t(jacobiPairs(k));
+  return (sizeof(double) * (size_t(k) + 2 * size_t(nE) + 2 * h) + sizeof(int) * 2 * h + 15) / 16 * 16;
+}
+
+__global__ void __launch_bounds__(kJacobiThreads) implicitDirectionKernel(const ImplicitDirectionArgs a) {
+  extern __shared__ __align__(16) double dsm[];
+  __shared__ int rotated;
+  __shared__ double floorK;
+  const int tid = threadIdx.x, nt = blockDim.x;
+  const int n = a.numParams, rows = a.rows, nE = a.numEnabled, ld = a.ldJ;
+  const bool rowsSide = rows <= nE;
+  const int k = rowsSide ? rows : nE, h = jacobiPairs(k), steps = jacobiSteps(k);
+  const size_t kp = jacobiPackedSize(k);
+  double* slot = a.scratch + size_t(blockIdx.x) * a.slotDoubles;
+  double2* rlog = reinterpret_cast<double2*>(slot);
+  double* K = a.gramInShared ? dsm : slot + jacobiLogDoubles(k);
+  double* y = dsm + (a.gramInShared ? kp : 0);
+  double* g = y + k;
+  double* vE = g + nE;
+  double* rc = vE + nE;
+  double* rs = rc + h;
+  int* rp = reinterpret_cast<int*>(rs + h);
+  int* rq = rp + h;
+  const int32_t* E = a.enabledList;
+  for (int b = blockIdx.x; b < a.batch; b += gridDim.x) {
+    const float* J = a.jacobian + size_t(b) * (n + 1) * ld;
+    const float* res = J + size_t(n) * ld;
+    for (int i = tid; i < nE; i += nt) g[i] = double(a.gradParameters[size_t(b) * n + E[i]]);
+    if (a.residual)
+      for (int r = tid; r < a.rowStride; r += nt) a.residual[size_t(b) * a.rowStride + r] = r < rows ? res[r] : 0.f;
+    __syncthreads();
+    for (int i = tid; i < nE; i += nt) {
+      const double gi = jacobiGradient(J, ld, E, rows, res, i);
+      vE[i] = gi * gi;
+    }
+    for (int r = 0; r < k; ++r)
+      for (int c = r + tid; c < k; c += nt) K[jacobiPacked(r, c, k)] = jacobiGram(J, ld, E, nE, rows, rowsSide, r, c);
+    for (int i = tid; i < k; i += nt) y[i] = jacobiRhs(J, ld, E, nE, rowsSide, g, i);
+    __syncthreads();
+    if (tid == 0) {
+      double s = 0.0, d = 0.0;
+      for (int i = 0; i < nE; ++i) s += vE[i];
+      if (a.gradientRms) a.gradientRms[b] = nE > 0 ? float(sqrt(s / nE)) : 0.f;
+      for (int i = 0; i < k; ++i) d = fmax(d, K[jacobiPacked(i, i, k)]);
+      floorK = jacobiFloor(d);
+    }
+    __syncthreads();
+    const double floor = floorK;
+    int sweeps = 0;
+    while (k > 1 && sweeps < kJacobiMaxSweeps) {
+      if (tid == 0) rotated = 0;
+      __syncthreads();
+      for (int st = 0; st < steps; ++st) {
+        double2* lg = rlog + (size_t(sweeps) * steps + st) * h;
+        for (int t = tid; t < h; t += nt) {
+          int p, q;
+          jacobiPair(k, st, t, p, q);
+          double c = 1.0, s = 0.0, tt = 0.0;
+          if (q >= 0 && jacobiRotation(K[jacobiPacked(p, p, k)], K[jacobiPacked(q, q, k)], K[jacobiPacked(p, q, k)], floor, c, s, tt)) {
+            jacobiRotateDiagonal(K, k, p, q, tt);
+            jacobiRotateTransposed(y, p, q, c, s);
+            rotated = 1;
+          }
+          rp[t] = p; rq[t] = q; rc[t] = c; rs[t] = s;
+          lg[t] = make_double2(c, s);
+        }
+        __syncthreads();
+        const int blocks = h * (h - 1) / 2;
+        for (int L = tid; L < blocks; L += nt) {
+          int i, j;
+          jacobiBlock(L, i, j);
+          if (rs[i] == 0.0 && rs[j] == 0.0) continue; // both identity
+          jacobiRotateBlock(K, k, rp[i], rq[i], rc[i], rs[i], rp[j], rq[j], rc[j], rs[j]);
+        }
+        __syncthreads();
+      }
+      const bool any = rotated != 0;
+      __syncthreads(); // every lane has read the flag before the next sweep clears it
+      if (!any) break; // a sweep without a rotation: converged (its log entries are identities and are not replayed)
+      ++sweeps;
+    }
+    for (int i = tid; i < k; i += nt) y[i] = jacobiScale(K[jacobiPacked(i, i, k)], y[i], rowsSide);
+    __syncthreads();
+    for (int st = sweeps * steps - 1; st >= 0; --st) { // z <- Q z: the rotations in reverse order
+      const double2* lg = rlog + size_t(st) * h;
+      const int step = st % steps;
+      for (int t = tid; t < h; t += nt) {
+        const double2 cs = lg[t];
+        if (cs.y == 0.0) continue;
+        int p, q;
+        jacobiPair(k, step, t, p, q);
+        jacobiRotateForward(y, p, q, cs.x, cs.y);
+      }
+      __syncthreads();
+    }
+    for (int i = tid; i < nE; i += nt) vE[i] = jacobiDirection(J, ld, E, rows, rowsSide, y, i);
+    float* dir = a.direction ? a.direction + size_t(b) * n : nullptr;
+    if (dir)
+      for (int c = tid; c < n; c += nt) dir[c] = 0.f;
+    __syncthreads();
+    if (dir)
+      for (int i = tid; i < nE; i += nt) dir[E[i]] = float(vE[i]);
+    if (a.jacobianDirection)
+      for (int r = tid; r < a.rowStride; r += nt)
+        a.jacobianDirection[size_t(b) * a.rowStride + r] = r < rows ? float(jacobiJv(J, ld, E, nE, vE, r)) : 0.f;
+    __syncthreads(); // the next instance overwrites g / v_E / y / K
+  }
+}
+
+cudaError_t implicitDirectionConfigure(const ImplicitDirectionArgs& a, ImplicitDirectionConfig& cfg) {
+  const int k = std::min(a.rows, a.numEnabled);
+  const size_t extra = implicitDirectionExtraBytes(k, a.numEnabled), gram = sizeof(double) * jacobiPackedSize(k);
+  cfg.gramInShared = extra + gram <= size_t(g_maxSmemOptin);
+  cfg.smem = extra + (cfg.gramInShared ? gram : 0);
+  if (cfg.smem > size_t(g_maxSmemOptin)) return cudaErrorInvalidConfiguration;
+  cfg.slotDoubles = (jacobiLogDoubles(k) + (cfg.gramInShared ? 0 : jacobiPackedSize(k)) + 1) & ~size_t(1); // slots stay 16-byte aligned
+  cudaError_t e = cudaFuncSetAttribute(implicitDirectionKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cfg.smem));
+  if (e != cudaSuccess) return e;
+  int perSm = 0;
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, implicitDirectionKernel, kJacobiThreads, cfg.smem);
+  if (e != cudaSuccess) return e;
+  long grid = long(std::max(g_numSms, 1)) * std::max(perSm, 1);
+  grid = std::min(grid, long(std::max(a.batch, 1)));
+  if (cfg.slotDoubles > 0) grid = std::min(grid, long(std::max<size_t>(1, kJacobiScratchBudget / (sizeof(double) * cfg.slotDoubles))));
+  cfg.grid = int(grid);
+  return cudaSuccess;
+}
+
+cudaError_t launchImplicitDirection(const ImplicitDirectionArgs& a, const ImplicitDirectionConfig& cfg, cudaStream_t stream) {
+  if (a.batch <= 0) return cudaSuccess;
+  implicitDirectionKernel<<<cfg.grid, kJacobiThreads, cfg.smem, stream>>>(a);
+  return cudaGetLastError();
 }
 
 

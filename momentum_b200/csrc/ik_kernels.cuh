@@ -172,6 +172,35 @@ struct InputGradientArgs {
   float* gradTargets;        // [B][nc][3|4] or null
 };
 cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream);
+// implicitDirectionKernel: per instance v = (2 J_E^T J_E)^+ g (the reference's hessianInverseTimes, ik_jacobi.cuh), J v, the residual
+// and the gradient RMS, from the K-major Jacobian [B][n + 1][ldJ] of a mode-0 plan
+struct ImplicitDirectionArgs {
+  int32_t batch;
+  int32_t numParams;         // n
+  int32_t rows;              // unpadded residual rows of the plan
+  int32_t rowStride;         // floats per instance of jacobianDirection / residual (>= rows; the rows past `rows` are written 0)
+  int32_t ldJ;
+  const float* jacobian;     // [B][n + 1][ldJ], column n = residual
+  const int32_t* enabledList; // E, ascending [numEnabled]
+  int32_t numEnabled;
+  const float* gradParameters; // [B][n] dLoss / d theta
+  float* direction;          // [B][n] v, 0 on disabled parameters; or null
+  float* jacobianDirection;  // [B][rowStride] J v; or null
+  float* residual;           // [B][rowStride]; or null
+  float* gradientRms;        // [B] sqrt(mean_E (2 J_E^T r)^2); or null
+  double* scratch;           // [grid][slotDoubles]: the rotation log, then K when it does not fit in shared memory
+  size_t slotDoubles;
+  int32_t gramInShared;
+};
+struct ImplicitDirectionConfig {
+  int grid{0};
+  size_t smem{0};
+  bool gramInShared{true};
+  size_t slotDoubles{0};     // scratch per CTA; the launch needs grid x slotDoubles doubles
+};
+// sizes the persistent grid (shared memory, occupancy, the scratch budget) for a.rows / a.numEnabled / a.batch
+cudaError_t implicitDirectionConfigure(const ImplicitDirectionArgs& a, ImplicitDirectionConfig& cfg);
+cudaError_t launchImplicitDirection(const ImplicitDirectionArgs& a, const ImplicitDirectionConfig& cfg, cudaStream_t stream);
 cudaError_t launchSweep(const SweepArgs& a, bool jacobian, cudaStream_t stream);
 size_t sweepSmemPerInstance(const FunctionTables& T, int warpsPerInstance);
 cudaError_t launchJtJSimt(const JtJArgs& a, cudaStream_t stream);

@@ -75,6 +75,7 @@ CABI_SYMBOLS = [
     "mb2_sharded_solver_shard_info", "mb2_sharded_solver_set_options", "mb2_sharded_solver_set_targets", "mb2_sharded_solver_solve", "mb2_sharded_solver_get_aggregate",
     "mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device",
     "mb2_add_orientation_error_function_instanced", "mb2_solver_function_input_gradients_device",
+    "mb2_solver_function_implicit_direction_device",
 ]
 
 _libs = {}
@@ -174,6 +175,8 @@ def load_library(path: Optional[str] = None):
     if hasattr(L, "mb2_solver_function_input_gradients_device"):
         L.mb2_add_orientation_error_function_instanced.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_int32, C.c_int32, _ip, _fp, _ip]
         L.mb2_solver_function_input_gradients_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
+    if hasattr(L, "mb2_solver_function_implicit_direction_device"):
+        L.mb2_solver_function_implicit_direction_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     _libs[path] = L
     return L
 
@@ -373,6 +376,16 @@ class SkeletonSolverFunction(_Base):
         self._check(self._L.mb2_solver_function_input_gradients_device(self._h, int(index), C.c_void_p(params_device_ptr), C.c_void_p(direction_device_ptr),
                                                                        C.c_void_p(grad_weights_ptr or None), C.c_void_p(grad_offsets_ptr or None),
                                                                        C.c_void_p(grad_targets_ptr or None), C.c_void_p(stream)))
+
+    def implicit_direction_device(self, params_device_ptr: int, grad_params_device_ptr: int, direction_ptr: int, jacobian_direction_ptr: int = 0,
+                                  residual_ptr: int = 0, gradient_rms_ptr: int = 0, stream: int = 0):
+        """The direction of solve_ik's implicit-function backward per instance: v = (2 J_E^T J_E)^+ g [B][n] (0 on disabled
+        parameters), J v and the residual [B][jacobian_rows] and the gradient RMS [B], from parameters and dLoss/dtheta [B][n]; float32
+        device memory (0 = skip that output; the direction is required), enqueued on ``stream``."""
+        self._check(self._L.mb2_solver_function_implicit_direction_device(self._h, C.c_void_p(params_device_ptr), C.c_void_p(grad_params_device_ptr),
+                                                                          C.c_void_p(direction_ptr or None), C.c_void_p(jacobian_direction_ptr or None),
+                                                                          C.c_void_p(residual_ptr or None), C.c_void_p(gradient_rms_ptr or None),
+                                                                          C.c_void_p(stream)))
 
     def set_error_function_weight(self, index: int, weight: float):
         self._check(self._L.mb2_set_error_function_weight(self._h, index, weight))

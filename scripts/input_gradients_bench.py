@@ -1,14 +1,17 @@
 """Timing of the input contraction of solve_ik's backward (mb2_solver_function_input_gradients_device) against the same contraction
 written in float32 torch autograd on the same GPU, and of one whole solve_ik backward split into its parts.
 
-    python scripts/input_gradients_bench.py [--reps 5] [--iters 50] [--warmup 10] [--batch 8192] [--backward-batch 1024]
+    python scripts/input_gradients_bench.py [--reps 5] [--iters 50] [--warmup 10] [--batch 8192] [--backward-batch 1024 8192] [--no-svd]
 
 1. Kernel: B x humanoid72 with cfg3's constraints (24 Position, 6 Orientation). Per block it prints microseconds per call, instances per
    second and the achieved HBM bytes per second from the algorithmic bytes per instance: theta and v (8 n), the block's records and
    weights, and the three outputs (4 nc (1 + 2 k) with k = 3 or 4). The torch side is grad_theta E . v by double autograd through the
    float32 FK of scripts/skeleton_state_bench.py, differentiated with respect to the same inputs.
-2. Backward: one solve_ik backward (Position + Orientation, every input requiring grad) at a batch where the float64 SVD finishes in
-   reasonable time, split into the Jacobian read (sweep + copy), the SVD, the kernel calls and the rest (total minus those).
+2. Backward: one solve_ik backward (Position + Orientation, every input requiring grad) at each --backward-batch, split into the
+   direction entry (mb2_solver_function_implicit_direction_device: Jacobian sweep + Jacobi kernel), the input kernels and the rest
+   (total minus those). At 1024 one float64 torch.linalg.svd of the same Jacobian, the algorithm the entry replaced, is the comparison.
+3. The direction entry alone on humanoid72 with Position + Orientation + Limit + Motion (k = 220) and on 32 x bodyhands300 cfg4
+   (k = 424, the Gram matrix in global memory).
 Times are CUDA events around `iters` calls after a warm-up; the median of `reps` windows is reported, with the fastest in brackets.
 The card and its power limit are printed first. There is no CPU path: without a GPU it fails.
 """
@@ -28,7 +31,7 @@ for p in (ROOT, os.path.join(ROOT, "scripts")):
 from momentum_b200 import character as mc  # noqa: E402
 from momentum_b200 import solver as ms  # noqa: E402
 from momentum_b200 import torch_ik as ti  # noqa: E402
-from momentum_b200.problems import humanoid_problem  # noqa: E402
+from momentum_b200.problems import add_test_limits, bodyhands_problem, humanoid_problem  # noqa: E402
 from skeleton_state_bench import TorchFK, card, timed  # noqa: E402
 
 
@@ -92,8 +95,9 @@ def kernel_case(args, dev, name):
         print(json.dumps({"case": f"{block}", "max_rel_diff_vs_torch_fp32": agree}))
 
 
-def backward_case(args, dev, name):
-    B = args.backward_batch
+def backward_case(args, dev, name, B, svd_column):
+    """one solve_ik backward at B x humanoid72 cfg3: total, the direction entry (Jacobian sweep + Jacobi kernel), the input kernels and
+    the rest; with ``svd_column`` also one float64 torch.linalg.svd of the same Jacobian, the algorithm the entry replaced"""
     ch, efs, _, theta_star = humanoid_problem(B, orientation=True)
     pos, ori = efs
     n = ch.num_params
@@ -129,17 +133,7 @@ def backward_case(args, dev, name):
     theta = torch.from_numpy(theta_star.astype(np.float32)).to(dev)
     v = torch.from_numpy(np.random.default_rng(2).normal(size=(B, n)).astype(np.float32)).to(dev)
     stream = torch.cuda.current_stream(dev).cuda_stream
-    rows = 3 * len(pos.parents) + 9 * len(ori.parents)
-
-    def jacobian():
-        ptr, ld = fn.get_jacobian_device(theta.data_ptr(), stream)
-        return ti._device_view(ptr, (B, n + 1, ld), dev).clone()
-
-    Jd = jacobian()[:, :n, :rows].transpose(1, 2).double()
-
-    def svd():
-        torch.linalg.svd(Jd, full_matrices=False)
-
+    parts = {"direction": direction_us(args, fn, theta, v, stream)}
     outs = {k: [torch.empty(B, len(e.parents), device=dev), torch.empty(B, len(e.parents), kk, device=dev), torch.empty(B, len(e.parents), kk, device=dev)]
             for k, e, kk in (("position", pos, 3), ("orientation", ori, 4))}
 
@@ -147,12 +141,40 @@ def backward_case(args, dev, name):
         for k in ("position", "orientation"):
             fn.input_gradients_device(blocks[k], theta.data_ptr(), v.data_ptr(), *(o.data_ptr() for o in outs[k]), stream=stream)
 
-    parts = {}
-    for label, f in (("jacobian_read", jacobian), ("svd", svd), ("kernel", kernels)):
-        parts[label] = timed(f, args.reps, max(1, args.iters // 10), 2)[0]
+    parts["input_kernels"] = timed(kernels, args.reps, max(1, args.iters // 10), 2)[0]
     parts["rest"] = t_total - sum(parts.values())
-    rec = {"case": f"solve_ik backward, {B} x humanoid72 cfg3", "total_us": round(t_total, 1), **{k + "_us": round(x, 1) for k, x in parts.items()}, "card": name}
+    rec = {"case": f"solve_ik backward, {B} x humanoid72 cfg3", "total_us": round(t_total, 1), **{k + "_us": round(x, 1) for k, x in parts.items()}}
+    if svd_column:  # a single call: it takes seconds
+        rows = 3 * len(pos.parents) + 9 * len(ori.parents)
+        ptr, ld = fn.get_jacobian_device(theta.data_ptr(), stream)
+        Jd = ti._device_view(ptr, (B, n + 1, ld), dev).clone()[:, :n, :rows].transpose(1, 2).double()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        torch.linalg.svd(Jd, full_matrices=False)
+        b.record()
+        b.synchronize()
+        rec["torch_f64_svd_us"] = round(a.elapsed_time(b) * 1e3, 1)
+    rec["card"] = name
     print(json.dumps(rec))
+
+
+def direction_us(args, fn, theta, g, stream):
+    """median microseconds of one mb2_solver_function_implicit_direction_device call (Jacobian sweep + Jacobi kernel)"""
+    B, n = theta.shape
+    out = [torch.empty(B, n, device=theta.device), torch.empty(B, fn.jacobian_rows, device=theta.device),
+           torch.empty(B, fn.jacobian_rows, device=theta.device), torch.empty(B, device=theta.device)]
+    f = lambda: fn.implicit_direction_device(theta.data_ptr(), g.data_ptr(), *(o.data_ptr() for o in out), stream=stream)
+    return timed(f, args.reps, max(1, args.iters // 10), 2)[0]
+
+
+def direction_case(args, dev, name, label, ch, efs, B, theta):
+    """the direction entry alone on a larger k"""
+    fn = ms.SkeletonSolverFunction(ch, B, efs, device=0)
+    fn.upload_targets()
+    th = torch.from_numpy(np.asarray(theta, np.float32)).to(dev)
+    g = torch.from_numpy(np.random.default_rng(3).normal(size=th.shape).astype(np.float32)).to(dev)
+    us = direction_us(args, fn, th, g, torch.cuda.current_stream(dev).cuda_stream)
+    print(json.dumps({"case": f"implicit direction, {B} x {label}", "direction_us": round(us, 1), "card": name}))
 
 
 def main():
@@ -161,7 +183,8 @@ def main():
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--batch", type=int, default=8192)
-    ap.add_argument("--backward-batch", type=int, default=1024)
+    ap.add_argument("--backward-batch", type=int, nargs="+", default=[1024, 8192])
+    ap.add_argument("--no-svd", action="store_true", help="skip the float64 torch SVD column (seconds per call)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("input_gradients_bench: no CUDA device (there is no CPU path)")
@@ -169,7 +192,18 @@ def main():
     name = card()
     print(f"card: {name} (name, power limit)")
     kernel_case(args, dev, name)
-    backward_case(args, dev, name)
+    for B in args.backward_batch:
+        backward_case(args, dev, name, B, svd_column=B == 1024 and not args.no_svd)
+    # Position + Orientation + Limit + Motion on humanoid72 (k = n_E = 220, the largest Gram matrix in shared memory)
+    B = args.backward_batch[0]
+    ch, efs, _, star = humanoid_problem(B, orientation=True)
+    rng = np.random.default_rng(4)
+    add_test_limits(ch, rng, ellipsoid=False)
+    efs = efs + [mc.LimitErrorFunction(weight=1.0), mc.ModelParametersErrorFunction(rng.uniform(0.3, 1.0, ch.num_params), star, weight=1.0)]
+    direction_case(args, dev, name, "humanoid72 Position + Orientation + Limit + Motion (k = 220)", ch, efs, B, star + 0.05 * rng.normal(size=star.shape))
+    # cfg4 (k = 424: the Gram matrix in global memory)
+    ch, efs, _, star = bodyhands_problem(32)
+    direction_case(args, dev, name, "bodyhands300 cfg4 (k = 424)", ch, efs, 32, star + 0.05 * rng.normal(size=star.shape))
 
 
 if __name__ == "__main__":
