@@ -263,6 +263,34 @@ int mb2_character_skeleton_state_backward_device(const mb2_character* c, int32_t
                                                  const float* grad_skeleton_state_device, float* grad_model_parameters_device,
                                                  void* cuda_stream);
 
+/* Linear-blend skinning of the character (SkinWeights, skin_weights.h:19-40, and Character::inverseBindPose), host arrays, replacing
+ * any earlier skinning: rest_vertices [V][3], skin_index / skin_weight [V][8] (a vertex's influences end at its first zero weight,
+ * linear_skinning.cpp:76-80; the slots after it are ignored whatever they hold), inverse_bind_pose [J][12] (the row-major top 3x4 of
+ * Affine3f::matrix()). An active slot's index outside [0, J) or non-finite weight, a non-finite vertex or inverse bind pose, or V < 1 is
+ * MB2_ERR_INVALID_ARGUMENT, and leaves any earlier skinning in place (as does a failed upload). The new tables go to fresh device
+ * buffers and the call synchronises the device before it frees the old ones, so skinning work already enqueued on any stream finishes
+ * with the tables it was enqueued with; the call must not run concurrently with another call on the same character from another host
+ * thread. mb2_character_clone copies the skinning. */
+int mb2_character_set_skinning(mb2_character* c, int32_t num_vertices, const float* rest_vertices, const int32_t* skin_index,
+                               const float* skin_weight, const float* inverse_bind_pose);
+/* V of the skinning, 0 when the character has none */
+int32_t mb2_character_num_vertices(const mb2_character* c);
+/* pymomentum Character.skin_points (pymomentum/torch/character.py:1050-1068; applySSD, linear_skinning.cpp:40-102, with
+ * computeSkinningTransforms, :22-37, and q normalised as skel_state_backend.py:435-512 does): skel_state [B][J][8] -> points [B][V][3].
+ * rest_points NULL = the character's rest mesh, else [V][3] shared by the batch (rest_points_batched == 0) or [B][V][3] (== 1).
+ * Device memory on `cuda_stream`, asynchronous; batch == 0 is a no-op. No skinning, a null required pointer, batch < 0 or a pointer
+ * that is not device memory on the character's device is MB2_ERR_INVALID_ARGUMENT. */
+int mb2_character_skin_points_device(const mb2_character* c, int32_t batch, const float* skel_state_device, const float* rest_points_device,
+                                     int32_t rest_points_batched, float* points_device, void* cuda_stream);
+/* its backward (SkinPointsFunction::backward, tensor_skinning.cpp:171-330) from dLoss/d points [B][V][3]: grad_skel_state [B][J][8],
+ * grad_rest_points in the rest-point layout ([V][3] = the batch sum when shared, :320-322), both overwritten, a NULL output is skipped.
+ * grad_rest_points must be NULL when the rest mesh is skinned. Same rules as the forward. The call takes stream-ordered scratch from
+ * the device's default memory pool (cudaMallocAsync / cudaFreeAsync on `cuda_stream`): at most 256 MiB for the skel-state gradient and
+ * 128 x V x 3 floats for a shared rest-point gradient. A framework's own caching allocator does not see it. */
+int mb2_character_skin_points_backward_device(const mb2_character* c, int32_t batch, const float* skel_state_device, const float* rest_points_device,
+                                              int32_t rest_points_batched, const float* grad_points_device, float* grad_skel_state_device,
+                                              float* grad_rest_points_device, void* cuda_stream);
+
 /* Input contraction of the implicit-function backward of solve_ik (diff_ik d_gradient_d_input_dot): for block `index` and every
  * instance b, the derivatives of grad_theta E_index(theta_b) . v_b with respect to the block's inputs, at the targets, constraint weights
  * and offsets the handle currently holds:

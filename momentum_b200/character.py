@@ -64,6 +64,24 @@ class ParameterLimit:
         return i, f
 
 
+MAX_SKIN_JOINTS = 8  # kMaxSkinJoints, skin_weights.h:19
+
+
+@dataclass
+class Skinning:
+    """Linear-blend skinning of a character: ``SkinWeights`` (skin_weights.h:19-40) and ``Character::inverseBindPose``. A vertex's
+    influences end at its first zero weight (linear_skinning.cpp:76-80); the slots after it are ignored."""
+
+    rest_vertices: np.ndarray  # float32 [V,3]
+    skin_index: np.ndarray  # int32 [V,8]
+    skin_weight: np.ndarray  # float32 [V,8]
+    inverse_bind_pose: np.ndarray  # float32 [J,3,4]: the top 3x4 of Affine3f::matrix()
+
+    @property
+    def num_vertices(self) -> int:
+        return int(self.rest_vertices.shape[0])
+
+
 @dataclass
 class Character:
     parents: np.ndarray  # int32 [J], -1 = root, parents precede children
@@ -76,6 +94,7 @@ class Character:
     pt_offsets: np.ndarray  # float32 [7J]
     limits: List[ParameterLimit] = field(default_factory=list)
     name: str = "character"
+    skinning: Optional[Skinning] = None
 
     @property
     def num_joints(self) -> int:
@@ -466,6 +485,85 @@ def world_points(ch: Character, theta, parents, offsets):
     if off.ndim == 2:
         off = off[None]
     return t[:, parents] + _qrot(q[:, parents], s[:, parents, None] * off)
+
+
+def _quat_matrix(q):
+    """Eigen toRotationMatrix of (normalised) quaternions [..., 4] xyzw -> [..., 3, 3]."""
+    x, y, z, w = q[..., 0], q[..., 1], q[..., 2], q[..., 3]
+    return np.stack([np.stack([1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)], -1),
+                     np.stack([2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)], -1),
+                     np.stack([2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)], -1)], -2)
+
+
+def synthetic_skinning(ch: Character, vertices_per_joint: int, seed: int = 0) -> Skinning:
+    """A seeded mesh around the bones of ``ch`` at theta = 0: each joint gets ``vertices_per_joint`` vertices scattered around the
+    segment from its parent to it (a blob for a root). Weights fall off with the distance to the joint, its parent and its children and
+    are normalised; the smallest are dropped so that a vertex keeps 1 to 8 influences, largest first. The inverse bind pose is the
+    inverse of the rest-pose world transform, as momentum builds it."""
+    rng = np.random.default_rng(seed)
+    J = ch.num_joints
+    t, q, s = forward_kinematics(ch, np.zeros((1, ch.num_params)))
+    t, q, s = t[0], q[0], s[0]
+    children = [[] for _ in range(J)]
+    for j, p in enumerate(ch.parents):
+        if p >= 0:
+            children[p].append(j)
+    verts, index, weight = [], [], []
+    for j in range(J):
+        p = int(ch.parents[j])
+        start = t[p] if p >= 0 else t[j]
+        length = float(np.linalg.norm(t[j] - start))
+        radius = 0.2 * length + 1.0
+        u = rng.uniform(0.0, 1.0, (vertices_per_joint, 1))
+        d = rng.normal(size=(vertices_per_joint, 3))
+        d *= (radius * rng.uniform(0.5, 1.0, (vertices_per_joint, 1))) / np.linalg.norm(d, axis=1, keepdims=True)
+        x = start + u * (t[j] - start) + d
+        cand = ([p] if p >= 0 else []) + [j] + children[j]
+        if p >= 0 and ch.parents[p] >= 0 and len(cand) < MAX_SKIN_JOINTS:
+            cand.append(int(ch.parents[p]))
+        cand = np.array(cand[:MAX_SKIN_JOINTS])
+        dist = np.linalg.norm(x[:, None, :] - t[cand][None], axis=-1)
+        w = np.exp(-(dist / (0.5 * length + 2.0)) ** 2) + 1e-12
+        w /= w.sum(1, keepdims=True)
+        w[w < rng.uniform(0.02, 0.3, (vertices_per_joint, 1))] = 0.0  # 1 to len(cand) influences per vertex
+        w[np.arange(vertices_per_joint), w.argmax(1)] = np.maximum(w.max(1), 1e-3)
+        order = np.argsort(-w, axis=1, kind="stable")
+        wi = np.zeros((vertices_per_joint, MAX_SKIN_JOINTS))
+        ii = np.zeros((vertices_per_joint, MAX_SKIN_JOINTS), np.int32)
+        wi[:, :len(cand)] = np.take_along_axis(w, order, 1)
+        ii[:, :len(cand)] = cand[order]
+        wi /= wi.sum(1, keepdims=True)
+        ii[wi == 0.0] = 0
+        verts.append(x); index.append(ii); weight.append(wi)
+    R = _quat_matrix(q)
+    Rt = np.swapaxes(R, -1, -2) / s[:, None, None]
+    ibp = np.concatenate([Rt, -(Rt @ t[:, :, None])], -1)
+    return Skinning(np.concatenate(verts).astype(np.float32), np.concatenate(index).astype(np.int32), np.concatenate(weight).astype(np.float32),
+                    ibp.astype(np.float32))
+
+
+def skin_points(ch: Character, skel_state, rest_points=None):
+    """Linear-blend skinning in float64 (applySSD, linear_skinning.cpp:40-102, with q normalised): skel_state [B,J,8] or [J,8]
+    (t, q xyzw, s) -> points [B,V,3] or [V,3]. rest_points: None = the rest mesh, [V,3] shared or [B,V,3]."""
+    sk = ch.skinning
+    st = np.asarray(skel_state, np.float64)
+    single = st.ndim == 2
+    st = st.reshape(-1, ch.num_joints, 8)
+    x = np.asarray(sk.rest_vertices if rest_points is None else rest_points, np.float64)
+    x = np.broadcast_to(x, (st.shape[0],) + x.shape[-2:])
+    qn = st[..., 3:7] / np.linalg.norm(st[..., 3:7], axis=-1, keepdims=True)
+    sR = _quat_matrix(qn) * st[..., 7, None, None]
+    ibp = np.asarray(sk.inverse_bind_pose, np.float64)
+    L = sR @ ibp[None, :, :, :3]
+    c = (sR @ ibp[None, :, :, 3:])[..., 0] + st[..., :3]
+    w = np.asarray(sk.skin_weight, np.float64)
+    active = np.cumprod(w != 0.0, axis=1).astype(bool)
+    out = np.zeros_like(x)
+    for k in range(MAX_SKIN_JOINTS):
+        j = np.where(active[:, k], sk.skin_index[:, k], 0)
+        wk = np.where(active[:, k], w[:, k], 0.0)
+        out += (np.einsum("bvrc,bvc->bvr", L[:, j], x) + c[:, j]) * wk[None, :, None]
+    return out[0] if single else out
 
 
 def world_rotations(ch: Character, theta, parents, offsets_q):

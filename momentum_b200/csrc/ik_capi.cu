@@ -98,6 +98,12 @@ struct NvtxRange {
 
 } // namespace
 
+// the device copy of a HostSkinning (SkinTables)
+struct SkinBuffers {
+  DeviceBuffer<float> rest, vertWeight, ibp, infWeight;
+  DeviceBuffer<int32_t> vertStart, vertJoint, infVertex, segStart, segJoint, jointSegStart;
+};
+
 struct mb2_character {
   int device{0};
   HostCharacter host;
@@ -106,6 +112,9 @@ struct mb2_character {
   DeviceBuffer<int32_t> childStart, children, ptColStart, ptColRows; // skeleton-state backward (HostCharacter::buildBackwardTables)
   DeviceBuffer<float> ptColVals;
   uint64_t limitsVersion{0};
+  // linear-blend skinning (mb2_character_set_skinning): numVertices == 0 when there is none
+  HostSkinning skin;
+  std::unique_ptr<SkinBuffers> skinDev; // replaced whole by mb2_character_set_skinning, never rewritten in place
 };
 
 struct DeviceSchedule {
@@ -608,9 +617,49 @@ int mb2_character_clone(const mb2_character* c, int device, mb2_character** out)
   if (rc != MB2_OK) return rc;
   copy->host.limits = h.limits;
   copy->limitsVersion = 1;
+  const HostSkinning& s = c->skin;
+  if (s.numVertices > 0) { // back to [V][8] slots: the active ones, then zero weights
+    std::vector<int32_t> index(size_t(s.numVertices) * kSkinMaxInfluences, 0);
+    std::vector<float> weight(index.size(), 0.f);
+    for (int v = 0; v < s.numVertices; ++v)
+      for (int k = s.vertStart[v]; k < s.vertStart[v + 1]; ++k) {
+        index[size_t(v) * kSkinMaxInfluences + (k - s.vertStart[v])] = s.vertJoint[k];
+        weight[size_t(v) * kSkinMaxInfluences + (k - s.vertStart[v])] = s.vertWeight[k];
+      }
+    rc = mb2_character_set_skinning(copy, s.numVertices, s.restVertices.data(), index.data(), weight.data(), s.inverseBindPose.data());
+    if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
+  }
   *out = copy;
   return MB2_OK;
 }
+
+int mb2_character_set_skinning(mb2_character* c, int32_t num_vertices, const float* rest_vertices, const int32_t* skin_index, const float* skin_weight,
+                               const float* inverse_bind_pose) {
+  MB2_CHECK(c != nullptr, "null character");
+  HostSkinning s;
+  const std::string err = makeSkinning(c->host, num_vertices, rest_vertices, skin_index, skin_weight, inverse_bind_pose, s);
+  if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
+  MB2_DEVICE_GUARD(c->device);
+  // fresh buffers: a failed upload leaves the earlier skinning whole; the device is synchronised before the swap, so no work in flight
+  // on any stream still reads the tables that are freed
+  auto d = std::make_unique<SkinBuffers>();
+  MB2_CUDA(d->rest.upload(s.restVertices, nullptr));
+  MB2_CUDA(d->vertStart.upload(s.vertStart, nullptr));
+  MB2_CUDA(d->vertJoint.upload(s.vertJoint, nullptr));
+  MB2_CUDA(d->vertWeight.upload(s.vertWeight, nullptr));
+  MB2_CUDA(d->ibp.upload(s.inverseBindPose, nullptr));
+  MB2_CUDA(d->infVertex.upload(s.infVertex, nullptr));
+  MB2_CUDA(d->infWeight.upload(s.infWeight, nullptr));
+  MB2_CUDA(d->segStart.upload(s.segStart, nullptr));
+  MB2_CUDA(d->segJoint.upload(s.segJoint, nullptr));
+  MB2_CUDA(d->jointSegStart.upload(s.jointSegStart, nullptr));
+  MB2_CUDA(cudaDeviceSynchronize());
+  c->skinDev = std::move(d);
+  c->skin = std::move(s);
+  return MB2_OK;
+}
+
+int32_t mb2_character_num_vertices(const mb2_character* c) { return c ? c->skin.numVertices : 0; }
 // The DEFINITION of a solver function (error-function blocks with their shared constraint data and weights, block weights, enabled
 // parameters) for `batch` instances of character `c` (normally a clone of f's character on another device). Per-instance data
 // (targets, per-instance weights / offsets) is not copied: it belongs to the instances the new function will hold.
@@ -940,6 +989,75 @@ int mb2_character_skeleton_state_device(const mb2_character* c, int32_t batch, c
 int mb2_character_skeleton_state_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
                                                  const float* grad_skeleton_state_device, float* grad_model_parameters_device, void* cuda_stream) {
   return skeletonStateDevice(c, batch, model_parameters_device, grad_skeleton_state_device, grad_model_parameters_device, cuda_stream, true);
+}
+
+namespace {
+// both directions of mb2_character_skin_points*_device: checks the arguments and fills the kernel arguments except the outputs
+int skinArgs(const mb2_character* c, int32_t batch, const float* skelState, const float* restPoints, int32_t restBatched, SkinArgs& a) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(c->skin.numVertices > 0, "skin points: the character has no skinning (mb2_character_set_skinning)");
+  MB2_CHECK(batch >= 0, "batch must not be negative");
+  MB2_CHECK(batch == 0 || restPoints != nullptr || restBatched == 0, "skin points: batched rest points need a rest_points array");
+  a = SkinArgs{};
+  const HostSkinning& s = c->skin;
+  a.S.numVertices = s.numVertices;
+  a.S.numSegments = s.numSegments();
+  a.S.restVertices = c->skinDev->rest.p;
+  a.S.vertStart = c->skinDev->vertStart.p;
+  a.S.vertJoint = c->skinDev->vertJoint.p;
+  a.S.vertWeight = c->skinDev->vertWeight.p;
+  a.S.inverseBindPose = c->skinDev->ibp.p;
+  a.S.infVertex = c->skinDev->infVertex.p;
+  a.S.infWeight = c->skinDev->infWeight.p;
+  a.S.segStart = c->skinDev->segStart.p;
+  a.S.segJoint = c->skinDev->segJoint.p;
+  a.S.jointSegStart = c->skinDev->jointSegStart.p;
+  a.numJoints = c->host.numJoints;
+  a.batch = batch;
+  a.skelState = skelState;
+  a.restPoints = restPoints != nullptr ? restPoints : c->skinDev->rest.p;
+  a.restBatched = restBatched != 0;
+  return MB2_OK;
+}
+} // namespace
+
+int mb2_character_skin_points_device(const mb2_character* c, int32_t batch, const float* skel_state_device, const float* rest_points_device,
+                                     int32_t rest_points_batched, float* points_device, void* cuda_stream) {
+  SkinArgs a;
+  int rc = skinArgs(c, batch, skel_state_device, rest_points_device, rest_points_batched, a);
+  if (rc != MB2_OK || batch == 0) return rc;
+  MB2_CHECK(skel_state_device != nullptr && points_device != nullptr, "null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(isDeviceMemoryOn(skel_state_device, c->device) && isDeviceMemoryOn(points_device, c->device) &&
+                (rest_points_device == nullptr || isDeviceMemoryOn(rest_points_device, c->device)),
+            "skin points: every array must be device memory on the character's device");
+  NvtxRange range("skinPoints");
+  a.points = points_device;
+  MB2_CUDA(launchSkinPoints(a, (cudaStream_t)cuda_stream));
+  return MB2_OK;
+}
+
+int mb2_character_skin_points_backward_device(const mb2_character* c, int32_t batch, const float* skel_state_device, const float* rest_points_device,
+                                              int32_t rest_points_batched, const float* grad_points_device, float* grad_skel_state_device,
+                                              float* grad_rest_points_device, void* cuda_stream) {
+  SkinArgs a;
+  int rc = skinArgs(c, batch, skel_state_device, rest_points_device, rest_points_batched, a);
+  if (rc != MB2_OK) return rc;
+  MB2_CHECK(rest_points_device != nullptr || grad_rest_points_device == nullptr,
+            "skin points: grad_rest_points must be null when the character's rest mesh is skinned");
+  if (batch == 0) return MB2_OK;
+  MB2_CHECK(skel_state_device != nullptr && grad_points_device != nullptr, "null argument");
+  MB2_DEVICE_GUARD(c->device);
+  bool onDevice = isDeviceMemoryOn(skel_state_device, c->device) && isDeviceMemoryOn(grad_points_device, c->device) &&
+                  (rest_points_device == nullptr || isDeviceMemoryOn(rest_points_device, c->device));
+  for (float* o : {grad_skel_state_device, grad_rest_points_device}) onDevice = onDevice && (o == nullptr || isDeviceMemoryOn(o, c->device));
+  MB2_CHECK(onDevice, "skin points: every array must be device memory on the character's device");
+  NvtxRange range("skinPointsBackward");
+  a.gradPoints = grad_points_device;
+  a.gradState = grad_skel_state_device;
+  a.gradRest = grad_rest_points_device;
+  MB2_CUDA(launchSkinPointsBackward(a, (cudaStream_t)cuda_stream));
+  return MB2_OK;
 }
 
 int mb2_solver_function_input_gradients_device(mb2_solver_function* f, int32_t index, const float* parameters_device, const float* direction_device,

@@ -823,4 +823,80 @@ MB2_HD void jacobianCell(const FunctionTables& T, int ci, const float* js, const
 #undef MB2_ROW
 }
 
+// ---- Linear-blend skinning (linear_skinning.cpp:22-102) and its backward -------------------------------------------------------------
+// M_j = T_j o IBP_j with T_j(y) = t + s R(q^) y (q^ = q / |q|, as pymomentum's skel-state backend normalises) and IBP_j = [N | c];
+// p_i = sum_k w_ik M_{j_ik}(x_i). m: row-major 3x4, m[4 r + 3] the translation.
+MB2_HD void skinTransform(const float* state, const float* ibp, float* m) {
+  const Q4 q = qnormalized(ld4(state + 3));
+  const float s = state[7];
+  float R[9];
+  qmat(q, R);
+  for (int r = 0; r < 3; ++r) {
+    const F3 sr = f3(s * R[r], s * R[3 + r], s * R[6 + r]); // row r of s R
+    m[4 * r + 0] = dot(sr, f3(ibp[0], ibp[4], ibp[8]));
+    m[4 * r + 1] = dot(sr, f3(ibp[1], ibp[5], ibp[9]));
+    m[4 * r + 2] = dot(sr, f3(ibp[2], ibp[6], ibp[10]));
+    m[4 * r + 3] = dot(sr, f3(ibp[3], ibp[7], ibp[11])) + state[r];
+  }
+}
+// one vertex: sum over its active slots of w (t + L x), slots in order (linear_skinning.cpp:84-90); M: [J][12]
+MB2_HD F3 skinBlend(const SkinTables& S, const float* M, int v, F3 x) {
+  F3 p = f3(0.f, 0.f, 0.f);
+  for (int k = S.vertStart[v]; k < S.vertStart[v + 1]; ++k) {
+    const float* m = M + S.vertJoint[k] * kSkinIbpStride;
+    const F3 temp = f3(m[3] + dot(ld3(m), x), m[7] + dot(ld3(m + 4), x), m[11] + dot(ld3(m + 8), x));
+    p = p + temp * S.vertWeight[k];
+  }
+  return p;
+}
+// Backward, with g_i = dL/dp_i and the bone-local point y_ij = N_j x_i + c_j, per joint: a_j = sum w g_i (12 floats: a, then
+// E_j = sum w g_i y_ij^T row-major). E is summed from the bone-local y: the expanded form (sum w g x^T) N^T + a c^T cancels
+// catastrophically for a mesh far from the origin.
+constexpr int kSkinAccFloats = 12;
+MB2_HD void skinAccumulate(const float* ibp, F3 x, F3 g, float w, float* acc) {
+  const F3 y = f3(dot(ld3(ibp), x) + ibp[3], dot(ld3(ibp + 4), x) + ibp[7], dot(ld3(ibp + 8), x) + ibp[11]);
+  const F3 wg = g * w;
+  acc[0] += wg.x; acc[1] += wg.y; acc[2] += wg.z;
+  acc[3] += wg.x * y.x; acc[4] += wg.x * y.y; acc[5] += wg.x * y.z;
+  acc[6] += wg.y * y.x; acc[7] += wg.y * y.y; acc[8] += wg.y * y.z;
+  acc[9] += wg.z * y.x; acc[10] += wg.z * y.y; acc[11] += wg.z * y.z;
+}
+// (a_j, E_j) and the joint's state -> dL/d(t, q xyzw, s): dt = a, ds = <E, R(q^)>, dq^ = s d<E, R(q^)>/dq^ through the
+// normalisation Jacobian (I - q^ q^T) / |q|
+MB2_HD void skinStateGradient(const float* acc, const float* state, float* out) {
+  const Q4 q = ld4(state + 3);
+  const float nq = sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
+  const Q4 u = q4(q.x / nq, q.y / nq, q.z / nq, q.w / nq);
+  const float s = state[7];
+  const float* E = acc + 3; // E[3 r + c]
+  float R[9];
+  qmat(u, R); // R[3 c + r]
+  float ds = 0.f;
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) ds += E[3 * r + c] * R[3 * c + r];
+  // d<E, R(u)>/du for Eigen's toRotationMatrix polynomial
+  const float s01 = E[1] + E[3], s02 = E[2] + E[6], s12 = E[5] + E[7];
+  const float d21 = E[7] - E[5], d02 = E[2] - E[6], d10 = E[3] - E[1];
+  const float gx = 2.f * (u.y * s01 + u.z * s02 + u.w * d21 - 2.f * u.x * (E[4] + E[8]));
+  const float gy = 2.f * (u.x * s01 + u.z * s12 + u.w * d02 - 2.f * u.y * (E[0] + E[8]));
+  const float gz = 2.f * (u.x * s02 + u.y * s12 + u.w * d10 - 2.f * u.z * (E[0] + E[4]));
+  const float gw = 2.f * (u.x * d21 + u.y * d02 + u.z * d10);
+  const Q4 gu = q4(s * gx, s * gy, s * gz, s * gw);
+  const float along = u.x * gu.x + u.y * gu.y + u.z * gu.z + u.w * gu.w;
+  out[0] = acc[0]; out[1] = acc[1]; out[2] = acc[2];
+  out[3] = (gu.x - u.x * along) / nq; out[4] = (gu.y - u.y * along) / nq;
+  out[5] = (gu.z - u.z * along) / nq; out[6] = (gu.w - u.w * along) / nq;
+  out[7] = ds;
+}
+// dL/dx_i = sum over the vertex's slots of w L_j^T g_i, slots in order
+MB2_HD F3 skinRestGradient(const SkinTables& S, const float* M, int v, F3 g) {
+  F3 r = f3(0.f, 0.f, 0.f);
+  for (int k = S.vertStart[v]; k < S.vertStart[v + 1]; ++k) {
+    const float* m = M + S.vertJoint[k] * kSkinIbpStride;
+    const F3 lt = f3(m[0] * g.x + m[4] * g.y + m[8] * g.z, m[1] * g.x + m[5] * g.y + m[9] * g.z, m[2] * g.x + m[6] * g.y + m[10] * g.z);
+    r = r + lt * S.vertWeight[k];
+  }
+  return r;
+}
+
 } // namespace mb2

@@ -382,6 +382,216 @@ cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaS
 }
 
 // ------------------------------------------------------------------------------------------------
+// Linear-blend skinning of a batch (ik_device.cuh skin*), three kernels. The skin tables are shared by the batch and stay in L2.
+//   skinVertexKernel<kMode>  a persistent grid of work items (instances, vertex range): per instance the CTA writes the J skinning
+//                            transforms M_j = T_j o IBP_j to shared memory, then lanes = vertices blend. kMode 0: points [B][V][3];
+//                            1: rest-point gradient per instance; 2: rest-point gradient summed over a fixed chunk of instances, in
+//                            instance order, into one row of bounded scratch (the chunks are summed in order by skinChunkSumKernel).
+//   skinStatePartialKernel   one warp per (instance, segment of a joint's influence list): lanes = influences, then a butterfly sum
+//                            of the 12 floats (a_j, E_j) to scratch.
+//   skinStateFinishKernel    lanes = (instance, joint): the joint's segments summed in order, then skinStateGradient.
+// No atomics: every output element is summed in a fixed order that depends on neither the batch size nor the launch shape.
+// ------------------------------------------------------------------------------------------------
+constexpr int kSkinThreads = 256;
+constexpr int kSkinVertsPerThread = 4;                              // kMode 2 keeps their sums in registers
+constexpr int kSkinChunkVerts = kSkinThreads * kSkinVertsPerThread; // vertex range of a kMode 2 work item
+constexpr int kSkinMaxBatchChunks = 128;                            // kMode 2 scratch: at most 128 x [V][3] floats
+constexpr size_t kSkinPartialBudget = size_t(256) << 20;            // skel-state backward scratch: instances processed in slices
+
+template <int kMode>
+__global__ void __launch_bounds__(kSkinThreads) skinVertexKernel(const SkinArgs a, int perChunk, int numChunks, int vSplit, int vLen, float* out) {
+  extern __shared__ __align__(16) float M[]; // [J][12]
+  const SkinTables S = a.S;
+  const int V = S.numVertices, J = a.numJoints;
+  const long items = long(numChunks) * vSplit;
+  for (long it = blockIdx.x; it < items; it += gridDim.x) {
+    const int c = int(it / vSplit), v0 = int(it % vSplit) * vLen, v1 = min(V, v0 + vLen);
+    F3 acc[kSkinVertsPerThread];
+#pragma unroll
+    for (int k = 0; k < kSkinVertsPerThread; ++k) acc[k] = f3(0.f, 0.f, 0.f);
+    const int b1 = min(a.batch, (c + 1) * perChunk);
+    for (int b = c * perChunk; b < b1; ++b) {
+      __syncthreads(); // the previous instance's readers of M are done
+      for (int j = threadIdx.x; j < J; j += blockDim.x)
+        skinTransform(a.skelState + (size_t(b) * J + j) * 8, S.inverseBindPose + j * kSkinIbpStride, M + j * kSkinIbpStride);
+      __syncthreads();
+      const float* x = a.restPoints + (a.restBatched ? size_t(b) * V * 3 : 0);
+      const size_t row = size_t(b) * V * 3;
+      if constexpr (kMode == 0) {
+        for (int v = v0 + threadIdx.x; v < v1; v += blockDim.x) {
+          const F3 p = skinBlend(S, M, v, ld3(x + 3 * v));
+          float* o = a.points + row + 3 * size_t(v);
+          o[0] = p.x; o[1] = p.y; o[2] = p.z;
+        }
+      } else if constexpr (kMode == 1) {
+        for (int v = v0 + threadIdx.x; v < v1; v += blockDim.x) {
+          const F3 r = skinRestGradient(S, M, v, ld3(a.gradPoints + row + 3 * size_t(v)));
+          float* o = out + row + 3 * size_t(v);
+          o[0] = r.x; o[1] = r.y; o[2] = r.z;
+        }
+      } else {
+#pragma unroll
+        for (int k = 0; k < kSkinVertsPerThread; ++k) {
+          const int v = v0 + threadIdx.x + k * kSkinThreads;
+          if (v < v1) acc[k] = acc[k] + skinRestGradient(S, M, v, ld3(a.gradPoints + row + 3 * size_t(v)));
+        }
+      }
+    }
+    if constexpr (kMode == 2) {
+#pragma unroll
+      for (int k = 0; k < kSkinVertsPerThread; ++k) {
+        const int v = v0 + threadIdx.x + k * kSkinThreads;
+        if (v < v1) {
+          float* o = out + size_t(c) * V * 3 + 3 * size_t(v);
+          o[0] = acc[k].x; o[1] = acc[k].y; o[2] = acc[k].z;
+        }
+      }
+    }
+  }
+}
+
+__global__ void skinChunkSumKernel(const float* partial, int numChunks, size_t n, float* out) {
+  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
+    float s = partial[i];
+    for (int c = 1; c < numChunks; ++c) s += partial[size_t(c) * n + i];
+    out[i] = s;
+  }
+}
+
+__global__ void __launch_bounds__(kSkinThreads) skinStatePartialKernel(const SkinArgs a, int b0, int nb, float* partial) {
+  const SkinTables S = a.S;
+  const int lane = threadIdx.x & 31, V = S.numVertices, numSeg = S.numSegments;
+  const long warps = long(gridDim.x) * (blockDim.x >> 5);
+  for (long it = long(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); it < long(nb) * numSeg; it += warps) {
+    const int b = b0 + int(it / numSeg), s = int(it % numSeg);
+    const float* ibp = S.inverseBindPose + S.segJoint[s] * kSkinIbpStride;
+    const float* x = a.restPoints + (a.restBatched ? size_t(b) * V * 3 : 0);
+    const float* g = a.gradPoints + size_t(b) * V * 3;
+    float acc[kSkinAccFloats];
+#pragma unroll
+    for (int r = 0; r < kSkinAccFloats; ++r) acc[r] = 0.f;
+    for (int k = S.segStart[s] + lane; k < S.segStart[s + 1]; k += 32) {
+      const int v = S.infVertex[k];
+      skinAccumulate(ibp, ld3(x + 3 * v), ld3(g + 3 * v), S.infWeight[k], acc);
+    }
+    float mine = 0.f;
+#pragma unroll
+    for (int r = 0; r < kSkinAccFloats; ++r) {
+      float t = acc[r];
+      for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o); // every lane ends with the same bits
+      if (lane == r) mine = t;
+    }
+    if (lane < kSkinAccFloats) partial[size_t(it) * kSkinAccFloats + lane] = mine;
+  }
+}
+
+__global__ void skinStateFinishKernel(const SkinArgs a, int b0, int nb, const float* partial) {
+  const SkinTables S = a.S;
+  const int J = a.numJoints;
+  for (long it = long(blockIdx.x) * blockDim.x + threadIdx.x; it < long(nb) * J; it += long(gridDim.x) * blockDim.x) {
+    const int bl = int(it / J), j = int(it % J);
+    float acc[kSkinAccFloats];
+#pragma unroll
+    for (int r = 0; r < kSkinAccFloats; ++r) acc[r] = 0.f;
+    for (int s = S.jointSegStart[j]; s < S.jointSegStart[j + 1]; ++s) {
+      const float* p = partial + (size_t(bl) * S.numSegments + s) * kSkinAccFloats;
+#pragma unroll
+      for (int r = 0; r < kSkinAccFloats; ++r) acc[r] += p[r];
+    }
+    const size_t at = (size_t(b0 + bl) * J + j) * 8;
+    skinStateGradient(acc, a.skelState + at, a.gradState + at);
+  }
+}
+
+namespace {
+// Grid of a persistent skin kernel: what the SMs hold at once, capped by the work.
+template <class K>
+cudaError_t skinGrid(K kernel, size_t smem, long work, int* grid) {
+  if (smem > size_t(g_maxSmemOptin)) return cudaErrorInvalidConfiguration;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (e != cudaSuccess) return e;
+  int perSm = 0;
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kernel, kSkinThreads, smem);
+  if (e != cudaSuccess) return e;
+  *grid = int(std::max(1L, std::min(long(std::max(g_numSms, 1)) * std::max(perSm, 1), work)));
+  return cudaSuccess;
+}
+
+// kMode 0 / 1: one work item per instance when the batch fills the grid, else each instance's vertices split over several
+template <int kMode>
+cudaError_t launchSkinPerInstance(const SkinArgs& a, float* out, cudaStream_t stream) {
+  const size_t smem = size_t(a.numJoints) * kSkinIbpStride * sizeof(float);
+  const int V = a.S.numVertices;
+  int slots = 0;
+  cudaError_t e = skinGrid(skinVertexKernel<kMode>, smem, 1L << 30, &slots);
+  if (e != cudaSuccess) return e;
+  const int vSplit = a.batch >= slots ? 1 : std::min((slots + a.batch - 1) / a.batch, (V + kSkinThreads - 1) / kSkinThreads);
+  const int vLen = (V + vSplit - 1) / vSplit;
+  const int grid = int(std::min(long(slots), long(a.batch) * vSplit));
+  skinVertexKernel<kMode><<<grid, kSkinThreads, smem, stream>>>(a, 1, a.batch, vSplit, vLen, out);
+  return cudaGetLastError();
+}
+} // namespace
+
+cudaError_t launchSkinPoints(const SkinArgs& a, cudaStream_t stream) {
+  if (a.batch <= 0) return cudaSuccess;
+  return launchSkinPerInstance<0>(a, nullptr, stream);
+}
+
+cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream) {
+  if (a.batch <= 0) return cudaSuccess;
+  const int V = a.S.numVertices, J = a.numJoints;
+  cudaError_t e = cudaSuccess;
+  if (a.gradState != nullptr && a.S.numSegments == 0) { // no influences at all: the gradient is zero
+    e = cudaMemsetAsync(a.gradState, 0, size_t(a.batch) * J * 8 * sizeof(float), stream);
+  } else if (a.gradState != nullptr) {
+    const size_t perInstance = size_t(a.S.numSegments) * kSkinAccFloats * sizeof(float);
+    const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(a.batch), kSkinPartialBudget / perInstance)));
+    float* partial = nullptr;
+    e = cudaMallocAsync(reinterpret_cast<void**>(&partial), perInstance * slice, stream);
+    if (e != cudaSuccess) return e;
+    int g1 = 0, g2 = 0;
+    e = skinGrid(skinStatePartialKernel, 0, (long(slice) * a.S.numSegments + 7) / 8, &g1);
+    if (e == cudaSuccess) e = skinGrid(skinStateFinishKernel, 0, (long(slice) * J + kSkinThreads - 1) / kSkinThreads, &g2);
+    for (int b0 = 0; e == cudaSuccess && b0 < a.batch; b0 += slice) {
+      const int nb = std::min(slice, a.batch - b0);
+      skinStatePartialKernel<<<g1, kSkinThreads, 0, stream>>>(a, b0, nb, partial);
+      skinStateFinishKernel<<<g2, kSkinThreads, 0, stream>>>(a, b0, nb, partial);
+      e = cudaGetLastError();
+    }
+    const cudaError_t f = cudaFreeAsync(partial, stream);
+    if (e == cudaSuccess) e = f;
+  }
+  if (e != cudaSuccess || a.gradRest == nullptr) return e;
+  if (a.restBatched) return launchSkinPerInstance<1>(a, a.gradRest, stream);
+  // shared rest points: the batch sum over fixed chunks of instances (the chunking depends on the batch size only)
+  const int perChunk = std::max(8, (a.batch + kSkinMaxBatchChunks - 1) / kSkinMaxBatchChunks);
+  const int numChunks = (a.batch + perChunk - 1) / perChunk;
+  const int vSplit = (V + kSkinChunkVerts - 1) / kSkinChunkVerts;
+  const size_t n = size_t(V) * 3, smem = size_t(J) * kSkinIbpStride * sizeof(float);
+  float* partial = a.gradRest;
+  if (numChunks > 1) {
+    e = cudaMallocAsync(reinterpret_cast<void**>(&partial), n * numChunks * sizeof(float), stream);
+    if (e != cudaSuccess) return e;
+  }
+  int grid = 0;
+  e = skinGrid(skinVertexKernel<2>, smem, long(numChunks) * vSplit, &grid);
+  if (e == cudaSuccess) {
+    skinVertexKernel<2><<<grid, kSkinThreads, smem, stream>>>(a, perChunk, numChunks, vSplit, kSkinChunkVerts, partial);
+    e = cudaGetLastError();
+  }
+  if (numChunks > 1) {
+    if (e == cudaSuccess) {
+      skinChunkSumKernel<<<unsigned(std::min<size_t>((n + kSkinThreads - 1) / kSkinThreads, 4096)), kSkinThreads, 0, stream>>>(partial, numChunks, n, a.gradRest);
+      e = cudaGetLastError();
+    }
+    const cudaError_t f = cudaFreeAsync(partial, stream);
+    if (e == cudaSuccess) e = f;
+  }
+  return e;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Input gradients of one Position / Orientation block, d/d input [grad_theta E . v] (ik_device.cuh tangent* / *InputGradient): laid out
 // like skeletonStateKernel, a persistent grid with one group of W warps per instance and the character tables in shared memory.
 //   lanes = parameters: theta, and v gated by the enabled set;  lanes = joints: FK with the DOF axes;  lanes = joints: each joint's own

@@ -153,6 +153,22 @@ struct SkeletonStateArgs {
   float* out;                // forward: [B][J][8] (t, q xyzw, s); backward: [B][n] dLoss / d theta, overwritten
 };
 cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream);
+// skinVertexKernel / skinStatePartialKernel / skinStateFinishKernel: linear-blend skinning of a batch (applySSD) and its backward
+struct SkinArgs {
+  SkinTables S;
+  int32_t numJoints;
+  int32_t batch;
+  const float* skelState;    // [B][J][8] (t, q xyzw, s)
+  const float* restPoints;   // [V][3] shared or [B][V][3]
+  int32_t restBatched;
+  const float* gradPoints;   // backward: [B][V][3] dLoss / d points
+  float* points;             // forward: [B][V][3]
+  float* gradState;          // backward, optional: [B][J][8]
+  float* gradRest;           // backward, optional: [B][V][3] when batched, else [V][3] (the batch sum)
+};
+// Both enqueue on `stream`; the backward takes bounded stream-ordered scratch (cudaMallocAsync) for its partial sums.
+cudaError_t launchSkinPoints(const SkinArgs& a, cudaStream_t stream);
+cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream);
 // inputGradientKernel: d/d input [grad_theta E . v] of one Position or Orientation (matrix difference) block with the L2 loss, per
 // instance: the input contraction of solve_ik's implicit-function backward
 struct InputGradientArgs {

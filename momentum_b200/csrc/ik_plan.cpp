@@ -125,6 +125,57 @@ std::string makeCharacter(int32_t numJoints, const int32_t* parents, const float
   return "";
 }
 
+std::string makeSkinning(const HostCharacter& ch, int32_t numVertices, const float* restVertices, const int32_t* skinIndex, const float* skinWeight,
+                         const float* inverseBindPose, HostSkinning& out) {
+  if (!(restVertices && skinIndex && skinWeight && inverseBindPose)) return "skinning: null argument";
+  if (numVertices < 1) return "skinning: the mesh must have at least one vertex";
+  const int J = ch.numJoints, V = numVertices;
+  for (size_t k = 0; k < size_t(V) * 3; ++k)
+    if (!std::isfinite(restVertices[k])) return "skinning: rest vertices must be finite";
+  for (size_t k = 0; k < size_t(J) * kSkinIbpStride; ++k)
+    if (!std::isfinite(inverseBindPose[k])) return "skinning: inverse bind poses must be finite";
+  HostSkinning s;
+  s.numVertices = V;
+  s.restVertices.assign(restVertices, restVertices + size_t(V) * 3);
+  s.inverseBindPose.assign(inverseBindPose, inverseBindPose + size_t(J) * kSkinIbpStride);
+  s.vertStart.assign(V + 1, 0);
+  for (int v = 0; v < V; ++v) {
+    for (int k = 0; k < kSkinMaxInfluences; ++k) {
+      const size_t at = size_t(v) * kSkinMaxInfluences + k;
+      if (skinWeight[at] == 0.f) break; // linear_skinning.cpp:76-80: the slots after it are not read, whatever they hold
+      if (!std::isfinite(skinWeight[at])) return "skinning: skin weights must be finite";
+      if (skinIndex[at] < 0 || skinIndex[at] >= J) return "skinning: skin index out of range [0, numJoints)";
+      s.vertJoint.push_back(skinIndex[at]);
+      s.vertWeight.push_back(skinWeight[at]);
+    }
+    s.vertStart[v + 1] = int32_t(s.vertJoint.size());
+  }
+  // by joint: a counting sort over ascending vertices keeps each joint's list in vertex (then slot) order
+  s.jointStart.assign(J + 1, 0);
+  for (int j : s.vertJoint) s.jointStart[j + 1]++;
+  for (int j = 0; j < J; ++j) s.jointStart[j + 1] += s.jointStart[j];
+  s.infVertex.resize(s.vertJoint.size());
+  s.infWeight.resize(s.vertJoint.size());
+  std::vector<int32_t> cursor(s.jointStart.begin(), s.jointStart.end() - 1);
+  for (int v = 0; v < V; ++v)
+    for (int k = s.vertStart[v]; k < s.vertStart[v + 1]; ++k) {
+      const int at = cursor[s.vertJoint[k]]++;
+      s.infVertex[at] = v;
+      s.infWeight[at] = s.vertWeight[k];
+    }
+  s.jointSegStart.assign(J + 1, 0);
+  for (int j = 0; j < J; ++j) {
+    for (int b = s.jointStart[j]; b < s.jointStart[j + 1]; b += kSkinSegment) {
+      s.segStart.push_back(b);
+      s.segJoint.push_back(j);
+    }
+    s.jointSegStart[j + 1] = int32_t(s.segJoint.size());
+  }
+  s.segStart.push_back(s.jointStart[J]);
+  out = std::move(s);
+  return "";
+}
+
 std::string setParameterLimits(HostCharacter& ch, int32_t count, const mb2_parameter_limit* limits) {
   if (!(count >= 0 && (count == 0 || limits))) return "invalid limits";
   ch.limits.clear();

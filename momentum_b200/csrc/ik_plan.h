@@ -45,6 +45,21 @@ struct HostCharacter {
   std::vector<uint8_t> computeActiveJointParams(const std::vector<uint8_t>& enabled) const;
 };
 
+// Linear-blend skinning of a character (SkinWeights + Character::inverseBindPose, skin_weights.h:19-40, character.h), flattened into
+// the tables of SkinTables (ik_types.h). Built and validated by makeSkinning only.
+struct HostSkinning {
+  int32_t numVertices{0};
+  std::vector<float> restVertices;             // [V][3]
+  std::vector<int32_t> vertStart, vertJoint;   // by vertex, active slots only
+  std::vector<float> vertWeight;
+  std::vector<float> inverseBindPose;          // [J][12]
+  std::vector<int32_t> jointStart, infVertex;  // by joint, vertices ascending
+  std::vector<float> infWeight;
+  std::vector<int32_t> segStart, segJoint, jointSegStart;
+  int32_t numInfluences() const { return int32_t(vertJoint.size()); }
+  int32_t numSegments() const { return int32_t(segJoint.size()); }
+};
+
 struct HostErrorFunction {
   int32_t kind{0}; // 0 position, 1 orientation, 2 orientation rot-diff, 3 state, 4 limit, 5 plane, 6 model parameters
   float weight{1.f};
@@ -86,6 +101,10 @@ struct HostFunction {
 std::string makeCharacter(int32_t numJoints, const int32_t* parents, const float* offsets, const float* prerot, int32_t numParams, const int32_t* outer,
                           const int32_t* inner, const float* vals, const float* ptOffsets, HostCharacter& out); // validated, tree levels built
 std::string setParameterLimits(HostCharacter& ch, int32_t count, const mb2_parameter_limit* limits);
+// restVertices [V][3], skinIndex / skinWeight [V][8], inverseBindPose [J][12]. A vertex's influences end at its first zero weight
+// (linear_skinning.cpp:76-80); the slots after it are ignored whatever they hold.
+std::string makeSkinning(const HostCharacter& ch, int32_t numVertices, const float* restVertices, const int32_t* skinIndex, const float* skinWeight,
+                         const float* inverseBindPose, HostSkinning& out);
 std::string positionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* offsets,
                                   const float* weights, HostErrorFunction& out);
 std::string instancedPositionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* weights,

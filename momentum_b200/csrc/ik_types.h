@@ -131,4 +131,24 @@ struct SkeletonTables {
   const float* ptColVals;    // [nnz]
 };
 
+// Linear-blend skinning tables (HostSkinning, makeSkinning), shared by the whole batch. The active influences of every vertex (the slots
+// before its first zero weight) are stored twice: by vertex for the blend, and by joint for the reductions of the backward, where each
+// joint's list is cut into segments of at most kSkinSegment influences that never cross a joint boundary.
+constexpr int kSkinMaxInfluences = 8;  // kMaxSkinJoints (skin_weights.h:19)
+constexpr int kSkinSegment = 128;      // influences per segment of the skel-state backward
+constexpr int kSkinIbpStride = 12;     // inverse bind pose: the row-major top 3x4 of Affine3f::matrix()
+struct SkinTables {
+  int32_t numVertices, numSegments;
+  const float* restVertices;    // [V][3]
+  const int32_t* vertStart;     // [V+1] active influences by vertex (CSR)
+  const int32_t* vertJoint;     // [nnz] slot order
+  const float* vertWeight;      // [nnz]
+  const float* inverseBindPose; // [J][12]
+  const int32_t* infVertex;     // [nnz] by joint (CSC), vertices ascending within a joint
+  const float* infWeight;       // [nnz]
+  const int32_t* segStart;      // [S+1] into infVertex / infWeight
+  const int32_t* segJoint;      // [S]
+  const int32_t* jointSegStart; // [J+1] segments of each joint, in list order
+};
+
 } // namespace mb2

@@ -76,6 +76,7 @@ CABI_SYMBOLS = [
     "mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device",
     "mb2_add_orientation_error_function_instanced", "mb2_solver_function_input_gradients_device",
     "mb2_solver_function_implicit_direction_device",
+    "mb2_character_set_skinning", "mb2_character_num_vertices", "mb2_character_skin_points_device", "mb2_character_skin_points_backward_device",
 ]
 
 _libs = {}
@@ -177,6 +178,11 @@ def load_library(path: Optional[str] = None):
         L.mb2_solver_function_input_gradients_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
     if hasattr(L, "mb2_solver_function_implicit_direction_device"):
         L.mb2_solver_function_implicit_direction_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
+    if hasattr(L, "mb2_character_set_skinning"):
+        L.mb2_character_set_skinning.argtypes = [vp, C.c_int32, _fp, _ip, _fp, _fp]
+        L.mb2_character_num_vertices.argtypes = [vp]
+        L.mb2_character_skin_points_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]
+        L.mb2_character_skin_points_backward_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp, vp, vp]
     _libs[path] = L
     return L
 
@@ -265,6 +271,37 @@ class DeviceCharacter(_Base):
                 for j in range(27):
                     arr[k].f[j] = float(ff[j])
             self._check(self._L.mb2_character_set_parameter_limits(self._h, len(character.limits), arr))
+        self.skinning = None
+        if character.skinning is not None:
+            self.set_skinning(character.skinning)
+
+    def set_skinning(self, skinning: mc.Skinning):
+        """Uploads ``skinning`` (replacing any earlier one); ``self.skinning`` is the object uploaded."""
+        V = skinning.num_vertices
+        rv, rvp = _f32(np.asarray(skinning.rest_vertices).reshape(V, 3))
+        si, sip = _i32(np.asarray(skinning.skin_index).reshape(V, mc.MAX_SKIN_JOINTS))
+        sw, swp = _f32(np.asarray(skinning.skin_weight).reshape(V, mc.MAX_SKIN_JOINTS))
+        ib, ibp = _f32(np.asarray(skinning.inverse_bind_pose).reshape(self.character.num_joints, 12))
+        self._check(self._L.mb2_character_set_skinning(self._h, V, rvp, sip, swp, ibp))
+        self.skinning = skinning
+
+    @property
+    def num_vertices(self) -> int:
+        return int(self._L.mb2_character_num_vertices(self._h))
+
+    def skin_points_device(self, batch: int, state_device_ptr: int, rest_device_ptr: int, rest_batched: bool, points_device_ptr: int, stream: int = 0):
+        """Skinned points [B][V][3] of skeleton states [B][J][8]; rest points: 0 = the rest mesh, else [V][3] (shared) or [B][V][3]
+        (``rest_batched``). float32 device memory on this character's device, enqueued on ``stream``."""
+        self._check(self._L.mb2_character_skin_points_device(self._h, int(batch), C.c_void_p(state_device_ptr), C.c_void_p(rest_device_ptr or None),
+                                                             int(bool(rest_batched)), C.c_void_p(points_device_ptr), C.c_void_p(stream)))
+
+    def skin_points_backward_device(self, batch: int, state_device_ptr: int, rest_device_ptr: int, rest_batched: bool, grad_points_device_ptr: int,
+                                    grad_state_device_ptr: int, grad_rest_device_ptr: int, stream: int = 0):
+        """dLoss/d skeleton state [B][J][8] and dLoss/d rest points (the rest-point layout; the batch sum when shared) from dLoss/d points
+        [B][V][3]. A 0 output pointer is skipped."""
+        self._check(self._L.mb2_character_skin_points_backward_device(
+            self._h, int(batch), C.c_void_p(state_device_ptr), C.c_void_p(rest_device_ptr or None), int(bool(rest_batched)),
+            C.c_void_p(grad_points_device_ptr), C.c_void_p(grad_state_device_ptr or None), C.c_void_p(grad_rest_device_ptr or None), C.c_void_p(stream)))
 
     def skeleton_state_device(self, batch: int, params_device_ptr: int, state_device_ptr: int, stream: int = 0):
         """Skeleton state [B][J][8] (t, q xyzw, s) of model parameters [B][n], float32 device memory on this character's device, enqueued

@@ -70,3 +70,91 @@ def model_parameters_to_skeleton_state(character, model_parameters: torch.Tensor
     if model_parameters.dim() not in (1, 2) or model_parameters.shape[-1] != ch.num_params:
         raise ValueError(f"model_parameters must be [n] or [B, n] with n = {ch.num_params}, got {tuple(model_parameters.shape)}")
     return _SkeletonState.apply(_device_character(character, model_parameters.device), model_parameters)
+
+
+class _SkinPoints(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, dc, skel_state, rest_points):
+        J, V = dc.character.num_joints, dc.skinning.num_vertices
+        dev = skel_state.device
+        st = skel_state.detach().to(torch.float32).reshape(-1, J, 8).contiguous()
+        B = st.shape[0]
+        rest = None if rest_points is None else rest_points.detach().to(device=dev, dtype=torch.float32).contiguous()
+        batched = rest is not None and rest.dim() == 3
+        out = torch.empty(B, V, 3, device=dev, dtype=torch.float32)
+        dc.skin_points_device(B, st.data_ptr(), 0 if rest is None else rest.data_ptr(), batched, out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        ctx.dc, ctx.skinning, ctx.V, ctx.batched, ctx.has_rest = dc, dc.skinning, V, batched, rest is not None
+        ctx.state_shape, ctx.state_dtype = skel_state.shape, skel_state.dtype
+        ctx.rest_dtype = None if rest_points is None else rest_points.dtype
+        ctx.save_for_backward(st, rest if rest is not None else st.new_empty(0))
+        return out.reshape(*skel_state.shape[:-2], V, 3).to(skel_state.dtype)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_points):
+        st, rest = ctx.saved_tensors
+        dc = ctx.dc
+        if dc.skinning is not ctx.skinning:
+            raise RuntimeError("skin_points backward: the DeviceCharacter's skinning was replaced (set_skinning) after the forward; "
+                               "keep one DeviceCharacter per skinning, or pass the Character and replace character.skinning instead")
+        B, J, _ = st.shape
+        dev = st.device
+        g = grad_points.to(device=dev, dtype=torch.float32).reshape(B, ctx.V, 3).contiguous()
+        need_state, need_rest = ctx.needs_input_grad[1], ctx.needs_input_grad[2] and ctx.has_rest
+        gs = torch.empty(B, J, 8, device=dev, dtype=torch.float32) if need_state else None
+        gr = torch.empty_like(rest) if need_rest else None
+        dc.skin_points_backward_device(B, st.data_ptr(), rest.data_ptr() if ctx.has_rest else 0, ctx.batched, g.data_ptr(),
+                                       gs.data_ptr() if gs is not None else 0, gr.data_ptr() if gr is not None else 0,
+                                       torch.cuda.current_stream(dev).cuda_stream)
+        return (None, None if gs is None else gs.reshape(ctx.state_shape).to(ctx.state_dtype),
+                None if gr is None else gr.to(ctx.rest_dtype))
+
+
+_skin_handles = {}
+
+
+def _skinned_device_character(ch: mc.Character, device: torch.device) -> ms.DeviceCharacter:
+    """One DeviceCharacter per (character, device) holding ``ch.skinning``. When ``character.skinning`` is replaced, a new handle is
+    made instead of uploading into the old one: a graph recorded with the old skinning keeps its handle (``ctx.dc``) and its tables, and
+    no kernel in flight on another stream reads tables that are being replaced. An old handle is freed with the last graph that uses it."""
+    index = device.index if device.index is not None else torch.cuda.current_device()
+    key = (id(ch), index)
+    entry = _skin_handles.get(key)
+    if entry is None or entry[1] is not ch.skinning:
+        entry = (ch, ch.skinning, ms.DeviceCharacter(ch, index))  # the character is kept alive so that its id stays unique
+        _skin_handles[key] = entry
+    return entry[2]
+
+
+def skin_points(character, skel_state: torch.Tensor, rest_points=None) -> torch.Tensor:
+    """Linear-blend skinning (pymomentum ``Character.skin_points``): ``skel_state`` [J, 8] or [B, J, 8] (t, q xyzw, s; q is normalised)
+    on a CUDA device -> points [V, 3] or [B, V, 3] in the input dtype, computed in float32. ``rest_points``: None = the rest mesh,
+    [V, 3] shared by the batch (its gradient is the batch sum) or [B, V, 3]. Differentiable once with respect to ``skel_state`` and
+    ``rest_points``.
+
+    ``character`` is a ``momentum_b200.character.Character``, skinned with ``character.skinning``: replacing that attribute is safe at
+    any time, and graphs recorded before keep the skinning they were recorded with. Or it is a ``solver.DeviceCharacter``, skinned with
+    what was uploaded to it (``DeviceCharacter.skinning``); the backward of a graph recorded before a later ``set_skinning`` on the same
+    handle raises."""
+    if not torch.is_tensor(skel_state) or not skel_state.is_cuda:
+        raise ValueError("skin_points runs on CUDA tensors (there is no CPU fallback)")
+    is_handle = isinstance(character, ms.DeviceCharacter)
+    ch = character.character if is_handle else character
+    if not isinstance(ch, mc.Character):
+        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
+    sk = character.skinning if is_handle else ch.skinning
+    if sk is None:
+        raise ValueError("the character has no skinning")
+    J, V = ch.num_joints, sk.num_vertices
+    if skel_state.shape[-2:] == (4, 4):
+        raise ValueError("skin_points takes skeleton states [.., J, 8] (t, q xyzw, s), not 4x4 matrices")
+    if skel_state.dim() not in (2, 3) or skel_state.shape[-2:] != (J, 8):
+        raise ValueError(f"skel_state must be [J, 8] or [B, J, 8] with J = {J}, got {tuple(skel_state.shape)}")
+    if rest_points is not None:
+        if not torch.is_tensor(rest_points) or rest_points.device != skel_state.device:
+            raise ValueError("rest_points must be a tensor on the skel_state's device")
+        B = skel_state.shape[0] if skel_state.dim() == 3 else None
+        if not (rest_points.shape == (V, 3) or (B is not None and rest_points.shape == (B, V, 3))):
+            raise ValueError(f"rest_points must be [V, 3] or [B, V, 3] with V = {V} and the skel_state's B, got {tuple(rest_points.shape)}")
+    dc = _device_character(character, skel_state.device) if is_handle else _skinned_device_character(ch, skel_state.device)
+    return _SkinPoints.apply(dc, skel_state, rest_points)
