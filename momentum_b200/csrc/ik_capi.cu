@@ -115,6 +115,7 @@ struct mb2_character {
   // linear-blend skinning (mb2_character_set_skinning): numVertices == 0 when there is none
   HostSkinning skin;
   std::unique_ptr<SkinBuffers> skinDev; // replaced whole by mb2_character_set_skinning, never rewritten in place
+  CharacterTables tables() const; // the device copies above, as the kernels read them
 };
 
 struct DeviceSchedule {
@@ -202,21 +203,26 @@ struct mb2_solver {
   }
 };
 
+CharacterTables mb2_character::tables() const {
+  CharacterTables C{};
+  C.numJoints = host.numJoints;
+  C.numParams = host.numParams;
+  C.parent = parent.p;
+  C.offset = offset.p;
+  C.prerot = prerot.p;
+  C.ptOuter = ptOuter.p;
+  C.ptInner = ptInner.p;
+  C.ptVals = ptVals.p;
+  C.ptOffsets = ptOffsets.p;
+  C.numLevels = int(host.levelStart.size()) - 1;
+  C.ptNnz = int(host.ptInner.size());
+  C.levelStart = levelStart.p;
+  C.levelJoints = levelJoints.p;
+  return C;
+}
+
 FunctionTables mb2_solver_function::tables() const {
-  FunctionTables T{};
-  const HostCharacter& h = ch->host;
-  T.numJoints = h.numJoints;
-  T.numParams = h.numParams;
-  T.parent = ch->parent.p;
-  T.offset = ch->offset.p;
-  T.prerot = ch->prerot.p;
-  T.ptOuter = ch->ptOuter.p;
-  T.ptInner = ch->ptInner.p;
-  T.ptVals = ch->ptVals.p;
-  T.ptOffsets = ch->ptOffsets.p;
-  T.numLevels = int(h.levelStart.size()) - 1;
-  T.levelStart = ch->levelStart.p;
-  T.levelJoints = ch->levelJoints.p;
+  FunctionTables T{ch->tables()};
   T.numEf = int(plan.efs.size());
   T.numUnits = int(plan.units.size());
   T.numCells = int(plan.cells.size());
@@ -232,7 +238,6 @@ FunctionTables mb2_solver_function::tables() const {
   T.numCols = plan.numCols;
   T.weightsPerInstance = host.weightsPerInstance ? 1 : 0;
   T.numWeights = host.numWeights;
-  T.ptNnz = int(h.ptInner.size());
   T.numContribs = int(plan.contribs.size());
   T.numLimitData = int(plan.limitData.size());
   const bool strips = planMode == 2 && planAlignRows && sched;
@@ -954,19 +959,7 @@ int skeletonStateDevice(const mb2_character* c, int32_t batch, const float* thet
   NvtxRange range(backward ? "skeletonStateBackward" : "skeletonState");
   const HostCharacter& h = c->host;
   SkeletonStateArgs a{};
-  a.T.numJoints = h.numJoints;
-  a.T.numParams = h.numParams;
-  a.T.parent = c->parent.p;
-  a.T.offset = c->offset.p;
-  a.T.prerot = c->prerot.p;
-  a.T.ptOuter = c->ptOuter.p;
-  a.T.ptInner = c->ptInner.p;
-  a.T.ptVals = c->ptVals.p;
-  a.T.ptOffsets = c->ptOffsets.p;
-  a.T.numLevels = int(h.levelStart.size()) - 1;
-  a.T.levelStart = c->levelStart.p;
-  a.T.levelJoints = c->levelJoints.p;
-  a.T.ptNnz = int(h.ptInner.size());
+  a.T = c->tables();
   a.S.childStart = c->childStart.p;
   a.S.children = c->children.p;
   a.S.ptColStart = c->ptColStart.p;

@@ -90,7 +90,7 @@ MB2_HD float lossDeriv(const EfDesc& e, float s) {
 }
 
 // ---- ParameterTransformT::apply, one row (parameter_transform.cpp:122) ----
-MB2_HD float jointParameterRow(const FunctionTables& T, int row, const float* theta) {
+MB2_HD float jointParameterRow(const CharacterTables& T, int row, const float* theta) {
   float s = 0.f;
   for (int k = T.ptOuter[row]; k < T.ptOuter[row + 1]; ++k) s += T.ptVals[k] * theta[T.ptInner[k]];
   return s + T.ptOffsets[row];
@@ -98,7 +98,7 @@ MB2_HD float jointParameterRow(const FunctionTables& T, int row, const float* th
 
 // ---- JointStateT::set for joint j (joint_state.cpp:22-65). js: kJointStateStride floats per joint ----
 template <bool kDeriv>
-MB2_HD void fkJoint(const FunctionTables& T, int j, const float* jp, float* js) {
+MB2_HD void fkJoint(const CharacterTables& T, int j, const float* jp, float* js) {
   const float* p = jp + j * kParametersPerJoint;
   const int par = T.parent[j];
   F3 tp = f3(0.f, 0.f, 0.f);
@@ -145,22 +145,22 @@ MB2_HD void fkJoint(const FunctionTables& T, int j, const float* jp, float* js) 
 //                                  rotated vector instead of a rotation by a quaternion product; equal up to rounding]
 // fkJoint above stays the statement-by-statement form (CPU emulation of the oracle order, tests).
 template <bool kDeriv>
-MB2_HD void fkLocalFromParameters(const FunctionTables& T, int j, const float* p, float* js);
+MB2_HD void fkLocalFromParameters(const CharacterTables& T, int j, const float* p, float* js);
 template <bool kDeriv>
-MB2_HD void fkLocal(const FunctionTables& T, int j, const float* jp, float* js) { fkLocalFromParameters<kDeriv>(T, j, jp + j * kParametersPerJoint, js); }
+MB2_HD void fkLocal(const CharacterTables& T, int j, const float* jp, float* js) { fkLocalFromParameters<kDeriv>(T, j, jp + j * kParametersPerJoint, js); }
 // the joint's seven parameters straight from theta (ParameterTransform rows 7 j .. 7 j + 6): no [7 J] array in shared memory, and the
 // transform is spread over lanes = joints (three rounds for 72 joints) instead of lanes = rows (sixteen rounds of dependent loads)
 template <bool kDeriv>
-MB2_HD void fkLocalFromTheta(const FunctionTables& T, int j, const float* theta, float* js) {
+MB2_HD void fkLocalFromTheta(const CharacterTables& T, int j, const float* theta, float* js) {
   float p[kParametersPerJoint];
 #pragma unroll
   for (int r = 0; r < kParametersPerJoint; ++r) p[r] = jointParameterRow(T, j * kParametersPerJoint + r, theta);
   fkLocalFromParameters<kDeriv>(T, j, p, js);
 }
 // jp == nullptr: the caller keeps no joint-parameter array (same value, recomputed from theta)
-MB2_HD float jointParameterAt(const FunctionTables& T, const float* jp, const float* theta, int row) { return jp != nullptr ? jp[row] : jointParameterRow(T, row, theta); }
+MB2_HD float jointParameterAt(const CharacterTables& T, const float* jp, const float* theta, int row) { return jp != nullptr ? jp[row] : jointParameterRow(T, row, theta); }
 template <bool kDeriv>
-MB2_HD void fkLocalFromParameters(const FunctionTables& T, int j, const float* p, float* js) {
+MB2_HD void fkLocalFromParameters(const CharacterTables& T, int j, const float* p, float* js) {
   Q4 ql = ld4(T.prerot + 4 * j);
   float* out = js + j * kJointStateStride;
 #pragma unroll
@@ -183,7 +183,7 @@ MB2_HD void fkLocalFromParameters(const FunctionTables& T, int j, const float* p
   out[7] = exp2f(p[6]);
 }
 // the parent (if any) already holds its world transform
-MB2_HD void fkCompose(const FunctionTables& T, int j, float* js) {
+MB2_HD void fkCompose(const CharacterTables& T, int j, float* js) {
   const int par = T.parent[j];
   if (par < 0) return; // identity parent: world = local, bit for bit
   const float* ps = js + par * kJointStateStride;
@@ -198,7 +198,7 @@ MB2_HD void fkCompose(const FunctionTables& T, int j, float* js) {
   out[7] = sp * out[7];
 }
 // after every joint is composed: world direction of DOF axis `index` of joint j
-MB2_HD void fkAxis(const FunctionTables& T, int j, int index, float* js) {
+MB2_HD void fkAxis(const CharacterTables& T, int j, int index, float* js) {
   const int par = T.parent[j];
   if (par < 0) return;
   float* a = js + j * kJointStateStride + 8 + 3 * index;
@@ -207,7 +207,7 @@ MB2_HD void fkAxis(const FunctionTables& T, int j, int index, float* js) {
 }
 
 // translationAxis of joint a = parent.toLinear() (joint_state.cpp:36-42), column d
-MB2_HD F3 translationAxisCol(const FunctionTables& T, const float* js, int a, int d) {
+MB2_HD F3 translationAxisCol(const CharacterTables& T, const float* js, int a, int d) {
   const int par = T.parent[a];
   if (par < 0) return f3(d == 0 ? 1.f : 0.f, d == 1 ? 1.f : 0.f, d == 2 ? 1.f : 0.f);
   const float* ps = js + par * kJointStateStride;
@@ -217,7 +217,7 @@ MB2_HD F3 rotationAxisCol(const float* js, int a, int d) { return ld3(js + a * k
 
 // derivative of a world point v attached below joint a w.r.t. joint-parameter dof d
 // (joint_state.cpp:68-82 + joint_error_function-inl.h:240-291)
-MB2_HD F3 pointDerivative(const FunctionTables& T, const float* js, int a, int d, F3 v) {
+MB2_HD F3 pointDerivative(const CharacterTables& T, const float* js, int a, int d, F3 v) {
   if (d < 3) return translationAxisCol(T, js, a, d);
   const F3 off = v - ld3(js + a * kJointStateStride);
   if (d < 6) return cross(rotationAxisCol(js, a, d - 3), off);
@@ -270,7 +270,7 @@ MB2_HD void skelGradFold(const SkeletonTables& S, const float* js, int a, float*
   A[7] = sc.x; A[8] = sc.y; A[9] = sc.z; A[10] = ss;
 }
 // dLoss / d joint parameter `row` (= 7 a + k) from the finished sums of joint a; js holds the world state and DOF axes (fkAxis)
-MB2_HD float skelGradJointParameter(const FunctionTables& T, const float* js, const float* acc, int row) {
+MB2_HD float skelGradJointParameter(const CharacterTables& T, const float* js, const float* acc, int row) {
   const int a = row / kParametersPerJoint, k = row - a * kParametersPerJoint;
   const float* A = acc + a * kSkelAccStride;
   if (k < 3) return dot(translationAxisCol(T, js, a, k), ld3(A));
@@ -294,13 +294,13 @@ MB2_HD float skelGradModelParameter(const SkeletonTables& S, const float* gjp, i
 constexpr int kTangentStride = 7; // w(3) sigma tdot(3); odd: conflict-free with lanes = joints
 
 // u[row] = (P v)[row] without ptOffsets (jointParameterRow adds them)
-MB2_HD float tangentJointParameter(const FunctionTables& T, int row, const float* v) {
+MB2_HD float tangentJointParameter(const CharacterTables& T, int row, const float* v) {
   float s = 0.f;
   for (int k = T.ptOuter[row]; k < T.ptOuter[row + 1]; ++k) s += T.ptVals[k] * v[T.ptInner[k]];
   return s;
 }
 // the joint's own share of its motion (all joints at once; js holds the world state and DOF axes, fkAxis)
-MB2_HD void tangentLocal(const FunctionTables& T, const float* js, int j, const float* v, float* tan) {
+MB2_HD void tangentLocal(const CharacterTables& T, const float* js, int j, const float* v, float* tan) {
   const int r0 = j * kParametersPerJoint;
   F3 w = f3(0.f, 0.f, 0.f), td = f3(0.f, 0.f, 0.f);
   for (int k = 0; k < 3; ++k) {
@@ -313,7 +313,7 @@ MB2_HD void tangentLocal(const FunctionTables& T, const float* js, int j, const 
   o[4] = td.x; o[5] = td.y; o[6] = td.z;
 }
 // level by level from the roots: adds the (finished) parent's motion to the joint's own share
-MB2_HD void tangentCompose(const FunctionTables& T, const float* js, int j, float* tan) {
+MB2_HD void tangentCompose(const CharacterTables& T, const float* js, int j, float* tan) {
   const int par = T.parent[j];
   if (par < 0) return;
   const float* P = tan + par * kTangentStride;
@@ -325,6 +325,93 @@ MB2_HD void tangentCompose(const FunctionTables& T, const float* js, int j, floa
   o[0] = w.x; o[1] = w.y; o[2] = w.z;
   o[3] = sp + o[3];
   o[4] = td.x; o[5] = td.y; o[6] = td.z;
+}
+
+// ---- Lane groups and the per-instance pass sequences -------------------------------------------------------------------------
+// A lane group is the set of lanes that work on one instance: `lane` in [0, size) and sync(), the barrier between two passes. The pass
+// functions below state each pass sequence with its barriers once, for the kernels and for the CPU emulators (tests/emu), which run
+// them with HostLanes. Only reduction-free passes are shared: within a pass no lane reads what another lane of the pass writes, so one
+// lane running every index in order computes the same bits.
+struct HostLanes {
+  static constexpr int size = 1, lane = 0;
+  MB2_HD void sync() const {}
+};
+#if defined(__CUDACC__)
+// W warps of a CTA per instance; group = warp / W waits on named barrier 1 + group (0 is __syncthreads), a single warp on __syncwarp
+template <int W>
+struct WarpLanes {
+  static constexpr int size = 32 * W;
+  int group, lane;
+  __device__ static WarpLanes of(int warp, int lane) { return {warp / W, (warp % W) * 32 + lane}; } // warp, lane of the CTA
+  MB2_HD void sync() const {
+#if defined(__CUDA_ARCH__)
+    if (W == 1) __syncwarp();
+    else asm volatile("bar.sync %0, %1;" ::"r"(1 + group), "r"(size) : "memory");
+#endif
+  }
+};
+// the whole CTA of kThreads threads on one instance
+template <int kThreads>
+struct CtaLanes {
+  static constexpr int size = kThreads;
+  int lane;
+  MB2_HD void sync() const {
+#if defined(__CUDA_ARCH__)
+    __syncthreads();
+#endif
+  }
+};
+#endif
+
+// SkeletonState::set of one instance in the three data-parallel passes above: the local part of every joint, its joint parameters
+// computed from theta or (kFromJointParameters) read from a staged [7 J] array, then the composition level by level from the roots, then
+// (kAxes) the DOF axes in world space. The axes pass ends without a barrier, so that the caller's next pass can share it.
+template <bool kAxes, bool kFromJointParameters, class Lanes>
+MB2_HD void fkPasses(const Lanes& g, const CharacterTables& C, const float* src, float* js) {
+  for (int j = g.lane; j < C.numJoints; j += g.size) {
+    if constexpr (kFromJointParameters) fkLocal<kAxes>(C, j, src, js);
+    else fkLocalFromTheta<kAxes>(C, j, src, js);
+  }
+  g.sync();
+  for (int lvl = 1; lvl < C.numLevels; ++lvl) { // level 0 = roots: world = local
+    const int end = C.levelStart[lvl + 1];
+    for (int k = C.levelStart[lvl] + g.lane; k < end; k += g.size) fkCompose(C, C.levelJoints[k], js);
+    g.sync();
+  }
+  if constexpr (kAxes)
+    for (int i = g.lane; i < 3 * C.numJoints; i += g.size) fkAxis(C, i / 3, i % 3, js);
+}
+
+// The skeleton-state backward of one instance, right after fkPasses<true> (fkAxis writes only the axes and the seed reads only t, q, s:
+// the seed shares the axes' barrier): every joint seeds its subtree sums from the upstream gradient grad [J][8], the levels from the
+// deepest up fold in their children, lanes = joint-parameter rows into gjp [7 J], lanes = model parameters into out [n]. Ends without a
+// barrier.
+template <class Lanes>
+MB2_HD void skelGradPasses(const Lanes& g, const CharacterTables& C, const SkeletonTables& S, const float* js, const float* grad, float* acc,
+                           float* gjp, float* out) {
+  for (int i = g.lane; i < C.numJoints; i += g.size) skelGradSeed(js, i, grad + 8 * i, acc);
+  g.sync();
+  for (int lvl = C.numLevels - 2; lvl >= 0; --lvl) { // the deepest level has no children
+    const int end = C.levelStart[lvl + 1];
+    for (int k = C.levelStart[lvl] + g.lane; k < end; k += g.size) skelGradFold(S, js, C.levelJoints[k], acc);
+    g.sync();
+  }
+  for (int row = g.lane; row < C.numJoints * kParametersPerJoint; row += g.size) gjp[row] = skelGradJointParameter(C, js, acc, row);
+  g.sync();
+  for (int p = g.lane; p < C.numParams; p += g.size) out[p] = skelGradModelParameter(S, gjp, p);
+}
+
+// The joint motions of one instance under the parameter direction v (js: world state and DOF axes, complete): every joint's own share,
+// then the parent's motion added level by level from the roots. Ends with a barrier.
+template <class Lanes>
+MB2_HD void tangentPasses(const Lanes& g, const CharacterTables& C, const float* js, const float* v, float* tan) {
+  for (int j = g.lane; j < C.numJoints; j += g.size) tangentLocal(C, js, j, v, tan);
+  g.sync();
+  for (int lvl = 1; lvl < C.numLevels; ++lvl) {
+    const int end = C.levelStart[lvl + 1];
+    for (int k = C.levelStart[lvl] + g.lane; k < end; k += g.size) tangentCompose(C, js, C.levelJoints[k], tan);
+    g.sync();
+  }
 }
 
 // Position constraint (L2), p = t_j + s_j R_j o, d = p - t, W = e.weight w_c / c^2, g = 2 W d . pdot:

@@ -87,7 +87,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
   double* errSlots = reinterpret_cast<double*>(th + np4); // 8 warp partials, then [8] = error of this iteration, [9] = lastError
   int* flags = reinterpret_cast<int*>(errSlots + 10);     // [0] Cholesky breakdown, [1] stop, [2] next instance, [3] non-finite
 
-  auto groupSync = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(1 + group), "r"(kFusedGroupThreads) : "memory"); };
+  const WarpLanes<kFusedGroupThreads / 32> g{group, gt};
   const int numJointParams = T.numJoints * kParametersPerJoint;
   const size_t sweepStripFloats = size_t(a.stripStride) + 64; // strips | residual | zero strip: what the Gram phase reads
   float parked[kFusedMaxRounds][8]; // Gram tiles that would overwrite live strips, indexed by the round: thread-local memory
@@ -100,7 +100,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
 
   while (true) {
     if (gt == 0) flags[2] = atomicAdd(a.workCounter, 1);
-    groupSync();
+    g.sync();
     const int b = flags[2];
     if (b >= a.batch) break;
     const float* targets = a.targets + size_t(b) * T.targetStride;
@@ -112,28 +112,21 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
     MB2_PH(kPhFetch)
     for (int it = 0; it < a.maxIterations; ++it) {
       // ---- ParameterTransform::apply + zero background of the strips (ResizeableMatrix::resizeAndSetZero, solver_function.cpp:96) ----
-      groupSync(); // theta (first iteration: the loads above; later: the update) is visible; the previous iteration is done with the tiles
+      g.sync(); // theta (first iteration: the loads above; later: the update) is visible; the previous iteration is done with the tiles
       for (int row = gt; row < numJointParams; row += kFusedGroupThreads) jp[row] = jointParameterRow(T, row, th);
       for (int i = gt; i < (a.stripStride + 64) / 4; i += kFusedGroupThreads) reinterpret_cast<float4*>(strips)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      groupSync();
+      g.sync();
       MB2_PH(kPhJointParams)
       // ---- SkeletonState::set, level by level (skeleton_state.cpp:87-121) ----
-      for (int j = gt; j < T.numJoints; j += kFusedGroupThreads) fkLocal<true>(T, j, jp, js);
-      groupSync();
-      for (int lvl = 1; lvl < T.numLevels; ++lvl) { // level 0 = roots: world = local
-        const int end = T.levelStart[lvl + 1];
-        for (int k = T.levelStart[lvl] + gt; k < end; k += kFusedGroupThreads) fkCompose(T, T.levelJoints[k], js);
-        groupSync();
-      }
-      for (int i = gt; i < 3 * T.numJoints; i += kFusedGroupThreads) fkAxis(T, i / 3, i % 3, js);
-      groupSync();
+      fkPasses<true, true>(g, T, jp, js);
+      g.sync();
       MB2_PH(kPhFk)
       // ---- residual + error (units), then the Jacobian cells into the strips ----
       double err = 0.0;
       for (int u = gt; u < T.numUnits; u += kFusedGroupThreads) err += (double)evalUnit<true>(T, u, th, jp, js, targets, cw, rec, resid);
       err = warpSumD(err);
       if (lane == 0) errSlots[warp] = err;
-      groupSync();
+      g.sync();
       MB2_PH(kPhUnits)
       for (int c = gt; c < T.numCells; c += kFusedGroupThreads) jacobianCell(T, c, js, rec, targets, strips);
       if (gt == 0) { // fixed order: deterministic
@@ -141,7 +134,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
         for (int w = 0; w < kFusedGroupThreads / 32; ++w) e += errSlots[w];
         errSlots[8] = e;
       }
-      groupSync();
+      g.sync();
       MB2_PH(kPhCells)
       // ---- tile-sparse Gram: a warp owns a tile at a time; a finished tile beyond the strips is stored at once, one that would
       //      overwrite strips still being read waits in thread-local memory ----
@@ -165,7 +158,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
         for (int K = hw; K < S.numTileCols; K += kFusedGroupThreads / 16)
           y[16 * K + hl] = gramVectorEntry(strips, resid, colStrip, stripRow, colStripStart[K], colStripStart[K + 1], hl);
       }
-      groupSync();
+      g.sync();
       MB2_PH(kPhGram)
       {
         int slot = 0;
@@ -182,7 +175,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
           if (p >= 0) gsub[p] = y[s];
         }
       }
-      groupSync();
+      g.sync();
       MB2_PH(kPhRestore)
       // ---- level-scheduled Cholesky (ik_chol_sched.h) ----
       for (int Lv = 0; Lv < S.numLevels; ++Lv) {
@@ -190,7 +183,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
           const int K = S.levelCols[ci];
           cholDiagTile(tiles + size_t(S.diagTile[K]) * 256, y + 16 * K, lane, a.regularization, flags);
         }
-        groupSync();
+        g.sync();
         MB2_PH(kPhDiag)
         for (int pi = S.levelPanelStart[Lv] + warp; pi < S.levelPanelStart[Lv + 1]; pi += kFusedGroupThreads / 32) {
           float* ptile = tiles + size_t(S.panelTile[pi]) * 256;
@@ -198,20 +191,20 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
           cholPanelProduct(ptile, tiles + size_t(S.panelDiag[pi]) * 256, lane, x);
           cholPanelStore(ptile, lane, x);
         }
-        groupSync();
+        g.sync();
         MB2_PH(kPhPanel)
         for (int oi = S.levelOrderStart8[Lv] + warp; oi < S.levelOrderStart8[Lv + 1]; oi += kFusedGroupThreads / 32) { const int ti = S.taskOrder8[oi]; if (ti >= 0) cholUpdateTask(tiles, S, ti, lane); }
         for (int vi = S.levelVTaskStart[Lv] + hw; vi < S.levelVTaskStart[Lv + 1]; vi += kFusedGroupThreads / 16) cholVectorTask(tiles, y, S, vi, hl);
-        groupSync();
+        g.sync();
         MB2_PH(kPhUpdate)
       }
       for (int Lv = S.numLevels - 1; Lv >= 0; --Lv) {
         for (int ci = S.levelColStart[Lv] + warp; ci < S.levelColStart[Lv + 1]; ci += kFusedGroupThreads / 32) cholBackwardColumn(tiles, y, S, S.levelCols[ci], lane);
-        groupSync();
+        g.sync();
       }
       MB2_PH(kPhBackward)
       for (int i = gt; i < S.nPad; i += kFusedGroupThreads) { const int p = S.perm[i]; if (p >= 0) dsub[p] = y[i]; }
-      groupSync();
+      g.sync();
       // ---- theta -= delta (skeleton_solver_function.cpp:153-159) and the SolverT bookkeeping (solver.cpp:92-122) ----
       for (int i = gt; i < n; i += kFusedGroupThreads) {
         const int c = cols[i];
@@ -226,7 +219,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
         if (!stop) errSlots[9] = error;
         flags[1] = stop ? 1 : 0;
       }
-      groupSync();
+      g.sync();
       MB2_PH(kPhFinish)
       if (flags[1] != 0) break;
     }
@@ -234,7 +227,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
     bool bad = false;
     for (int i = gt; i < T.numParams; i += kFusedGroupThreads) bad = bad || !isfinite(th[i]);
     if (bad) flags[3] = 1;
-    groupSync();
+    g.sync();
     const bool nonFinite = flags[3] != 0;
     if (!nonFinite)
       for (int i = gt; i < T.numParams; i += kFusedGroupThreads) thetaG[i] = th[i];

@@ -47,13 +47,17 @@ MB2_HD size_t tableWords(size_t count, size_t elemBytes) { return (count * elemB
 // mode 1: every table; mode 2: everything except the two big ones, cells and contributions (large rigs: those are streamed through
 // L1 / L2, one sequential record per lane and iteration, while the tables walked by dependent loads - character, units, error functions -
 // still sit in shared memory)
+// the character tables, staged first by every kernel that stages tables (stageCharacterTables)
+size_t characterTableWords(const CharacterTables& C) {
+  const size_t J = C.numJoints;
+  size_t w = tableWords(J, 4) + tableWords(3 * J, 4) + tableWords(4 * J, 4);                 // parent, offset, prerot
+  w += tableWords(7 * J + 1, 4) + tableWords(C.ptNnz, 4) * 2 + tableWords(7 * J, 4);         // ptOuter, ptInner, ptVals, ptOffsets
+  w += tableWords(C.numLevels + 1, 4) + tableWords(J, 4);                                    // levelStart, levelJoints
+  return w;
+}
 size_t sweepTableBytes(const FunctionTables& T, int mode) {
   if (mode == 0) return 0;
-  const size_t J = T.numJoints;
-  size_t w = 0;
-  w += tableWords(J, 4) + tableWords(3 * J, 4) + tableWords(4 * J, 4);                       // parent, offset, prerot
-  w += tableWords(7 * J + 1, 4) + tableWords(T.ptNnz, 4) * 2 + tableWords(7 * J, 4);         // ptOuter, ptInner, ptVals, ptOffsets
-  w += tableWords(T.numLevels + 1, 4) + tableWords(J, 4);                                    // levelStart, levelJoints
+  size_t w = characterTableWords(T);
   w += tableWords(T.numEf, sizeof(EfDesc)) + tableWords(T.numUnits, sizeof(UnitDesc)) + tableWords(T.numLimitData, 4);
   if (mode == 1) w += tableWords(T.numCells, sizeof(CellDesc)) + tableWords(T.numContribs, sizeof(ContribDesc));
   return w * 4;
@@ -78,6 +82,14 @@ __device__ __forceinline__ void stageTable(const E*& table, size_t count, uint32
   table = reinterpret_cast<const E*>(cursor);
   cursor += tableWords(count, sizeof(E));
 }
+// C's pointers move to the copies at cursor (characterTableWords(C) words); the caller syncs the CTA before they are read
+__device__ __forceinline__ void stageCharacterTables(CharacterTables& C, uint32_t*& cursor) {
+  const size_t J = C.numJoints;
+  stageTable(C.parent, J, cursor); stageTable(C.offset, 3 * J, cursor); stageTable(C.prerot, 4 * J, cursor);
+  stageTable(C.ptOuter, 7 * J + 1, cursor); stageTable(C.ptInner, C.ptNnz, cursor); stageTable(C.ptVals, C.ptNnz, cursor);
+  stageTable(C.ptOffsets, 7 * J, cursor);
+  stageTable(C.levelStart, C.numLevels + 1, cursor); stageTable(C.levelJoints, J, cursor);
+}
 
 // kStage (1 all tables, 2 all but cells / contributions, 0 none): the tables live in shared memory for the whole kernel. A template parameter rather than a run-time branch so that every
 // table pointer is PROVABLY a shared-memory address: with `if (a.stageTables)` the pointers could be either and all 273 table loads
@@ -89,67 +101,45 @@ __global__ void __launch_bounds__(32 * kSweepMaxWarps) sweepKernel(const SweepAr
   extern __shared__ __align__(16) float smem[];
   FunctionTables T = a.T;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // a group of W warps works on one instance: gl = lane within the group, gs = lanes of the group
-  const int group = warp / W, gl = (warp % W) * 32 + lane;
-  constexpr int gs = 32 * W;
+  const WarpLanes<W> g = WarpLanes<W>::of(warp, lane); // a group of W warps works on one instance
   const int groupsPerCta = (blockDim.x >> 5) / W;
   const int nPad = (T.numParams + 3) & ~3;
   // (kJointStateStride is odd: an odd joint count gets one float of padding so that the doubles below stay 8-byte aligned)
   const int jpFloats = W > 1 ? ((T.numJoints * kParametersPerJoint + 1) & ~1) : 0;
   const int perGroup = nPad + jpFloats + ((T.numJoints * kJointStateStride + 1) & ~1) + ((T.recStride + 1) & ~1) + 4 + 2 * W;
-  float* th = smem + size_t(group) * perGroup;
+  float* th = smem + size_t(g.group) * perGroup;
   float* jp = W > 1 ? th + nPad : nullptr;
   float* js = th + nPad + jpFloats;
   float* rec = js + ((T.numJoints * kJointStateStride + 1) & ~1);
   double* errSlots = reinterpret_cast<double*>(rec + ((T.recStride + 1) & ~1)); // W partial sums (8-byte aligned: every preceding size is even)
-  auto groupSync = [&]() {
-    if (W == 1) __syncwarp();
-    else asm volatile("bar.sync %0, %1;" ::"r"(1 + group), "r"(gs) : "memory");
-  };
   if constexpr (kStage != 0) {
     uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + ((size_t(groupsPerCta) * perGroup + 3) & ~size_t(3)));
-    const size_t J = T.numJoints;
-    stageTable(T.parent, J, cursor); stageTable(T.offset, 3 * J, cursor); stageTable(T.prerot, 4 * J, cursor);
-    stageTable(T.ptOuter, 7 * J + 1, cursor); stageTable(T.ptInner, T.ptNnz, cursor); stageTable(T.ptVals, T.ptNnz, cursor);
-    stageTable(T.ptOffsets, 7 * J, cursor);
-    stageTable(T.levelStart, T.numLevels + 1, cursor); stageTable(T.levelJoints, J, cursor);
+    stageCharacterTables(T, cursor);
     stageTable(T.efs, T.numEf, cursor); stageTable(T.units, T.numUnits, cursor); stageTable(T.limitData, T.numLimitData, cursor);
     if constexpr (kStage == 1) { stageTable(T.cells, T.numCells, cursor); stageTable(T.contribs, T.numContribs, cursor); }
     __syncthreads();
   }
 
-  for (int b = blockIdx.x * groupsPerCta + group; b < a.batch; b += gridDim.x * groupsPerCta) {
+  for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
     if (a.active != nullptr && a.active[b] == 0) continue; // (the whole group skips together)
     const float* theta = a.theta + size_t(b) * a.ldTheta;
-    for (int i = gl; i < T.numParams; i += gs) th[i] = theta[i];
-    groupSync();
+    for (int i = g.lane; i < T.numParams; i += g.size) th[i] = theta[i];
+    g.sync();
     if (W == 1) { // touch the next instance's parameters now: by the time this one is done they sit in L1 / L2 (one warp = one 880-byte row)
       const int bn = b + gridDim.x * groupsPerCta;
-      if (bn < a.batch) { const float* tn = a.theta + size_t(bn) * a.ldTheta; for (int i = gl * 8; i < T.numParams; i += gs * 8) asm volatile("prefetch.global.L2 [%0];" ::"l"(tn + i)); }
+      if (bn < a.batch) { const float* tn = a.theta + size_t(bn) * a.ldTheta; for (int i = g.lane * 8; i < T.numParams; i += g.size * 8) asm volatile("prefetch.global.L2 [%0];" ::"l"(tn + i)); }
     }
-    // SkeletonState::set in three data-parallel passes (ik_device.cuh): every joint's local part at once (its seven joint parameters
-    // come straight from theta: ParameterTransform::apply row by row), ~50 dependent flops per tree level, then the derivative axes
-    // (one warp per instance: three rounds of lanes = joints, each walking its seven rows; several warps per instance: lanes = rows first)
+    // SkeletonState::set (fkPasses): one warp per instance takes each joint's seven parameters straight from theta (three rounds of
+    // lanes = joints, each walking its seven rows); several warps per instance stage them first with lanes = rows
     if constexpr (W > 1) {
-      for (int row = gl; row < T.numJoints * kParametersPerJoint; row += gs) jp[row] = jointParameterRow(T, row, th);
-      groupSync();
-      for (int j = gl; j < T.numJoints; j += gs) fkLocal<kJacobian>(T, j, jp, js);
-    } else {
-      for (int j = gl; j < T.numJoints; j += gs) fkLocalFromTheta<kJacobian>(T, j, th, js);
+      for (int row = g.lane; row < T.numJoints * kParametersPerJoint; row += g.size) jp[row] = jointParameterRow(T, row, th);
+      g.sync();
     }
-    groupSync();
-    for (int lvl = 1; lvl < T.numLevels; ++lvl) { // level 0 = roots: world = local
-      const int end = T.levelStart[lvl + 1];
-      for (int k = T.levelStart[lvl] + gl; k < end; k += gs) fkCompose(T, T.levelJoints[k], js);
-      groupSync();
-    }
-    if (kJacobian) {
-      for (int i = gl; i < 3 * T.numJoints; i += gs) fkAxis(T, i / 3, i % 3, js);
-      groupSync();
-    }
+    fkPasses<kJacobian, (W > 1)>(g, T, W > 1 ? jp : th, js);
+    if constexpr (kJacobian) g.sync();
     if (a.stateOut != nullptr) {
       float* so = a.stateOut + size_t(b) * T.numJoints * 8;
-      for (int i = gl; i < T.numJoints * 8; i += gs) so[i] = js[(i >> 3) * kJointStateStride + (i & 7)];
+      for (int i = g.lane; i < T.numJoints * 8; i += g.size) so[i] = js[(i >> 3) * kJointStateStride + (i & 7)];
     }
     const float* targets = a.targets + size_t(b) * T.targetStride;
     const float* cw = a.cweights + (T.weightsPerInstance ? size_t(b) * T.numWeights : 0);
@@ -157,18 +147,18 @@ __global__ void __launch_bounds__(32 * kSweepMaxWarps) sweepKernel(const SweepAr
     // the residual is the last column of the device matrix, or follows the strips
     float* residual = kJacobian ? J + (T.stripMode ? size_t(T.residOff) : size_t(T.numCols) * T.ldJ) : nullptr;
     double err = 0.0;
-    for (int u = gl; u < T.numUnits; u += gs) err += (double)evalUnit<kJacobian>(T, u, th, jp, js, targets, cw, rec, residual);
+    for (int u = g.lane; u < T.numUnits; u += g.size) err += (double)evalUnit<kJacobian>(T, u, th, jp, js, targets, cw, rec, residual);
     err = warpSum(err);
     if (W > 1 && lane == 0) errSlots[warp % W] = err;
-    groupSync();
+    g.sync();
     if (kJacobian)
-      for (int c = gl; c < T.numCells; c += gs) jacobianCell(T, c, js, rec, targets, J);
-    if (gl == 0) {
+      for (int c = g.lane; c < T.numCells; c += g.size) jacobianCell(T, c, js, rec, targets, J);
+    if (g.lane == 0) {
       if (W > 1) { err = 0.0; for (int w = 0; w < W; ++w) err += errSlots[w]; } // fixed order: deterministic
       // getError() rounds through float (skeleton_solver_function.cpp:82); the Jacobian pass keeps double
       a.errors[b] = kJacobian ? err : (double)(float)err;
     }
-    groupSync();
+    g.sync();
   }
 }
 
@@ -244,11 +234,13 @@ cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream)
 }
 
 // ------------------------------------------------------------------------------------------------
-// Skeleton state of a batch of model parameters, and its backward (ik_device.cuh skelGrad*): a persistent grid, one group of W warps
-// per instance, the character tables staged in shared memory once per CTA.
-//   forward:   lanes = joints (local part from theta), level by level compose, [J][8] out
-//   backward:  the same FK with the DOF axes, then lanes = joints seed their 11 subtree sums from G, levels from the deepest up fold
-//              in their children, lanes = joint-parameter rows, lanes = model parameters over the CSC ParameterTransform.
+// Skeleton state of a batch of model parameters, and its backward (ik_device.cuh skelGrad*).
+// The per-instance frame, shared with inputGradientKernel: a persistent grid sized by launchInstanceGroups, one group of W warps per
+// instance (WarpLanes<W>), the character tables staged in shared memory once per CTA (stageCharacterTables, kernel-specific tables after
+// them), then per instance the pass functions of ik_device.cuh, which the CPU emulators run too.
+//   forward:   fkPasses from theta, [J][8] out
+//   backward:  fkPasses with the DOF axes, then skelGradPasses: lanes = joints seed their 11 subtree sums from G, levels from the
+//              deepest up fold in their children, lanes = joint-parameter rows, lanes = model parameters over the CSC ParameterTransform.
 // Every output element is written by one lane in a fixed order: no atomics, the result does not depend on the launch shape.
 // ------------------------------------------------------------------------------------------------
 constexpr int kSkelMaxWarps = 16;
@@ -260,125 +252,102 @@ MB2_HD size_t skeletonStateSmemPerInstanceFloats(int J, int n, bool backward) {
   if (backward) f += skelAligned(size_t(J) * kSkelAccStride) + skelAligned(size_t(J) * kParametersPerJoint);
   return f;
 }
-size_t skeletonStateSmemPerInstance(const FunctionTables& T, bool backward) {
-  return sizeof(float) * skeletonStateSmemPerInstanceFloats(T.numJoints, T.numParams, backward);
+size_t skeletonStateSmemPerInstance(const CharacterTables& C, bool backward) {
+  return sizeof(float) * skeletonStateSmemPerInstanceFloats(C.numJoints, C.numParams, backward);
 }
 
 size_t skeletonStateTableBytes(const SkeletonStateArgs& a, bool backward) {
-  const FunctionTables& T = a.T;
-  const size_t J = T.numJoints;
-  size_t w = tableWords(J, 4) + tableWords(3 * J, 4) + tableWords(4 * J, 4);                   // parent, offset, prerot
-  w += tableWords(7 * J + 1, 4) + tableWords(T.ptNnz, 4) * 2 + tableWords(7 * J, 4);          // ptOuter, ptInner, ptVals, ptOffsets
-  w += tableWords(T.numLevels + 1, 4) + tableWords(J, 4);                                     // levelStart, levelJoints
-  if (backward) w += tableWords(J + 1, 4) + tableWords(a.numChildren, 4) + tableWords(T.numParams + 1, 4) + tableWords(T.ptNnz, 4) * 2;
+  const CharacterTables& C = a.T;
+  size_t w = characterTableWords(C);
+  if (backward) w += tableWords(C.numJoints + 1, 4) + tableWords(a.numChildren, 4) + tableWords(C.numParams + 1, 4) + tableWords(C.ptNnz, 4) * 2;
   return w * 4;
 }
 
 template <bool kBackward, int W>
 __global__ void __launch_bounds__(32 * kSkelMaxWarps) skeletonStateKernel(const SkeletonStateArgs a) {
   extern __shared__ __align__(16) float smem[];
-  FunctionTables T = a.T;
+  CharacterTables T = a.T;
   SkeletonTables S = a.S;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int group = warp / W, gl = (warp % W) * 32 + lane;
-  constexpr int gs = 32 * W;
+  const WarpLanes<W> g = WarpLanes<W>::of(threadIdx.x >> 5, threadIdx.x & 31);
   const int groupsPerCta = (blockDim.x >> 5) / W;
   const int J = T.numJoints, n = T.numParams;
   const int thF = int(skelAligned(n)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
   const int accF = kBackward ? int(skelAligned(size_t(J) * kSkelAccStride)) : 0;
   const int perGroup = int(skeletonStateSmemPerInstanceFloats(J, n, kBackward));
-  float* th = smem + size_t(group) * perGroup;
+  float* th = smem + size_t(g.group) * perGroup;
   float* js = th + thF;
   float* acc = js + jsF;
   float* gjp = acc + accF;
-  auto groupSync = [&]() {
-    if (W == 1) __syncwarp();
-    else asm volatile("bar.sync %0, %1;" ::"r"(1 + group), "r"(gs) : "memory");
-  };
   {
     uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
-    const size_t Jz = J;
-    stageTable(T.parent, Jz, cursor); stageTable(T.offset, 3 * Jz, cursor); stageTable(T.prerot, 4 * Jz, cursor);
-    stageTable(T.ptOuter, 7 * Jz + 1, cursor); stageTable(T.ptInner, T.ptNnz, cursor); stageTable(T.ptVals, T.ptNnz, cursor);
-    stageTable(T.ptOffsets, 7 * Jz, cursor);
-    stageTable(T.levelStart, T.numLevels + 1, cursor); stageTable(T.levelJoints, Jz, cursor);
+    stageCharacterTables(T, cursor);
     if constexpr (kBackward) {
-      stageTable(S.childStart, Jz + 1, cursor); stageTable(S.children, a.numChildren, cursor);
+      stageTable(S.childStart, size_t(J) + 1, cursor); stageTable(S.children, a.numChildren, cursor);
       stageTable(S.ptColStart, n + 1, cursor); stageTable(S.ptColRows, T.ptNnz, cursor); stageTable(S.ptColVals, T.ptNnz, cursor);
     }
     __syncthreads();
   }
-  for (int b = blockIdx.x * groupsPerCta + group; b < a.batch; b += gridDim.x * groupsPerCta) {
+  for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
     const float* theta = a.theta + size_t(b) * n;
-    for (int i = gl; i < n; i += gs) th[i] = theta[i];
-    groupSync();
-    for (int j = gl; j < J; j += gs) fkLocalFromTheta<kBackward>(T, j, th, js);
-    groupSync();
-    for (int lvl = 1; lvl < T.numLevels; ++lvl) { // level 0 = roots: world = local
-      const int end = T.levelStart[lvl + 1];
-      for (int k = T.levelStart[lvl] + gl; k < end; k += gs) fkCompose(T, T.levelJoints[k], js);
-      groupSync();
-    }
+    for (int i = g.lane; i < n; i += g.size) th[i] = theta[i];
+    g.sync();
+    fkPasses<kBackward, false>(g, T, th, js);
     if constexpr (!kBackward) {
       float* so = a.out + size_t(b) * J * 8;
-      for (int i = gl; i < J * 8; i += gs) so[i] = js[(i >> 3) * kJointStateStride + (i & 7)];
+      for (int i = g.lane; i < J * 8; i += g.size) so[i] = js[(i >> 3) * kJointStateStride + (i & 7)];
     } else {
-      // fkAxis writes only the axes and skelGradSeed reads only (t, q, s): one barrier for both
-      for (int i = gl; i < 3 * J; i += gs) fkAxis(T, i / 3, i % 3, js);
-      const float* G = a.gradState + size_t(b) * J * 8;
-      for (int i = gl; i < J; i += gs) skelGradSeed(js, i, G + 8 * i, acc);
-      groupSync();
-      for (int lvl = T.numLevels - 2; lvl >= 0; --lvl) { // the deepest level has no children
-        const int end = T.levelStart[lvl + 1];
-        for (int k = T.levelStart[lvl] + gl; k < end; k += gs) skelGradFold(S, js, T.levelJoints[k], acc);
-        groupSync();
-      }
-      for (int row = gl; row < J * kParametersPerJoint; row += gs) gjp[row] = skelGradJointParameter(T, js, acc, row);
-      groupSync();
-      float* go = a.out + size_t(b) * n;
-      for (int p = gl; p < n; p += gs) go[p] = skelGradModelParameter(S, gjp, p);
+      skelGradPasses(g, T, S, js, a.gradState + size_t(b) * J * 8, acc, gjp, a.out + size_t(b) * n);
     }
-    groupSync(); // the next instance overwrites th / js / gjp
+    g.sync(); // the next instance overwrites th / js / gjp
   }
 }
 
-cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream) {
+namespace {
+// Grid of a persistent kernel: what the SMs hold at once, capped by the work.
+template <class K>
+cudaError_t persistentGrid(K kernel, int threads, size_t smem, long work, int* grid) {
+  if (smem > size_t(g_maxSmemOptin)) return cudaErrorInvalidConfiguration;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (e != cudaSuccess) return e;
+  int perSm = 0;
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kernel, threads, smem);
+  if (e != cudaSuccess) return e;
+  *grid = int(std::max(1L, std::min(long(std::max(g_numSms, 1)) * std::max(perSm, 1), work)));
+  return cudaSuccess;
+}
+
+// A persistent kernel with one group of W warps per instance and the tables staged once per CTA (skeletonStateKernel,
+// inputGradientKernel). As many instances per CTA as shared memory holds next to the tables, one warp each up to kSkelMaxWarps. When
+// fewer than eight fit (large rigs), several warps share an instance. A batch smaller than one instance group per SM is spread over the
+// SMs. kernels[0..3]: the instantiations for W = 1, 2, 4, 8.
+template <class Args>
+cudaError_t launchInstanceGroups(void (*const kernels[4])(Args), const Args& a, size_t perInstance, size_t tableBytes, cudaStream_t stream) {
   if (a.batch <= 0) return cudaSuccess;
-  // As many instances per CTA as shared memory holds next to the tables, one warp each up to kSkelMaxWarps. When fewer than eight fit
-  // (large rigs), several warps share an instance. A batch smaller than one instance group per SM is spread over the SMs.
   const size_t budget = size_t(g_maxSmemOptin);
-  const size_t tableBytes = skeletonStateTableBytes(a, backward) + 16;
-  const size_t per = skeletonStateSmemPerInstance(a.T, backward);
-  if (tableBytes + per > budget) return cudaErrorInvalidConfiguration;
-  const int fit = int((budget - tableBytes) / per);
-  int W = 1, groups = std::min(fit, kSkelMaxWarps);
+  tableBytes += 16;
+  if (tableBytes + perInstance > budget) return cudaErrorInvalidConfiguration;
+  const int fit = int((budget - tableBytes) / perInstance);
+  int W = 1, w = 0, groups = std::min(fit, kSkelMaxWarps);
   if (fit < 8)
-    while (W < 8 && groups * W * 2 <= kSkelMaxWarps) W *= 2; // named barriers 1..groups
+    while (W < 8 && groups * W * 2 <= kSkelMaxWarps) { W *= 2; ++w; } // named barriers 1..groups
   const int sms = std::max(g_numSms, 1);
   if (a.batch < sms * groups) groups = std::max(1, (a.batch + sms - 1) / sms);
-  const size_t smem = per * groups + tableBytes;
+  const size_t smem = perInstance * groups + tableBytes;
   const int threads = groups * W * 32;
-  auto launch = [&](auto kernel) -> cudaError_t {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-    if (e != cudaSuccess) return e;
-    int perSm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kernel, threads, smem);
-    if (e != cudaSuccess) return e;
-    const long needed = (long(a.batch) + groups - 1) / groups;
-    const int grid = int(std::max(1L, std::min(long(sms) * std::max(perSm, 1), needed)));
-    kernel<<<grid, threads, smem, stream>>>(a);
-    return cudaGetLastError();
-  };
-  auto pick = [&](auto bwd) -> cudaError_t {
-    constexpr bool kB = decltype(bwd)::value;
-    switch (W) {
-      case 1: return launch(skeletonStateKernel<kB, 1>);
-      case 2: return launch(skeletonStateKernel<kB, 2>);
-      case 4: return launch(skeletonStateKernel<kB, 4>);
-      default: return launch(skeletonStateKernel<kB, 8>);
-    }
-  };
-  return backward ? pick(std::true_type{}) : pick(std::false_type{});
+  int grid = 0;
+  const cudaError_t e = persistentGrid(kernels[w], threads, smem, (long(a.batch) + groups - 1) / groups, &grid);
+  if (e != cudaSuccess) return e;
+  kernels[w]<<<grid, threads, smem, stream>>>(a);
+  return cudaGetLastError();
+}
+} // namespace
+
+cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream) {
+  static void (*const forward[4])(SkeletonStateArgs) = {skeletonStateKernel<false, 1>, skeletonStateKernel<false, 2>, skeletonStateKernel<false, 4>,
+                                                         skeletonStateKernel<false, 8>};
+  static void (*const reverse[4])(SkeletonStateArgs) = {skeletonStateKernel<true, 1>, skeletonStateKernel<true, 2>, skeletonStateKernel<true, 4>,
+                                                         skeletonStateKernel<true, 8>};
+  return launchInstanceGroups(backward ? reverse : forward, a, skeletonStateSmemPerInstance(a.T, backward), skeletonStateTableBytes(a, backward), stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -504,26 +473,13 @@ __global__ void skinStateFinishKernel(const SkinArgs a, int b0, int nb, const fl
 }
 
 namespace {
-// Grid of a persistent skin kernel: what the SMs hold at once, capped by the work.
-template <class K>
-cudaError_t skinGrid(K kernel, size_t smem, long work, int* grid) {
-  if (smem > size_t(g_maxSmemOptin)) return cudaErrorInvalidConfiguration;
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-  if (e != cudaSuccess) return e;
-  int perSm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kernel, kSkinThreads, smem);
-  if (e != cudaSuccess) return e;
-  *grid = int(std::max(1L, std::min(long(std::max(g_numSms, 1)) * std::max(perSm, 1), work)));
-  return cudaSuccess;
-}
-
 // kMode 0 / 1: one work item per instance when the batch fills the grid, else each instance's vertices split over several
 template <int kMode>
 cudaError_t launchSkinPerInstance(const SkinArgs& a, float* out, cudaStream_t stream) {
   const size_t smem = size_t(a.numJoints) * kSkinIbpStride * sizeof(float);
   const int V = a.S.numVertices;
   int slots = 0;
-  cudaError_t e = skinGrid(skinVertexKernel<kMode>, smem, 1L << 30, &slots);
+  cudaError_t e = persistentGrid(skinVertexKernel<kMode>, kSkinThreads, smem, 1L << 30, &slots);
   if (e != cudaSuccess) return e;
   const int vSplit = a.batch >= slots ? 1 : std::min((slots + a.batch - 1) / a.batch, (V + kSkinThreads - 1) / kSkinThreads);
   const int vLen = (V + vSplit - 1) / vSplit;
@@ -551,8 +507,8 @@ cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream) {
     e = cudaMallocAsync(reinterpret_cast<void**>(&partial), perInstance * slice, stream);
     if (e != cudaSuccess) return e;
     int g1 = 0, g2 = 0;
-    e = skinGrid(skinStatePartialKernel, 0, (long(slice) * a.S.numSegments + 7) / 8, &g1);
-    if (e == cudaSuccess) e = skinGrid(skinStateFinishKernel, 0, (long(slice) * J + kSkinThreads - 1) / kSkinThreads, &g2);
+    e = persistentGrid(skinStatePartialKernel, kSkinThreads, 0, (long(slice) * a.S.numSegments + 7) / 8, &g1);
+    if (e == cudaSuccess) e = persistentGrid(skinStateFinishKernel, kSkinThreads, 0, (long(slice) * J + kSkinThreads - 1) / kSkinThreads, &g2);
     for (int b0 = 0; e == cudaSuccess && b0 < a.batch; b0 += slice) {
       const int nb = std::min(slice, a.batch - b0);
       skinStatePartialKernel<<<g1, kSkinThreads, 0, stream>>>(a, b0, nb, partial);
@@ -575,7 +531,7 @@ cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream) {
     if (e != cudaSuccess) return e;
   }
   int grid = 0;
-  e = skinGrid(skinVertexKernel<2>, smem, long(numChunks) * vSplit, &grid);
+  e = persistentGrid(skinVertexKernel<2>, kSkinThreads, smem, long(numChunks) * vSplit, &grid);
   if (e == cudaSuccess) {
     skinVertexKernel<2><<<grid, kSkinThreads, smem, stream>>>(a, perChunk, numChunks, vSplit, kSkinChunkVerts, partial);
     e = cudaGetLastError();
@@ -592,10 +548,10 @@ cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Input gradients of one Position / Orientation block, d/d input [grad_theta E . v] (ik_device.cuh tangent* / *InputGradient): laid out
-// like skeletonStateKernel, a persistent grid with one group of W warps per instance and the character tables in shared memory.
-//   lanes = parameters: theta, and v gated by the enabled set;  lanes = joints: FK with the DOF axes;  lanes = joints: each joint's own
-//   motion;  level by level: the parent's motion added;  lanes = constraints of the block.
+// Input gradients of one Position / Orientation block, d/d input [grad_theta E . v] (ik_device.cuh tangent* / *InputGradient), in the
+// per-instance frame of skeletonStateKernel:
+//   lanes = parameters: theta, and v gated by the enabled set;  fkPasses with the DOF axes;  tangentPasses: each joint's own motion,
+//   then level by level the parent's motion added;  lanes = constraints of the block.
 // Every output element is written by one lane: no atomics, the result does not depend on the launch shape.
 // ------------------------------------------------------------------------------------------------
 // per instance: theta [n], v [n], joint states [J][17], joint motions [J][7]
@@ -603,70 +559,39 @@ MB2_HD size_t inputGradientSmemPerInstanceFloats(int J, int n) {
   return 2 * skelAligned(size_t(n)) + skelAligned(size_t(J) * kJointStateStride) + skelAligned(size_t(J) * kTangentStride);
 }
 
-size_t inputGradientTableBytes(const FunctionTables& T) {
-  const size_t J = T.numJoints;
-  size_t w = tableWords(J, 4) + tableWords(3 * J, 4) + tableWords(4 * J, 4);
-  w += tableWords(7 * J + 1, 4) + tableWords(T.ptNnz, 4) * 2 + tableWords(7 * J, 4);
-  w += tableWords(T.numLevels + 1, 4) + tableWords(J, 4);
-  return w * 4;
-}
-
 template <int W>
 __global__ void __launch_bounds__(32 * kSkelMaxWarps) inputGradientKernel(const InputGradientArgs a) {
   extern __shared__ __align__(16) float smem[];
   FunctionTables T = a.T;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int group = warp / W, gl = (warp % W) * 32 + lane;
-  constexpr int gs = 32 * W;
+  const WarpLanes<W> g = WarpLanes<W>::of(threadIdx.x >> 5, threadIdx.x & 31);
   const int groupsPerCta = (blockDim.x >> 5) / W;
   const int J = T.numJoints, n = T.numParams, nc = a.numConstraints;
   const int thF = int(skelAligned(n)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
   const int perGroup = int(inputGradientSmemPerInstanceFloats(J, n));
-  float* th = smem + size_t(group) * perGroup;
+  float* th = smem + size_t(g.group) * perGroup;
   float* vs = th + thF;
   float* js = vs + thF;
   float* tan = js + jsF;
-  auto groupSync = [&]() {
-    if (W == 1) __syncwarp();
-    else asm volatile("bar.sync %0, %1;" ::"r"(1 + group), "r"(gs) : "memory");
-  };
   {
     uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
-    const size_t Jz = J;
-    stageTable(T.parent, Jz, cursor); stageTable(T.offset, 3 * Jz, cursor); stageTable(T.prerot, 4 * Jz, cursor);
-    stageTable(T.ptOuter, 7 * Jz + 1, cursor); stageTable(T.ptInner, T.ptNnz, cursor); stageTable(T.ptVals, T.ptNnz, cursor);
-    stageTable(T.ptOffsets, 7 * Jz, cursor);
-    stageTable(T.levelStart, T.numLevels + 1, cursor); stageTable(T.levelJoints, Jz, cursor);
+    stageCharacterTables(T, cursor);
     __syncthreads();
   }
   const EfDesc e = T.efs[T.units[a.unitBegin].ef];
   const bool position = a.kind == kUnitPosition;
   const int per = position ? 3 : 4;
-  for (int b = blockIdx.x * groupsPerCta + group; b < a.batch; b += gridDim.x * groupsPerCta) {
+  for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
     const float* theta = a.theta + size_t(b) * n;
     const float* dir = a.direction + size_t(b) * n;
-    for (int i = gl; i < n; i += gs) { th[i] = theta[i]; vs[i] = 0.f; }
-    groupSync();
-    for (int k = gl; k < a.numEnabled; k += gs) { const int p = a.enabledList[k]; vs[p] = dir[p]; }
-    for (int j = gl; j < J; j += gs) fkLocalFromTheta<true>(T, j, th, js);
-    groupSync();
-    for (int lvl = 1; lvl < T.numLevels; ++lvl) {
-      const int end = T.levelStart[lvl + 1];
-      for (int k = T.levelStart[lvl] + gl; k < end; k += gs) fkCompose(T, T.levelJoints[k], js);
-      groupSync();
-    }
-    for (int i = gl; i < 3 * J; i += gs) fkAxis(T, i / 3, i % 3, js);
-    groupSync();
-    for (int j = gl; j < J; j += gs) tangentLocal(T, js, j, vs, tan);
-    groupSync();
-    for (int lvl = 1; lvl < T.numLevels; ++lvl) {
-      const int end = T.levelStart[lvl + 1];
-      for (int k = T.levelStart[lvl] + gl; k < end; k += gs) tangentCompose(T, js, T.levelJoints[k], tan);
-      groupSync();
-    }
+    for (int i = g.lane; i < n; i += g.size) { th[i] = theta[i]; vs[i] = 0.f; }
+    g.sync();
+    for (int k = g.lane; k < a.numEnabled; k += g.size) { const int p = a.enabledList[k]; vs[p] = dir[p]; }
+    fkPasses<true, false>(g, T, th, js);
+    g.sync();
+    tangentPasses(g, T, js, vs, tan);
     const float* targets = a.targets + size_t(b) * T.targetStride;
     const float* cweights = a.cweights + (T.weightsPerInstance ? size_t(b) * T.numWeights : 0);
-    for (int c = gl; c < nc; c += gs) {
+    for (int c = g.lane; c < nc; c += g.size) {
       const UnitDesc& u = T.units[a.unitBegin + c];
       const size_t o = size_t(b) * nc + c;
       float* gW = a.gradWeights ? a.gradWeights + o : nullptr;
@@ -675,43 +600,14 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps) inputGradientKernel(const 
       if (position) positionInputGradient(u, e, js, tan, targets + u.targetOff, cweights[u.weightIdx], gW, gO, gT);
       else orientationInputGradient(u, e, js, tan, targets + u.targetOff, cweights[u.weightIdx], gW, gO, gT);
     }
-    groupSync(); // the next instance overwrites th / vs / js / tan
+    g.sync(); // the next instance overwrites th / vs / js / tan
   }
 }
 
 cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream) {
-  if (a.batch <= 0) return cudaSuccess;
-  // the sizing rule of launchSkeletonState: as many instances per CTA as shared memory holds beside the tables, several warps per
-  // instance for large rigs, a small batch spread over the SMs
-  const size_t budget = size_t(g_maxSmemOptin);
-  const size_t tableBytes = inputGradientTableBytes(a.T) + 16;
+  static void (*const kernels[4])(InputGradientArgs) = {inputGradientKernel<1>, inputGradientKernel<2>, inputGradientKernel<4>, inputGradientKernel<8>};
   const size_t per = sizeof(float) * inputGradientSmemPerInstanceFloats(a.T.numJoints, a.T.numParams);
-  if (tableBytes + per > budget) return cudaErrorInvalidConfiguration;
-  const int fit = int((budget - tableBytes) / per);
-  int W = 1, groups = std::min(fit, kSkelMaxWarps);
-  if (fit < 8)
-    while (W < 8 && groups * W * 2 <= kSkelMaxWarps) W *= 2;
-  const int sms = std::max(g_numSms, 1);
-  if (a.batch < sms * groups) groups = std::max(1, (a.batch + sms - 1) / sms);
-  const size_t smem = per * groups + tableBytes;
-  const int threads = groups * W * 32;
-  auto launch = [&](auto kernel) -> cudaError_t {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-    if (e != cudaSuccess) return e;
-    int perSm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kernel, threads, smem);
-    if (e != cudaSuccess) return e;
-    const long needed = (long(a.batch) + groups - 1) / groups;
-    const int grid = int(std::max(1L, std::min(long(sms) * std::max(perSm, 1), needed)));
-    kernel<<<grid, threads, smem, stream>>>(a);
-    return cudaGetLastError();
-  };
-  switch (W) {
-    case 1: return launch(inputGradientKernel<1>);
-    case 2: return launch(inputGradientKernel<2>);
-    case 4: return launch(inputGradientKernel<4>);
-    default: return launch(inputGradientKernel<8>);
-  }
+  return launchInstanceGroups(kernels, a, per, characterTableWords(a.T) * 4, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -842,18 +738,10 @@ cudaError_t implicitDirectionConfigure(const ImplicitDirectionArgs& a, ImplicitD
   const size_t extra = implicitDirectionExtraBytes(k, a.numEnabled), gram = sizeof(double) * jacobiPackedSize(k);
   cfg.gramInShared = extra + gram <= size_t(g_maxSmemOptin);
   cfg.smem = extra + (cfg.gramInShared ? gram : 0);
-  if (cfg.smem > size_t(g_maxSmemOptin)) return cudaErrorInvalidConfiguration;
   cfg.slotDoubles = (jacobiLogDoubles(k) + (cfg.gramInShared ? 0 : jacobiPackedSize(k)) + 1) & ~size_t(1); // slots stay 16-byte aligned
-  cudaError_t e = cudaFuncSetAttribute(implicitDirectionKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cfg.smem));
-  if (e != cudaSuccess) return e;
-  int perSm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, implicitDirectionKernel, kJacobiThreads, cfg.smem);
-  if (e != cudaSuccess) return e;
-  long grid = long(std::max(g_numSms, 1)) * std::max(perSm, 1);
-  grid = std::min(grid, long(std::max(a.batch, 1)));
-  if (cfg.slotDoubles > 0) grid = std::min(grid, long(std::max<size_t>(1, kJacobiScratchBudget / (sizeof(double) * cfg.slotDoubles))));
-  cfg.grid = int(grid);
-  return cudaSuccess;
+  long work = std::max(a.batch, 1);
+  if (cfg.slotDoubles > 0) work = std::min(work, long(std::max<size_t>(1, kJacobiScratchBudget / (sizeof(double) * cfg.slotDoubles))));
+  return persistentGrid(implicitDirectionKernel, kJacobiThreads, cfg.smem, work, &cfg.grid);
 }
 
 cudaError_t launchImplicitDirection(const ImplicitDirectionArgs& a, const ImplicitDirectionConfig& cfg, cudaStream_t stream) {

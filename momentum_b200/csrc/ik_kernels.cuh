@@ -144,7 +144,7 @@ cudaError_t launchQrSolve(const QrArgs& a, int maxChunkRows, cudaStream_t stream
 // skeletonStateKernel<kBackward>: pymomentum's model_parameters_to_skeleton_state for a batch on the character alone (no solver
 // function), and its backward
 struct SkeletonStateArgs {
-  FunctionTables T;          // character part only (parent .. levelJoints, numParams, ptNnz)
+  CharacterTables T;
   SkeletonTables S;          // backward only
   int32_t numChildren;       // entries of S.children
   int32_t batch;

@@ -176,6 +176,24 @@ std::string makeSkinning(const HostCharacter& ch, int32_t numVertices, const flo
   return "";
 }
 
+CharacterTables hostCharacterTables(const HostCharacter& ch) {
+  CharacterTables C{};
+  C.numJoints = ch.numJoints;
+  C.numParams = ch.numParams;
+  C.parent = ch.parent.data();
+  C.offset = ch.offset.data();
+  C.prerot = ch.prerot.data();
+  C.ptOuter = ch.ptOuter.data();
+  C.ptInner = ch.ptInner.data();
+  C.ptVals = ch.ptVals.data();
+  C.ptOffsets = ch.ptOffsets.data();
+  C.numLevels = int32_t(ch.levelStart.size()) - 1;
+  C.ptNnz = int32_t(ch.ptInner.size());
+  C.levelStart = ch.levelStart.data();
+  C.levelJoints = ch.levelJoints.data();
+  return C;
+}
+
 std::string setParameterLimits(HostCharacter& ch, int32_t count, const mb2_parameter_limit* limits) {
   if (!(count >= 0 && (count == 0 || limits))) return "invalid limits";
   ch.limits.clear();

@@ -100,6 +100,8 @@ struct HostFunction {
 // Each returns an empty string when the arguments are accepted, else the message of the first rejected one.
 std::string makeCharacter(int32_t numJoints, const int32_t* parents, const float* offsets, const float* prerot, int32_t numParams, const int32_t* outer,
                           const int32_t* inner, const float* vals, const float* ptOffsets, HostCharacter& out); // validated, tree levels built
+// CharacterTables on the host copy (the CPU emulators' view of what mb2_character::tables gives the kernels)
+CharacterTables hostCharacterTables(const HostCharacter& ch);
 std::string setParameterLimits(HostCharacter& ch, int32_t count, const mb2_parameter_limit* limits);
 // restVertices [V][3], skinIndex / skinWeight [V][8], inverseBindPose [J][12]. A vertex's influences end at its first zero weight
 // (linear_skinning.cpp:76-80); the slots after it are ignored whatever they hold.

@@ -81,12 +81,7 @@ __device__ void trFoldDiagonal(float* R, float* y, float* D, float* dvec, float*
 // through float (skeleton_solver_function.cpp:64-83). js: [J][kJointStateStride] scratch.
 __device__ double trGetError(const FunctionTables& T, const float* th, float* js, const float* targets, const float* cw, double* dred) {
   const int tid = threadIdx.x;
-  for (int j = tid; j < T.numJoints; j += kQrThreads) fkLocalFromTheta<false>(T, j, th, js);
-  __syncthreads();
-  for (int lvl = 1; lvl < T.numLevels; ++lvl) {
-    for (int k = T.levelStart[lvl] + tid; k < T.levelStart[lvl + 1]; k += kQrThreads) fkCompose(T, T.levelJoints[k], js);
-    __syncthreads();
-  }
+  fkPasses<false, false>(CtaLanes<kQrThreads>{tid}, T, th, js);
   double err = 0.0;
   for (int u = tid; u < T.numUnits; u += kQrThreads) err += (double)evalUnit<false>(T, u, th, nullptr, js, targets, cw, nullptr, nullptr);
   for (int o = 16; o > 0; o >>= 1) err += __shfl_xor_sync(0xffffffffu, err, o);

@@ -85,9 +85,10 @@ struct ContribDesc {
   float coef;
 };
 
-// Everything the FK / residual / Jacobian kernels need (device pointers), passed by value.
-struct FunctionTables {
-  // character
+// The character as the FK reads it: skeleton, ParameterTransform (CSR) and the depth levels of the joint tree. Passed by value; the
+// pointers are device addresses in the kernels' arguments (mb2_character::tables) and host addresses in the emulators
+// (hostCharacterTables).
+struct CharacterTables {
   int32_t numJoints, numParams;
   const int32_t* parent;     // [J]
   const float* offset;       // [J*3]
@@ -99,7 +100,11 @@ struct FunctionTables {
   int32_t numLevels;         // depth levels of the joint tree
   const int32_t* levelStart; // [numLevels+1]
   const int32_t* levelJoints; // [J] joints sorted by depth
-  // objective
+  int32_t ptNnz;             // entries of ptInner / ptVals
+};
+
+// Everything the FK / residual / Jacobian kernels need (device pointers), passed by value: the character, then the objective.
+struct FunctionTables : CharacterTables {
   int32_t numEf, numUnits, numCells;
   const EfDesc* efs;
   const UnitDesc* units;
@@ -115,14 +120,14 @@ struct FunctionTables {
   int32_t weightsPerInstance; // 0: cweights [numWeights] shared, 1: [B][numWeights]
   int32_t numWeights;
   // table sizes (the sweep kernel stages every table in shared memory when they fit)
-  int32_t ptNnz, numContribs, numLimitData;
+  int32_t numContribs, numLimitData;
   // Jacobian output layout. 0: K-major matrix [numCols + 1][ldJ] (column numCols = residual). 1: strips (GramPlan in
   // ik_chol_sched.h): [numStrips][16 columns][4 rows] then the residual at residOff, rows numbered with 4-aligned row groups.
   int32_t stripMode, residOff;
   size_t jacobianStride;     // floats per instance in the Jacobian buffer
 };
 
-// What the skeleton-state backward walks besides the character part of FunctionTables (HostCharacter::buildBackwardTables)
+// What the skeleton-state backward walks besides CharacterTables (HostCharacter::buildBackwardTables)
 struct SkeletonTables {
   const int32_t* childStart; // [J+1]
   const int32_t* children;   // [J - roots], ascending within a joint

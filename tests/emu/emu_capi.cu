@@ -76,12 +76,7 @@ static std::string planTiles(mb2_solver_function* f, int cholMode, bool strips, 
 }
 
 static FunctionTables tables(const mb2_solver_function* f) {
-  FunctionTables T{};
-  const HostCharacter& h = f->ch->host;
-  T.numJoints = h.numJoints; T.numParams = h.numParams;
-  T.parent = h.parent.data(); T.offset = h.offset.data(); T.prerot = h.prerot.data();
-  T.ptOuter = h.ptOuter.data(); T.ptInner = h.ptInner.data(); T.ptVals = h.ptVals.data(); T.ptOffsets = h.ptOffsets.data();
-  T.numLevels = int(h.levelStart.size()) - 1; T.levelStart = h.levelStart.data(); T.levelJoints = h.levelJoints.data();
+  FunctionTables T{hostCharacterTables(f->ch->host)};
   T.numEf = int(f->plan.efs.size()); T.numUnits = int(f->plan.units.size()); T.numCells = int(f->plan.cells.size());
   T.efs = f->plan.efs.data(); T.units = f->plan.units.data(); T.cells = f->plan.cells.data(); T.contribs = f->plan.contribs.data();
   T.limitData = f->plan.limitData.data();
@@ -97,12 +92,7 @@ template <bool kJacobian>
 static void sweepOne(mb2_solver_function* f, const FunctionTables& T, int b, const float* theta, double* errOut, float* stateOut) {
   std::vector<float> jp(size_t(T.numJoints) * 7), js(size_t(T.numJoints) * kJointStateStride), rec(T.recStride + 4);
   for (int row = 0; row < T.numJoints * 7; ++row) jp[row] = jointParameterRow(T, row, theta);
-  // the kernels' three passes
-  for (int j = 0; j < T.numJoints; ++j) fkLocalFromTheta<kJacobian>(T, j, theta, js.data()); // as sweepKernel: joint parameters straight from theta
-  for (int lvl = 1; lvl < T.numLevels; ++lvl)
-    for (int k = T.levelStart[lvl]; k < T.levelStart[lvl + 1]; ++k) fkCompose(T, T.levelJoints[k], js.data());
-  if (kJacobian)
-    for (int i = 0; i < 3 * T.numJoints; ++i) fkAxis(T, i / 3, i % 3, js.data());
+  fkPasses<kJacobian, false>(HostLanes{}, T, theta, js.data()); // as sweepKernel with one warp: joint parameters straight from theta
   if (stateOut)
     for (int i = 0; i < T.numJoints * 8; ++i) stateOut[i] = js[(i >> 3) * kJointStateStride + (i & 7)];
   const float* tg = f->targets.data() + size_t(b) * T.targetStride;

@@ -2,8 +2,8 @@
 // tests/test_solve_ik_input_gradients.py into a temporary directory together with ik_plan.cpp / ik_chol_sched.cpp.
 //
 // The character is made by the library's own makeCharacter and the block by the library's own error-function constructors and planner
-// (the units the kernel reads); the __host__ __device__ building blocks of ik_device.cuh then run pass by pass, the lanes of each pass in
-// sequence. It is not part of the product library and nothing in momentum_b200/ loads it.
+// (the units the kernel reads); the kernel's own pass functions of ik_device.cuh (fkPasses, tangentPasses) then run with HostLanes, the
+// lanes of each pass in sequence. It is not part of the product library and nothing in momentum_b200/ loads it.
 #include <cmath>
 #include <cstdint>
 #include <string>
@@ -52,12 +52,7 @@ extern "C" int emu_input_gradients(int32_t numJoints, const int32_t* parents, co
         const float n = sqrtf(p[0] * p[0] + p[1] * p[1] + p[2] * p[2] + p[3] * p[3]);
         p[0] /= n; p[1] /= n; p[2] /= n; p[3] /= n;
       }
-  FunctionTables T{};
-  T.numJoints = h.numJoints; T.numParams = h.numParams;
-  T.parent = h.parent.data(); T.offset = h.offset.data(); T.prerot = h.prerot.data();
-  T.ptOuter = h.ptOuter.data(); T.ptInner = h.ptInner.data(); T.ptVals = h.ptVals.data(); T.ptOffsets = h.ptOffsets.data();
-  T.numLevels = int(h.levelStart.size()) - 1; T.levelStart = h.levelStart.data(); T.levelJoints = h.levelJoints.data();
-  T.ptNnz = int(h.ptInner.size());
+  FunctionTables T{hostCharacterTables(h)};
   T.efs = plan.efs.data(); T.units = plan.units.data();
   T.targetStride = stride;
   T.weightsPerInstance = 1; T.numWeights = nc;
@@ -67,13 +62,8 @@ extern "C" int emu_input_gradients(int32_t numJoints, const int32_t* parents, co
     const float* th = theta + size_t(b) * n;
     for (int i = 0; i < n; ++i) vs[i] = 0.f;
     for (int p : plan.enabledList) vs[p] = direction[size_t(b) * n + p];
-    for (int j = 0; j < J; ++j) fkLocalFromTheta<true>(T, j, th, js.data());
-    for (int lvl = 1; lvl < T.numLevels; ++lvl)
-      for (int k = T.levelStart[lvl]; k < T.levelStart[lvl + 1]; ++k) fkCompose(T, T.levelJoints[k], js.data());
-    for (int i = 0; i < 3 * J; ++i) fkAxis(T, i / 3, i % 3, js.data());
-    for (int j = 0; j < J; ++j) tangentLocal(T, js.data(), j, vs.data(), tan.data());
-    for (int lvl = 1; lvl < T.numLevels; ++lvl)
-      for (int k = T.levelStart[lvl]; k < T.levelStart[lvl + 1]; ++k) tangentCompose(T, js.data(), T.levelJoints[k], tan.data());
+    fkPasses<true, false>(HostLanes{}, T, th, js.data());
+    tangentPasses(HostLanes{}, T, js.data(), vs.data(), tan.data());
     const float* tg = rec.data() + size_t(b) * stride;
     const float* cw = cweights + size_t(b) * nc;
     for (int c = 0; c < nc; ++c) {
