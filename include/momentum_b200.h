@@ -373,6 +373,14 @@ int mb2_solver_get_plan_stats(mb2_solver* s, int64_t stats[12]);
  * [7] Cholesky diagonal tiles, [8] panel tiles, [9] updates, [10] backward substitution, [11] update + bookkeeping + write-back.
  * groups = instance groups per CTA of the persistent kernel. Any output pointer may be NULL. No reference counterpart. */
 int mb2_solver_get_fused_profile(mb2_solver* s, int32_t* fused, int32_t* groups, double* kernel_ms, uint64_t phase_cycles[12]);
+/* Which variant of the FK + residual sweep the handle last launched, for the Jacobian sweep (jacobian != 0: get_jacobian[_device],
+ * get_jtjr, the implicit direction, a solver's per-iteration Jacobian pass) or the error-only sweep (jacobian == 0: get_error,
+ * get_skeleton_state, a solver's line-search trials): [0] table staging (1 every read-only table in shared memory, 2 all but the
+ * Jacobian cells and chain-rule contributions, 0 none), [1] warps per instance (1, 2, 4 or 8), [2] instances per CTA, [3] CTAs,
+ * [4] dynamic shared memory per CTA in bytes. All zero before the first such sweep and after a sweep whose instance does not fit in
+ * shared memory (the entry that launched it failed). The fused persistent kernel runs its own sweep and records nothing here.
+ * No reference counterpart. */
+int mb2_solver_function_get_sweep_launch(mb2_solver_function* f, int32_t jacobian, int64_t out[5]);
 
 /* ---- Mixed-rig batches (BASELINE.json configs[4]): heterogeneous instances -> buckets sharing one plan -> batched solves --------
  * The reference treats a batch element by element (pymomentum/tensor_ik/tensor_ik.cpp:127-177 builds error functions, solver function

@@ -160,6 +160,7 @@ struct mb2_solver_function {
   DeviceBuffer<double> dErrors;
   DeviceBuffer<double> dJacobi;          // implicit direction: per-CTA rotation logs (and Gram matrices too large for shared memory)
   std::unique_ptr<DeviceSchedule> sched; // Cholesky schedule of the current (compact) plan
+  SweepLaunch lastSweep[2]{};            // what launchSweep last chose: [0] error-only (K4), [1] Jacobian (K1)
   FunctionTables tables() const;
 };
 
@@ -848,7 +849,7 @@ int mb2_solver_function_get_error(mb2_solver_function* f, const float* params, d
   if (rc != MB2_OK) return rc;
   const size_t n = f->ch->host.numParams;
   MB2_CUDA(cudaMemcpyAsync(f->dTheta.p, params, size_t(f->B) * n * sizeof(float), cudaMemcpyHostToDevice, f->stream));
-  MB2_CUDA(launchSweep(sweepArgs(f, f->dTheta.p, nullptr), false, f->stream));
+  MB2_CUDA(launchSweep(sweepArgs(f, f->dTheta.p, nullptr), false, f->stream, &f->lastSweep[0]));
   MB2_CUDA(cudaMemcpyAsync(errors, f->dErrors.p, size_t(f->B) * sizeof(double), cudaMemcpyDeviceToHost, f->stream));
   MB2_CUDA(cudaStreamSynchronize(f->stream));
   return MB2_OK;
@@ -862,7 +863,7 @@ int mb2_solver_function_get_jacobian(mb2_solver_function* f, const float* params
   const size_t n = f->ch->host.numParams;
   const int rows = mb2_solver_function_jacobian_rows(f);
   MB2_CUDA(cudaMemcpyAsync(f->dTheta.p, params, size_t(f->B) * n * sizeof(float), cudaMemcpyHostToDevice, f->stream));
-  MB2_CUDA(launchSweep(sweepArgs(f, f->dTheta.p, nullptr), true, f->stream));
+  MB2_CUDA(launchSweep(sweepArgs(f, f->dTheta.p, nullptr), true, f->stream, &f->lastSweep[1]));
   for (int b = 0; b < f->B && rows > 0; ++b) { // parity/debug entry point: one strided copy per instance
     const float* Jb = f->dJ.p + size_t(b) * (n + 1) * f->ldJ;
     if (jac)
@@ -885,7 +886,7 @@ int mb2_solver_function_get_jacobian_device(mb2_solver_function* f, const float*
   int rc = ensurePlan(f, 0);
   if (rc != MB2_OK) return rc;
   cudaStream_t st = stream ? (cudaStream_t)stream : f->stream;
-  MB2_CUDA(launchSweep(sweepArgs(f, params_device, nullptr), true, st));
+  MB2_CUDA(launchSweep(sweepArgs(f, params_device, nullptr), true, st, &f->lastSweep[1]));
   *jacobian_device = f->dJ.p;
   if (ld) *ld = f->ldJ;
   return MB2_OK;
@@ -905,7 +906,7 @@ int mb2_solver_function_get_jtjr(mb2_solver_function* f, const float* params, in
   const size_t hElems = size_t(f->B) * (ap + 1) * ldH;
   MB2_CUDA(f->dH.resize(hElems));
   MB2_CUDA(cudaMemcpyAsync(f->dTheta.p, params, size_t(f->B) * n * sizeof(float), cudaMemcpyHostToDevice, f->stream));
-  MB2_CUDA(launchSweep(sweepArgs(f, f->dTheta.p, nullptr), true, f->stream));
+  MB2_CUDA(launchSweep(sweepArgs(f, f->dTheta.p, nullptr), true, f->stream, &f->lastSweep[1]));
   MB2_CUDA(cudaMemsetAsync(f->dH.p, 0, hElems * sizeof(float), f->stream));
   rc = runJtJ(f, mode, ap, f->dH.p, ldH, size_t(ap + 1) * ldH, nullptr, f->stream);
   if (rc != MB2_OK) return rc;
@@ -934,7 +935,7 @@ int mb2_solver_function_get_skeleton_state(mb2_solver_function* f, const float* 
   MB2_CUDA(cudaMemcpyAsync(f->dTheta.p, params, size_t(f->B) * n * sizeof(float), cudaMemcpyHostToDevice, f->stream));
   SweepArgs a = sweepArgs(f, f->dTheta.p, nullptr);
   a.stateOut = f->dState.p;
-  MB2_CUDA(launchSweep(a, false, f->stream));
+  MB2_CUDA(launchSweep(a, false, f->stream, &f->lastSweep[0]));
   MB2_CUDA(cudaMemcpyAsync(state, f->dState.p, sz * sizeof(float), cudaMemcpyDeviceToHost, f->stream));
   MB2_CUDA(cudaStreamSynchronize(f->stream));
   return MB2_OK;
@@ -1118,7 +1119,7 @@ int mb2_solver_function_implicit_direction_device(mb2_solver_function* f, const 
   if (rc != MB2_OK) return rc;
   NvtxRange range("implicitDirection");
   cudaStream_t st = (cudaStream_t)cuda_stream;
-  MB2_CUDA(launchSweep(sweepArgs(f, parameters_device, nullptr), true, st));
+  MB2_CUDA(launchSweep(sweepArgs(f, parameters_device, nullptr), true, st, &f->lastSweep[1]));
   ImplicitDirectionArgs a{};
   a.batch = f->B;
   a.numParams = f->ch->host.numParams;
@@ -1379,7 +1380,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
     MB2_CUDA(cudaMemsetAsync(s->dActiveCount.p, 0, sizeof(int), st));
     // --- doIteration (gauss_newton_solver.cpp:224-280) ---
     recordPhaseStart(s, 0, st);
-    MB2_CUDA(launchSweep(sweepArgs(f, theta, s->dActive.p), true, st));
+    MB2_CUDA(launchSweep(sweepArgs(f, theta, s->dActive.p), true, st, &f->lastSweep[1]));
     recordPhaseStop(s, st);
     GramArgs g{};
     if (!useGramChol && !useQr) recordPhaseStart(s, 1, st);
@@ -1503,7 +1504,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
         SweepArgs ea = sweepArgs(f, theta, s->dSearching.p);
         ea.errors = s->dTrialErrors.p;
         recordPhaseStart(s, 3, st);
-        MB2_CUDA(launchSweep(ea, false, st));
+        MB2_CUDA(launchSweep(ea, false, st, &f->lastSweep[0]));
         recordPhaseStop(s, st);
         LineSearchArgs la{};
         la.batch = B; la.ns = ns; la.numParams = n; la.ldTheta = n;
@@ -1679,6 +1680,17 @@ int mb2_solver_get_fused_profile(mb2_solver* s, int32_t* fused, int32_t* groups,
       }
     }
   }
+  return MB2_OK;
+}
+
+int mb2_solver_function_get_sweep_launch(mb2_solver_function* f, int32_t jacobian, int64_t out[5]) {
+  MB2_CHECK(f != nullptr && out != nullptr, "null argument");
+  const SweepLaunch& l = f->lastSweep[jacobian ? 1 : 0];
+  out[0] = l.stageTables;
+  out[1] = l.warpsPerInstance;
+  out[2] = l.groupsPerCta;
+  out[3] = l.grid;
+  out[4] = l.smemBytes;
   return MB2_OK;
 }
 

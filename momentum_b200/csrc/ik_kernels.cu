@@ -166,8 +166,9 @@ static int g_numSms = 0;
 static int g_maxSmemOptin = 0;
 static int g_maxSmemPerSm = 0;
 
-cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream) {
+cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream, SweepLaunch* out) {
   SweepArgs a = a0;
+  if (out) *out = SweepLaunch{}; // a rejected configuration leaves an all-zero record
   const size_t budget = size_t(g_maxSmemOptin);
   // Persistent CTAs. As many instances in flight as shared memory holds next to the staged tables: all of them when they fit with at
   // least two instances, else all but the cell / contribution records (large rigs), else none. One warp per instance, up to
@@ -207,6 +208,7 @@ cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream)
   int grid = g_numSms * ctasPerSm;
   if (grid > ctasNeeded) grid = ctasNeeded;
   if (grid < 1) grid = 1;
+  if (out) *out = SweepLaunch{a.stageTables, W, groups, grid, int64_t(smem)};
   auto launch = [&](auto kernel) -> cudaError_t {
     const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     if (e != cudaSuccess) return e;

@@ -217,7 +217,15 @@ struct ImplicitDirectionConfig {
 // sizes the persistent grid (shared memory, occupancy, the scratch budget) for a.rows / a.numEnabled / a.batch
 cudaError_t implicitDirectionConfigure(const ImplicitDirectionArgs& a, ImplicitDirectionConfig& cfg);
 cudaError_t launchImplicitDirection(const ImplicitDirectionArgs& a, const ImplicitDirectionConfig& cfg, cudaStream_t stream);
-cudaError_t launchSweep(const SweepArgs& a, bool jacobian, cudaStream_t stream);
+struct SweepLaunch {         // the variant and launch shape launchSweep chose (mb2_solver_function_get_sweep_launch)
+  int32_t stageTables;       // 1 every read-only table in shared memory, 2 all but cells / contributions, 0 none
+  int32_t warpsPerInstance;  // W: 1, 2, 4 or 8
+  int32_t groupsPerCta;      // instances in flight per CTA
+  int32_t grid;              // CTAs
+  int64_t smemBytes;         // dynamic shared memory per CTA
+};
+// `out` (optional) receives the decision before the kernel is enqueued, all zero when no configuration fits
+cudaError_t launchSweep(const SweepArgs& a, bool jacobian, cudaStream_t stream, SweepLaunch* out = nullptr);
 size_t sweepSmemPerInstance(const FunctionTables& T, int warpsPerInstance);
 cudaError_t launchJtJSimt(const JtJArgs& a, cudaStream_t stream);
 cudaError_t launchCholesky(const CholArgs& a, cudaStream_t stream);

@@ -75,7 +75,7 @@ CABI_SYMBOLS = [
     "mb2_sharded_solver_shard_info", "mb2_sharded_solver_set_options", "mb2_sharded_solver_set_targets", "mb2_sharded_solver_solve", "mb2_sharded_solver_get_aggregate",
     "mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device",
     "mb2_add_orientation_error_function_instanced", "mb2_solver_function_input_gradients_device",
-    "mb2_solver_function_implicit_direction_device",
+    "mb2_solver_function_implicit_direction_device", "mb2_solver_function_get_sweep_launch",
     "mb2_character_set_skinning", "mb2_character_num_vertices", "mb2_character_skin_points_device", "mb2_character_skin_points_backward_device",
 ]
 
@@ -173,11 +173,14 @@ def load_library(path: Optional[str] = None):
     if hasattr(L, "mb2_character_skeleton_state_device"):
         L.mb2_character_skeleton_state_device.argtypes = [vp, C.c_int32, vp, vp, vp]
         L.mb2_character_skeleton_state_backward_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
-    if hasattr(L, "mb2_solver_function_input_gradients_device"):
+    if hasattr(L, "mb2_add_orientation_error_function_instanced"):
         L.mb2_add_orientation_error_function_instanced.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_int32, C.c_int32, _ip, _fp, _ip]
+    if hasattr(L, "mb2_solver_function_input_gradients_device"):
         L.mb2_solver_function_input_gradients_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
     if hasattr(L, "mb2_solver_function_implicit_direction_device"):
         L.mb2_solver_function_implicit_direction_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
+    if hasattr(L, "mb2_solver_function_get_sweep_launch"):
+        L.mb2_solver_function_get_sweep_launch.argtypes = [vp, C.c_int32, C.POINTER(C.c_int64)]
     if hasattr(L, "mb2_character_set_skinning"):
         L.mb2_character_set_skinning.argtypes = [vp, C.c_int32, _fp, _ip, _fp, _fp]
         L.mb2_character_num_vertices.argtypes = [vp]
@@ -476,6 +479,14 @@ class SkeletonSolverFunction(_Base):
         out = np.zeros((self.batch, self.character.num_joints, 8), np.float32)
         self._check(self._L.mb2_solver_function_get_skeleton_state(self._h, pp, out.ctypes.data_as(_fp)))
         return out
+
+    def get_sweep_launch(self, jacobian: bool = True) -> dict:
+        """The variant of the FK + residual sweep this handle last launched, for the Jacobian sweep or the error-only one: table
+        staging (1 all tables in shared memory, 2 all but cells / contributions, 0 none), warps per instance, instances per CTA, CTAs
+        and dynamic shared memory bytes. All zero before the first such sweep and after one whose instance did not fit."""
+        out = (C.c_int64 * 5)()
+        self._check(self._L.mb2_solver_function_get_sweep_launch(self._h, int(bool(jacobian)), out))
+        return dict(zip(("stage", "warps", "groups", "grid", "smem"), (int(v) for v in out)))
 
 
 class GaussNewtonSolver(_Base):

@@ -321,6 +321,11 @@ int mb2_add_orientation_error_function(mb2_solver_function* f, float weight, flo
   HostErrorFunction ef;
   return addBlock(f, orientationErrorFunction(f->ch->host, weight, alpha, c, rotDiff, nc, parents, offsets, weights, ef), ef, outIndex);
 }
+int mb2_add_orientation_error_function_instanced(mb2_solver_function* f, float weight, float alpha, float c, int32_t rotDiff, int32_t nc,
+                                                 const int32_t* parents, const float* weights, int32_t* outIndex) {
+  HostErrorFunction ef;
+  return addBlock(f, instancedOrientationErrorFunction(f->ch->host, weight, alpha, c, rotDiff, nc, parents, weights, ef), ef, outIndex);
+}
 int mb2_add_state_error_function(mb2_solver_function* f, float weight, int32_t rotationErrorType, float posWgt, float rotWgt, const float* posW,
                                  const float* rotW, int32_t* outIndex) {
   HostErrorFunction ef;
@@ -337,7 +342,7 @@ int mb2_set_targets(mb2_solver_function* f, int32_t index, const float* targets)
     float* dst = f->targets.data() + size_t(b) * f->host.targetStride + ef.targetOff;
     std::memcpy(dst, targets + size_t(b) * ef.targetSize, size_t(ef.targetSize) * sizeof(float));
     if (ef.kind == 1 || ef.kind == 2)
-      for (int q = 0; q < ef.numConstraints(); ++q) {
+      for (int q = 0; q < (ef.instanceOffsets ? 2 : 1) * ef.numConstraints(); ++q) { // (an instanced block: target, then offset)
         float* p = dst + 4 * q;
         const float n = sqrtf(p[0] * p[0] + p[1] * p[1] + p[2] * p[2] + p[3] * p[3]);
         p[0] /= n; p[1] /= n; p[2] /= n; p[3] /= n;
