@@ -108,7 +108,7 @@ typedef enum mb2_cholesky_mode {
  * functions, results agree to float rounding).
  *   GRAM_CHOLESKY  two launches per iteration: FK / residual / Jacobian strips, then ONE kernel that forms the stored tiles of
  *                  J^T J + lambda I from the strips on the tensor cores (a tile that would overwrite strips still being read waits in
- *                  thread-local memory), writes them over the dead strips in shared memory and runs the tile Cholesky + update on them.
+ *                  an L2-resident scratch slot), writes them over the dead strips in shared memory and runs the tile Cholesky + update on them.
  *   OFF            three launches per iteration (sweep, tile-sparse Gram to HBM, tile Cholesky).
  *   PERSISTENT     ONE launch per solve: groups of 256 threads keep an instance in shared memory for all of its iterations (FK sweep
  *                  included) and stop it on the device; no host round trip, no HBM traffic beyond theta / targets / results. Needs no
@@ -381,6 +381,16 @@ int mb2_solver_get_fused_profile(mb2_solver* s, int32_t* fused, int32_t* groups,
  * shared memory (the entry that launched it failed). The fused persistent kernel runs its own sweep and records nothing here.
  * No reference counterpart. */
 int mb2_solver_function_get_sweep_launch(mb2_solver_function* f, int32_t jacobian, int64_t out[5]);
+/* The linear-solve path the solver's last solve ran, as one host function chose it (the CPU emulator of the tests runs the same
+ * choice): [0] kind (1 JtJ + dense Eigen-structured Cholesky, 2 JtJ + tile-scheduled Cholesky, 3 tile-sparse Gram + tile Cholesky
+ * in two launches, 4 Gram + Cholesky in one launch, 5 the persistent kernel, 6 QR, 7 trust-region QR), [1] plan mode (1 compact
+ * columns, 2 tile schedule), [2] dense tile pattern, [3] Jacobian in strips, [4] mb2_jtj_mode after AUTO, [5] dense Cholesky block
+ * size NB, [6] its matrix in shared memory, [7] / [8] threads of the Gram / tile Cholesky kernels (256 or 512), [9] Jacobian rows
+ * the QR kernels fold at once (the limit), [10] QR row chunks, [11] rows of the widest chunk, [12] floats of the trust-region R kept
+ * per instance, [13] instance groups per CTA of the persistent kernel (any plan with strips), [14] its dynamic shared memory in
+ * bytes. All zero before the first solve and after a refused solve (by its options, or no resident Gram + Cholesky CTA); a CUDA error
+ * later in a solve leaves the path it had chosen. No reference counterpart. */
+int mb2_solver_get_solve_path(mb2_solver* s, int64_t out[15]);
 
 /* ---- Mixed-rig batches (BASELINE.json configs[4]): heterogeneous instances -> buckets sharing one plan -> batched solves --------
  * The reference treats a batch element by element (pymomentum/tensor_ik/tensor_ik.cpp:127-177 builds error functions, solver function

@@ -21,6 +21,7 @@
 #include "ik_jtj_tc.cuh"
 #include "ik_kernels.cuh"
 #include "ik_plan.h"
+#include "ik_solve_path.h"
 
 using namespace mb2;
 
@@ -133,7 +134,7 @@ struct DeviceSchedule {
   // fused persistent kernel (ik_fused.cuh): every table of the plan as one blob + how many instance groups fit beside it
   DeviceBuffer<int32_t> fBlob;
   FusedBlobLayout fLayout{};
-  FusedConfig fConfig{};
+  int fusedGroups{0}; // SolvePath::fused of the solve that requested this plan
 };
 
 struct mb2_solver_function {
@@ -178,8 +179,7 @@ struct mb2_solver {
   DeviceBuffer<unsigned long long> dPhaseCycles;
   DeviceBuffer<float> dPark;          // gramCholeskyKernel: parked Gram tiles, one slot per resident CTA
   DeviceBuffer<uint32_t> dParkSlots;  // its slot bitmap (zero between launches)
-  bool lastFused{false}, lastGramChol{false};
-  int lastFusedGroups{0};
+  SolvePath path; // what the last solve ran (chooseSolvePath)
   cudaEvent_t fusedStart{nullptr}, fusedStop{nullptr};
   double fusedMs{0};
   int* hActiveCount{nullptr}; // pinned
@@ -300,44 +300,6 @@ int uploadWeights(mb2_solver_function* f) {
   return MB2_OK;
 }
 
-// Every table the fused kernel walks, as one 16-byte-aligned blob (bulk-copied into shared memory once per CTA).
-int buildFusedBlob(mb2_solver_function* f, DeviceSchedule& ds, const std::vector<int32_t>& gramBlob, const std::vector<int32_t>& schedBlob, cudaStream_t s) {
-  std::vector<int32_t> blob;
-  auto add = [&](const void* data, size_t bytes) {
-    const int32_t off = int32_t(blob.size());
-    const size_t words = (bytes + 3) / 4;
-    blob.resize(blob.size() + words, 0);
-    if (bytes) std::memcpy(blob.data() + off, data, bytes);
-    while (blob.size() % 4) blob.push_back(0);
-    return off;
-  };
-  const HostCharacter& h = f->ch->host;
-  const Plan& p = f->plan;
-  FusedBlobLayout& L = ds.fLayout;
-  L.parent = add(h.parent.data(), h.parent.size() * 4);
-  L.offset = add(h.offset.data(), h.offset.size() * 4);
-  L.prerot = add(h.prerot.data(), h.prerot.size() * 4);
-  L.ptOuter = add(h.ptOuter.data(), h.ptOuter.size() * 4);
-  L.ptInner = add(h.ptInner.data(), h.ptInner.size() * 4);
-  L.ptVals = add(h.ptVals.data(), h.ptVals.size() * 4);
-  L.ptOffsets = add(h.ptOffsets.data(), h.ptOffsets.size() * 4);
-  L.levelStart = add(h.levelStart.data(), h.levelStart.size() * 4);
-  L.levelJoints = add(h.levelJoints.data(), h.levelJoints.size() * 4);
-  L.efs = add(p.efs.data(), p.efs.size() * sizeof(EfDesc));
-  L.units = add(p.units.data(), p.units.size() * sizeof(UnitDesc));
-  L.cells = add(p.cells.data(), p.cells.size() * sizeof(CellDesc));
-  L.contribs = add(p.contribs.data(), p.contribs.size() * sizeof(ContribDesc));
-  L.limitData = add(p.limitData.data(), p.limitData.size() * 4);
-  L.cols = add(p.deviceCols.data(), p.deviceCols.size() * 4);
-  L.gram = add(gramBlob.data(), gramBlob.size() * 4);
-  L.sched = add(schedBlob.data(), schedBlob.size() * 4);
-  if (blob.empty()) blob.push_back(0);
-  while (blob.size() % 4) blob.push_back(0);
-  L.words = int32_t(blob.size());
-  MB2_CUDA(ds.fBlob.upload(blob, s));
-  return MB2_OK;
-}
-
 // mode 0: every column at its model-parameter index (getJacobian / getJtJR parity);
 // mode 1: solver, only the enabled columns, ascending (dense Eigen-structured Cholesky);
 // mode 2: solver, enabled columns in the Cholesky elimination order + tile schedule (schedDense: dense pattern).
@@ -379,8 +341,7 @@ int ensurePlan(mb2_solver_function* f, int mode, bool schedDense = false, bool a
       } else if (ds->gcValid) {
         MB2_CUDA(ds->gcTab.upload(ds->gc.tab, s));
       }
-      const int rc = buildFusedBlob(f, *ds, gblob, sblob, s);
-      if (rc != MB2_OK) return rc;
+      MB2_CUDA(ds->fBlob.upload(makeFusedBlob(f->ch->host, f->plan, gblob, sblob, ds->fLayout), s));
     }
     f->sched = std::move(ds);
   }
@@ -410,12 +371,6 @@ int ensurePlan(mb2_solver_function* f, int mode, bool schedDense = false, bool a
   if (rc != MB2_OK) return rc;
   rc = uploadWeights(f);
   if (rc != MB2_OK) return rc;
-  if (stripLayout) {
-    int dev = 0, optin = 0;
-    MB2_CUDA(cudaGetDevice(&dev));
-    MB2_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    f->sched->fConfig = fusedConfigure(f->tables(), f->sched->fLayout, f->sched->dev, f->sched->gram.stride, int(f->sched->gram.tileOrder.size()) / kGramWarps, optin);
-  }
   // Plan tables, schedule / Gram blobs, weights and the Jacobian zero fill were issued on the handle's stream; the solve may run on a
   // caller's stream. A plan build is a rare host-side event: wait for it here instead of threading events through every launch.
   MB2_CUDA(cudaStreamSynchronize(s));
@@ -496,13 +451,6 @@ __global__ void finalizeKernel(int batch, int n, float* theta, const float* thet
     for (int i = threadIdx.x; i < n; i += blockDim.x) theta[size_t(b) * n + i] = theta0[size_t(b) * n + i];
     if (threadIdx.x == 0) status[b] = MB2_INSTANCE_NON_FINITE;
   }
-}
-
-int resolveJtjMode(const mb2_solver_function* f, int requested, int ns) {
-  if (requested == MB2_JTJ_FP32_SIMT) return MB2_JTJ_FP32_SIMT;
-  const bool ok = jtjTensorSupported(ns, f->plan.numCols, f->ldJ);
-  if (requested == MB2_JTJ_AUTO) return ok ? MB2_JTJ_TF32X3 : MB2_JTJ_FP32_SIMT;
-  return ok ? requested : -1;
 }
 
 int runJtJ(mb2_solver_function* f, int mode, int ns, float* H, int ldH, size_t hStride, const int32_t* active, cudaStream_t st, float* g = nullptr, int ldG = 0) {
@@ -900,7 +848,7 @@ int mb2_solver_function_get_jtjr(mb2_solver_function* f, const float* params, in
   const size_t n = f->ch->host.numParams;
   const int ap = f->plan.actualParameters;
   MB2_CHECK(ap > 0, "no enabled parameters");
-  const int mode = resolveJtjMode(f, jtjMode, ap);
+  const int mode = resolveJtjMode(jtjMode, jtjTensorSupported(ap, f->plan.numCols, f->ldJ));
   if (mode < 0) return fail(MB2_ERR_UNSUPPORTED, "tensor-core JtJ does not support this shape");
   const int ldH = roundUp(ap + 1, 16);
   const size_t hElems = size_t(f->B) * (ap + 1) * ldH;
@@ -1174,193 +1122,53 @@ int mb2_solver_set_profiling(mb2_solver* s, int32_t enabled) {
   return MB2_OK;
 }
 
+namespace {
+// the figures chooseSolvePath weighs, of the plan ensurePlan builds (or keeps) for a request
+int planFigures(mb2_solver_function* f, int mode, bool schedDense, bool strips, PlanFigures& F, std::string& msg) {
+  const int rc = ensurePlan(f, mode, schedDense, strips);
+  if (rc != MB2_OK) { msg = g_lastError; return rc; }
+  F = PlanFigures{};
+  F.numCols = f->plan.numCols;
+  F.recStride = f->plan.recStride;
+  F.jtjTensor = jtjTensorSupported(F.numCols, F.numCols, f->ldJ);
+  if (const DeviceSchedule* ds = f->planMode == 2 ? f->sched.get() : nullptr) {
+    F.nPad = ds->host.nPad;
+    F.numTiles = ds->host.numTiles;
+    F.schedBlobInts = ds->dev.blobInts;
+    F.stripStride = ds->gram.stride;
+    F.gramBlobInts = ds->gBlobInts;
+    F.orderEntries = int(ds->gram.tileOrder.size());
+    F.gramCholValid = ds->gcValid;
+    F.fusedBlobWords = ds->fLayout.words;
+  }
+  return MB2_OK;
+}
+
+} // namespace
+
 int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   MB2_CHECK(s != nullptr && theta != nullptr, "null argument");
   mb2_solver_function* f = s->fn;
   MB2_DEVICE_GUARD(f->ch->device);
   NvtxRange nvtxSolve("mb2::SolverT::solve");
   const mb2_gauss_newton_options& o = s->opt;
-  // Cholesky path: 0 auto, 1 dense Eigen-structured kernel, 2 tile schedule on the dense pattern, 3 tile schedule on the sparse pattern
-  int cholMode = resolveCholeskyMode(o.cholesky_mode, f->host.enabled);
-  // GaussNewtonSolverQRT's step: Householder QR of the K-major Jacobian (ik_qr.cuh); TrustRegionQRT's iteration builds on the same fold (ik_tr_qr.cuh)
-  const bool useTr = o.linear_solver == MB2_LINEAR_SOLVER_TRUST_REGION_QR;
-  const bool useQr = o.linear_solver == MB2_LINEAR_SOLVER_QR || useTr;
-  if (useTr && !(o.trust_region_radius > 0.f)) return fail(MB2_ERR_INVALID_ARGUMENT, "trust_region_radius must be positive");
-  if (useQr) {
-    if (o.jtj_mode == MB2_JTJ_SPARSE_TILES || o.cholesky_mode >= 2 || o.fused_mode >= MB2_FUSED_PERSISTENT)
-      return fail(MB2_ERR_UNSUPPORTED, "the QR step works on the dense Jacobian: it excludes the tile-sparse Gram, the tile Cholesky and the fused kernels");
-    cholMode = 1;
+  const DeviceLimits lim = deviceLimits();
+  std::string msg;
+  const PlanFiguresFn plan = [f](int mode, bool schedDense, bool strips, PlanFigures& F, std::string& m) { return planFigures(f, mode, schedDense, strips, F, m); };
+  int rc = chooseSolvePath(o, f->B, f->ch->host, f->host, plan, lim, s->path, msg);
+  if (s->path.planMode != 0 && f->sched) f->sched->fusedGroups = s->path.fused.groups;
+  if (rc != MB2_OK) {
+    s->path = SolvePath{};
+    return fail(rc, msg);
   }
-  // tile-sparse Gram: default whenever the tile-scheduled Cholesky runs (MB2_JTJ_AUTO), or on request
-  bool useGram = cholMode >= 2 && (o.jtj_mode == MB2_JTJ_AUTO || o.jtj_mode == MB2_JTJ_SPARSE_TILES);
-  if (o.jtj_mode == MB2_JTJ_SPARSE_TILES && cholMode < 2) return fail(MB2_ERR_UNSUPPORTED, "MB2_JTJ_SPARSE_TILES needs the tile-scheduled Cholesky");
-  int rc = ensurePlan(f, cholMode >= 2 ? 2 : 1, cholMode == 2, useGram);
-  if (rc != MB2_OK) return rc;
-  bool useSchedule = cholMode >= 2;
-  if (useSchedule && choleskyScheduledSmemBytes(f->plan.numCols, f->sched->host.nPad, f->sched->host.numTiles, f->sched->dev.blobInts) > size_t(200 * 1024)) {
-    if (o.cholesky_mode >= 2) return fail(MB2_ERR_UNSUPPORTED, "tile schedule does not fit in shared memory for this system");
-    useSchedule = false; // fall back to the dense kernel (matrix in global memory)
-    useGram = false;
-    rc = ensurePlan(f, 1);
-    if (rc != MB2_OK) return rc;
-  }
+  const SolvePath& P = s->path;
   cudaStream_t st = cudaStream ? (cudaStream_t)cudaStream : f->stream;
   const int B = f->B, n = f->ch->host.numParams;
   const int ns = f->plan.numCols;
   const int maxIt = int(std::min<uint64_t>(o.max_iterations, 1u << 30));
   const int minIt = int(std::min<uint64_t>(o.min_iterations, 1u << 30));
-  MB2_CHECK(ns > 0, "no enabled parameters");
-  if (useGram && gramTilesSmemBytes(size_t(f->sched->gram.stride), f->sched->gBlobInts) > size_t(200 * 1024)) {
-    if (o.jtj_mode == MB2_JTJ_SPARSE_TILES) return fail(MB2_ERR_UNSUPPORTED, "Jacobian strips do not fit in shared memory for this system");
-    useGram = false;
-    rc = ensurePlan(f, 2, cholMode == 2, false);
-    if (rc != MB2_OK) return rc;
-  }
-  // ---- fused persistent kernel: the whole solve in one launch (ik_fused.cuh) ----
-  s->lastFused = false;
-  {
-    const bool eligible = useGram && useSchedule && o.do_line_search == 0 && f->sched->fConfig.groups >= 1 && f->sched->fBlob.p != nullptr;
-    if (o.fused_mode == MB2_FUSED_PERSISTENT && !eligible)
-      return fail(MB2_ERR_UNSUPPORTED, "the fused kernel needs the tile-sparse Gram + tile-scheduled Cholesky path, no line search, and a plan that fits in shared memory");
-    // AUTO takes the persistent kernel when the whole batch is one wave of instance groups: a single launch with no host round trip
-    // saves ~2 launches per iteration there (H100 80GB HBM3 at 400 W, 256 x humanoid72 x 10 iterations: 0.68 - 0.71 vs 0.83 ms); at
-    // thousands of instances the per-iteration kernels keep more instances in flight per SM (the persistent kernel holds at most three)
-    // and AUTO keeps them (8192 instances: 13.0 vs 9.8 - 9.9 ms)
-    int smCount = 0;
-    if (eligible && o.fused_mode == MB2_FUSED_AUTO) {
-      int dev0 = 0;
-      MB2_CUDA(cudaGetDevice(&dev0));
-      MB2_CUDA(cudaDeviceGetAttribute(&smCount, cudaDevAttrMultiProcessorCount, dev0));
-    }
-    const bool oneWave = eligible && o.fused_mode == MB2_FUSED_AUTO && B <= f->sched->fConfig.groups * smCount;
-    if ((o.fused_mode == MB2_FUSED_PERSISTENT || oneWave) && eligible) {
-      const DeviceSchedule& ds = *f->sched;
-      MB2_CUDA(s->dIterations.resize(B));
-      MB2_CUDA(s->dStatus.resize(B));
-      MB2_CUDA(s->dWorkCounter.resize(1));
-      MB2_CUDA(cudaMemsetAsync(s->dWorkCounter.p, 0, sizeof(int32_t), st));
-      if (o.store_error_history) {
-        MB2_CUDA(s->dHistory.resize(size_t(B) * std::max(maxIt, 1)));
-        MB2_CUDA(cudaMemsetAsync(s->dHistory.p, 0, size_t(B) * std::max(maxIt, 1) * sizeof(double), st));
-        s->historyStride = size_t(std::max(maxIt, 1));
-      }
-      FusedArgs fa{};
-      fa.batch = B;
-      fa.T = f->tables();
-      fa.blob = ds.fBlob.p;
-      fa.L = ds.fLayout;
-      fa.S = ds.dev;
-      fa.schedGlobal = ds.dev.blob;
-      for (int k = 0; k < 8; ++k) fa.gramOff[k] = ds.gOffsets[k];
-      fa.numStrips = ds.gram.numStrips;
-      fa.stripStride = ds.gram.stride;
-      fa.residOff = ds.gram.residOff;
-      fa.numOrder = int32_t(ds.gram.tileOrder.size());
-      fa.regularization = o.regularization;
-      fa.threshold = o.threshold;
-      fa.minIterations = minIt;
-      fa.maxIterations = maxIt;
-      fa.theta = theta;
-      fa.ldTheta = n;
-      fa.targets = f->dTargets.p;
-      fa.cweights = f->dWeights.p;
-      fa.errors = f->dErrors.p;
-      fa.iterations = s->dIterations.p;
-      fa.status = s->dStatus.p;
-      fa.history = o.store_error_history ? s->dHistory.p : nullptr;
-      fa.workCounter = s->dWorkCounter.p;
-      fa.phaseCycles = nullptr;
-      if (s->profiling) {
-        MB2_CUDA(s->dPhaseCycles.resize(16));
-        MB2_CUDA(cudaMemsetAsync(s->dPhaseCycles.p, 0, 16 * sizeof(unsigned long long), st));
-        fa.phaseCycles = s->inKernelProfile ? s->dPhaseCycles.p : nullptr;
-        if (!s->fusedStart) { MB2_CUDA(cudaEventCreate(&s->fusedStart)); MB2_CUDA(cudaEventCreate(&s->fusedStop)); }
-        MB2_CUDA(cudaEventRecord(s->fusedStart, st));
-      }
-      int dev = 0, sms = 0;
-      MB2_CUDA(cudaGetDevice(&dev));
-      MB2_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-      {
-        NvtxRange nvtxIt("mb2::fusedSolveKernel (GaussNewtonSolverT::doIteration x maxIterations)");
-        MB2_CUDA(launchFusedSolve(fa, ds.fConfig, sms, s->inKernelProfile, st));
-      }
-      if (s->profiling) MB2_CUDA(cudaEventRecord(s->fusedStop, st));
-      for (auto& e : s->events) { cudaEventDestroy(e.start); cudaEventDestroy(e.stop); }
-      s->events.clear();
-      s->kernelLaunches = 1;
-      s->lastFused = true;
-      s->lastFusedGroups = ds.fConfig.groups;
-      return MB2_OK;
-    }
-  }
-  // ---- Gram + Cholesky in one launch per iteration (gramCholeskyKernel): the default on the tile path ----
-  bool useGramChol = false;
-  if (useGram && useSchedule) {
-    const DeviceSchedule& ds = *f->sched;
-    const int rounds = std::max(int(ds.gram.tileOrder.size()) / kGramWarps, 1);
-    const bool fits = gramCholeskySmemBytes(size_t(ds.gram.stride), ds.gBlobInts, ns, ds.host.nPad, ds.host.numTiles, ds.dev.blobInts) <= size_t(200 * 1024) && rounds <= kGramCholMaxRounds &&
-                      ds.gcValid;
-    if (o.fused_mode == MB2_FUSED_GRAM_CHOLESKY && !fits) return fail(MB2_ERR_UNSUPPORTED, "Gram + Cholesky fusion: strips / tiles of this plan do not fit in shared memory, or too many tiles per warp");
-    useGramChol = fits && (o.fused_mode == MB2_FUSED_AUTO || o.fused_mode == MB2_FUSED_GRAM_CHOLESKY);
-  } else if (o.fused_mode == MB2_FUSED_GRAM_CHOLESKY) {
-    return fail(MB2_ERR_UNSUPPORTED, "Gram + Cholesky fusion needs the tile-sparse Gram + tile-scheduled Cholesky path");
-  }
-  s->lastGramChol = useGramChol;
-  if (useGramChol && s->profiling) {
-    MB2_CUDA(s->dPhaseCycles.resize(16));
-    MB2_CUDA(cudaMemsetAsync(s->dPhaseCycles.p, 0, 16 * sizeof(unsigned long long), st));
-  }
-  const int mode = useGram ? MB2_JTJ_SPARSE_TILES : resolveJtjMode(f, o.jtj_mode == MB2_JTJ_SPARSE_TILES ? MB2_JTJ_AUTO : o.jtj_mode, ns);
-  if (mode < 0) return fail(MB2_ERR_UNSUPPORTED, "tensor-core JtJ does not support this shape");
-  // normal equations: full symmetric [ns+1][ldH] in device-column order (row/column ns = J^T r)
-  const int ldH = roundUp(ns + 1, 16);
-  const size_t hStride = size_t(ns + 1) * ldH;
-  if (!useGram && !useQr) MB2_CUDA(s->dH.resize(size_t(B) * hStride));
-  int qrMaxRows = 0, qrChunks = 0;
-  if (useQr) { // row chunks: one per error-function block (the reference adds block by block), split when a block does not fit beside R
-    qrMaxRows = qrMaxChunkRows(ns, size_t(200 * 1024));
-    if (qrMaxRows < 8) return fail(MB2_ERR_UNSUPPORTED, "the QR step keeps R in shared memory: too many enabled parameters for this kernel");
-    if (useTr) { // R and the damping rows D (both packed triangles) + the in-kernel getError scratch; the Jacobian chunk shares D's storage
-      qrMaxRows = std::min(qrMaxRows, std::max(8, ns / 2));
-      if (trQrSmemFloats(ns, n, f->ch->host.numJoints, qrMaxRows) * sizeof(float) > size_t(220 * 1024))
-        return fail(MB2_ERR_UNSUPPORTED, "the trust-region QR kernel keeps R and the damping rows in shared memory: too many enabled parameters / joints");
-    }
-    std::vector<int32_t> starts{0};
-    int r0 = 0, widest = 0;
-    for (const auto& ef : f->host.efs) {
-      if (!(ef.weight > 0.f)) continue;
-      const int size = jacobianBlockSize(f->ch->host, ef);
-      for (int done = 0; done < size; done += qrMaxRows) { const int p = std::min(qrMaxRows, size - done); starts.push_back(r0 + done + p); widest = std::max(widest, p); }
-      r0 += size;
-    }
-    qrChunks = int(starts.size()) - 1;
-    qrMaxRows = std::max(widest, 1);
-    MB2_CUDA(s->dQrChunks.upload(starts, st));
-    if (useTr) { // TrustRegionQRT::initializeSolver (trust_region_qr.cpp:38-40): the current radius starts at the option's value
-      MB2_CUDA(s->dRadius.upload(std::vector<float>(size_t(B), o.trust_region_radius), st));
-      MB2_CUDA(s->dRSaved.resize(size_t(B) * ((size_t(ns) * (ns + 1) / 2 + 3) & ~size_t(3))));
-    }
-  }
-  float* Hbuf = s->dH.p;
-  const size_t tilesStride = useGram ? size_t(f->sched->host.numTiles) * 256 + f->sched->host.nPad : 0;
-  if (useGram && !(o.fused_mode == MB2_FUSED_AUTO || o.fused_mode == MB2_FUSED_GRAM_CHOLESKY)) MB2_CUDA(s->dTiles.resize(size_t(B) * tilesStride));
-  const int ldG = cholGradientLd(ns);
-  MB2_CUDA(s->dGrad.resize(size_t(B) * ldG));
-  MB2_CUDA(s->dDelta.resize(size_t(B) * ns));
-  MB2_CUDA(s->dTheta0.resize(size_t(B) * n));
-  MB2_CUDA(s->dLastErrors.resize(B));
-  MB2_CUDA(s->dActive.resize(B));
   MB2_CUDA(s->dIterations.resize(B));
   MB2_CUDA(s->dStatus.resize(B));
-  MB2_CUDA(s->dActiveCount.resize(1));
-  const bool lineSearch = o.do_line_search != 0 && !useTr; // (TrustRegionQRT has no line search: steps are accepted or rejected by rho)
-  if (lineSearch) {
-    MB2_CUDA(s->dThetaOrig.resize(size_t(B) * n));
-    MB2_CUDA(s->dTrialErrors.resize(B));
-    MB2_CUDA(s->dScale.resize(B));
-    MB2_CUDA(s->dSearching.resize(B));
-    MB2_CUDA(s->dGradDotDelta.resize(B));
-  }
   if (o.store_error_history) {
     MB2_CUDA(s->dHistory.resize(size_t(B) * std::max(maxIt, 1)));
     MB2_CUDA(cudaMemsetAsync(s->dHistory.p, 0, size_t(B) * std::max(maxIt, 1) * sizeof(double), st));
@@ -1368,8 +1176,193 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   }
   for (auto& e : s->events) { cudaEventDestroy(e.start); cudaEventDestroy(e.stop); }
   s->events.clear();
-  s->kernelLaunches = 0;
+  if (s->profiling && (P.kind == kSolvePersistent || P.kind == kSolveGramCholesky)) {
+    MB2_CUDA(s->dPhaseCycles.resize(16));
+    MB2_CUDA(cudaMemsetAsync(s->dPhaseCycles.p, 0, 16 * sizeof(unsigned long long), st));
+  }
+  if (P.kind == kSolvePersistent) { // the whole solve in one launch
+    const DeviceSchedule& ds = *f->sched;
+    MB2_CUDA(s->dWorkCounter.resize(1));
+    MB2_CUDA(cudaMemsetAsync(s->dWorkCounter.p, 0, sizeof(int32_t), st));
+    FusedArgs fa{};
+    fa.batch = B;
+    fa.T = f->tables();
+    fa.blob = ds.fBlob.p;
+    fa.L = ds.fLayout;
+    fa.S = ds.dev;
+    fa.schedGlobal = ds.dev.blob;
+    for (int k = 0; k < 8; ++k) fa.gramOff[k] = ds.gOffsets[k];
+    fa.numStrips = ds.gram.numStrips;
+    fa.stripStride = ds.gram.stride;
+    fa.residOff = ds.gram.residOff;
+    fa.numOrder = int32_t(ds.gram.tileOrder.size());
+    fa.regularization = o.regularization;
+    fa.threshold = o.threshold;
+    fa.minIterations = minIt;
+    fa.maxIterations = maxIt;
+    fa.theta = theta;
+    fa.ldTheta = n;
+    fa.targets = f->dTargets.p;
+    fa.cweights = f->dWeights.p;
+    fa.errors = f->dErrors.p;
+    fa.iterations = s->dIterations.p;
+    fa.status = s->dStatus.p;
+    fa.history = o.store_error_history ? s->dHistory.p : nullptr;
+    fa.workCounter = s->dWorkCounter.p;
+    fa.phaseCycles = s->inKernelProfile ? s->dPhaseCycles.p : nullptr;
+    if (s->profiling) {
+      if (!s->fusedStart) { MB2_CUDA(cudaEventCreate(&s->fusedStart)); MB2_CUDA(cudaEventCreate(&s->fusedStop)); }
+      MB2_CUDA(cudaEventRecord(s->fusedStart, st));
+    }
+    {
+      NvtxRange nvtxIt("mb2::fusedSolveKernel (GaussNewtonSolverT::doIteration x maxIterations)");
+      MB2_CUDA(launchFusedSolve(fa, P.fused, lim.numSms, s->inKernelProfile, st));
+    }
+    if (s->profiling) MB2_CUDA(cudaEventRecord(s->fusedStop, st));
+    s->kernelLaunches = 1;
+    return MB2_OK;
+  }
+  // normal equations of the JtJ kernels: full symmetric [ns+1][ldH] in device-column order (row/column ns = J^T r)
+  const int ldH = roundUp(ns + 1, 16);
+  const size_t hStride = size_t(ns + 1) * ldH;
+  if (P.kind == kSolveDense || P.kind == kSolveTilesKMajor) MB2_CUDA(s->dH.resize(size_t(B) * hStride));
+  const size_t tilesStride = P.strips ? size_t(f->sched->host.numTiles) * 256 + f->sched->host.nPad : 0;
+  if (P.kind == kSolveTiles) MB2_CUDA(s->dTiles.resize(size_t(B) * tilesStride));
+  const bool qr = P.kind == kSolveQr || P.kind == kSolveTrustRegionQr;
+  if (qr) MB2_CUDA(s->dQrChunks.upload(P.qrChunkStarts, st));
+  if (P.kind == kSolveTrustRegionQr) { // TrustRegionQRT::initializeSolver (trust_region_qr.cpp:38-40): the current radius starts at the option's value
+    MB2_CUDA(s->dRadius.upload(std::vector<float>(size_t(B), o.trust_region_radius), st));
+    MB2_CUDA(s->dRSaved.resize(size_t(B) * P.trRSavedFloats));
+  }
+  const int ldG = cholGradientLd(ns);
+  MB2_CUDA(s->dGrad.resize(size_t(B) * ldG));
+  MB2_CUDA(s->dDelta.resize(size_t(B) * ns));
+  MB2_CUDA(s->dTheta0.resize(size_t(B) * n));
+  MB2_CUDA(s->dLastErrors.resize(B));
+  MB2_CUDA(s->dActive.resize(B));
+  MB2_CUDA(s->dActiveCount.resize(1));
+  const bool lineSearch = o.do_line_search != 0 && P.kind != kSolveTrustRegionQr; // (TrustRegionQRT has no line search: steps are accepted or rejected by rho)
+  if (lineSearch) {
+    MB2_CUDA(s->dThetaOrig.resize(size_t(B) * n));
+    MB2_CUDA(s->dTrialErrors.resize(B));
+    MB2_CUDA(s->dScale.resize(B));
+    MB2_CUDA(s->dSearching.resize(B));
+    MB2_CUDA(s->dGradDotDelta.resize(B));
+  }
+  double* history = o.store_error_history ? s->dHistory.p : nullptr;
 
+  // ---- kernel arguments: only the iteration changes from one iteration to the next ----
+  const SweepArgs sweep = sweepArgs(f, theta, s->dActive.p);
+  GramArgs g{};
+  if (P.strips) {
+    const DeviceSchedule& ds = *f->sched;
+    g.batch = B;
+    g.strips = f->dJ.p;
+    g.stripStride = size_t(ds.gram.stride);
+    g.residOff = ds.gram.residOff;
+    g.active = s->dActive.p;
+    g.numStrips = ds.gram.numStrips;
+    g.numTiles = ds.host.numTiles;
+    g.numTileCols = ds.host.numTileCols;
+    g.nPad = ds.host.nPad;
+    g.numOrder = int32_t(ds.gram.tileOrder.size());
+    g.blob = ds.gBlob.p;
+    g.blobInts = ds.gBlobInts;
+    g.offTileOrder = ds.gOffsets[0]; g.offTilePairStart = ds.gOffsets[1]; g.offPairA = ds.gOffsets[2]; g.offPairB = ds.gOffsets[3];
+    g.offColStripStart = ds.gOffsets[4]; g.offColStrip = ds.gOffsets[5]; g.offStripRow = ds.gOffsets[6]; g.offTileInfo = ds.gOffsets[7];
+    g.regularization = o.regularization;
+    g.out = s->dTiles.p;
+    g.outStride = tilesStride;
+  }
+  CholArgs c{};
+  c.batch = B;
+  c.H = s->dH.p;
+  c.ns = ns;
+  c.ldH = ldH;
+  c.hStride = hStride;
+  c.regularization = o.regularization;
+  c.cols = f->dDeviceCols.p;
+  c.theta = theta;
+  c.ldTheta = n;
+  c.delta = s->dDelta.p;
+  c.applyUpdate = lineSearch ? 0 : 1;
+  c.errors = f->dErrors.p;
+  c.lastErrors = s->dLastErrors.p;
+  c.active = s->dActive.p;
+  c.iterations = s->dIterations.p;
+  c.status = s->dStatus.p;
+  c.history = history;
+  c.minIterations = minIt;
+  c.maxIterations = maxIt;
+  c.threshold = o.threshold;
+  c.activeCount = s->dActiveCount.p;
+  c.bookkeeping = lineSearch ? 0 : 1;
+  c.gradDotDelta = lineSearch ? s->dGradDotDelta.p : nullptr;
+  c.g = s->dGrad.p;
+  c.ldG = ldG;
+  c.tilesIn = P.strips ? s->dTiles.p : nullptr;
+  c.tilesStride = tilesStride;
+  TrQrArgs t{};
+  t.q.c = c;
+  t.q.jacobian = f->dJ.p;
+  t.q.numCols = f->plan.numCols;
+  t.q.ldJ = f->ldJ;
+  t.q.chunkStart = s->dQrChunks.p;
+  t.q.numChunks = int32_t(P.qrChunkStarts.size()) - 1;
+  t.T = f->tables();
+  t.targets = f->dTargets.p;
+  t.cweights = f->dWeights.p;
+  t.radius = s->dRadius.p;
+  t.rSaved = s->dRSaved.p;
+  t.maxRadius = 10.f; // trust_region_qr.h:73
+  t.maxChunkRows = P.qrWidestChunk;
+  GramCholArgs gc{};
+  gc.g = g;
+  gc.c = c;
+  gc.c.tilesIn = nullptr;
+  gc.phaseCycles = s->inKernelProfile ? s->dPhaseCycles.p : nullptr;
+  GramCholGlobalTables gt{};
+  if (P.kind == kSolveGramCholesky) {
+    const DeviceSchedule& ds = *f->sched;
+    gc.parkTiles = ds.gc.parkTiles;
+    if (gc.parkTiles > 0) {
+      const int slots = gramCholeskyParkSlots(gc, ds.dev, ds.gcParams != nullptr);
+      if (slots < 1) {
+        s->path = SolvePath{};
+        return fail(MB2_ERR_CUDA, "Gram + Cholesky fusion: no resident CTA");
+      }
+      if (s->dParkSlots.n < size_t(slots / 32)) { // grown only here, and every launch leaves it all zero
+        MB2_CUDA(s->dParkSlots.resize(size_t(slots / 32)));
+        MB2_CUDA(cudaMemsetAsync(s->dParkSlots.p, 0, s->dParkSlots.n * sizeof(uint32_t), st));
+      }
+      MB2_CUDA(s->dPark.resize(size_t(slots) * size_t(gc.parkTiles) * 256));
+      gc.park = s->dPark.p;
+      gc.parkSlots = s->dParkSlots.p;
+      gc.parkSlotWords = int32_t(slots / 32);
+    }
+    gt.L = ds.gc.L;
+    gt.tab = ds.gcTab.p;
+  }
+  CholArgs& step = qr ? t.q.c : (P.kind == kSolveGramCholesky ? gc.c : c); // the arguments of the linear-solve launch
+  SweepArgs trial = sweepArgs(f, theta, s->dSearching.p);
+  trial.errors = s->dTrialErrors.p;
+  LineSearchArgs la{};
+  la.batch = B; la.ns = ns; la.numParams = n; la.ldTheta = n;
+  la.errors = f->dErrors.p;
+  la.trialErrors = s->dTrialErrors.p;
+  la.gradDotDelta = s->dGradDotDelta.p;
+  la.scale = s->dScale.p;
+  la.searching = s->dSearching.p;
+  la.subsetVariant = o.subset_line_search;
+  la.active = s->dActive.p;
+  BookkeepingArgs ba{};
+  ba.batch = B;
+  ba.errors = f->dErrors.p; ba.lastErrors = s->dLastErrors.p; ba.active = s->dActive.p; ba.iterations = s->dIterations.p;
+  ba.status = s->dStatus.p; ba.history = history;
+  ba.theta = theta; ba.ldTheta = n; ba.numParams = n;
+  ba.minIterations = minIt; ba.maxIterations = maxIt; ba.threshold = o.threshold; ba.activeCount = s->dActiveCount.p;
+
+  s->kernelLaunches = 0;
   initSolveStateKernel<<<(B + 127) / 128, 128, 0, st>>>(B, s->dActive.p, s->dIterations.p, s->dStatus.p, s->dLastErrors.p, f->dErrors.p);
   MB2_CUDA(cudaGetLastError());
   MB2_CUDA(cudaMemcpyAsync(s->dTheta0.p, theta, size_t(B) * n * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -1380,151 +1373,49 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
     MB2_CUDA(cudaMemsetAsync(s->dActiveCount.p, 0, sizeof(int), st));
     // --- doIteration (gauss_newton_solver.cpp:224-280) ---
     recordPhaseStart(s, 0, st);
-    MB2_CUDA(launchSweep(sweepArgs(f, theta, s->dActive.p), true, st, &f->lastSweep[1]));
+    MB2_CUDA(launchSweep(sweep, true, st, &f->lastSweep[1]));
     recordPhaseStop(s, st);
-    GramArgs g{};
-    if (!useGramChol && !useQr) recordPhaseStart(s, 1, st);
-    if (useQr) {
-      // nothing: the QR kernel reads the Jacobian directly
-    } else if (useGram) {
-      const DeviceSchedule& ds = *f->sched;
-      g.batch = B;
-      g.strips = f->dJ.p;
-      g.stripStride = size_t(ds.gram.stride);
-      g.residOff = ds.gram.residOff;
-      g.active = s->dActive.p;
-      g.numStrips = ds.gram.numStrips;
-      g.numTiles = ds.host.numTiles;
-      g.numTileCols = ds.host.numTileCols;
-      g.nPad = ds.host.nPad;
-      g.numOrder = int32_t(ds.gram.tileOrder.size());
-      g.blob = ds.gBlob.p;
-      g.blobInts = ds.gBlobInts;
-      g.offTileOrder = ds.gOffsets[0]; g.offTilePairStart = ds.gOffsets[1]; g.offPairA = ds.gOffsets[2]; g.offPairB = ds.gOffsets[3];
-      g.offColStripStart = ds.gOffsets[4]; g.offColStrip = ds.gOffsets[5]; g.offStripRow = ds.gOffsets[6]; g.offTileInfo = ds.gOffsets[7];
-      g.regularization = o.regularization;
-      g.out = s->dTiles.p;
-      g.outStride = tilesStride;
-      if (!useGramChol) {
-        if (s->dTiles.n < size_t(B) * tilesStride) MB2_CUDA(s->dTiles.resize(size_t(B) * tilesStride));
-        g.out = s->dTiles.p;
-        MB2_CUDA(launchGramTiles(g, st));
-      }
-    } else {
-      rc = runJtJ(f, mode, ns, Hbuf, ldH, hStride, s->dActive.p, st, s->dGrad.p, ldG);
-      if (rc != MB2_OK) return rc;
-    }
-    if (!useGramChol && !useQr) recordPhaseStop(s, st);
-    CholArgs c{};
-    c.batch = B;
-    c.H = Hbuf;
-    c.ns = ns;
-    c.ldH = ldH;
-    c.hStride = hStride;
-    c.regularization = o.regularization;
-    c.cols = f->dDeviceCols.p;
-    c.theta = theta;
-    c.ldTheta = n;
-    c.delta = s->dDelta.p;
-    c.applyUpdate = lineSearch ? 0 : 1;
-    c.errors = f->dErrors.p;
-    c.lastErrors = s->dLastErrors.p;
-    c.active = s->dActive.p;
-    c.iterations = s->dIterations.p;
-    c.status = s->dStatus.p;
-    c.history = o.store_error_history ? s->dHistory.p : nullptr;
-    c.iteration = it;
-    c.minIterations = minIt;
-    c.maxIterations = maxIt;
-    c.threshold = o.threshold;
-    c.activeCount = s->dActiveCount.p;
-    c.bookkeeping = lineSearch ? 0 : 1;
-    c.gradDotDelta = lineSearch ? s->dGradDotDelta.p : nullptr;
-    c.g = s->dGrad.p;
-    c.ldG = ldG;
-    c.tilesIn = useGram ? s->dTiles.p : nullptr;
-    c.tilesStride = tilesStride;
-    c.profile = (it == 0 && cholProfile) ? 1 : 0;
-    recordPhaseStart(s, 2, st);
-    if (useQr) {
-      QrArgs q{};
-      q.c = c;
-      q.jacobian = f->dJ.p;
-      q.numCols = f->plan.numCols;
-      q.ldJ = f->ldJ;
-      q.chunkStart = s->dQrChunks.p;
-      q.numChunks = qrChunks;
-      if (useTr) {
-        TrQrArgs t{};
-        t.q = q;
-        t.T = f->tables();
-        t.targets = f->dTargets.p;
-        t.cweights = f->dWeights.p;
-        t.radius = s->dRadius.p;
-        t.rSaved = s->dRSaved.p;
-        t.maxRadius = 10.f; // trust_region_qr.h:73
-        t.maxChunkRows = qrMaxRows;
+    step.iteration = it;
+    step.profile = (it == 0 && cholProfile) ? 1 : 0;
+    switch (P.kind) {
+      case kSolveDense:
+      case kSolveTilesKMajor:
+      case kSolveTiles: // the normal equations in a launch of their own, then the factorisation
+        recordPhaseStart(s, 1, st);
+        if (P.kind == kSolveTiles) MB2_CUDA(launchGramTiles(g, P.gramThreads, st));
+        else if ((rc = runJtJ(f, P.jtjMode, ns, c.H, ldH, hStride, s->dActive.p, st, s->dGrad.p, ldG)) != MB2_OK) return rc;
+        recordPhaseStop(s, st);
+        recordPhaseStart(s, 2, st);
+        if (P.kind == kSolveDense) MB2_CUDA(launchCholesky(c, P.denseNb, P.denseInSmem, st));
+        else MB2_CUDA(launchCholeskyScheduled(c, f->sched->dev, P.cholThreads, st));
+        break;
+      case kSolveGramCholesky:
+        recordPhaseStart(s, 2, st);
+        MB2_CUDA(launchGramCholesky(gc, f->sched->dev, f->sched->gcParams.get(), gt, s->inKernelProfile, st));
+        break;
+      case kSolveQr: // the QR kernels read the Jacobian directly
+        recordPhaseStart(s, 2, st);
+        MB2_CUDA(launchQrSolve(t.q, P.qrWidestChunk, st));
+        break;
+      default:
+        recordPhaseStart(s, 2, st);
         MB2_CUDA(launchTrustRegionQr(t, st));
-      } else {
-        MB2_CUDA(launchQrSolve(q, qrMaxRows, st));
-      }
-    } else if (useGramChol) {
-      GramCholArgs gc{};
-      gc.g = g;
-      gc.c = c;
-      gc.c.tilesIn = nullptr;
-      gc.phaseCycles = s->inKernelProfile ? s->dPhaseCycles.p : nullptr;
-      const DeviceSchedule& ds = *f->sched;
-      gc.parkTiles = ds.gc.parkTiles;
-      if (gc.parkTiles > 0) {
-        const int slots = gramCholeskyParkSlots(gc, ds.dev, ds.gcParams != nullptr);
-        if (slots < 1) return fail(MB2_ERR_CUDA, "Gram + Cholesky fusion: no resident CTA");
-        if (s->dParkSlots.n < size_t(slots / 32)) { // grown only here, and every launch leaves it all zero
-          MB2_CUDA(s->dParkSlots.resize(size_t(slots / 32)));
-          MB2_CUDA(cudaMemsetAsync(s->dParkSlots.p, 0, s->dParkSlots.n * sizeof(uint32_t), st));
-        }
-        MB2_CUDA(s->dPark.resize(size_t(slots) * size_t(gc.parkTiles) * 256));
-        gc.park = s->dPark.p;
-        gc.parkSlots = s->dParkSlots.p;
-        gc.parkSlotWords = int32_t(slots / 32);
-      }
-      GramCholGlobalTables gt{};
-      gt.L = ds.gc.L;
-      gt.tab = ds.gcTab.p;
-      MB2_CUDA(launchGramCholesky(gc, ds.dev, ds.gcParams.get(), gt, s->inKernelProfile, st));
-    } else if (useSchedule) MB2_CUDA(launchCholeskyScheduled(c, f->sched->dev, st));
-    else MB2_CUDA(launchCholesky(c, st));
+    }
     recordPhaseStop(s, st);
     if (lineSearch) { // gauss_newton_solver.cpp:283-313 / subset_gauss_newton_solver.cpp:119-141
       MB2_CUDA(cudaMemcpyAsync(s->dThetaOrig.p, theta, size_t(B) * n * sizeof(float), cudaMemcpyDeviceToDevice, st));
       initLineSearchKernel<<<(B + 127) / 128, 128, 0, st>>>(B, s->dActive.p, s->dSearching.p, s->dScale.p);
       MB2_CUDA(cudaGetLastError());
-      for (int step = 0; step < 10; ++step) {
+      for (int k = 0; k < 10; ++k) {
         MB2_CUDA(launchTrialUpdate(B, s->dThetaOrig.p, n, s->dDelta.p, ns, f->dDeviceCols.p, s->dScale.p, theta, s->dSearching.p, st));
-        SweepArgs ea = sweepArgs(f, theta, s->dSearching.p);
-        ea.errors = s->dTrialErrors.p;
         recordPhaseStart(s, 3, st);
-        MB2_CUDA(launchSweep(ea, false, st, &f->lastSweep[0]));
+        MB2_CUDA(launchSweep(trial, false, st, &f->lastSweep[0]));
         recordPhaseStop(s, st);
-        LineSearchArgs la{};
-        la.batch = B; la.ns = ns; la.numParams = n; la.ldTheta = n;
-        la.errors = f->dErrors.p;
-        la.trialErrors = s->dTrialErrors.p;
-        la.gradDotDelta = s->dGradDotDelta.p;
-        la.scale = s->dScale.p;
-        la.searching = s->dSearching.p;
-        la.step = step;
-        la.subsetVariant = o.subset_line_search;
-        la.active = s->dActive.p;
+        la.step = k;
         MB2_CUDA(launchLineSearchStep(la, st));
         s->kernelLaunches += 2;
       }
-      BookkeepingArgs ba{};
-      ba.batch = B;
-      ba.errors = f->dErrors.p; ba.lastErrors = s->dLastErrors.p; ba.active = s->dActive.p; ba.iterations = s->dIterations.p;
-      ba.status = s->dStatus.p; ba.history = o.store_error_history ? s->dHistory.p : nullptr;
-      ba.theta = theta; ba.ldTheta = n; ba.numParams = n;
-      ba.iteration = it; ba.minIterations = minIt; ba.maxIterations = maxIt; ba.threshold = o.threshold; ba.activeCount = s->dActiveCount.p;
+      ba.iteration = it;
       MB2_CUDA(launchBookkeeping(ba, st));
       s->kernelLaunches += 1;
     }
@@ -1544,7 +1435,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
 }
 
 static void collectProfile(mb2_solver* s) {
-  if (s->profiling && s->lastFused && s->fusedStart) {
+  if (s->profiling && s->path.kind == kSolvePersistent && s->fusedStart) {
     float ms = 0.f;
     s->fusedMs = cudaEventElapsedTime(&ms, s->fusedStart, s->fusedStop) == cudaSuccess ? double(ms) : 0.0;
   }
@@ -1657,22 +1548,23 @@ int mb2_solver_get_plan_stats(mb2_solver* s, int64_t stats[12]) {
   stats[8] = gram ? f->sched->gram.stride : 0;
   stats[9] = gram ? f->sched->gram.macs : 0;
   stats[10] = gram ? int64_t(f->sched->gram.pairA.size()) : 0;
-  stats[11] = gram ? f->sched->fConfig.groups : 0;
+  stats[11] = gram ? f->sched->fusedGroups : 0;
   return MB2_OK;
 }
 
 int mb2_solver_get_fused_profile(mb2_solver* s, int32_t* fused, int32_t* groups, double* kernelMs, uint64_t phaseCycles[12]) {
   MB2_CHECK(s != nullptr, "null solver");
-  if (fused) *fused = s->lastFused ? 1 : (s->lastGramChol ? 2 : 0);
-  if (groups) *groups = s->lastFused ? s->lastFusedGroups : 0;
-  if (kernelMs) *kernelMs = s->lastFused ? s->fusedMs : (s->lastGramChol ? s->phaseMs[2] : 0.0);
+  const bool persistent = s->path.kind == kSolvePersistent, gramChol = s->path.kind == kSolveGramCholesky;
+  if (fused) *fused = persistent ? 1 : (gramChol ? 2 : 0);
+  if (groups) *groups = persistent ? s->path.fused.groups : 0;
+  if (kernelMs) *kernelMs = persistent ? s->fusedMs : (gramChol ? s->phaseMs[2] : 0.0);
   if (phaseCycles) {
     for (int k = 0; k < 12; ++k) phaseCycles[k] = 0;
-    if ((s->lastFused || s->lastGramChol) && s->profiling && s->dPhaseCycles.p) {
+    if ((persistent || gramChol) && s->profiling && s->dPhaseCycles.p) {
       MB2_DEVICE_GUARD(s->fn->ch->device);
       unsigned long long h[12];
       MB2_CUDA(cudaMemcpy(h, s->dPhaseCycles.p, sizeof(h), cudaMemcpyDeviceToHost));
-      if (s->lastFused) {
+      if (persistent) {
         for (int k = 0; k < 12; ++k) phaseCycles[k] = h[k];
       } else { // gramCholeskyKernel (block 0, summed over the iterations): prologue, gram, parked tiles, diag, panel, update, backward, finish
         phaseCycles[0] = h[0];
@@ -1691,6 +1583,12 @@ int mb2_solver_function_get_sweep_launch(mb2_solver_function* f, int32_t jacobia
   out[2] = l.groupsPerCta;
   out[3] = l.grid;
   out[4] = l.smemBytes;
+  return MB2_OK;
+}
+
+int mb2_solver_get_solve_path(mb2_solver* s, int64_t out[15]) {
+  MB2_CHECK(s != nullptr && out != nullptr, "null argument");
+  solvePathWords(s->path, out);
   return MB2_OK;
 }
 

@@ -247,25 +247,6 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
 
 } // namespace
 
-FusedConfig fusedConfigure(const FunctionTables& T, const FusedBlobLayout& L, const CholSchedDev& S, int stripStride, int orderRounds, int maxSmemOptin) {
-  FusedConfig c;
-  const int nc4 = (S.n + 3) & ~3, np4 = (T.numParams + 3) & ~3;
-  const int sweep = stripStride + 64 + ((T.numJoints * kJointStateStride + 3) & ~3) + ((T.numJoints * kParametersPerJoint + 3) & ~3) + ((T.recStride + 3) & ~3);
-  c.unionFloats = (std::max(S.numTiles * 256, sweep) + 3) & ~3;
-  c.groupFloats = c.unionFloats + S.nPad + 2 * nc4 + np4 + 32; // + 10 doubles and 4 ints of per-instance state
-  if (orderRounds > kFusedMaxRounds) return c; // more parked tiles per warp than the kernel holds
-  const size_t fixed = 128 + size_t(L.words) * 4 + 16;
-  for (int g = kFusedMaxGroups; g >= 1; --g) {
-    const size_t need = fixed + size_t(g) * c.groupFloats * sizeof(float);
-    if (need <= size_t(maxSmemOptin)) {
-      c.groups = g;
-      c.smemBytes = need;
-      break;
-    }
-  }
-  return c;
-}
-
 cudaError_t launchFusedSolve(const FusedArgs& a0, const FusedConfig& cfg, int numSms, bool profile, cudaStream_t stream) {
   if (cfg.groups < 1) return cudaErrorInvalidConfiguration;
   FusedArgs a = a0;

@@ -17,23 +17,12 @@
 #include <cuda_runtime.h>
 
 #include "ik_chol_sched.cuh"
+#include "ik_solve_path.h"
 #include "ik_types.h"
 
 namespace mb2 {
 
 constexpr int kFusedGroupThreads = 256;
-constexpr int kFusedMaxGroups = 3;
-constexpr int kFusedMaxRounds = 32; // rounds of the Gram tile-order table a warp can park (fusedConfigure refuses larger plans)
-
-// word (4-byte) offsets of the tables inside the plan blob (every table starts on a 16-byte boundary)
-struct FusedBlobLayout {
-  int32_t parent, offset, prerot, ptOuter, ptInner, ptVals, ptOffsets, levelStart, levelJoints;
-  int32_t efs, units, cells, contribs, limitData;
-  int32_t cols;       // device column -> model parameter (-1: alignment column)
-  int32_t gram;       // Gram plan blob (makeGramBlob), gramOff[] are relative to it
-  int32_t sched;      // Cholesky schedule blob (makeScheduleBlob)
-  int32_t words;      // total size, multiple of 4
-};
 
 struct FusedArgs {
   int32_t batch;
@@ -61,14 +50,7 @@ struct FusedArgs {
   int32_t unionFloats;         // ... of which the strips / tiles union region
 };
 
-struct FusedConfig {
-  int groups{0};
-  int groupFloats{0}, unionFloats{0};
-  size_t smemBytes{0};
-};
-// how many groups fit next to the staged tables (0: the fused kernel cannot run this plan)
-// orderRounds: rounds of the Gram tile-order table (tiles per warp at most)
-FusedConfig fusedConfigure(const FunctionTables& T, const FusedBlobLayout& L, const CholSchedDev& S, int stripStride, int orderRounds, int maxSmemOptin);
+// cfg: SolvePath::fused (ik_solve_path.h)
 cudaError_t launchFusedSolve(const FusedArgs& a, const FusedConfig& cfg, int numSms, bool profile, cudaStream_t stream);
 
 } // namespace mb2

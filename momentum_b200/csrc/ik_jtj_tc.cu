@@ -44,7 +44,7 @@ namespace {
 
 constexpr int kConsumerThreads = 256; // two warpgroups
 constexpr int kTcThreads = kConsumerThreads + 32;
-constexpr int kKBlock = 32;         // floats per K block = one 128-byte swizzle row
+constexpr int kKBlock = kJtjKBlock; // floats per K block = one 128-byte swizzle row
 constexpr int kRowBytes = 128;
 constexpr int kWgmmaK = 8;          // tf32: 32 bytes of K per instruction
 
@@ -312,8 +312,7 @@ cudaError_t makeTensorMap3d(CUtensorMap* map, const float* base, const uint64_t 
 }
 
 bool jtjTensorSupported(int ns, int numCols, int ldJ) {
-  if (encodeTiled() == nullptr) return false;
-  return ns >= 1 && ns <= numCols && numCols + 1 <= 512 && (ldJ % kKBlock) == 0; // at most four row tiles, at most one far item per tile
+  return encodeTiled() != nullptr && jtjTensorShape(ns, numCols, ldJ);
 }
 
 cudaError_t launchJtJTensor(const JtJArgs& a, int passes, cudaStream_t stream) {

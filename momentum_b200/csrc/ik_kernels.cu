@@ -969,19 +969,9 @@ __global__ void __launch_bounds__(kCholThreads) choleskyKernel(const CholArgs a,
   cholFinish(a, b, n, y, gsave, flags[0] != 0);
 }
 
-static size_t cholSmemBytes(int n, int NB, bool matrixInSmem) {
-  const size_t ldp = ((n + 1 + 3) & ~3) + 4;
-  size_t s = sizeof(float) * (NB * ldp + ((n + 3) & ~3)) + 4 * sizeof(int);
-  if (matrixInSmem) s += sizeof(float) * size_t(n + 1) * (n | 1);
-  return s;
-}
-
-cudaError_t launchCholesky(const CholArgs& a, cudaStream_t stream) {
-  const int n = a.ns;
-  const int eig = cholBlockSize(n, 32);
-  const int NB = eig <= 8 ? 8 : (eig <= 16 ? 16 : 32);
-  bool inSmem = cholSmemBytes(n, NB, true) <= size_t(g_maxSmemOptin);
-  const size_t smem = cholSmemBytes(n, NB, inSmem);
+cudaError_t launchCholesky(const CholArgs& a, int NB, bool inSmem, cudaStream_t stream) {
+  const size_t smem = cholSmemBytes(a.ns, NB, inSmem);
+  if (NB != 8 && NB != 16 && NB != 32) return cudaErrorInvalidConfiguration;
   cudaError_t e = cudaSuccess;
 #define MB2_LAUNCH_CHOL(NBV)                                                                                   \
   e = cudaFuncSetAttribute(choleskyKernel<NBV>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));       \
@@ -999,8 +989,6 @@ cudaError_t launchCholesky(const CholArgs& a, cudaStream_t stream) {
 // TMA box of the K-major Jacobian, a warp owns a tile at a time, the output is already in the Cholesky kernel's tile layout.
 // ------------------------------------------------------------------------------------------------
 constexpr int kGramThreads = 32 * kGramWarps;
-
-size_t gramTilesSmemBytes(size_t stripStride, int blobInts) { return 128 + sizeof(float) * (stripStride + 64) + 16 + sizeof(int32_t) * size_t((blobInts + 3) & ~3); }
 
 // kThreads = 256 (eight warps, the width the tile-order table is dealt for), or 512 when the strips of an instance leave room for only
 // one CTA per SM anyway (bodyhands300: 155 KB): the sixteen warps then walk the same table two rounds at a time.
@@ -1049,10 +1037,10 @@ __global__ void __launch_bounds__(kThreads) gramTilesKernel(const GramArgs a) {
     y[16 * K + hl] = gramVectorEntry(strips, resid, colStrip, stripRow, colStripStart[K], colStripStart[K + 1], hl);
 }
 
-cudaError_t launchGramTiles(const GramArgs& a, cudaStream_t stream) {
+cudaError_t launchGramTiles(const GramArgs& a, int threads, cudaStream_t stream) {
   const size_t smem = gramTilesSmemBytes(a.stripStride, a.blobInts);
-  if (smem > size_t(g_maxSmemOptin) || (a.stripStride & 3) != 0) return cudaErrorInvalidConfiguration;
-  const bool wide = 2 * (smem + 1024) > size_t(g_maxSmemPerSm); // one CTA per SM anyway: give it 16 warps
+  if (smem > size_t(g_maxSmemOptin) || (a.stripStride & 3) != 0 || (threads != 256 && threads != 512)) return cudaErrorInvalidConfiguration;
+  const bool wide = threads == 512;
   cudaError_t e = wide ? cudaFuncSetAttribute(gramTilesKernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem))
                        : cudaFuncSetAttribute(gramTilesKernel<kGramThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
   if (e != cudaSuccess) return e;
@@ -1068,11 +1056,6 @@ cudaError_t launchGramTiles(const GramArgs& a, cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------------
 // 256 threads and three CTAs per SM when the tiles of one instance take a third of shared memory (humanoid-size rigs); 512 threads in
 // the single resident CTA when one instance needs more than half of it (body + hands)
-
-size_t choleskyScheduledSmemBytes(int n, int nPad, int numTiles, int blobInts) {
-  return 1024 /*tile storage is aligned to the TMA swizzle atom*/ + sizeof(float) * (size_t(numTiles) * 256 + size_t(nPad) + 2 * size_t((n + 3) & ~3)) +
-         sizeof(int32_t) * size_t((blobInts + 3) & ~3) + 32;
-}
 
 // kProfile: per-phase cycle counters of block 0 (MB2_CHOL_PROFILE=1); a separate instantiation so that the production kernel does not
 // carry the counters in its register budget
@@ -1191,10 +1174,10 @@ __global__ void __launch_bounds__(kSchedThreads, kSchedThreads == 256 ? 3 : 1) c
 #undef MB2_PROF
 }
 
-cudaError_t launchCholeskyScheduled(const CholArgs& a, const CholSchedDev& sched, cudaStream_t stream) {
+cudaError_t launchCholeskyScheduled(const CholArgs& a, const CholSchedDev& sched, int threads, cudaStream_t stream) {
   const size_t smem = choleskyScheduledSmemBytes(a.ns, sched.nPad, sched.numTiles, sched.blobInts);
-  if (smem > size_t(g_maxSmemOptin)) return cudaErrorInvalidConfiguration;
-  const bool wide = 2 * (smem + 1024) > size_t(g_maxSmemPerSm); // one CTA per SM anyway: give it 16 warps
+  if (smem > size_t(g_maxSmemOptin) || (threads != 256 && threads != 512)) return cudaErrorInvalidConfiguration;
+  const bool wide = threads == 512;
   const bool prof = (a.profile & 1) != 0;
   cudaError_t e;
   if (wide) e = prof ? cudaFuncSetAttribute(choleskyScheduledKernel<512, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem))
@@ -1227,12 +1210,6 @@ cudaError_t launchCholeskyScheduled(const CholArgs& a, const CholSchedDev& sched
 //   Cholesky   level-scheduled tile factorisation, both substitutions, theta -= delta, SolverT bookkeeping (cholFinish)
 // The stored tiles (0.45 GB per iteration on the cfg3 shard) never exist in HBM and the second launch is gone.
 // ------------------------------------------------------------------------------------------------
-size_t gramCholeskySmemBytes(size_t stripStride, int gramBlobInts, int n, int nPad, int numTiles, int schedBlobInts) {
-  (void)gramBlobInts; (void)schedBlobInts; // the plan tables are not staged in shared memory: see the kernel
-  const size_t uni = std::max<size_t>(size_t(numTiles) * 256, stripStride + 64);
-  return 128 + sizeof(float) * (((uni + 3) & ~size_t(3)) + size_t(nPad) + size_t((n + 3) & ~3)) + 32;
-}
-
 // A free parking slot (see GramCholArgs): the search starts at a word that depends on the instance so that the CTAs of a wave do not
 // all contend for the first word.
 __device__ int acquireParkSlot(uint32_t* words, int numWords, int start) {
@@ -1393,7 +1370,7 @@ static cudaError_t prepareGramCholesky(size_t smem) {
 }
 
 int gramCholeskyParkSlots(const GramCholArgs& a, const CholSchedDev& sched, bool paramTables) {
-  const size_t smem = gramCholeskySmemBytes(a.g.stripStride, a.g.blobInts, a.c.ns, sched.nPad, sched.numTiles, sched.blobInts);
+  const size_t smem = gramCholeskySmemBytes(a.g.stripStride, a.c.ns, sched.nPad, sched.numTiles);
   // the profiling instantiations carry more registers: never more resident CTAs than the production ones
   cudaError_t e = paramTables ? prepareGramCholesky<false, GramCholParamTables>(smem) : prepareGramCholesky<false, GramCholGlobalTables>(smem);
   int perSm = 0;
@@ -1406,7 +1383,7 @@ int gramCholeskyParkSlots(const GramCholArgs& a, const CholSchedDev& sched, bool
 
 cudaError_t launchGramCholesky(const GramCholArgs& a, const CholSchedDev& sched, const GramCholParamTables* inParams, const GramCholGlobalTables& inGlobal, bool profile,
                                cudaStream_t stream) {
-  const size_t smem = gramCholeskySmemBytes(a.g.stripStride, a.g.blobInts, a.c.ns, sched.nPad, sched.numTiles, sched.blobInts);
+  const size_t smem = gramCholeskySmemBytes(a.g.stripStride, a.c.ns, sched.nPad, sched.numTiles);
   if (smem > size_t(g_maxSmemOptin) || (a.g.stripStride & 3) != 0) return cudaErrorInvalidConfiguration;
   if (a.parkTiles > 0 && (a.park == nullptr || a.parkSlots == nullptr || a.parkSlotWords < 1)) return cudaErrorInvalidValue;
   cudaError_t e;
@@ -1531,5 +1508,7 @@ cudaError_t launchNormalizeQuats(float* base, int count, int strideFloats, int q
   normalizeQuatsKernel<<<(total + 127) / 128, 128, 0, stream>>>(base, count, strideFloats, quatsPerRecord, batch);
   return cudaGetLastError();
 }
+
+DeviceLimits deviceLimits() { return DeviceLimits{g_numSms, g_maxSmemOptin, g_maxSmemPerSm}; }
 
 } // namespace mb2

@@ -5,6 +5,7 @@
 
 #include "ik_chol_sched.cuh"
 #include "ik_chol_sched.h"
+#include "ik_solve_path.h"
 #include "ik_types.h"
 
 namespace mb2 {
@@ -83,8 +84,8 @@ struct GramArgs {            // K2s: stored tiles of J^T J + lambda I and J^T r 
   float* out;                // [B][outStride]: numTiles x 256 floats in tile storage order, then the slot-ordered J^T r [nPad]
   size_t outStride;
 };
-cudaError_t launchGramTiles(const GramArgs& a, cudaStream_t stream);
-size_t gramTilesSmemBytes(size_t stripStride, int blobInts);
+// threads: SolvePath::gramThreads
+cudaError_t launchGramTiles(const GramArgs& a, int threads, cudaStream_t stream);
 
 // K2s + K3 in one launch: strips in (bulk copy), tiles beyond the strips stored at once, the others parked in an L2-resident scratch
 // slot and written over the strips once they are dead, tile Cholesky, update. No second launch; `g.out` is unused.
@@ -110,7 +111,6 @@ struct GramCholGlobalTables {
   GramCholLayout L;
   const uint16_t* tab;
 };
-size_t gramCholeskySmemBytes(size_t stripStride, int gramBlobInts, int n, int nPad, int numTiles, int schedBlobInts);
 // scratch slots for the parked tiles: resident CTAs of the launch on this device, rounded up to whole 32-bit words of parkSlots
 int gramCholeskyParkSlots(const GramCholArgs& a, const CholSchedDev& sched, bool paramTables);
 // tables: exactly one of inParams (non-null) or inGlobal is used
@@ -136,10 +136,7 @@ struct TrQrArgs {
   float maxRadius;    // maxTrustRegionRadius_ = 10 (trust_region_qr.h:73)
   int32_t maxChunkRows;
 };
-size_t trQrSmemFloats(int n, int numParams, int numJoints, int maxChunkRows);
 cudaError_t launchTrustRegionQr(const TrQrArgs& a, cudaStream_t stream);
-size_t qrSmemFloats(int n, int maxChunkRows);
-int qrMaxChunkRows(int n, size_t smemBytes); // rows of Jacobian that fit beside R (0: the system is too large for this kernel)
 cudaError_t launchQrSolve(const QrArgs& a, int maxChunkRows, cudaStream_t stream);
 // skeletonStateKernel<kBackward>: pymomentum's model_parameters_to_skeleton_state for a batch on the character alone (no solver
 // function), and its backward
@@ -228,13 +225,14 @@ struct SweepLaunch {         // the variant and launch shape launchSweep chose (
 cudaError_t launchSweep(const SweepArgs& a, bool jacobian, cudaStream_t stream, SweepLaunch* out = nullptr);
 size_t sweepSmemPerInstance(const FunctionTables& T, int warpsPerInstance);
 cudaError_t launchJtJSimt(const JtJArgs& a, cudaStream_t stream);
-cudaError_t launchCholesky(const CholArgs& a, cudaStream_t stream);
+// NB, inSmem: SolvePath::denseNb / denseInSmem
+cudaError_t launchCholesky(const CholArgs& a, int NB, bool inSmem, cudaStream_t stream);
 // level-scheduled tile-sparse variant (ik_chol_sched.h); returns cudaErrorInvalidConfiguration when the tiles do not fit in shared memory
-// `a.H` is the full symmetric system in device-column (= elimination) order
-cudaError_t launchCholeskyScheduled(const CholArgs& a, const CholSchedDev& sched, cudaStream_t stream);
+// `a.H` is the full symmetric system in device-column (= elimination) order; threads: SolvePath::cholThreads
+cudaError_t launchCholeskyScheduled(const CholArgs& a, const CholSchedDev& sched, int threads, cudaStream_t stream);
 inline int cholGradientLd(int ns) { return (ns + 3) & ~3; }
-size_t choleskyScheduledSmemBytes(int n, int nPad, int numTiles, int blobInts);
 cudaError_t initKernelAttributes();
+DeviceLimits deviceLimits(); // of the device initKernelAttributes last read
 
 // line-search helpers
 cudaError_t launchTrialUpdate(int batch, const float* thetaOrig, int ldTheta, const float* delta, int ns, const int32_t* cols, const float* scale /*[B]*/,

@@ -122,18 +122,6 @@ __global__ void __launch_bounds__(kQrThreads, 1) qrSolveKernel(const QrArgs a) {
   cholFinish(c, b, n, x, g, false);
 }
 
-size_t qrSmemFloats(int n, int maxChunkRows) {
-  return (size_t(n) * (n + 1) / 2 + 3 & ~size_t(3)) + 3 * size_t((n + 3) & ~3) + size_t((n + 4) & ~3) + size_t(n + 1) * size_t(maxChunkRows | 1) + 8;
-}
-int qrMaxChunkRows(int n, size_t smemBytes) {
-  const size_t fixed = qrSmemFloats(n, 0) - size_t(n + 1);
-  const size_t floats = smemBytes / sizeof(float);
-  if (floats <= fixed + size_t(n + 1) * 9) return 0;
-  int p = int((floats - fixed) / size_t(n + 1)) - 1;
-  p = std::min(p, 128) & ~1; // even: p | 1 = p + 1 stays inside the budget
-  return p;
-}
-
 cudaError_t launchQrSolve(const QrArgs& a, int maxChunkRows, cudaStream_t stream) {
   const size_t smem = qrSmemFloats(a.c.ns, maxChunkRows) * sizeof(float);
   cudaError_t e = cudaFuncSetAttribute(qrSolveKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));

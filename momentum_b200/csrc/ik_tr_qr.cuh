@@ -93,13 +93,6 @@ __device__ double trGetError(const FunctionTables& T, const float* th, float* js
   return (double)(float)e;
 }
 
-size_t trQrSmemFloats(int n, int numParams, int numJoints, int maxChunkRows) {
-  const size_t packed = (size_t(n) * (n + 1) / 2 + 3) & ~size_t(3);
-  const size_t n4 = size_t((n + 3) & ~3), np4 = size_t((numParams + 3) & ~3);
-  const size_t chunk = (size_t(n + 1) * size_t(maxChunkRows | 1) + 3) & ~size_t(3);
-  return packed + std::max(packed, chunk) + 7 * n4 + size_t((n + 4) & ~3) + 2 * np4 + size_t((numJoints * kJointStateStride + 3) & ~3) + 64;
-}
-
 __global__ void __launch_bounds__(kQrThreads, 1) trustRegionQrKernel(const TrQrArgs a) {
   extern __shared__ __align__(16) float trSmem[];
   const CholArgs& c = a.q.c;

@@ -75,7 +75,7 @@ CABI_SYMBOLS = [
     "mb2_sharded_solver_shard_info", "mb2_sharded_solver_set_options", "mb2_sharded_solver_set_targets", "mb2_sharded_solver_solve", "mb2_sharded_solver_get_aggregate",
     "mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device",
     "mb2_add_orientation_error_function_instanced", "mb2_solver_function_input_gradients_device",
-    "mb2_solver_function_implicit_direction_device", "mb2_solver_function_get_sweep_launch",
+    "mb2_solver_function_implicit_direction_device", "mb2_solver_function_get_sweep_launch", "mb2_solver_get_solve_path",
     "mb2_character_set_skinning", "mb2_character_num_vertices", "mb2_character_skin_points_device", "mb2_character_skin_points_backward_device",
 ]
 
@@ -181,6 +181,8 @@ def load_library(path: Optional[str] = None):
         L.mb2_solver_function_implicit_direction_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     if hasattr(L, "mb2_solver_function_get_sweep_launch"):
         L.mb2_solver_function_get_sweep_launch.argtypes = [vp, C.c_int32, C.POINTER(C.c_int64)]
+    if hasattr(L, "mb2_solver_get_solve_path"):
+        L.mb2_solver_get_solve_path.argtypes = [vp, C.POINTER(C.c_int64)]
     if hasattr(L, "mb2_character_set_skinning"):
         L.mb2_character_set_skinning.argtypes = [vp, C.c_int32, _fp, _ip, _fp, _fp]
         L.mb2_character_num_vertices.argtypes = [vp]
@@ -586,6 +588,19 @@ class GaussNewtonSolver(_Base):
         fused = C.c_int32(0); groups = C.c_int32(0); ms_ = C.c_double(0.0); cyc = (C.c_uint64 * 12)()
         self._check(self._L.mb2_solver_get_fused_profile(self._h, C.byref(fused), C.byref(groups), C.byref(ms_), cyc))
         return {"fused": int(fused.value), "groups": groups.value, "kernel_ms": ms_.value, "phase_cycles": dict(zip(self.FUSED_PHASES, (int(v) for v in cyc)))}
+
+    SOLVE_PATH_KINDS = {0: None, 1: "dense", 2: "tiles_kmajor", 3: "tiles", 4: "gram_cholesky", 5: "persistent", 6: "qr", 7: "trust_region_qr"}
+    SOLVE_PATH_KEYS = ["kind", "plan_mode", "sched_dense", "strips", "jtj_mode", "dense_nb", "dense_in_smem", "gram_threads", "chol_threads",
+                       "qr_max_chunk_rows", "qr_chunks", "qr_widest_chunk", "tr_r_floats", "fused_groups", "fused_smem"]
+
+    def get_solve_path(self) -> dict:
+        """The linear-solve path of the last solve (mb2_solver_get_solve_path): kind as a name (None before the first solve), the
+        plan request, the resolved JtJ mode and the launch variants of the kernels it runs."""
+        out = (C.c_int64 * 15)()
+        self._check(self._L.mb2_solver_get_solve_path(self._h, out))
+        d = dict(zip(self.SOLVE_PATH_KEYS, (int(v) for v in out)))
+        d["kind"] = self.SOLVE_PATH_KINDS[d["kind"]]
+        return d
 
     def set_profiling(self, level):
         """0 off, 1 CUDA events around every launch (production kernels), 2 + in-kernel phase cycles (instrumented, slower kernels)."""

@@ -19,6 +19,7 @@
 #include "../../momentum_b200/csrc/ik_chol_sched.h"
 #include "../../momentum_b200/csrc/ik_device.cuh"
 #include "../../momentum_b200/csrc/ik_plan.h"
+#include "../../momentum_b200/csrc/ik_solve_path.h"
 
 using namespace mb2;
 
@@ -45,7 +46,10 @@ struct mb2_solver {
   std::vector<double> errors, history;
   std::vector<int32_t> iterations, status;
   uint64_t totalIterations{0};
+  SolvePath path;
 };
+// the device the solve path is chosen for (emu_set_device_limits): an H100 SXM by default
+static DeviceLimits g_limits{132, 227 * 1024, 228 * 1024};
 
 static int roundUp(int v, int m) { return (v + m - 1) / m * m; }
 
@@ -168,10 +172,9 @@ static int cholOne(float* Hg, int n, int ldH, float reg, float* delta, float* gd
   return flag;
 }
 
-static int cholDispatch(float* Hg, int n, int ldH, float reg, float* delta, float* gdd) {
-  const int eig = cholBlockSize(n, 32);
-  if (eig <= 8) return cholOne<8>(Hg, n, ldH, reg, delta, gdd);
-  if (eig <= 16) return cholOne<16>(Hg, n, ldH, reg, delta, gdd);
+static int cholDispatch(int NB, float* Hg, int n, int ldH, float reg, float* delta, float* gdd) {
+  if (NB == 8) return cholOne<8>(Hg, n, ldH, reg, delta, gdd);
+  if (NB == 16) return cholOne<16>(Hg, n, ldH, reg, delta, gdd);
   return cholOne<32>(Hg, n, ldH, reg, delta, gdd);
 }
 
@@ -429,19 +432,71 @@ void mb2_solver_destroy(mb2_solver* s) { delete s; }
 int mb2_solver_set_options(mb2_solver* s, const mb2_gauss_newton_options* opt) { s->opt = *opt; return MB2_OK; }
 int mb2_solver_set_enabled_parameters(mb2_solver* s, const uint64_t* bits) { return mb2_solver_function_set_enabled_parameters(s->fn, bits); }
 
-// emulation of mb2_solver_solve_device's launch sequence, instance by instance
+// the tile plan of a solve: schedule, Gram plan, and the schedule's tables as the kernels read them (S points into blob)
+struct TilePlan {
+  CholSchedule sched;
+  GramPlan gram;
+  std::vector<int32_t> blob;
+  CholSchedDev S{};
+};
+
+// the plan of a solve-path request (PlanFiguresFn), with the figures the library reports for it
+static int planFigures(mb2_solver_function* f, int mode, bool schedDense, bool strips, TilePlan& tp, PlanFigures& F, std::string& msg) {
+  const CholSchedule& sched = tp.sched;
+  const GramPlan& gram = tp.gram;
+  msg = mode == 2 ? planTiles(f, schedDense ? MB2_CHOLESKY_TILES_DENSE : MB2_CHOLESKY_TILES_SPARSE, strips, tp.sched, tp.gram) : plan(f, true);
+  if (!msg.empty()) return MB2_ERR_INVALID_ARGUMENT;
+  F = PlanFigures{};
+  F.numCols = f->plan.numCols;
+  F.recStride = f->plan.recStride;
+  F.jtjTensor = jtjTensorShape(F.numCols, F.numCols, f->ldJ);
+  if (mode != 2) return MB2_OK;
+  makeScheduleBlob(sched, tp.blob, tp.S);
+  F.nPad = sched.nPad;
+  F.numTiles = sched.numTiles;
+  F.schedBlobInts = tp.S.blobInts;
+  if (!strips) return MB2_OK;
+  std::vector<int32_t> gblob;
+  int32_t offsets[8];
+  makeGramBlob(gram, sched, gblob, offsets);
+  GramCholTables gc;
+  FusedBlobLayout L;
+  F.stripStride = gram.stride;
+  F.gramBlobInts = int(gblob.size());
+  F.orderEntries = int(gram.tileOrder.size());
+  F.gramCholValid = makeGramCholTables(gram, sched, gc).empty();
+  F.fusedBlobWords = int(makeFusedBlob(f->ch->host, f->plan, gblob, tp.blob, L).size());
+  return MB2_OK;
+}
+
+// the library's choice of path (chooseSolvePath) for this solver, with the plan it leaves in f and tp
+static int choosePath(mb2_solver* s, TilePlan& tp) {
+  mb2_solver_function* f = s->fn;
+  std::string msg;
+  const PlanFiguresFn figures = [&](int mode, bool dense, bool strips, PlanFigures& F, std::string& m) { return planFigures(f, mode, dense, strips, tp, F, m); };
+  const int rc = chooseSolvePath(s->opt, f->B, f->ch->host, f->host, figures, g_limits, s->path, msg);
+  if (rc != MB2_OK) {
+    s->path = SolvePath{};
+    return fail(rc, msg);
+  }
+  return MB2_OK;
+}
+
+// emulation of mb2_solver_solve_device's launch sequence, instance by instance, on the path the library chooses. The Gram + Cholesky
+// and persistent kernels run the arithmetic of the Gram and tile Cholesky kernels (bit-identical, respectively equal to float
+// rounding on the device), so they are emulated as those two.
 int mb2_solver_solve(mb2_solver* s, float* params, double* errors, int32_t* iterations, int32_t* status) {
   mb2_solver_function* f = s->fn;
   const auto& o = s->opt;
-  const int cholMode = resolveCholeskyMode(o.cholesky_mode, f->host.enabled);
-  const bool useGram = cholMode >= 2 && (o.jtj_mode == MB2_JTJ_AUTO || o.jtj_mode == MB2_JTJ_SPARSE_TILES);
-  CholSchedule sched;
-  GramPlan gram;
-  const std::string e = cholMode >= 2 ? planTiles(f, cholMode, useGram, sched, gram) : plan(f, true);
-  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
-  std::vector<int32_t> blob;
-  CholSchedDev S{};
-  if (cholMode >= 2) makeScheduleBlob(sched, blob, S);
+  TilePlan tp;
+  const int rc = choosePath(s, tp);
+  if (rc != MB2_OK) return rc;
+  const SolvePath& P = s->path;
+  if (P.kind == kSolveQr || P.kind == kSolveTrustRegionQr) return fail(MB2_ERR_UNSUPPORTED, "the CPU emulator does not emulate the QR solvers");
+  const bool useGram = P.strips;
+  const CholSchedule& sched = tp.sched;
+  const GramPlan& gram = tp.gram;
+  const CholSchedDev& S = tp.S;
   const FunctionTables T = tables(f);
   const int n = T.numParams, ns = f->plan.numCols, ldH = roundUp(ns + 1, 16);
   const int maxIt = int(o.max_iterations), minIt = int(o.min_iterations);
@@ -463,8 +518,8 @@ int mb2_solver_solve(mb2_solver* s, float* params, double* errors, int32_t* iter
       } else {
         std::fill(H.begin(), H.end(), std::nanf("")); // entries the device never writes (lower triangle) are garbage there: poison them here
         jtjOne(f, b, ns, H.data(), ldH);
-        failed = cholMode >= 2 ? cholScheduledOne(S, H.data(), ldH, ns, o.regularization, delta.data(), &gdd)
-                               : cholDispatch(H.data(), ns, ldH, o.regularization, delta.data(), &gdd);
+        failed = P.kind == kSolveDense ? cholDispatch(P.denseNb, H.data(), ns, ldH, o.regularization, delta.data(), &gdd)
+                                       : cholScheduledOne(S, H.data(), ldH, ns, o.regularization, delta.data(), &gdd);
       }
       if (failed && s->status[b] == 0) s->status[b] = MB2_INSTANCE_CHOLESKY_BREAKDOWN;
       if (!o.do_line_search) {
@@ -507,6 +562,10 @@ int mb2_solver_get_error_history(mb2_solver* s, double* history) {
 int mb2_solver_get_counters(mb2_solver* s, uint64_t* totalIterations, uint64_t* kernelLaunches) {
   if (totalIterations) *totalIterations = s->totalIterations;
   if (kernelLaunches) *kernelLaunches = 0;
+  return MB2_OK;
+}
+int mb2_solver_get_solve_path(mb2_solver* s, int64_t out[15]) {
+  solvePathWords(s->path, out);
   return MB2_OK;
 }
 
@@ -566,4 +625,13 @@ extern "C" int emu_store_invariants(mb2_solver_function* f, int64_t out[6]) {
   }
   out[0] = offQuad; out[1] = overlap; out[2] = unaligned; out[3] = disorder; out[4] = multi; out[5] = int64_t(p.cells.size());
   return MB2_OK;
+}
+
+// The device the solve path is chosen for (SM count, opt-in shared memory per block, shared memory per SM).
+extern "C" void emu_set_device_limits(int32_t numSms, int32_t smemOptin, int32_t smemPerSm) { g_limits = DeviceLimits{numSms, smemOptin, smemPerSm}; }
+
+// The solve path of the solver's next solve (mb2_solver_get_solve_path afterwards), without solving: planning only.
+extern "C" int emu_choose_solve_path(mb2_solver* s) {
+  TilePlan tp;
+  return choosePath(s, tp);
 }

@@ -105,15 +105,6 @@ def solve_limit(n, path="dense"):
     return SOLVE_K[path] * max(n, 16) * EPS24
 
 
-def qr_max_chunk_rows(n, smem_bytes=200 * 1024):
-    """Jacobian rows the QR step folds at once beside R (qrMaxChunkRows): a block with more rows is split into several chunks."""
-    fixed = ((n * (n + 1) // 2 + 3) & ~3) + 3 * ((n + 3) & ~3) + ((n + 4) & ~3) + 8
-    floats = smem_bytes // 4
-    if floats <= fixed + (n + 1) * 9:
-        return 0
-    return min((floats - fixed) // (n + 1) - 1, 128) & ~1
-
-
 def one_step(ch, efs, theta0, opts, lib_path=None, enabled=None, rel_damping=None):
     """One Gauss-Newton step without line search from ``theta0`` (float32, B instances) with ``opts`` (min = max = 1 iteration).
     ``rel_damping``: raise the damping to that fraction of the largest diagonal entry of JtJ, so that the float factorisation completes
@@ -138,18 +129,6 @@ def one_step(ch, efs, theta0, opts, lib_path=None, enabled=None, rel_damping=Non
     out = solver.solve(theta0)
     delta = theta0.astype(np.float64)[:, cols] - out["params"].astype(np.float64)[:, cols]
     return solver, out, J, r, cols, delta, float(np.float32(opts.regularization))
-
-
-def dense_cholesky_dispatch(n, smem_optin):
-    """(NB, matrix in shared memory) of the dense Eigen-structured Cholesky for n unknowns, restating cholBlockSize / cholSmemBytes /
-    launchCholesky. This is a recomputation, not an observation: no entry point reports which variant launched, so a change of the
-    launcher's rule that this function does not follow goes unnoticed (the bound still holds on whichever variant ran)."""
-    eig = n if n < 32 else min(max((n // 8) // 16 * 16, 8), 128)
-    eig = max(eig, 1)
-    NB = 8 if eig <= 8 else (16 if eig <= 16 else 32)
-    ldp = ((n + 1 + 3) & ~3) + 4
-    smem = 4 * (NB * ldp + ((n + 3) & ~3)) + 16 + 4 * (n + 1) * (n | 1)
-    return NB, smem <= smem_optin
 
 
 def chain_case(n, positions, planes=0, B=1, seed=0, spread=0.1):

@@ -191,8 +191,8 @@ def test_chain22_cfg1():
 def test_dense_cholesky_backward_error(n):
     """One Gauss-Newton step through the dense Eigen-structured Cholesky at every block size (tests/f64ref.py: normwise backward error
     against the float64 normal equations of the emulator's own float Jacobian). The emulator factors on the host, so the kernel's
-    shared / global memory branch and the TF32 JtJ modes are GPU-only (tests/test_gpu_kernel_bounds.py). No path is asserted here: the
-    emulator has no plan statistics and no fallback, so the explicit cholesky_mode alone decides what it runs."""
+    shared / global memory branch and the TF32 JtJ modes are GPU-only (tests/test_gpu_kernel_bounds.py). The emulator runs the path the
+    library's chooseSolvePath picks (tests/test_solve_path.py asserts which); the explicit cholesky_mode pins it to the dense kernel."""
     from tests import f64ref as R
 
     if n < 10:
@@ -210,17 +210,17 @@ def test_dense_cholesky_backward_error(n):
 
 @pytest.mark.parametrize("chol", [ms.CHOLESKY_TILES_DENSE, ms.CHOLESKY_TILES_SPARSE])
 @pytest.mark.parametrize("jtj", [ms.JTJ_SPARSE_TILES, ms.JTJ_FP32_SIMT])
-@pytest.mark.parametrize("rig", ["humanoid", "humanoid_subset", "chain330"])
+@pytest.mark.parametrize("rig", ["humanoid", "humanoid_subset", "chain240"])
 def test_tile_cholesky_backward_error(rig, jtj, chol):
     """The level-scheduled tile Cholesky fed by the tile-sparse Gram and by the K-major JtJ, same bound as the dense kernel. The
-    emulator has no shared-memory budget: the 330-parameter chain, whose dense schedule sends CHOLESKY_AUTO to the dense kernel on the
-    device, runs the tile schedule here; the fused kernels, the 256 / 512-thread variants and the QR step are GPU-only. As above, the
-    explicit modes decide the path and none is asserted."""
+    240-parameter chain is a long system whose dense tile schedule still fits in shared memory; the 330-parameter chain's does not,
+    and the library, and with it the emulator, refuses the explicit tile modes there (tests/test_solve_path.py). The explicit modes decide the path;
+    the 256 / 512-thread variants and the QR step are GPU-only."""
     from tests import f64ref as R
 
     en = None
-    if rig == "chain330":
-        ch, efs, _ = R.chain_case(330, positions=12, seed=330)
+    if rig == "chain240":
+        ch, efs, _ = R.chain_case(240, positions=12, seed=240)
     else:
         ch, efs, _, _ = humanoid_problem(1, orientation=True)
         if rig == "humanoid_subset":

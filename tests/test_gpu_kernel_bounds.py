@@ -2,8 +2,8 @@
 dispatch edges of every launcher: wgmma work-item boundaries, the 32-row K block, leading-block stores, the dense Cholesky's block sizes
 and shared / global branch, the tile schedule's 256 / 512-thread rule, the fused kernels, the QR step, and batches larger than one wave.
 
-Every case asserts which path it ran (plan stats, fused profile, the dispatch rules recomputed from device attributes), so a change of a
-launch rule that sends a case down another path fails here instead of silently losing coverage. No oracle is used."""
+Every case asserts which path it ran (plan stats, fused profile, and the launch variants the solver reports with get_solve_path), so a
+change of a launch rule that sends a case down another path fails here instead of silently losing coverage. No oracle is used."""
 import numpy as np
 import pytest
 
@@ -206,8 +206,7 @@ def _dense_case(n):
     return ch, efs, None
 
 
-# n -> (NB, matrix in shared memory) on a device with 227 KB of opt-in shared memory per block. The variant is recomputed from the
-# launcher's rule (R.dense_cholesky_dispatch), not observed: plan stats only show that the dense kernel ran (no tiles, no strips).
+# n -> (NB, matrix in shared memory) on a device with 227 KB of opt-in shared memory per block, as the solver reports the variant it ran.
 DENSE = {1: (8, True), 8: (8, True), 9: (16, True), 16: (16, True), 17: (32, True), 31: (32, True), 32: (8, True), 127: (8, True),
          128: (16, True), 231: (16, True), 232: (16, False), 255: (16, False), 256: (32, False), 424: (32, False)}
 SOLVE_WORST = {}
@@ -215,12 +214,12 @@ SOLVE_WORST = {}
 
 @pytest.mark.parametrize("jtj", [ms.JTJ_FP32_SIMT, ms.JTJ_TF32X3])
 def test_dense_cholesky_backward_error_at_every_block_size(jtj):
-    optin, _, _ = _device()
     rows, fails = [], []
     for n, expected in DENSE.items():
-        assert R.dense_cholesky_dispatch(n, optin) == expected, (n, R.dense_cholesky_dispatch(n, optin), optin)
         ch, efs, en = _dense_case(n)
         solver, be, ns, _ = _step_case(ch, efs, np.zeros((1, ch.num_params)), _opts(cholesky_mode=ms.CHOLESKY_DENSE_EIGEN, jtj_mode=jtj), en)
+        path = solver.get_solve_path()
+        assert path["kind"] == "dense" and (path["dense_nb"], bool(path["dense_in_smem"])) == expected, (n, path)
         st = solver.get_plan_stats()
         assert ns == n and st["cholesky_tiles"] == 0 and st["strip_floats"] == 0 and solver.get_fused_profile()["fused"] == 0
         k = be / R.solve_limit(n) * R.SOLVE_K["dense"]
@@ -254,11 +253,11 @@ def test_backward_error_rejects_a_swapped_or_tile_dropped_step():
 def test_cholesky_auto_falls_back_to_the_dense_global_memory_kernel():
     """A chain with a constraint on its end effector couples every parameter pair: the dense tile schedule of n = 330 needs more than
     200 KB, so CHOLESKY_AUTO runs the dense kernel with the matrix in global memory, and an explicit tile request raises."""
-    optin, _, _ = _device()
     n = 330
     ch, efs, _ = R.chain_case(n, positions=12, seed=n)
-    assert R.dense_cholesky_dispatch(n, optin) == (32, False)
     solver, be, ns, _ = _step_case(ch, efs, np.zeros((1, n)), _opts(cholesky_mode=ms.CHOLESKY_AUTO))
+    path = solver.get_solve_path()
+    assert path["kind"] == "dense" and (path["dense_nb"], path["dense_in_smem"]) == (32, 0), path
     assert solver.get_plan_stats()["cholesky_tiles"] == 0 and solver.get_fused_profile()["fused"] == 0
     print(f"\n[AUTO fallback n=330] backward error {be:.3e} limit {R.solve_limit(n):.3e} k {be / R.solve_limit(n) * R.SOLVE_K['dense']:.3f}")
     SOLVE_WORST["dense"] = max(SOLVE_WORST.get("dense", 0.0), be / R.solve_limit(n) * R.SOLVE_K["dense"])
@@ -267,14 +266,6 @@ def test_cholesky_auto_falls_back_to_the_dense_global_memory_kernel():
     for mode in (ms.CHOLESKY_TILES_DENSE,):
         with pytest.raises(ms.MomentumB200Error):
             ms.GaussNewtonSolver(_opts(cholesky_mode=mode), fn).solve(np.zeros((1, n)))
-
-
-def _wide(bytes_lower, bytes_upper, smem_per_sm):
-    """The 512-thread rule of the tile kernels (2 (smem + 1 KB) > shared memory per SM), decided from bounds on the kernel's smem."""
-    if 2 * (bytes_lower + 1024) > smem_per_sm:
-        return True
-    assert 2 * (bytes_upper + 1024) <= smem_per_sm, (bytes_lower, bytes_upper)
-    return False
 
 
 TILE_CASES = {  # name: (rig, cholesky mode, jtj mode, fused mode, 512-thread variants expected (None: not asserted))
@@ -304,7 +295,6 @@ def _rig(name, B=1):
 @pytest.mark.parametrize("case", list(TILE_CASES))
 def test_tile_path_backward_error(case):
     rig, chol, jtj, fused, wide = TILE_CASES[case]
-    _, smem_per_sm, _ = _device()
     ch, efs, _, en = _rig(rig)
     solver, be, n, _ = _step_case(ch, efs, np.zeros((1, ch.num_params)), _opts(cholesky_mode=chol, jtj_mode=jtj, fused_mode=fused), en)
     st, prof = solver.get_plan_stats(), solver.get_fused_profile()
@@ -312,17 +302,13 @@ def test_tile_path_backward_error(case):
     assert prof["fused"] == {ms.FUSED_OFF: 0, ms.FUSED_PERSISTENT: 1, ms.FUSED_GRAM_CHOLESKY: 2}[fused]
     gram = jtj == ms.JTJ_AUTO
     assert (st["strip_floats"] > 0) == gram  # tile-sparse Gram on the strip layout, else K-major H through TMA
-    if fused == ms.FUSED_OFF and wide is not None:
-        # choleskyScheduledKernel: tiles + vectors (+ the schedule tables, below 24 KB on these rigs); gramTilesKernel: strips + tables
-        tiles = 1024 * st["cholesky_tiles"] + 1024
-        assert _wide(tiles, tiles + 24 * 1024 + 16 * n, smem_per_sm) == wide
-        if gram:
-            strips = 4 * st["strip_floats"]
-            assert _wide(strips, strips + 24 * 1024, smem_per_sm) == wide
+    if fused == ms.FUSED_OFF and wide is not None:  # choleskyScheduledKernel and gramTilesKernel: 512 threads when one CTA per SM fits
+        path = solver.get_solve_path()
+        assert path["chol_threads"] == (512 if wide else 256) and path["gram_threads"] == ((512 if wide else 256) if gram else 0), path
     if fused == ms.FUSED_GRAM_CHOLESKY:
         # Every Cholesky tile is dealt to one of the 8 warps (buildGramPlan), so the plan has at least ceil(tiles / 8) rounds per warp,
         # and the kernel launched, so at most kGramCholMaxRounds = 8: cfg3's plan sits within one round of the limit. A tile whose
-        # storage overlaps the strips (t * 256 < strip floats + 64) is parked in thread-local memory until the strips are dead.
+        # storage overlaps the strips (t * 256 < strip floats + 64) is parked in an L2 scratch slot until the strips are dead.
         tiles = st["cholesky_tiles"]
         assert -(-tiles // 8) >= 7, tiles
         parked = min(tiles, -(-(st["strip_floats"] + 64) // 256))
@@ -352,9 +338,11 @@ def test_qr_step_backward_error(case):
     solver, be, n, _ = _step_case(ch, efs, th0, _opts(linear_solver=ms.LINEAR_SOLVER_QR), en)
     st = solver.get_plan_stats()
     assert solver.get_fused_profile()["fused"] == 0 and st["cholesky_tiles"] == 0 and st["strip_floats"] == 0  # dense Jacobian layout
-    # chunking rule of the launcher (qrMaxChunkRows, recomputed): the widest block must need more than one chunk on the split case
-    chunk, widest = R.qr_max_chunk_rows(n), max(3 * len(e.parents) for e in efs)
-    assert chunk >= 8 and (widest > chunk) == (case == "humanoid_split_block"), (chunk, widest)
+    # the chunk rows the QR step ran with: the widest block must need more than one chunk on the split case
+    path = solver.get_solve_path()
+    chunk, widest = path["qr_max_chunk_rows"], max(3 * len(e.parents) for e in efs)
+    assert path["kind"] == "qr" and chunk >= 8 and (widest > chunk) == (case == "humanoid_split_block"), (chunk, widest)
+    assert (path["qr_chunks"] > len(efs)) == (case == "humanoid_split_block") and path["qr_widest_chunk"] == min(chunk, widest), path
     lim = R.solve_limit(n, "qr")
     SOLVE_WORST["qr"] = max(SOLVE_WORST.get("qr", 0.0), be / lim * R.SOLVE_K["qr"])
     print(f"\n[QR {case}] n={n} chunk rows {chunk}, widest block {widest}: backward error {be:.3e} limit {lim:.3e} k {be / lim * R.SOLVE_K['qr']:.5f}")
@@ -411,7 +399,7 @@ def test_instance_result_does_not_depend_on_the_batch(path):
     """About three waves plus a remainder (3 x SMs x 3 + 17 instances), instances starting at, near and far from their solution so that
     they stop at different iterations. A seeded sample re-solved alone must match its result inside the shuffled batch bit for bit."""
     rig, kw, expect = BATCH_PATHS[path]
-    optin, smem_per_sm, sms = _device()
+    _, _, sms = _device()
     B = 3 * sms * 3 + 17
     ch, efs, ts, rel_damping = _batch_rig(rig, B)
     rng = np.random.default_rng(11)
@@ -427,18 +415,16 @@ def test_instance_result_does_not_depend_on_the_batch(path):
     opts = ms.GaussNewtonSolverOptions(min_iterations=1, max_iterations=10, threshold=1e4, regularization=lam, **kw)
     solver = ms.GaussNewtonSolver(opts, fn)
     full = solver.solve(th_p)
-    st, fused = solver.get_plan_stats(), solver.get_fused_profile()["fused"]
+    st, fused, path = solver.get_plan_stats(), solver.get_fused_profile()["fused"], solver.get_solve_path()
     assert fused == {ms.FUSED_OFF: 0, ms.FUSED_PERSISTENT: 1, ms.FUSED_GRAM_CHOLESKY: 2}[opts.fused_mode]
     if expect == "dense":
         assert st["cholesky_tiles"] == 0 and st["strip_floats"] == 0
-        if rig.startswith("chain"):  # the global-memory branch, NB from the block-size rule (recomputed, see dense_cholesky_dispatch)
-            assert R.dense_cholesky_dispatch(ch.num_params, optin) == ((16 if ch.num_params < 256 else 32), False)
+        if rig.startswith("chain"):  # the global-memory branch, NB from the block-size rule
+            assert (path["dense_nb"], path["dense_in_smem"]) == ((16 if ch.num_params < 256 else 32), 0), path
     else:
         assert st["cholesky_tiles"] > 0 and (st["strip_floats"] > 0) == (opts.jtj_mode == ms.JTJ_SPARSE_TILES)
         if expect == "tiles_wide":
-            assert _wide(1024 * st["cholesky_tiles"] + 1024, None, smem_per_sm)
-            if st["strip_floats"] > 0:
-                assert _wide(4 * st["strip_floats"], None, smem_per_sm)
+            assert path["chol_threads"] == 512 and path["gram_threads"] == (512 if st["strip_floats"] > 0 else 0), path
     assert np.all(full["status"] == 0), np.unique(full["status"], return_counts=True)
     assert len(np.unique(full["iterations"])) >= 2, np.unique(full["iterations"])
     for k in np.random.default_rng(12).choice(B, 16, replace=False):
