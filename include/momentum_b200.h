@@ -291,6 +291,31 @@ int mb2_character_skin_points_backward_device(const mb2_character* c, int32_t ba
                                               int32_t rest_points_batched, const float* grad_points_device, float* grad_skel_state_device,
                                               float* grad_rest_points_device, void* cuda_stream);
 
+/* The identity blend shape of the character (BlendShape, blend_shape.h), host arrays, replacing any earlier one: base_shape [V][3] and
+ * shape_vectors [K][V][3] (shapeVectors_, 3V x K column-major, as it lies in memory). K < 1, V < 1, a null array or a non-finite value is
+ * MB2_ERR_INVALID_ARGUMENT and leaves any earlier blend shape in place (as does a failed upload). Fresh device buffers and a device
+ * synchronisation before the old ones are freed, as mb2_character_set_skinning. V is checked against the skinning's when skinning.
+ * mb2_character_clone copies the blend shape. */
+int mb2_character_set_blend_shape(mb2_character* c, int32_t num_shapes, int32_t num_vertices, const float* base_shape, const float* shape_vectors);
+/* K of the blend shape, 0 when the character has none */
+int32_t mb2_character_num_blend_shapes(const mb2_character* c);
+/* skinWithBlendShapes (blend_shape_skinning.cpp:50-140): the rest point of every vertex is base_shape + the first num_weights shape
+ * vectors weighted by blend_weights [B][num_weights] (1 <= num_weights <= K, computeDeltas' leftCols, blend_shape_base.cpp:18-24), then
+ * skinned as mb2_character_skin_points_device skins: skel_state [B][J][8] -> points [B][V][3]. No shaped rest mesh is written. Device
+ * memory on `cuda_stream`, asynchronous; batch == 0 is a no-op. No skinning or no blend shape, a blend shape whose V differs from the
+ * skinning's, num_weights out of range or so large that the weights of a 4-instance tile and the J transforms do not fit in shared
+ * memory, a null required pointer, batch < 0 or a pointer that is not device memory on the character's
+ * device is MB2_ERR_INVALID_ARGUMENT. */
+int mb2_character_skin_with_blend_shapes_device(const mb2_character* c, int32_t batch, const float* skel_state_device, const float* blend_weights_device,
+                                                int32_t num_weights, float* points_device, void* cuda_stream);
+/* its backward from dLoss/d points [B][V][3]: grad_skel_state [B][J][8] and grad_blend_weights [B][num_weights], both overwritten, a NULL
+ * output is skipped. Same rules as the forward. The call takes stream-ordered scratch from the device's default memory pool
+ * (cudaMallocAsync / cudaFreeAsync on `cuda_stream`): at most 256 MiB of shaped rest points plus the skin-points backward's scratch for
+ * the skel-state gradient, and at most 256 MiB of partial sums for the weight gradient. */
+int mb2_character_skin_with_blend_shapes_backward_device(const mb2_character* c, int32_t batch, const float* skel_state_device,
+                                                         const float* blend_weights_device, int32_t num_weights, const float* grad_points_device,
+                                                         float* grad_skel_state_device, float* grad_blend_weights_device, void* cuda_stream);
+
 /* Input contraction of the implicit-function backward of solve_ik (diff_ik d_gradient_d_input_dot): for block `index` and every
  * instance b, the derivatives of grad_theta E_index(theta_b) . v_b with respect to the block's inputs, at the targets, constraint weights
  * and offsets the handle currently holds:

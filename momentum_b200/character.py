@@ -83,6 +83,23 @@ class Skinning:
 
 
 @dataclass
+class BlendShape:
+    """The identity blend shape of a character (``BlendShape``, blend_shape.h): the rest mesh of blend weights w is
+    ``base_shape + sum_k w_k shape_vectors[k]`` over the first len(w) shape vectors (blend_shape_base.cpp:18-24)."""
+
+    base_shape: np.ndarray  # float32 [V,3]
+    shape_vectors: np.ndarray  # float32 [K,V,3]: shapeVectors_ (3V x K, column-major) as it lies in memory
+
+    @property
+    def num_shapes(self) -> int:
+        return int(self.shape_vectors.shape[0])
+
+    @property
+    def num_vertices(self) -> int:
+        return int(self.base_shape.shape[0])
+
+
+@dataclass
 class Character:
     parents: np.ndarray  # int32 [J], -1 = root, parents precede children
     offsets: np.ndarray  # float32 [J,3] translationOffset
@@ -95,6 +112,7 @@ class Character:
     limits: List[ParameterLimit] = field(default_factory=list)
     name: str = "character"
     skinning: Optional[Skinning] = None
+    blend_shape: Optional["BlendShape"] = None
 
     @property
     def num_joints(self) -> int:
@@ -564,6 +582,37 @@ def skin_points(ch: Character, skel_state, rest_points=None):
         wk = np.where(active[:, k], w[:, k], 0.0)
         out += (np.einsum("bvrc,bvc->bvr", L[:, j], x) + c[:, j]) * wk[None, :, None]
     return out[0] if single else out
+
+
+def synthetic_blend_shape(ch: Character, skinning: Skinning, num_shapes: int, seed: int = 0) -> BlendShape:
+    """A seeded blend shape over ``skinning``'s mesh: ``base_shape`` is its rest mesh, and each shape vector is a smooth displacement
+    field of three Gaussian bumps centred on random joints at theta = 0, each as wide as its bone and with an amplitude of 1 to 4 % of
+    the bone length, in a random direction."""
+    rng = np.random.default_rng(seed)
+    t, _, _ = forward_kinematics(ch, np.zeros((1, ch.num_params)))
+    t = t[0]
+    parents = np.asarray(ch.parents)
+    length = np.where(parents >= 0, np.linalg.norm(t - t[np.maximum(parents, 0)], axis=-1), 0.0)
+    length = np.where(length > 0, length, max(float(length.max()), 1.0))
+    x = np.asarray(skinning.rest_vertices, np.float64)
+    S = np.zeros((num_shapes,) + x.shape)
+    for k in range(num_shapes):
+        for j in rng.integers(0, ch.num_joints, 3):
+            d = rng.normal(size=3)
+            d *= rng.uniform(0.01, 0.04) * length[j] / np.linalg.norm(d)
+            sigma = length[j] + 1.0
+            S[k] += np.exp(-0.5 * np.sum((x - t[j]) ** 2, axis=-1) / sigma ** 2)[:, None] * d
+    return BlendShape(x.astype(np.float32), S.astype(np.float32))
+
+
+def skin_with_blend_shapes(ch: Character, skel_state, blend_weights):
+    """skinWithBlendShapes in float64 (blend_shape_skinning.cpp:50-140): the rest mesh base_shape + sum_k w_k shape_vectors[k] over the
+    first K' = len(w) shape vectors, skinned by ``skin_points``. skel_state [B,J,8] or [J,8]; blend_weights [K'] (shared) or [B,K']."""
+    bs = ch.blend_shape
+    w = np.asarray(blend_weights, np.float64)
+    S = np.asarray(bs.shape_vectors[:w.shape[-1]], np.float64)
+    rest = np.asarray(bs.base_shape, np.float64) + np.einsum("...k,kvc->...vc", w, S)
+    return skin_points(ch, skel_state, rest)
 
 
 def world_rotations(ch: Character, theta, parents, offsets_q):

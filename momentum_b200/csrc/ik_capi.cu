@@ -104,6 +104,10 @@ struct SkinBuffers {
   DeviceBuffer<float> rest, vertWeight, ibp, infWeight;
   DeviceBuffer<int32_t> vertStart, vertJoint, infVertex, segStart, segJoint, jointSegStart;
 };
+// the device copy of a HostBlendShape (BlendShapeTables)
+struct BlendShapeBuffers {
+  DeviceBuffer<float> baseShape, shapeVectors;
+};
 
 struct mb2_character {
   int device{0};
@@ -116,6 +120,9 @@ struct mb2_character {
   // linear-blend skinning (mb2_character_set_skinning): numVertices == 0 when there is none
   HostSkinning skin;
   std::unique_ptr<SkinBuffers> skinDev; // replaced whole by mb2_character_set_skinning, never rewritten in place
+  // identity blend shape (mb2_character_set_blend_shape): numShapes == 0 when there is none
+  HostBlendShape blend;
+  std::unique_ptr<BlendShapeBuffers> blendDev; // replaced whole by mb2_character_set_blend_shape
   CharacterTables tables() const; // the device copies above, as the kernels read them
 };
 
@@ -583,6 +590,11 @@ int mb2_character_clone(const mb2_character* c, int device, mb2_character** out)
     rc = mb2_character_set_skinning(copy, s.numVertices, s.restVertices.data(), index.data(), weight.data(), s.inverseBindPose.data());
     if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
   }
+  const HostBlendShape& bs = c->blend;
+  if (bs.numShapes > 0) {
+    rc = mb2_character_set_blend_shape(copy, bs.numShapes, bs.numVertices, bs.baseShape.data(), bs.shapeVectors.data());
+    if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
+  }
   *out = copy;
   return MB2_OK;
 }
@@ -614,6 +626,24 @@ int mb2_character_set_skinning(mb2_character* c, int32_t num_vertices, const flo
 }
 
 int32_t mb2_character_num_vertices(const mb2_character* c) { return c ? c->skin.numVertices : 0; }
+
+int mb2_character_set_blend_shape(mb2_character* c, int32_t num_shapes, int32_t num_vertices, const float* base_shape, const float* shape_vectors) {
+  MB2_CHECK(c != nullptr, "null character");
+  HostBlendShape b;
+  const std::string err = makeBlendShape(num_shapes, num_vertices, base_shape, shape_vectors, b);
+  if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
+  MB2_DEVICE_GUARD(c->device);
+  // as mb2_character_set_skinning: fresh buffers, and the device synchronised before the old ones are freed
+  auto d = std::make_unique<BlendShapeBuffers>();
+  MB2_CUDA(d->baseShape.upload(b.baseShape, nullptr));
+  MB2_CUDA(d->shapeVectors.upload(b.shapeVectors, nullptr));
+  MB2_CUDA(cudaDeviceSynchronize());
+  c->blendDev = std::move(d);
+  c->blend = std::move(b);
+  return MB2_OK;
+}
+
+int32_t mb2_character_num_blend_shapes(const mb2_character* c) { return c ? c->blend.numShapes : 0; }
 // The DEFINITION of a solver function (error-function blocks with their shared constraint data and weights, block weights, enabled
 // parameters) for `batch` instances of character `c` (normally a clone of f's character on another device). Per-instance data
 // (targets, per-instance weights / offsets) is not copied: it belongs to the instances the new function will hold.
@@ -999,6 +1029,62 @@ int mb2_character_skin_points_backward_device(const mb2_character* c, int32_t ba
   a.gradState = grad_skel_state_device;
   a.gradRest = grad_rest_points_device;
   MB2_CUDA(launchSkinPointsBackward(a, (cudaStream_t)cuda_stream));
+  return MB2_OK;
+}
+
+namespace {
+// both directions of mb2_character_skin_with_blend_shapes*_device: checks the arguments and fills the kernel arguments except the outputs
+int blendSkinArgs(const mb2_character* c, int32_t batch, const float* skelState, const float* blendWeights, int32_t numWeights, BlendSkinArgs& a) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(c->skin.numVertices > 0, "skin with blend shapes: the character has no skinning (mb2_character_set_skinning)");
+  MB2_CHECK(c->blend.numShapes > 0, "skin with blend shapes: the character has no blend shape (mb2_character_set_blend_shape)");
+  MB2_CHECK(c->blend.numVertices == c->skin.numVertices, "skin with blend shapes: the blend shape's vertex count differs from the skinning's");
+  MB2_CHECK(numWeights >= 1 && numWeights <= c->blend.numShapes, "skin with blend shapes: num_weights must be in [1, number of shape vectors]");
+  int rc = skinArgs(c, batch, skelState, nullptr, 0, a.skin);
+  if (rc != MB2_OK) return rc;
+  a.Bs = BlendShapeTables{c->blend.numShapes, c->blendDev->baseShape.p, c->blendDev->shapeVectors.p};
+  a.skin.restPoints = nullptr;
+  a.numWeights = numWeights;
+  a.blendWeights = blendWeights;
+  a.gradWeights = nullptr;
+  return MB2_OK;
+}
+} // namespace
+
+int mb2_character_skin_with_blend_shapes_device(const mb2_character* c, int32_t batch, const float* skel_state_device, const float* blend_weights_device,
+                                                int32_t num_weights, float* points_device, void* cuda_stream) {
+  BlendSkinArgs a{};
+  int rc = blendSkinArgs(c, batch, skel_state_device, blend_weights_device, num_weights, a);
+  if (rc != MB2_OK || batch == 0) return rc;
+  MB2_CHECK(skel_state_device != nullptr && blend_weights_device != nullptr && points_device != nullptr, "null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(isDeviceMemoryOn(skel_state_device, c->device) && isDeviceMemoryOn(blend_weights_device, c->device) && isDeviceMemoryOn(points_device, c->device),
+            "skin with blend shapes: every array must be device memory on the character's device");
+  MB2_CHECK(blendSkinFits(a), "skin with blend shapes: num_weights is too large for the device's shared memory");
+  NvtxRange range("skinWithBlendShapes");
+  a.skin.points = points_device;
+  MB2_CUDA(launchSkinWithBlendShapes(a, (cudaStream_t)cuda_stream));
+  return MB2_OK;
+}
+
+int mb2_character_skin_with_blend_shapes_backward_device(const mb2_character* c, int32_t batch, const float* skel_state_device,
+                                                         const float* blend_weights_device, int32_t num_weights, const float* grad_points_device,
+                                                         float* grad_skel_state_device, float* grad_blend_weights_device, void* cuda_stream) {
+  BlendSkinArgs a{};
+  int rc = blendSkinArgs(c, batch, skel_state_device, blend_weights_device, num_weights, a);
+  if (rc != MB2_OK || batch == 0) return rc;
+  MB2_CHECK(skel_state_device != nullptr && blend_weights_device != nullptr && grad_points_device != nullptr, "null argument");
+  MB2_DEVICE_GUARD(c->device);
+  bool onDevice = isDeviceMemoryOn(skel_state_device, c->device) && isDeviceMemoryOn(blend_weights_device, c->device) &&
+                  isDeviceMemoryOn(grad_points_device, c->device);
+  for (float* o : {grad_skel_state_device, grad_blend_weights_device}) onDevice = onDevice && (o == nullptr || isDeviceMemoryOn(o, c->device));
+  MB2_CHECK(onDevice, "skin with blend shapes: every array must be device memory on the character's device");
+  MB2_CHECK(blendSkinFits(a), "skin with blend shapes: num_weights is too large for the device's shared memory");
+  NvtxRange range("skinWithBlendShapesBackward");
+  a.skin.gradPoints = grad_points_device;
+  a.skin.gradState = grad_skel_state_device;
+  a.gradWeights = grad_blend_weights_device;
+  MB2_CUDA(launchSkinWithBlendShapesBackward(a, (cudaStream_t)cuda_stream));
   return MB2_OK;
 }
 

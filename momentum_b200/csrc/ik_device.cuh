@@ -986,4 +986,26 @@ MB2_HD F3 skinRestGradient(const SkinTables& S, const float* M, int v, F3 g) {
   return r;
 }
 
+// ---- Blend-shape skinning (skinWithBlendShapes, blend_shape_skinning.cpp:50-140) ----------------------------------------------------
+// The rest point of vertex v for T instances at once, x_t = base_v + sum_{k < K'} S_kv w_tk with k in order: each S_kv is read once
+// for all T. w: [K'][T], instance fastest. The sum of an instance does not depend on T or on the other instances.
+template <int T>
+MB2_HD void blendShapeRest(const BlendShapeTables& Bs, int V, int v, const float* w, int numWeights, F3 (&x)[T]) {
+  const F3 b = ld3(Bs.baseShape + 3 * size_t(v));
+#pragma unroll
+  for (int t = 0; t < T; ++t) x[t] = b;
+  for (int k = 0; k < numWeights; ++k) {
+    const F3 s = ld3(Bs.shapeVectors + (size_t(k) * V + v) * 3);
+#pragma unroll
+    for (int t = 0; t < T; ++t) x[t] = x[t] + s * w[k * T + t];
+  }
+}
+// Backward: dL/dw_k = sum_v <S_kv, r_v> with r_v = dL/dx_v (skinRestGradient). One vertex's contribution, component by component.
+MB2_HD float blendWeightAccumulate(float acc, F3 s, F3 r) {
+  acc += s.x * r.x;
+  acc += s.y * r.y;
+  acc += s.z * r.z;
+  return acc;
+}
+
 } // namespace mb2

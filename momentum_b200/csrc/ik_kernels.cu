@@ -550,6 +550,232 @@ cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Skinning with an identity blend shape (ik_device.cuh blendShapeRest / blendWeightAccumulate), on the skinning's building blocks.
+// A work item is (a tile of T instances, a block of kSkinThreads vertices, one per thread).
+//   blendSkinKernel<T, kRestOnly>   the tile's weights [K'][T] in shared memory; each thread forms its vertex's rest points for the T
+//                                   instances in registers (every shape-vector element it loads serves the whole tile), then per
+//                                   instance the CTA writes the J skinning transforms to shared memory and blends. kRestOnly writes
+//                                   the rest points instead (the backward's scratch for the skel-state gradient).
+//   blendWeightPartialKernel<T>     per instance the rest-point gradient of the block's vertices (skinRestGradient) to shared memory,
+//                                   then threads = (quarter of the block, k) sum <S_kv, r_tv> over their quarter's vertices in order;
+//                                   the quarters are added in order into one partial sum per (vertex block, instance, k).
+//   blendWeightFinishKernel         lanes = (instance, k): the vertex blocks summed in order.
+// No atomics; an instance's sums run in an order fixed by V and K' alone, so neither the batch, the tile nor the grid changes a bit.
+// ------------------------------------------------------------------------------------------------
+constexpr int kBlendTileMax = 16;                        // instances per tile when the batch fills the grid with them
+constexpr int kBlendTileMin = 4;                         // otherwise
+constexpr int kBlendGroups = kSkinThreads / 64;          // blendWeightPartialKernel: thread = (group, k of a 64-wide block of K')
+constexpr int kBlendGroupVerts = kSkinThreads / kBlendGroups;
+constexpr size_t kBlendRestBudget = size_t(256) << 20;   // skel-state backward: shaped rest points of a slice of instances
+
+template <int T, bool kRestOnly>
+__global__ void __launch_bounds__(kSkinThreads, 2) blendSkinKernel(const BlendSkinArgs a, int b0, int nb, float* rest) {
+  extern __shared__ __align__(16) float sm[];
+  const SkinTables& S = a.skin.S;
+  const int V = S.numVertices, J = a.skin.numJoints, Kp = a.numWeights;
+  float* W = sm;                // [K'][T]
+  float* M = sm + Kp * T;       // [J][12], one instance at a time
+  const int vBlocks = (V + kSkinThreads - 1) / kSkinThreads;
+  const long items = long((nb + T - 1) / T) * vBlocks;
+  for (long it = blockIdx.x; it < items; it += gridDim.x) {
+    const int tb = b0 + int(it / vBlocks) * T, nt = min(T, b0 + nb - tb);
+    const int v = int(it % vBlocks) * kSkinThreads + threadIdx.x;
+    __syncthreads(); // the previous item's readers of W and M are done
+    for (int i = threadIdx.x; i < Kp * T; i += blockDim.x) {
+      const int k = i / T, t = i % T;
+      W[i] = t < nt ? a.blendWeights[size_t(tb + t) * Kp + k] : 0.f;
+    }
+    __syncthreads();
+    F3 x[T];
+    if (v < V) blendShapeRest<T>(a.Bs, V, v, W, Kp, x);
+#pragma unroll
+    for (int t = 0; t < T; ++t) {
+      if (t >= nt) break;
+      if constexpr (kRestOnly) {
+        if (v < V) {
+          float* o = rest + (size_t(tb - b0 + t) * V + v) * 3;
+          o[0] = x[t].x; o[1] = x[t].y; o[2] = x[t].z;
+        }
+      } else {
+        __syncthreads();
+        for (int j = threadIdx.x; j < J; j += blockDim.x)
+          skinTransform(a.skin.skelState + (size_t(tb + t) * J + j) * 8, S.inverseBindPose + j * kSkinIbpStride, M + j * kSkinIbpStride);
+        __syncthreads();
+        if (v < V) {
+          const F3 p = skinBlend(S, M, v, x[t]);
+          float* o = a.skin.points + (size_t(tb + t) * V + v) * 3;
+          o[0] = p.x; o[1] = p.y; o[2] = p.z;
+        }
+      }
+    }
+  }
+}
+
+// partial: [vBlocks][nb][K']
+template <int T>
+__global__ void __launch_bounds__(kSkinThreads) blendWeightPartialKernel(const BlendSkinArgs a, int b0, int nb, float* partial) {
+  extern __shared__ __align__(16) float sm[];
+  constexpr int kStride = 3 * T + 4;                        // floats per vertex of R: 16-byte rows, fewer bank conflicts on the writes
+  const SkinTables& S = a.skin.S;
+  const int V = S.numVertices, J = a.skin.numJoints, Kp = a.numWeights;
+  float* R = sm;                                             // [kSkinThreads][kStride]: r_tv at 3 t
+  float* P = R + kSkinThreads * kStride;                     // [kBlendGroups][T][64]
+  float* M = P + kBlendGroups * T * 64;                      // [J][12]
+  const int vBlocks = (V + kSkinThreads - 1) / kSkinThreads;
+  const long items = long((nb + T - 1) / T) * vBlocks;
+  const int g = threadIdx.x / 64, kl = threadIdx.x % 64;
+  for (long it = blockIdx.x; it < items; it += gridDim.x) {
+    const int tb = b0 + int(it / vBlocks) * T, nt = min(T, b0 + nb - tb);
+    const int vb = int(it % vBlocks), v = vb * kSkinThreads + threadIdx.x;
+    float* mine = R + threadIdx.x * kStride;
+    for (int t = 0; t < nt; ++t) {
+      __syncthreads(); // the previous readers of M (and, at t = 0, of R and P) are done
+      for (int j = threadIdx.x; j < J; j += blockDim.x)
+        skinTransform(a.skin.skelState + (size_t(tb + t) * J + j) * 8, S.inverseBindPose + j * kSkinIbpStride, M + j * kSkinIbpStride);
+      __syncthreads();
+      const F3 r = v < V ? skinRestGradient(S, M, v, ld3(a.skin.gradPoints + (size_t(tb + t) * V + v) * 3)) : f3(0.f, 0.f, 0.f);
+      mine[3 * t] = r.x; mine[3 * t + 1] = r.y; mine[3 * t + 2] = r.z;
+    }
+    for (int t = nt; t < T; ++t) mine[3 * t] = mine[3 * t + 1] = mine[3 * t + 2] = 0.f;
+    const int vEnd = min(kBlendGroupVerts, V - vb * kSkinThreads - g * kBlendGroupVerts); // this group's vertices in the block
+    for (int kb = 0; kb < Kp; kb += 64) {
+      __syncthreads(); // R is complete; the previous k block's readers of P are done
+      const int k = kb + kl;
+      float acc[T];
+#pragma unroll
+      for (int t = 0; t < T; ++t) acc[t] = 0.f;
+      if (k < Kp) {
+        const float* sv = a.Bs.shapeVectors + (size_t(k) * V + vb * kSkinThreads + g * kBlendGroupVerts) * 3;
+        const float* rv = R + g * kBlendGroupVerts * kStride;
+        for (int i = 0; i < vEnd; ++i) {
+          const F3 s = ld3(sv + 3 * i);
+#pragma unroll
+          for (int t = 0; t < T; ++t) acc[t] = blendWeightAccumulate(acc[t], s, ld3(rv + i * kStride + 3 * t));
+        }
+      }
+#pragma unroll
+      for (int t = 0; t < T; ++t) P[(g * T + t) * 64 + kl] = acc[t];
+      __syncthreads();
+      for (int i = threadIdx.x; i < nt * 64; i += blockDim.x) {
+        const int t = i / 64, kk = i % 64;
+        if (kb + kk >= Kp) continue;
+        float s = P[t * 64 + kk];
+        for (int q = 1; q < kBlendGroups; ++q) s += P[(q * T + t) * 64 + kk];
+        partial[(size_t(vb) * nb + (tb - b0 + t)) * Kp + kb + kk] = s;
+      }
+    }
+  }
+}
+
+__global__ void blendWeightFinishKernel(const float* partial, int vBlocks, int nb, int Kp, float* out) {
+  const size_t n = size_t(nb) * Kp;
+  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
+    float s = partial[i];
+    for (int c = 1; c < vBlocks; ++c) s += partial[size_t(c) * n + i];
+    out[i] = s;
+  }
+}
+
+namespace {
+size_t blendSkinSmem(const BlendSkinArgs& a, int T) { return (size_t(a.numWeights) * T + size_t(a.skin.numJoints) * kSkinIbpStride) * sizeof(float); }
+size_t blendWeightSmem(const BlendSkinArgs& a, int T) {
+  return (size_t(kSkinThreads) * (3 * T + 4) + size_t(kBlendGroups) * T * 64 + size_t(a.skin.numJoints) * kSkinIbpStride) * sizeof(float);
+}
+} // namespace
+
+bool blendSkinFits(const BlendSkinArgs& a) {
+  return blendSkinSmem(a, kBlendTileMin) <= size_t(g_maxSmemOptin) && blendWeightSmem(a, kBlendTileMin) <= size_t(g_maxSmemOptin);
+}
+
+namespace {
+
+// The widest tile that still gives every resident CTA a work item and fits in shared memory; the tile changes how often a shape vector
+// is read, not the result.
+template <class K16, class K4>
+cudaError_t chooseBlendTile(K16 wide, size_t smemWide, K4 narrow, size_t smemNarrow, int V, int nb, int* T, int* grid) {
+  const long vBlocks = (V + kSkinThreads - 1) / kSkinThreads;
+  if (smemWide <= size_t(g_maxSmemOptin)) {
+    int slots = 0;
+    const cudaError_t e = persistentGrid(wide, kSkinThreads, smemWide, 1L << 30, &slots);
+    if (e != cudaSuccess) return e;
+    const long wideItems = (nb + kBlendTileMax - 1) / kBlendTileMax * vBlocks;
+    if (wideItems >= slots) { *T = kBlendTileMax; *grid = slots; return cudaSuccess; }
+  }
+  *T = kBlendTileMin;
+  return persistentGrid(narrow, kSkinThreads, smemNarrow, (nb + kBlendTileMin - 1) / kBlendTileMin * vBlocks, grid);
+}
+
+template <bool kRestOnly>
+cudaError_t launchBlendSkin(const BlendSkinArgs& a, int b0, int nb, float* rest, cudaStream_t stream) {
+  int T = 0, grid = 0;
+  const size_t s16 = blendSkinSmem(a, kBlendTileMax), s4 = blendSkinSmem(a, kBlendTileMin);
+  cudaError_t e = chooseBlendTile(blendSkinKernel<kBlendTileMax, kRestOnly>, s16, blendSkinKernel<kBlendTileMin, kRestOnly>, s4, a.skin.S.numVertices, nb, &T, &grid);
+  if (e != cudaSuccess) return e;
+  if (T == kBlendTileMax) blendSkinKernel<kBlendTileMax, kRestOnly><<<grid, kSkinThreads, s16, stream>>>(a, b0, nb, rest);
+  else blendSkinKernel<kBlendTileMin, kRestOnly><<<grid, kSkinThreads, s4, stream>>>(a, b0, nb, rest);
+  return cudaGetLastError();
+}
+} // namespace
+
+cudaError_t launchSkinWithBlendShapes(const BlendSkinArgs& a, cudaStream_t stream) {
+  if (a.skin.batch <= 0) return cudaSuccess;
+  return launchBlendSkin<false>(a, 0, a.skin.batch, nullptr, stream);
+}
+
+cudaError_t launchSkinWithBlendShapesBackward(const BlendSkinArgs& a, cudaStream_t stream) {
+  const int B = a.skin.batch, V = a.skin.S.numVertices, J = a.skin.numJoints, Kp = a.numWeights;
+  if (B <= 0) return cudaSuccess;
+  cudaError_t e = cudaSuccess;
+  if (a.skin.gradState != nullptr) {
+    // the shaped rest points of a slice of instances, then skin_points' own state-gradient path with them as batched rest points
+    const size_t perInstance = size_t(V) * 3 * sizeof(float);
+    const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(B), kBlendRestBudget / perInstance)));
+    float* rest = nullptr;
+    e = cudaMallocAsync(reinterpret_cast<void**>(&rest), perInstance * slice, stream);
+    if (e != cudaSuccess) return e;
+    for (int b0 = 0; e == cudaSuccess && b0 < B; b0 += slice) {
+      const int nb = std::min(slice, B - b0);
+      e = launchBlendSkin<true>(a, b0, nb, rest, stream);
+      SkinArgs s = a.skin;
+      s.batch = nb;
+      s.skelState += size_t(b0) * J * 8;
+      s.gradPoints += size_t(b0) * V * 3;
+      s.gradState += size_t(b0) * J * 8;
+      s.restPoints = rest;
+      s.restBatched = 1;
+      s.points = nullptr;
+      s.gradRest = nullptr;
+      if (e == cudaSuccess) e = launchSkinPointsBackward(s, stream);
+    }
+    const cudaError_t f = cudaFreeAsync(rest, stream);
+    if (e == cudaSuccess) e = f;
+  }
+  if (e != cudaSuccess || a.gradWeights == nullptr) return e;
+  const int vBlocks = (V + kSkinThreads - 1) / kSkinThreads;
+  const size_t perInstance = size_t(vBlocks) * Kp * sizeof(float);
+  const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(B), kSkinPartialBudget / perInstance)));
+  float* partial = nullptr;
+  e = cudaMallocAsync(reinterpret_cast<void**>(&partial), perInstance * slice, stream);
+  if (e != cudaSuccess) return e;
+  for (int b0 = 0; e == cudaSuccess && b0 < B; b0 += slice) {
+    const int nb = std::min(slice, B - b0);
+    int T = 0, grid = 0;
+    const size_t s16 = blendWeightSmem(a, kBlendTileMax), s4 = blendWeightSmem(a, kBlendTileMin);
+    e = chooseBlendTile(blendWeightPartialKernel<kBlendTileMax>, s16, blendWeightPartialKernel<kBlendTileMin>, s4, V, nb, &T, &grid);
+    if (e != cudaSuccess) break;
+    if (T == kBlendTileMax) blendWeightPartialKernel<kBlendTileMax><<<grid, kSkinThreads, s16, stream>>>(a, b0, nb, partial);
+    else blendWeightPartialKernel<kBlendTileMin><<<grid, kSkinThreads, s4, stream>>>(a, b0, nb, partial);
+    const size_t n = size_t(nb) * Kp;
+    blendWeightFinishKernel<<<unsigned(std::min<size_t>((n + kSkinThreads - 1) / kSkinThreads, 4096)), kSkinThreads, 0, stream>>>(
+        partial, vBlocks, nb, Kp, a.gradWeights + size_t(b0) * Kp);
+    e = cudaGetLastError();
+  }
+  const cudaError_t f = cudaFreeAsync(partial, stream);
+  if (e == cudaSuccess) e = f;
+  return e;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Input gradients of one Position / Orientation block, d/d input [grad_theta E . v] (ik_device.cuh tangent* / *InputGradient), in the
 // per-instance frame of skeletonStateKernel:
 //   lanes = parameters: theta, and v gated by the enabled set;  fkPasses with the DOF axes;  tangentPasses: each joint's own motion,

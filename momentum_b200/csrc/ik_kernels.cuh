@@ -166,6 +166,21 @@ struct SkinArgs {
 // Both enqueue on `stream`; the backward takes bounded stream-ordered scratch (cudaMallocAsync) for its partial sums.
 cudaError_t launchSkinPoints(const SkinArgs& a, cudaStream_t stream);
 cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream);
+// blendSkinKernel / blendWeightPartialKernel / blendWeightFinishKernel: skinning with an identity blend shape (skinWithBlendShapes,
+// blend_shape_skinning.cpp:50-140) and its backward
+struct BlendSkinArgs {
+  SkinArgs skin;             // S, numJoints, batch, skelState; forward: points; backward: gradPoints, gradState (optional). No rest points.
+  BlendShapeTables Bs;
+  int32_t numWeights;        // K', 1 <= K' <= K
+  const float* blendWeights; // [B][K']
+  float* gradWeights;        // backward, optional: [B][K']
+};
+// Both enqueue on `stream`; the backward takes bounded stream-ordered scratch (cudaMallocAsync): the shaped rest points of a slice of
+// instances for the skel-state gradient (then launchSkinPointsBackward on them), and per-vertex-block partial sums of the weight gradient.
+// Whether the narrowest tile's shared memory (its weights [K'][4] and the J transforms) fits on the device: K' and J bound it
+bool blendSkinFits(const BlendSkinArgs& a);
+cudaError_t launchSkinWithBlendShapes(const BlendSkinArgs& a, cudaStream_t stream);
+cudaError_t launchSkinWithBlendShapesBackward(const BlendSkinArgs& a, cudaStream_t stream);
 // inputGradientKernel: d/d input [grad_theta E . v] of one Position or Orientation (matrix difference) block with the L2 loss, per
 // instance: the input contraction of solve_ik's implicit-function backward
 struct InputGradientArgs {

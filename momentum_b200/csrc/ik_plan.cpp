@@ -176,6 +176,24 @@ std::string makeSkinning(const HostCharacter& ch, int32_t numVertices, const flo
   return "";
 }
 
+std::string makeBlendShape(int32_t numShapes, int32_t numVertices, const float* baseShape, const float* shapeVectors, HostBlendShape& out) {
+  if (numVertices < 1) return "blend shape: the mesh must have at least one vertex";
+  if (numShapes < 1) return "blend shape: there must be at least one shape vector";
+  if (!(baseShape && shapeVectors)) return "blend shape: null argument";
+  const size_t n = size_t(numVertices) * 3;
+  for (size_t k = 0; k < n; ++k)
+    if (!std::isfinite(baseShape[k])) return "blend shape: the base shape must be finite";
+  for (size_t k = 0; k < n * size_t(numShapes); ++k)
+    if (!std::isfinite(shapeVectors[k])) return "blend shape: shape vectors must be finite";
+  HostBlendShape b;
+  b.numShapes = numShapes;
+  b.numVertices = numVertices;
+  b.baseShape.assign(baseShape, baseShape + n);
+  b.shapeVectors.assign(shapeVectors, shapeVectors + n * size_t(numShapes));
+  out = std::move(b);
+  return "";
+}
+
 CharacterTables hostCharacterTables(const HostCharacter& ch) {
   CharacterTables C{};
   C.numJoints = ch.numJoints;

@@ -60,6 +60,14 @@ struct HostSkinning {
   int32_t numSegments() const { return int32_t(segJoint.size()); }
 };
 
+// The identity blend shape of a character (BlendShape, blend_shape.h / blend_shape_base.h): the rest mesh is
+// baseShape + shapeVectors.leftCols(K') w (blend_shape_skinning.cpp:50-140). Built and validated by makeBlendShape only.
+struct HostBlendShape {
+  int32_t numShapes{0}, numVertices{0};
+  std::vector<float> baseShape;    // [V][3]
+  std::vector<float> shapeVectors; // [K][V][3]: shapeVectors_ (3V x K, column-major) as it lies in memory
+};
+
 struct HostErrorFunction {
   int32_t kind{0}; // 0 position, 1 orientation, 2 orientation rot-diff, 3 state, 4 limit, 5 plane, 6 model parameters
   float weight{1.f};
@@ -107,6 +115,9 @@ std::string setParameterLimits(HostCharacter& ch, int32_t count, const mb2_param
 // (linear_skinning.cpp:76-80); the slots after it are ignored whatever they hold.
 std::string makeSkinning(const HostCharacter& ch, int32_t numVertices, const float* restVertices, const int32_t* skinIndex, const float* skinWeight,
                          const float* inverseBindPose, HostSkinning& out);
+// baseShape [V][3], shapeVectors [K][V][3]; K >= 1, V >= 1, every value finite. The blend shape's V is checked against the skinning's
+// where both are used, not here: either may be replaced first.
+std::string makeBlendShape(int32_t numShapes, int32_t numVertices, const float* baseShape, const float* shapeVectors, HostBlendShape& out);
 std::string positionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* offsets,
                                   const float* weights, HostErrorFunction& out);
 std::string instancedPositionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* weights,

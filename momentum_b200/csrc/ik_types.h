@@ -156,4 +156,11 @@ struct SkinTables {
   const int32_t* jointSegStart; // [J+1] segments of each joint, in list order
 };
 
+// Blend-shape tables (HostBlendShape, makeBlendShape), shared by the whole batch; the mesh's V is the skinning's.
+struct BlendShapeTables {
+  int32_t numShapes;            // K; an instance uses the first K' <= K (computeDeltas' leftCols, blend_shape_base.cpp:18-24)
+  const float* baseShape;       // [V][3]
+  const float* shapeVectors;    // [K][V][3]
+};
+
 } // namespace mb2

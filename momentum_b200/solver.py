@@ -77,6 +77,8 @@ CABI_SYMBOLS = [
     "mb2_add_orientation_error_function_instanced", "mb2_solver_function_input_gradients_device",
     "mb2_solver_function_implicit_direction_device", "mb2_solver_function_get_sweep_launch", "mb2_solver_get_solve_path",
     "mb2_character_set_skinning", "mb2_character_num_vertices", "mb2_character_skin_points_device", "mb2_character_skin_points_backward_device",
+    "mb2_character_set_blend_shape", "mb2_character_num_blend_shapes", "mb2_character_skin_with_blend_shapes_device",
+    "mb2_character_skin_with_blend_shapes_backward_device",
 ]
 
 _libs = {}
@@ -188,6 +190,11 @@ def load_library(path: Optional[str] = None):
         L.mb2_character_num_vertices.argtypes = [vp]
         L.mb2_character_skin_points_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]
         L.mb2_character_skin_points_backward_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp, vp, vp]
+    if hasattr(L, "mb2_character_set_blend_shape"):
+        L.mb2_character_set_blend_shape.argtypes = [vp, C.c_int32, C.c_int32, _fp, _fp]
+        L.mb2_character_num_blend_shapes.argtypes = [vp]
+        L.mb2_character_skin_with_blend_shapes_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]
+        L.mb2_character_skin_with_blend_shapes_backward_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp, vp, vp]
     _libs[path] = L
     return L
 
@@ -279,6 +286,14 @@ class DeviceCharacter(_Base):
         self.skinning = None
         if character.skinning is not None:
             self.set_skinning(character.skinning)
+        # A blend shape the library rejects is reported by the blend-shape calls, not here: the rig, its skinning and every other use of
+        # the handle do not depend on it.
+        self.blend_shape, self.blend_shape_error = None, None
+        if character.blend_shape is not None:
+            try:
+                self.set_blend_shape(character.blend_shape)
+            except (MomentumB200Error, ValueError) as e:
+                self.blend_shape_error = str(e)
 
     def set_skinning(self, skinning: mc.Skinning):
         """Uploads ``skinning`` (replacing any earlier one); ``self.skinning`` is the object uploaded."""
@@ -307,6 +322,36 @@ class DeviceCharacter(_Base):
         self._check(self._L.mb2_character_skin_points_backward_device(
             self._h, int(batch), C.c_void_p(state_device_ptr), C.c_void_p(rest_device_ptr or None), int(bool(rest_batched)),
             C.c_void_p(grad_points_device_ptr), C.c_void_p(grad_state_device_ptr or None), C.c_void_p(grad_rest_device_ptr or None), C.c_void_p(stream)))
+
+    def set_blend_shape(self, blend_shape: mc.BlendShape):
+        """Uploads ``blend_shape`` (replacing any earlier one); ``self.blend_shape`` is the object uploaded."""
+        base, vectors = np.asarray(blend_shape.base_shape), np.asarray(blend_shape.shape_vectors)
+        if base.ndim != 2 or base.shape[1] != 3 or vectors.ndim != 3 or vectors.shape[1:] != base.shape:
+            raise ValueError(f"blend shape: base_shape must be [V, 3] and shape_vectors [K, V, 3] with the same V, got {base.shape} and {vectors.shape}")
+        K, V = vectors.shape[0], base.shape[0]
+        bs, bsp = _f32(base)
+        sv, svp = _f32(vectors)
+        self._check(self._L.mb2_character_set_blend_shape(self._h, K, V, bsp, svp))
+        self.blend_shape, self.blend_shape_error = blend_shape, None
+
+    @property
+    def num_blend_shapes(self) -> int:
+        return int(self._L.mb2_character_num_blend_shapes(self._h))
+
+    def skin_with_blend_shapes_device(self, batch: int, state_device_ptr: int, weights_device_ptr: int, num_weights: int, points_device_ptr: int,
+                                      stream: int = 0):
+        """Points [B][V][3] of skeleton states [B][J][8], the rest mesh shaped by blend weights [B][num_weights]. float32 device memory on
+        this character's device, enqueued on ``stream``."""
+        self._check(self._L.mb2_character_skin_with_blend_shapes_device(self._h, int(batch), C.c_void_p(state_device_ptr), C.c_void_p(weights_device_ptr),
+                                                                        int(num_weights), C.c_void_p(points_device_ptr), C.c_void_p(stream)))
+
+    def skin_with_blend_shapes_backward_device(self, batch: int, state_device_ptr: int, weights_device_ptr: int, num_weights: int,
+                                               grad_points_device_ptr: int, grad_state_device_ptr: int, grad_weights_device_ptr: int, stream: int = 0):
+        """dLoss/d skeleton state [B][J][8] and dLoss/d blend weights [B][num_weights] from dLoss/d points [B][V][3]. A 0 output pointer
+        is skipped."""
+        self._check(self._L.mb2_character_skin_with_blend_shapes_backward_device(
+            self._h, int(batch), C.c_void_p(state_device_ptr), C.c_void_p(weights_device_ptr), int(num_weights), C.c_void_p(grad_points_device_ptr),
+            C.c_void_p(grad_state_device_ptr or None), C.c_void_p(grad_weights_device_ptr or None), C.c_void_p(stream)))
 
     def skeleton_state_device(self, batch: int, params_device_ptr: int, state_device_ptr: int, stream: int = 0):
         """Skeleton state [B][J][8] (t, q xyzw, s) of model parameters [B][n], float32 device memory on this character's device, enqueued

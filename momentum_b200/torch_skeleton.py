@@ -114,16 +114,16 @@ _skin_handles = {}
 
 
 def _skinned_device_character(ch: mc.Character, device: torch.device) -> ms.DeviceCharacter:
-    """One DeviceCharacter per (character, device) holding ``ch.skinning``. When ``character.skinning`` is replaced, a new handle is
+    """One DeviceCharacter per (character, device) holding ``ch.skinning`` and ``ch.blend_shape``. When either is replaced, a new handle is
     made instead of uploading into the old one: a graph recorded with the old skinning keeps its handle (``ctx.dc``) and its tables, and
     no kernel in flight on another stream reads tables that are being replaced. An old handle is freed with the last graph that uses it."""
     index = device.index if device.index is not None else torch.cuda.current_device()
     key = (id(ch), index)
     entry = _skin_handles.get(key)
-    if entry is None or entry[1] is not ch.skinning:
-        entry = (ch, ch.skinning, ms.DeviceCharacter(ch, index))  # the character is kept alive so that its id stays unique
+    if entry is None or entry[1] is not ch.skinning or entry[2] is not ch.blend_shape:
+        entry = (ch, ch.skinning, ch.blend_shape, ms.DeviceCharacter(ch, index))  # the character is kept alive so that its id stays unique
         _skin_handles[key] = entry
-    return entry[2]
+    return entry[3]
 
 
 def skin_points(character, skel_state: torch.Tensor, rest_points=None) -> torch.Tensor:
@@ -158,3 +158,83 @@ def skin_points(character, skel_state: torch.Tensor, rest_points=None) -> torch.
             raise ValueError(f"rest_points must be [V, 3] or [B, V, 3] with V = {V} and the skel_state's B, got {tuple(rest_points.shape)}")
     dc = _device_character(character, skel_state.device) if is_handle else _skinned_device_character(ch, skel_state.device)
     return _SkinPoints.apply(dc, skel_state, rest_points)
+
+
+class _SkinWithBlendShapes(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, dc, skel_state, blend_weights):
+        J, V = dc.character.num_joints, dc.skinning.num_vertices
+        dev = skel_state.device
+        st = skel_state.detach().to(torch.float32).reshape(-1, J, 8).contiguous()
+        B, K = st.shape[0], blend_weights.shape[-1]
+        w = blend_weights.detach().to(device=dev, dtype=torch.float32).expand(B, K).contiguous()
+        out = torch.empty(B, V, 3, device=dev, dtype=torch.float32)
+        dc.skin_with_blend_shapes_device(B, st.data_ptr(), w.data_ptr(), K, out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        ctx.dc, ctx.skinning, ctx.blend_shape, ctx.V = dc, dc.skinning, dc.blend_shape, V
+        ctx.state_shape, ctx.state_dtype = skel_state.shape, skel_state.dtype
+        ctx.weights_shape, ctx.weights_dtype = blend_weights.shape, blend_weights.dtype
+        ctx.save_for_backward(st, w)
+        return out.reshape(*skel_state.shape[:-2], V, 3).to(skel_state.dtype)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_points):
+        st, w = ctx.saved_tensors
+        dc = ctx.dc
+        if dc.skinning is not ctx.skinning or dc.blend_shape is not ctx.blend_shape:
+            raise RuntimeError("skin_with_blend_shapes backward: the DeviceCharacter's skinning or blend shape was replaced (set_skinning / "
+                               "set_blend_shape) after the forward; keep one DeviceCharacter per mesh, or pass the Character and replace "
+                               "its attributes instead")
+        B, J, _ = st.shape
+        K = w.shape[1]
+        dev = st.device
+        g = grad_points.to(device=dev, dtype=torch.float32).reshape(B, ctx.V, 3).contiguous()
+        need_state, need_weights = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        gs = torch.empty(B, J, 8, device=dev, dtype=torch.float32) if need_state else None
+        gw = torch.empty(B, K, device=dev, dtype=torch.float32) if need_weights else None
+        dc.skin_with_blend_shapes_backward_device(B, st.data_ptr(), w.data_ptr(), K, g.data_ptr(), gs.data_ptr() if gs is not None else 0,
+                                                  gw.data_ptr() if gw is not None else 0, torch.cuda.current_stream(dev).cuda_stream)
+        if gw is not None and len(ctx.weights_shape) == 1:
+            gw = gw.sum(0)  # weights shared by the batch
+        return (None, None if gs is None else gs.reshape(ctx.state_shape).to(ctx.state_dtype),
+                None if gw is None else gw.to(ctx.weights_dtype))
+
+
+def skin_with_blend_shapes(character, skel_state: torch.Tensor, blend_weights: torch.Tensor) -> torch.Tensor:
+    """Skinning with the character's identity blend shape (momentum ``skinWithBlendShapes``): the rest mesh of each instance is
+    ``base_shape + sum_k w_k shape_vectors[k]`` over the first K' = ``blend_weights.shape[-1]`` shape vectors, skinned as ``skin_points``
+    skins, without a shaped rest mesh in memory. ``skel_state`` [J, 8] or [B, J, 8] on a CUDA device; ``blend_weights`` [K'] shared by
+    the batch (its gradient is the batch sum) or [B, K'], 1 <= K' <= K. Returns points [V, 3] or [B, V, 3] in the skel_state's dtype,
+    computed in float32. Differentiable once with respect to ``skel_state`` and ``blend_weights``.
+
+    ``character`` is a ``momentum_b200.character.Character`` with ``skinning`` and ``blend_shape`` set: replacing either attribute is safe
+    at any time, and graphs recorded before keep what they were recorded with. Or it is a ``solver.DeviceCharacter``, which uses what was
+    uploaded to it; the backward of a graph recorded before a later ``set_skinning`` or ``set_blend_shape`` on that handle raises."""
+    if not torch.is_tensor(skel_state) or not skel_state.is_cuda:
+        raise ValueError("skin_with_blend_shapes runs on CUDA tensors (there is no CPU fallback)")
+    is_handle = isinstance(character, ms.DeviceCharacter)
+    ch = character.character if is_handle else character
+    if not isinstance(ch, mc.Character):
+        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
+    sk = character.skinning if is_handle else ch.skinning
+    bs = character.blend_shape if is_handle else ch.blend_shape
+    if sk is None:
+        raise ValueError("the character has no skinning")
+    if bs is None:
+        rejected = character.blend_shape_error if is_handle else None
+        raise ValueError("the character has no blend shape" + (f" (its upload was rejected: {rejected})" if rejected else ""))
+    if bs.num_vertices != sk.num_vertices:
+        raise ValueError(f"the blend shape has {bs.num_vertices} vertices but the skinning has {sk.num_vertices}")
+    J = ch.num_joints
+    if skel_state.dim() not in (2, 3) or skel_state.shape[-2:] != (J, 8):
+        raise ValueError(f"skel_state must be [J, 8] or [B, J, 8] with J = {J}, got {tuple(skel_state.shape)}")
+    if not torch.is_tensor(blend_weights) or blend_weights.device != skel_state.device:
+        raise ValueError("blend_weights must be a tensor on the skel_state's device")
+    B = skel_state.shape[0] if skel_state.dim() == 3 else None
+    K = blend_weights.shape[-1] if blend_weights.dim() in (1, 2) else 0
+    if not (1 <= K <= bs.num_shapes and (blend_weights.dim() == 1 or (B is not None and blend_weights.shape[0] == B))):
+        raise ValueError(f"blend_weights must be [K'] or [B, K'] with 1 <= K' <= {bs.num_shapes} and the skel_state's B, got {tuple(blend_weights.shape)}")
+    dc = _device_character(character, skel_state.device) if is_handle else _skinned_device_character(ch, skel_state.device)
+    if dc.blend_shape is None:
+        raise ValueError(f"the character's blend shape was rejected: {dc.blend_shape_error}")
+    return _SkinWithBlendShapes.apply(dc, skel_state, blend_weights)
