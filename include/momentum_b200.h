@@ -316,6 +316,28 @@ int mb2_character_skin_with_blend_shapes_backward_device(const mb2_character* c,
                                                          const float* blend_weights_device, int32_t num_weights, const float* grad_points_device,
                                                          float* grad_skel_state_device, float* grad_blend_weights_device, void* cuda_stream);
 
+/* The triangles of the character's mesh (Mesh::faces, mesh.h), a host array faces [F][3] of vertex indices in [0, num_vertices),
+ * replacing any earlier ones; num_faces == 0 with a null array removes them. num_vertices < 1, num_faces < 0, 3 x num_faces beyond
+ * int32, a null array with num_faces > 0 or an index out of range is MB2_ERR_INVALID_ARGUMENT and leaves the earlier faces in place
+ * (as does a failed upload). Degenerate faces and faces that repeat an index are accepted. The vertex -> corner table the kernels
+ * gather from is built here, once. Fresh device buffers and a device synchronisation before the old ones are freed, as
+ * mb2_character_set_skinning. mb2_character_clone copies the faces. */
+int mb2_character_set_mesh_faces(mb2_character* c, int32_t num_vertices, int32_t num_faces, const int32_t* faces);
+/* F of the mesh faces, 0 when the character has none */
+int32_t mb2_character_num_faces(const mb2_character* c);
+/* Area-weighted vertex normals (pymomentum compute_vertex_normals, tensor_skinning.cpp:354-383): n_v = the sum of (x1 - x0) x (x2 - x0)
+ * over every corner of every face that is vertex v, faces ascending, corners in order (the sum of MeshT::updateNormals, mesh.cpp:17-51),
+ * and normals = n_v / max(|n_v|, 1e-12) (torch.nn.functional.normalize): an isolated vertex gives 0. positions [B][V][3] -> normals
+ * [B][V][3], V = the faces' num_vertices. Non-finite positions propagate (updateNormals' skip of NaN faces is not copied). Device
+ * memory on `cuda_stream`, asynchronous; batch == 0 is a no-op. No faces, a null pointer, batch < 0 or a pointer that is not device
+ * memory on the character's device is MB2_ERR_INVALID_ARGUMENT. No atomics: an instance gets the same bits alone as in any batch. */
+int mb2_character_vertex_normals_device(const mb2_character* c, int32_t batch, const float* positions_device, float* normals_device, void* cuda_stream);
+/* its backward from dLoss/d normals [B][V][3]: grad_positions [B][V][3], overwritten, the exact derivative including the clamp branch.
+ * Same rules as the forward. The call takes stream-ordered scratch from the device's default memory pool (cudaMallocAsync /
+ * cudaFreeAsync on `cuda_stream`): [slice][V][3] floats of at most 256 MiB, the instances processed in slices. */
+int mb2_character_vertex_normals_backward_device(const mb2_character* c, int32_t batch, const float* positions_device, const float* grad_normals_device,
+                                                 float* grad_positions_device, void* cuda_stream);
+
 /* Input contraction of the implicit-function backward of solve_ik (diff_ik d_gradient_d_input_dot): for block `index` and every
  * instance b, the derivatives of grad_theta E_index(theta_b) . v_b with respect to the block's inputs, at the targets, constraint weights
  * and offsets the handle currently holds:

@@ -76,6 +76,7 @@ class Skinning:
     skin_index: np.ndarray  # int32 [V,8]
     skin_weight: np.ndarray  # float32 [V,8]
     inverse_bind_pose: np.ndarray  # float32 [J,3,4]: the top 3x4 of Affine3f::matrix()
+    faces: Optional[np.ndarray] = None  # int32 [F,3]: the triangles over rest_vertices (Mesh::faces, mesh.h)
 
     @property
     def num_vertices(self) -> int:
@@ -513,21 +514,59 @@ def _quat_matrix(q):
                      np.stack([2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)], -1)], -2)
 
 
+def _rest_frames(ch: Character):
+    """World positions of the joints at theta = 0, and the inverse bind pose (the inverse of the rest-pose world transform, as momentum
+    builds it) as float64 [J,3,4]."""
+    t, q, s = forward_kinematics(ch, np.zeros((1, ch.num_params)))
+    t, q, s = t[0], q[0], s[0]
+    R = _quat_matrix(q)
+    Rt = np.swapaxes(R, -1, -2) / s[:, None, None]
+    return t, np.concatenate([Rt, -(Rt @ t[:, :, None])], -1)
+
+
+def _children(ch: Character):
+    children = [[] for _ in range(ch.num_joints)]
+    for j, p in enumerate(ch.parents):
+        if p >= 0:
+            children[p].append(j)
+    return children
+
+
+def _bone_skin_weights(ch: Character, t, children, j: int, length: float, x, rng):
+    """The skin index and weights [n,8] of vertices x [n,3] around the bone of joint j: weights fall off with the distance to the joint,
+    its parent, its children and its grandparent and are normalised; the smallest are dropped so that a vertex keeps 1 to 8 influences,
+    largest first."""
+    n = x.shape[0]
+    p = int(ch.parents[j])
+    cand = ([p] if p >= 0 else []) + [j] + children[j]
+    if p >= 0 and ch.parents[p] >= 0 and len(cand) < MAX_SKIN_JOINTS:
+        cand.append(int(ch.parents[p]))
+    cand = np.array(cand[:MAX_SKIN_JOINTS])
+    dist = np.linalg.norm(x[:, None, :] - t[cand][None], axis=-1)
+    w = np.exp(-(dist / (0.5 * length + 2.0)) ** 2) + 1e-12
+    w /= w.sum(1, keepdims=True)
+    w[w < rng.uniform(0.02, 0.3, (n, 1))] = 0.0  # 1 to len(cand) influences per vertex
+    w[np.arange(n), w.argmax(1)] = np.maximum(w.max(1), 1e-3)
+    order = np.argsort(-w, axis=1, kind="stable")
+    wi = np.zeros((n, MAX_SKIN_JOINTS))
+    ii = np.zeros((n, MAX_SKIN_JOINTS), np.int32)
+    wi[:, :len(cand)] = np.take_along_axis(w, order, 1)
+    ii[:, :len(cand)] = cand[order]
+    wi /= wi.sum(1, keepdims=True)
+    ii[wi == 0.0] = 0
+    return ii, wi
+
+
 def synthetic_skinning(ch: Character, vertices_per_joint: int, seed: int = 0) -> Skinning:
     """A seeded mesh around the bones of ``ch`` at theta = 0: each joint gets ``vertices_per_joint`` vertices scattered around the
     segment from its parent to it (a blob for a root). Weights fall off with the distance to the joint, its parent and its children and
     are normalised; the smallest are dropped so that a vertex keeps 1 to 8 influences, largest first. The inverse bind pose is the
     inverse of the rest-pose world transform, as momentum builds it."""
     rng = np.random.default_rng(seed)
-    J = ch.num_joints
-    t, q, s = forward_kinematics(ch, np.zeros((1, ch.num_params)))
-    t, q, s = t[0], q[0], s[0]
-    children = [[] for _ in range(J)]
-    for j, p in enumerate(ch.parents):
-        if p >= 0:
-            children[p].append(j)
+    t, ibp = _rest_frames(ch)
+    children = _children(ch)
     verts, index, weight = [], [], []
-    for j in range(J):
+    for j in range(ch.num_joints):
         p = int(ch.parents[j])
         start = t[p] if p >= 0 else t[j]
         length = float(np.linalg.norm(t[j] - start))
@@ -536,28 +575,74 @@ def synthetic_skinning(ch: Character, vertices_per_joint: int, seed: int = 0) ->
         d = rng.normal(size=(vertices_per_joint, 3))
         d *= (radius * rng.uniform(0.5, 1.0, (vertices_per_joint, 1))) / np.linalg.norm(d, axis=1, keepdims=True)
         x = start + u * (t[j] - start) + d
-        cand = ([p] if p >= 0 else []) + [j] + children[j]
-        if p >= 0 and ch.parents[p] >= 0 and len(cand) < MAX_SKIN_JOINTS:
-            cand.append(int(ch.parents[p]))
-        cand = np.array(cand[:MAX_SKIN_JOINTS])
-        dist = np.linalg.norm(x[:, None, :] - t[cand][None], axis=-1)
-        w = np.exp(-(dist / (0.5 * length + 2.0)) ** 2) + 1e-12
-        w /= w.sum(1, keepdims=True)
-        w[w < rng.uniform(0.02, 0.3, (vertices_per_joint, 1))] = 0.0  # 1 to len(cand) influences per vertex
-        w[np.arange(vertices_per_joint), w.argmax(1)] = np.maximum(w.max(1), 1e-3)
-        order = np.argsort(-w, axis=1, kind="stable")
-        wi = np.zeros((vertices_per_joint, MAX_SKIN_JOINTS))
-        ii = np.zeros((vertices_per_joint, MAX_SKIN_JOINTS), np.int32)
-        wi[:, :len(cand)] = np.take_along_axis(w, order, 1)
-        ii[:, :len(cand)] = cand[order]
-        wi /= wi.sum(1, keepdims=True)
-        ii[wi == 0.0] = 0
+        ii, wi = _bone_skin_weights(ch, t, children, j, length, x, rng)
         verts.append(x); index.append(ii); weight.append(wi)
-    R = _quat_matrix(q)
-    Rt = np.swapaxes(R, -1, -2) / s[:, None, None]
-    ibp = np.concatenate([Rt, -(Rt @ t[:, :, None])], -1)
     return Skinning(np.concatenate(verts).astype(np.float32), np.concatenate(index).astype(np.int32), np.concatenate(weight).astype(np.float32),
                     ibp.astype(np.float32))
+
+
+def synthetic_tube_mesh(ch: Character, rings: int, segments: int, seed: int = 0) -> Skinning:
+    """A seeded, closed, triangulated mesh around the bones of ``ch`` at theta = 0, skinned by ``synthetic_skinning``'s weight rule: each
+    joint gets a tube of ``rings`` x ``segments`` vertices along the segment from its parent to it (for a root or a zero-length bone, a
+    tube along y as long as its diameter), with a seeded jitter of the radius per vertex so that face areas differ. Each quad is split
+    into two triangles, and a fan closes each end; every triangle's (x1 - x0) x (x2 - x0) points out of its tube, so each edge of a tube
+    appears once in each direction. rings = 12, segments = 12 gives 10 368 vertices on humanoid72; rings = segments = 8 gives 19 200 on
+    bodyhands300."""
+    assert rings >= 2 and segments >= 3
+    rng = np.random.default_rng(seed)
+    t, ibp = _rest_frames(ch)
+    children = _children(ch)
+    R, S = rings, segments
+    ring_idx = np.arange(R)[:, None] * S
+    k = np.arange(S)[None, :]
+    k1 = (k + 1) % S
+    a, b, c, d = (ring_idx[:-1] + k), (ring_idx[:-1] + k1), (ring_idx[1:] + k), (ring_idx[1:] + k1)
+    quads = np.concatenate([np.stack([a, b, c], -1).reshape(-1, 3), np.stack([b, d, c], -1).reshape(-1, 3)])
+    fan = np.arange(1, S - 1)
+    cap0 = np.stack([np.zeros_like(fan), fan + 1, fan], -1)
+    cap1 = (R - 1) * S + np.stack([np.zeros_like(fan), fan, fan + 1], -1)
+    tube_faces = np.concatenate([quads, cap0, cap1]).astype(np.int64)
+    theta = 2.0 * np.pi * np.arange(S) / S
+    verts, index, weight, faces = [], [], [], []
+    for j in range(ch.num_joints):
+        p = int(ch.parents[j])
+        start = t[p] if p >= 0 else t[j]
+        length = float(np.linalg.norm(t[j] - start))
+        radius = 0.2 * length + 1.0
+        if length > 0.0:
+            axis, end = (t[j] - start) / length, t[j]
+        else:
+            axis = np.array([0.0, 1.0, 0.0])
+            start, end = t[j] - radius * axis, t[j] + radius * axis
+        helper = np.array([1.0, 0.0, 0.0]) if abs(axis[0]) < 0.9 else np.array([0.0, 0.0, 1.0])
+        b1 = np.cross(axis, helper)
+        b1 /= np.linalg.norm(b1)
+        b2 = np.cross(axis, b1)  # (b1, b2, axis) is right-handed
+        r = radius * rng.uniform(0.7, 1.0, (R, S, 1))
+        radial = np.cos(theta)[:, None] * b1 + np.sin(theta)[:, None] * b2
+        s = (np.arange(R) / (R - 1))[:, None, None]
+        x = (start + s * (end - start) + r * radial[None]).reshape(R * S, 3)
+        ii, wi = _bone_skin_weights(ch, t, children, j, length, x, rng)
+        faces.append(tube_faces + j * R * S)
+        verts.append(x); index.append(ii); weight.append(wi)
+    return Skinning(np.concatenate(verts).astype(np.float32), np.concatenate(index).astype(np.int32), np.concatenate(weight).astype(np.float32),
+                    ibp.astype(np.float32), np.concatenate(faces).astype(np.int32))
+
+
+def vertex_normals(faces, positions):
+    """Area-weighted vertex normals in float64 (pymomentum compute_vertex_normals, tensor_skinning.cpp:354-383): per vertex the sum of
+    (x1 - x0) x (x2 - x0) over every corner of every face that is that vertex, faces ascending and corners in order, then
+    n / max(|n|, 1e-12). positions [B,V,3] or [V,3]; non-finite positions propagate."""
+    x = np.asarray(positions, np.float64)
+    single = x.ndim == 2
+    x = x.reshape((-1,) + x.shape[-2:])
+    f = np.asarray(faces, np.int64).reshape(-1, 3)
+    n_f = np.cross(x[:, f[:, 1]] - x[:, f[:, 0]], x[:, f[:, 2]] - x[:, f[:, 0]])
+    n = np.zeros_like(x)
+    # ufunc.at applies the corners in the order given: face-major, corners in order
+    np.add.at(n, (slice(None), f.reshape(-1)), np.repeat(n_f, 3, axis=1))
+    out = n / np.maximum(np.linalg.norm(n, axis=-1, keepdims=True), 1e-12)
+    return out[0] if single else out
 
 
 def skin_points(ch: Character, skel_state, rest_points=None):

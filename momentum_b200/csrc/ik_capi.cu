@@ -108,6 +108,10 @@ struct SkinBuffers {
 struct BlendShapeBuffers {
   DeviceBuffer<float> baseShape, shapeVectors;
 };
+// the device copy of a HostMeshFaces (MeshFaceTables)
+struct MeshFaceBuffers {
+  DeviceBuffer<int32_t> faces, vertStart, vertCorner;
+};
 
 struct mb2_character {
   int device{0};
@@ -123,6 +127,9 @@ struct mb2_character {
   // identity blend shape (mb2_character_set_blend_shape): numShapes == 0 when there is none
   HostBlendShape blend;
   std::unique_ptr<BlendShapeBuffers> blendDev; // replaced whole by mb2_character_set_blend_shape
+  // mesh faces (mb2_character_set_mesh_faces): numVertices == 0 when there are none
+  HostMeshFaces faces;
+  std::unique_ptr<MeshFaceBuffers> facesDev; // replaced whole by mb2_character_set_mesh_faces
   CharacterTables tables() const; // the device copies above, as the kernels read them
 };
 
@@ -595,6 +602,11 @@ int mb2_character_clone(const mb2_character* c, int device, mb2_character** out)
     rc = mb2_character_set_blend_shape(copy, bs.numShapes, bs.numVertices, bs.baseShape.data(), bs.shapeVectors.data());
     if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
   }
+  const HostMeshFaces& mf = c->faces;
+  if (mf.numVertices > 0) {
+    rc = mb2_character_set_mesh_faces(copy, mf.numVertices, mf.numFaces, mf.faces.data());
+    if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
+  }
   *out = copy;
   return MB2_OK;
 }
@@ -644,6 +656,30 @@ int mb2_character_set_blend_shape(mb2_character* c, int32_t num_shapes, int32_t 
 }
 
 int32_t mb2_character_num_blend_shapes(const mb2_character* c) { return c ? c->blend.numShapes : 0; }
+
+int mb2_character_set_mesh_faces(mb2_character* c, int32_t num_vertices, int32_t num_faces, const int32_t* faces) {
+  MB2_CHECK(c != nullptr, "null character");
+  HostMeshFaces m;
+  if (!(num_faces == 0 && faces == nullptr)) { // that pair removes the faces
+    const std::string err = makeMeshFaces(num_vertices, num_faces, faces, m);
+    if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
+  }
+  MB2_DEVICE_GUARD(c->device);
+  // as mb2_character_set_skinning: fresh buffers, and the device synchronised before the old ones are freed
+  std::unique_ptr<MeshFaceBuffers> d;
+  if (m.numVertices > 0) {
+    d = std::make_unique<MeshFaceBuffers>();
+    MB2_CUDA(d->faces.upload(m.faces, nullptr));
+    MB2_CUDA(d->vertStart.upload(m.vertStart, nullptr));
+    MB2_CUDA(d->vertCorner.upload(m.vertCorner, nullptr));
+  }
+  MB2_CUDA(cudaDeviceSynchronize());
+  c->facesDev = std::move(d);
+  c->faces = std::move(m);
+  return MB2_OK;
+}
+
+int32_t mb2_character_num_faces(const mb2_character* c) { return c ? c->faces.numFaces : 0; }
 // The DEFINITION of a solver function (error-function blocks with their shared constraint data and weights, block weights, enabled
 // parameters) for `batch` instances of character `c` (normally a clone of f's character on another device). Per-instance data
 // (targets, per-instance weights / offsets) is not copied: it belongs to the instances the new function will hold.
@@ -1085,6 +1121,52 @@ int mb2_character_skin_with_blend_shapes_backward_device(const mb2_character* c,
   a.skin.gradState = grad_skel_state_device;
   a.gradWeights = grad_blend_weights_device;
   MB2_CUDA(launchSkinWithBlendShapesBackward(a, (cudaStream_t)cuda_stream));
+  return MB2_OK;
+}
+
+namespace {
+// both directions of mb2_character_vertex_normals*_device: checks the arguments and fills the tables
+int normalArgs(const mb2_character* c, int32_t batch, NormalArgs& a) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(c->faces.numVertices > 0, "vertex normals: the character has no mesh faces (mb2_character_set_mesh_faces)");
+  MB2_CHECK(batch >= 0, "batch must not be negative");
+  a = NormalArgs{};
+  a.M = MeshFaceTables{c->faces.numVertices, c->faces.numFaces, c->facesDev->faces.p, c->facesDev->vertStart.p, c->facesDev->vertCorner.p};
+  a.batch = batch;
+  return MB2_OK;
+}
+} // namespace
+
+int mb2_character_vertex_normals_device(const mb2_character* c, int32_t batch, const float* positions_device, float* normals_device, void* cuda_stream) {
+  NormalArgs a;
+  int rc = normalArgs(c, batch, a);
+  if (rc != MB2_OK || batch == 0) return rc;
+  MB2_CHECK(positions_device != nullptr && normals_device != nullptr, "vertex normals: null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(isDeviceMemoryOn(positions_device, c->device) && isDeviceMemoryOn(normals_device, c->device),
+            "vertex normals: every array must be device memory on the character's device");
+  NvtxRange range("vertexNormals");
+  a.positions = positions_device;
+  a.normals = normals_device;
+  MB2_CUDA(launchVertexNormals(a, (cudaStream_t)cuda_stream));
+  return MB2_OK;
+}
+
+int mb2_character_vertex_normals_backward_device(const mb2_character* c, int32_t batch, const float* positions_device, const float* grad_normals_device,
+                                                 float* grad_positions_device, void* cuda_stream) {
+  NormalArgs a;
+  int rc = normalArgs(c, batch, a);
+  if (rc != MB2_OK || batch == 0) return rc;
+  MB2_CHECK(positions_device != nullptr && grad_normals_device != nullptr && grad_positions_device != nullptr, "vertex normals: null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(isDeviceMemoryOn(positions_device, c->device) && isDeviceMemoryOn(grad_normals_device, c->device) &&
+                isDeviceMemoryOn(grad_positions_device, c->device),
+            "vertex normals: every array must be device memory on the character's device");
+  NvtxRange range("vertexNormalsBackward");
+  a.positions = positions_device;
+  a.gradNormals = grad_normals_device;
+  a.gradPositions = grad_positions_device;
+  MB2_CUDA(launchVertexNormalsBackward(a, (cudaStream_t)cuda_stream));
   return MB2_OK;
 }
 

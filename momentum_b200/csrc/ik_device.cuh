@@ -1008,4 +1008,27 @@ MB2_HD float blendWeightAccumulate(float acc, F3 s, F3 r) {
   return acc;
 }
 
+// ---- Vertex normals (pymomentum compute_vertex_normals, tensor_skinning.cpp:354-383; the sum of MeshT::updateNormals, mesh.cpp:17-51) --
+// n_v = sum over the corners of the faces that are v of the face's (x1 - x0) x (x2 - x0), faces ascending, corners in order; the normal
+// is n_v / max(|n_v|, 1e-12) (torch.nn.functional.normalize). Non-finite positions propagate (updateNormals' NaN-face skip is not copied).
+constexpr float kNormalEps = 1e-12f;
+
+MB2_HD F3 faceNormal(F3 x0, F3 x1, F3 x2) { return cross(x1 - x0, x2 - x0); }
+MB2_HD F3 normalizeClamped(F3 n) {
+  const float d = fmaxf(sqrtf(dot(n, n)), kNormalEps);
+  return f3(n.x / d, n.y / d, n.z / d);
+}
+// Backward of normalizeClamped at n for the upstream g: h = (g - u (u . g)) / |n| with u = n / |n|, or g / 1e-12 on the clamp branch
+// (|n| < 1e-12, an isolated vertex or one whose faces have zero area included).
+MB2_HD F3 normalGradient(F3 n, F3 g) {
+  const float len = sqrtf(dot(n, n));
+  if (len < kNormalEps) return f3(g.x / kNormalEps, g.y / kNormalEps, g.z / kNormalEps);
+  const F3 u = f3(n.x / len, n.y / len, n.z / len);
+  const F3 p = g - u * dot(u, g);
+  return f3(p.x / len, p.y / len, p.z / len);
+}
+// The gradient that corner k of a face adds to its vertex, with G the sum of h over the face's corners in order:
+// d/dx_k [G . (x1 - x0) x (x2 - x0)] = (x_{k+1} - x_{k+2}) x G, corners mod 3.
+MB2_HD F3 cornerGradient(F3 xNext, F3 xPrev, F3 G) { return cross(xNext - xPrev, G); }
+
 } // namespace mb2

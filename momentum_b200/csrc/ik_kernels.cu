@@ -776,6 +776,132 @@ cudaError_t launchSkinWithBlendShapesBackward(const BlendSkinArgs& a, cudaStream
 }
 
 // ------------------------------------------------------------------------------------------------
+// Vertex normals (ik_device.cuh faceNormal / normalizeClamped / normalGradient / cornerGradient). A thread serves one vertex for a tile
+// of kNormalTile instances: each entry of the vertex's corner list and its face are read once for the whole tile, then the positions of
+// each instance are gathered. Work items are (tile, block of kNormalThreads vertices) with the vertex blocks fastest, so the CTAs in
+// flight gather from the positions of a few instances, which stay in L2.
+//   vertexNormalKernel<false>   n_v summed over the vertex's corner list in order, then normalised: the normals.
+//   vertexNormalKernel<true>    the same n_v, then h_v = normalGradient(n_v, upstream) to scratch: the first pass of the backward.
+//   vertexNormalGradKernel      per corner k of face f in the list, G_f = h_i0 + h_i1 + h_i2, then cornerGradient: the second pass.
+// No atomics: every output is a sum in the order of the corner list, the same for any batch and launch shape.
+// ------------------------------------------------------------------------------------------------
+constexpr int kNormalThreads = 256;
+constexpr int kNormalTile = 4;
+constexpr size_t kNormalScratchBudget = size_t(256) << 20; // h of a slice of instances
+
+template <bool kGrad>
+__global__ void __launch_bounds__(kNormalThreads) vertexNormalKernel(const NormalArgs a, int b0, int nb, float* h) {
+  const MeshFaceTables M = a.M;
+  const int V = M.numVertices;
+  const int vBlocks = (V + kNormalThreads - 1) / kNormalThreads;
+  const long items = long((nb + kNormalTile - 1) / kNormalTile) * vBlocks;
+  for (long it = blockIdx.x; it < items; it += gridDim.x) {
+    const int v = int(it % vBlocks) * kNormalThreads + threadIdx.x;
+    if (v >= V) continue;
+    const int tb = b0 + int(it / vBlocks) * kNormalTile, nt = min(kNormalTile, b0 + nb - tb);
+    F3 n[kNormalTile];
+#pragma unroll
+    for (int t = 0; t < kNormalTile; ++t) n[t] = f3(0.f, 0.f, 0.f);
+    for (int c = M.vertStart[v]; c < M.vertStart[v + 1]; ++c) {
+      const int* f = M.faces + (M.vertCorner[c] / 3) * 3;
+      const int i0 = f[0], i1 = f[1], i2 = f[2];
+#pragma unroll
+      for (int t = 0; t < kNormalTile; ++t)
+        if (t < nt) {
+          const float* x = a.positions + size_t(tb + t) * V * 3;
+          n[t] = n[t] + faceNormal(ld3(x + 3 * i0), ld3(x + 3 * i1), ld3(x + 3 * i2));
+        }
+    }
+#pragma unroll
+    for (int t = 0; t < kNormalTile; ++t)
+      if (t < nt) {
+        const size_t at = (size_t(tb + t) * V + v) * 3;
+        F3 r;
+        float* o;
+        if constexpr (kGrad) {
+          r = normalGradient(n[t], ld3(a.gradNormals + at));
+          o = h + (size_t(tb + t - b0) * V + v) * 3;
+        } else {
+          r = normalizeClamped(n[t]);
+          o = a.normals + at;
+        }
+        o[0] = r.x; o[1] = r.y; o[2] = r.z;
+      }
+  }
+}
+
+// h: [nb][V][3] of the instances b0 .. b0 + nb
+__global__ void __launch_bounds__(kNormalThreads) vertexNormalGradKernel(const NormalArgs a, int b0, int nb, const float* h) {
+  const MeshFaceTables M = a.M;
+  const int V = M.numVertices;
+  const int vBlocks = (V + kNormalThreads - 1) / kNormalThreads;
+  const long items = long((nb + kNormalTile - 1) / kNormalTile) * vBlocks;
+  for (long it = blockIdx.x; it < items; it += gridDim.x) {
+    const int v = int(it % vBlocks) * kNormalThreads + threadIdx.x;
+    if (v >= V) continue;
+    const int tb = b0 + int(it / vBlocks) * kNormalTile, nt = min(kNormalTile, b0 + nb - tb);
+    F3 g[kNormalTile];
+#pragma unroll
+    for (int t = 0; t < kNormalTile; ++t) g[t] = f3(0.f, 0.f, 0.f);
+    for (int c = M.vertStart[v]; c < M.vertStart[v + 1]; ++c) {
+      const int fc = M.vertCorner[c], k = fc % 3;
+      const int* f = M.faces + (fc - k);
+      const int i0 = f[0], i1 = f[1], i2 = f[2];
+      const int next = k == 0 ? i1 : (k == 1 ? i2 : i0), prev = k == 0 ? i2 : (k == 1 ? i0 : i1);
+#pragma unroll
+      for (int t = 0; t < kNormalTile; ++t)
+        if (t < nt) {
+          const float* x = a.positions + size_t(tb + t) * V * 3;
+          const float* hb = h + size_t(tb + t - b0) * V * 3;
+          const F3 G = ld3(hb + 3 * i0) + ld3(hb + 3 * i1) + ld3(hb + 3 * i2);
+          g[t] = g[t] + cornerGradient(ld3(x + 3 * next), ld3(x + 3 * prev), G);
+        }
+    }
+#pragma unroll
+    for (int t = 0; t < kNormalTile; ++t)
+      if (t < nt) {
+        float* o = a.gradPositions + (size_t(tb + t) * V + v) * 3;
+        o[0] = g[t].x; o[1] = g[t].y; o[2] = g[t].z;
+      }
+  }
+}
+
+namespace {
+template <class K, class P>
+cudaError_t launchNormalPass(K kernel, const NormalArgs& a, int b0, int nb, P h, cudaStream_t stream) {
+  const long vBlocks = (a.M.numVertices + kNormalThreads - 1) / kNormalThreads;
+  int grid = 0;
+  const cudaError_t e = persistentGrid(kernel, kNormalThreads, 0, (nb + kNormalTile - 1) / kNormalTile * vBlocks, &grid);
+  if (e != cudaSuccess) return e;
+  kernel<<<grid, kNormalThreads, 0, stream>>>(a, b0, nb, h);
+  return cudaGetLastError();
+}
+} // namespace
+
+cudaError_t launchVertexNormals(const NormalArgs& a, cudaStream_t stream) {
+  if (a.batch <= 0) return cudaSuccess;
+  return launchNormalPass(vertexNormalKernel<false>, a, 0, a.batch, static_cast<float*>(nullptr), stream);
+}
+
+cudaError_t launchVertexNormalsBackward(const NormalArgs& a, cudaStream_t stream) {
+  const int B = a.batch;
+  if (B <= 0) return cudaSuccess;
+  const size_t perInstance = size_t(a.M.numVertices) * 3 * sizeof(float);
+  const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(B), kNormalScratchBudget / perInstance)));
+  float* h = nullptr;
+  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&h), perInstance * slice, stream);
+  if (e != cudaSuccess) return e;
+  for (int b0 = 0; e == cudaSuccess && b0 < B; b0 += slice) {
+    const int nb = std::min(slice, B - b0);
+    e = launchNormalPass(vertexNormalKernel<true>, a, b0, nb, h, stream);
+    if (e == cudaSuccess) e = launchNormalPass(vertexNormalGradKernel, a, b0, nb, static_cast<const float*>(h), stream);
+  }
+  const cudaError_t f = cudaFreeAsync(h, stream);
+  if (e == cudaSuccess) e = f;
+  return e;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Input gradients of one Position / Orientation block, d/d input [grad_theta E . v] (ik_device.cuh tangent* / *InputGradient), in the
 // per-instance frame of skeletonStateKernel:
 //   lanes = parameters: theta, and v gated by the enabled set;  fkPasses with the DOF axes;  tangentPasses: each joint's own motion,

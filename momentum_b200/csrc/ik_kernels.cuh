@@ -181,6 +181,19 @@ struct BlendSkinArgs {
 bool blendSkinFits(const BlendSkinArgs& a);
 cudaError_t launchSkinWithBlendShapes(const BlendSkinArgs& a, cudaStream_t stream);
 cudaError_t launchSkinWithBlendShapesBackward(const BlendSkinArgs& a, cudaStream_t stream);
+// vertexNormalKernel / vertexNormalGradKernel: area-weighted vertex normals of [B][V][3] positions over the mesh's faces
+// (compute_vertex_normals, tensor_skinning.cpp:354-383) and their backward to the positions
+struct NormalArgs {
+  MeshFaceTables M;
+  int32_t batch;
+  const float* positions;   // [B][V][3]
+  float* normals;           // forward: [B][V][3]
+  const float* gradNormals; // backward: [B][V][3]
+  float* gradPositions;     // backward: [B][V][3]
+};
+// Both enqueue on `stream`; the backward takes stream-ordered scratch (cudaMallocAsync) for h of a slice of instances, at most 256 MiB.
+cudaError_t launchVertexNormals(const NormalArgs& a, cudaStream_t stream);
+cudaError_t launchVertexNormalsBackward(const NormalArgs& a, cudaStream_t stream);
 // inputGradientKernel: d/d input [grad_theta E . v] of one Position or Orientation (matrix difference) block with the L2 loss, per
 // instance: the input contraction of solve_ik's implicit-function backward
 struct InputGradientArgs {

@@ -194,6 +194,28 @@ std::string makeBlendShape(int32_t numShapes, int32_t numVertices, const float* 
   return "";
 }
 
+std::string makeMeshFaces(int32_t numVertices, int32_t numFaces, const int32_t* faces, HostMeshFaces& out) {
+  if (numVertices < 1) return "mesh faces: the mesh must have at least one vertex";
+  if (numFaces < 0) return "mesh faces: the number of faces must not be negative";
+  if (numFaces > INT32_MAX / 3) return "mesh faces: too many faces (3 x num_faces must fit in int32)";
+  if (numFaces > 0 && faces == nullptr) return "mesh faces: null argument";
+  const size_t corners = size_t(numFaces) * 3;
+  for (size_t c = 0; c < corners; ++c)
+    if (faces[c] < 0 || faces[c] >= numVertices) return "mesh faces: a face index is outside [0, num_vertices)";
+  HostMeshFaces m;
+  m.numVertices = numVertices;
+  m.numFaces = numFaces;
+  m.faces.assign(faces, faces + corners);
+  m.vertStart.assign(size_t(numVertices) + 1, 0);
+  for (size_t c = 0; c < corners; ++c) ++m.vertStart[size_t(m.faces[c]) + 1];
+  for (int32_t v = 0; v < numVertices; ++v) m.vertStart[v + 1] += m.vertStart[v];
+  m.vertCorner.resize(corners);
+  std::vector<int32_t> fill(m.vertStart.begin(), m.vertStart.end() - 1);
+  for (size_t c = 0; c < corners; ++c) m.vertCorner[size_t(fill[m.faces[c]]++)] = int32_t(c); // c = 3 f + k ascending
+  out = std::move(m);
+  return "";
+}
+
 CharacterTables hostCharacterTables(const HostCharacter& ch) {
   CharacterTables C{};
   C.numJoints = ch.numJoints;

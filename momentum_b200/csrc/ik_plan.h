@@ -68,6 +68,15 @@ struct HostBlendShape {
   std::vector<float> shapeVectors; // [K][V][3]: shapeVectors_ (3V x K, column-major) as it lies in memory
 };
 
+// The triangles of a mesh (Mesh::faces, mesh.h) with, per vertex, the corners that are that vertex: vertCorner[vertStart[v] ..
+// vertStart[v + 1]) holds 3 f + k for every corner k of every face f with faces[3 f + k] == v, faces ascending, corners ascending within a
+// face (a face that lists v twice is there twice). Built and validated by makeMeshFaces only (MeshFaceTables).
+struct HostMeshFaces {
+  int32_t numVertices{0}, numFaces{0};
+  std::vector<int32_t> faces;                 // [F][3]
+  std::vector<int32_t> vertStart, vertCorner; // [V + 1], [3 F]
+};
+
 struct HostErrorFunction {
   int32_t kind{0}; // 0 position, 1 orientation, 2 orientation rot-diff, 3 state, 4 limit, 5 plane, 6 model parameters
   float weight{1.f};
@@ -118,6 +127,9 @@ std::string makeSkinning(const HostCharacter& ch, int32_t numVertices, const flo
 // baseShape [V][3], shapeVectors [K][V][3]; K >= 1, V >= 1, every value finite. The blend shape's V is checked against the skinning's
 // where both are used, not here: either may be replaced first.
 std::string makeBlendShape(int32_t numShapes, int32_t numVertices, const float* baseShape, const float* shapeVectors, HostBlendShape& out);
+// faces [F][3] over V vertices; V >= 1, F >= 0, 3 F within int32, every index in [0, V). Degenerate faces and faces that repeat an index
+// are accepted (they add a zero normal, and a repeated vertex counts once per corner).
+std::string makeMeshFaces(int32_t numVertices, int32_t numFaces, const int32_t* faces, HostMeshFaces& out);
 std::string positionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* offsets,
                                   const float* weights, HostErrorFunction& out);
 std::string instancedPositionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* weights,

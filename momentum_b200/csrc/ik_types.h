@@ -163,4 +163,12 @@ struct BlendShapeTables {
   const float* shapeVectors;    // [K][V][3]
 };
 
+// Mesh-face tables (HostMeshFaces, makeMeshFaces), shared by the whole batch.
+struct MeshFaceTables {
+  int32_t numVertices, numFaces;
+  const int32_t* faces;      // [F][3]
+  const int32_t* vertStart;  // [V+1] into vertCorner
+  const int32_t* vertCorner; // [3F]: 3 f + k of the corners that are the vertex, faces ascending, corners ascending
+};
+
 } // namespace mb2

@@ -79,6 +79,7 @@ CABI_SYMBOLS = [
     "mb2_character_set_skinning", "mb2_character_num_vertices", "mb2_character_skin_points_device", "mb2_character_skin_points_backward_device",
     "mb2_character_set_blend_shape", "mb2_character_num_blend_shapes", "mb2_character_skin_with_blend_shapes_device",
     "mb2_character_skin_with_blend_shapes_backward_device",
+    "mb2_character_set_mesh_faces", "mb2_character_num_faces", "mb2_character_vertex_normals_device", "mb2_character_vertex_normals_backward_device",
 ]
 
 _libs = {}
@@ -195,6 +196,11 @@ def load_library(path: Optional[str] = None):
         L.mb2_character_num_blend_shapes.argtypes = [vp]
         L.mb2_character_skin_with_blend_shapes_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]
         L.mb2_character_skin_with_blend_shapes_backward_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp, vp, vp]
+    if hasattr(L, "mb2_character_set_mesh_faces"):
+        L.mb2_character_set_mesh_faces.argtypes = [vp, C.c_int32, C.c_int32, _ip]
+        L.mb2_character_num_faces.argtypes = [vp]
+        L.mb2_character_vertex_normals_device.argtypes = [vp, C.c_int32, vp, vp, vp]
+        L.mb2_character_vertex_normals_backward_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
     _libs[path] = L
     return L
 
@@ -283,7 +289,7 @@ class DeviceCharacter(_Base):
                 for j in range(27):
                     arr[k].f[j] = float(ff[j])
             self._check(self._L.mb2_character_set_parameter_limits(self._h, len(character.limits), arr))
-        self.skinning = None
+        self.skinning, self.faces, self.faces_error = None, None, None
         if character.skinning is not None:
             self.set_skinning(character.skinning)
         # A blend shape the library rejects is reported by the blend-shape calls, not here: the rig, its skinning and every other use of
@@ -296,7 +302,9 @@ class DeviceCharacter(_Base):
                 self.blend_shape_error = str(e)
 
     def set_skinning(self, skinning: mc.Skinning):
-        """Uploads ``skinning`` (replacing any earlier one); ``self.skinning`` is the object uploaded."""
+        """Uploads ``skinning`` (replacing any earlier one) and its ``faces``, or removes the faces when it has none; ``self.skinning`` and
+        ``self.faces`` are the objects uploaded. Faces the library rejects do not fail the skinning upload: ``self.faces`` is then None
+        and ``self.faces_error`` the reason, which ``torch_skeleton.compute_vertex_normals`` raises."""
         V = skinning.num_vertices
         rv, rvp = _f32(np.asarray(skinning.rest_vertices).reshape(V, 3))
         si, sip = _i32(np.asarray(skinning.skin_index).reshape(V, mc.MAX_SKIN_JOINTS))
@@ -304,6 +312,42 @@ class DeviceCharacter(_Base):
         ib, ibp = _f32(np.asarray(skinning.inverse_bind_pose).reshape(self.character.num_joints, 12))
         self._check(self._L.mb2_character_set_skinning(self._h, V, rvp, sip, swp, ibp))
         self.skinning = skinning
+        self.faces, self.faces_error = None, None
+        try:
+            self._set_mesh_faces(V, skinning.faces)
+            self.faces = skinning.faces
+        except (MomentumB200Error, ValueError) as e:
+            self._check(self._L.mb2_character_set_mesh_faces(self._h, 0, 0, None))  # no faces left from an earlier skinning
+            self.faces_error = str(e)
+
+    def _set_mesh_faces(self, num_vertices: int, faces):
+        if faces is None:
+            self._check(self._L.mb2_character_set_mesh_faces(self._h, 0, 0, None))
+            return
+        f = np.asarray(faces)
+        if f.ndim != 2 or f.shape[1] != 3 or f.dtype.kind not in "iu":
+            raise ValueError(f"mesh faces: faces must be an integer array [F, 3], got {f.dtype} {f.shape}")
+        if f.size and (f.min() < np.iinfo(np.int32).min or f.max() > np.iinfo(np.int32).max):
+            raise ValueError("mesh faces: a face index is outside [0, num_vertices)")
+        fa, fp = _i32(f)
+        self._check(self._L.mb2_character_set_mesh_faces(self._h, int(num_vertices), int(f.shape[0]), fp))
+
+    @property
+    def num_faces(self) -> int:
+        return int(self._L.mb2_character_num_faces(self._h))
+
+    def vertex_normals_device(self, batch: int, positions_device_ptr: int, normals_device_ptr: int, stream: int = 0):
+        """Area-weighted vertex normals [B][V][3] of vertex positions [B][V][3] over the uploaded faces. float32 device memory on this
+        character's device, enqueued on ``stream``."""
+        self._check(self._L.mb2_character_vertex_normals_device(self._h, int(batch), C.c_void_p(positions_device_ptr), C.c_void_p(normals_device_ptr),
+                                                                C.c_void_p(stream)))
+
+    def vertex_normals_backward_device(self, batch: int, positions_device_ptr: int, grad_normals_device_ptr: int, grad_positions_device_ptr: int,
+                                       stream: int = 0):
+        """dLoss/d positions [B][V][3] (overwritten) from dLoss/d normals [B][V][3]."""
+        self._check(self._L.mb2_character_vertex_normals_backward_device(self._h, int(batch), C.c_void_p(positions_device_ptr),
+                                                                         C.c_void_p(grad_normals_device_ptr), C.c_void_p(grad_positions_device_ptr),
+                                                                         C.c_void_p(stream)))
 
     @property
     def num_vertices(self) -> int:

@@ -114,16 +114,18 @@ _skin_handles = {}
 
 
 def _skinned_device_character(ch: mc.Character, device: torch.device) -> ms.DeviceCharacter:
-    """One DeviceCharacter per (character, device) holding ``ch.skinning`` and ``ch.blend_shape``. When either is replaced, a new handle is
-    made instead of uploading into the old one: a graph recorded with the old skinning keeps its handle (``ctx.dc``) and its tables, and
-    no kernel in flight on another stream reads tables that are being replaced. An old handle is freed with the last graph that uses it."""
+    """One DeviceCharacter per (character, device) holding ``ch.skinning`` (with its ``faces``) and ``ch.blend_shape``. When any of them is
+    replaced, a new handle is made instead of uploading into the old one: a graph recorded with the old skinning keeps its handle
+    (``ctx.dc``) and its tables, and no kernel in flight on another stream reads tables that are being replaced. An old handle is freed
+    with the last graph that uses it."""
     index = device.index if device.index is not None else torch.cuda.current_device()
     key = (id(ch), index)
     entry = _skin_handles.get(key)
-    if entry is None or entry[1] is not ch.skinning or entry[2] is not ch.blend_shape:
-        entry = (ch, ch.skinning, ch.blend_shape, ms.DeviceCharacter(ch, index))  # the character is kept alive so that its id stays unique
+    faces = None if ch.skinning is None else ch.skinning.faces
+    if entry is None or entry[1] is not ch.skinning or entry[2] is not ch.blend_shape or entry[3] is not faces:
+        entry = (ch, ch.skinning, ch.blend_shape, faces, ms.DeviceCharacter(ch, index))  # the character is kept alive so that its id stays unique
         _skin_handles[key] = entry
-    return entry[3]
+    return entry[4]
 
 
 def skin_points(character, skel_state: torch.Tensor, rest_points=None) -> torch.Tensor:
@@ -238,3 +240,69 @@ def skin_with_blend_shapes(character, skel_state: torch.Tensor, blend_weights: t
     if dc.blend_shape is None:
         raise ValueError(f"the character's blend shape was rejected: {dc.blend_shape_error}")
     return _SkinWithBlendShapes.apply(dc, skel_state, blend_weights)
+
+
+class _VertexNormals(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, dc, vertex_positions):
+        V = dc.skinning.num_vertices
+        dev = vertex_positions.device
+        x = vertex_positions.detach().to(torch.float32).reshape(-1, V, 3).contiguous()
+        B = x.shape[0]
+        out = torch.empty(B, V, 3, device=dev, dtype=torch.float32)
+        dc.vertex_normals_device(B, x.data_ptr(), out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        ctx.dc, ctx.skinning, ctx.faces = dc, dc.skinning, dc.faces
+        ctx.in_shape, ctx.in_dtype = vertex_positions.shape, vertex_positions.dtype
+        ctx.save_for_backward(x)
+        return out.reshape(vertex_positions.shape).to(vertex_positions.dtype)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_normals):
+        (x,) = ctx.saved_tensors
+        dc = ctx.dc
+        if dc.skinning is not ctx.skinning or dc.faces is not ctx.faces:
+            raise RuntimeError("compute_vertex_normals backward: the DeviceCharacter's skinning was replaced (set_skinning) after the forward; "
+                               "keep one DeviceCharacter per mesh, or pass the Character and replace character.skinning instead")
+        B, V, _ = x.shape
+        dev = x.device
+        g = grad_normals.to(device=dev, dtype=torch.float32).reshape(B, V, 3).contiguous()
+        gx = torch.empty_like(x)
+        dc.vertex_normals_backward_device(B, x.data_ptr(), g.data_ptr(), gx.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        return None, gx.reshape(ctx.in_shape).to(ctx.in_dtype)
+
+
+def compute_vertex_normals(character, vertex_positions: torch.Tensor) -> torch.Tensor:
+    """Area-weighted vertex normals (pymomentum ``diff_geometry.compute_vertex_normals``): ``vertex_positions`` [V, 3] or [B, V, 3] on a
+    CUDA device -> normals of the same shape in the input dtype, computed in float32. Per vertex, the sum of (x1 - x0) x (x2 - x0) over
+    every corner of every face that is that vertex, faces ascending and corners in order, divided by max(|n|, 1e-12): an isolated vertex
+    gives exactly 0. Non-finite positions propagate (momentum's ``Mesh::updateNormals`` skips NaN faces; this does not). Differentiable
+    once with respect to ``vertex_positions``, with the exact derivative of the clamp.
+
+    The faces are ``character.skinning.faces`` (int32 [F, 3] over the rest vertices), not an argument as in pymomentum's
+    ``(vertex_positions, triangles)``: the library validates them and builds its vertex -> face table once, when they are uploaded, so
+    a call copies nothing from the device to the host. ``character`` is a ``momentum_b200.character.Character``: replacing
+    ``character.skinning`` or its ``faces`` is safe at any time, and graphs recorded before keep the faces they were recorded with. Or it
+    is a ``solver.DeviceCharacter``, which uses what was uploaded with its skinning; the backward of a graph recorded before a later
+    ``set_skinning`` on that handle raises."""
+    if not torch.is_tensor(vertex_positions) or not vertex_positions.is_cuda:
+        raise ValueError("compute_vertex_normals runs on CUDA tensors (there is no CPU fallback)")
+    is_handle = isinstance(character, ms.DeviceCharacter)
+    ch = character.character if is_handle else character
+    if not isinstance(ch, mc.Character):
+        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
+    sk = character.skinning if is_handle else ch.skinning
+    if sk is None:
+        raise ValueError("the character has no skinning, so no mesh faces")
+    if is_handle and character.faces is None:
+        rejected = character.faces_error
+        raise ValueError("the character has no mesh faces" + (f" (their upload was rejected: {rejected})" if rejected else ""))
+    if not is_handle and sk.faces is None:
+        raise ValueError("the character has no mesh faces (character.skinning.faces)")
+    V = sk.num_vertices
+    if vertex_positions.dim() not in (2, 3) or vertex_positions.shape[-2:] != (V, 3):
+        raise ValueError(f"vertex_positions must be [V, 3] or [B, V, 3] with V = {V}, got {tuple(vertex_positions.shape)}")
+    dc = _device_character(character, vertex_positions.device) if is_handle else _skinned_device_character(ch, vertex_positions.device)
+    if dc.faces is None:
+        raise ValueError(f"the character's mesh faces were rejected: {dc.faces_error}")
+    return _VertexNormals.apply(dc, vertex_positions)
