@@ -338,6 +338,26 @@ int mb2_character_vertex_normals_device(const mb2_character* c, int32_t batch, c
 int mb2_character_vertex_normals_backward_device(const mb2_character* c, int32_t batch, const float* positions_device, const float* grad_normals_device,
                                                  float* grad_positions_device, void* cuda_stream);
 
+/* The bounding-volume tree that mb2_character_closest_points_on_mesh_device searches, built from the current mesh faces over the host
+ * array reference_positions [num_vertices][3] (normally the rest mesh) and replacing any earlier one; num_vertices == 0 with a null array
+ * removes it. Only the topology is kept: each call refits the boxes to the instance's vertices, so the reference pose changes the speed of
+ * the queries, never their results. No faces, num_vertices other than the faces', a null array or a non-finite position is
+ * MB2_ERR_INVALID_ARGUMENT and leaves the earlier tree in place. Fresh device buffers and a device synchronisation before the old ones are
+ * freed, as mb2_character_set_mesh_faces. mb2_character_set_mesh_faces drops the tree; mb2_character_clone copies it. */
+int mb2_character_set_mesh_tree(mb2_character* c, int32_t num_vertices, const float* reference_positions);
+/* The closest point on the mesh of each query point (pymomentum find_closest_points_on_mesh, array_kd_tree.cpp): for instance b and point
+ * p = points[b][n], over the faces f of the mesh with vertices vertex_positions[b] ([B][V][3], V = the faces' num_vertices), the face with
+ * the smallest (d2_f, f), d2_f = |q_f - p|^2 and (q_f, bary_f) the closest point of face f to p (Ericson 5.1.5, axel::projectOnTriangle),
+ * among the candidates: faces with finite vertices and finite d2_f <= max_dist * max_dist (in float; max_dist may be +inf). Writes
+ * out_points [B][N][3] = q, out_face [B][N] = f and out_bary [B][N][3]; without a candidate (a non-finite query included) -1 and zeros.
+ * The result does not depend on the tree. Device memory on `cuda_stream`, asynchronous; batch == 0 or num_points == 0 is a no-op. No
+ * faces or no tree, batch < 0, num_points < 0, a NaN or negative max_dist, a null pointer or a pointer that is not device memory on the
+ * character's device is MB2_ERR_INVALID_ARGUMENT. Stream-ordered scratch from the device's default memory pool: the boxes of a slice of
+ * instances, at most 256 MiB. No atomics: an instance gets the same bits alone as in any batch. */
+int mb2_character_closest_points_on_mesh_device(const mb2_character* c, int32_t batch, int32_t num_points, const float* vertex_positions_device,
+                                                const float* points_device, float max_dist, float* out_points_device, int32_t* out_face_device,
+                                                float* out_bary_device, void* cuda_stream);
+
 /* Input contraction of the implicit-function backward of solve_ik (diff_ik d_gradient_d_input_dot): for block `index` and every
  * instance b, the derivatives of grad_theta E_index(theta_b) . v_b with respect to the block's inputs, at the targets, constraint weights
  * and offsets the handle currently holds:

@@ -112,6 +112,10 @@ struct BlendShapeBuffers {
 struct MeshFaceBuffers {
   DeviceBuffer<int32_t> faces, vertStart, vertCorner;
 };
+// the device copy of a HostMeshTree (MeshTreeTables)
+struct MeshTreeBuffers {
+  DeviceBuffer<int32_t> nodeStart, nodeCount, leafFaces, levelStart;
+};
 
 struct mb2_character {
   int device{0};
@@ -130,6 +134,9 @@ struct mb2_character {
   // mesh faces (mb2_character_set_mesh_faces): numVertices == 0 when there are none
   HostMeshFaces faces;
   std::unique_ptr<MeshFaceBuffers> facesDev; // replaced whole by mb2_character_set_mesh_faces
+  // bounding-volume tree over the faces (mb2_character_set_mesh_tree): numNodes == 0 when there is none
+  HostMeshTree tree;
+  std::unique_ptr<MeshTreeBuffers> treeDev; // replaced whole by mb2_character_set_mesh_tree, dropped by mb2_character_set_mesh_faces
   CharacterTables tables() const; // the device copies above, as the kernels read them
 };
 
@@ -235,6 +242,26 @@ CharacterTables mb2_character::tables() const {
   C.levelJoints = levelJoints.p;
   return C;
 }
+
+namespace {
+// installs tree t (numNodes == 0: none) as mb2_character_set_mesh_faces installs its tables: fresh buffers, and the device synchronised
+// before the old ones are freed
+int installMeshTree(mb2_character* c, HostMeshTree&& t) {
+  MB2_DEVICE_GUARD(c->device);
+  std::unique_ptr<MeshTreeBuffers> d;
+  if (t.numNodes > 0) {
+    d = std::make_unique<MeshTreeBuffers>();
+    MB2_CUDA(d->nodeStart.upload(t.nodeStart, nullptr));
+    MB2_CUDA(d->nodeCount.upload(t.nodeCount, nullptr));
+    MB2_CUDA(d->leafFaces.upload(t.leafFaces, nullptr));
+    MB2_CUDA(d->levelStart.upload(t.levelStart, nullptr));
+  }
+  MB2_CUDA(cudaDeviceSynchronize());
+  c->treeDev = std::move(d);
+  c->tree = std::move(t);
+  return MB2_OK;
+}
+} // namespace
 
 FunctionTables mb2_solver_function::tables() const {
   FunctionTables T{ch->tables()};
@@ -607,6 +634,10 @@ int mb2_character_clone(const mb2_character* c, int device, mb2_character** out)
     rc = mb2_character_set_mesh_faces(copy, mf.numVertices, mf.numFaces, mf.faces.data());
     if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
   }
+  if (c->tree.numNodes > 0) {
+    rc = installMeshTree(copy, HostMeshTree(c->tree));
+    if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
+  }
   *out = copy;
   return MB2_OK;
 }
@@ -676,10 +707,22 @@ int mb2_character_set_mesh_faces(mb2_character* c, int32_t num_vertices, int32_t
   MB2_CUDA(cudaDeviceSynchronize());
   c->facesDev = std::move(d);
   c->faces = std::move(m);
+  c->treeDev.reset(); // built over the faces it replaced
+  c->tree = HostMeshTree{};
   return MB2_OK;
 }
 
 int32_t mb2_character_num_faces(const mb2_character* c) { return c ? c->faces.numFaces : 0; }
+
+int mb2_character_set_mesh_tree(mb2_character* c, int32_t num_vertices, const float* reference_positions) {
+  MB2_CHECK(c != nullptr, "null character");
+  HostMeshTree t;
+  if (!(num_vertices == 0 && reference_positions == nullptr)) { // that pair removes the tree
+    const std::string err = makeMeshTree(c->faces, num_vertices, reference_positions, t);
+    if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
+  }
+  return installMeshTree(c, std::move(t));
+}
 // The DEFINITION of a solver function (error-function blocks with their shared constraint data and weights, block weights, enabled
 // parameters) for `batch` instances of character `c` (normally a clone of f's character on another device). Per-instance data
 // (targets, per-instance weights / offsets) is not copied: it belongs to the instances the new function will hold.
@@ -1149,6 +1192,40 @@ int mb2_character_vertex_normals_device(const mb2_character* c, int32_t batch, c
   a.positions = positions_device;
   a.normals = normals_device;
   MB2_CUDA(launchVertexNormals(a, (cudaStream_t)cuda_stream));
+  return MB2_OK;
+}
+
+int mb2_character_closest_points_on_mesh_device(const mb2_character* c, int32_t batch, int32_t num_points, const float* vertex_positions_device,
+                                                const float* points_device, float max_dist, float* out_points_device, int32_t* out_face_device,
+                                                float* out_bary_device, void* cuda_stream) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(c->faces.numVertices > 0, "closest points: the character has no mesh faces (mb2_character_set_mesh_faces)");
+  MB2_CHECK(c->tree.numNodes > 0, "closest points: the character has no mesh tree (mb2_character_set_mesh_tree)");
+  MB2_CHECK(batch >= 0 && num_points >= 0, "closest points: batch and num_points must not be negative");
+  MB2_CHECK(max_dist >= 0.f, "closest points: max_dist must be >= 0 and not NaN (+inf for no bound)");
+  if (batch == 0 || num_points == 0) return MB2_OK;
+  MB2_CHECK(vertex_positions_device != nullptr && points_device != nullptr && out_points_device != nullptr && out_face_device != nullptr &&
+                out_bary_device != nullptr,
+            "closest points: null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(isDeviceMemoryOn(vertex_positions_device, c->device) && isDeviceMemoryOn(points_device, c->device) &&
+                isDeviceMemoryOn(out_points_device, c->device) && isDeviceMemoryOn(out_face_device, c->device) &&
+                isDeviceMemoryOn(out_bary_device, c->device),
+            "closest points: every array must be device memory on the character's device");
+  NvtxRange range("closestPointsOnMesh");
+  ClosestPointArgs a{};
+  a.M = MeshFaceTables{c->faces.numVertices, c->faces.numFaces, c->facesDev->faces.p, c->facesDev->vertStart.p, c->facesDev->vertCorner.p};
+  a.T = MeshTreeTables{c->tree.numNodes, c->tree.depth, c->treeDev->nodeStart.p, c->treeDev->nodeCount.p, c->treeDev->leafFaces.p,
+                       c->treeDev->levelStart.p};
+  a.batch = batch;
+  a.numPoints = num_points;
+  a.maxDist2 = max_dist * max_dist;
+  a.vertices = vertex_positions_device;
+  a.points = points_device;
+  a.outPoints = out_points_device;
+  a.outFace = out_face_device;
+  a.outBary = out_bary_device;
+  MB2_CUDA(launchClosestPointsOnMesh(a, (cudaStream_t)cuda_stream));
   return MB2_OK;
 }
 

@@ -1031,4 +1031,91 @@ MB2_HD F3 normalGradient(F3 n, F3 g) {
 // d/dx_k [G . (x1 - x0) x (x2 - x0)] = (x_{k+1} - x_{k+2}) x G, corners mod 3.
 MB2_HD F3 cornerGradient(F3 xNext, F3 xPrev, F3 G) { return cross(xNext - xPrev, G); }
 
+// ---- Closest point on a triangle mesh (pymomentum find_closest_points_on_mesh over axel::TriBvh) ----------------------------------
+// The closest point q of triangle (a, b, c) to p and its barycentrics (Ericson, Real-Time Collision Detection, 5.1.5; the region tests of
+// axel::projectOnTriangle in the same order): the three vertex regions, the three edge regions, then the interior. A zero-area face whose
+// point falls through to the interior gives NaN there.
+MB2_HD void closestPointOnTriangle(F3 p, F3 a, F3 b, F3 c, F3& q, F3& bary) {
+  const F3 ab = b - a, ac = c - a, ap = p - a;
+  const float d1 = dot(ab, ap), d2 = dot(ac, ap);
+  if (d1 <= 0.f && d2 <= 0.f) { q = a; bary = f3(1.f, 0.f, 0.f); return; }
+  const F3 bp = p - b;
+  const float d3 = dot(ab, bp), d4 = dot(ac, bp);
+  if (d3 >= 0.f && d4 <= d3) { q = b; bary = f3(0.f, 1.f, 0.f); return; }
+  const float vc = d1 * d4 - d3 * d2;
+  if (vc <= 0.f && d1 >= 0.f && d3 <= 0.f) {
+    const float v = d1 / (d1 - d3);
+    q = a + v * ab; bary = f3(1.f - v, v, 0.f); return;
+  }
+  const F3 cp = p - c;
+  const float d5 = dot(ab, cp), d6 = dot(ac, cp);
+  if (d6 >= 0.f && d5 <= d6) { q = c; bary = f3(0.f, 0.f, 1.f); return; }
+  const float vb = d5 * d2 - d1 * d6;
+  if (vb <= 0.f && d2 >= 0.f && d6 <= 0.f) {
+    const float w = d2 / (d2 - d6);
+    q = a + w * ac; bary = f3(1.f - w, 0.f, w); return;
+  }
+  const float va = d3 * d6 - d5 * d4;
+  if (va <= 0.f && (d4 - d3) >= 0.f && (d5 - d6) >= 0.f) {
+    const float w = (d4 - d3) / ((d4 - d3) + (d5 - d6));
+    q = b + w * (c - b); bary = f3(0.f, 1.f - w, w); return;
+  }
+  const float denom = 1.f / (va + vb + vc);
+  const float v = vb * denom, w = vc * denom;
+  q = a + ab * v + ac * w;
+  bary = f3(1.f - v - w, v, w);
+}
+
+MB2_HD bool finite3(F3 a) { return fabsf(a.x) <= FLT_MAX && fabsf(a.y) <= FLT_MAX && fabsf(a.z) <= FLT_MAX; }
+
+// d^2 = |q - p|^2 of face (a, b, c) with its q and barycentrics; NaN when a vertex is not finite, so that such a face is never a candidate
+MB2_HD float faceDistance2(F3 p, F3 a, F3 b, F3 c, F3& q, F3& bary) {
+  closestPointOnTriangle(p, a, b, c, q, bary);
+  const F3 e = q - p;
+  const float d2 = dot(e, e);
+  return finite3(a) && finite3(b) && finite3(c) ? d2 : NAN;
+}
+
+// Face f with d2 is a candidate when d2 is finite and d2 <= maxDist2; the result is the candidate with the smallest (d2, f). With
+// (best, bestFace) initialised to (maxDist2, INT_MAX), a candidate beats it exactly when closerFace holds.
+MB2_HD bool closerFace(float d2, int f, float best, int bestFace) {
+  return fabsf(d2) <= FLT_MAX && (d2 < best || (d2 == best && f < bestFace));
+}
+
+// A lower bound, in float, of the d2 that any face whose vertices lie in the box [lo, hi] can give at p (p finite). Per axis the gap
+// g = max(lo - p, p - hi) is reduced by 2^-18 (M + |p|), M = max(|lo|, |hi|): that covers q of a face leaving the box by its rounding
+// (at most 26 u M) and g's own rounding (u (M + |p|)), u = 2^-24; the sum of squares is then scaled by 1 - 2^-20 against the rounding of
+// this sum (4 u) and of d2 (6 u). A non-finite box gives 0. DESIGN §4 has the argument. A subtree is pruned only when this is > best.
+MB2_HD float boxLowerBound(const float* box, F3 p) { // box: lo xyz, hi xyz
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float pk = comp(p, k), lo = box[k], hi = box[3 + k];
+    const float g = fmaxf(lo - pk, pk - hi);
+    const float tau = 0x1p-18f * (fmaxf(fabsf(lo), fabsf(hi)) + fabsf(pk));
+    const float h = fmaxf(g - tau, 0.f); // NaN (a non-finite box) gives 0
+    s += h * h;
+  }
+  return s * (1.f - 0x1p-20f);
+}
+MB2_HD bool pruneBox(float lowerBound, float best) { return lowerBound > best; } // never on >=: an equal bound may hold a lower face index
+
+// Refit: the box of a leaf is the exact min / max of its faces' vertices, the box of an internal node that of its two children's boxes.
+// fminf / fmaxf skip NaN coordinates; a face with one is never a candidate (faceDistance2).
+MB2_HD void boxEmpty(float* box) {
+  box[0] = box[1] = box[2] = INFINITY;
+  box[3] = box[4] = box[5] = -INFINITY;
+}
+MB2_HD void boxGrow(float* box, F3 x) {
+  box[0] = fminf(box[0], x.x); box[1] = fminf(box[1], x.y); box[2] = fminf(box[2], x.z);
+  box[3] = fmaxf(box[3], x.x); box[4] = fmaxf(box[4], x.y); box[5] = fmaxf(box[5], x.z);
+}
+MB2_HD void boxUnion(float* box, const float* l, const float* r) {
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    box[k] = fminf(l[k], r[k]);
+    box[3 + k] = fmaxf(l[3 + k], r[3 + k]);
+  }
+}
+
 } // namespace mb2

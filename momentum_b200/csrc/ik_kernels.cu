@@ -902,6 +902,144 @@ cudaError_t launchVertexNormalsBackward(const NormalArgs& a, cudaStream_t stream
 }
 
 // ------------------------------------------------------------------------------------------------
+// Closest points on the mesh (ik_device.cuh closestPointOnTriangle / faceDistance2 / closerFace / boxLowerBound / pruneBox / box*). The
+// tree's topology is shared; each slice of instances gets its boxes [nb][numNodes][lo xyz, hi xyz] refitted in scratch, then queried.
+//   meshTreeRefitKernel   one CTA per instance: the levels from the deepest up, a thread per node, __syncthreads between levels.
+//   closestPointKernel    one thread per (instance, query): depth-first from the root, the nearer child first and the other on a stack
+//                         of kTreeStack (node, lower bound) entries, re-checked when popped. The stack is indexed dynamically, so it
+//                         lives in local memory.
+// The result is the smallest (d2, face) over the candidates, whatever the tree and the visiting order: a subtree is skipped only when
+// its lower bound is strictly above the best d2, which no face in it can then reach. No atomics.
+// ------------------------------------------------------------------------------------------------
+constexpr int kRefitThreads = 256;
+constexpr int kClosestThreads = 128;
+constexpr size_t kTreeScratchBudget = size_t(256) << 20; // the boxes of a slice of instances
+
+__global__ void __launch_bounds__(kRefitThreads) meshTreeRefitKernel(const ClosestPointArgs a, int b0, int nb, float* boxes) {
+  const MeshTreeTables T = a.T;
+  const int V = a.M.numVertices;
+  for (int i = blockIdx.x; i < nb; i += gridDim.x) {
+    const float* x = a.vertices + size_t(b0 + i) * V * 3;
+    float* bx = boxes + size_t(i) * T.numNodes * 6;
+    for (int L = T.depth - 1; L >= 0; --L) {
+      const int end = T.levelStart[L + 1];
+      for (int n = T.levelStart[L] + threadIdx.x; n < end; n += kRefitThreads) {
+        const int start = T.nodeStart[n], count = T.nodeCount[n];
+        float box[6];
+        if (count == 0) {
+          boxUnion(box, bx + size_t(start) * 6, bx + size_t(start + 1) * 6);
+        } else {
+          boxEmpty(box);
+          for (int k = 0; k < count; ++k) {
+            const int* f = a.M.faces + size_t(T.leafFaces[start + k]) * 3;
+            boxGrow(box, ld3(x + 3 * size_t(f[0])));
+            boxGrow(box, ld3(x + 3 * size_t(f[1])));
+            boxGrow(box, ld3(x + 3 * size_t(f[2])));
+          }
+        }
+        float* o = bx + size_t(n) * 6;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) o[k] = box[k];
+      }
+      __syncthreads(); // the next level reads these boxes
+    }
+  }
+}
+
+// boxes: [nb][numNodes][6] of the instances b0 .. b0 + nb
+__global__ void __launch_bounds__(kClosestThreads) closestPointKernel(const ClosestPointArgs a, int b0, int nb, const float* boxes) {
+  const MeshTreeTables T = a.T;
+  const int V = a.M.numVertices;
+  const long N = a.numPoints, total = long(nb) * N;
+  for (long it = long(blockIdx.x) * kClosestThreads + threadIdx.x; it < total; it += long(gridDim.x) * kClosestThreads) {
+    const int i = int(it / N);
+    const size_t qi = size_t(b0 + i) * N + size_t(it % N);
+    const F3 p = ld3(a.points + 3 * qi);
+    const float* x = a.vertices + size_t(b0 + i) * V * 3;
+    const float* bx = boxes + size_t(i) * T.numNodes * 6;
+    float best = a.maxDist2;
+    int bestFace = INT_MAX;
+    F3 bestQ = f3(0.f, 0.f, 0.f), bestBary = f3(0.f, 0.f, 0.f);
+    int stackNode[kTreeStack];
+    float stackLb[kTreeStack];
+    int sp = 0, node = 0;
+    bool go = finite3(p) && !pruneBox(boxLowerBound(bx, p), best);
+    while (go) {
+      const int start = T.nodeStart[node], count = T.nodeCount[node];
+      if (count == 0) {
+        const float lb0 = boxLowerBound(bx + size_t(start) * 6, p), lb1 = boxLowerBound(bx + size_t(start + 1) * 6, p);
+        const bool in0 = !pruneBox(lb0, best), in1 = !pruneBox(lb1, best);
+        if (in0 && in1) {
+          const bool first1 = lb1 < lb0;
+          stackNode[sp] = first1 ? start : start + 1;
+          stackLb[sp] = first1 ? lb0 : lb1;
+          ++sp;
+          node = first1 ? start + 1 : start;
+          continue;
+        }
+        if (in0 || in1) {
+          node = in0 ? start : start + 1;
+          continue;
+        }
+      } else {
+        for (int k = 0; k < count; ++k) {
+          const int f = T.leafFaces[start + k];
+          const int* fv = a.M.faces + size_t(f) * 3;
+          F3 q, bary;
+          const float d2 = faceDistance2(p, ld3(x + 3 * size_t(fv[0])), ld3(x + 3 * size_t(fv[1])), ld3(x + 3 * size_t(fv[2])), q, bary);
+          if (closerFace(d2, f, best, bestFace)) {
+            best = d2; bestFace = f; bestQ = q; bestBary = bary;
+          }
+        }
+      }
+      go = false;
+      while (sp > 0) {
+        --sp;
+        if (!pruneBox(stackLb[sp], best)) {
+          node = stackNode[sp];
+          go = true;
+          break;
+        }
+      }
+    }
+    const bool found = bestFace != INT_MAX;
+    float* oq = a.outPoints + 3 * qi;
+    float* ob = a.outBary + 3 * qi;
+    if (!found) bestQ = bestBary = f3(0.f, 0.f, 0.f);
+    oq[0] = bestQ.x; oq[1] = bestQ.y; oq[2] = bestQ.z;
+    ob[0] = bestBary.x; ob[1] = bestBary.y; ob[2] = bestBary.z;
+    a.outFace[qi] = found ? bestFace : -1;
+  }
+}
+
+cudaError_t launchClosestPointsOnMesh(const ClosestPointArgs& a, cudaStream_t stream) {
+  const int B = a.batch;
+  if (B <= 0 || a.numPoints <= 0) return cudaSuccess;
+  const size_t perInstance = size_t(a.T.numNodes) * 6 * sizeof(float);
+  const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(B), kTreeScratchBudget / perInstance)));
+  int refitGrid = 0, queryGrid = 0;
+  cudaError_t e = persistentGrid(meshTreeRefitKernel, kRefitThreads, 0, slice, &refitGrid);
+  if (e == cudaSuccess)
+    e = persistentGrid(closestPointKernel, kClosestThreads, 0, (long(slice) * a.numPoints + kClosestThreads - 1) / kClosestThreads, &queryGrid);
+  if (e != cudaSuccess) return e;
+  float* boxes = nullptr;
+  e = cudaMallocAsync(reinterpret_cast<void**>(&boxes), perInstance * slice, stream);
+  if (e != cudaSuccess) return e;
+  for (int b0 = 0; e == cudaSuccess && b0 < B; b0 += slice) {
+    const int nb = std::min(slice, B - b0);
+    meshTreeRefitKernel<<<std::min(refitGrid, nb), kRefitThreads, 0, stream>>>(a, b0, nb, boxes);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) break;
+    const long blocks = (long(nb) * a.numPoints + kClosestThreads - 1) / kClosestThreads;
+    closestPointKernel<<<int(std::min<long>(queryGrid, blocks)), kClosestThreads, 0, stream>>>(a, b0, nb, boxes);
+    e = cudaGetLastError();
+  }
+  const cudaError_t f = cudaFreeAsync(boxes, stream);
+  if (e == cudaSuccess) e = f;
+  return e;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Input gradients of one Position / Orientation block, d/d input [grad_theta E . v] (ik_device.cuh tangent* / *InputGradient), in the
 // per-instance frame of skeletonStateKernel:
 //   lanes = parameters: theta, and v gated by the enabled set;  fkPasses with the DOF axes;  tangentPasses: each joint's own motion,

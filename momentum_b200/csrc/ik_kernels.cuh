@@ -194,6 +194,21 @@ struct NormalArgs {
 // Both enqueue on `stream`; the backward takes stream-ordered scratch (cudaMallocAsync) for h of a slice of instances, at most 256 MiB.
 cudaError_t launchVertexNormals(const NormalArgs& a, cudaStream_t stream);
 cudaError_t launchVertexNormalsBackward(const NormalArgs& a, cudaStream_t stream);
+// meshTreeRefitKernel / closestPointKernel: the closest point on each instance's mesh of each of its query points (pymomentum
+// find_closest_points_on_mesh), over the shared tree topology refitted to the instance's vertices
+struct ClosestPointArgs {
+  MeshFaceTables M;
+  MeshTreeTables T;
+  int32_t batch, numPoints;
+  float maxDist2;        // max_dist * max_dist; +inf for no bound
+  const float* vertices; // [B][V][3]
+  const float* points;   // [B][N][3]
+  float* outPoints;      // [B][N][3]
+  int32_t* outFace;      // [B][N]
+  float* outBary;        // [B][N][3]
+};
+// Enqueues on `stream`; the boxes of a slice of instances go to stream-ordered scratch (cudaMallocAsync), at most 256 MiB.
+cudaError_t launchClosestPointsOnMesh(const ClosestPointArgs& a, cudaStream_t stream);
 // inputGradientKernel: d/d input [grad_theta E . v] of one Position or Orientation (matrix difference) block with the L2 loss, per
 // instance: the input contraction of solve_ik's implicit-function backward
 struct InputGradientArgs {

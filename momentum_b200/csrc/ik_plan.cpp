@@ -216,6 +216,70 @@ std::string makeMeshFaces(int32_t numVertices, int32_t numFaces, const int32_t* 
   return "";
 }
 
+std::string makeMeshTree(const HostMeshFaces& faces, int32_t numVertices, const float* referencePositions, HostMeshTree& out) {
+  if (faces.numFaces < 1) return "mesh tree: the mesh has no faces";
+  if (numVertices != faces.numVertices) return "mesh tree: num_vertices differs from the mesh faces' num_vertices";
+  if (referencePositions == nullptr) return "mesh tree: null argument";
+  const int32_t F = faces.numFaces;
+  for (size_t i = 0; i < size_t(numVertices) * 3; ++i)
+    if (!std::isfinite(referencePositions[i])) return "mesh tree: a reference position is not finite";
+  std::vector<double> centroid(size_t(F) * 3);
+  for (int32_t f = 0; f < F; ++f)
+    for (int k = 0; k < 3; ++k) {
+      double s = 0.0;
+      for (int c = 0; c < 3; ++c) s += referencePositions[size_t(faces.faces[size_t(f) * 3 + c]) * 3 + k];
+      centroid[size_t(f) * 3 + k] = s / 3.0;
+    }
+  HostMeshTree t;
+  t.numVertices = numVertices;
+  t.numFaces = F;
+  t.leafFaces.resize(size_t(F));
+  for (int32_t f = 0; f < F; ++f) t.leafFaces[f] = f;
+  // level by level: the nodes of a level are face ranges [lo, hi) of leafFaces; the children of a split node are appended to the next
+  // level in order, so the two are adjacent
+  std::vector<std::pair<int32_t, int32_t>> level{{0, F}}, next;
+  while (!level.empty()) {
+    if (t.depth == kTreeStack) return "mesh tree: the tree is deeper than the traversal stack";
+    t.levelStart.push_back(t.numNodes);
+    const int32_t nextFirst = t.numNodes + int32_t(level.size());
+    next.clear();
+    for (const auto& r : level) {
+      const int32_t lo = r.first, hi = r.second, n = hi - lo;
+      if (n <= kLeafFaces) {
+        t.nodeStart.push_back(lo);
+        t.nodeCount.push_back(n);
+        continue;
+      }
+      double bmin[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, bmax[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
+      for (int32_t i = lo; i < hi; ++i)
+        for (int k = 0; k < 3; ++k) {
+          const double c = centroid[size_t(t.leafFaces[i]) * 3 + k];
+          bmin[k] = std::min(bmin[k], c);
+          bmax[k] = std::max(bmax[k], c);
+        }
+      int axis = 0;
+      for (int k = 1; k < 3; ++k)
+        if (bmax[k] - bmin[k] > bmax[axis] - bmin[axis]) axis = k;
+      std::sort(t.leafFaces.begin() + lo, t.leafFaces.begin() + hi, [&](int32_t a, int32_t b) {
+        const double ca = centroid[size_t(a) * 3 + axis], cb = centroid[size_t(b) * 3 + axis];
+        return ca < cb || (ca == cb && a < b);
+      });
+      t.nodeStart.push_back(nextFirst + int32_t(next.size()));
+      t.nodeCount.push_back(0);
+      const int32_t groups = (n + kLeafFaces - 1) / kLeafFaces; // the median rounded to whole leaves: all leaves but one are full
+      const int32_t mid = lo + (groups + 1) / 2 * kLeafFaces;
+      next.push_back({lo, mid});
+      next.push_back({mid, hi});
+    }
+    t.numNodes += int32_t(level.size());
+    ++t.depth;
+    level.swap(next);
+  }
+  t.levelStart.push_back(t.numNodes);
+  out = std::move(t);
+  return "";
+}
+
 CharacterTables hostCharacterTables(const HostCharacter& ch) {
   CharacterTables C{};
   C.numJoints = ch.numJoints;

@@ -77,6 +77,15 @@ struct HostMeshFaces {
   std::vector<int32_t> vertStart, vertCorner; // [V + 1], [3 F]
 };
 
+// The topology of a bounding-volume tree over a mesh's faces (MeshTreeTables): nodes level by level, leaves of 1 .. kLeafFaces faces.
+// Built by makeMeshTree only; numNodes == 0 when there is none.
+struct HostMeshTree {
+  int32_t numVertices{0}, numFaces{0}, numNodes{0}, depth{0};
+  std::vector<int32_t> nodeStart, nodeCount; // [numNodes]
+  std::vector<int32_t> leafFaces;            // [F]
+  std::vector<int32_t> levelStart;           // [depth + 1]
+};
+
 struct HostErrorFunction {
   int32_t kind{0}; // 0 position, 1 orientation, 2 orientation rot-diff, 3 state, 4 limit, 5 plane, 6 model parameters
   float weight{1.f};
@@ -130,6 +139,12 @@ std::string makeBlendShape(int32_t numShapes, int32_t numVertices, const float* 
 // faces [F][3] over V vertices; V >= 1, F >= 0, 3 F within int32, every index in [0, V). Degenerate faces and faces that repeat an index
 // are accepted (they add a zero normal, and a repeated vertex counts once per corner).
 std::string makeMeshFaces(int32_t numVertices, int32_t numFaces, const int32_t* faces, HostMeshFaces& out);
+// The topology of a bounding-volume tree over `faces` (MeshTreeTables), built from the face centroids of referencePositions [V][3]: a
+// node's faces are ordered by (centroid along the longest axis of their centroid bounds, face index) and split at the median rounded
+// up to whole leaves (the first ceil(g / 2) kLeafFaces faces left, g = ceil(n / kLeafFaces)), until at most kLeafFaces are left, so
+// every leaf but one per level is full. Deterministic. No faces, numVertices other than the
+// faces' V, a null array or a non-finite position is rejected with a message.
+std::string makeMeshTree(const HostMeshFaces& faces, int32_t numVertices, const float* referencePositions, HostMeshTree& out);
 std::string positionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* offsets,
                                   const float* weights, HostErrorFunction& out);
 std::string instancedPositionErrorFunction(const HostCharacter& ch, float weight, float alpha, float c, int32_t nc, const int32_t* parents, const float* weights,

@@ -171,4 +171,18 @@ struct MeshFaceTables {
   const int32_t* vertCorner; // [3F]: 3 f + k of the corners that are the vertex, faces ascending, corners ascending
 };
 
+// Bounding-volume tree over the mesh faces (HostMeshTree, makeMeshTree): the topology only, shared by the whole batch; each instance's
+// boxes are refitted to its vertices per call. Nodes are numbered level by level from the root (node 0); an internal node has its two
+// children at nodeStart, nodeStart + 1 on the next level and nodeCount 0; a leaf holds the faces leafFaces[nodeStart .. + nodeCount),
+// 1 <= nodeCount <= kLeafFaces.
+constexpr int kLeafFaces = 4;  // faces per leaf (DESIGN §4, §7)
+constexpr int kTreeStack = 32; // the traversal's stack: the tree's depth is at most this
+struct MeshTreeTables {
+  int32_t numNodes, depth;
+  const int32_t* nodeStart;  // [numNodes]
+  const int32_t* nodeCount;  // [numNodes]
+  const int32_t* leafFaces;  // [F]: face indices, leaf by leaf
+  const int32_t* levelStart; // [depth + 1]: the nodes of level L are levelStart[L] .. levelStart[L + 1)
+};
+
 } // namespace mb2

@@ -80,6 +80,7 @@ CABI_SYMBOLS = [
     "mb2_character_set_blend_shape", "mb2_character_num_blend_shapes", "mb2_character_skin_with_blend_shapes_device",
     "mb2_character_skin_with_blend_shapes_backward_device",
     "mb2_character_set_mesh_faces", "mb2_character_num_faces", "mb2_character_vertex_normals_device", "mb2_character_vertex_normals_backward_device",
+    "mb2_character_set_mesh_tree", "mb2_character_closest_points_on_mesh_device",
 ]
 
 _libs = {}
@@ -201,6 +202,9 @@ def load_library(path: Optional[str] = None):
         L.mb2_character_num_faces.argtypes = [vp]
         L.mb2_character_vertex_normals_device.argtypes = [vp, C.c_int32, vp, vp, vp]
         L.mb2_character_vertex_normals_backward_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
+    if hasattr(L, "mb2_character_set_mesh_tree"):
+        L.mb2_character_set_mesh_tree.argtypes = [vp, C.c_int32, _fp]
+        L.mb2_character_closest_points_on_mesh_device.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, C.c_float, vp, vp, vp, vp]
     _libs[path] = L
     return L
 
@@ -289,7 +293,7 @@ class DeviceCharacter(_Base):
                 for j in range(27):
                     arr[k].f[j] = float(ff[j])
             self._check(self._L.mb2_character_set_parameter_limits(self._h, len(character.limits), arr))
-        self.skinning, self.faces, self.faces_error = None, None, None
+        self.skinning, self.faces, self.faces_error, self.mesh_tree_error = None, None, None, None
         if character.skinning is not None:
             self.set_skinning(character.skinning)
         # A blend shape the library rejects is reported by the blend-shape calls, not here: the rig, its skinning and every other use of
@@ -313,12 +317,41 @@ class DeviceCharacter(_Base):
         self._check(self._L.mb2_character_set_skinning(self._h, V, rvp, sip, swp, ibp))
         self.skinning = skinning
         self.faces, self.faces_error = None, None
+        self.mesh_tree_error = None
         try:
             self._set_mesh_faces(V, skinning.faces)
             self.faces = skinning.faces
         except (MomentumB200Error, ValueError) as e:
             self._check(self._L.mb2_character_set_mesh_faces(self._h, 0, 0, None))  # no faces left from an earlier skinning
             self.faces_error = str(e)
+        if self.faces is not None and self.faces.shape[0] > 0:
+            # the closest-point tree over the rest mesh; replacing the faces above dropped any earlier one
+            try:
+                self.set_mesh_tree(skinning.rest_vertices)
+            except MomentumB200Error as e:
+                self.mesh_tree_error = str(e)
+
+    def set_mesh_tree(self, reference_positions):
+        """Builds the closest-point tree over the uploaded faces from ``reference_positions`` [V, 3] (``set_skinning`` uses the rest mesh),
+        or removes it when None. The pose changes how fast ``closest_points_on_mesh_device`` is, never what it returns."""
+        if reference_positions is None:
+            self._check(self._L.mb2_character_set_mesh_tree(self._h, 0, None))
+            return
+        x = np.asarray(reference_positions)
+        if x.ndim != 2 or x.shape[1] != 3:
+            raise ValueError(f"mesh tree: reference_positions must be [V, 3], got {x.shape}")
+        xa, xp = _f32(x)
+        self._check(self._L.mb2_character_set_mesh_tree(self._h, int(x.shape[0]), xp))
+        self.mesh_tree_error = None
+
+    def closest_points_on_mesh_device(self, batch: int, num_points: int, vertices_device_ptr: int, points_device_ptr: int, max_dist: float,
+                                      out_points_device_ptr: int, out_face_device_ptr: int, out_bary_device_ptr: int, stream: int = 0):
+        """The closest point on each instance's mesh (vertices [B][V][3]) of its query points [B][N][3]: out points [B][N][3], faces
+        [B][N] int32 (-1 without a face within ``max_dist``) and barycentrics [B][N][3]. Device memory on this character's device,
+        enqueued on ``stream``."""
+        self._check(self._L.mb2_character_closest_points_on_mesh_device(
+            self._h, int(batch), int(num_points), C.c_void_p(vertices_device_ptr), C.c_void_p(points_device_ptr), float(max_dist),
+            C.c_void_p(out_points_device_ptr), C.c_void_p(out_face_device_ptr), C.c_void_p(out_bary_device_ptr), C.c_void_p(stream)))
 
     def _set_mesh_faces(self, num_vertices: int, faces):
         if faces is None:

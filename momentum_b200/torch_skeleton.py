@@ -306,3 +306,80 @@ def compute_vertex_normals(character, vertex_positions: torch.Tensor) -> torch.T
     if dc.faces is None:
         raise ValueError(f"the character's mesh faces were rejected: {dc.faces_error}")
     return _VertexNormals.apply(dc, vertex_positions)
+
+
+def find_closest_points_on_mesh(character, points_source: torch.Tensor, vertices_target: torch.Tensor, max_dist: float = float("inf")):
+    """The closest point on the character's posed mesh of each query point (pymomentum ``geometry.find_closest_points_on_mesh``):
+    ``points_source`` [N, 3] or [B, N, 3] and ``vertices_target`` [V, 3] or [B, V, 3] on one CUDA device; B broadcasts when one side is
+    unbatched. Returns ``(valid, points, face_index, bary)`` in pymomentum's order: bool [.., N], the closest points [.., N, 3] and the
+    barycentrics [.., N, 3] in the inputs' dtype (computed in float32), and int32 face indices [.., N]. Per query the result is the face
+    with the smallest (squared distance, face index) among the faces with finite vertices within ``max_dist`` (default: no bound); a
+    query without one (a non-finite query included) gives valid False, face -1 and zeros. It does not depend on the search tree.
+
+    The faces are ``character.skinning.faces``, as in ``compute_vertex_normals``; the search tree is built once over the rest mesh when
+    they are uploaded, and each call refits its boxes to ``vertices_target``. ``character`` is a ``momentum_b200.character.Character``
+    or a ``solver.DeviceCharacter``.
+
+    Not differentiable: the outputs carry no gradient. For fitting, recompose the point from the vertices with the returned face and
+    barycentrics, ``q = sum_k bary[..., k] * x[face[..., k]]``::
+
+        with torch.no_grad():
+            valid, _, face, bary = find_closest_points_on_mesh(ch, p, x)
+        tri = faces_t[face.clamp(min=0).long()]                                 # [B, N, 3] vertex indices
+        corners = torch.gather(x, 1, tri.reshape(B, -1, 1).expand(-1, -1, 3)).reshape(B, N, 3, 3)
+        q = (bary.unsqueeze(-1) * corners).sum(-2)
+        loss = (((p - q) ** 2).sum(-1) * valid).sum()
+
+    Wherever the closest face is unique, the gradient of ``|p - q|^2`` through this composition, with respect to p and to x, is the exact
+    gradient of the squared point-to-mesh distance (the envelope theorem: the closest point moves along the surface, orthogonally to
+    p - q)."""
+    for name, t in (("points_source", points_source), ("vertices_target", vertices_target)):
+        if not torch.is_tensor(t) or not t.is_cuda:
+            raise ValueError(f"find_closest_points_on_mesh runs on CUDA tensors (there is no CPU fallback); {name} is not one")
+    if points_source.device != vertices_target.device:
+        raise ValueError("points_source and vertices_target must be on the same device")
+    is_handle = isinstance(character, ms.DeviceCharacter)
+    ch = character.character if is_handle else character
+    if not isinstance(ch, mc.Character):
+        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
+    sk = character.skinning if is_handle else ch.skinning
+    if sk is None:
+        raise ValueError("the character has no skinning, so no mesh faces")
+    if is_handle and character.faces is None:
+        rejected = character.faces_error
+        raise ValueError("the character has no mesh faces" + (f" (their upload was rejected: {rejected})" if rejected else ""))
+    if not is_handle and sk.faces is None:
+        raise ValueError("the character has no mesh faces (character.skinning.faces)")
+    V = sk.num_vertices
+    if vertices_target.dim() not in (2, 3) or vertices_target.shape[-2:] != (V, 3):
+        raise ValueError(f"vertices_target must be [V, 3] or [B, V, 3] with V = {V}, got {tuple(vertices_target.shape)}")
+    if points_source.dim() not in (2, 3) or points_source.shape[-1] != 3:
+        raise ValueError(f"points_source must be [N, 3] or [B, N, 3], got {tuple(points_source.shape)}")
+    if points_source.dim() == 3 and vertices_target.dim() == 3 and points_source.shape[0] != vertices_target.shape[0]:
+        raise ValueError(f"points_source and vertices_target have batches {points_source.shape[0]} and {vertices_target.shape[0]}")
+    max_dist = float(max_dist)
+    if not max_dist >= 0.0:
+        raise ValueError(f"max_dist must be >= 0 (float('inf') for no bound), got {max_dist}")
+    dev = points_source.device
+    dc = _device_character(character, dev) if is_handle else _skinned_device_character(ch, dev)
+    if dc.faces is None:
+        raise ValueError(f"the character's mesh faces were rejected: {dc.faces_error}")
+    if dc.faces.shape[0] == 0 or dc.mesh_tree_error is not None:
+        raise ValueError("the character's mesh has no closest-point tree" + (f": {dc.mesh_tree_error}" if dc.mesh_tree_error else " (no faces)"))
+    batched = points_source.dim() == 3 or vertices_target.dim() == 3
+    B = points_source.shape[0] if points_source.dim() == 3 else (vertices_target.shape[0] if vertices_target.dim() == 3 else 1)
+    N = points_source.shape[-2]
+    dtype = torch.promote_types(points_source.dtype, vertices_target.dtype)
+    with torch.no_grad():
+        p = points_source.detach().to(torch.float32).expand(B, N, 3).contiguous()
+        x = vertices_target.detach().to(torch.float32).expand(B, V, 3).contiguous()
+        q = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
+        face = torch.empty(B, N, device=dev, dtype=torch.int32)
+        bary = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
+        dc.closest_points_on_mesh_device(B, N, x.data_ptr(), p.data_ptr(), max_dist, q.data_ptr(), face.data_ptr(), bary.data_ptr(),
+                                         torch.cuda.current_stream(dev).cuda_stream)
+        valid = face >= 0
+        q, bary = q.to(dtype), bary.to(dtype)
+    if not batched:
+        valid, q, face, bary = valid[0], q[0], face[0], bary[0]
+    return valid, q, face, bary
