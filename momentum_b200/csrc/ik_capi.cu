@@ -137,7 +137,13 @@ struct mb2_character {
   // bounding-volume tree over the faces (mb2_character_set_mesh_tree): numNodes == 0 when there is none
   HostMeshTree tree;
   std::unique_ptr<MeshTreeBuffers> treeDev; // replaced whole by mb2_character_set_mesh_tree, dropped by mb2_character_set_mesh_faces
-  CharacterTables tables() const; // the device copies above, as the kernels read them
+  // the device copies above, as the kernels read them; each mesh table only while it is installed
+  CharacterTables tables() const;
+  SkeletonTables skeletonTables() const; // the skeleton-state backward's
+  SkinTables skinTables() const;
+  BlendShapeTables blendShapeTables() const;
+  MeshFaceTables meshFaceTables() const;
+  MeshTreeTables meshTreeTables() const;
 };
 
 struct DeviceSchedule {
@@ -243,23 +249,53 @@ CharacterTables mb2_character::tables() const {
   return C;
 }
 
+SkeletonTables mb2_character::skeletonTables() const { return SkeletonTables{childStart.p, children.p, ptColStart.p, ptColRows.p, ptColVals.p}; }
+
+SkinTables mb2_character::skinTables() const {
+  const SkinBuffers& d = *skinDev;
+  return SkinTables{skin.numVertices, skin.numSegments(), d.rest.p, d.vertStart.p, d.vertJoint.p, d.vertWeight.p,
+                    d.ibp.p, d.infVertex.p, d.infWeight.p, d.segStart.p, d.segJoint.p, d.jointSegStart.p};
+}
+
+BlendShapeTables mb2_character::blendShapeTables() const { return BlendShapeTables{blend.numShapes, blendDev->baseShape.p, blendDev->shapeVectors.p}; }
+
+MeshFaceTables mb2_character::meshFaceTables() const {
+  return MeshFaceTables{faces.numVertices, faces.numFaces, facesDev->faces.p, facesDev->vertStart.p, facesDev->vertCorner.p};
+}
+
+MeshTreeTables mb2_character::meshTreeTables() const {
+  return MeshTreeTables{tree.numNodes, tree.depth, treeDev->nodeStart.p, treeDev->nodeCount.p, treeDev->leafFaces.p, treeDev->levelStart.p};
+}
+
 namespace {
-// installs tree t (numNodes == 0: none) as mb2_character_set_mesh_faces installs its tables: fresh buffers, and the device synchronised
-// before the old ones are freed
-int installMeshTree(mb2_character* c, HostMeshTree&& t) {
-  MB2_DEVICE_GUARD(c->device);
-  std::unique_ptr<MeshTreeBuffers> d;
-  if (t.numNodes > 0) {
-    d = std::make_unique<MeshTreeBuffers>();
-    MB2_CUDA(d->nodeStart.upload(t.nodeStart, nullptr));
-    MB2_CUDA(d->nodeCount.upload(t.nodeCount, nullptr));
-    MB2_CUDA(d->leafFaces.upload(t.leafFaces, nullptr));
-    MB2_CUDA(d->levelStart.upload(t.levelStart, nullptr));
+// Replaces one of a character's mesh tables: fresh device buffers, filled by upload(buffers, fresh) when `present` (else none), so that a
+// failed upload leaves the earlier table whole; the device is synchronised before the swap, so no work in flight on any stream still
+// reads the buffers that are freed.
+template <class Buffers, class Host, class Upload>
+int installTables(int device, std::unique_ptr<Buffers>& dev, Host& host, Host&& fresh, Upload upload, bool present = true) {
+  MB2_DEVICE_GUARD(device);
+  std::unique_ptr<Buffers> d;
+  if (present) {
+    d = std::make_unique<Buffers>();
+    const int rc = upload(*d, fresh);
+    if (rc != MB2_OK) return rc;
   }
   MB2_CUDA(cudaDeviceSynchronize());
-  c->treeDev = std::move(d);
-  c->tree = std::move(t);
+  dev = std::move(d);
+  host = std::move(fresh);
   return MB2_OK;
+}
+
+// installs tree t (numNodes == 0: none)
+int installMeshTree(mb2_character* c, HostMeshTree&& t) {
+  const bool present = t.numNodes > 0;
+  return installTables(c->device, c->treeDev, c->tree, std::move(t), [](MeshTreeBuffers& d, const HostMeshTree& t) -> int {
+    MB2_CUDA(d.nodeStart.upload(t.nodeStart, nullptr));
+    MB2_CUDA(d.nodeCount.upload(t.nodeCount, nullptr));
+    MB2_CUDA(d.leafFaces.upload(t.leafFaces, nullptr));
+    MB2_CUDA(d.levelStart.upload(t.levelStart, nullptr));
+    return MB2_OK;
+  }, present);
 }
 } // namespace
 
@@ -648,24 +684,19 @@ int mb2_character_set_skinning(mb2_character* c, int32_t num_vertices, const flo
   HostSkinning s;
   const std::string err = makeSkinning(c->host, num_vertices, rest_vertices, skin_index, skin_weight, inverse_bind_pose, s);
   if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
-  MB2_DEVICE_GUARD(c->device);
-  // fresh buffers: a failed upload leaves the earlier skinning whole; the device is synchronised before the swap, so no work in flight
-  // on any stream still reads the tables that are freed
-  auto d = std::make_unique<SkinBuffers>();
-  MB2_CUDA(d->rest.upload(s.restVertices, nullptr));
-  MB2_CUDA(d->vertStart.upload(s.vertStart, nullptr));
-  MB2_CUDA(d->vertJoint.upload(s.vertJoint, nullptr));
-  MB2_CUDA(d->vertWeight.upload(s.vertWeight, nullptr));
-  MB2_CUDA(d->ibp.upload(s.inverseBindPose, nullptr));
-  MB2_CUDA(d->infVertex.upload(s.infVertex, nullptr));
-  MB2_CUDA(d->infWeight.upload(s.infWeight, nullptr));
-  MB2_CUDA(d->segStart.upload(s.segStart, nullptr));
-  MB2_CUDA(d->segJoint.upload(s.segJoint, nullptr));
-  MB2_CUDA(d->jointSegStart.upload(s.jointSegStart, nullptr));
-  MB2_CUDA(cudaDeviceSynchronize());
-  c->skinDev = std::move(d);
-  c->skin = std::move(s);
-  return MB2_OK;
+  return installTables(c->device, c->skinDev, c->skin, std::move(s), [](SkinBuffers& d, const HostSkinning& s) -> int {
+    MB2_CUDA(d.rest.upload(s.restVertices, nullptr));
+    MB2_CUDA(d.vertStart.upload(s.vertStart, nullptr));
+    MB2_CUDA(d.vertJoint.upload(s.vertJoint, nullptr));
+    MB2_CUDA(d.vertWeight.upload(s.vertWeight, nullptr));
+    MB2_CUDA(d.ibp.upload(s.inverseBindPose, nullptr));
+    MB2_CUDA(d.infVertex.upload(s.infVertex, nullptr));
+    MB2_CUDA(d.infWeight.upload(s.infWeight, nullptr));
+    MB2_CUDA(d.segStart.upload(s.segStart, nullptr));
+    MB2_CUDA(d.segJoint.upload(s.segJoint, nullptr));
+    MB2_CUDA(d.jointSegStart.upload(s.jointSegStart, nullptr));
+    return MB2_OK;
+  });
 }
 
 int32_t mb2_character_num_vertices(const mb2_character* c) { return c ? c->skin.numVertices : 0; }
@@ -675,15 +706,11 @@ int mb2_character_set_blend_shape(mb2_character* c, int32_t num_shapes, int32_t 
   HostBlendShape b;
   const std::string err = makeBlendShape(num_shapes, num_vertices, base_shape, shape_vectors, b);
   if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
-  MB2_DEVICE_GUARD(c->device);
-  // as mb2_character_set_skinning: fresh buffers, and the device synchronised before the old ones are freed
-  auto d = std::make_unique<BlendShapeBuffers>();
-  MB2_CUDA(d->baseShape.upload(b.baseShape, nullptr));
-  MB2_CUDA(d->shapeVectors.upload(b.shapeVectors, nullptr));
-  MB2_CUDA(cudaDeviceSynchronize());
-  c->blendDev = std::move(d);
-  c->blend = std::move(b);
-  return MB2_OK;
+  return installTables(c->device, c->blendDev, c->blend, std::move(b), [](BlendShapeBuffers& d, const HostBlendShape& b) -> int {
+    MB2_CUDA(d.baseShape.upload(b.baseShape, nullptr));
+    MB2_CUDA(d.shapeVectors.upload(b.shapeVectors, nullptr));
+    return MB2_OK;
+  });
 }
 
 int32_t mb2_character_num_blend_shapes(const mb2_character* c) { return c ? c->blend.numShapes : 0; }
@@ -695,19 +722,15 @@ int mb2_character_set_mesh_faces(mb2_character* c, int32_t num_vertices, int32_t
     const std::string err = makeMeshFaces(num_vertices, num_faces, faces, m);
     if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
   }
-  MB2_DEVICE_GUARD(c->device);
-  // as mb2_character_set_skinning: fresh buffers, and the device synchronised before the old ones are freed
-  std::unique_ptr<MeshFaceBuffers> d;
-  if (m.numVertices > 0) {
-    d = std::make_unique<MeshFaceBuffers>();
-    MB2_CUDA(d->faces.upload(m.faces, nullptr));
-    MB2_CUDA(d->vertStart.upload(m.vertStart, nullptr));
-    MB2_CUDA(d->vertCorner.upload(m.vertCorner, nullptr));
-  }
-  MB2_CUDA(cudaDeviceSynchronize());
-  c->facesDev = std::move(d);
-  c->faces = std::move(m);
-  c->treeDev.reset(); // built over the faces it replaced
+  const bool present = m.numVertices > 0;
+  const int rc = installTables(c->device, c->facesDev, c->faces, std::move(m), [](MeshFaceBuffers& d, const HostMeshFaces& m) -> int {
+    MB2_CUDA(d.faces.upload(m.faces, nullptr));
+    MB2_CUDA(d.vertStart.upload(m.vertStart, nullptr));
+    MB2_CUDA(d.vertCorner.upload(m.vertCorner, nullptr));
+    return MB2_OK;
+  }, present);
+  if (rc != MB2_OK) return rc;
+  c->treeDev.reset(); // built over the faces it replaced; the swap above synchronised the device
   c->tree = HostMeshTree{};
   return MB2_OK;
 }
@@ -1005,6 +1028,15 @@ bool isDeviceMemoryOn(const void* p, int device) {
   return attr.type == cudaMemoryTypeDevice && attr.device == device;
 }
 
+// every `required` array, and every non-null `optional` one, is device memory on `device`
+bool onDevice(int device, std::initializer_list<const void*> required, std::initializer_list<const void*> optional = {}) {
+  for (const void* p : required)
+    if (!isDeviceMemoryOn(p, device)) return false;
+  for (const void* p : optional)
+    if (p != nullptr && !isDeviceMemoryOn(p, device)) return false;
+  return true;
+}
+
 // both directions of mb2_character_skeleton_state*_device (gradState is read by the backward only)
 int skeletonStateDevice(const mb2_character* c, int32_t batch, const float* theta, const float* gradState, float* out, void* stream, bool backward) {
   MB2_CHECK(c != nullptr, "null character");
@@ -1012,18 +1044,12 @@ int skeletonStateDevice(const mb2_character* c, int32_t batch, const float* thet
   if (batch == 0) return MB2_OK;
   MB2_CHECK(theta != nullptr && out != nullptr && (!backward || gradState != nullptr), "null argument");
   MB2_DEVICE_GUARD(c->device);
-  MB2_CHECK(isDeviceMemoryOn(theta, c->device) && isDeviceMemoryOn(out, c->device) && (!backward || isDeviceMemoryOn(gradState, c->device)),
-            "skeleton state: every array must be device memory on the character's device");
+  MB2_CHECK(onDevice(c->device, {theta, out}, {gradState}), "skeleton state: every array must be device memory on the character's device");
   NvtxRange range(backward ? "skeletonStateBackward" : "skeletonState");
-  const HostCharacter& h = c->host;
   SkeletonStateArgs a{};
   a.T = c->tables();
-  a.S.childStart = c->childStart.p;
-  a.S.children = c->children.p;
-  a.S.ptColStart = c->ptColStart.p;
-  a.S.ptColRows = c->ptColRows.p;
-  a.S.ptColVals = c->ptColVals.p;
-  a.numChildren = int(h.children.size());
+  a.S = c->skeletonTables();
+  a.numChildren = int(c->host.children.size());
   a.batch = batch;
   a.theta = theta;
   a.gradState = gradState;
@@ -1050,19 +1076,7 @@ int skinArgs(const mb2_character* c, int32_t batch, const float* skelState, cons
   MB2_CHECK(batch >= 0, "batch must not be negative");
   MB2_CHECK(batch == 0 || restPoints != nullptr || restBatched == 0, "skin points: batched rest points need a rest_points array");
   a = SkinArgs{};
-  const HostSkinning& s = c->skin;
-  a.S.numVertices = s.numVertices;
-  a.S.numSegments = s.numSegments();
-  a.S.restVertices = c->skinDev->rest.p;
-  a.S.vertStart = c->skinDev->vertStart.p;
-  a.S.vertJoint = c->skinDev->vertJoint.p;
-  a.S.vertWeight = c->skinDev->vertWeight.p;
-  a.S.inverseBindPose = c->skinDev->ibp.p;
-  a.S.infVertex = c->skinDev->infVertex.p;
-  a.S.infWeight = c->skinDev->infWeight.p;
-  a.S.segStart = c->skinDev->segStart.p;
-  a.S.segJoint = c->skinDev->segJoint.p;
-  a.S.jointSegStart = c->skinDev->jointSegStart.p;
+  a.S = c->skinTables();
   a.numJoints = c->host.numJoints;
   a.batch = batch;
   a.skelState = skelState;
@@ -1079,8 +1093,7 @@ int mb2_character_skin_points_device(const mb2_character* c, int32_t batch, cons
   if (rc != MB2_OK || batch == 0) return rc;
   MB2_CHECK(skel_state_device != nullptr && points_device != nullptr, "null argument");
   MB2_DEVICE_GUARD(c->device);
-  MB2_CHECK(isDeviceMemoryOn(skel_state_device, c->device) && isDeviceMemoryOn(points_device, c->device) &&
-                (rest_points_device == nullptr || isDeviceMemoryOn(rest_points_device, c->device)),
+  MB2_CHECK(onDevice(c->device, {skel_state_device, points_device}, {rest_points_device}),
             "skin points: every array must be device memory on the character's device");
   NvtxRange range("skinPoints");
   a.points = points_device;
@@ -1099,10 +1112,8 @@ int mb2_character_skin_points_backward_device(const mb2_character* c, int32_t ba
   if (batch == 0) return MB2_OK;
   MB2_CHECK(skel_state_device != nullptr && grad_points_device != nullptr, "null argument");
   MB2_DEVICE_GUARD(c->device);
-  bool onDevice = isDeviceMemoryOn(skel_state_device, c->device) && isDeviceMemoryOn(grad_points_device, c->device) &&
-                  (rest_points_device == nullptr || isDeviceMemoryOn(rest_points_device, c->device));
-  for (float* o : {grad_skel_state_device, grad_rest_points_device}) onDevice = onDevice && (o == nullptr || isDeviceMemoryOn(o, c->device));
-  MB2_CHECK(onDevice, "skin points: every array must be device memory on the character's device");
+  MB2_CHECK(onDevice(c->device, {skel_state_device, grad_points_device}, {rest_points_device, grad_skel_state_device, grad_rest_points_device}),
+            "skin points: every array must be device memory on the character's device");
   NvtxRange range("skinPointsBackward");
   a.gradPoints = grad_points_device;
   a.gradState = grad_skel_state_device;
@@ -1121,7 +1132,7 @@ int blendSkinArgs(const mb2_character* c, int32_t batch, const float* skelState,
   MB2_CHECK(numWeights >= 1 && numWeights <= c->blend.numShapes, "skin with blend shapes: num_weights must be in [1, number of shape vectors]");
   int rc = skinArgs(c, batch, skelState, nullptr, 0, a.skin);
   if (rc != MB2_OK) return rc;
-  a.Bs = BlendShapeTables{c->blend.numShapes, c->blendDev->baseShape.p, c->blendDev->shapeVectors.p};
+  a.Bs = c->blendShapeTables();
   a.skin.restPoints = nullptr;
   a.numWeights = numWeights;
   a.blendWeights = blendWeights;
@@ -1137,7 +1148,7 @@ int mb2_character_skin_with_blend_shapes_device(const mb2_character* c, int32_t 
   if (rc != MB2_OK || batch == 0) return rc;
   MB2_CHECK(skel_state_device != nullptr && blend_weights_device != nullptr && points_device != nullptr, "null argument");
   MB2_DEVICE_GUARD(c->device);
-  MB2_CHECK(isDeviceMemoryOn(skel_state_device, c->device) && isDeviceMemoryOn(blend_weights_device, c->device) && isDeviceMemoryOn(points_device, c->device),
+  MB2_CHECK(onDevice(c->device, {skel_state_device, blend_weights_device, points_device}),
             "skin with blend shapes: every array must be device memory on the character's device");
   MB2_CHECK(blendSkinFits(a), "skin with blend shapes: num_weights is too large for the device's shared memory");
   NvtxRange range("skinWithBlendShapes");
@@ -1154,10 +1165,8 @@ int mb2_character_skin_with_blend_shapes_backward_device(const mb2_character* c,
   if (rc != MB2_OK || batch == 0) return rc;
   MB2_CHECK(skel_state_device != nullptr && blend_weights_device != nullptr && grad_points_device != nullptr, "null argument");
   MB2_DEVICE_GUARD(c->device);
-  bool onDevice = isDeviceMemoryOn(skel_state_device, c->device) && isDeviceMemoryOn(blend_weights_device, c->device) &&
-                  isDeviceMemoryOn(grad_points_device, c->device);
-  for (float* o : {grad_skel_state_device, grad_blend_weights_device}) onDevice = onDevice && (o == nullptr || isDeviceMemoryOn(o, c->device));
-  MB2_CHECK(onDevice, "skin with blend shapes: every array must be device memory on the character's device");
+  MB2_CHECK(onDevice(c->device, {skel_state_device, blend_weights_device, grad_points_device}, {grad_skel_state_device, grad_blend_weights_device}),
+            "skin with blend shapes: every array must be device memory on the character's device");
   MB2_CHECK(blendSkinFits(a), "skin with blend shapes: num_weights is too large for the device's shared memory");
   NvtxRange range("skinWithBlendShapesBackward");
   a.skin.gradPoints = grad_points_device;
@@ -1174,7 +1183,7 @@ int normalArgs(const mb2_character* c, int32_t batch, NormalArgs& a) {
   MB2_CHECK(c->faces.numVertices > 0, "vertex normals: the character has no mesh faces (mb2_character_set_mesh_faces)");
   MB2_CHECK(batch >= 0, "batch must not be negative");
   a = NormalArgs{};
-  a.M = MeshFaceTables{c->faces.numVertices, c->faces.numFaces, c->facesDev->faces.p, c->facesDev->vertStart.p, c->facesDev->vertCorner.p};
+  a.M = c->meshFaceTables();
   a.batch = batch;
   return MB2_OK;
 }
@@ -1186,8 +1195,7 @@ int mb2_character_vertex_normals_device(const mb2_character* c, int32_t batch, c
   if (rc != MB2_OK || batch == 0) return rc;
   MB2_CHECK(positions_device != nullptr && normals_device != nullptr, "vertex normals: null argument");
   MB2_DEVICE_GUARD(c->device);
-  MB2_CHECK(isDeviceMemoryOn(positions_device, c->device) && isDeviceMemoryOn(normals_device, c->device),
-            "vertex normals: every array must be device memory on the character's device");
+  MB2_CHECK(onDevice(c->device, {positions_device, normals_device}), "vertex normals: every array must be device memory on the character's device");
   NvtxRange range("vertexNormals");
   a.positions = positions_device;
   a.normals = normals_device;
@@ -1208,15 +1216,12 @@ int mb2_character_closest_points_on_mesh_device(const mb2_character* c, int32_t 
                 out_bary_device != nullptr,
             "closest points: null argument");
   MB2_DEVICE_GUARD(c->device);
-  MB2_CHECK(isDeviceMemoryOn(vertex_positions_device, c->device) && isDeviceMemoryOn(points_device, c->device) &&
-                isDeviceMemoryOn(out_points_device, c->device) && isDeviceMemoryOn(out_face_device, c->device) &&
-                isDeviceMemoryOn(out_bary_device, c->device),
+  MB2_CHECK(onDevice(c->device, {vertex_positions_device, points_device, out_points_device, out_face_device, out_bary_device}),
             "closest points: every array must be device memory on the character's device");
   NvtxRange range("closestPointsOnMesh");
   ClosestPointArgs a{};
-  a.M = MeshFaceTables{c->faces.numVertices, c->faces.numFaces, c->facesDev->faces.p, c->facesDev->vertStart.p, c->facesDev->vertCorner.p};
-  a.T = MeshTreeTables{c->tree.numNodes, c->tree.depth, c->treeDev->nodeStart.p, c->treeDev->nodeCount.p, c->treeDev->leafFaces.p,
-                       c->treeDev->levelStart.p};
+  a.M = c->meshFaceTables();
+  a.T = c->meshTreeTables();
   a.batch = batch;
   a.numPoints = num_points;
   a.maxDist2 = max_dist * max_dist;
@@ -1236,8 +1241,7 @@ int mb2_character_vertex_normals_backward_device(const mb2_character* c, int32_t
   if (rc != MB2_OK || batch == 0) return rc;
   MB2_CHECK(positions_device != nullptr && grad_normals_device != nullptr && grad_positions_device != nullptr, "vertex normals: null argument");
   MB2_DEVICE_GUARD(c->device);
-  MB2_CHECK(isDeviceMemoryOn(positions_device, c->device) && isDeviceMemoryOn(grad_normals_device, c->device) &&
-                isDeviceMemoryOn(grad_positions_device, c->device),
+  MB2_CHECK(onDevice(c->device, {positions_device, grad_normals_device, grad_positions_device}),
             "vertex normals: every array must be device memory on the character's device");
   NvtxRange range("vertexNormalsBackward");
   a.positions = positions_device;
@@ -1258,9 +1262,8 @@ int mb2_solver_function_input_gradients_device(mb2_solver_function* f, int32_t i
   MB2_CHECK(parameters_device != nullptr && direction_device != nullptr, "null parameters or direction");
   MB2_DEVICE_GUARD(f->ch->device);
   float* outs[3] = {grad_weights_device, grad_offsets_device, grad_targets_device};
-  bool onDevice = isDeviceMemoryOn(parameters_device, f->ch->device) && isDeviceMemoryOn(direction_device, f->ch->device);
-  for (float* o : outs) onDevice = onDevice && (o == nullptr || isDeviceMemoryOn(o, f->ch->device));
-  MB2_CHECK(onDevice, "input gradients: every array must be device memory on the function's device");
+  MB2_CHECK(onDevice(f->ch->device, {parameters_device, direction_device}, {grad_weights_device, grad_offsets_device, grad_targets_device}),
+            "input gradients: every array must be device memory on the function's device");
   int rc = ensurePlan(f, f->planMode, f->planSchedDense, f->planAlignRows);
   if (rc != MB2_OK) return rc;
   NvtxRange range("inputGradients");
@@ -1302,12 +1305,9 @@ int mb2_solver_function_implicit_direction_device(mb2_solver_function* f, const 
   MB2_CHECK(parameters_device != nullptr && grad_parameters_device != nullptr, "null parameters or gradient");
   MB2_CHECK(direction_device != nullptr, "null direction");
   MB2_DEVICE_GUARD(f->ch->device);
-  const float* ins[2] = {parameters_device, grad_parameters_device};
-  float* outs[4] = {direction_device, jacobian_direction_device, residual_device, gradient_rms_device};
-  bool onDevice = true;
-  for (const float* p : ins) onDevice = onDevice && isDeviceMemoryOn(p, f->ch->device);
-  for (float* o : outs) onDevice = onDevice && (o == nullptr || isDeviceMemoryOn(o, f->ch->device));
-  MB2_CHECK(onDevice, "implicit direction: every array must be device memory on the function's device");
+  MB2_CHECK(onDevice(f->ch->device, {parameters_device, grad_parameters_device},
+                     {direction_device, jacobian_direction_device, residual_device, gradient_rms_device}),
+            "implicit direction: every array must be device memory on the function's device");
   int rc = ensurePlan(f, 0); // the API-order Jacobian: column c = model parameter c
   if (rc != MB2_OK) return rc;
   NvtxRange range("implicitDirection");

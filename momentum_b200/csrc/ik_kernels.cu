@@ -352,6 +352,26 @@ cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaS
   return launchInstanceGroups(backward ? reverse : forward, a, skeletonStateSmemPerInstance(a.T, backward), skeletonStateTableBytes(a, backward), stream);
 }
 
+// The per-instance scratch of the skinning, blend-shape and normals backward passes and of the closest-point refit: at most
+// kSliceScratchBudget bytes at once, the instances run in slices that fit (at least one instance each). No instance's result depends on
+// the slice it falls in.
+constexpr size_t kSliceScratchBudget = size_t(256) << 20;
+
+namespace {
+// One stream-ordered allocation of slice x perInstance bytes, then body(scratch, slice, b0, nb) for the instances b0 .. b0 + nb of each
+// slice in order; nb < slice for the last one. Returns the first error.
+template <class Body>
+cudaError_t forEachInstanceSlice(int batch, size_t perInstance, cudaStream_t stream, Body body) {
+  const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(batch), kSliceScratchBudget / perInstance)));
+  float* scratch = nullptr;
+  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&scratch), perInstance * slice, stream);
+  if (e != cudaSuccess) return e;
+  for (int b0 = 0; e == cudaSuccess && b0 < batch; b0 += slice) e = body(scratch, slice, b0, std::min(slice, batch - b0));
+  const cudaError_t f = cudaFreeAsync(scratch, stream);
+  return e != cudaSuccess ? e : f;
+}
+} // namespace
+
 // ------------------------------------------------------------------------------------------------
 // Linear-blend skinning of a batch (ik_device.cuh skin*), three kernels. The skin tables are shared by the batch and stay in L2.
 //   skinVertexKernel<kMode>  a persistent grid of work items (instances, vertex range): per instance the CTA writes the J skinning
@@ -367,7 +387,6 @@ constexpr int kSkinThreads = 256;
 constexpr int kSkinVertsPerThread = 4;                              // kMode 2 keeps their sums in registers
 constexpr int kSkinChunkVerts = kSkinThreads * kSkinVertsPerThread; // vertex range of a kMode 2 work item
 constexpr int kSkinMaxBatchChunks = 128;                            // kMode 2 scratch: at most 128 x [V][3] floats
-constexpr size_t kSkinPartialBudget = size_t(256) << 20;            // skel-state backward scratch: instances processed in slices
 
 template <int kMode>
 __global__ void __launch_bounds__(kSkinThreads) skinVertexKernel(const SkinArgs a, int perChunk, int numChunks, int vSplit, int vLen, float* out) {
@@ -503,22 +522,16 @@ cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream) {
   if (a.gradState != nullptr && a.S.numSegments == 0) { // no influences at all: the gradient is zero
     e = cudaMemsetAsync(a.gradState, 0, size_t(a.batch) * J * 8 * sizeof(float), stream);
   } else if (a.gradState != nullptr) {
-    const size_t perInstance = size_t(a.S.numSegments) * kSkinAccFloats * sizeof(float);
-    const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(a.batch), kSkinPartialBudget / perInstance)));
-    float* partial = nullptr;
-    e = cudaMallocAsync(reinterpret_cast<void**>(&partial), perInstance * slice, stream);
-    if (e != cudaSuccess) return e;
-    int g1 = 0, g2 = 0;
-    e = persistentGrid(skinStatePartialKernel, kSkinThreads, 0, (long(slice) * a.S.numSegments + 7) / 8, &g1);
-    if (e == cudaSuccess) e = persistentGrid(skinStateFinishKernel, kSkinThreads, 0, (long(slice) * J + kSkinThreads - 1) / kSkinThreads, &g2);
-    for (int b0 = 0; e == cudaSuccess && b0 < a.batch; b0 += slice) {
-      const int nb = std::min(slice, a.batch - b0);
+    e = forEachInstanceSlice(a.batch, size_t(a.S.numSegments) * kSkinAccFloats * sizeof(float), stream, [&](float* partial, int slice, int b0, int nb) {
+      // grids sized for a whole slice, the last one included
+      int g1 = 0, g2 = 0;
+      cudaError_t r = persistentGrid(skinStatePartialKernel, kSkinThreads, 0, (long(slice) * a.S.numSegments + 7) / 8, &g1);
+      if (r == cudaSuccess) r = persistentGrid(skinStateFinishKernel, kSkinThreads, 0, (long(slice) * J + kSkinThreads - 1) / kSkinThreads, &g2);
+      if (r != cudaSuccess) return r;
       skinStatePartialKernel<<<g1, kSkinThreads, 0, stream>>>(a, b0, nb, partial);
       skinStateFinishKernel<<<g2, kSkinThreads, 0, stream>>>(a, b0, nb, partial);
-      e = cudaGetLastError();
-    }
-    const cudaError_t f = cudaFreeAsync(partial, stream);
-    if (e == cudaSuccess) e = f;
+      return cudaGetLastError();
+    });
   }
   if (e != cudaSuccess || a.gradRest == nullptr) return e;
   if (a.restBatched) return launchSkinPerInstance<1>(a, a.gradRest, stream);
@@ -566,7 +579,6 @@ constexpr int kBlendTileMax = 16;                        // instances per tile w
 constexpr int kBlendTileMin = 4;                         // otherwise
 constexpr int kBlendGroups = kSkinThreads / 64;          // blendWeightPartialKernel: thread = (group, k of a 64-wide block of K')
 constexpr int kBlendGroupVerts = kSkinThreads / kBlendGroups;
-constexpr size_t kBlendRestBudget = size_t(256) << 20;   // skel-state backward: shaped rest points of a slice of instances
 
 template <int T, bool kRestOnly>
 __global__ void __launch_bounds__(kSkinThreads, 2) blendSkinKernel(const BlendSkinArgs a, int b0, int nb, float* rest) {
@@ -727,15 +739,11 @@ cudaError_t launchSkinWithBlendShapesBackward(const BlendSkinArgs& a, cudaStream
   if (B <= 0) return cudaSuccess;
   cudaError_t e = cudaSuccess;
   if (a.skin.gradState != nullptr) {
-    // the shaped rest points of a slice of instances, then skin_points' own state-gradient path with them as batched rest points
-    const size_t perInstance = size_t(V) * 3 * sizeof(float);
-    const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(B), kBlendRestBudget / perInstance)));
-    float* rest = nullptr;
-    e = cudaMallocAsync(reinterpret_cast<void**>(&rest), perInstance * slice, stream);
-    if (e != cudaSuccess) return e;
-    for (int b0 = 0; e == cudaSuccess && b0 < B; b0 += slice) {
-      const int nb = std::min(slice, B - b0);
-      e = launchBlendSkin<true>(a, b0, nb, rest, stream);
+    // the shaped rest points of a slice of instances, then skin_points' own state-gradient path with them as batched rest points (its
+    // partial sums are allocated while the slice's rest points are)
+    e = forEachInstanceSlice(B, size_t(V) * 3 * sizeof(float), stream, [&](float* rest, int, int b0, int nb) {
+      const cudaError_t r = launchBlendSkin<true>(a, b0, nb, rest, stream);
+      if (r != cudaSuccess) return r;
       SkinArgs s = a.skin;
       s.batch = nb;
       s.skelState += size_t(b0) * J * 8;
@@ -745,34 +753,23 @@ cudaError_t launchSkinWithBlendShapesBackward(const BlendSkinArgs& a, cudaStream
       s.restBatched = 1;
       s.points = nullptr;
       s.gradRest = nullptr;
-      if (e == cudaSuccess) e = launchSkinPointsBackward(s, stream);
-    }
-    const cudaError_t f = cudaFreeAsync(rest, stream);
-    if (e == cudaSuccess) e = f;
+      return launchSkinPointsBackward(s, stream);
+    });
   }
   if (e != cudaSuccess || a.gradWeights == nullptr) return e;
   const int vBlocks = (V + kSkinThreads - 1) / kSkinThreads;
-  const size_t perInstance = size_t(vBlocks) * Kp * sizeof(float);
-  const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(B), kSkinPartialBudget / perInstance)));
-  float* partial = nullptr;
-  e = cudaMallocAsync(reinterpret_cast<void**>(&partial), perInstance * slice, stream);
-  if (e != cudaSuccess) return e;
-  for (int b0 = 0; e == cudaSuccess && b0 < B; b0 += slice) {
-    const int nb = std::min(slice, B - b0);
+  return forEachInstanceSlice(B, size_t(vBlocks) * Kp * sizeof(float), stream, [&](float* partial, int, int b0, int nb) {
     int T = 0, grid = 0;
     const size_t s16 = blendWeightSmem(a, kBlendTileMax), s4 = blendWeightSmem(a, kBlendTileMin);
-    e = chooseBlendTile(blendWeightPartialKernel<kBlendTileMax>, s16, blendWeightPartialKernel<kBlendTileMin>, s4, V, nb, &T, &grid);
-    if (e != cudaSuccess) break;
+    const cudaError_t r = chooseBlendTile(blendWeightPartialKernel<kBlendTileMax>, s16, blendWeightPartialKernel<kBlendTileMin>, s4, V, nb, &T, &grid);
+    if (r != cudaSuccess) return r;
     if (T == kBlendTileMax) blendWeightPartialKernel<kBlendTileMax><<<grid, kSkinThreads, s16, stream>>>(a, b0, nb, partial);
     else blendWeightPartialKernel<kBlendTileMin><<<grid, kSkinThreads, s4, stream>>>(a, b0, nb, partial);
     const size_t n = size_t(nb) * Kp;
     blendWeightFinishKernel<<<unsigned(std::min<size_t>((n + kSkinThreads - 1) / kSkinThreads, 4096)), kSkinThreads, 0, stream>>>(
         partial, vBlocks, nb, Kp, a.gradWeights + size_t(b0) * Kp);
-    e = cudaGetLastError();
-  }
-  const cudaError_t f = cudaFreeAsync(partial, stream);
-  if (e == cudaSuccess) e = f;
-  return e;
+    return cudaGetLastError();
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -787,7 +784,6 @@ cudaError_t launchSkinWithBlendShapesBackward(const BlendSkinArgs& a, cudaStream
 // ------------------------------------------------------------------------------------------------
 constexpr int kNormalThreads = 256;
 constexpr int kNormalTile = 4;
-constexpr size_t kNormalScratchBudget = size_t(256) << 20; // h of a slice of instances
 
 template <bool kGrad>
 __global__ void __launch_bounds__(kNormalThreads) vertexNormalKernel(const NormalArgs a, int b0, int nb, float* h) {
@@ -884,21 +880,11 @@ cudaError_t launchVertexNormals(const NormalArgs& a, cudaStream_t stream) {
 }
 
 cudaError_t launchVertexNormalsBackward(const NormalArgs& a, cudaStream_t stream) {
-  const int B = a.batch;
-  if (B <= 0) return cudaSuccess;
-  const size_t perInstance = size_t(a.M.numVertices) * 3 * sizeof(float);
-  const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(B), kNormalScratchBudget / perInstance)));
-  float* h = nullptr;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&h), perInstance * slice, stream);
-  if (e != cudaSuccess) return e;
-  for (int b0 = 0; e == cudaSuccess && b0 < B; b0 += slice) {
-    const int nb = std::min(slice, B - b0);
-    e = launchNormalPass(vertexNormalKernel<true>, a, b0, nb, h, stream);
-    if (e == cudaSuccess) e = launchNormalPass(vertexNormalGradKernel, a, b0, nb, static_cast<const float*>(h), stream);
-  }
-  const cudaError_t f = cudaFreeAsync(h, stream);
-  if (e == cudaSuccess) e = f;
-  return e;
+  if (a.batch <= 0) return cudaSuccess;
+  return forEachInstanceSlice(a.batch, size_t(a.M.numVertices) * 3 * sizeof(float), stream, [&](float* h, int, int b0, int nb) {
+    const cudaError_t r = launchNormalPass(vertexNormalKernel<true>, a, b0, nb, h, stream);
+    return r != cudaSuccess ? r : launchNormalPass(vertexNormalGradKernel, a, b0, nb, static_cast<const float*>(h), stream);
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -913,7 +899,6 @@ cudaError_t launchVertexNormalsBackward(const NormalArgs& a, cudaStream_t stream
 // ------------------------------------------------------------------------------------------------
 constexpr int kRefitThreads = 256;
 constexpr int kClosestThreads = 128;
-constexpr size_t kTreeScratchBudget = size_t(256) << 20; // the boxes of a slice of instances
 
 __global__ void __launch_bounds__(kRefitThreads) meshTreeRefitKernel(const ClosestPointArgs a, int b0, int nb, float* boxes) {
   const MeshTreeTables T = a.T;
@@ -1013,30 +998,21 @@ __global__ void __launch_bounds__(kClosestThreads) closestPointKernel(const Clos
 }
 
 cudaError_t launchClosestPointsOnMesh(const ClosestPointArgs& a, cudaStream_t stream) {
-  const int B = a.batch;
-  if (B <= 0 || a.numPoints <= 0) return cudaSuccess;
-  const size_t perInstance = size_t(a.T.numNodes) * 6 * sizeof(float);
-  const int slice = int(std::max<size_t>(1, std::min<size_t>(size_t(B), kTreeScratchBudget / perInstance)));
-  int refitGrid = 0, queryGrid = 0;
-  cudaError_t e = persistentGrid(meshTreeRefitKernel, kRefitThreads, 0, slice, &refitGrid);
-  if (e == cudaSuccess)
-    e = persistentGrid(closestPointKernel, kClosestThreads, 0, (long(slice) * a.numPoints + kClosestThreads - 1) / kClosestThreads, &queryGrid);
-  if (e != cudaSuccess) return e;
-  float* boxes = nullptr;
-  e = cudaMallocAsync(reinterpret_cast<void**>(&boxes), perInstance * slice, stream);
-  if (e != cudaSuccess) return e;
-  for (int b0 = 0; e == cudaSuccess && b0 < B; b0 += slice) {
-    const int nb = std::min(slice, B - b0);
+  if (a.batch <= 0 || a.numPoints <= 0) return cudaSuccess;
+  return forEachInstanceSlice(a.batch, size_t(a.T.numNodes) * 6 * sizeof(float), stream, [&](float* boxes, int slice, int b0, int nb) {
+    // grids sized for a whole slice, capped by the work of this one
+    int refitGrid = 0, queryGrid = 0;
+    cudaError_t r = persistentGrid(meshTreeRefitKernel, kRefitThreads, 0, slice, &refitGrid);
+    if (r == cudaSuccess)
+      r = persistentGrid(closestPointKernel, kClosestThreads, 0, (long(slice) * a.numPoints + kClosestThreads - 1) / kClosestThreads, &queryGrid);
+    if (r != cudaSuccess) return r;
     meshTreeRefitKernel<<<std::min(refitGrid, nb), kRefitThreads, 0, stream>>>(a, b0, nb, boxes);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) break;
+    r = cudaGetLastError();
+    if (r != cudaSuccess) return r;
     const long blocks = (long(nb) * a.numPoints + kClosestThreads - 1) / kClosestThreads;
     closestPointKernel<<<int(std::min<long>(queryGrid, blocks)), kClosestThreads, 0, stream>>>(a, b0, nb, boxes);
-    e = cudaGetLastError();
-  }
-  const cudaError_t f = cudaFreeAsync(boxes, stream);
-  if (e == cudaSuccess) e = f;
-  return e;
+    return cudaGetLastError();
+  });
 }
 
 // ------------------------------------------------------------------------------------------------

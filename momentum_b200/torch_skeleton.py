@@ -19,16 +19,42 @@ _handles = {}
 
 
 def _device_character(character, device: torch.device) -> ms.DeviceCharacter:
-    """One DeviceCharacter per (character, device), kept for the life of the process like torch_ik's solver functions."""
+    """The handle every operation here runs on: a DeviceCharacter as given, or for a Character the one DeviceCharacter per (character,
+    device) holding ``character.skinning`` (with its ``faces``) and ``character.blend_shape``. When any of them is replaced, a new handle
+    is made instead of uploading into the old one: a graph recorded with the old skinning keeps its handle (``ctx.dc``) and its tables,
+    and no kernel in flight on another stream reads tables that are being replaced. An old handle is freed with the last graph that uses
+    it."""
     index = device.index if device.index is not None else torch.cuda.current_device()
     if isinstance(character, ms.DeviceCharacter):
         if character.device != index:
             raise ValueError(f"model parameters are on cuda:{index} but the device character lives on cuda:{character.device}")
         return character
     key = (id(character), index)
-    if key not in _handles:
-        _handles[key] = (character, ms.DeviceCharacter(character, index))  # the character is kept alive so that its id stays unique
-    return _handles[key][1]
+    entry = _handles.get(key)
+    faces = None if character.skinning is None else character.skinning.faces
+    if entry is None or entry[1] is not character.skinning or entry[2] is not character.blend_shape or entry[3] is not faces:
+        # the character is kept alive so that its id stays unique
+        entry = (character, character.skinning, character.blend_shape, faces, ms.DeviceCharacter(character, index))
+        _handles[key] = entry
+    return entry[4]
+
+
+def _resolve(character, need=None):
+    """(Character, skinning) of a ``Character`` (its attributes) or of a ``DeviceCharacter`` (what was uploaded to it). ``need`` "skinning"
+    raises without a skinning, "faces" without a skinning with mesh faces."""
+    is_handle = isinstance(character, ms.DeviceCharacter)
+    ch = character.character if is_handle else character
+    if not isinstance(ch, mc.Character):
+        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
+    sk = character.skinning
+    if need is not None and sk is None:
+        raise ValueError("the character has no skinning" + (", so no mesh faces" if need == "faces" else ""))
+    if need == "faces" and is_handle and character.faces is None:
+        rejected = character.faces_error
+        raise ValueError("the character has no mesh faces" + (f" (their upload was rejected: {rejected})" if rejected else ""))
+    if need == "faces" and not is_handle and sk.faces is None:
+        raise ValueError("the character has no mesh faces (character.skinning.faces)")
+    return ch, sk
 
 
 class _SkeletonState(torch.autograd.Function):
@@ -64,9 +90,7 @@ def model_parameters_to_skeleton_state(character, model_parameters: torch.Tensor
     tensor's device. Differentiable once with respect to ``model_parameters``."""
     if not torch.is_tensor(model_parameters) or not model_parameters.is_cuda:
         raise ValueError("model_parameters_to_skeleton_state runs on CUDA tensors (there is no CPU fallback)")
-    ch = character.character if isinstance(character, ms.DeviceCharacter) else character
-    if not isinstance(ch, mc.Character):
-        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
+    ch, _ = _resolve(character)
     if model_parameters.dim() not in (1, 2) or model_parameters.shape[-1] != ch.num_params:
         raise ValueError(f"model_parameters must be [n] or [B, n] with n = {ch.num_params}, got {tuple(model_parameters.shape)}")
     return _SkeletonState.apply(_device_character(character, model_parameters.device), model_parameters)
@@ -110,24 +134,6 @@ class _SkinPoints(torch.autograd.Function):
                 None if gr is None else gr.to(ctx.rest_dtype))
 
 
-_skin_handles = {}
-
-
-def _skinned_device_character(ch: mc.Character, device: torch.device) -> ms.DeviceCharacter:
-    """One DeviceCharacter per (character, device) holding ``ch.skinning`` (with its ``faces``) and ``ch.blend_shape``. When any of them is
-    replaced, a new handle is made instead of uploading into the old one: a graph recorded with the old skinning keeps its handle
-    (``ctx.dc``) and its tables, and no kernel in flight on another stream reads tables that are being replaced. An old handle is freed
-    with the last graph that uses it."""
-    index = device.index if device.index is not None else torch.cuda.current_device()
-    key = (id(ch), index)
-    entry = _skin_handles.get(key)
-    faces = None if ch.skinning is None else ch.skinning.faces
-    if entry is None or entry[1] is not ch.skinning or entry[2] is not ch.blend_shape or entry[3] is not faces:
-        entry = (ch, ch.skinning, ch.blend_shape, faces, ms.DeviceCharacter(ch, index))  # the character is kept alive so that its id stays unique
-        _skin_handles[key] = entry
-    return entry[4]
-
-
 def skin_points(character, skel_state: torch.Tensor, rest_points=None) -> torch.Tensor:
     """Linear-blend skinning (pymomentum ``Character.skin_points``): ``skel_state`` [J, 8] or [B, J, 8] (t, q xyzw, s; q is normalised)
     on a CUDA device -> points [V, 3] or [B, V, 3] in the input dtype, computed in float32. ``rest_points``: None = the rest mesh,
@@ -140,13 +146,7 @@ def skin_points(character, skel_state: torch.Tensor, rest_points=None) -> torch.
     handle raises."""
     if not torch.is_tensor(skel_state) or not skel_state.is_cuda:
         raise ValueError("skin_points runs on CUDA tensors (there is no CPU fallback)")
-    is_handle = isinstance(character, ms.DeviceCharacter)
-    ch = character.character if is_handle else character
-    if not isinstance(ch, mc.Character):
-        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
-    sk = character.skinning if is_handle else ch.skinning
-    if sk is None:
-        raise ValueError("the character has no skinning")
+    ch, sk = _resolve(character, "skinning")
     J, V = ch.num_joints, sk.num_vertices
     if skel_state.shape[-2:] == (4, 4):
         raise ValueError("skin_points takes skeleton states [.., J, 8] (t, q xyzw, s), not 4x4 matrices")
@@ -158,8 +158,7 @@ def skin_points(character, skel_state: torch.Tensor, rest_points=None) -> torch.
         B = skel_state.shape[0] if skel_state.dim() == 3 else None
         if not (rest_points.shape == (V, 3) or (B is not None and rest_points.shape == (B, V, 3))):
             raise ValueError(f"rest_points must be [V, 3] or [B, V, 3] with V = {V} and the skel_state's B, got {tuple(rest_points.shape)}")
-    dc = _device_character(character, skel_state.device) if is_handle else _skinned_device_character(ch, skel_state.device)
-    return _SkinPoints.apply(dc, skel_state, rest_points)
+    return _SkinPoints.apply(_device_character(character, skel_state.device), skel_state, rest_points)
 
 
 class _SkinWithBlendShapes(torch.autograd.Function):
@@ -214,16 +213,10 @@ def skin_with_blend_shapes(character, skel_state: torch.Tensor, blend_weights: t
     uploaded to it; the backward of a graph recorded before a later ``set_skinning`` or ``set_blend_shape`` on that handle raises."""
     if not torch.is_tensor(skel_state) or not skel_state.is_cuda:
         raise ValueError("skin_with_blend_shapes runs on CUDA tensors (there is no CPU fallback)")
-    is_handle = isinstance(character, ms.DeviceCharacter)
-    ch = character.character if is_handle else character
-    if not isinstance(ch, mc.Character):
-        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
-    sk = character.skinning if is_handle else ch.skinning
-    bs = character.blend_shape if is_handle else ch.blend_shape
-    if sk is None:
-        raise ValueError("the character has no skinning")
+    ch, sk = _resolve(character, "skinning")
+    bs = character.blend_shape
     if bs is None:
-        rejected = character.blend_shape_error if is_handle else None
+        rejected = character.blend_shape_error if isinstance(character, ms.DeviceCharacter) else None
         raise ValueError("the character has no blend shape" + (f" (its upload was rejected: {rejected})" if rejected else ""))
     if bs.num_vertices != sk.num_vertices:
         raise ValueError(f"the blend shape has {bs.num_vertices} vertices but the skinning has {sk.num_vertices}")
@@ -236,7 +229,7 @@ def skin_with_blend_shapes(character, skel_state: torch.Tensor, blend_weights: t
     K = blend_weights.shape[-1] if blend_weights.dim() in (1, 2) else 0
     if not (1 <= K <= bs.num_shapes and (blend_weights.dim() == 1 or (B is not None and blend_weights.shape[0] == B))):
         raise ValueError(f"blend_weights must be [K'] or [B, K'] with 1 <= K' <= {bs.num_shapes} and the skel_state's B, got {tuple(blend_weights.shape)}")
-    dc = _device_character(character, skel_state.device) if is_handle else _skinned_device_character(ch, skel_state.device)
+    dc = _device_character(character, skel_state.device)
     if dc.blend_shape is None:
         raise ValueError(f"the character's blend shape was rejected: {dc.blend_shape_error}")
     return _SkinWithBlendShapes.apply(dc, skel_state, blend_weights)
@@ -287,22 +280,11 @@ def compute_vertex_normals(character, vertex_positions: torch.Tensor) -> torch.T
     ``set_skinning`` on that handle raises."""
     if not torch.is_tensor(vertex_positions) or not vertex_positions.is_cuda:
         raise ValueError("compute_vertex_normals runs on CUDA tensors (there is no CPU fallback)")
-    is_handle = isinstance(character, ms.DeviceCharacter)
-    ch = character.character if is_handle else character
-    if not isinstance(ch, mc.Character):
-        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
-    sk = character.skinning if is_handle else ch.skinning
-    if sk is None:
-        raise ValueError("the character has no skinning, so no mesh faces")
-    if is_handle and character.faces is None:
-        rejected = character.faces_error
-        raise ValueError("the character has no mesh faces" + (f" (their upload was rejected: {rejected})" if rejected else ""))
-    if not is_handle and sk.faces is None:
-        raise ValueError("the character has no mesh faces (character.skinning.faces)")
+    _, sk = _resolve(character, "faces")
     V = sk.num_vertices
     if vertex_positions.dim() not in (2, 3) or vertex_positions.shape[-2:] != (V, 3):
         raise ValueError(f"vertex_positions must be [V, 3] or [B, V, 3] with V = {V}, got {tuple(vertex_positions.shape)}")
-    dc = _device_character(character, vertex_positions.device) if is_handle else _skinned_device_character(ch, vertex_positions.device)
+    dc = _device_character(character, vertex_positions.device)
     if dc.faces is None:
         raise ValueError(f"the character's mesh faces were rejected: {dc.faces_error}")
     return _VertexNormals.apply(dc, vertex_positions)
@@ -338,18 +320,7 @@ def find_closest_points_on_mesh(character, points_source: torch.Tensor, vertices
             raise ValueError(f"find_closest_points_on_mesh runs on CUDA tensors (there is no CPU fallback); {name} is not one")
     if points_source.device != vertices_target.device:
         raise ValueError("points_source and vertices_target must be on the same device")
-    is_handle = isinstance(character, ms.DeviceCharacter)
-    ch = character.character if is_handle else character
-    if not isinstance(ch, mc.Character):
-        raise ValueError("character must be a momentum_b200.character.Character or a DeviceCharacter")
-    sk = character.skinning if is_handle else ch.skinning
-    if sk is None:
-        raise ValueError("the character has no skinning, so no mesh faces")
-    if is_handle and character.faces is None:
-        rejected = character.faces_error
-        raise ValueError("the character has no mesh faces" + (f" (their upload was rejected: {rejected})" if rejected else ""))
-    if not is_handle and sk.faces is None:
-        raise ValueError("the character has no mesh faces (character.skinning.faces)")
+    _, sk = _resolve(character, "faces")
     V = sk.num_vertices
     if vertices_target.dim() not in (2, 3) or vertices_target.shape[-2:] != (V, 3):
         raise ValueError(f"vertices_target must be [V, 3] or [B, V, 3] with V = {V}, got {tuple(vertices_target.shape)}")
@@ -361,7 +332,7 @@ def find_closest_points_on_mesh(character, points_source: torch.Tensor, vertices
     if not max_dist >= 0.0:
         raise ValueError(f"max_dist must be >= 0 (float('inf') for no bound), got {max_dist}")
     dev = points_source.device
-    dc = _device_character(character, dev) if is_handle else _skinned_device_character(ch, dev)
+    dc = _device_character(character, dev)
     if dc.faces is None:
         raise ValueError(f"the character's mesh faces were rejected: {dc.faces_error}")
     if dc.faces.shape[0] == 0 or dc.mesh_tree_error is not None:

@@ -34,7 +34,7 @@ from momentum_b200 import torch_skeleton as tsk  # noqa: E402
 CASES = [("humanoid72", 1024, 16), ("humanoid72", 1024, 64), ("humanoid72", 4096, 16), ("humanoid72", 4096, 64), ("bodyhands300", 512, 64),
          ("humanoid72", 32, 64)]
 VERTICES_PER_JOINT = {"humanoid72": 139, "bodyhands300": 67}
-BUDGET = 256 << 20  # the launchers' per-slice scratch budget (kBlendRestBudget, kSkinPartialBudget)
+BUDGET = 256 << 20  # the launchers' per-slice scratch budget (kSliceScratchBudget)
 
 
 def card():
@@ -93,7 +93,7 @@ def main():
         G = torch.from_numpy(rng.normal(size=(B, V, 3)).astype(np.float32)).to(dev)
         base = torch.from_numpy(ch.blend_shape.base_shape).to(dev)
         S = torch.from_numpy(ch.blend_shape.shape_vectors).to(dev).reshape(K, V * 3)
-        dc = tsk._skinned_device_character(ch, dev)
+        dc = tsk._device_character(ch, dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
         pts = torch.empty(B, V, 3, device=dev)
         gst = torch.empty(B, J, 8, device=dev)

@@ -32,7 +32,7 @@ from momentum_b200 import torch_skeleton as tsk  # noqa: E402
 
 CASES = [("humanoid72", 1), ("humanoid72", 64), ("humanoid72", 1024), ("humanoid72", 4096), ("bodyhands300", 512), ("bodyhands300", 2048)]
 TUBES = {"humanoid72": (mc.humanoid72, 12, 12), "bodyhands300": (mc.bodyhands300, 8, 8)}
-BUDGET = 256 << 20  # the backward's per-slice scratch budget (kNormalScratchBudget)
+BUDGET = 256 << 20  # the backward's per-slice scratch budget (kSliceScratchBudget)
 BYTES_FORWARD, BYTES_BACKWARD = 24, 72  # per vertex-instance: positions + normals; positions, upstream, h written and read, gradient
 
 
