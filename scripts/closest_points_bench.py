@@ -14,12 +14,10 @@ repeated) with the tree built on the rest mesh and with a tree built by set_mesh
 in the same run. There is no CPU path for the timings: without a GPU they fail.
 """
 import argparse
-import ctypes
 import json
 import os
 import subprocess
 import sys
-import tempfile
 
 import numpy as np
 import torch
@@ -149,19 +147,10 @@ def brute_force(faces, x, p):
 
 def visits():
     """Nodes visited per query from the CPU emulator (tests/emu/emu_closest_points.cu), rest tree against pose tree."""
-    sys.path.insert(0, ROOT)
+    from tests import emu_lib
     from tests import test_closest_points_on_mesh as t
 
-    d = tempfile.mkdtemp()
-    lib = os.path.join(d, "libemu_closest_points.so")
-    csrc = os.path.join(ROOT, "momentum_b200", "csrc")
-    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-ffp-contract=off", "--fmad=false", "-shared", "-o", lib,
-                           os.path.join(ROOT, "tests", "emu", "emu_closest_points.cu"), os.path.join(csrc, "ik_plan.cpp"),
-                           os.path.join(csrc, "ik_chol_sched.cpp")])
-    L = ctypes.CDLL(lib)
-    L.emu_closest_points_last_error.restype = ctypes.c_char_p
-    L.emu_closest_points.argtypes = [ctypes.c_int32] * 2 + [ctypes.c_void_p] * 2 + [ctypes.c_int32] * 2 + [ctypes.c_void_p] * 2 + \
-        [ctypes.c_float, ctypes.c_int32] + [ctypes.c_void_p] * 4
+    L = emu_lib.load()
     print("| rig | queries | rest tree: mean / p99 nodes | pose tree: mean / p99 nodes | (CPU emulator) |")
     print("|---|---|---|---|---|")
     for name in TUBES:

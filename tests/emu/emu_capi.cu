@@ -20,6 +20,7 @@
 #include "../../momentum_b200/csrc/ik_device.cuh"
 #include "../../momentum_b200/csrc/ik_plan.h"
 #include "../../momentum_b200/csrc/ik_solve_path.h"
+#include "emu_error.h"
 
 using namespace mb2;
 
@@ -570,6 +571,9 @@ int mb2_solver_get_solve_path(mb2_solver* s, int64_t out[15]) {
 }
 
 } // extern "C"
+
+// the message of the last emu_* entry of the other emulators (emu_*.cu) that failed on this thread
+extern "C" const char* emu_last_error(void) { return g_emuErr.c_str(); }
 
 // schedule / Gram-plan figures of the solver plan (cholesky_mode 3 with strips): out = {levels, tiles, tile columns, nPad, device
 // columns, strips, pairs, misaligned tile starts, odd pair lists, cells outside their strip}

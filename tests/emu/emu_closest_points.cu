@@ -1,5 +1,5 @@
-// TEST HARNESS ONLY — CPU lane-emulation of the closest-point kernels (mb2_character_closest_points_on_mesh_device), built by
-// tests/test_closest_points_on_mesh.py into a temporary directory together with ik_plan.cpp / ik_chol_sched.cpp.
+// TEST HARNESS ONLY — CPU lane-emulation of the closest-point kernels (mb2_character_closest_points_on_mesh_device), part of
+// tests/emu/libmb2_emu.so.
 //
 // The face tables and the tree are made by the library's own makeMeshFaces / makeMeshTree; the __host__ __device__ building blocks of
 // ik_device.cuh then run in the kernels' order: boxGrow / boxUnion level by level from the deepest (meshTreeRefitKernel), and per query
@@ -10,26 +10,22 @@
 #include <algorithm>
 #include <climits>
 #include <cstdint>
-#include <string>
 #include <vector>
 
 #include "../../include/momentum_b200.h"
 #include "../../momentum_b200/csrc/ik_device.cuh"
 #include "../../momentum_b200/csrc/ik_plan.h"
+#include "emu_error.h"
 
 using namespace mb2;
-
-static thread_local std::string g_err;
-
-extern "C" const char* emu_closest_points_last_error(void) { return g_err.c_str(); }
 
 namespace {
 enum Mode { kTraverse = 0, kScan = 1, kPruneOnEqual = 2, kDropLastLeafFace = 3 };
 
 int make(int32_t V, int32_t F, const int32_t* faces, const float* ref, HostMeshFaces& m, HostMeshTree& t) {
-  g_err = makeMeshFaces(V, F, faces, m);
-  if (g_err.empty()) g_err = makeMeshTree(m, V, ref, t);
-  return g_err.empty() ? MB2_OK : MB2_ERR_INVALID_ARGUMENT;
+  g_emuErr = makeMeshFaces(V, F, faces, m);
+  if (g_emuErr.empty()) g_emuErr = makeMeshTree(m, V, ref, t);
+  return g_emuErr.empty() ? MB2_OK : MB2_ERR_INVALID_ARGUMENT;
 }
 
 // meshTreeRefitKernel for one instance: boxes [numNodes][6]
@@ -114,9 +110,9 @@ extern "C" int emu_mesh_tree(int32_t V, int32_t F, const int32_t* faces, int32_t
                              int32_t* nodeCount, int32_t* leafFaces, int32_t* levelStart) {
   HostMeshFaces m;
   HostMeshTree t;
-  g_err = makeMeshFaces(V, F, faces, m);
-  if (g_err.empty()) g_err = makeMeshTree(m, Vt, ref, t);
-  if (!g_err.empty()) return MB2_ERR_INVALID_ARGUMENT;
+  g_emuErr = makeMeshFaces(V, F, faces, m);
+  if (g_emuErr.empty()) g_emuErr = makeMeshTree(m, Vt, ref, t);
+  if (!g_emuErr.empty()) return MB2_ERR_INVALID_ARGUMENT;
   sizes[0] = t.numNodes;
   sizes[1] = t.depth;
   std::copy(t.nodeStart.begin(), t.nodeStart.end(), nodeStart);

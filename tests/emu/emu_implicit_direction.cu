@@ -1,5 +1,5 @@
-// TEST HARNESS ONLY — CPU lane-emulation of implicitDirectionKernel (mb2_solver_function_implicit_direction_device), built by
-// tests/test_implicit_direction.py into a temporary directory.
+// TEST HARNESS ONLY — CPU lane-emulation of implicitDirectionKernel (mb2_solver_function_implicit_direction_device), part of
+// tests/emu/libmb2_emu.so.
 //
 // The __host__ __device__ building blocks of ik_jacobi.cuh run pass by pass in the kernel's order, the lanes of each pass in sequence,
 // on any rows x n_E float32 matrix. It also reports the sweeps the Jacobi iteration used. It is not part of the product library and

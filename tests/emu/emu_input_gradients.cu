@@ -1,23 +1,19 @@
-// TEST HARNESS ONLY — CPU lane-emulation of inputGradientKernel (mb2_solver_function_input_gradients_device), built by
-// tests/test_solve_ik_input_gradients.py into a temporary directory together with ik_plan.cpp / ik_chol_sched.cpp.
+// TEST HARNESS ONLY — CPU lane-emulation of inputGradientKernel (mb2_solver_function_input_gradients_device), part of
+// tests/emu/libmb2_emu.so.
 //
 // The character is made by the library's own makeCharacter and the block by the library's own error-function constructors and planner
 // (the units the kernel reads); the kernel's own pass functions of ik_device.cuh (fkPasses, tangentPasses) then run with HostLanes, the
 // lanes of each pass in sequence. It is not part of the product library and nothing in momentum_b200/ loads it.
 #include <cmath>
 #include <cstdint>
-#include <string>
 #include <vector>
 
 #include "../../include/momentum_b200.h"
 #include "../../momentum_b200/csrc/ik_device.cuh"
 #include "../../momentum_b200/csrc/ik_plan.h"
+#include "emu_error.h"
 
 using namespace mb2;
-
-static thread_local std::string g_err;
-
-extern "C" const char* emu_input_gradients_last_error(void) { return g_err.c_str(); }
 
 // character arrays as mb2_character_create takes them; one block: kind 0 Position / 1 Orientation (matrix difference), shared offsets
 // [nc][3|4] or (instanced) none; records [B][targetSize] as mb2_set_targets takes them, constraint weights [B][nc], enabled [n];
@@ -28,21 +24,21 @@ extern "C" int emu_input_gradients(int32_t numJoints, const int32_t* parents, co
                                    const uint8_t* enabled, int32_t batch, const float* records, const float* cweights, const float* theta,
                                    const float* direction, float* gradWeights, float* gradOffsets, float* gradTargets) {
   HostCharacter h;
-  g_err = makeCharacter(numJoints, parents, offsets, prerot, numParams, outer, inner, vals, ptOffsets, h);
-  if (!g_err.empty()) return MB2_ERR_INVALID_ARGUMENT;
+  g_emuErr = makeCharacter(numJoints, parents, offsets, prerot, numParams, outer, inner, vals, ptOffsets, h);
+  if (!g_emuErr.empty()) return MB2_ERR_INVALID_ARGUMENT;
   std::vector<float> ones(size_t(nc), 1.f);
   HostErrorFunction ef;
-  if (kind == 0) g_err = instanced ? instancedPositionErrorFunction(h, weight, 2.f, lossC, nc, cparents, ones.data(), ef)
+  if (kind == 0) g_emuErr = instanced ? instancedPositionErrorFunction(h, weight, 2.f, lossC, nc, cparents, ones.data(), ef)
                                    : positionErrorFunction(h, weight, 2.f, lossC, nc, cparents, coffsets, ones.data(), ef);
-  else g_err = instanced ? instancedOrientationErrorFunction(h, weight, 2.f, lossC, 0, nc, cparents, ones.data(), ef)
+  else g_emuErr = instanced ? instancedOrientationErrorFunction(h, weight, 2.f, lossC, 0, nc, cparents, ones.data(), ef)
                          : orientationErrorFunction(h, weight, 2.f, lossC, 0, nc, cparents, coffsets, ones.data(), ef);
-  if (!g_err.empty()) return MB2_ERR_INVALID_ARGUMENT;
+  if (!g_emuErr.empty()) return MB2_ERR_INVALID_ARGUMENT;
   HostFunction hf;
   hf.enabled.assign(enabled, enabled + numParams);
   hf.add(ef, nullptr);
   Plan plan;
-  g_err = buildPlan(h, hf.efs, hf.enabled, false, plan);
-  if (!g_err.empty()) return MB2_ERR_INVALID_ARGUMENT;
+  g_emuErr = buildPlan(h, hf.efs, hf.enabled, false, plan);
+  if (!g_emuErr.empty()) return MB2_ERR_INVALID_ARGUMENT;
   const int stride = hf.targetStride, per = kind == 0 ? 3 : 4;
   std::vector<float> rec(records, records + size_t(batch) * stride);
   if (kind == 1) // what the upload does (launchNormalizeQuats): every quaternion of the record normalised

@@ -1,31 +1,27 @@
-// TEST HARNESS ONLY — CPU lane-emulation of skeletonStateKernel<true> (mb2_character_skeleton_state_backward_device), built by
-// tests/test_skeleton_state.py into a temporary directory together with ik_plan.cpp / ik_chol_sched.cpp.
+// TEST HARNESS ONLY — CPU lane-emulation of skeletonStateKernel<true> (mb2_character_skeleton_state_backward_device), part of
+// tests/emu/libmb2_emu.so.
 //
 // The character is made by the library's own makeCharacter, which builds the tables the kernel walks (levels, children in CSR, the
 // ParameterTransform in CSC); the kernel's own pass functions of ik_device.cuh (fkPasses, skelGradPasses) then run with HostLanes, the
 // lanes of each pass in sequence. It is not part of the product library and nothing in momentum_b200/ loads it.
 #include <cstdint>
-#include <string>
 #include <vector>
 
 #include "../../include/momentum_b200.h"
 #include "../../momentum_b200/csrc/ik_device.cuh"
 #include "../../momentum_b200/csrc/ik_plan.h"
+#include "emu_error.h"
 
 using namespace mb2;
-
-static thread_local std::string g_err;
-
-extern "C" const char* emu_skeleton_state_last_error(void) { return g_err.c_str(); }
 
 // character arrays as mb2_character_create takes them; theta [B][n], grad_state [B][J][8] -> grad_theta [B][n] (host memory)
 extern "C" int emu_skeleton_state_backward(int32_t numJoints, const int32_t* parents, const float* offsets, const float* prerot, int32_t numParams,
                                            const int32_t* outer, const int32_t* inner, const float* vals, const float* ptOffsets, int32_t batch,
                                            const float* theta, const float* gradState, float* gradTheta) {
   HostCharacter h;
-  g_err = makeCharacter(numJoints, parents, offsets, prerot, numParams, outer, inner, vals, ptOffsets, h);
-  if (!g_err.empty()) return MB2_ERR_INVALID_ARGUMENT;
-  if (batch < 0 || (batch > 0 && !(theta && gradState && gradTheta))) { g_err = "null argument"; return MB2_ERR_INVALID_ARGUMENT; }
+  g_emuErr = makeCharacter(numJoints, parents, offsets, prerot, numParams, outer, inner, vals, ptOffsets, h);
+  if (!g_emuErr.empty()) return MB2_ERR_INVALID_ARGUMENT;
+  if (batch < 0 || (batch > 0 && !(theta && gradState && gradTheta))) { g_emuErr = "null argument"; return MB2_ERR_INVALID_ARGUMENT; }
   const CharacterTables C = hostCharacterTables(h);
   const SkeletonTables S{h.childStart.data(), h.children.data(), h.ptColStart.data(), h.ptColRows.data(), h.ptColVals.data()};
   const int J = C.numJoints, n = C.numParams;

@@ -1,5 +1,5 @@
-// TEST HARNESS ONLY — CPU lane-emulation of the vertex-normal kernels (mb2_character_vertex_normals*_device), built by
-// tests/test_vertex_normals.py into a temporary directory together with ik_plan.cpp / ik_chol_sched.cpp.
+// TEST HARNESS ONLY — CPU lane-emulation of the vertex-normal kernels (mb2_character_vertex_normals*_device), part of
+// tests/emu/libmb2_emu.so.
 //
 // The face tables are made by the library's own makeMeshFaces; the __host__ __device__ building blocks of ik_device.cuh then run in the
 // kernels' order for each vertex: its corner list in order with faceNormal, then normalizeClamped (vertexNormalKernel); for the backward
@@ -8,23 +8,19 @@
 // of the product library and nothing in momentum_b200/ loads it.
 #include <algorithm>
 #include <cstdint>
-#include <string>
 #include <vector>
 
 #include "../../include/momentum_b200.h"
 #include "../../momentum_b200/csrc/ik_device.cuh"
 #include "../../momentum_b200/csrc/ik_plan.h"
+#include "emu_error.h"
 
 using namespace mb2;
 
-static thread_local std::string g_err;
-
-extern "C" const char* emu_vertex_normals_last_error(void) { return g_err.c_str(); }
-
 namespace {
 int make(int32_t V, int32_t F, const int32_t* faces, HostMeshFaces& m) {
-  g_err = makeMeshFaces(V, F, faces, m);
-  return g_err.empty() ? MB2_OK : MB2_ERR_INVALID_ARGUMENT;
+  g_emuErr = makeMeshFaces(V, F, faces, m);
+  return g_emuErr.empty() ? MB2_OK : MB2_ERR_INVALID_ARGUMENT;
 }
 
 // n_v of one instance, over the vertex's corner list in order

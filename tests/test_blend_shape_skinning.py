@@ -11,8 +11,6 @@ and on an H100; x is the float64 shaped rest point:
 """
 import ctypes
 import copy
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -20,10 +18,9 @@ import torch
 
 from momentum_b200 import character as mc
 from momentum_b200 import solver as ms
+from tests import emu_lib
 from tests import test_skinning as tsn
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU_DIR = os.path.join(ROOT, "tests", "emu")
 EPS32 = 2.0 ** -24
 
 # worst measured ratios over these fixtures and three seeds, on the emulator / on an H100 80GB HBM3 at a 700 W power limit: forward
@@ -186,19 +183,8 @@ def test_synthetic_blend_shape():
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    lib = str(tmp_path_factory.mktemp("emu_blend_skinning") / "libemu_blend_skinning.so")
-    csrc = os.path.join(ROOT, "momentum_b200", "csrc")
-    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-ffp-contract=off", "--fmad=false", "-shared", "-o", lib,
-                           os.path.join(EMU_DIR, "emu_blend_skinning.cu"), os.path.join(csrc, "ik_plan.cpp"), os.path.join(csrc, "ik_chol_sched.cpp")])
-    L = ctypes.CDLL(lib)
-    L.emu_blend_skinning_last_error.restype = ctypes.c_char_p
-    head = ([ctypes.c_int32] + [ctypes.c_void_p] * 3 + [ctypes.c_int32] + [ctypes.c_void_p] * 4 + [ctypes.c_int32] + [ctypes.c_void_p] * 4
-            + [ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p])
-    L.emu_skin_with_blend_shapes.argtypes = head + [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p]
-    L.emu_skin_with_blend_shapes_backward.argtypes = head + [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32] + [ctypes.c_void_p] * 3
-    L.emu_blend_shape_replace.argtypes = ([ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p] * 2) + [ctypes.c_void_p]
-    return L
+def emu():
+    return emu_lib.load()
 
 
 def _head(ch, keep, base=None, vectors=None, K=None):
@@ -225,7 +211,7 @@ def _emu_backward(L, ch, st, w, G):
     gw = np.full(w.shape, np.nan, np.float32)
     rc = L.emu_skin_with_blend_shapes_backward(*_head(ch, keep), st.shape[0], st.ctypes.data, w.ctypes.data, w.shape[1], G.ctypes.data,
                                                gs.ctypes.data, gw.ctypes.data)
-    assert rc == 0, L.emu_blend_skinning_last_error().decode()
+    assert rc == 0, L.emu_last_error().decode()
     return gs, gw
 
 
@@ -237,7 +223,7 @@ def test_emulated_forward_and_backward_meet_the_bounds(emu, name):
     w = _weights(B, Kp, 13)
     G = tsn._upstream(ch, B, 12)
     rc, p = _emu_forward(emu, ch, st, w)
-    assert rc == 0, emu.emu_blend_skinning_last_error().decode()
+    assert rc == 0, emu.emu_last_error().decode()
     gs, gw = _emu_backward(emu, ch, st, w, G)
     _check(_ratios(ch, st, w, G, p, gs, gw), name)
 
@@ -272,17 +258,17 @@ def test_rejected_blend_shapes(emu):
     for kw, msg in cases:
         rc, _ = _emu_forward(emu, ch, st, w, **kw)
         assert rc == 1, kw  # MB2_ERR_INVALID_ARGUMENT
-        assert msg in emu.emu_blend_skinning_last_error().decode(), (msg, emu.emu_blend_skinning_last_error())
+        assert msg in emu.emu_last_error().decode(), (msg, emu.emu_last_error())
     for Kp in (0, 5):
         rc, _ = _emu_forward(emu, ch, st, np.zeros((1, Kp), np.float32))
-        assert rc == 1 and "num_weights" in emu.emu_blend_skinning_last_error().decode(), Kp
+        assert rc == 1 and "num_weights" in emu.emu_last_error().decode(), Kp
     # a null array with a positive count, and a rejected blend shape leaves the earlier one in place
     base, vec = np.ascontiguousarray(bs.base_shape), np.ascontiguousarray(bs.shape_vectors)
     k_after = ctypes.c_int32(-1)
     for b2, v2, msg in ((None, vec, "null"), (base, None, "null"), (nan_base, vec, "finite")):
         rc = emu.emu_blend_shape_replace(4, 1, base.ctypes.data, vec.ctypes.data, 2, 1, None if b2 is None else np.ascontiguousarray(b2).ctypes.data,
                                          None if v2 is None else v2.ctypes.data, ctypes.byref(k_after))
-        assert rc == 1 and msg in emu.emu_blend_skinning_last_error().decode() and k_after.value == 4, (msg, k_after.value)
+        assert rc == 1 and msg in emu.emu_last_error().decode() and k_after.value == 4, (msg, k_after.value)
     rc = emu.emu_blend_shape_replace(4, 1, base.ctypes.data, vec.ctypes.data, 2, 1, base.ctypes.data, vec.ctypes.data, ctypes.byref(k_after))
     assert rc == 0 and k_after.value == 2
 

@@ -13,9 +13,6 @@ The self-checks show that these reject a projection without the edge regions, th
 and (through the tree-independence check) a leaf that skips its last face and a prune on >=.
 """
 import copy
-import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -23,9 +20,9 @@ import torch
 
 from momentum_b200 import character as mc
 from momentum_b200 import solver as ms
+from tests import emu_lib
+from tests.test_vertex_normals import _tube
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU_DIR = os.path.join(ROOT, "tests", "emu")
 EPS32 = 2.0 ** -24
 LEAF_FACES, TREE_STACK = 4, 32  # kLeafFaces, kTreeStack (ik_types.h)
 
@@ -36,16 +33,6 @@ K_B = 10.0
 
 
 # ---- fixtures ----------------------------------------------------------------------------------------------------------------------
-def _tube(make, rings, segments, seed, name, far=False):
-    ch = make()
-    if far:  # the root, and with it the mesh, 100 units out
-        ch.offsets = ch.offsets.copy()
-        ch.offsets[0] += np.float32(100.0)
-    ch.skinning = mc.synthetic_tube_mesh(ch, rings, segments, seed)
-    ch.name = name
-    return ch
-
-
 def _edge_mesh():
     """A single triangle; an isolated vertex; a zero-area face on exactly collinear points; a face that repeats an index; a small fan.
     Positions on a 1/64 grid."""
@@ -292,18 +279,8 @@ def test_numpy_reference_agrees_with_an_independent_minimisation():
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    lib = str(tmp_path_factory.mktemp("emu_closest_points") / "libemu_closest_points.so")
-    csrc = os.path.join(ROOT, "momentum_b200", "csrc")
-    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-ffp-contract=off", "--fmad=false", "-shared", "-o", lib,
-                           os.path.join(EMU_DIR, "emu_closest_points.cu"), os.path.join(csrc, "ik_plan.cpp"), os.path.join(csrc, "ik_chol_sched.cpp")])
-    L = ctypes.CDLL(lib)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int32
-    L.emu_closest_points_last_error.restype = ctypes.c_char_p
-    L.emu_mesh_tree.argtypes = [i32, i32, vp, i32, vp, vp, vp, vp, vp, vp]
-    L.emu_mesh_tree_boxes.argtypes = [i32, i32, vp, vp, vp, vp]
-    L.emu_closest_points.argtypes = [i32, i32, vp, vp, i32, i32, vp, vp, ctypes.c_float, i32, vp, vp, vp, vp]
-    return L
+def emu():
+    return emu_lib.load()
 
 
 def _c(a, dt):
@@ -316,7 +293,7 @@ def _emu_tree(L, faces, ref):
     sizes = np.zeros(2, np.int32)
     ns, nc, lf, ls = np.full(2 * F, -7, np.int32), np.full(2 * F, -7, np.int32), np.full(F, -7, np.int32), np.full(TREE_STACK + 1, -7, np.int32)
     rc = L.emu_mesh_tree(V, F, faces.ctypes.data, V, ref.ctypes.data, sizes.ctypes.data, ns.ctypes.data, nc.ctypes.data, lf.ctypes.data, ls.ctypes.data)
-    assert rc == 0, L.emu_closest_points_last_error()
+    assert rc == 0, L.emu_last_error()
     n, depth = int(sizes[0]), int(sizes[1])
     return n, depth, ns[:n], nc[:n], lf, ls[:depth + 1]
 
@@ -329,7 +306,7 @@ def _emu_run(L, faces, ref, x, p, max_dist=np.inf, mode=0, visits=False):
     vis = np.zeros((B, N), np.int32)
     rc = L.emu_closest_points(V, faces.shape[0], faces.ctypes.data, ref.ctypes.data, B, N, x.ctypes.data, p.ctypes.data, float(max_dist), mode,
                               q.ctypes.data, face.ctypes.data, bary.ctypes.data, vis.ctypes.data if visits else None)
-    assert rc == 0, L.emu_closest_points_last_error()
+    assert rc == 0, L.emu_last_error()
     return (q, face, bary, vis) if visits else (q, face, bary)
 
 
@@ -393,7 +370,7 @@ def test_mesh_tree_is_rejected_with_a_message(emu):
     inf = x.copy(); inf[0, 0] = np.inf
     for args, msg in (((3, 0, None, 3, x), "no faces"), ((3, 1, faces, 4, np.zeros((4, 3), np.float32)), "differs"), ((3, 1, faces, 3, None), "null"),
                       ((3, 1, faces, 3, nan), "not finite"), ((3, 1, faces, 3, inf), "not finite")):
-        assert call(*args) == 1 and msg in emu.emu_closest_points_last_error().decode(), (msg, emu.emu_closest_points_last_error())
+        assert call(*args) == 1 and msg in emu.emu_last_error().decode(), (msg, emu.emu_last_error())
     assert call(3, 1, faces, 3, x) == 0  # all vertices equal: a degenerate but valid reference
 
 

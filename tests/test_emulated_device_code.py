@@ -3,24 +3,20 @@
 Validates, without a GPU: the planner (units / cells / chain-rule contributions / gating), the
 per-lane FK + residual + Jacobian code, the Eigen-structured blocked Cholesky phases and the batched
 solve loop — i.e. everything in momentum_b200/csrc that is not CUDA launch glue."""
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 from momentum_b200 import character as mc
 from momentum_b200 import solver as ms
 from momentum_b200.problems import chain_problem, chain22_problem, humanoid_problem
+from tests import emu_lib
 from tests import parity
-
-EMU_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu")
-EMU_LIB = os.path.join(EMU_DIR, "libmb2_emu.so")
+from tests.emu_lib import EMU_LIB
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _build_emu():
-    subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
+    emu_lib.build()
 
 
 FAMS = [("position",), ("orientation",), ("state",), ("limit",), ("position", "orientation", "state", "limit"), ("plane",), ("halfplane",),

@@ -7,10 +7,6 @@ J v. Every fixture keeps its s^2 at least 1e-3 tau away from the truncation thre
 accident; one fixture sits there on purpose. The CPU emulator (tests/emu/emu_implicit_direction.cu) runs the kernel's building blocks on
 the oracle's float32 Jacobian, the GPU tests run the kernel through the C-ABI.
 """
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 import torch
@@ -18,9 +14,8 @@ import torch
 from momentum_b200 import character as mc
 from momentum_b200 import solver as ms
 from momentum_b200.problems import add_test_limits, bodyhands_problem, chain_problem, humanoid_problem
+from tests import emu_lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU_DIR = os.path.join(ROOT, "tests", "emu")
 TAU = 1e-5
 MAX_SWEEPS = 32  # kJacobiMaxSweeps (ik_jacobi.cuh)
 
@@ -94,14 +89,8 @@ def _oracle_jacobian(ch, efs, enabled, theta_b, b, rows):
 
 # ---- CPU: the emulator ----------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    """tests/emu/emu_implicit_direction.cu compiled like the other emulators (no FMA contraction) into a temporary directory."""
-    lib = str(tmp_path_factory.mktemp("emu_implicit_direction") / "libemu_implicit_direction.so")
-    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-ffp-contract=off", "--fmad=false", "-shared", "-o", lib,
-                           os.path.join(EMU_DIR, "emu_implicit_direction.cu")])
-    L = ctypes.CDLL(lib)
-    L.emu_implicit_direction.argtypes = [ctypes.c_int32, ctypes.c_int32] + [ctypes.c_void_p] * 7
-    return L
+def emu():
+    return emu_lib.load()
 
 
 def _emu(L, JE, r, g):

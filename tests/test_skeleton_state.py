@@ -6,19 +6,14 @@ g passes when ||g - g64||_inf <= K * max(||g64||_inf, 1) per instance. K is pinn
 the fixtures below (emulator and H100); the self-checks show that the bound rejects a backward that drops the quaternion term or swaps
 two rotation DOFs.
 """
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
 from momentum_b200 import character as mc
 from momentum_b200 import solver as ms
+from tests import emu_lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU_DIR = os.path.join(ROOT, "tests", "emu")
 
 # worst measured ||g - g64||_inf / max(||g64||_inf, 1) over these fixtures and seeds: 1.64e-6 on the emulator, 1.77e-6 on an
 # H100 80GB HBM3 at a 700 W power limit (humanoid72 both times); the quaternion-term and swapped-DOF errors below are >= 5e-3
@@ -150,29 +145,17 @@ def _bound_ratio(g, g64):
 
 # ---- CPU: the emulator runs the device functions lane by lane ------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    """tests/emu/emu_skeleton_state.cu with the library's host code, compiled like the other emulator (no FMA contraction) into a
-    temporary directory."""
-    lib = str(tmp_path_factory.mktemp("emu_skeleton_state") / "libemu_skeleton_state.so")
-    csrc = os.path.join(ROOT, "momentum_b200", "csrc")
-    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-ffp-contract=off", "--fmad=false", "-shared", "-o", lib,
-                           os.path.join(EMU_DIR, "emu_skeleton_state.cu"), os.path.join(csrc, "ik_plan.cpp"), os.path.join(csrc, "ik_chol_sched.cpp")])
-    L = ctypes.CDLL(lib)
-    L.emu_skeleton_state_last_error.restype = ctypes.c_char_p
-    L.emu_skeleton_state_backward.argtypes = [ctypes.c_int32] + [ctypes.c_void_p] * 3 + [ctypes.c_int32] + [ctypes.c_void_p] * 4 + [ctypes.c_int32] + [ctypes.c_void_p] * 3
-    return L
+def emu():
+    return emu_lib.load()
 
 
 def _emu_backward(L, ch, theta, G):
-    arrays = [np.ascontiguousarray(ch.parents, np.int32), np.ascontiguousarray(ch.offsets, np.float32), np.ascontiguousarray(ch.prerot, np.float32),
-              np.ascontiguousarray(ch.pt_outer, np.int32), np.ascontiguousarray(ch.pt_inner, np.int32), np.ascontiguousarray(ch.pt_vals, np.float32),
-              np.ascontiguousarray(ch.pt_offsets, np.float32)]
-    pa, of, pr, ou, inn, va, po = (a.ctypes.data for a in arrays)
+    keep = []
     theta = np.ascontiguousarray(theta, np.float32)
     G = np.ascontiguousarray(G, np.float32)
     out = np.full(theta.shape, np.nan, np.float32)
-    rc = L.emu_skeleton_state_backward(ch.num_joints, pa, of, pr, ch.num_params, ou, inn, va, po, theta.shape[0], theta.ctypes.data, G.ctypes.data, out.ctypes.data)
-    assert rc == 0, L.emu_skeleton_state_last_error().decode()
+    rc = L.emu_skeleton_state_backward(*emu_lib.character_args(ch, keep), theta.shape[0], theta.ctypes.data, G.ctypes.data, out.ctypes.data)
+    assert rc == 0, L.emu_last_error().decode()
     return out
 
 

@@ -10,8 +10,6 @@ The self-checks show that each bound rejects a skinning that drops the inverse-b
 backward without the normalisation Jacobian, and E_j accumulated in the uncentred form on the fixture 100 units from the origin.
 """
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,9 +17,8 @@ import torch
 
 from momentum_b200 import character as mc
 from momentum_b200 import solver as ms
+from tests import emu_lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU_DIR = os.path.join(ROOT, "tests", "emu")
 EPS32 = 2.0 ** -24
 
 # worst measured ratios over these fixtures, three seeds and the three rest-point layouts, on the emulator / on an H100 80GB HBM3 at a
@@ -205,33 +202,19 @@ def _rest_ratio(g, g64):
 
 # ---- CPU: the emulator runs the device functions pass by pass -----------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    lib = str(tmp_path_factory.mktemp("emu_skinning") / "libemu_skinning.so")
-    csrc = os.path.join(ROOT, "momentum_b200", "csrc")
-    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-ffp-contract=off", "--fmad=false", "-shared", "-o", lib,
-                           os.path.join(EMU_DIR, "emu_skinning.cu"), os.path.join(csrc, "ik_plan.cpp"), os.path.join(csrc, "ik_chol_sched.cpp")])
-    L = ctypes.CDLL(lib)
-    L.emu_skinning_last_error.restype = ctypes.c_char_p
-    head = [ctypes.c_int32] + [ctypes.c_void_p] * 3 + [ctypes.c_int32] + [ctypes.c_void_p] * 4 + [ctypes.c_int32] + [ctypes.c_void_p] * 4
-    L.emu_skinning_tables.argtypes = head + [ctypes.c_void_p] * 2
-    L.emu_skin_points.argtypes = head + [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p]
-    L.emu_skin_points_backward.argtypes = head + [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32] + [ctypes.c_void_p] * 3
-    return L
+def emu():
+    return emu_lib.load()
 
 
 def _head(ch, keep, rest=None, index=None, weight=None, ibp=None):
     sk = ch.skinning
-    arrays = [np.ascontiguousarray(ch.parents, np.int32), np.ascontiguousarray(ch.offsets, np.float32), np.ascontiguousarray(ch.prerot, np.float32),
-              np.ascontiguousarray(ch.pt_outer, np.int32), np.ascontiguousarray(ch.pt_inner, np.int32), np.ascontiguousarray(ch.pt_vals, np.float32),
-              np.ascontiguousarray(ch.pt_offsets, np.float32),
-              np.ascontiguousarray(sk.rest_vertices if rest is None else rest, np.float32),
+    arrays = [np.ascontiguousarray(sk.rest_vertices if rest is None else rest, np.float32),
               np.ascontiguousarray(sk.skin_index if index is None else index, np.int32),
               np.ascontiguousarray(sk.skin_weight if weight is None else weight, np.float32),
               np.ascontiguousarray(sk.inverse_bind_pose if ibp is None else ibp, np.float32)]
     keep.extend(arrays)
-    p = [a.ctypes.data for a in arrays]
-    V = arrays[7].shape[0] if arrays[7].ndim == 2 else 0
-    return [ch.num_joints] + p[:3] + [ch.num_params] + p[3:7] + [V] + p[7:]
+    V = arrays[0].shape[0] if arrays[0].ndim == 2 else 0
+    return emu_lib.character_args(ch, keep) + [V] + [a.ctypes.data for a in arrays]
 
 
 def _ptr(a):
@@ -244,7 +227,7 @@ def _emu_forward(L, ch, st, rest=None, batched=False):
     out = np.full((st.shape[0], ch.skinning.num_vertices, 3), np.nan, np.float32)
     rest = None if rest is None else np.ascontiguousarray(rest, np.float32)
     rc = L.emu_skin_points(*_head(ch, keep), st.shape[0], st.ctypes.data, _ptr(rest), int(batched), out.ctypes.data)
-    assert rc == 0, L.emu_skinning_last_error().decode()
+    assert rc == 0, L.emu_last_error().decode()
     return out
 
 
@@ -255,7 +238,7 @@ def _emu_backward(L, ch, st, rest, batched, G, want_rest=True):
     gr = np.full(np.shape(rest), np.nan, np.float32) if (rest is not None and want_rest) else None
     rest = None if rest is None else np.ascontiguousarray(rest, np.float32)
     rc = L.emu_skin_points_backward(*_head(ch, keep), st.shape[0], st.ctypes.data, _ptr(rest), int(batched), G.ctypes.data, gs.ctypes.data, _ptr(gr))
-    assert rc == 0, L.emu_skinning_last_error().decode()
+    assert rc == 0, L.emu_last_error().decode()
     return gs, gr
 
 
@@ -328,7 +311,7 @@ def test_rejected_skinning_inputs(emu):
     def rc_msg(**kw):
         keep = []
         rc = emu.emu_skin_points(*_head(ch, keep, **kw), 1, st.ctypes.data, None, 0, out.ctypes.data)
-        return rc, emu.emu_skinning_last_error().decode()
+        return rc, emu.emu_last_error().decode()
 
     bad_idx = sk.skin_index.copy(); bad_idx[1, 0] = ch.num_joints
     neg_idx = sk.skin_index.copy(); neg_idx[0, 0] = -1

@@ -6,20 +6,15 @@ normalised values the device stores). The reference is checked first: its J v ag
 gradients against central differences. A float32 result g passes when ||g - g64||_inf <= K * max(||g64||_inf, 1) per instance, the
 outputs of one instance taken together. The self-checks show that the bound rejects the four errors a closed form most easily makes.
 """
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
 from momentum_b200 import character as mc
 from momentum_b200 import solver as ms
+from tests import emu_lib
 from tests.test_skeleton_state import FIXTURES, _fk64, _pt_dense, _qmul, _qrot
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU_DIR = os.path.join(ROOT, "tests", "emu")
 
 # worst measured ||g - g64||_inf / max(||g64||_inf, 1) over the fixtures below: 1.36e-5 on the emulator (humanoid72) and 1.84e-5 on an
 # H100 80GB HBM3 at a 400 W power limit (bodyhands300), both Position blocks; pinned about four times above. The errors of the self-check
@@ -219,35 +214,21 @@ def test_closed_form_is_the_reference_and_the_bound_rejects_its_likely_errors():
 
 # ---- CPU: the emulator runs the device functions lane by lane ------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    """tests/emu/emu_input_gradients.cu with the library's host code, compiled like the other emulators (no FMA contraction) into a
-    temporary directory."""
-    lib = str(tmp_path_factory.mktemp("emu_input_gradients") / "libemu_input_gradients.so")
-    csrc = os.path.join(ROOT, "momentum_b200", "csrc")
-    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-ffp-contract=off", "--fmad=false", "-shared", "-o", lib,
-                           os.path.join(EMU_DIR, "emu_input_gradients.cu"), os.path.join(csrc, "ik_plan.cpp"), os.path.join(csrc, "ik_chol_sched.cpp")])
-    L = ctypes.CDLL(lib)
-    L.emu_input_gradients_last_error.restype = ctypes.c_char_p
-    vp = ctypes.c_void_p
-    L.emu_input_gradients.argtypes = ([ctypes.c_int32, vp, vp, vp, ctypes.c_int32, vp, vp, vp, vp, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, vp, vp,
-                                       ctypes.c_float, ctypes.c_float, vp, ctypes.c_int32] + [vp] * 7)
-    return L
+def emu():
+    return emu_lib.load()
 
 
 def _emu(L, ch, P):
-    keep = [np.ascontiguousarray(ch.parents, np.int32), np.ascontiguousarray(ch.offsets, np.float32), np.ascontiguousarray(ch.prerot, np.float32),
-            np.ascontiguousarray(ch.pt_outer, np.int32), np.ascontiguousarray(ch.pt_inner, np.int32), np.ascontiguousarray(ch.pt_vals, np.float32),
-            np.ascontiguousarray(ch.pt_offsets, np.float32)]
+    keep = []
     B, nc, k = P["off"].shape
     arrs = dict(cp=np.ascontiguousarray(P["parents"], np.int32), co=np.ascontiguousarray(P["off"][0], np.float32),
                 en=np.ascontiguousarray(P["enabled"], np.uint8), rec=_records(P), cw=np.ascontiguousarray(P["cw"], np.float32),
                 th=np.ascontiguousarray(P["theta"], np.float32), v=np.ascontiguousarray(P["v"], np.float32))
     out = [np.full((B, nc), np.nan, np.float32), np.full((B, nc, k), np.nan, np.float32), np.full((B, nc, k), np.nan, np.float32)]
-    a = [x.ctypes.data for x in keep]
-    rc = L.emu_input_gradients(ch.num_joints, a[0], a[1], a[2], ch.num_params, a[3], a[4], a[5], a[6], P["kind"], int(P["instanced"]), nc,
+    rc = L.emu_input_gradients(*emu_lib.character_args(ch, keep), P["kind"], int(P["instanced"]), nc,
                                arrs["cp"].ctypes.data, arrs["co"].ctypes.data, P["ew"], P["c"], arrs["en"].ctypes.data, B, arrs["rec"].ctypes.data,
                                arrs["cw"].ctypes.data, arrs["th"].ctypes.data, arrs["v"].ctypes.data, *(o.ctypes.data for o in out))
-    assert rc == 0, L.emu_input_gradients_last_error().decode()
+    assert rc == 0, L.emu_last_error().decode()
     return out
 
 

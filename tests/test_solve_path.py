@@ -4,24 +4,21 @@ for the CPU emulator, and mb2_solver_get_solve_path reports it.
 CPU: the emulator evaluates the choice for every row of PATHS (planning only, no solve) with the limits of an H100 SXM, and runs the
 chosen path. GPU: the library reports the same record as the emulator given the device's own limits, and refuses with the same message.
 The runtime refusal "Gram + Cholesky fusion: no resident CTA" (the occupancy query finds no resident CTA) is not reached by any fixture."""
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 from momentum_b200 import solver as ms
 from momentum_b200.problems import bodyhands_problem, humanoid_problem
+from tests import emu_lib
 from tests import f64ref as R
+from tests.emu_lib import EMU_LIB
 
-EMU_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu")
-EMU_LIB = os.path.join(EMU_DIR, "libmb2_emu.so")
 H100_SXM = (132, 227 * 1024, 228 * 1024)  # SMs, opt-in shared memory per block, shared memory per SM
 
 
 @pytest.fixture(scope="module")
 def emu():
-    subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
+    emu_lib.build()
     return ms.load_library(EMU_LIB)
 
 

@@ -9,8 +9,6 @@ GPU part (-m gpu): every fixture and every launch variant of the sweep (warps pe
 spread, several waves) through get_jacobian, get_jacobian_device, get_error, get_skeleton_state and one solver step; each case asserts
 the variant it reached from get_sweep_launch, and test_zz_report_sweep_bounds prints the worst k per variant and per family."""
 import dataclasses
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -18,10 +16,8 @@ import pytest
 from momentum_b200 import character as mc
 from momentum_b200 import solver as ms
 from momentum_b200.problems import chain_problem, humanoid_problem, random_unit_quats, small_rotation_quats
+from tests import emu_lib
 from tests import f64ref as R
-
-EMU_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu")
-EMU_LIB = os.path.join(EMU_DIR, "libmb2_emu.so")
 
 
 @dataclasses.dataclass
@@ -304,8 +300,7 @@ def oracle32_ratios(fx, refs):
 # ------------------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu():
-    subprocess.check_call(["make", "-C", EMU_DIR, "-s"])
-    return EMU_LIB
+    return emu_lib.build()
 
 
 _CPU_NAMES = [f.name for f in fixtures()]

@@ -11,9 +11,6 @@ The self-checks show that the bounds reject averaged unit face normals, a droppe
 projection and swapped next / previous corners.
 """
 import copy
-import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -21,9 +18,8 @@ import torch
 
 from momentum_b200 import character as mc
 from momentum_b200 import solver as ms
+from tests import emu_lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMU_DIR = os.path.join(ROOT, "tests", "emu")
 EPS32 = 2.0 ** -24
 
 # worst measured ratios over these fixtures and several seeds, on the emulator / on an H100 80GB HBM3 at a 700 W power limit: forward
@@ -244,17 +240,8 @@ def test_tube_mesh_generator():
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    lib = str(tmp_path_factory.mktemp("emu_vertex_normals") / "libemu_vertex_normals.so")
-    csrc = os.path.join(ROOT, "momentum_b200", "csrc")
-    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-ffp-contract=off", "--fmad=false", "-shared", "-o", lib,
-                           os.path.join(EMU_DIR, "emu_vertex_normals.cu"), os.path.join(csrc, "ik_plan.cpp"), os.path.join(csrc, "ik_chol_sched.cpp")])
-    L = ctypes.CDLL(lib)
-    L.emu_vertex_normals_last_error.restype = ctypes.c_char_p
-    L.emu_mesh_faces_tables.argtypes = [ctypes.c_int32, ctypes.c_int32] + [ctypes.c_void_p] * 3
-    L.emu_vertex_normals.argtypes = [ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]
-    L.emu_vertex_normals_backward.argtypes = [ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32] + [ctypes.c_void_p] * 3
-    return L
+def emu():
+    return emu_lib.load()
 
 
 def _emu_run(L, faces, x, G):
@@ -294,7 +281,7 @@ def test_mesh_faces_are_rejected_with_a_message(emu):
              (3, 1, np.array([(0, -1, 2)], np.int32), "outside"))
     for V, F, f, msg in cases:
         rc = emu.emu_mesh_faces_tables(V, F, None if f is None else f.ctypes.data, start.ctypes.data, corner.ctypes.data)
-        assert rc == 1 and msg in emu.emu_vertex_normals_last_error().decode(), (V, F, msg, emu.emu_vertex_normals_last_error())
+        assert rc == 1 and msg in emu.emu_last_error().decode(), (V, F, msg, emu.emu_last_error())
     # degenerate faces, repeated indices and no faces at all are accepted
     for V, F, f in ((3, 1, np.array([(1, 1, 1)], np.int32)), (3, 0, None)):
         assert emu.emu_mesh_faces_tables(V, F, None if f is None else f.ctypes.data, start.ctypes.data, corner.ctypes.data) == 0
