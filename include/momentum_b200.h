@@ -358,6 +358,23 @@ int mb2_character_closest_points_on_mesh_device(const mb2_character* c, int32_t 
                                                 const float* points_device, float max_dist, float* out_points_device, int32_t* out_face_device,
                                                 float* out_bary_device, void* cuda_stream);
 
+/* The closest target point of each query point (pymomentum find_closest_points, tensor_kd_tree.cpp / axel::SimdKdTree): for instance b
+ * and query p = source[b][n], over the targets t_j = target[b or 0][j] (j = 0 .. M-1), the j with the smallest (d2_j, j),
+ * d2_j = fmaf(dx, dx, fmaf(dy, dy, dz * dz)) with d = t_j - p, among the candidates: finite t_j with a finite d2_j <= max_dist * max_dist
+ * (in float; max_dist may be +inf) and, when normals are given, dot(n_p, n_j) >= max_normal_dot (an fmaf chain; NaN fails). Writes
+ * out_index [B][N] = j, out_points [B][N][3] = t_j and, with normals, out_normals [B][N][3] = n_j, copied bit for bit; without a
+ * candidate (a non-finite query included) -1 and zeros. Points and normals are [B][N][3] / [B or 1][M][3] float32 device memory on
+ * `device`; target_batched == 0 shares one target over the batch. The two normal arrays are both null (the plain variant) or both set
+ * (with num_target == 0 the target arrays are not read and may be null), and out_normals is set exactly when normals are given. The result is a linear scan's, whatever the tree: each call builds, per target instance
+ * and on `cuda_stream` with no host round trip, a tree over the target sorted by Morton code, in stream-ordered scratch of at most
+ * 256 MiB per slice of instances. Asynchronous; batch == 0 or num_source == 0 is a no-op, num_target == 0 gives every query -1. A
+ * negative device or size, a NaN or negative max_dist, a NaN max_normal_dot, a null or mismatched pointer or memory that is not device
+ * memory on `device` is MB2_ERR_INVALID_ARGUMENT. No atomics: an instance gets the same bits alone as in any batch. */
+int mb2_closest_points_device(int device, int32_t batch, int32_t num_source, int32_t num_target, int32_t target_batched,
+                              const float* source_device, const float* source_normals_device, const float* target_device,
+                              const float* target_normals_device, float max_dist, float max_normal_dot, float* out_points_device,
+                              float* out_normals_device, int32_t* out_index_device, void* cuda_stream);
+
 /* Input contraction of the implicit-function backward of solve_ik (diff_ik d_gradient_d_input_dot): for block `index` and every
  * instance b, the derivatives of grad_theta E_index(theta_b) . v_b with respect to the block's inputs, at the targets, constraint weights
  * and offsets the handle currently holds:

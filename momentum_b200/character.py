@@ -629,6 +629,34 @@ def synthetic_tube_mesh(ch: Character, rings: int, segments: int, seed: int = 0)
                     ibp.astype(np.float32), np.concatenate(faces).astype(np.int32))
 
 
+def synthetic_scan(ch: Character, num_points: int, theta=None, noise: Optional[float] = None, seed: int = 0):
+    """A seeded scan-like point cloud of ``ch``'s mesh (``ch.skinning``, e.g. a ``synthetic_tube_mesh``) posed at model parameters
+    ``theta`` (default zero): ``num_points`` samples, uniform by area over the posed faces, each moved along its face's unit normal by a
+    uniform offset in [-noise, noise] (default 1 % of the mean bone length). Returns (points, normals) float32 [num_points, 3], the normals
+    those of the sampled faces."""
+    sk = ch.skinning
+    if sk is None or sk.faces is None or len(sk.faces) == 0:
+        raise ValueError("synthetic_scan needs a skinned character with mesh faces")
+    rng = np.random.default_rng(seed)
+    th = np.zeros((1, ch.num_params)) if theta is None else np.asarray(theta, np.float64).reshape(1, ch.num_params)
+    t, q, s = forward_kinematics(ch, th)
+    x = skin_points(ch, np.concatenate([t, q, s[..., None]], -1))[0]
+    if noise is None:
+        t0, _, _ = forward_kinematics(ch, np.zeros((1, ch.num_params)))
+        p = np.asarray(ch.parents)
+        d = np.linalg.norm(t0[0][p >= 0] - t0[0][p[p >= 0]], axis=-1)
+        noise = 0.01 * float(d[d > 0].mean()) if np.any(d > 0) else 0.0
+    f = np.asarray(sk.faces, np.int64)
+    n = np.cross(x[f[:, 1]] - x[f[:, 0]], x[f[:, 2]] - x[f[:, 0]])
+    area = np.linalg.norm(n, axis=-1)
+    fi = rng.choice(len(f), size=num_points, p=area / area.sum())
+    r1, r2 = np.sqrt(rng.uniform(size=num_points)), rng.uniform(size=num_points)
+    w = np.stack([1.0 - r1, r1 * (1.0 - r2), r1 * r2], -1)  # uniform over each triangle
+    nf = n[fi] / np.maximum(area[fi], 1e-300)[:, None]
+    pts = np.einsum("nk,nkc->nc", w, x[f[fi]]) + rng.uniform(-noise, noise, (num_points, 1)) * nf
+    return pts.astype(np.float32), nf.astype(np.float32)
+
+
 def vertex_normals(faces, positions):
     """Area-weighted vertex normals in float64 (pymomentum compute_vertex_normals, tensor_skinning.cpp:354-383): per vertex the sum of
     (x1 - x0) x (x2 - x0) over every corner of every face that is that vertex, faces ascending and corners in order, then

@@ -1234,6 +1234,47 @@ int mb2_character_closest_points_on_mesh_device(const mb2_character* c, int32_t 
   return MB2_OK;
 }
 
+int mb2_closest_points_device(int device, int32_t batch, int32_t num_source, int32_t num_target, int32_t target_batched,
+                              const float* source_device, const float* source_normals_device, const float* target_device,
+                              const float* target_normals_device, float max_dist, float max_normal_dot, float* out_points_device,
+                              float* out_normals_device, int32_t* out_index_device, void* cuda_stream) {
+  MB2_CHECK(device >= 0, "closest points on cloud: device must not be negative");
+  MB2_CHECK(batch >= 0 && num_source >= 0 && num_target >= 0, "closest points on cloud: batch, num_source and num_target must not be negative");
+  MB2_CHECK(max_dist >= 0.f, "closest points on cloud: max_dist must be >= 0 and not NaN (+inf for no bound)");
+  MB2_CHECK(max_normal_dot == max_normal_dot, "closest points on cloud: max_normal_dot must not be NaN");
+  const bool normals = source_normals_device != nullptr;
+  MB2_CHECK(num_target == 0 || normals == (target_normals_device != nullptr), // with no target, neither target array is read
+            "closest points on cloud: source_normals and target_normals must be both null or both set");
+  MB2_CHECK(normals == (out_normals_device != nullptr), "closest points on cloud: out_normals must be set exactly when normals are given");
+  if (batch == 0 || num_source == 0) return MB2_OK;
+  MB2_CHECK(source_device != nullptr && out_points_device != nullptr && out_index_device != nullptr && (num_target == 0 || target_device != nullptr),
+            "closest points on cloud: null argument");
+  MB2_DEVICE_GUARD(device);
+  int rc = requireDevice(device);
+  if (rc != MB2_OK) return rc;
+  MB2_CHECK(onDevice(device, {source_device, out_points_device, out_index_device},
+                     {source_normals_device, out_normals_device, num_target > 0 ? target_device : nullptr,
+                      num_target > 0 ? target_normals_device : nullptr}),
+            "closest points on cloud: every array must be device memory on the given device");
+  NvtxRange range("closestPointsOnCloud");
+  ClosestCloudArgs a{};
+  a.batch = batch;
+  a.numSource = num_source;
+  a.numTarget = num_target;
+  a.targetBatched = target_batched != 0;
+  a.maxDist2 = max_dist * max_dist;
+  a.maxNormalDot = max_normal_dot;
+  a.source = source_device;
+  a.sourceNormals = source_normals_device;
+  a.target = target_device;
+  a.targetNormals = target_normals_device;
+  a.outPoints = out_points_device;
+  a.outNormals = out_normals_device;
+  a.outIndex = out_index_device;
+  MB2_CUDA(launchClosestPointsOnCloud(a, (cudaStream_t)cuda_stream));
+  return MB2_OK;
+}
+
 int mb2_character_vertex_normals_backward_device(const mb2_character* c, int32_t batch, const float* positions_device, const float* grad_normals_device,
                                                  float* grad_positions_device, void* cuda_stream) {
   NormalArgs a;

@@ -1118,4 +1118,48 @@ MB2_HD void boxUnion(float* box, const float* l, const float* r) {
   }
 }
 
+// ---- Closest point of a point cloud (pymomentum find_closest_points over axel::SimdKdTree) ---------------------------------------
+// d^2 = |t - p|^2 as an explicit fmaf chain, so that the device and the CPU emulator give the same bits with or without contraction;
+// NaN when t is not finite, so that such a target is never a candidate (closerFace).
+MB2_HD float pointDistance2(F3 p, F3 t) {
+  const float dx = t.x - p.x, dy = t.y - p.y, dz = t.z - p.z;
+  const float d2 = fmaf(dx, dx, fmaf(dy, dy, dz * dz));
+  return finite3(t) ? d2 : NAN;
+}
+// The normal variant's filter: dot(n_p, n_t) >= maxNormalDot, the dot an explicit fmaf chain; a NaN dot never passes.
+MB2_HD bool normalCompatible(F3 np, F3 nt, float maxNormalDot) { return fmaf(np.x, nt.x, fmaf(np.y, nt.y, np.z * nt.z)) >= maxNormalDot; }
+
+// A box with no point on some axis (lo > hi: a padding leaf, or a leaf whose points all have a NaN there) holds no finite point.
+MB2_HD bool boxVoid(const float* box) { return !(box[0] <= box[3] && box[1] <= box[4] && box[2] <= box[5]); }
+
+// 10 bits of v spread to every third bit
+MB2_HD uint32_t mortonSpread(uint32_t v) {
+  v = (v | (v << 16)) & 0x030000FFu;
+  v = (v | (v << 8)) & 0x0300F00Fu;
+  v = (v | (v << 4)) & 0x030C30C3u;
+  v = (v | (v << 2)) & 0x09249249u;
+  return v;
+}
+// The 30-bit Morton code of x quantised to 1024 cells per axis of its instance's bounds [lo xyz, hi xyz] over the finite points: an
+// axis of zero (or non-finite) extent gives 0 there; a point with a non-finite coordinate gets kMortonNonFinite, which sorts last.
+MB2_HD uint32_t mortonCode(F3 x, const float* bounds) {
+  if (!finite3(x)) return kMortonNonFinite;
+  uint32_t c = 0;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float lo = bounds[k], ext = bounds[3 + k] - lo;
+    const float s = (comp(x, k) - lo) / ext * 1024.f; // NaN or not >= 1 when ext is 0 or not finite
+    const uint32_t q = ext > 0.f && s >= 1.f ? uint32_t(fminf(s, 1023.f)) : 0u;
+    c |= mortonSpread(q) << (2 - k);
+  }
+  return c;
+}
+// The implicit tree over m sorted points: the number of real leaves and P, the leaves padded to a power of two (P = 1 for m <= kLeafPoints)
+MB2_HD int cloudLeaves(int m) { return (m + kLeafPoints - 1) / kLeafPoints; }
+MB2_HD int cloudPadded(int m) {
+  int P = 1;
+  while (P < cloudLeaves(m)) P *= 2;
+  return P;
+}
+
 } // namespace mb2

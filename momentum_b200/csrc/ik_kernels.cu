@@ -352,9 +352,9 @@ cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaS
   return launchInstanceGroups(backward ? reverse : forward, a, skeletonStateSmemPerInstance(a.T, backward), skeletonStateTableBytes(a, backward), stream);
 }
 
-// The per-instance scratch of the skinning, blend-shape and normals backward passes and of the closest-point refit: at most
-// kSliceScratchBudget bytes at once, the instances run in slices that fit (at least one instance each). No instance's result depends on
-// the slice it falls in.
+// The per-instance scratch of the skinning, blend-shape and normals backward passes, of the closest-point refit and of the point-cloud
+// tree build: at most kSliceScratchBudget bytes at once, the instances run in slices that fit (at least one instance each). No
+// instance's result depends on the slice it falls in.
 constexpr size_t kSliceScratchBudget = size_t(256) << 20;
 
 namespace {
@@ -1012,6 +1012,430 @@ cudaError_t launchClosestPointsOnMesh(const ClosestPointArgs& a, cudaStream_t st
     const long blocks = (long(nb) * a.numPoints + kClosestThreads - 1) / kClosestThreads;
     closestPointKernel<<<int(std::min<long>(queryGrid, blocks)), kClosestThreads, 0, stream>>>(a, b0, nb, boxes);
     return cudaGetLastError();
+  });
+}
+
+// ------------------------------------------------------------------------------------------------
+// Closest points of a point cloud (ik_device.cuh pointDistance2 / normalCompatible / mortonCode / closerFace / boxLowerBound /
+// pruneBox / box*). Per call, each target instance of a slice gets a tree built in scratch (CloudScratch), all on the call's stream:
+//   cloudBoundsKernel        (instance, tile of kSortTile points): the box of the tile's finite points
+//   cloudBoundsReduceKernel  one CTA per instance: the union of its tile boxes (min / max is exact: the order does not matter)
+//   cloudCodeKernel          thread per point: (mortonCode, index)
+//   kSortPasses x            a stable segmented LSD radix sort of (code, index), kSortBits per pass:
+//     cloudSortCountKernel     (instance, tile): the tile's digit counts
+//     cloudSortScanKernel      one CTA per instance: per digit the exclusive scan over the tiles, and each digit's start
+//     cloudSortScatterKernel   (instance, tile): each point to start[d] + scan[tile][d] + its rank among the tile's points with digit d
+//   cloudGatherKernel        thread per point: the sorted copy of the points (and normals)
+//   cloudBoxKernel           groups of up to 256 nodes of one level: their boxes (the leaves' from the sorted points), then up to 8
+//                            levels above them in shared memory; launched from the leaves up until the root is written
+// then closestCloudKernel runs one thread per (instance, query), depth first as closestPointKernel. Ranks within a tile come from
+// __match_any_sync and per-warp counts in shared memory: no atomics anywhere, so an instance gets the same bits alone as in any batch.
+// ------------------------------------------------------------------------------------------------
+constexpr int kCloudThreads = 256;
+constexpr int kSortDigits = 1 << kSortBits;
+constexpr int kSortGroups = kSortTile / 32; // warp-sized groups of a tile, in point order
+static_assert(kSortDigits == kCloudThreads && kSortTile % kCloudThreads == 0, "a thread per digit, whole rounds per tile");
+
+// The per-instance scratch of a tree over M points, each array [slice][its count]
+struct CloudScratch {
+  int M, tiles, P;
+  float* tileBox;     // [tiles][6]
+  float* bounds;      // [6]
+  uint32_t* keys[2];  // [M]
+  int32_t* index[2];  // [M]
+  int32_t* tileScan;  // [tiles][kSortDigits]
+  int32_t* digitStart; // [kSortDigits]
+  float* sorted;      // [M][3]
+  float* sortedNormals; // [M][3], when there are normals
+  float* boxes;       // [2P - 1][6]
+  size_t floats(bool normals) const { // per instance, in 4-byte words
+    return size_t(tiles) * 6 + 6 + 4 * size_t(M) + size_t(tiles) * kSortDigits + kSortDigits + (normals ? 6 : 3) * size_t(M) +
+           (2 * size_t(P) - 1) * 6;
+  }
+  void carve(float* base, int slice, bool normals) {
+    float* p = base;
+    auto take = [&](size_t n) { float* r = p; p += n * slice; return r; };
+    tileBox = take(size_t(tiles) * 6);
+    bounds = take(6);
+    keys[0] = reinterpret_cast<uint32_t*>(take(M));
+    keys[1] = reinterpret_cast<uint32_t*>(take(M));
+    index[0] = reinterpret_cast<int32_t*>(take(M));
+    index[1] = reinterpret_cast<int32_t*>(take(M));
+    tileScan = reinterpret_cast<int32_t*>(take(size_t(tiles) * kSortDigits));
+    digitStart = reinterpret_cast<int32_t*>(take(kSortDigits));
+    sorted = take(size_t(M) * 3);
+    sortedNormals = normals ? take(size_t(M) * 3) : nullptr;
+    boxes = take((2 * size_t(P) - 1) * 6);
+  }
+};
+
+// The instance's box over its finite points, tile by tile; tb0: the first target instance of the slice
+__global__ void __launch_bounds__(kCloudThreads) cloudBoundsKernel(const ClosestCloudArgs a, int tb0, int nt, CloudScratch S) {
+  __shared__ float red[6][kCloudThreads];
+  const int M = S.M;
+  for (long w = blockIdx.x; w < long(nt) * S.tiles; w += gridDim.x) {
+    const int i = int(w / S.tiles), tile = int(w % S.tiles);
+    const float* x = a.target + size_t(tb0 + i) * M * 3;
+    float box[6];
+    boxEmpty(box);
+    for (int e = tile * kSortTile + threadIdx.x; e < min(M, (tile + 1) * kSortTile); e += kCloudThreads) {
+      const F3 p = ld3(x + 3 * size_t(e));
+      if (finite3(p)) boxGrow(box, p);
+    }
+#pragma unroll
+    for (int k = 0; k < 6; ++k) red[k][threadIdx.x] = box[k];
+    __syncthreads();
+    for (int s = kCloudThreads / 2; s > 0; s >>= 1) {
+      if (threadIdx.x < s)
+        for (int k = 0; k < 6; ++k)
+          red[k][threadIdx.x] = k < 3 ? fminf(red[k][threadIdx.x], red[k][threadIdx.x + s]) : fmaxf(red[k][threadIdx.x], red[k][threadIdx.x + s]);
+      __syncthreads();
+    }
+    if (threadIdx.x < 6) S.tileBox[(size_t(i) * S.tiles + tile) * 6 + threadIdx.x] = red[threadIdx.x][0];
+    __syncthreads(); // red is reused by the next tile
+  }
+}
+
+__global__ void __launch_bounds__(kCloudThreads) cloudBoundsReduceKernel(int nt, CloudScratch S) {
+  __shared__ float red[6][kCloudThreads];
+  for (int i = blockIdx.x; i < nt; i += gridDim.x) {
+    float box[6];
+    boxEmpty(box);
+    for (int t = threadIdx.x; t < S.tiles; t += kCloudThreads) {
+      const float* b = S.tileBox + (size_t(i) * S.tiles + t) * 6;
+      boxUnion(box, box, b);
+    }
+#pragma unroll
+    for (int k = 0; k < 6; ++k) red[k][threadIdx.x] = box[k];
+    __syncthreads();
+    for (int s = kCloudThreads / 2; s > 0; s >>= 1) {
+      if (threadIdx.x < s)
+        for (int k = 0; k < 6; ++k)
+          red[k][threadIdx.x] = k < 3 ? fminf(red[k][threadIdx.x], red[k][threadIdx.x + s]) : fmaxf(red[k][threadIdx.x], red[k][threadIdx.x + s]);
+      __syncthreads();
+    }
+    if (threadIdx.x < 6) S.bounds[size_t(i) * 6 + threadIdx.x] = red[threadIdx.x][0];
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(kCloudThreads) cloudCodeKernel(const ClosestCloudArgs a, int tb0, int nt, CloudScratch S) {
+  const long M = S.M;
+  for (long it = long(blockIdx.x) * kCloudThreads + threadIdx.x; it < nt * M; it += long(gridDim.x) * kCloudThreads) {
+    const int i = int(it / M);
+    const int m = int(it % M);
+    S.keys[0][size_t(i) * M + m] = mortonCode(ld3(a.target + (size_t(tb0 + i) * M + m) * 3), S.bounds + size_t(i) * 6);
+    S.index[0][size_t(i) * M + m] = m;
+  }
+}
+
+// The digit of each of the thread's kSortTile / kCloudThreads points of `tile` (point r * 256 + threadIdx.x of the tile in round r;
+// kSortDigits for a point past M) and its rank among the tile's points with that digit, in point order. On return cnt[g][d] holds
+// the number of points with digit d in the groups before g of the tile and total[d] the tile's count; the caller syncs before reuse.
+__device__ __forceinline__ void cloudTileRanks(const uint32_t* keys, int M, int tile, int shift, uint16_t (*cnt)[kSortDigits], int* total,
+                                               int* digit, int* rank) {
+  constexpr int kRounds = kSortTile / kCloudThreads;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int g = 0; g < kSortGroups; ++g) cnt[g][threadIdx.x] = 0;
+  __syncthreads();
+#pragma unroll
+  for (int r = 0; r < kRounds; ++r) {
+    const int e = tile * kSortTile + r * kCloudThreads + threadIdx.x;
+    const int d = e < M ? int((keys[e] >> shift) & (kSortDigits - 1)) : kSortDigits;
+    const unsigned same = __match_any_sync(0xffffffffu, d);
+    digit[r] = d;
+    rank[r] = __popc(same & ((1u << lane) - 1));
+    if (d < kSortDigits && lane == __ffs(same) - 1) cnt[r * (kCloudThreads / 32) + warp][d] = uint16_t(__popc(same));
+  }
+  __syncthreads();
+  int run = 0; // thread = digit: the exclusive scan over the groups, in place
+  for (int g = 0; g < kSortGroups; ++g) {
+    const int c = cnt[g][threadIdx.x];
+    cnt[g][threadIdx.x] = uint16_t(run);
+    run += c;
+  }
+  total[threadIdx.x] = run;
+  __syncthreads();
+#pragma unroll
+  for (int r = 0; r < kRounds; ++r)
+    if (digit[r] < kSortDigits) rank[r] += cnt[r * (kCloudThreads / 32) + warp][digit[r]];
+}
+
+__global__ void __launch_bounds__(kCloudThreads) cloudSortCountKernel(int nt, CloudScratch S, int src, int shift) {
+  __shared__ uint16_t cnt[kSortGroups][kSortDigits];
+  __shared__ int total[kSortDigits];
+  constexpr int kRounds = kSortTile / kCloudThreads;
+  int digit[kRounds], rank[kRounds];
+  for (long w = blockIdx.x; w < long(nt) * S.tiles; w += gridDim.x) {
+    const int i = int(w / S.tiles), tile = int(w % S.tiles);
+    cloudTileRanks((src ? S.keys[1] : S.keys[0]) + size_t(i) * S.M, S.M, tile, shift, cnt, total, digit, rank);
+    S.tileScan[(size_t(i) * S.tiles + tile) * kSortDigits + threadIdx.x] = total[threadIdx.x];
+    __syncthreads();
+  }
+}
+
+// thread = digit: tileScan becomes the exclusive scan over the tiles, digitStart the exclusive scan of the digits' totals
+__global__ void __launch_bounds__(kCloudThreads) cloudSortScanKernel(int nt, CloudScratch S) {
+  __shared__ int tot[kSortDigits];
+  for (int i = blockIdx.x; i < nt; i += gridDim.x) {
+    int* h = S.tileScan + size_t(i) * S.tiles * kSortDigits + threadIdx.x;
+    int run = 0;
+    for (int t = 0; t < S.tiles; ++t) {
+      const int c = h[size_t(t) * kSortDigits];
+      h[size_t(t) * kSortDigits] = run;
+      run += c;
+    }
+    tot[threadIdx.x] = run;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int s = 0;
+      for (int d = 0; d < kSortDigits; ++d) {
+        const int c = tot[d];
+        tot[d] = s;
+        s += c;
+      }
+    }
+    __syncthreads();
+    S.digitStart[size_t(i) * kSortDigits + threadIdx.x] = tot[threadIdx.x];
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(kCloudThreads) cloudSortScatterKernel(int nt, CloudScratch S, int src, int shift) {
+  __shared__ uint16_t cnt[kSortGroups][kSortDigits];
+  __shared__ int total[kSortDigits];
+  __shared__ int start[kSortDigits];
+  constexpr int kRounds = kSortTile / kCloudThreads;
+  int digit[kRounds], rank[kRounds];
+  const size_t M = S.M;
+  for (long w = blockIdx.x; w < long(nt) * S.tiles; w += gridDim.x) {
+    const int i = int(w / S.tiles), tile = int(w % S.tiles);
+    // src selects by value: an indexed parameter array would go through local memory
+    const uint32_t* kin = (src ? S.keys[1] : S.keys[0]) + i * M;
+    const int32_t* xin = (src ? S.index[1] : S.index[0]) + i * M;
+    uint32_t* kout = (src ? S.keys[0] : S.keys[1]) + i * M;
+    int32_t* xout = (src ? S.index[0] : S.index[1]) + i * M;
+    cloudTileRanks(kin, S.M, tile, shift, cnt, total, digit, rank);
+    start[threadIdx.x] = S.digitStart[size_t(i) * kSortDigits + threadIdx.x] + S.tileScan[(size_t(i) * S.tiles + tile) * kSortDigits + threadIdx.x];
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < kRounds; ++r) {
+      if (digit[r] == kSortDigits) continue;
+      const int e = tile * kSortTile + r * kCloudThreads + threadIdx.x;
+      const int o = start[digit[r]] + rank[r];
+      kout[o] = kin[e];
+      xout[o] = xin[e];
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(kCloudThreads) cloudGatherKernel(const ClosestCloudArgs a, int tb0, int nt, CloudScratch S) {
+  const long M = S.M;
+  for (long it = long(blockIdx.x) * kCloudThreads + threadIdx.x; it < nt * M; it += long(gridDim.x) * kCloudThreads) {
+    const size_t i = size_t(it / M);
+    const size_t j = size_t(S.index[0][it]);
+    const size_t from = ((tb0 + i) * M + j) * 3;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) S.sorted[3 * it + k] = a.target[from + k];
+    if (S.sortedNormals)
+#pragma unroll
+      for (int k = 0; k < 3; ++k) S.sortedNormals[3 * it + k] = a.targetNormals[from + k];
+  }
+}
+
+// Groups of 2^h nodes of level `bottom` (2^bottom nodes, the first at heap index 2^bottom - 1): their boxes, from the sorted points when
+// bottom is the leaf level (`leaves`), else as written by an earlier launch; then the h levels above them, each node the union of its
+// two children.
+__global__ void __launch_bounds__(kCloudThreads) cloudBoxKernel(int nt, CloudScratch S, int bottom, int h, bool leaves) {
+  __shared__ float sb[kCloudThreads][6];
+  const long groups = (1L << bottom) >> h;
+  const int M = S.M;
+  for (long w = blockIdx.x; w < nt * groups; w += gridDim.x) {
+    const size_t i = size_t(w / groups);
+    const long g = w % groups;
+    float* bx = S.boxes + i * (2 * size_t(S.P) - 1) * 6;
+    float box[6];
+    if (threadIdx.x < (1 << h)) {
+      const long j = (g << h) + threadIdx.x;
+      const size_t n = size_t((1L << bottom) - 1 + j);
+      if (leaves) {
+        boxEmpty(box);
+        const float* x = S.sorted + i * size_t(M) * 3;
+        for (long m = j * kLeafPoints; m < min(long(M), (j + 1) * kLeafPoints); ++m) boxGrow(box, ld3(x + 3 * m));
+#pragma unroll
+        for (int k = 0; k < 6; ++k) bx[n * 6 + k] = box[k];
+      } else {
+#pragma unroll
+        for (int k = 0; k < 6; ++k) box[k] = bx[n * 6 + k];
+      }
+#pragma unroll
+      for (int k = 0; k < 6; ++k) sb[threadIdx.x][k] = box[k];
+    }
+    __syncthreads();
+    for (int lev = 1; lev <= h; ++lev) {
+      const int count = 1 << (h - lev);
+      if (threadIdx.x < count) boxUnion(box, sb[2 * threadIdx.x], sb[2 * threadIdx.x + 1]);
+      __syncthreads();
+      if (threadIdx.x < count) {
+        const size_t n = size_t((1L << (bottom - lev)) - 1 + g * count + threadIdx.x);
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+          sb[threadIdx.x][k] = box[k];
+          bx[n * 6 + k] = box[k];
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// One thread per (instance, query) of the instances b0 .. b0 + nb; the trees in S are those of target instances tb0 .. (one when the
+// target is not batched). Depth first from the root as closestPointKernel: both children's bounds, the nearer entered and the other
+// pushed with its bound, re-checked when popped; a void box is never entered. The normal filter does not prune.
+__global__ void __launch_bounds__(kClosestThreads) closestCloudKernel(const ClosestCloudArgs a, int b0, int nb, int tb0, CloudScratch S) {
+  const long N = a.numSource, total = long(nb) * N;
+  const int M = S.M, P = S.P;
+  const bool normals = a.sourceNormals != nullptr;
+  for (long it = long(blockIdx.x) * kClosestThreads + threadIdx.x; it < total; it += long(gridDim.x) * kClosestThreads) {
+    const int i = int(it / N);
+    const size_t qi = size_t(b0 + i) * N + size_t(it % N);
+    const size_t ti = a.targetBatched ? size_t(b0 + i - tb0) : 0;
+    const F3 p = ld3(a.source + 3 * qi);
+    const F3 np = normals ? ld3(a.sourceNormals + 3 * qi) : f3(0.f, 0.f, 0.f);
+    const float* x = S.sorted + ti * M * 3;
+    const float* xn = normals ? S.sortedNormals + ti * M * 3 : nullptr;
+    const int32_t* idx = S.index[0] + ti * M;
+    const float* bx = S.boxes + ti * (2 * size_t(P) - 1) * 6;
+    float best = a.maxDist2;
+    int bestIndex = INT_MAX;
+    int stackNode[kTreeStack];
+    float stackLb[kTreeStack];
+    int sp = 0, node = 0;
+    bool go = finite3(p) && !boxVoid(bx) && !pruneBox(boxLowerBound(bx, p), best);
+    while (go) {
+      if (node < P - 1) {
+        const int c0 = 2 * node + 1;
+        const float* b0x = bx + size_t(c0) * 6;
+        const float lb0 = boxLowerBound(b0x, p), lb1 = boxLowerBound(b0x + 6, p);
+        const bool in0 = !boxVoid(b0x) && !pruneBox(lb0, best), in1 = !boxVoid(b0x + 6) && !pruneBox(lb1, best);
+        if (in0 && in1) {
+          const bool first1 = lb1 < lb0;
+          stackNode[sp] = first1 ? c0 : c0 + 1;
+          stackLb[sp] = first1 ? lb0 : lb1;
+          ++sp;
+          node = first1 ? c0 + 1 : c0;
+          continue;
+        }
+        if (in0 || in1) {
+          node = in0 ? c0 : c0 + 1;
+          continue;
+        }
+      } else {
+        const int m0 = (node - (P - 1)) * kLeafPoints, m1 = min(M, m0 + kLeafPoints);
+        for (int m = m0; m < m1; ++m) {
+          const float d2 = pointDistance2(p, ld3(x + 3 * size_t(m)));
+          if (!(d2 <= best)) continue; // closerFace needs d2 <= best: the index is read only then
+          const int j = idx[m];
+          if (closerFace(d2, j, best, bestIndex) && (!normals || normalCompatible(np, ld3(xn + 3 * size_t(m)), a.maxNormalDot))) {
+            best = d2;
+            bestIndex = j;
+          }
+        }
+      }
+      go = false;
+      while (sp > 0) {
+        --sp;
+        if (!pruneBox(stackLb[sp], best)) {
+          node = stackNode[sp];
+          go = true;
+          break;
+        }
+      }
+    }
+    const bool found = bestIndex != INT_MAX;
+    const size_t from = ((a.targetBatched ? size_t(b0 + i) : 0) * M + size_t(found ? bestIndex : 0)) * 3;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      a.outPoints[3 * qi + k] = found ? a.target[from + k] : 0.f;
+      if (normals) a.outNormals[3 * qi + k] = found ? a.targetNormals[from + k] : 0.f;
+    }
+    a.outIndex[qi] = found ? bestIndex : -1;
+  }
+}
+
+namespace {
+// Builds the trees of target instances tb0 .. tb0 + nt into S (carved for at least nt instances)
+cudaError_t buildCloudTrees(const ClosestCloudArgs& a, int tb0, int nt, int slice, const CloudScratch& S, cudaStream_t stream) {
+  int g = 0;
+  const long tileWork = long(slice) * S.tiles, pointWork = (long(slice) * S.M + kCloudThreads - 1) / kCloudThreads;
+  auto grid = [&](auto kernel, long sliceWork, long work) -> cudaError_t { // sized for a whole slice, capped by this one's work
+    const cudaError_t e = persistentGrid(kernel, kCloudThreads, 0, sliceWork, &g);
+    g = int(std::max(1L, std::min<long>(g, work)));
+    return e;
+  };
+  cudaError_t e = grid(cloudBoundsKernel, tileWork, long(nt) * S.tiles);
+  if (e != cudaSuccess) return e;
+  cloudBoundsKernel<<<g, kCloudThreads, 0, stream>>>(a, tb0, nt, S);
+  if ((e = grid(cloudBoundsReduceKernel, slice, nt)) != cudaSuccess) return e;
+  cloudBoundsReduceKernel<<<g, kCloudThreads, 0, stream>>>(nt, S);
+  if ((e = grid(cloudCodeKernel, pointWork, (long(nt) * S.M + kCloudThreads - 1) / kCloudThreads)) != cudaSuccess) return e;
+  cloudCodeKernel<<<g, kCloudThreads, 0, stream>>>(a, tb0, nt, S);
+  for (int pass = 0; pass < kSortPasses; ++pass) {
+    const int src = pass & 1;
+    if ((e = grid(cloudSortCountKernel, tileWork, long(nt) * S.tiles)) != cudaSuccess) return e;
+    cloudSortCountKernel<<<g, kCloudThreads, 0, stream>>>(nt, S, src, pass * kSortBits);
+    if ((e = grid(cloudSortScanKernel, slice, nt)) != cudaSuccess) return e;
+    cloudSortScanKernel<<<g, kCloudThreads, 0, stream>>>(nt, S);
+    if ((e = grid(cloudSortScatterKernel, tileWork, long(nt) * S.tiles)) != cudaSuccess) return e;
+    cloudSortScatterKernel<<<g, kCloudThreads, 0, stream>>>(nt, S, src, pass * kSortBits);
+  }
+  static_assert(kSortPasses % 2 == 0, "the sorted (code, index) end in keys[0] / index[0]");
+  if ((e = grid(cloudGatherKernel, pointWork, (long(nt) * S.M + kCloudThreads - 1) / kCloudThreads)) != cudaSuccess) return e;
+  cloudGatherKernel<<<g, kCloudThreads, 0, stream>>>(a, tb0, nt, S);
+  int bottom = 0;
+  while ((1 << bottom) < S.P) ++bottom;
+  for (bool leaves = true; leaves || bottom > 0; leaves = false) {
+    const int h = std::min(8, bottom);
+    const long groups = (1L << bottom) >> h;
+    if ((e = grid(cloudBoxKernel, long(slice) * groups, long(nt) * groups)) != cudaSuccess) return e;
+    cloudBoxKernel<<<g, kCloudThreads, 0, stream>>>(nt, S, bottom, h, leaves);
+    bottom -= h;
+  }
+  return cudaGetLastError();
+}
+} // namespace
+
+cudaError_t launchClosestPointsOnCloud(const ClosestCloudArgs& a, cudaStream_t stream) {
+  const long B = a.batch, N = a.numSource;
+  if (B <= 0 || N <= 0) return cudaSuccess;
+  const bool normals = a.sourceNormals != nullptr;
+  if (a.numTarget <= 0) { // no target: index -1 and zeros everywhere
+    cudaError_t e = cudaMemsetAsync(a.outIndex, 0xff, size_t(B) * N * sizeof(int32_t), stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.outPoints, 0, size_t(B) * N * 3 * sizeof(float), stream);
+    if (e == cudaSuccess && normals) e = cudaMemsetAsync(a.outNormals, 0, size_t(B) * N * 3 * sizeof(float), stream);
+    return e;
+  }
+  CloudScratch S{};
+  S.M = a.numTarget;
+  S.tiles = (a.numTarget + kSortTile - 1) / kSortTile;
+  S.P = cloudPadded(a.numTarget);
+  const size_t perInstance = S.floats(normals) * sizeof(float);
+  int queryGrid = 0;
+  cudaError_t e = persistentGrid(closestCloudKernel, kClosestThreads, 0, (B * N + kClosestThreads - 1) / kClosestThreads, &queryGrid);
+  if (e != cudaSuccess) return e;
+  auto query = [&](int b0, int nb, int tb0, const CloudScratch& s) {
+    const long blocks = (long(nb) * N + kClosestThreads - 1) / kClosestThreads;
+    closestCloudKernel<<<int(std::min<long>(queryGrid, blocks)), kClosestThreads, 0, stream>>>(a, b0, nb, tb0, s);
+    return cudaGetLastError();
+  };
+  // an unbatched target: one tree, then every instance's queries in one launch
+  return forEachInstanceSlice(a.targetBatched ? int(B) : 1, perInstance, stream, [&](float* scratch, int slice, int b0, int nb) {
+    CloudScratch s = S;
+    s.carve(scratch, slice, normals);
+    cudaError_t r = buildCloudTrees(a, a.targetBatched ? b0 : 0, nb, slice, s, stream);
+    if (r != cudaSuccess) return r;
+    return a.targetBatched ? query(b0, nb, b0, s) : query(0, int(B), 0, s);
   });
 }
 

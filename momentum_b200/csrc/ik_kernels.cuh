@@ -209,6 +209,23 @@ struct ClosestPointArgs {
 };
 // Enqueues on `stream`; the boxes of a slice of instances go to stream-ordered scratch (cudaMallocAsync), at most 256 MiB.
 cudaError_t launchClosestPointsOnMesh(const ClosestPointArgs& a, cudaStream_t stream);
+// cloud*Kernel / closestCloudKernel: the closest target point of each query point (pymomentum find_closest_points), over a tree built
+// per call on the device for each target instance
+struct ClosestCloudArgs {
+  int32_t batch, numSource, numTarget;
+  bool targetBatched;          // target [B][M][3], else [1][M][3]: one tree for the whole batch
+  float maxDist2;              // max_dist * max_dist; +inf for no bound
+  float maxNormalDot;          // the normal variant's lower bound on dot(n_p, n_t)
+  const float* source;         // [B][N][3]
+  const float* sourceNormals;  // [B][N][3], or null: the plain variant
+  const float* target;         // [B or 1][M][3]
+  const float* targetNormals;  // [B or 1][M][3] when sourceNormals is set
+  float* outPoints;            // [B][N][3]
+  float* outNormals;           // [B][N][3] when sourceNormals is set
+  int32_t* outIndex;           // [B][N]
+};
+// Enqueues on `stream`; the trees of a slice of target instances go to stream-ordered scratch (cudaMallocAsync), at most 256 MiB.
+cudaError_t launchClosestPointsOnCloud(const ClosestCloudArgs& a, cudaStream_t stream);
 // inputGradientKernel: d/d input [grad_theta E . v] of one Position or Orientation (matrix difference) block with the L2 loss, per
 // instance: the input contraction of solve_ik's implicit-function backward
 struct InputGradientArgs {

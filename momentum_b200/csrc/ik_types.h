@@ -185,4 +185,13 @@ struct MeshTreeTables {
   const int32_t* levelStart; // [depth + 1]: the nodes of level L are levelStart[L] .. levelStart[L + 1)
 };
 
+// Point-cloud tree (find_closest_points), built per call and per target instance: the points sorted by Morton code, leaves of
+// kLeafPoints consecutive sorted points, an implicit complete binary tree over the leaves padded to a power of two P (node 0 the root,
+// the children of n at 2n + 1 and 2n + 2, leaf l at node P - 1 + l; a padding leaf has an empty box).
+constexpr int kLeafPoints = 8;    // points per leaf (DESIGN §4, §7)
+constexpr int kSortBits = 8;      // radix digit of the segmented LSD sort
+constexpr int kSortPasses = 4;    // 32 bits: a code is at most 2^30
+constexpr int kSortTile = 1024;   // points per (instance, tile) histogram
+constexpr uint32_t kMortonNonFinite = 1u << 30; // the code of a point with a non-finite coordinate: after every finite one
+
 } // namespace mb2

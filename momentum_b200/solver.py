@@ -81,6 +81,7 @@ CABI_SYMBOLS = [
     "mb2_character_skin_with_blend_shapes_backward_device",
     "mb2_character_set_mesh_faces", "mb2_character_num_faces", "mb2_character_vertex_normals_device", "mb2_character_vertex_normals_backward_device",
     "mb2_character_set_mesh_tree", "mb2_character_closest_points_on_mesh_device",
+    "mb2_closest_points_device",
 ]
 
 _libs = {}
@@ -205,8 +206,28 @@ def load_library(path: Optional[str] = None):
     if hasattr(L, "mb2_character_set_mesh_tree"):
         L.mb2_character_set_mesh_tree.argtypes = [vp, C.c_int32, _fp]
         L.mb2_character_closest_points_on_mesh_device.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, C.c_float, vp, vp, vp, vp]
+    if hasattr(L, "mb2_closest_points_device"):
+        L.mb2_closest_points_device.argtypes = [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_float, C.c_float,
+                                                vp, vp, vp, vp]
     _libs[path] = L
     return L
+
+
+def closest_points_device(device: int, batch: int, num_source: int, num_target: int, target_batched: bool, source_ptr: int,
+                          source_normals_ptr: int, target_ptr: int, target_normals_ptr: int, max_dist: float, max_normal_dot: float,
+                          out_points_ptr: int, out_normals_ptr: int, out_index_ptr: int, stream: int = 0, lib: Optional[str] = None):
+    """mb2_closest_points_device: the closest target point of each query point, source [B][N][3] against target [B or 1][M][3] (one
+    shared target unless ``target_batched``), device float32 memory on ``device``; the normal pointers are all 0 (the plain variant) or
+    all set. Writes out points [B][N][3], out normals [B][N][3] and out index [B][N] int32 (-1 without a candidate), enqueued on
+    ``stream``. Raises MomentumB200Error with the library's message when it rejects the call."""
+    L = load_library(lib)
+    rc = L.mb2_closest_points_device(int(device), int(batch), int(num_source), int(num_target), int(bool(target_batched)),
+                                     C.c_void_p(source_ptr or None), C.c_void_p(source_normals_ptr or None), C.c_void_p(target_ptr or None),
+                                     C.c_void_p(target_normals_ptr or None), float(max_dist), float(max_normal_dot),
+                                     C.c_void_p(out_points_ptr or None), C.c_void_p(out_normals_ptr or None), C.c_void_p(out_index_ptr or None),
+                                     C.c_void_p(stream or None))
+    if rc != 0:
+        raise MomentumB200Error(L.mb2_last_error().decode())
 
 
 def _f32(a):

@@ -354,3 +354,114 @@ def find_closest_points_on_mesh(character, points_source: torch.Tensor, vertices
     if not batched:
         valid, q, face, bary = valid[0], q[0], face[0], bary[0]
     return valid, q, face, bary
+
+
+def find_closest_points(*args, **kwargs):
+    """The closest target point of each query point (pymomentum ``geometry.find_closest_points``), in its two overloads, told apart by
+    the number of leading tensor arguments (neither takes a character)::
+
+        points, index, valid = find_closest_points(points_source, points_target, max_dist=inf)
+        points, normals, index, valid = find_closest_points(points_source, normals_source, points_target, normals_target,
+                                                            max_dist=inf, max_normal_dot=0.0)
+
+    Sources are [N, D] or [B, N, D] and targets [M, D] or [B, M, D], D = 2 or 3 (3 for the normal variant), on one CUDA device; B
+    broadcasts when one side is unbatched, and an unbatched target is searched as one cloud for the whole batch. Per query p the result
+    is the target j with the smallest (squared distance, j) among the candidates: finite targets within ``max_dist`` (d² ≤ max_dist², as
+    ``find_closest_points_on_mesh``; pymomentum's kd-tree uses <) and, in the normal variant, with dot(n_p, n_j) ≥ ``max_normal_dot``.
+    Despite its pymomentum name, ``max_normal_dot`` is that lower bound: 0 keeps targets facing the same half-space. Equal distances go
+    to the lowest index (pymomentum leaves the choice open). A query without a candidate (a non-finite query included) gives valid
+    False, index -1 and zeros. Returned: the target points [.., N, D] (and normals [.., N, 3]) copied from the targets, int32 indices
+    [.., N] and bool validity [.., N]; computed in float32 and returned in the promoted input dtype. D = 2 is searched with z = 0, which
+    gives the same squared distances. A tree is built over each target cloud on the device per call; the result does not depend on it.
+
+    Not differentiable: the outputs carry no gradient. For fitting, gather the targets with the returned indices outside the query::
+
+        with torch.no_grad():
+            _, _, index, valid = find_closest_points(x, n, scan, scan_normals, max_dist=d, max_normal_dot=0.5)
+        t = torch.gather(scan, -2, index.clamp(min=0).long().unsqueeze(-1).expand(*index.shape, 3))
+        nt = torch.gather(scan_normals, -2, index.clamp(min=0).long().unsqueeze(-1).expand(*index.shape, 3))
+        loss = ((((x - t) * nt).sum(-1) ** 2) * valid).sum()             # point-to-plane, differentiable in x (and the scan)
+    """
+    names = ("points_source", "points_target", "max_dist")
+    names_n = ("points_source", "normals_source", "points_target", "normals_target", "max_dist", "max_normal_dot")
+    lead = 0
+    while lead < len(args) and torch.is_tensor(args[lead]):
+        lead += 1
+    normals = lead >= 4 or "normals_source" in kwargs or "normals_target" in kwargs
+    order = names_n if normals else names
+    if len(args) > len(order):
+        raise TypeError(f"find_closest_points takes at most {len(order)} positional arguments, got {len(args)}")
+    given = dict(zip(order, args))
+    for k, v in kwargs.items():
+        if k not in order:
+            raise TypeError(f"find_closest_points got an unexpected keyword argument {k!r}")
+        if k in given:
+            raise TypeError(f"find_closest_points got multiple values for {k!r}")
+        given[k] = v
+    tensors = [n for n in order if n.startswith(("points", "normals"))]
+    missing = [n for n in tensors if n not in given]
+    if missing:
+        raise TypeError(f"find_closest_points is missing {', '.join(missing)}")
+    for n in tensors:
+        t = given[n]
+        if not torch.is_tensor(t) or not t.is_cuda:
+            raise ValueError(f"find_closest_points runs on CUDA tensors (there is no CPU fallback); {n} is not one")
+    src, tgt = given["points_source"], given["points_target"]
+    dev = src.device
+    if any(given[n].device != dev for n in tensors):
+        raise ValueError("find_closest_points: every tensor must be on the same device")
+    max_dist = float(given.get("max_dist", float("inf")))
+    max_normal_dot = float(given.get("max_normal_dot", 0.0))
+    if not max_dist >= 0.0:
+        raise ValueError(f"max_dist must be >= 0 (float('inf') for no bound), got {max_dist}")
+    if max_normal_dot != max_normal_dot:
+        raise ValueError("max_normal_dot must not be NaN")
+    if src.dim() not in (2, 3) or src.shape[-1] not in (2, 3):
+        raise ValueError(f"points_source must be [N, D] or [B, N, D] with D = 2 or 3, got {tuple(src.shape)}")
+    D = src.shape[-1]
+    if tgt.dim() not in (2, 3) or tgt.shape[-1] != D:
+        raise ValueError(f"points_target must be [M, {D}] or [B, M, {D}] like points_source, got {tuple(tgt.shape)}")
+    if src.dim() == 3 and tgt.dim() == 3 and src.shape[0] != tgt.shape[0]:
+        raise ValueError(f"points_source and points_target have batches {src.shape[0]} and {tgt.shape[0]}")
+    if normals:
+        if D != 3:
+            raise ValueError("the normal variant takes 3-D points and normals")
+        for pn, nn in (("points_source", "normals_source"), ("points_target", "normals_target")):
+            if given[nn].shape != given[pn].shape:
+                raise ValueError(f"{nn} must have the shape of {pn}, {tuple(given[pn].shape)}, got {tuple(given[nn].shape)}")
+    batched = src.dim() == 3 or tgt.dim() == 3
+    B = src.shape[0] if src.dim() == 3 else (tgt.shape[0] if tgt.dim() == 3 else 1)
+    N, M = src.shape[-2], tgt.shape[-2]
+    dtype = src.dtype
+    for n in tensors[1:]:
+        dtype = torch.promote_types(dtype, given[n].dtype)
+    if not dtype.is_floating_point:
+        dtype = torch.float32
+    target_batched = tgt.dim() == 3
+
+    def prep(t, rows, shared):
+        t = t.detach().to(torch.float32)
+        if D == 2:
+            t = torch.nn.functional.pad(t, (0, 1))
+        t = t if t.dim() == 3 else t.unsqueeze(0)
+        return (t if shared else t.expand(B, rows, 3)).contiguous()
+
+    index = dev.index if dev.index is not None else torch.cuda.current_device()
+    with torch.no_grad(), torch.cuda.device(index):
+        p = prep(src, N, False)
+        x = prep(tgt, M, not target_batched)
+        pn = prep(given["normals_source"], N, False) if normals else None
+        xn = prep(given["normals_target"], M, not target_batched) if normals else None
+        q = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
+        qn = torch.empty(B, N, 3, device=dev, dtype=torch.float32) if normals else None
+        idx = torch.empty(B, N, device=dev, dtype=torch.int32)
+        ptr = lambda t: 0 if t is None or t.numel() == 0 else t.data_ptr()  # noqa: E731
+        if B * N > 0:
+            ms.closest_points_device(index, B, N, M, target_batched, ptr(p), ptr(pn), ptr(x), ptr(xn), max_dist, max_normal_dot, ptr(q),
+                                     ptr(qn), ptr(idx), torch.cuda.current_stream(dev).cuda_stream)
+        valid = idx >= 0
+        q = q[..., :D].to(dtype)
+        qn = qn.to(dtype) if normals else None
+    if not batched:
+        q, qn, idx, valid = q[0], (qn[0] if normals else None), idx[0], valid[0]
+    return (q, qn, idx, valid) if normals else (q, idx, valid)
