@@ -263,6 +263,46 @@ int mb2_character_skeleton_state_backward_device(const mb2_character* c, int32_t
                                                  const float* grad_skeleton_state_device, float* grad_model_parameters_device,
                                                  void* cuda_stream);
 
+/* The skeleton-state family on the character alone, both directions, with the argument rules of mb2_character_skeleton_state_device.
+ * Joint parameters are [B][7 J] (joint j's seven values t xyz, rx ry rz, log2 scale at 7 j), states [B][J][8] (t, q xyzw, s). Every
+ * backward overwrites dLoss / d its forward's input from dLoss / d its forward's output.
+ * pymomentum apply_parameter_transform (diff_transform_pybind.cpp:27, tensor_parameter_transform.cpp:195-209): [B][n] -> P theta + o
+ * [B][7 J]; its backward is P^T, so it reads no input (model_parameters_device may be null there). */
+int mb2_character_apply_parameter_transform_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                   float* joint_parameters_device, void* cuda_stream);
+int mb2_character_apply_parameter_transform_backward_device(const mb2_character* c, int32_t batch, const float* grad_joint_parameters_device,
+                                                            float* grad_model_parameters_device, void* cuda_stream);
+/* pymomentum joint_parameters_to_skeleton_state (tensor_skeleton_state.cpp:203-343, :488-491): the forward kinematics of
+ * mb2_character_skeleton_state_device from joint parameters [B][7 J] -> [B][J][8] */
+int mb2_character_joint_parameters_to_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                            float* skeleton_state_device, void* cuda_stream);
+int mb2_character_joint_parameters_to_skeleton_state_backward_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                                     const float* grad_skeleton_state_device, float* grad_joint_parameters_device,
+                                                                     void* cuda_stream);
+/* pymomentum joint_parameters_to_local_skeleton_state (:346-484, backward computeLocalSkelStateBackward :139, :493-498): each joint's
+ * transform to its parent, t = offset + p[0:3], q = preRot Rz(p5) Ry(p4) Rx(p3), s = 2^p6: [B][7 J] -> [B][J][8] */
+int mb2_character_joint_parameters_to_local_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                                  float* local_skeleton_state_device, void* cuda_stream);
+int mb2_character_joint_parameters_to_local_skeleton_state_backward_device(const mb2_character* c, int32_t batch,
+                                                                           const float* joint_parameters_device,
+                                                                           const float* grad_local_skeleton_state_device,
+                                                                           float* grad_joint_parameters_device, void* cuda_stream);
+/* pymomentum local_skeleton_state_to_joint_parameters (:611-648): t - offset, the XYZ Euler angles of inv(preRot) q (the asin argument
+ * clamped to [-1, 1], where its derivative is 0), log2 s: [B][J][8] -> [B][J][7] */
+int mb2_character_local_skeleton_state_to_joint_parameters_device(const mb2_character* c, int32_t batch, const float* local_skeleton_state_device,
+                                                                  float* joint_parameters_device, void* cuda_stream);
+int mb2_character_local_skeleton_state_to_joint_parameters_backward_device(const mb2_character* c, int32_t batch,
+                                                                           const float* local_skeleton_state_device,
+                                                                           const float* grad_joint_parameters_device,
+                                                                           float* grad_local_skeleton_state_device, void* cuda_stream);
+/* pymomentum skeleton_state_to_joint_parameters (:650-668): the local states inv(X_parent) X_j (identity above a root), then the rule
+ * above: [B][J][8] -> [B][J][7] */
+int mb2_character_skeleton_state_to_joint_parameters_device(const mb2_character* c, int32_t batch, const float* skeleton_state_device,
+                                                            float* joint_parameters_device, void* cuda_stream);
+int mb2_character_skeleton_state_to_joint_parameters_backward_device(const mb2_character* c, int32_t batch, const float* skeleton_state_device,
+                                                                     const float* grad_joint_parameters_device, float* grad_skeleton_state_device,
+                                                                     void* cuda_stream);
+
 /* Linear-blend skinning of the character (SkinWeights, skin_weights.h:19-40, and Character::inverseBindPose), host arrays, replacing
  * any earlier skinning: rest_vertices [V][3], skin_index / skin_weight [V][8] (a vertex's influences end at its first zero weight,
  * linear_skinning.cpp:76-80; the slots after it are ignored whatever they hold), inverse_bind_pose [J][12] (the row-major top 3x4 of

@@ -1038,7 +1038,8 @@ bool onDevice(int device, std::initializer_list<const void*> required, std::init
 }
 
 // both directions of mb2_character_skeleton_state*_device (gradState is read by the backward only)
-int skeletonStateDevice(const mb2_character* c, int32_t batch, const float* theta, const float* gradState, float* out, void* stream, bool backward) {
+int skeletonStateDevice(const mb2_character* c, int32_t batch, const float* theta, const float* gradState, float* out, void* stream, bool backward,
+                        bool joint = false) {
   MB2_CHECK(c != nullptr, "null character");
   MB2_CHECK(batch >= 0, "batch must not be negative");
   if (batch == 0) return MB2_OK;
@@ -1054,7 +1055,31 @@ int skeletonStateDevice(const mb2_character* c, int32_t batch, const float* thet
   a.theta = theta;
   a.gradState = gradState;
   a.out = out;
+  a.fromJointParameters = joint;
   MB2_CUDA(launchSkeletonState(a, backward, (cudaStream_t)stream));
+  return MB2_OK;
+}
+
+// both directions of the flat joint-parameter operations (launchJointOp); `in` is optional only for the linear parameter transform's
+// backward, which does not read it
+int jointOpDevice(const mb2_character* c, int32_t batch, JointOp op, const char* name, const float* in, const float* grad, float* out, void* stream,
+                  bool backward) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(batch >= 0, "batch must not be negative");
+  if (batch == 0) return MB2_OK;
+  const bool needIn = !(backward && op == kJointOpParameterTransform);
+  MB2_CHECK((in != nullptr || !needIn) && out != nullptr && (!backward || grad != nullptr), "null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(onDevice(c->device, {out}, {in, grad}), std::string(name) + ": every array must be device memory on the character's device");
+  NvtxRange range(name);
+  JointOpArgs a{};
+  a.T = c->tables();
+  a.S = c->skeletonTables();
+  a.batch = batch;
+  a.in = in;
+  a.grad = grad;
+  a.out = out;
+  MB2_CUDA(launchJointOp(a, op, backward, (cudaStream_t)stream));
   return MB2_OK;
 }
 } // namespace
@@ -1066,6 +1091,58 @@ int mb2_character_skeleton_state_device(const mb2_character* c, int32_t batch, c
 int mb2_character_skeleton_state_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
                                                  const float* grad_skeleton_state_device, float* grad_model_parameters_device, void* cuda_stream) {
   return skeletonStateDevice(c, batch, model_parameters_device, grad_skeleton_state_device, grad_model_parameters_device, cuda_stream, true);
+}
+
+int mb2_character_apply_parameter_transform_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                   float* joint_parameters_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpParameterTransform, "applyParameterTransform", model_parameters_device, nullptr, joint_parameters_device, cuda_stream, false);
+}
+int mb2_character_apply_parameter_transform_backward_device(const mb2_character* c, int32_t batch, const float* grad_joint_parameters_device,
+                                                            float* grad_model_parameters_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpParameterTransform, "applyParameterTransformBackward", nullptr, grad_joint_parameters_device, grad_model_parameters_device,
+                       cuda_stream, true);
+}
+int mb2_character_joint_parameters_to_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                            float* skeleton_state_device, void* cuda_stream) {
+  return skeletonStateDevice(c, batch, joint_parameters_device, nullptr, skeleton_state_device, cuda_stream, false, true);
+}
+int mb2_character_joint_parameters_to_skeleton_state_backward_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                                     const float* grad_skeleton_state_device, float* grad_joint_parameters_device,
+                                                                     void* cuda_stream) {
+  return skeletonStateDevice(c, batch, joint_parameters_device, grad_skeleton_state_device, grad_joint_parameters_device, cuda_stream, true, true);
+}
+int mb2_character_joint_parameters_to_local_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                                  float* local_skeleton_state_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpLocalState, "localSkeletonState", joint_parameters_device, nullptr, local_skeleton_state_device, cuda_stream, false);
+}
+int mb2_character_joint_parameters_to_local_skeleton_state_backward_device(const mb2_character* c, int32_t batch,
+                                                                           const float* joint_parameters_device,
+                                                                           const float* grad_local_skeleton_state_device,
+                                                                           float* grad_joint_parameters_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpLocalState, "localSkeletonStateBackward", joint_parameters_device, grad_local_skeleton_state_device,
+                       grad_joint_parameters_device, cuda_stream, true);
+}
+int mb2_character_local_skeleton_state_to_joint_parameters_device(const mb2_character* c, int32_t batch, const float* local_skeleton_state_device,
+                                                                  float* joint_parameters_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpFromLocal, "localSkeletonStateToJointParameters", local_skeleton_state_device, nullptr, joint_parameters_device,
+                       cuda_stream, false);
+}
+int mb2_character_local_skeleton_state_to_joint_parameters_backward_device(const mb2_character* c, int32_t batch,
+                                                                           const float* local_skeleton_state_device,
+                                                                           const float* grad_joint_parameters_device,
+                                                                           float* grad_local_skeleton_state_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpFromLocal, "localSkeletonStateToJointParametersBackward", local_skeleton_state_device, grad_joint_parameters_device,
+                       grad_local_skeleton_state_device, cuda_stream, true);
+}
+int mb2_character_skeleton_state_to_joint_parameters_device(const mb2_character* c, int32_t batch, const float* skeleton_state_device,
+                                                            float* joint_parameters_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpFromWorld, "skeletonStateToJointParameters", skeleton_state_device, nullptr, joint_parameters_device, cuda_stream, false);
+}
+int mb2_character_skeleton_state_to_joint_parameters_backward_device(const mb2_character* c, int32_t batch, const float* skeleton_state_device,
+                                                                     const float* grad_joint_parameters_device, float* grad_skeleton_state_device,
+                                                                     void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpFromWorld, "skeletonStateToJointParametersBackward", skeleton_state_device, grad_joint_parameters_device,
+                       grad_skeleton_state_device, cuda_stream, true);
 }
 
 namespace {

@@ -144,10 +144,13 @@ MB2_HD void fkJoint(const CharacterTables& T, int j, const float* jp, float* js)
 //   fkAxis    (all joints x 3)     rotationAxis.col(i) = q_p a_i   [= (q_p preRot ...) e_i of joint_state.cpp:51-55: one rotation of a
 //                                  rotated vector instead of a rotation by a quaternion product; equal up to rounding]
 // fkJoint above stays the statement-by-statement form (CPU emulation of the oracle order, tests).
+// out: the joint's own slot (8 floats, or kJointStateStride with kDeriv)
 template <bool kDeriv>
-MB2_HD void fkLocalFromParameters(const CharacterTables& T, int j, const float* p, float* js);
+MB2_HD void fkLocalFromParameters(const CharacterTables& T, int j, const float* p, float* out);
 template <bool kDeriv>
-MB2_HD void fkLocal(const CharacterTables& T, int j, const float* jp, float* js) { fkLocalFromParameters<kDeriv>(T, j, jp + j * kParametersPerJoint, js); }
+MB2_HD void fkLocal(const CharacterTables& T, int j, const float* jp, float* js) {
+  fkLocalFromParameters<kDeriv>(T, j, jp + j * kParametersPerJoint, js + j * kJointStateStride);
+}
 // the joint's seven parameters straight from theta (ParameterTransform rows 7 j .. 7 j + 6): no [7 J] array in shared memory, and the
 // transform is spread over lanes = joints (three rounds for 72 joints) instead of lanes = rows (sixteen rounds of dependent loads)
 template <bool kDeriv>
@@ -155,14 +158,13 @@ MB2_HD void fkLocalFromTheta(const CharacterTables& T, int j, const float* theta
   float p[kParametersPerJoint];
 #pragma unroll
   for (int r = 0; r < kParametersPerJoint; ++r) p[r] = jointParameterRow(T, j * kParametersPerJoint + r, theta);
-  fkLocalFromParameters<kDeriv>(T, j, p, js);
+  fkLocalFromParameters<kDeriv>(T, j, p, js + j * kJointStateStride);
 }
 // jp == nullptr: the caller keeps no joint-parameter array (same value, recomputed from theta)
 MB2_HD float jointParameterAt(const CharacterTables& T, const float* jp, const float* theta, int row) { return jp != nullptr ? jp[row] : jointParameterRow(T, row, theta); }
 template <bool kDeriv>
-MB2_HD void fkLocalFromParameters(const CharacterTables& T, int j, const float* p, float* js) {
+MB2_HD void fkLocalFromParameters(const CharacterTables& T, int j, const float* p, float* out) {
   Q4 ql = ld4(T.prerot + 4 * j);
-  float* out = js + j * kJointStateStride;
 #pragma unroll
   for (int index = 2; index >= 0; --index) {
     if (kDeriv) {
@@ -284,6 +286,176 @@ MB2_HD float skelGradModelParameter(const SkeletonTables& S, const float* gjp, i
   return s;
 }
 
+// ---- Joint parameters <-> local and world skeleton states, one joint at a time (pymomentum tensor_skeleton_state.cpp:139-185, :346-498,
+// :589-668, tensor_transforms.cpp:86-164, tensor_quaternion.cpp:179-230) ----------------------------------------------------------------
+// The local state of joint j from its seven parameters is fkLocalFromParameters. Its backward, from the kDeriv local state ls (the DOF
+// axes a_k in the parent frame after t, q, s): g_p[0..2] = g_t; g_p[3+k] = a_k . 1/2 (w g_v + v x g_v - g_w v), since
+// dq/dp[3+k] = 1/2 (a_k, 0) (x) q for a unit pre-rotation (the S_c term of skelGradSeed); g_p[6] = ln2 s g_s.
+MB2_HD void localStateGradient(const float* ls, const float* g, float* gp) {
+  const F3 v = ld3(ls + 3), gv = ld3(g + 3);
+  const float w = ls[6], gw = g[6];
+  const F3 sc = 0.5f * (w * gv + cross(v, gv) - gw * v);
+  gp[0] = g[0]; gp[1] = g[1]; gp[2] = g[2];
+  for (int k = 0; k < 3; ++k) gp[3 + k] = dot(ld3(ls + 8 + 3 * k), sc);
+  gp[6] = kLn2 * (ls[7] * g[7]);
+}
+
+// pymomentum's quaternion inverse conj(q) / |q|^2 and rotation v + 2 (w (u x v) + u x (u x v)), as written: neither normalises q
+MB2_HD Q4 qinverse(Q4 q) {
+  const float n2 = q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w;
+  return q4(-q.x / n2, -q.y / n2, -q.z / n2, q.w / n2);
+}
+MB2_HD F3 qrotWritten(Q4 q, F3 v) {
+  const F3 u = f3(q.x, q.y, q.z);
+  const F3 av = cross(u, v), aav = cross(u, av);
+  return v + 2.f * (av * q.w + aav);
+}
+// the asin argument clamped to [-1, 1]; a NaN passes through (fminf / fmaxf would replace it)
+MB2_HD float clampUnit(float a) { return a > 1.f ? 1.f : (a < -1.f ? -1.f : a); }
+
+// joint parameters p [7] of joint j from its local state ls [8] (localSkeletonStateToJointParameters, :611-648): t - offset_j, the XYZ
+// Euler angles of r = inv(preRot_j) (x) q (quaternionToXYZEuler, on r as it is, unit or not), log2 s
+MB2_HD void jointParametersFromLocal(const CharacterTables& T, int j, const float* ls, float* p) {
+  p[0] = ls[0] - T.offset[3 * j]; p[1] = ls[1] - T.offset[3 * j + 1]; p[2] = ls[2] - T.offset[3 * j + 2];
+  const Q4 r = qmul(qinverse(ld4(T.prerot + 4 * j)), ld4(ls + 3));
+  p[3] = atan2f(2.f * (r.w * r.x + r.y * r.z), 1.f - 2.f * (r.x * r.x + r.y * r.y));
+  p[4] = asinf(clampUnit(2.f * (r.w * r.y - r.z * r.x)));
+  p[5] = atan2f(2.f * (r.w * r.z + r.x * r.y), 1.f - 2.f * (r.y * r.y + r.z * r.z));
+  p[6] = log2f(ls[7]);
+}
+// its backward: g [8] = (dp / d ls)^T gp. d atan2(Y, X) = (X dY - Y dX) / (X^2 + Y^2), skipped for a zero upstream angle gradient (at
+// gimbal lock X = Y = 0 can hold exactly, and 0 / 0 would turn the other angles' gradient into NaN); d asin(A) = dA / sqrt(1 - A^2), 0
+// where the clamp holds (|A| >= 1); r is linear in q, so g_q = conj(inv(preRot)) (x) g_r; d log2 s = ds / (s ln2)
+MB2_HD void jointParametersFromLocalGradient(const CharacterTables& T, int j, const float* ls, const float* gp, float* g) {
+  g[0] = gp[0]; g[1] = gp[1]; g[2] = gp[2];
+  const Q4 pinv = qinverse(ld4(T.prerot + 4 * j));
+  const Q4 r = qmul(pinv, ld4(ls + 3));
+  float gx, gy, gz, gw;
+  { // rx = atan2(Y, X), Y = 2 (w x + y z), X = 1 - 2 (x^2 + y^2)
+    const float Y = 2.f * (r.w * r.x + r.y * r.z), X = 1.f - 2.f * (r.x * r.x + r.y * r.y);
+    const float c = gp[3] == 0.f ? 0.f : gp[3] / (X * X + Y * Y), cY = c * X, cX = -c * Y;
+    gx = 2.f * cY * r.w - 4.f * cX * r.x; gy = 2.f * cY * r.z - 4.f * cX * r.y; gz = 2.f * cY * r.y; gw = 2.f * cY * r.x;
+  }
+  { // ry = asin(A), A = 2 (w y - z x)
+    const float A = 2.f * (r.w * r.y - r.z * r.x);
+    const float cA = (A >= 1.f || A <= -1.f) ? 0.f : gp[4] / sqrtf(1.f - A * A);
+    gx -= 2.f * cA * r.z; gy += 2.f * cA * r.w; gz -= 2.f * cA * r.x; gw += 2.f * cA * r.y;
+  }
+  { // rz = atan2(Z, W), Z = 2 (w z + x y), W = 1 - 2 (y^2 + z^2)
+    const float Z = 2.f * (r.w * r.z + r.x * r.y), W = 1.f - 2.f * (r.y * r.y + r.z * r.z);
+    const float c = gp[5] == 0.f ? 0.f : gp[5] / (W * W + Z * Z), cZ = c * W, cW = -c * Z;
+    gx += 2.f * cZ * r.y; gy += 2.f * cZ * r.x - 4.f * cW * r.y; gz += 2.f * cZ * r.w - 4.f * cW * r.z; gw += 2.f * cZ * r.z;
+  }
+  const Q4 gq = qmul(qconj(pinv), q4(gx, gy, gz, gw));
+  g[3] = gq.x; g[4] = gq.y; g[5] = gq.z; g[6] = gq.w;
+  g[7] = gp[6] / (ls[7] * kLn2);
+}
+
+// local state ls [8] of joint j from the world states X [J][8] of its instance (skeletonStateToJointParameters, :650-668):
+// inv(X_parent) o X_j, with inv(t, q, s) = (-s^-1 rot(q^-1, t), q^-1, s^-1) and (t1, q1, s1) o (t2, q2, s2) = (t1 + rot(q1, s1 t2),
+// q1 (x) q2, s1 s2) as written; above a root is the identity, so a root's local state is its world state
+MB2_HD void localFromWorld(const CharacterTables& T, int j, const float* X, float* ls) {
+  const float* c = X + 8 * j;
+  const int par = T.parent[j];
+  if (par < 0) {
+    for (int k = 0; k < 8; ++k) ls[k] = c[k];
+    return;
+  }
+  const float* P = X + 8 * par;
+  const Q4 qi = qinverse(ld4(P + 3));
+  const float si = 1.f / P[7];
+  const F3 t = (-si) * qrotWritten(qi, ld3(P)) + qrotWritten(qi, si * ld3(c));
+  const Q4 q = qmul(qi, ld4(c + 3));
+  ls[0] = t.x; ls[1] = t.y; ls[2] = t.z;
+  ls[3] = q.x; ls[4] = q.y; ls[5] = q.z; ls[6] = q.w;
+  ls[7] = si * c[7];
+}
+// The backward of local = inv(P) o C for the local state's gradient gl [8], with qi = q_P^-1, si = 1 / s_P, d = t_C - t_P and
+// M = rot(qi, .), so that t = si M d, q = qi q_C, s = si s_C (M^T h = rot(conj(qi), h)):
+//   to C (written): g_tC = si M^T g_t, g_qC = conj(qi) (x) g_q, g_sC = si g_s
+MB2_HD void localFromWorldChildGradient(const float* P, const float* gl, float* gc) {
+  const Q4 qi = qinverse(ld4(P + 3));
+  const float si = 1.f / P[7];
+  const F3 gt = qrotWritten(qconj(qi), si * ld3(gl));
+  const Q4 gq = qmul(qconj(qi), ld4(gl + 3));
+  gc[0] = gt.x; gc[1] = gt.y; gc[2] = gt.z;
+  gc[3] = gq.x; gc[4] = gq.y; gc[5] = gq.z; gc[6] = gq.w;
+  gc[7] = si * gl[7];
+}
+//   to P (added to gp): g_tP = -si M^T g_t, g_sP = -si (g_t . t + g_s s), and through qi: g_qi = g_q (x) conj(q_C) + d/dqi [h . rot(qi, d)]
+//   (h = si g_t: 2 h . (u x d) for w; 2 w (d x h) + 2 (u . d) h + 2 (h . u) d - 4 (h . d) u for u), g_qP = (conj(g_qi) - 2 (qi . g_qi) q_P) / |q_P|^2
+MB2_HD void localFromWorldParentGradient(const float* P, const float* C, const float* ls, const float* gl, float* gp) {
+  const Q4 qp = ld4(P + 3);
+  const Q4 qi = qinverse(qp);
+  const float si = 1.f / P[7];
+  const F3 h = si * ld3(gl), d = ld3(C) - ld3(P), u = f3(qi.x, qi.y, qi.z);
+  const F3 gt = qrotWritten(qconj(qi), h);
+  const Q4 gqc = qmul(ld4(gl + 3), qconj(ld4(C + 3)));
+  const F3 gu = 2.f * (qi.w * cross(d, h) + dot(u, d) * h + dot(h, u) * d) - 4.f * dot(h, d) * u;
+  const Q4 gqi = q4(gqc.x + gu.x, gqc.y + gu.y, gqc.z + gu.z, gqc.w + 2.f * dot(h, cross(u, d)));
+  const float n2 = qp.x * qp.x + qp.y * qp.y + qp.z * qp.z + qp.w * qp.w;
+  const float dq = 2.f * (qi.x * gqi.x + qi.y * gqi.y + qi.z * gqi.z + qi.w * gqi.w);
+  gp[0] -= gt.x; gp[1] -= gt.y; gp[2] -= gt.z;
+  gp[3] += (-gqi.x - dq * qp.x) / n2; gp[4] += (-gqi.y - dq * qp.y) / n2; gp[5] += (-gqi.z - dq * qp.z) / n2;
+  gp[6] += (gqi.w - dq * qp.w) / n2;
+  gp[7] -= si * (dot(ld3(gl), ld3(ls)) + gl[7] * ls[7]);
+}
+// dLoss / d X_j [8] from the joint-parameter gradient gjp [J][7] of the instance: the own local's term, then for each child in ascending
+// index order the term of its local with respect to its parent (no atomics: every output is gathered by one thread)
+MB2_HD void worldStateGradient(const CharacterTables& T, const SkeletonTables& S, int j, const float* X, const float* gjp, float* gX) {
+  float ls[8], gl[8];
+  localFromWorld(T, j, X, ls);
+  jointParametersFromLocalGradient(T, j, ls, gjp + kParametersPerJoint * j, gl);
+  if (T.parent[j] < 0)
+    for (int k = 0; k < 8; ++k) gX[k] = gl[k];
+  else
+    localFromWorldChildGradient(X + 8 * T.parent[j], gl, gX);
+  for (int k = S.childStart[j]; k < S.childStart[j + 1]; ++k) {
+    const int c = S.children[k];
+    localFromWorld(T, c, X, ls);
+    jointParametersFromLocalGradient(T, c, ls, gjp + kParametersPerJoint * c, gl);
+    localFromWorldParentGradient(X + 8 * j, X + 8 * c, ls, gl, gX);
+  }
+}
+
+// The flat operations of a batch (JointOp), one element per thread: kOp's per-instance item count (rows, parameters or joints) and
+// element i of the batch, for input `in`, upstream gradient `grad` (backward) and output `out`, every array [B][...] dense.
+template <int kOp, bool kBackward>
+MB2_HD int jointOpItems(const CharacterTables& T) {
+  if constexpr (kOp == kJointOpParameterTransform) return kBackward ? T.numParams : T.numJoints * kParametersPerJoint;
+  else return T.numJoints;
+}
+template <int kOp, bool kBackward>
+MB2_HD void jointOpElement(const CharacterTables& T, const SkeletonTables& S, long i, const float* in, const float* grad, float* out) {
+  const int per = jointOpItems<kOp, kBackward>(T);
+  const long b = i / per;
+  const int k = int(i - b * per), J = T.numJoints, n = T.numParams;
+  if constexpr (kOp == kJointOpParameterTransform) {
+    if constexpr (kBackward) out[i] = skelGradModelParameter(S, grad + b * (7L * J), k);
+    else out[i] = jointParameterRow(T, k, in + b * n);
+  } else if constexpr (kOp == kJointOpLocalState) {
+    if constexpr (kBackward) {
+      float ls[kJointStateStride];
+      fkLocalFromParameters<true>(T, k, in + 7 * i, ls);
+      localStateGradient(ls, grad + 8 * i, out + 7 * i);
+    } else {
+      fkLocalFromParameters<false>(T, k, in + 7 * i, out + 8 * i);
+    }
+  } else if constexpr (kOp == kJointOpFromLocal) {
+    if constexpr (kBackward) jointParametersFromLocalGradient(T, k, in + 8 * i, grad + 7 * i, out + 8 * i);
+    else jointParametersFromLocal(T, k, in + 8 * i, out + 7 * i);
+  } else {
+    const float* X = in + b * (8L * J);
+    if constexpr (kBackward) {
+      worldStateGradient(T, S, k, X, grad + b * (7L * J), out + 8 * i);
+    } else {
+      float ls[8];
+      localFromWorld(T, k, X, ls);
+      jointParametersFromLocal(T, k, ls, out + 7 * i);
+    }
+  }
+}
+
 // ---- Input contractions of the implicit-function backward of solve_ik: d/d input [grad_theta E_c . v] ----
 // Under the parameter direction v every joint moves rigidly: angular velocity w, log-scale rate sigma, origin velocity tdot. With the
 // joint-parameter velocity u = P v (linear part of the ParameterTransform; its offsets do not move) and pi = parent(j):
@@ -384,8 +556,8 @@ MB2_HD void fkPasses(const Lanes& g, const CharacterTables& C, const float* src,
 
 // The skeleton-state backward of one instance, right after fkPasses<true> (fkAxis writes only the axes and the seed reads only t, q, s:
 // the seed shares the axes' barrier): every joint seeds its subtree sums from the upstream gradient grad [J][8], the levels from the
-// deepest up fold in their children, lanes = joint-parameter rows into gjp [7 J], lanes = model parameters into out [n]. Ends without a
-// barrier.
+// deepest up fold in their children, lanes = joint-parameter rows into gjp [7 J], lanes = model parameters into out [n] (out == nullptr:
+// stops after gjp). Ends without a barrier.
 template <class Lanes>
 MB2_HD void skelGradPasses(const Lanes& g, const CharacterTables& C, const SkeletonTables& S, const float* js, const float* grad, float* acc,
                            float* gjp, float* out) {
@@ -397,6 +569,7 @@ MB2_HD void skelGradPasses(const Lanes& g, const CharacterTables& C, const Skele
     g.sync();
   }
   for (int row = g.lane; row < C.numJoints * kParametersPerJoint; row += g.size) gjp[row] = skelGradJointParameter(C, js, acc, row);
+  if (out == nullptr) return; // the joint-parameter gradient is the result (joint_parameters_to_skeleton_state)
   g.sync();
   for (int p = g.lane; p < C.numParams; p += g.size) out[p] = skelGradModelParameter(S, gjp, p);
 }

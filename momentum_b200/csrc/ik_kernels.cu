@@ -243,29 +243,33 @@ cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream,
 //   forward:   fkPasses from theta, [J][8] out
 //   backward:  fkPasses with the DOF axes, then skelGradPasses: lanes = joints seed their 11 subtree sums from G, levels from the
 //              deepest up fold in their children, lanes = joint-parameter rows, lanes = model parameters over the CSC ParameterTransform.
+// kJoint (joint_parameters_to_skeleton_state): the input is the joint parameters [7 J], staged where theta is staged otherwise; the
+// backward writes the joint-parameter gradient straight out and stops before the ParameterTransform.
 // Every output element is written by one lane in a fixed order: no atomics, the result does not depend on the launch shape.
 // ------------------------------------------------------------------------------------------------
 constexpr int kSkelMaxWarps = 16;
 MB2_HD size_t skelAligned(size_t floats) { return (floats + 3) & ~size_t(3); } // 16-byte aligned regions
 
-// per instance: theta [n], joint states [J][17], backward: subtree sums [J][11] and the joint-parameter gradient [7 J]
-MB2_HD size_t skeletonStateSmemPerInstanceFloats(int J, int n, bool backward) {
-  size_t f = skelAligned(size_t(n)) + skelAligned(size_t(J) * kJointStateStride);
-  if (backward) f += skelAligned(size_t(J) * kSkelAccStride) + skelAligned(size_t(J) * kParametersPerJoint);
+// per instance: the input (theta [n], or the joint parameters [7 J]), joint states [J][17], backward: subtree sums [J][11] and, from
+// theta, the joint-parameter gradient [7 J]
+MB2_HD size_t skeletonStateSmemPerInstanceFloats(int J, int n, bool backward, bool joint) {
+  size_t f = skelAligned(joint ? size_t(J) * kParametersPerJoint : size_t(n)) + skelAligned(size_t(J) * kJointStateStride);
+  if (backward) f += skelAligned(size_t(J) * kSkelAccStride) + (joint ? 0 : skelAligned(size_t(J) * kParametersPerJoint));
   return f;
 }
-size_t skeletonStateSmemPerInstance(const CharacterTables& C, bool backward) {
-  return sizeof(float) * skeletonStateSmemPerInstanceFloats(C.numJoints, C.numParams, backward);
+size_t skeletonStateSmemPerInstance(const CharacterTables& C, bool backward, bool joint) {
+  return sizeof(float) * skeletonStateSmemPerInstanceFloats(C.numJoints, C.numParams, backward, joint);
 }
 
-size_t skeletonStateTableBytes(const SkeletonStateArgs& a, bool backward) {
+size_t skeletonStateTableBytes(const SkeletonStateArgs& a, bool backward, bool joint) {
   const CharacterTables& C = a.T;
   size_t w = characterTableWords(C);
-  if (backward) w += tableWords(C.numJoints + 1, 4) + tableWords(a.numChildren, 4) + tableWords(C.numParams + 1, 4) + tableWords(C.ptNnz, 4) * 2;
+  if (backward) w += tableWords(C.numJoints + 1, 4) + tableWords(a.numChildren, 4);
+  if (backward && !joint) w += tableWords(C.numParams + 1, 4) + tableWords(C.ptNnz, 4) * 2;
   return w * 4;
 }
 
-template <bool kBackward, int W>
+template <bool kBackward, int W, bool kJoint>
 __global__ void __launch_bounds__(32 * kSkelMaxWarps) skeletonStateKernel(const SkeletonStateArgs a) {
   extern __shared__ __align__(16) float smem[];
   CharacterTables T = a.T;
@@ -273,9 +277,10 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps) skeletonStateKernel(const 
   const WarpLanes<W> g = WarpLanes<W>::of(threadIdx.x >> 5, threadIdx.x & 31);
   const int groupsPerCta = (blockDim.x >> 5) / W;
   const int J = T.numJoints, n = T.numParams;
-  const int thF = int(skelAligned(n)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
+  const int inN = kJoint ? J * kParametersPerJoint : n; // floats per instance of the input
+  const int thF = int(skelAligned(inN)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
   const int accF = kBackward ? int(skelAligned(size_t(J) * kSkelAccStride)) : 0;
-  const int perGroup = int(skeletonStateSmemPerInstanceFloats(J, n, kBackward));
+  const int perGroup = int(skeletonStateSmemPerInstanceFloats(J, n, kBackward, kJoint));
   float* th = smem + size_t(g.group) * perGroup;
   float* js = th + thF;
   float* acc = js + jsF;
@@ -285,18 +290,20 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps) skeletonStateKernel(const 
     stageCharacterTables(T, cursor);
     if constexpr (kBackward) {
       stageTable(S.childStart, size_t(J) + 1, cursor); stageTable(S.children, a.numChildren, cursor);
-      stageTable(S.ptColStart, n + 1, cursor); stageTable(S.ptColRows, T.ptNnz, cursor); stageTable(S.ptColVals, T.ptNnz, cursor);
+      if constexpr (!kJoint) { stageTable(S.ptColStart, n + 1, cursor); stageTable(S.ptColRows, T.ptNnz, cursor); stageTable(S.ptColVals, T.ptNnz, cursor); }
     }
     __syncthreads();
   }
   for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
-    const float* theta = a.theta + size_t(b) * n;
-    for (int i = g.lane; i < n; i += g.size) th[i] = theta[i];
+    const float* theta = a.theta + size_t(b) * inN;
+    for (int i = g.lane; i < inN; i += g.size) th[i] = theta[i];
     g.sync();
-    fkPasses<kBackward, false>(g, T, th, js);
+    fkPasses<kBackward, kJoint>(g, T, th, js);
     if constexpr (!kBackward) {
       float* so = a.out + size_t(b) * J * 8;
       for (int i = g.lane; i < J * 8; i += g.size) so[i] = js[(i >> 3) * kJointStateStride + (i & 7)];
+    } else if constexpr (kJoint) {
+      skelGradPasses(g, T, S, js, a.gradState + size_t(b) * J * 8, acc, a.out + size_t(b) * inN, nullptr);
     } else {
       skelGradPasses(g, T, S, js, a.gradState + size_t(b) * J * 8, acc, gjp, a.out + size_t(b) * n);
     }
@@ -345,11 +352,52 @@ cudaError_t launchInstanceGroups(void (*const kernels[4])(Args), const Args& a, 
 } // namespace
 
 cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream) {
-  static void (*const forward[4])(SkeletonStateArgs) = {skeletonStateKernel<false, 1>, skeletonStateKernel<false, 2>, skeletonStateKernel<false, 4>,
-                                                         skeletonStateKernel<false, 8>};
-  static void (*const reverse[4])(SkeletonStateArgs) = {skeletonStateKernel<true, 1>, skeletonStateKernel<true, 2>, skeletonStateKernel<true, 4>,
-                                                         skeletonStateKernel<true, 8>};
-  return launchInstanceGroups(backward ? reverse : forward, a, skeletonStateSmemPerInstance(a.T, backward), skeletonStateTableBytes(a, backward), stream);
+  using K = void (*)(SkeletonStateArgs);
+  static const K kernels[2][2][4] = {
+      {{skeletonStateKernel<false, 1, false>, skeletonStateKernel<false, 2, false>, skeletonStateKernel<false, 4, false>, skeletonStateKernel<false, 8, false>},
+       {skeletonStateKernel<true, 1, false>, skeletonStateKernel<true, 2, false>, skeletonStateKernel<true, 4, false>, skeletonStateKernel<true, 8, false>}},
+      {{skeletonStateKernel<false, 1, true>, skeletonStateKernel<false, 2, true>, skeletonStateKernel<false, 4, true>, skeletonStateKernel<false, 8, true>},
+       {skeletonStateKernel<true, 1, true>, skeletonStateKernel<true, 2, true>, skeletonStateKernel<true, 4, true>, skeletonStateKernel<true, 8, true>}}};
+  const bool joint = a.fromJointParameters != 0;
+  return launchInstanceGroups(kernels[joint][backward], a, skeletonStateSmemPerInstance(a.T, backward, joint), skeletonStateTableBytes(a, backward, joint),
+                              stream);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Joint parameters <-> skeleton states, one element per thread (ik_device.cuh jointOpElement): flat grid-stride kernels over
+// (instance, row), (instance, parameter) or (instance, joint). The character tables are read from global memory: they are shared by the
+// batch and stay in L1 / L2. Each output element is written by one thread, so an instance gets the same bits in any batch.
+// ------------------------------------------------------------------------------------------------
+constexpr int kJointOpThreads = 256;
+constexpr int kJointOpCtasPerSm = 8;
+
+template <int kOp, bool kBackward>
+__device__ __forceinline__ void jointOpGrid(const JointOpArgs& a) {
+  const long items = long(a.batch) * jointOpItems<kOp, kBackward>(a.T);
+  for (long i = blockIdx.x * long(blockDim.x) + threadIdx.x; i < items; i += long(gridDim.x) * blockDim.x)
+    jointOpElement<kOp, kBackward>(a.T, a.S, i, a.in, a.grad, a.out);
+}
+__global__ void __launch_bounds__(kJointOpThreads) parameterTransformKernel(const JointOpArgs a) { jointOpGrid<kJointOpParameterTransform, false>(a); }
+__global__ void __launch_bounds__(kJointOpThreads) parameterTransformBackwardKernel(const JointOpArgs a) { jointOpGrid<kJointOpParameterTransform, true>(a); }
+__global__ void __launch_bounds__(kJointOpThreads) localStateKernel(const JointOpArgs a) { jointOpGrid<kJointOpLocalState, false>(a); }
+__global__ void __launch_bounds__(kJointOpThreads) localStateBackwardKernel(const JointOpArgs a) { jointOpGrid<kJointOpLocalState, true>(a); }
+__global__ void __launch_bounds__(kJointOpThreads) localToJointParametersKernel(const JointOpArgs a) { jointOpGrid<kJointOpFromLocal, false>(a); }
+__global__ void __launch_bounds__(kJointOpThreads) localToJointParametersBackwardKernel(const JointOpArgs a) { jointOpGrid<kJointOpFromLocal, true>(a); }
+__global__ void __launch_bounds__(kJointOpThreads) worldToJointParametersKernel(const JointOpArgs a) { jointOpGrid<kJointOpFromWorld, false>(a); }
+__global__ void __launch_bounds__(kJointOpThreads) worldToJointParametersBackwardKernel(const JointOpArgs a) { jointOpGrid<kJointOpFromWorld, true>(a); }
+
+cudaError_t launchJointOp(const JointOpArgs& a, JointOp op, bool backward, cudaStream_t stream) {
+  using K = void (*)(JointOpArgs);
+  static const K kernels[4][2] = {{parameterTransformKernel, parameterTransformBackwardKernel}, {localStateKernel, localStateBackwardKernel},
+                                  {localToJointParametersKernel, localToJointParametersBackwardKernel},
+                                  {worldToJointParametersKernel, worldToJointParametersBackwardKernel}};
+  if (a.batch <= 0) return cudaSuccess;
+  const long per = op == kJointOpParameterTransform ? (backward ? a.T.numParams : long(a.T.numJoints) * kParametersPerJoint) : a.T.numJoints;
+  const long items = long(a.batch) * per;
+  if (items == 0) return cudaSuccess;
+  const int grid = int(std::min<long>((items + kJointOpThreads - 1) / kJointOpThreads, long(std::max(g_numSms, 1)) * kJointOpCtasPerSm));
+  kernels[op][backward]<<<grid, kJointOpThreads, 0, stream>>>(a);
+  return cudaGetLastError();
 }
 
 // The per-instance scratch of the skinning, blend-shape and normals backward passes, of the closest-point refit and of the point-cloud

@@ -145,11 +145,23 @@ struct SkeletonStateArgs {
   SkeletonTables S;          // backward only
   int32_t numChildren;       // entries of S.children
   int32_t batch;
-  const float* theta;        // [B][n]
+  const float* theta;        // [B][n], or [B][7 J] joint parameters when fromJointParameters
   const float* gradState;    // backward: [B][J][8] dLoss / d state
-  float* out;                // forward: [B][J][8] (t, q xyzw, s); backward: [B][n] dLoss / d theta, overwritten
+  float* out;                // forward: [B][J][8] (t, q xyzw, s); backward: [B][n] dLoss / d theta ([B][7 J] d joint parameters), overwritten
+  int32_t fromJointParameters; // joint_parameters_to_skeleton_state: the FK from joint parameters, S.ptCol* unused
 };
 cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream);
+// parameterTransformKernel ... worldToJointParametersBackwardKernel: the flat joint-parameter operations of ik_device.cuh jointOpElement
+// for a batch, forward or backward; arrays [B][...] dense, device memory
+struct JointOpArgs {
+  CharacterTables T;
+  SkeletonTables S;          // the backward of kJointOpParameterTransform (ptCol*) and of kJointOpFromWorld (children)
+  int32_t batch;
+  const float* in;           // the forward's input (backward: the forward's input, unused by the linear kJointOpParameterTransform)
+  const float* grad;         // backward: dLoss / d the forward's output
+  float* out;                // forward: the output; backward: dLoss / d in, overwritten
+};
+cudaError_t launchJointOp(const JointOpArgs& a, JointOp op, bool backward, cudaStream_t stream);
 // skinVertexKernel / skinStatePartialKernel / skinStateFinishKernel: linear-blend skinning of a batch (applySSD) and its backward
 struct SkinArgs {
   SkinTables S;

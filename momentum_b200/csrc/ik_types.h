@@ -136,6 +136,13 @@ struct SkeletonTables {
   const float* ptColVals;    // [nnz]
 };
 
+// The flat joint-parameter operations (ik_device.cuh jointOpElement), forward / backward:
+//   kJointOpParameterTransform  jp [7 J] = P theta + o (jointParameterRow)      /  g_theta [n] = P^T g_jp
+//   kJointOpLocalState          local states [J][8] of jp [J][7]                /  g_jp [J][7] of g_local [J][8]
+//   kJointOpFromLocal           jp [J][7] of local states [J][8]                /  g_local [J][8] of g_jp [J][7]
+//   kJointOpFromWorld           jp [J][7] of world states [J][8]                /  g_world [J][8] of g_jp [J][7]
+enum JointOp : int32_t { kJointOpParameterTransform = 0, kJointOpLocalState = 1, kJointOpFromLocal = 2, kJointOpFromWorld = 3 };
+
 // Linear-blend skinning tables (HostSkinning, makeSkinning), shared by the whole batch. The active influences of every vertex (the slots
 // before its first zero weight) are stored twice: by vertex for the blend, and by joint for the reductions of the backward, where each
 // joint's list is cut into segments of at most kSkinSegment influences that never cross a joint boundary.

@@ -82,7 +82,19 @@ CABI_SYMBOLS = [
     "mb2_character_set_mesh_faces", "mb2_character_num_faces", "mb2_character_vertex_normals_device", "mb2_character_vertex_normals_backward_device",
     "mb2_character_set_mesh_tree", "mb2_character_closest_points_on_mesh_device",
     "mb2_closest_points_device",
+    "mb2_character_apply_parameter_transform_device", "mb2_character_apply_parameter_transform_backward_device",
+    "mb2_character_joint_parameters_to_skeleton_state_device", "mb2_character_joint_parameters_to_skeleton_state_backward_device",
+    "mb2_character_joint_parameters_to_local_skeleton_state_device", "mb2_character_joint_parameters_to_local_skeleton_state_backward_device",
+    "mb2_character_local_skeleton_state_to_joint_parameters_device", "mb2_character_local_skeleton_state_to_joint_parameters_backward_device",
+    "mb2_character_skeleton_state_to_joint_parameters_device", "mb2_character_skeleton_state_to_joint_parameters_backward_device",
 ]
+
+# the skeleton-state family of DeviceCharacter.joint_op_device: name -> (forward entry, backward entry)
+JOINT_OPS = {
+    name: (f"mb2_character_{name}_device", f"mb2_character_{name}_backward_device")
+    for name in ("apply_parameter_transform", "joint_parameters_to_skeleton_state", "joint_parameters_to_local_skeleton_state",
+                 "local_skeleton_state_to_joint_parameters", "skeleton_state_to_joint_parameters")
+}
 
 _libs = {}
 
@@ -209,6 +221,13 @@ def load_library(path: Optional[str] = None):
     if hasattr(L, "mb2_closest_points_device"):
         L.mb2_closest_points_device.argtypes = [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_float, C.c_float,
                                                 vp, vp, vp, vp]
+    if hasattr(L, "mb2_character_apply_parameter_transform_device"):
+        L.mb2_character_apply_parameter_transform_device.argtypes = [vp, C.c_int32, vp, vp, vp]
+        L.mb2_character_apply_parameter_transform_backward_device.argtypes = [vp, C.c_int32, vp, vp, vp]
+        for name, (fwd, bwd) in JOINT_OPS.items():
+            if name != "apply_parameter_transform":
+                getattr(L, fwd).argtypes = [vp, C.c_int32, vp, vp, vp]
+                getattr(L, bwd).argtypes = [vp, C.c_int32, vp, vp, vp, vp]
     _libs[path] = L
     return L
 
@@ -461,6 +480,15 @@ class DeviceCharacter(_Base):
         """dLoss/d model parameters [B][n] (overwritten) from dLoss/d skeleton state [B][J][8], float32 device memory, on ``stream``."""
         self._check(self._L.mb2_character_skeleton_state_backward_device(self._h, int(batch), C.c_void_p(params_device_ptr), C.c_void_p(grad_state_device_ptr),
                                                                          C.c_void_p(grad_params_device_ptr), C.c_void_p(stream)))
+
+    def joint_op_device(self, name: str, backward: bool, batch: int, *ptrs: int, stream: int = 0):
+        """One direction of an operation of the skeleton-state family (``JOINT_OPS``: apply_parameter_transform,
+        joint_parameters_to_skeleton_state, joint_parameters_to_local_skeleton_state, local_skeleton_state_to_joint_parameters,
+        skeleton_state_to_joint_parameters), float32 device memory on this character's device, enqueued on ``stream``. ``ptrs``: forward
+        (input, output); backward (input, dLoss/d output, dLoss/d input), except apply_parameter_transform's backward, which takes
+        (dLoss/d joint parameters, dLoss/d model parameters). A 0 pointer is passed as null."""
+        fn = getattr(self._L, JOINT_OPS[name][1 if backward else 0])
+        self._check(fn(self._h, int(batch), *[C.c_void_p(p or None) for p in ptrs], C.c_void_p(stream or None)))
 
     def __del__(self):
         if getattr(self, "_h", None):

@@ -1,4 +1,5 @@
-"""Differentiable forward kinematics on CUDA tensors: ``model_parameters_to_skeleton_state``.
+"""Differentiable forward kinematics on CUDA tensors: ``model_parameters_to_skeleton_state`` and the rest of pymomentum's skeleton-state
+family (``apply_parameter_transform``, joint parameters to world and local states, and back), then skinning, normals and closest points.
 
 Mirror of ``pymomentum.geometry.model_parameters_to_skeleton_state`` (pymomentum/tensor_momentum/tensor_skeleton_state.cpp:500-502:
 ``jointParametersToSkeletonState(applyParamTransform(theta))``) for the batched device path. The forward pass is the solver's own FK
@@ -9,6 +10,7 @@ positions or rotations after ``torch_ik.solve_ik`` back-propagates to the solver
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 from torch.autograd.function import once_differentiable
 
@@ -94,6 +96,124 @@ def model_parameters_to_skeleton_state(character, model_parameters: torch.Tensor
     if model_parameters.dim() not in (1, 2) or model_parameters.shape[-1] != ch.num_params:
         raise ValueError(f"model_parameters must be [n] or [B, n] with n = {ch.num_params}, got {tuple(model_parameters.shape)}")
     return _SkeletonState.apply(_device_character(character, model_parameters.device), model_parameters)
+
+
+class _JointOp(torch.autograd.Function):
+    """One operation of the skeleton-state family (``solver.JOINT_OPS``) on [B, in_numel] float32 rows, forward and backward on the
+    device."""
+
+    @staticmethod
+    def forward(ctx, dc, name, x, out_trailing):
+        dev = x.device
+        lead = x.shape[:-2] if name.endswith("to_joint_parameters") else x.shape[:-1]
+        rows = x.detach().to(torch.float32).reshape(-1, int(np.prod(x.shape[len(lead):]))).contiguous()
+        B = rows.shape[0]
+        out = torch.empty(B, int(np.prod(out_trailing)), device=dev, dtype=torch.float32)
+        dc.joint_op_device(name, False, B, rows.data_ptr(), out.data_ptr(), stream=torch.cuda.current_stream(dev).cuda_stream)
+        ctx.dc, ctx.name, ctx.out_numel = dc, name, out.shape[1]
+        ctx.in_shape, ctx.in_dtype = x.shape, x.dtype
+        ctx.save_for_backward(rows)
+        return out.reshape(*lead, *out_trailing).to(x.dtype)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        (rows,) = ctx.saved_tensors
+        B = rows.shape[0]
+        dev = rows.device
+        g = grad_out.to(device=dev, dtype=torch.float32).reshape(B, ctx.out_numel).contiguous()
+        gx = torch.empty_like(rows)
+        ptrs = (g.data_ptr(), gx.data_ptr())
+        if ctx.name != "apply_parameter_transform":  # P^T: the only one that does not read its input
+            ptrs = (rows.data_ptr(),) + ptrs
+        ctx.dc.joint_op_device(ctx.name, True, B, *ptrs, stream=torch.cuda.current_stream(dev).cuda_stream)
+        return None, None, gx.reshape(ctx.in_shape).to(ctx.in_dtype), None
+
+
+def _joint_op(name, character, x, what, trailing, out_trailing):
+    """Checks x ([*trailing] or [B, *trailing], a CUDA tensor) before any library call, then runs the operation."""
+    if not torch.is_tensor(x):
+        raise ValueError(f"{name}: {what} must be a tensor")
+    k = len(trailing)
+    if x.dim() not in (k, k + 1) or tuple(x.shape[-k:]) != tuple(trailing):
+        shape = ", ".join(str(t) for t in trailing)
+        raise ValueError(f"{name}: {what} must be [{shape}] or [B, {shape}], got {tuple(x.shape)}")
+    if not x.is_cuda:
+        raise ValueError(f"{name} runs on CUDA tensors (there is no CPU fallback)")
+    return _JointOp.apply(_device_character(character, x.device), name, x, tuple(out_trailing))
+
+
+def apply_parameter_transform(character, model_parameters: torch.Tensor) -> torch.Tensor:
+    """Joint parameters P theta + o of ``model_parameters`` (pymomentum ``apply_parameter_transform``): [n] or [B, n] on a CUDA device
+    -> [7 J] or [B, 7 J] in the input dtype, computed in float32, each row's products summed in the ParameterTransform's order.
+    ``character`` is a ``momentum_b200.character.Character`` or a ``solver.DeviceCharacter`` on the tensor's device. Differentiable
+    once; the gradient is P^T applied on the device."""
+    ch, _ = _resolve(character)
+    return _joint_op("apply_parameter_transform", character, model_parameters, f"model_parameters (n = {ch.num_params})", (ch.num_params,),
+                     (7 * ch.num_joints,))
+
+
+def joint_parameters_to_skeleton_state(character, joint_parameters: torch.Tensor) -> torch.Tensor:
+    """Skeleton state of flat ``joint_parameters`` (pymomentum ``joint_parameters_to_skeleton_state``): [7 J] or [B, 7 J] on a CUDA
+    device -> [J, 8] or [B, J, 8] rows (t, q xyzw, s) in the input dtype, computed in float32 by the forward kinematics of
+    ``model_parameters_to_skeleton_state``. Differentiable once; the backward is that of ``model_parameters_to_skeleton_state``
+    without the ParameterTransform."""
+    ch, _ = _resolve(character)
+    J = ch.num_joints
+    return _joint_op("joint_parameters_to_skeleton_state", character, joint_parameters, f"joint_parameters (7 J = {7 * J})", (7 * J,), (J, 8))
+
+
+def joint_parameters_to_local_skeleton_state(character, joint_parameters: torch.Tensor) -> torch.Tensor:
+    """Local skeleton state, each joint's transform to its parent, of flat ``joint_parameters`` (pymomentum
+    ``joint_parameters_to_local_skeleton_state``): [7 J] or [B, 7 J] on a CUDA device -> [J, 8] or [B, J, 8] rows (t, q xyzw, s) in
+    the input dtype, computed in float32. Joint j's seven parameters p give t = offset_j + p[0:3], q = preRot_j Rz(p5) Ry(p4) Rx(p3),
+    s = 2^p6, bit for bit the local part of the forward kinematics. Differentiable once."""
+    ch, _ = _resolve(character)
+    J = ch.num_joints
+    return _joint_op("joint_parameters_to_local_skeleton_state", character, joint_parameters, f"joint_parameters (7 J = {7 * J})", (7 * J,),
+                     (J, 8))
+
+
+def model_parameters_to_local_skeleton_state(character, model_parameters: torch.Tensor) -> torch.Tensor:
+    """``joint_parameters_to_local_skeleton_state(apply_parameter_transform(model_parameters))``, as pymomentum composes
+    ``model_parameters_to_local_skeleton_state``: [n] or [B, n] -> [J, 8] or [B, J, 8]. Differentiable once."""
+    return joint_parameters_to_local_skeleton_state(character, apply_parameter_transform(character, model_parameters))
+
+
+_EULER_NOTE = """
+    The rotation parameters are the XYZ Euler angles of r = inv(preRot_j) q, with inv(q) = conj(q) / |q|^2, read off r as it is (a
+    slightly non-unit q is not normalised): rx = atan2(2 (w x + y z), 1 - 2 (x^2 + y^2)), ry = asin(2 (w y - z x)),
+    rz = atan2(2 (w z + x y), 1 - 2 (y^2 + z^2)). One deliberate difference from pymomentum: the asin argument is clamped to [-1, 1],
+    so that a float32 state at gimbal lock, whose argument can round to 1 + eps, gives ry = +-pi/2 where pymomentum gives NaN; where
+    the clamp holds (|argument| >= 1) the derivative of ry is 0. Other non-finite inputs, and s <= 0, propagate as in torch.
+    Differentiable once."""
+
+
+def local_skeleton_state_to_joint_parameters(character, local_skel_state: torch.Tensor) -> torch.Tensor:
+    """Joint parameters of local skeleton states (pymomentum ``local_skeleton_state_to_joint_parameters``): [J, 8] or [B, J, 8] on a
+    CUDA device -> [J, 7] or [B, J, 7] in the input dtype, computed in float32 (``.flatten(-2)`` gives the [.., 7 J] layout the other
+    functions take): t - offset_j, the Euler angles below, log2 s.
+    """
+    ch, _ = _resolve(character)
+    J = ch.num_joints
+    return _joint_op("local_skeleton_state_to_joint_parameters", character, local_skel_state, f"local_skel_state (J = {J})", (J, 8), (J, 7))
+
+
+def skeleton_state_to_joint_parameters(character, skel_state: torch.Tensor) -> torch.Tensor:
+    """Joint parameters of world skeleton states (pymomentum ``skeleton_state_to_joint_parameters``): [J, 8] or [B, J, 8] on a CUDA
+    device -> [J, 7] or [B, J, 7] in the input dtype, computed in float32 (``.flatten(-2)`` gives the [.., 7 J] layout). Each joint's
+    local state is inv(X_parent) X_j (the identity above a root), with inv(t, q, s) = (-s^-1 rot(q^-1, t), q^-1, s^-1) and
+    (t1, q1, s1)(t2, q2, s2) = (t1 + rot(q1, s1 t2), q1 q2, s1 s2), rot(q, v) = v + 2 (w (u x v) + u x (u x v)) unnormalised, as
+    pymomentum writes them; then ``local_skeleton_state_to_joint_parameters``. The gradient of X_j gathers its own local's term and its
+    children's, in a fixed order.
+    """
+    ch, _ = _resolve(character)
+    J = ch.num_joints
+    return _joint_op("skeleton_state_to_joint_parameters", character, skel_state, f"skel_state (J = {J})", (J, 8), (J, 7))
+
+
+local_skeleton_state_to_joint_parameters.__doc__ += _EULER_NOTE
+skeleton_state_to_joint_parameters.__doc__ += _EULER_NOTE
 
 
 class _SkinPoints(torch.autograd.Function):
