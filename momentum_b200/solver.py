@@ -52,48 +52,128 @@ _fp = C.POINTER(C.c_float)
 _ip = C.POINTER(C.c_int32)
 _dp = C.POINTER(C.c_double)
 _up = C.POINTER(C.c_uint64)
+_lp = C.POINTER(C.c_int64)
 
-# every symbol include/momentum_b200.h declares (checked by tests/test_cabi_symbols.py)
-CABI_SYMBOLS = [
-    "mb2_last_error", "mb2_device_count", "mb2_default_gauss_newton_options", "mb2_character_create", "mb2_character_set_parameter_limits",
-    "mb2_character_destroy", "mb2_solver_function_create", "mb2_solver_function_destroy", "mb2_solver_function_num_parameters",
-    "mb2_solver_function_actual_parameters", "mb2_solver_function_batch", "mb2_solver_function_jacobian_rows",
-    "mb2_solver_function_jacobian_stride", "mb2_add_position_error_function", "mb2_add_position_error_function_instanced", "mb2_add_orientation_error_function",
-    "mb2_add_plane_error_function", "mb2_add_model_parameters_error_function",
-    "mb2_add_state_error_function", "mb2_add_limit_error_function", "mb2_set_error_function_weight", "mb2_set_targets",
-    "mb2_set_targets_device", "mb2_set_constraint_weights", "mb2_solver_function_set_enabled_parameters", "mb2_solver_function_get_error",
-    "mb2_solver_function_get_jacobian", "mb2_solver_function_get_jtjr", "mb2_solver_function_get_skeleton_state", "mb2_solver_create",
-    "mb2_solver_destroy", "mb2_solver_set_options", "mb2_solver_set_enabled_parameters", "mb2_solver_solve", "mb2_solver_solve_device",
-    "mb2_solver_get_results", "mb2_solver_get_error_history", "mb2_solver_get_counters", "mb2_solver_set_profiling",
-    "mb2_solver_get_phase_times", "mb2_solver_get_plan_stats", "mb2_solver_get_fused_profile", "mb2_solver_solve_async", "mb2_solver_wait",
-    "mb2_set_constraint_weights_device", "mb2_solver_function_get_jacobian_device",
-    "mb2_mixed_batch_last_error", "mb2_mixed_batch_create", "mb2_mixed_batch_destroy", "mb2_mixed_batch_add_rig", "mb2_mixed_batch_use_limits",
-    "mb2_mixed_batch_add_instance", "mb2_mixed_batch_set_parameters", "mb2_mixed_batch_solve", "mb2_mixed_batch_get_result", "mb2_mixed_batch_get_results",
-    "mb2_mixed_batch_stats", "mb2_mixed_batch_bucket_info",
-    "mb2_character_clone", "mb2_solver_function_clone", "mb2_character_device", "mb2_solver_function_character", "mb2_solver_function_num_error_functions",
-    "mb2_solver_function_target_size", "mb2_sharded_last_error", "mb2_sharded_solver_create", "mb2_sharded_solver_destroy", "mb2_sharded_solver_num_shards",
-    "mb2_sharded_solver_shard_info", "mb2_sharded_solver_set_options", "mb2_sharded_solver_set_targets", "mb2_sharded_solver_solve", "mb2_sharded_solver_get_aggregate",
-    "mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device",
-    "mb2_add_orientation_error_function_instanced", "mb2_solver_function_input_gradients_device",
-    "mb2_solver_function_implicit_direction_device", "mb2_solver_function_get_sweep_launch", "mb2_solver_get_solve_path",
-    "mb2_character_set_skinning", "mb2_character_num_vertices", "mb2_character_skin_points_device", "mb2_character_skin_points_backward_device",
-    "mb2_character_set_blend_shape", "mb2_character_num_blend_shapes", "mb2_character_skin_with_blend_shapes_device",
-    "mb2_character_skin_with_blend_shapes_backward_device",
-    "mb2_character_set_mesh_faces", "mb2_character_num_faces", "mb2_character_vertex_normals_device", "mb2_character_vertex_normals_backward_device",
-    "mb2_character_set_mesh_tree", "mb2_character_closest_points_on_mesh_device",
-    "mb2_closest_points_device",
-    "mb2_character_apply_parameter_transform_device", "mb2_character_apply_parameter_transform_backward_device",
-    "mb2_character_joint_parameters_to_skeleton_state_device", "mb2_character_joint_parameters_to_skeleton_state_backward_device",
-    "mb2_character_joint_parameters_to_local_skeleton_state_device", "mb2_character_joint_parameters_to_local_skeleton_state_backward_device",
-    "mb2_character_local_skeleton_state_to_joint_parameters_device", "mb2_character_local_skeleton_state_to_joint_parameters_backward_device",
-    "mb2_character_skeleton_state_to_joint_parameters_device", "mb2_character_skeleton_state_to_joint_parameters_backward_device",
-]
+# The signature, (restype, argtypes), of every function include/momentum_b200.h declares, in its order (tests/test_cabi_symbols.py
+# checks the names and argument counts against the header). Handles, device memory and streams are c_void_p: a plain int is a
+# pointer and 0 is NULL. Host arrays keep their element type.
+_vp, _int, _int32, _float = C.c_void_p, C.c_int, C.c_int32, C.c_float
+_out, _opt = C.POINTER(_vp), C.POINTER(_Options)
+CABI_SIGNATURES = {
+    "mb2_last_error": (C.c_char_p, []),
+    "mb2_device_count": (_int, []),
+    "mb2_default_gauss_newton_options": (None, [_opt]),
+    "mb2_character_create": (_int, [_int, _int32, _ip, _fp, _fp, _int32, _ip, _ip, _fp, _fp, _out]),
+    "mb2_character_set_parameter_limits": (_int, [_vp, _int32, C.POINTER(_Limit)]),
+    "mb2_character_destroy": (None, [_vp]),
+    "mb2_solver_function_create": (_int, [_vp, _int32, _out]),
+    "mb2_solver_function_destroy": (None, [_vp]),
+    "mb2_solver_function_num_parameters": (_int32, [_vp]),
+    "mb2_solver_function_actual_parameters": (_int32, [_vp]),
+    "mb2_solver_function_batch": (_int32, [_vp]),
+    "mb2_solver_function_jacobian_rows": (_int32, [_vp]),
+    "mb2_solver_function_jacobian_stride": (_int32, [_vp]),
+    "mb2_add_position_error_function": (_int, [_vp, _float, _float, _float, _int32, _ip, _fp, _fp, _ip]),
+    "mb2_add_position_error_function_instanced": (_int, [_vp, _float, _float, _float, _int32, _ip, _fp, _ip]),
+    "mb2_add_orientation_error_function_instanced": (_int, [_vp, _float, _float, _float, _int32, _int32, _ip, _fp, _ip]),
+    "mb2_add_plane_error_function": (_int, [_vp, _float, _float, _float, _int32, _int32, _ip, _fp, _fp, _ip]),
+    "mb2_add_model_parameters_error_function": (_int, [_vp, _float, _fp, _ip]),
+    "mb2_add_orientation_error_function": (_int, [_vp, _float, _float, _float, _int32, _int32, _ip, _fp, _fp, _ip]),
+    "mb2_add_state_error_function": (_int, [_vp, _float, _int32, _float, _float, _fp, _fp, _ip]),
+    "mb2_add_limit_error_function": (_int, [_vp, _float, _float, _float, _ip]),
+    "mb2_set_error_function_weight": (_int, [_vp, _int32, _float]),
+    "mb2_set_targets": (_int, [_vp, _int32, _fp]),
+    "mb2_set_targets_device": (_int, [_vp, _int32, _vp, _vp]),
+    "mb2_set_constraint_weights": (_int, [_vp, _int32, _fp, _int32]),
+    "mb2_set_constraint_weights_device": (_int, [_vp, _int32, _vp, _vp]),
+    "mb2_solver_function_set_enabled_parameters": (_int, [_vp, _up]),
+    "mb2_solver_function_get_error": (_int, [_vp, _fp, _dp]),
+    "mb2_solver_function_get_jacobian": (_int, [_vp, _fp, _fp, _fp, _dp, _ip]),
+    "mb2_solver_function_get_jacobian_device": (_int, [_vp, _vp, _out, _ip, _vp]),
+    "mb2_solver_function_get_jtjr": (_int, [_vp, _fp, _int32, _fp, _fp, _dp]),
+    "mb2_solver_function_get_skeleton_state": (_int, [_vp, _fp, _fp]),
+    "mb2_character_skeleton_state_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_skeleton_state_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_apply_parameter_transform_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_apply_parameter_transform_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_joint_parameters_to_skeleton_state_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_joint_parameters_to_skeleton_state_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_joint_parameters_to_local_skeleton_state_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_joint_parameters_to_local_skeleton_state_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_local_skeleton_state_to_joint_parameters_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_local_skeleton_state_to_joint_parameters_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_skeleton_state_to_joint_parameters_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_skeleton_state_to_joint_parameters_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_set_skinning": (_int, [_vp, _int32, _fp, _ip, _fp, _fp]),
+    "mb2_character_num_vertices": (_int32, [_vp]),
+    "mb2_character_skin_points_device": (_int, [_vp, _int32, _vp, _vp, _int32, _vp, _vp]),
+    "mb2_character_skin_points_backward_device": (_int, [_vp, _int32, _vp, _vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_set_blend_shape": (_int, [_vp, _int32, _int32, _fp, _fp]),
+    "mb2_character_num_blend_shapes": (_int32, [_vp]),
+    "mb2_character_skin_with_blend_shapes_device": (_int, [_vp, _int32, _vp, _vp, _int32, _vp, _vp]),
+    "mb2_character_skin_with_blend_shapes_backward_device": (_int, [_vp, _int32, _vp, _vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_set_mesh_faces": (_int, [_vp, _int32, _int32, _ip]),
+    "mb2_character_num_faces": (_int32, [_vp]),
+    "mb2_character_vertex_normals_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_vertex_normals_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_set_mesh_tree": (_int, [_vp, _int32, _fp]),
+    "mb2_character_closest_points_on_mesh_device": (_int, [_vp, _int32, _int32, _vp, _vp, _float, _vp, _vp, _vp, _vp]),
+    "mb2_closest_points_device": (_int, [_int, _int32, _int32, _int32, _int32, _vp, _vp, _vp, _vp, _float, _float, _vp, _vp, _vp, _vp]),
+    "mb2_solver_function_input_gradients_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mb2_solver_function_implicit_direction_device": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mb2_solver_create": (_int, [_vp, _opt, _out]),
+    "mb2_solver_destroy": (None, [_vp]),
+    "mb2_solver_set_options": (_int, [_vp, _opt]),
+    "mb2_solver_set_enabled_parameters": (_int, [_vp, _up]),
+    "mb2_solver_solve": (_int, [_vp, _vp, _dp, _ip, _ip]),
+    "mb2_solver_solve_async": (_int, [_vp, _vp]),
+    "mb2_solver_wait": (_int, [_vp, _dp, _ip, _ip]),
+    "mb2_solver_solve_device": (_int, [_vp, _vp, _vp]),
+    "mb2_solver_get_results": (_int, [_vp, _dp, _ip, _ip]),
+    "mb2_solver_get_error_history": (_int, [_vp, _dp]),
+    "mb2_solver_get_counters": (_int, [_vp, _up, _up]),
+    "mb2_solver_set_profiling": (_int, [_vp, _int32]),
+    "mb2_solver_get_phase_times": (_int, [_vp, _dp, _up]),
+    "mb2_solver_get_plan_stats": (_int, [_vp, _lp]),
+    "mb2_solver_get_fused_profile": (_int, [_vp, _ip, _ip, _dp, _up]),
+    "mb2_solver_function_get_sweep_launch": (_int, [_vp, _int32, _lp]),
+    "mb2_solver_get_solve_path": (_int, [_vp, _lp]),
+    "mb2_mixed_batch_last_error": (C.c_char_p, []),
+    "mb2_mixed_batch_create": (_int, [_int, _int32, _out]),
+    "mb2_mixed_batch_destroy": (None, [_vp]),
+    "mb2_mixed_batch_add_rig": (_int, [_vp, _vp, _int32, _ip]),
+    "mb2_mixed_batch_use_limits": (_int, [_vp, _int32, _float]),
+    "mb2_mixed_batch_add_instance": (_int, [_vp, _int32, _int32, _ip, _fp, _fp, _fp, _fp, _ip]),
+    "mb2_mixed_batch_set_parameters": (_int, [_vp, _int32, _fp]),
+    "mb2_mixed_batch_solve": (_int, [_vp, _opt]),
+    "mb2_mixed_batch_get_result": (_int, [_vp, _int32, _fp, _dp, _ip, _ip]),
+    "mb2_mixed_batch_get_results": (_int, [_vp, _fp, _lp, _dp, _ip, _ip]),
+    "mb2_mixed_batch_stats": (_int, [_vp, _lp]),
+    "mb2_mixed_batch_bucket_info": (_int, [_vp, _int32, _lp]),
+    "mb2_character_clone": (_int, [_vp, _int, _out]),
+    "mb2_solver_function_clone": (_int, [_vp, _vp, _int32, _out]),
+    "mb2_character_device": (_int, [_vp]),
+    "mb2_solver_function_character": (_vp, [_vp]),
+    "mb2_solver_function_num_error_functions": (_int32, [_vp]),
+    "mb2_solver_function_target_size": (_int32, [_vp, _int32]),
+    "mb2_sharded_last_error": (C.c_char_p, []),
+    "mb2_sharded_solver_create": (_int, [_vp, _int32, _int32, _ip, _opt, _out]),
+    "mb2_sharded_solver_destroy": (None, [_vp]),
+    "mb2_sharded_solver_num_shards": (_int32, [_vp]),
+    "mb2_sharded_solver_shard_info": (_int, [_vp, _int32, _ip]),
+    "mb2_sharded_solver_set_options": (_int, [_vp, _opt]),
+    "mb2_sharded_solver_set_targets": (_int, [_vp, _int32, _fp]),
+    "mb2_sharded_solver_solve": (_int, [_vp, _vp, _dp, _ip, _ip]),
+    "mb2_sharded_solver_get_aggregate": (_int, [_vp, _dp]),
+}
+CABI_SYMBOLS = sorted(CABI_SIGNATURES)
 
 # the skeleton-state family of DeviceCharacter.joint_op_device: name -> (forward entry, backward entry)
 JOINT_OPS = {
-    name: (f"mb2_character_{name}_device", f"mb2_character_{name}_backward_device")
-    for name in ("apply_parameter_transform", "joint_parameters_to_skeleton_state", "joint_parameters_to_local_skeleton_state",
-                 "local_skeleton_state_to_joint_parameters", "skeleton_state_to_joint_parameters")
+    "model_parameters_to_skeleton_state": ("mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device"),
+    **{name: (f"mb2_character_{name}_device", f"mb2_character_{name}_backward_device")
+       for name in ("apply_parameter_transform", "joint_parameters_to_skeleton_state", "joint_parameters_to_local_skeleton_state",
+                    "local_skeleton_state_to_joint_parameters", "skeleton_state_to_joint_parameters")},
 }
 
 _libs = {}
@@ -107,127 +187,10 @@ def load_library(path: Optional[str] = None):
         raise MomentumB200Error(f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                                 "(momentum_b200 has no CPU fallback)")
     L = C.CDLL(path)
-    L.mb2_last_error.restype = C.c_char_p
-    vp = C.c_void_p
-    L.mb2_character_create.argtypes = [C.c_int, C.c_int32, _ip, _fp, _fp, C.c_int32, _ip, _ip, _fp, _fp, C.POINTER(vp)]
-    L.mb2_character_set_parameter_limits.argtypes = [vp, C.c_int32, C.POINTER(_Limit)]
-    L.mb2_character_destroy.argtypes = [vp]
-    L.mb2_solver_function_create.argtypes = [vp, C.c_int32, C.POINTER(vp)]
-    L.mb2_solver_function_destroy.argtypes = [vp]
-    for name in ("num_parameters", "actual_parameters", "batch", "jacobian_rows", "jacobian_stride"):
-        getattr(L, f"mb2_solver_function_{name}").argtypes = [vp]
-    L.mb2_add_position_error_function.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_int32, _ip, _fp, _fp, _ip]
-    if hasattr(L, "mb2_add_position_error_function_instanced"):
-        L.mb2_add_position_error_function_instanced.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_int32, _ip, _fp, _ip]
-    L.mb2_add_orientation_error_function.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_int32, C.c_int32, _ip, _fp, _fp, _ip]
-    L.mb2_add_state_error_function.argtypes = [vp, C.c_float, C.c_int32, C.c_float, C.c_float, _fp, _fp, _ip]
-    L.mb2_add_limit_error_function.argtypes = [vp, C.c_float, C.c_float, C.c_float, _ip]
-    if hasattr(L, "mb2_add_plane_error_function"):
-        L.mb2_add_plane_error_function.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_int32, C.c_int32, _ip, _fp, _fp, _ip]
-        L.mb2_add_model_parameters_error_function.argtypes = [vp, C.c_float, _fp, _ip]
-    L.mb2_set_error_function_weight.argtypes = [vp, C.c_int32, C.c_float]
-    L.mb2_set_targets.argtypes = [vp, C.c_int32, _fp]
-    if hasattr(L, "mb2_set_targets_device"):
-        L.mb2_set_targets_device.argtypes = [vp, C.c_int32, vp, vp]
-    L.mb2_set_constraint_weights.argtypes = [vp, C.c_int32, _fp, C.c_int32]
-    L.mb2_solver_function_set_enabled_parameters.argtypes = [vp, _up]
-    L.mb2_solver_function_get_error.argtypes = [vp, _fp, _dp]
-    L.mb2_solver_function_get_jacobian.argtypes = [vp, _fp, _fp, _fp, _dp, _ip]
-    L.mb2_solver_function_get_jtjr.argtypes = [vp, _fp, C.c_int32, _fp, _fp, _dp]
-    L.mb2_solver_function_get_skeleton_state.argtypes = [vp, _fp, _fp]
-    L.mb2_solver_create.argtypes = [vp, C.POINTER(_Options), C.POINTER(vp)]
-    L.mb2_solver_destroy.argtypes = [vp]
-    L.mb2_solver_set_options.argtypes = [vp, C.POINTER(_Options)]
-    L.mb2_solver_set_enabled_parameters.argtypes = [vp, _up]
-    L.mb2_solver_solve.argtypes = [vp, vp, _dp, _ip, _ip]
-    if hasattr(L, "mb2_solver_solve_device"):
-        L.mb2_solver_solve_device.argtypes = [vp, vp, vp]
-        L.mb2_solver_get_results.argtypes = [vp, _dp, _ip, _ip]
-        L.mb2_solver_set_profiling.argtypes = [vp, C.c_int32]
-        L.mb2_solver_get_phase_times.argtypes = [vp, _dp, _up]
-    L.mb2_solver_get_error_history.argtypes = [vp, _dp]
-    L.mb2_solver_get_counters.argtypes = [vp, _up, _up]
-    if hasattr(L, "mb2_solver_get_plan_stats"):
-        L.mb2_solver_get_plan_stats.argtypes = [vp, C.POINTER(C.c_int64)]
-    if hasattr(L, "mb2_solver_get_fused_profile"):
-        L.mb2_solver_get_fused_profile.argtypes = [vp, _ip, _ip, _dp, _up]
-    L.mb2_default_gauss_newton_options.argtypes = [C.POINTER(_Options)]
-    if hasattr(L, "mb2_set_constraint_weights_device"):
-        L.mb2_set_constraint_weights_device.argtypes = [vp, C.c_int32, vp, vp]
-        L.mb2_solver_function_get_jacobian_device.argtypes = [vp, vp, C.POINTER(vp), _ip, vp]
-    if hasattr(L, "mb2_mixed_batch_create"):
-        L.mb2_solver_solve_async.argtypes = [vp, vp]
-        L.mb2_solver_wait.argtypes = [vp, _dp, _ip, _ip]
-        L.mb2_mixed_batch_last_error.restype = C.c_char_p
-        L.mb2_mixed_batch_create.argtypes = [C.c_int, C.c_int32, C.POINTER(vp)]
-        L.mb2_mixed_batch_destroy.argtypes = [vp]
-        L.mb2_mixed_batch_add_rig.argtypes = [vp, vp, C.c_int32, _ip]
-        L.mb2_mixed_batch_use_limits.argtypes = [vp, C.c_int32, C.c_float]
-        L.mb2_mixed_batch_add_instance.argtypes = [vp, C.c_int32, C.c_int32, _ip, _fp, _fp, _fp, _fp, _ip]
-        L.mb2_mixed_batch_set_parameters.argtypes = [vp, C.c_int32, _fp]
-        L.mb2_mixed_batch_solve.argtypes = [vp, C.POINTER(_Options)]
-        L.mb2_mixed_batch_get_result.argtypes = [vp, C.c_int32, _fp, _dp, _ip, _ip]
-        L.mb2_mixed_batch_get_results.argtypes = [vp, _fp, C.POINTER(C.c_int64), _dp, _ip, _ip]
-        L.mb2_mixed_batch_stats.argtypes = [vp, C.POINTER(C.c_int64)]
-        L.mb2_mixed_batch_bucket_info.argtypes = [vp, C.c_int32, C.POINTER(C.c_int64)]
-    if hasattr(L, "mb2_sharded_solver_create"):
-        L.mb2_sharded_last_error.restype = C.c_char_p
-        L.mb2_character_clone.argtypes = [vp, C.c_int, C.POINTER(vp)]
-        L.mb2_solver_function_clone.argtypes = [vp, vp, C.c_int32, C.POINTER(vp)]
-        L.mb2_character_device.argtypes = [vp]
-        L.mb2_solver_function_character.argtypes = [vp]
-        L.mb2_solver_function_character.restype = vp
-        L.mb2_solver_function_num_error_functions.argtypes = [vp]
-        L.mb2_solver_function_target_size.argtypes = [vp, C.c_int32]
-        L.mb2_sharded_solver_create.argtypes = [vp, C.c_int32, C.c_int32, _ip, C.POINTER(_Options), C.POINTER(vp)]
-        L.mb2_sharded_solver_destroy.argtypes = [vp]
-        L.mb2_sharded_solver_num_shards.argtypes = [vp]
-        L.mb2_sharded_solver_shard_info.argtypes = [vp, C.c_int32, _ip]
-        L.mb2_sharded_solver_set_options.argtypes = [vp, C.POINTER(_Options)]
-        L.mb2_sharded_solver_set_targets.argtypes = [vp, C.c_int32, _fp]
-        L.mb2_sharded_solver_solve.argtypes = [vp, vp, _dp, _ip, _ip]
-        L.mb2_sharded_solver_get_aggregate.argtypes = [vp, _dp]
-    if hasattr(L, "mb2_character_skeleton_state_device"):
-        L.mb2_character_skeleton_state_device.argtypes = [vp, C.c_int32, vp, vp, vp]
-        L.mb2_character_skeleton_state_backward_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
-    if hasattr(L, "mb2_add_orientation_error_function_instanced"):
-        L.mb2_add_orientation_error_function_instanced.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_int32, C.c_int32, _ip, _fp, _ip]
-    if hasattr(L, "mb2_solver_function_input_gradients_device"):
-        L.mb2_solver_function_input_gradients_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
-    if hasattr(L, "mb2_solver_function_implicit_direction_device"):
-        L.mb2_solver_function_implicit_direction_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
-    if hasattr(L, "mb2_solver_function_get_sweep_launch"):
-        L.mb2_solver_function_get_sweep_launch.argtypes = [vp, C.c_int32, C.POINTER(C.c_int64)]
-    if hasattr(L, "mb2_solver_get_solve_path"):
-        L.mb2_solver_get_solve_path.argtypes = [vp, C.POINTER(C.c_int64)]
-    if hasattr(L, "mb2_character_set_skinning"):
-        L.mb2_character_set_skinning.argtypes = [vp, C.c_int32, _fp, _ip, _fp, _fp]
-        L.mb2_character_num_vertices.argtypes = [vp]
-        L.mb2_character_skin_points_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]
-        L.mb2_character_skin_points_backward_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp, vp, vp]
-    if hasattr(L, "mb2_character_set_blend_shape"):
-        L.mb2_character_set_blend_shape.argtypes = [vp, C.c_int32, C.c_int32, _fp, _fp]
-        L.mb2_character_num_blend_shapes.argtypes = [vp]
-        L.mb2_character_skin_with_blend_shapes_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]
-        L.mb2_character_skin_with_blend_shapes_backward_device.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp, vp, vp]
-    if hasattr(L, "mb2_character_set_mesh_faces"):
-        L.mb2_character_set_mesh_faces.argtypes = [vp, C.c_int32, C.c_int32, _ip]
-        L.mb2_character_num_faces.argtypes = [vp]
-        L.mb2_character_vertex_normals_device.argtypes = [vp, C.c_int32, vp, vp, vp]
-        L.mb2_character_vertex_normals_backward_device.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
-    if hasattr(L, "mb2_character_set_mesh_tree"):
-        L.mb2_character_set_mesh_tree.argtypes = [vp, C.c_int32, _fp]
-        L.mb2_character_closest_points_on_mesh_device.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, C.c_float, vp, vp, vp, vp]
-    if hasattr(L, "mb2_closest_points_device"):
-        L.mb2_closest_points_device.argtypes = [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_float, C.c_float,
-                                                vp, vp, vp, vp]
-    if hasattr(L, "mb2_character_apply_parameter_transform_device"):
-        L.mb2_character_apply_parameter_transform_device.argtypes = [vp, C.c_int32, vp, vp, vp]
-        L.mb2_character_apply_parameter_transform_backward_device.argtypes = [vp, C.c_int32, vp, vp, vp]
-        for name, (fwd, bwd) in JOINT_OPS.items():
-            if name != "apply_parameter_transform":
-                getattr(L, fwd).argtypes = [vp, C.c_int32, vp, vp, vp]
-                getattr(L, bwd).argtypes = [vp, C.c_int32, vp, vp, vp, vp]
+    for name, (restype, argtypes) in CABI_SIGNATURES.items():
+        if hasattr(L, name):  # the CPU emulator library of the tests exports a subset of the C-ABI
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
     _libs[path] = L
     return L
 
@@ -240,11 +203,9 @@ def closest_points_device(device: int, batch: int, num_source: int, num_target: 
     all set. Writes out points [B][N][3], out normals [B][N][3] and out index [B][N] int32 (-1 without a candidate), enqueued on
     ``stream``. Raises MomentumB200Error with the library's message when it rejects the call."""
     L = load_library(lib)
-    rc = L.mb2_closest_points_device(int(device), int(batch), int(num_source), int(num_target), int(bool(target_batched)),
-                                     C.c_void_p(source_ptr or None), C.c_void_p(source_normals_ptr or None), C.c_void_p(target_ptr or None),
-                                     C.c_void_p(target_normals_ptr or None), float(max_dist), float(max_normal_dot),
-                                     C.c_void_p(out_points_ptr or None), C.c_void_p(out_normals_ptr or None), C.c_void_p(out_index_ptr or None),
-                                     C.c_void_p(stream or None))
+    rc = L.mb2_closest_points_device(int(device), int(batch), int(num_source), int(num_target), int(bool(target_batched)), source_ptr,
+                                     source_normals_ptr, target_ptr, target_normals_ptr, float(max_dist), float(max_normal_dot), out_points_ptr,
+                                     out_normals_ptr, out_index_ptr, stream)
     if rc != 0:
         raise MomentumB200Error(L.mb2_last_error().decode())
 
@@ -257,6 +218,13 @@ def _f32(a):
 def _i32(a):
     a = np.ascontiguousarray(a, np.int32)
     return a, a.ctypes.data_as(_ip)
+
+
+def _results(n: int):
+    """Per-instance results of n instances, {errors float64, iterations int32, status int32} zeroed, and their pointers in the
+    C-ABI's (errors, iterations, status) order."""
+    r = {"errors": np.zeros(n, np.float64), "iterations": np.zeros(n, np.int32), "status": np.zeros(n, np.int32)}
+    return r, (r["errors"].ctypes.data_as(_dp), r["iterations"].ctypes.data_as(_ip), r["status"].ctypes.data_as(_ip))
 
 
 def parameter_set_bits(enabled: Sequence[bool]) -> np.ndarray:
@@ -389,9 +357,9 @@ class DeviceCharacter(_Base):
         """The closest point on each instance's mesh (vertices [B][V][3]) of its query points [B][N][3]: out points [B][N][3], faces
         [B][N] int32 (-1 without a face within ``max_dist``) and barycentrics [B][N][3]. Device memory on this character's device,
         enqueued on ``stream``."""
-        self._check(self._L.mb2_character_closest_points_on_mesh_device(
-            self._h, int(batch), int(num_points), C.c_void_p(vertices_device_ptr), C.c_void_p(points_device_ptr), float(max_dist),
-            C.c_void_p(out_points_device_ptr), C.c_void_p(out_face_device_ptr), C.c_void_p(out_bary_device_ptr), C.c_void_p(stream)))
+        self._check(self._L.mb2_character_closest_points_on_mesh_device(self._h, int(batch), int(num_points), vertices_device_ptr, points_device_ptr,
+                                                                        float(max_dist), out_points_device_ptr, out_face_device_ptr,
+                                                                        out_bary_device_ptr, stream))
 
     def _set_mesh_faces(self, num_vertices: int, faces):
         if faces is None:
@@ -412,15 +380,13 @@ class DeviceCharacter(_Base):
     def vertex_normals_device(self, batch: int, positions_device_ptr: int, normals_device_ptr: int, stream: int = 0):
         """Area-weighted vertex normals [B][V][3] of vertex positions [B][V][3] over the uploaded faces. float32 device memory on this
         character's device, enqueued on ``stream``."""
-        self._check(self._L.mb2_character_vertex_normals_device(self._h, int(batch), C.c_void_p(positions_device_ptr), C.c_void_p(normals_device_ptr),
-                                                                C.c_void_p(stream)))
+        self._check(self._L.mb2_character_vertex_normals_device(self._h, int(batch), positions_device_ptr, normals_device_ptr, stream))
 
     def vertex_normals_backward_device(self, batch: int, positions_device_ptr: int, grad_normals_device_ptr: int, grad_positions_device_ptr: int,
                                        stream: int = 0):
         """dLoss/d positions [B][V][3] (overwritten) from dLoss/d normals [B][V][3]."""
-        self._check(self._L.mb2_character_vertex_normals_backward_device(self._h, int(batch), C.c_void_p(positions_device_ptr),
-                                                                         C.c_void_p(grad_normals_device_ptr), C.c_void_p(grad_positions_device_ptr),
-                                                                         C.c_void_p(stream)))
+        self._check(self._L.mb2_character_vertex_normals_backward_device(self._h, int(batch), positions_device_ptr, grad_normals_device_ptr,
+                                                                         grad_positions_device_ptr, stream))
 
     @property
     def num_vertices(self) -> int:
@@ -429,16 +395,15 @@ class DeviceCharacter(_Base):
     def skin_points_device(self, batch: int, state_device_ptr: int, rest_device_ptr: int, rest_batched: bool, points_device_ptr: int, stream: int = 0):
         """Skinned points [B][V][3] of skeleton states [B][J][8]; rest points: 0 = the rest mesh, else [V][3] (shared) or [B][V][3]
         (``rest_batched``). float32 device memory on this character's device, enqueued on ``stream``."""
-        self._check(self._L.mb2_character_skin_points_device(self._h, int(batch), C.c_void_p(state_device_ptr), C.c_void_p(rest_device_ptr or None),
-                                                             int(bool(rest_batched)), C.c_void_p(points_device_ptr), C.c_void_p(stream)))
+        self._check(self._L.mb2_character_skin_points_device(self._h, int(batch), state_device_ptr, rest_device_ptr, int(bool(rest_batched)),
+                                                             points_device_ptr, stream))
 
     def skin_points_backward_device(self, batch: int, state_device_ptr: int, rest_device_ptr: int, rest_batched: bool, grad_points_device_ptr: int,
                                     grad_state_device_ptr: int, grad_rest_device_ptr: int, stream: int = 0):
         """dLoss/d skeleton state [B][J][8] and dLoss/d rest points (the rest-point layout; the batch sum when shared) from dLoss/d points
         [B][V][3]. A 0 output pointer is skipped."""
-        self._check(self._L.mb2_character_skin_points_backward_device(
-            self._h, int(batch), C.c_void_p(state_device_ptr), C.c_void_p(rest_device_ptr or None), int(bool(rest_batched)),
-            C.c_void_p(grad_points_device_ptr), C.c_void_p(grad_state_device_ptr or None), C.c_void_p(grad_rest_device_ptr or None), C.c_void_p(stream)))
+        self._check(self._L.mb2_character_skin_points_backward_device(self._h, int(batch), state_device_ptr, rest_device_ptr, int(bool(rest_batched)),
+                                                                      grad_points_device_ptr, grad_state_device_ptr, grad_rest_device_ptr, stream))
 
     def set_blend_shape(self, blend_shape: mc.BlendShape):
         """Uploads ``blend_shape`` (replacing any earlier one); ``self.blend_shape`` is the object uploaded."""
@@ -459,36 +424,26 @@ class DeviceCharacter(_Base):
                                       stream: int = 0):
         """Points [B][V][3] of skeleton states [B][J][8], the rest mesh shaped by blend weights [B][num_weights]. float32 device memory on
         this character's device, enqueued on ``stream``."""
-        self._check(self._L.mb2_character_skin_with_blend_shapes_device(self._h, int(batch), C.c_void_p(state_device_ptr), C.c_void_p(weights_device_ptr),
-                                                                        int(num_weights), C.c_void_p(points_device_ptr), C.c_void_p(stream)))
+        self._check(self._L.mb2_character_skin_with_blend_shapes_device(self._h, int(batch), state_device_ptr, weights_device_ptr, int(num_weights),
+                                                                        points_device_ptr, stream))
 
     def skin_with_blend_shapes_backward_device(self, batch: int, state_device_ptr: int, weights_device_ptr: int, num_weights: int,
                                                grad_points_device_ptr: int, grad_state_device_ptr: int, grad_weights_device_ptr: int, stream: int = 0):
         """dLoss/d skeleton state [B][J][8] and dLoss/d blend weights [B][num_weights] from dLoss/d points [B][V][3]. A 0 output pointer
         is skipped."""
-        self._check(self._L.mb2_character_skin_with_blend_shapes_backward_device(
-            self._h, int(batch), C.c_void_p(state_device_ptr), C.c_void_p(weights_device_ptr), int(num_weights), C.c_void_p(grad_points_device_ptr),
-            C.c_void_p(grad_state_device_ptr or None), C.c_void_p(grad_weights_device_ptr or None), C.c_void_p(stream)))
-
-    def skeleton_state_device(self, batch: int, params_device_ptr: int, state_device_ptr: int, stream: int = 0):
-        """Skeleton state [B][J][8] (t, q xyzw, s) of model parameters [B][n], float32 device memory on this character's device, enqueued
-        on ``stream`` (0: the legacy default stream)."""
-        self._check(self._L.mb2_character_skeleton_state_device(self._h, int(batch), C.c_void_p(params_device_ptr), C.c_void_p(state_device_ptr),
-                                                                C.c_void_p(stream)))
-
-    def skeleton_state_backward_device(self, batch: int, params_device_ptr: int, grad_state_device_ptr: int, grad_params_device_ptr: int, stream: int = 0):
-        """dLoss/d model parameters [B][n] (overwritten) from dLoss/d skeleton state [B][J][8], float32 device memory, on ``stream``."""
-        self._check(self._L.mb2_character_skeleton_state_backward_device(self._h, int(batch), C.c_void_p(params_device_ptr), C.c_void_p(grad_state_device_ptr),
-                                                                         C.c_void_p(grad_params_device_ptr), C.c_void_p(stream)))
+        self._check(self._L.mb2_character_skin_with_blend_shapes_backward_device(self._h, int(batch), state_device_ptr, weights_device_ptr,
+                                                                                 int(num_weights), grad_points_device_ptr, grad_state_device_ptr,
+                                                                                 grad_weights_device_ptr, stream))
 
     def joint_op_device(self, name: str, backward: bool, batch: int, *ptrs: int, stream: int = 0):
-        """One direction of an operation of the skeleton-state family (``JOINT_OPS``: apply_parameter_transform,
-        joint_parameters_to_skeleton_state, joint_parameters_to_local_skeleton_state, local_skeleton_state_to_joint_parameters,
-        skeleton_state_to_joint_parameters), float32 device memory on this character's device, enqueued on ``stream``. ``ptrs``: forward
-        (input, output); backward (input, dLoss/d output, dLoss/d input), except apply_parameter_transform's backward, which takes
-        (dLoss/d joint parameters, dLoss/d model parameters). A 0 pointer is passed as null."""
+        """One direction of an operation of the skeleton-state family (``JOINT_OPS``: model_parameters_to_skeleton_state,
+        apply_parameter_transform, joint_parameters_to_skeleton_state, joint_parameters_to_local_skeleton_state,
+        local_skeleton_state_to_joint_parameters, skeleton_state_to_joint_parameters), float32 device memory on this character's device,
+        enqueued on ``stream`` (0: the legacy default stream). ``ptrs``: forward (input, output); backward (input, dLoss/d output,
+        dLoss/d input), except apply_parameter_transform's backward, which takes (dLoss/d joint parameters, dLoss/d model parameters). A
+        0 pointer is passed as null."""
         fn = getattr(self._L, JOINT_OPS[name][1 if backward else 0])
-        self._check(fn(self._h, int(batch), *[C.c_void_p(p or None) for p in ptrs], C.c_void_p(stream or None)))
+        self._check(fn(self._h, int(batch), *ptrs, stream))
 
     def __del__(self):
         if getattr(self, "_h", None):
@@ -566,19 +521,19 @@ class SkeletonSolverFunction(_Base):
         self._check(self._L.mb2_set_targets(self._h, index, tp))
 
     def set_targets_device(self, index: int, device_ptr: int, stream: int = 0):
-        self._check(self._L.mb2_set_targets_device(self._h, index, C.c_void_p(device_ptr), C.c_void_p(stream)))
+        self._check(self._L.mb2_set_targets_device(self._h, index, device_ptr, stream))
 
     def set_constraint_weights(self, index: int, weights, per_instance: bool = False):
         w, wp = _f32(weights)
         self._check(self._L.mb2_set_constraint_weights(self._h, index, wp, int(per_instance)))
 
     def set_constraint_weights_device(self, index: int, device_ptr: int, stream: int = 0):
-        self._check(self._L.mb2_set_constraint_weights_device(self._h, index, C.c_void_p(device_ptr), C.c_void_p(stream)))
+        self._check(self._L.mb2_set_constraint_weights_device(self._h, index, device_ptr, stream))
 
     def get_jacobian_device(self, params_device_ptr: int, stream: int = 0):
         """(device pointer to [B][n + 1][ld] floats, ld): Jacobian columns then the residual column, in the handle's own buffer."""
         ptr = C.c_void_p(); ld = C.c_int32(0)
-        self._check(self._L.mb2_solver_function_get_jacobian_device(self._h, C.c_void_p(params_device_ptr), C.byref(ptr), C.byref(ld), C.c_void_p(stream)))
+        self._check(self._L.mb2_solver_function_get_jacobian_device(self._h, params_device_ptr, C.byref(ptr), C.byref(ld), stream))
         return ptr.value, ld.value
 
     def input_gradients_device(self, index: int, params_device_ptr: int, direction_device_ptr: int, grad_weights_ptr: int = 0,
@@ -586,19 +541,16 @@ class SkeletonSolverFunction(_Base):
         """d/d input [grad_theta E_index . v] per instance for a Position or Orientation (matrix difference, L2) block: constraint weights
         [B][nc], offsets and targets [B][nc][3|4] (0 = skip that output), from parameters and directions [B][n]; float32 device memory,
         enqueued on ``stream``."""
-        self._check(self._L.mb2_solver_function_input_gradients_device(self._h, int(index), C.c_void_p(params_device_ptr), C.c_void_p(direction_device_ptr),
-                                                                       C.c_void_p(grad_weights_ptr or None), C.c_void_p(grad_offsets_ptr or None),
-                                                                       C.c_void_p(grad_targets_ptr or None), C.c_void_p(stream)))
+        self._check(self._L.mb2_solver_function_input_gradients_device(self._h, int(index), params_device_ptr, direction_device_ptr, grad_weights_ptr,
+                                                                       grad_offsets_ptr, grad_targets_ptr, stream))
 
     def implicit_direction_device(self, params_device_ptr: int, grad_params_device_ptr: int, direction_ptr: int, jacobian_direction_ptr: int = 0,
                                   residual_ptr: int = 0, gradient_rms_ptr: int = 0, stream: int = 0):
         """The direction of solve_ik's implicit-function backward per instance: v = (2 J_E^T J_E)^+ g [B][n] (0 on disabled
         parameters), J v and the residual [B][jacobian_rows] and the gradient RMS [B], from parameters and dLoss/dtheta [B][n]; float32
         device memory (0 = skip that output; the direction is required), enqueued on ``stream``."""
-        self._check(self._L.mb2_solver_function_implicit_direction_device(self._h, C.c_void_p(params_device_ptr), C.c_void_p(grad_params_device_ptr),
-                                                                          C.c_void_p(direction_ptr or None), C.c_void_p(jacobian_direction_ptr or None),
-                                                                          C.c_void_p(residual_ptr or None), C.c_void_p(gradient_rms_ptr or None),
-                                                                          C.c_void_p(stream)))
+        self._check(self._L.mb2_solver_function_implicit_direction_device(self._h, params_device_ptr, grad_params_device_ptr, direction_ptr,
+                                                                          jacobian_direction_ptr, residual_ptr, gradient_rms_ptr, stream))
 
     def set_error_function_weight(self, index: int, weight: float):
         self._check(self._L.mb2_set_error_function_weight(self._h, index, weight))
@@ -694,43 +646,38 @@ class GaussNewtonSolver(_Base):
         """SolverT::solve for every instance. ``params`` [B, n] float32 (host). Returns dict with
         params, errors (objective before the last update, what ``solve`` returns), iterations, status."""
         p = np.ascontiguousarray(params, np.float32).copy()
-        B = self.fn.batch
-        err = np.zeros(B, np.float64); it = np.zeros(B, np.int32); st = np.zeros(B, np.int32)
-        self._check(self._L.mb2_solver_solve(self._h, p.ctypes.data_as(C.c_void_p), err.ctypes.data_as(_dp), it.ctypes.data_as(_ip),
-                                             st.ctypes.data_as(_ip)))
-        return {"params": p, "errors": err, "iterations": it, "status": st}
+        r, ptrs = _results(self.fn.batch)
+        self._check(self._L.mb2_solver_solve(self._h, p.ctypes.data, *ptrs))
+        return {"params": p, **r}
 
     def solve_host_pointer(self, host_ptr: int, results: bool = False):
         """Same through a raw (e.g. pinned) host pointer; per-instance results returned when ``results`` (one mb2_solver_solve call),
         else via get_results()."""
         if not results:
-            self._check(self._L.mb2_solver_solve(self._h, C.c_void_p(host_ptr), None, None, None))
+            self._check(self._L.mb2_solver_solve(self._h, host_ptr, None, None, None))
             return None
-        B = self.fn.batch
-        err = np.zeros(B, np.float64); it = np.zeros(B, np.int32); st = np.zeros(B, np.int32)
-        self._check(self._L.mb2_solver_solve(self._h, C.c_void_p(host_ptr), err.ctypes.data_as(_dp), it.ctypes.data_as(_ip), st.ctypes.data_as(_ip)))
-        return {"errors": err, "iterations": it, "status": st}
+        r, ptrs = _results(self.fn.batch)
+        self._check(self._L.mb2_solver_solve(self._h, host_ptr, *ptrs))
+        return r
 
     def solve_host_pointer_async(self, host_ptr: int):
         """mb2_solver_solve_async: H2D of the parameters, the solve and the D2H of the result are enqueued on the handle's stream; the
         (pinned) buffer belongs to the library until wait()."""
-        self._check(self._L.mb2_solver_solve_async(self._h, C.c_void_p(host_ptr)))
+        self._check(self._L.mb2_solver_solve_async(self._h, host_ptr))
 
     def wait(self):
         """mb2_solver_wait: blocks until the asynchronous solve is done; per-instance results."""
-        B = self.fn.batch
-        err = np.zeros(B, np.float64); it = np.zeros(B, np.int32); st = np.zeros(B, np.int32)
-        self._check(self._L.mb2_solver_wait(self._h, err.ctypes.data_as(_dp), it.ctypes.data_as(_ip), st.ctypes.data_as(_ip)))
-        return {"errors": err, "iterations": it, "status": st}
+        r, ptrs = _results(self.fn.batch)
+        self._check(self._L.mb2_solver_wait(self._h, *ptrs))
+        return r
 
     def solve_device(self, device_ptr: int, stream: int = 0):
-        self._check(self._L.mb2_solver_solve_device(self._h, C.c_void_p(device_ptr), C.c_void_p(stream)))
+        self._check(self._L.mb2_solver_solve_device(self._h, device_ptr, stream))
 
     def get_results(self):
-        B = self.fn.batch
-        err = np.zeros(B, np.float64); it = np.zeros(B, np.int32); st = np.zeros(B, np.int32)
-        self._check(self._L.mb2_solver_get_results(self._h, err.ctypes.data_as(_dp), it.ctypes.data_as(_ip), st.ctypes.data_as(_ip)))
-        return {"errors": err, "iterations": it, "status": st}
+        r, ptrs = _results(self.fn.batch)
+        self._check(self._L.mb2_solver_get_results(self._h, *ptrs))
+        return r
 
     def get_error_history(self):
         B = self.fn.batch
@@ -834,10 +781,9 @@ class MixedBatch(_Base):
         offs = np.zeros(N + 1, np.int64)
         np.cumsum(self._sizes, out=offs[1:])
         theta = np.zeros(int(offs[-1]), np.float32)
-        err = np.zeros(N, np.float64); it = np.zeros(N, np.int32); st = np.zeros(N, np.int32)
-        self._check(self._L.mb2_mixed_batch_get_results(self._h, theta.ctypes.data_as(_fp), offs.ctypes.data_as(C.POINTER(C.c_int64)), err.ctypes.data_as(_dp),
-                                                        it.ctypes.data_as(_ip), st.ctypes.data_as(_ip)))
-        return {"params": [theta[offs[i]:offs[i + 1]] for i in range(N)], "errors": err, "iterations": it, "status": st}
+        r, ptrs = _results(N)
+        self._check(self._L.mb2_mixed_batch_get_results(self._h, theta.ctypes.data_as(_fp), offs.ctypes.data_as(_lp), *ptrs))
+        return {"params": [theta[offs[i]:offs[i + 1]] for i in range(N)], **r}
 
     def stats(self):
         st = (C.c_int64 * 6)()
@@ -897,16 +843,13 @@ class ShardedGaussNewtonSolver(_Base):
     def solve(self, theta0):
         p = np.ascontiguousarray(theta0, np.float32).copy()
         assert p.shape == (self.total_batch, self.num_params)
-        B = self.total_batch
-        err = np.zeros(B, np.float64); it = np.zeros(B, np.int32); st = np.zeros(B, np.int32)
-        self._check(self._L.mb2_sharded_solver_solve(self._h, p.ctypes.data_as(C.c_void_p), err.ctypes.data_as(_dp), it.ctypes.data_as(_ip), st.ctypes.data_as(_ip)))
-        agg = (C.c_double * 3)()
-        self._check(self._L.mb2_sharded_solver_get_aggregate(self._h, agg))
-        return {"params": p, "errors": err, "iterations": it, "status": st, "aggregate": {"error_sum": agg[0], "iterations": int(agg[1]), "instances_ok": int(agg[2])}}
+        r, ptrs = _results(self.total_batch)
+        self._check(self._L.mb2_sharded_solver_solve(self._h, p.ctypes.data, *ptrs))
+        return {"params": p, **r, "aggregate": self.get_aggregate()}
 
     def solve_host_pointer(self, host_ptr: int):
         """In place on a raw (pinned) host buffer [total_batch][n]; the aggregate via get_aggregate()."""
-        self._check(self._L.mb2_sharded_solver_solve(self._h, C.c_void_p(host_ptr), None, None, None))
+        self._check(self._L.mb2_sharded_solver_solve(self._h, host_ptr, None, None, None))
 
     def get_aggregate(self):
         agg = (C.c_double * 3)()

@@ -59,45 +59,6 @@ def _resolve(character, need=None):
     return ch, sk
 
 
-class _SkeletonState(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, dc, model_parameters):
-        n, J = dc.character.num_params, dc.character.num_joints
-        dev = model_parameters.device
-        theta = model_parameters.detach().to(torch.float32).reshape(-1, n).contiguous()
-        B = theta.shape[0]
-        state = torch.empty(B, J, 8, device=dev, dtype=torch.float32)
-        dc.skeleton_state_device(B, theta.data_ptr(), state.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-        ctx.dc = dc
-        ctx.in_shape, ctx.in_dtype = model_parameters.shape, model_parameters.dtype
-        ctx.save_for_backward(theta)
-        return state.reshape(*model_parameters.shape[:-1], J, 8).to(model_parameters.dtype)
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_state):
-        (theta,) = ctx.saved_tensors
-        dc = ctx.dc
-        B, n = theta.shape
-        dev = theta.device
-        g = grad_state.to(device=dev, dtype=torch.float32).reshape(B, dc.character.num_joints, 8).contiguous()
-        grad_theta = torch.empty(B, n, device=dev, dtype=torch.float32)
-        dc.skeleton_state_backward_device(B, theta.data_ptr(), g.data_ptr(), grad_theta.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-        return None, grad_theta.reshape(ctx.in_shape).to(ctx.in_dtype)
-
-
-def model_parameters_to_skeleton_state(character, model_parameters: torch.Tensor) -> torch.Tensor:
-    """Skeleton state of ``model_parameters`` ([n] or [B, n], on a CUDA device): [J, 8] or [B, J, 8] rows (t, q xyzw, s) in the input
-    dtype, computed in float32. ``character`` is a ``momentum_b200.character.Character`` or a ``solver.DeviceCharacter`` on the
-    tensor's device. Differentiable once with respect to ``model_parameters``."""
-    if not torch.is_tensor(model_parameters) or not model_parameters.is_cuda:
-        raise ValueError("model_parameters_to_skeleton_state runs on CUDA tensors (there is no CPU fallback)")
-    ch, _ = _resolve(character)
-    if model_parameters.dim() not in (1, 2) or model_parameters.shape[-1] != ch.num_params:
-        raise ValueError(f"model_parameters must be [n] or [B, n] with n = {ch.num_params}, got {tuple(model_parameters.shape)}")
-    return _SkeletonState.apply(_device_character(character, model_parameters.device), model_parameters)
-
-
 class _JointOp(torch.autograd.Function):
     """One operation of the skeleton-state family (``solver.JOINT_OPS``) on [B, in_numel] float32 rows, forward and backward on the
     device."""
@@ -141,6 +102,15 @@ def _joint_op(name, character, x, what, trailing, out_trailing):
     if not x.is_cuda:
         raise ValueError(f"{name} runs on CUDA tensors (there is no CPU fallback)")
     return _JointOp.apply(_device_character(character, x.device), name, x, tuple(out_trailing))
+
+
+def model_parameters_to_skeleton_state(character, model_parameters: torch.Tensor) -> torch.Tensor:
+    """Skeleton state of ``model_parameters`` ([n] or [B, n], on a CUDA device): [J, 8] or [B, J, 8] rows (t, q xyzw, s) in the input
+    dtype, computed in float32. ``character`` is a ``momentum_b200.character.Character`` or a ``solver.DeviceCharacter`` on the
+    tensor's device. Differentiable once with respect to ``model_parameters``."""
+    ch, _ = _resolve(character)
+    return _joint_op("model_parameters_to_skeleton_state", character, model_parameters, f"model_parameters (n = {ch.num_params})",
+                     (ch.num_params,), (ch.num_joints, 8))
 
 
 def apply_parameter_transform(character, model_parameters: torch.Tensor) -> torch.Tensor:

@@ -210,7 +210,8 @@ def main():
         # the FK from joint parameters beside the FK from model parameters
         st = torch.empty(B, J, 8, device=dev)
         jpc = jp.contiguous()
-        for label, f in (("model_parameters_to_skeleton_state", lambda: dc.skeleton_state_device(B, theta.data_ptr(), st.data_ptr(), stream)),
+        for label, f in (("model_parameters_to_skeleton_state", lambda: dc.joint_op_device("model_parameters_to_skeleton_state", False, B, theta.data_ptr(),
+                                                                                          st.data_ptr(), stream=stream)),
                          ("joint_parameters_to_skeleton_state", lambda: dc.joint_op_device("joint_parameters_to_skeleton_state", False, B, jpc.data_ptr(),
                                                                                           st.data_ptr(), stream=stream))):
             med, best = timed(f, args.reps, args.iters, args.warmup)

@@ -25,6 +25,7 @@ from momentum_b200 import character as mc  # noqa: E402
 from momentum_b200 import torch_skeleton as tsk  # noqa: E402
 
 CASES = [("humanoid72", 8192), ("bodyhands300", 2048), ("humanoid72", 256)]
+OP = "model_parameters_to_skeleton_state"
 
 
 def card():
@@ -131,11 +132,11 @@ def main():
         stream = torch.cuda.current_stream(dev).cuda_stream
 
         def ours_fwd():
-            dc.skeleton_state_device(B, theta.data_ptr(), state.data_ptr(), stream)
+            dc.joint_op_device(OP, False, B, theta.data_ptr(), state.data_ptr(), stream=stream)
 
         def ours_fwd_bwd():
-            dc.skeleton_state_device(B, theta.data_ptr(), state.data_ptr(), stream)
-            dc.skeleton_state_backward_device(B, theta.data_ptr(), G.data_ptr(), grad.data_ptr(), stream)
+            dc.joint_op_device(OP, False, B, theta.data_ptr(), state.data_ptr(), stream=stream)
+            dc.joint_op_device(OP, True, B, theta.data_ptr(), G.data_ptr(), grad.data_ptr(), stream=stream)
 
         fk = TorchFK(ch, dev)
         th_req = theta.clone().requires_grad_(True)

@@ -25,6 +25,11 @@ def test_header_symbols_exported(lib):
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in momentum_b200.h but not exported"
     assert sorted(ms.CABI_SYMBOLS) == declared
+    # every binding takes as many arguments as its prototype declares (comments dropped: some hold commas or calls)
+    prototypes = dict(re.findall(r"\b(mb2_[a-z0-9_]+)\s*\(([^)]*)\)", re.sub(r"/\*.*?\*/", "", header, flags=re.S)))
+    for name, (_, argtypes) in ms.CABI_SIGNATURES.items():
+        params = prototypes[name].strip()
+        assert len(argtypes) == (0 if params in ("", "void") else params.count(",") + 1), (name, params, argtypes)
 
 
 def test_no_cpu_fallback_without_device(lib):

@@ -19,6 +19,8 @@ from tests import emu_lib
 # H100 80GB HBM3 at a 700 W power limit (humanoid72 both times); the quaternion-term and swapped-DOF errors below are >= 5e-3
 K_BOUND = 7e-6
 
+OP = "model_parameters_to_skeleton_state"  # its entry in solver.JOINT_OPS
+
 
 # ---- fixtures ----------------------------------------------------------------------------------------------------------------------
 def _far_humanoid():
@@ -283,7 +285,7 @@ def _many_waves(ch):
 
 
 @pytest.mark.gpu
-def test_large_batch_bound_and_determinism():
+def test_large_batch_bound_and_determinism_through_joint_op_device():
     from momentum_b200 import torch_skeleton as tsk
 
     ch = mc.humanoid72()[0]
@@ -295,12 +297,12 @@ def test_large_batch_bound_and_determinism():
 
     def backward(t, g):
         out = torch.empty_like(t)
-        dc.skeleton_state_backward_device(t.shape[0], t.data_ptr(), g.contiguous().data_ptr(), out.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        dc.joint_op_device(OP, True, t.shape[0], t.data_ptr(), g.contiguous().data_ptr(), out.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
         return out
 
     def forward(t):
         out = torch.empty(t.shape[0], ch.num_joints, 8, device=t.device)
-        dc.skeleton_state_device(t.shape[0], t.data_ptr(), out.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        dc.joint_op_device(OP, False, t.shape[0], t.data_ptr(), out.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
         return out
 
     g1, g2 = backward(th, Gd), backward(th, Gd)
@@ -370,7 +372,7 @@ def test_torch_wrapper_shapes_dtypes_streams_and_errors():
 
 
 @pytest.mark.gpu
-def test_c_abi_rejects_bad_arguments():
+def test_c_abi_rejects_bad_arguments_through_joint_op_device():
     ch = mc.create_test_character(4)
     dc = ms.DeviceCharacter(ch, 0)
     n, J = ch.num_params, ch.num_joints
@@ -378,15 +380,15 @@ def test_c_abi_rejects_bad_arguments():
     st = torch.zeros(2, J, 8, device="cuda")
     host = np.zeros((2, J, 8), np.float32)
     with pytest.raises(ms.MomentumB200Error, match="device memory"):
-        dc.skeleton_state_device(2, th.data_ptr(), host.ctypes.data)
+        dc.joint_op_device(OP, False, 2, th.data_ptr(), host.ctypes.data)
     with pytest.raises(ms.MomentumB200Error, match="null"):
-        dc.skeleton_state_device(2, 0, st.data_ptr())
+        dc.joint_op_device(OP, False, 2, 0, st.data_ptr())
     with pytest.raises(ms.MomentumB200Error, match="negative"):
-        dc.skeleton_state_device(-1, th.data_ptr(), st.data_ptr())
+        dc.joint_op_device(OP, False, -1, th.data_ptr(), st.data_ptr())
     with pytest.raises(ms.MomentumB200Error, match="null"):
-        dc.skeleton_state_backward_device(2, th.data_ptr(), 0, th.data_ptr())
-    dc.skeleton_state_device(0, 0, 0)  # batch 0: nothing to do
-    dc.skeleton_state_backward_device(0, 0, 0, 0)
+        dc.joint_op_device(OP, True, 2, th.data_ptr(), 0, th.data_ptr())
+    dc.joint_op_device(OP, False, 0, 0, 0)  # batch 0: nothing to do
+    dc.joint_op_device(OP, True, 0, 0, 0, 0)
 
 
 @pytest.mark.gpu
