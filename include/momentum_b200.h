@@ -303,6 +303,32 @@ int mb2_character_skeleton_state_to_joint_parameters_backward_device(const mb2_c
                                                                      const float* grad_joint_parameters_device, float* grad_skeleton_state_device,
                                                                      void* cuda_stream);
 
+/* pymomentum model_parameters_to_positions / joint_parameters_to_positions (geometry_pybind.cpp:1131-1171,
+ * tensor_joint_parameters_to_positions.cpp:33-52, :320-327): the world positions of num_points points fixed in joints' frames,
+ * p_i = t_a + rot(q_a, s_a offsets_i) with (t_a, q_a, s_a) the world state of joint a = parents[i] (the position constraint's point).
+ * Parameters [B][n] (model) or [B][7 J] (joint), parents [num_points] in HOST memory, offsets [num_points][3] shared by the batch
+ * (offsets_batched == 0) or [B][num_points][3], positions [B][num_points][3]. The argument rules of mb2_character_skeleton_state_device;
+ * besides, num_points < 0 or a parent outside [0, J) (checkValidBoneIndex) is MB2_ERR_INVALID_ARGUMENT. num_points == 0 is valid: the
+ * point arrays may then be NULL. The call uploads the points grouped by joint into stream-ordered scratch (cudaMallocAsync). */
+int mb2_character_model_parameters_to_positions_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                       int32_t num_points, const int32_t* parents, const float* offsets_device,
+                                                       int32_t offsets_batched, float* positions_device, void* cuda_stream);
+int mb2_character_joint_parameters_to_positions_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                       int32_t num_points, const int32_t* parents, const float* offsets_device,
+                                                       int32_t offsets_batched, float* positions_device, void* cuda_stream);
+/* their backward (d_jointParametersToPositions, :54-119; the model variant then the ParameterTransform transposed) from dLoss/d positions
+ * [B][num_points][3]: grad_params [B][n] ([B][7 J]) and grad_offsets in the offset layout ([num_points][3] = the batch sum when shared),
+ * both overwritten. Either output may be NULL, not both. Same rules as the forward. A shared-offset gradient takes stream-ordered scratch
+ * from the device's default memory pool: at most 256 MiB of per-instance rows and 128 x num_points x 3 floats of chunk sums. */
+int mb2_character_model_parameters_to_positions_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                                int32_t num_points, const int32_t* parents, const float* offsets_device,
+                                                                int32_t offsets_batched, const float* grad_positions_device,
+                                                                float* grad_model_parameters_device, float* grad_offsets_device, void* cuda_stream);
+int mb2_character_joint_parameters_to_positions_backward_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                                int32_t num_points, const int32_t* parents, const float* offsets_device,
+                                                                int32_t offsets_batched, const float* grad_positions_device,
+                                                                float* grad_joint_parameters_device, float* grad_offsets_device, void* cuda_stream);
+
 /* Linear-blend skinning of the character (SkinWeights, skin_weights.h:19-40, and Character::inverseBindPose), host arrays, replacing
  * any earlier skinning: rest_vertices [V][3], skin_index / skin_weight [V][8] (a vertex's influences end at its first zero weight,
  * linear_skinning.cpp:76-80; the slots after it are ignored whatever they hold), inverse_bind_pose [J][12] (the row-major top 3x4 of

@@ -1146,6 +1146,77 @@ int mb2_character_skeleton_state_to_joint_parameters_backward_device(const mb2_c
 }
 
 namespace {
+// both directions and both variants of mb2_character_*_parameters_to_positions*_device; positions is the forward's output, gradPositions
+// the backward's input
+int positionsDevice(const mb2_character* c, int32_t batch, const float* params, int32_t numPoints, const int32_t* parents, const float* offsets,
+                    int32_t offsetsBatched, float* positions, const float* gradPositions, float* gradParams, float* gradOffsets, void* stream,
+                    bool backward, bool joint) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(batch >= 0, "batch must not be negative");
+  std::vector<int32_t> points;
+  const std::string rejected = makePointTables(c->host.numJoints, numPoints, parents, points);
+  MB2_CHECK(rejected.empty(), rejected);
+  MB2_CHECK(!backward || gradParams != nullptr || gradOffsets != nullptr, "positions backward: grad_params and grad_offsets are both null");
+  if (batch == 0) return MB2_OK;
+  MB2_CHECK(params != nullptr && (numPoints == 0 || (offsets != nullptr && (backward ? gradPositions != nullptr : positions != nullptr))), "null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(onDevice(c->device, {params}, {offsets, positions, gradPositions, gradParams, gradOffsets}),
+            "positions: every array must be device memory on the character's device");
+  NvtxRange range(joint ? (backward ? "jointParametersToPositionsBackward" : "jointParametersToPositions")
+                        : (backward ? "modelParametersToPositionsBackward" : "modelParametersToPositions"));
+  const cudaStream_t s = (cudaStream_t)stream;
+  PositionArgs a{};
+  a.T = c->tables();
+  a.S = c->skeletonTables();
+  a.numChildren = int(c->host.children.size());
+  a.batch = batch;
+  a.params = params;
+  a.offsets = offsets;
+  a.offsetsBatched = offsetsBatched != 0;
+  a.positions = positions;
+  a.gradPositions = gradPositions;
+  a.gradParams = gradParams;
+  a.gradOffsets = gradOffsets;
+  a.fromJointParameters = joint;
+  int32_t* dPoints = nullptr;
+  if (numPoints > 0) MB2_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&dPoints), points.size() * sizeof(int32_t), s));
+  a.P = pointTablesAt(dPoints, c->host.numJoints, numPoints);
+  cudaError_t e = numPoints > 0 ? cudaMemcpyAsync(dPoints, points.data(), points.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s) : cudaSuccess;
+  if (e == cudaSuccess) e = backward ? launchPositionsBackward(a, s) : launchPositions(a, s);
+  const cudaError_t f = numPoints > 0 ? cudaFreeAsync(dPoints, s) : cudaSuccess;
+  MB2_CUDA(e != cudaSuccess ? e : f);
+  return MB2_OK;
+}
+} // namespace
+
+int mb2_character_model_parameters_to_positions_device(const mb2_character* c, int32_t batch, const float* model_parameters_device, int32_t num_points,
+                                                       const int32_t* parents, const float* offsets_device, int32_t offsets_batched,
+                                                       float* positions_device, void* cuda_stream) {
+  return positionsDevice(c, batch, model_parameters_device, num_points, parents, offsets_device, offsets_batched, positions_device, nullptr, nullptr,
+                         nullptr, cuda_stream, false, false);
+}
+int mb2_character_joint_parameters_to_positions_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device, int32_t num_points,
+                                                       const int32_t* parents, const float* offsets_device, int32_t offsets_batched,
+                                                       float* positions_device, void* cuda_stream) {
+  return positionsDevice(c, batch, joint_parameters_device, num_points, parents, offsets_device, offsets_batched, positions_device, nullptr, nullptr,
+                         nullptr, cuda_stream, false, true);
+}
+int mb2_character_model_parameters_to_positions_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                                int32_t num_points, const int32_t* parents, const float* offsets_device,
+                                                                int32_t offsets_batched, const float* grad_positions_device,
+                                                                float* grad_model_parameters_device, float* grad_offsets_device, void* cuda_stream) {
+  return positionsDevice(c, batch, model_parameters_device, num_points, parents, offsets_device, offsets_batched, nullptr, grad_positions_device,
+                         grad_model_parameters_device, grad_offsets_device, cuda_stream, true, false);
+}
+int mb2_character_joint_parameters_to_positions_backward_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                                int32_t num_points, const int32_t* parents, const float* offsets_device,
+                                                                int32_t offsets_batched, const float* grad_positions_device,
+                                                                float* grad_joint_parameters_device, float* grad_offsets_device, void* cuda_stream) {
+  return positionsDevice(c, batch, joint_parameters_device, num_points, parents, offsets_device, offsets_batched, nullptr, grad_positions_device,
+                         grad_joint_parameters_device, grad_offsets_device, cuda_stream, true, true);
+}
+
+namespace {
 // both directions of mb2_character_skin_points*_device: checks the arguments and fills the kernel arguments except the outputs
 int skinArgs(const mb2_character* c, int32_t batch, const float* skelState, const float* restPoints, int32_t restBatched, SkinArgs& a) {
   MB2_CHECK(c != nullptr, "null character");

@@ -286,6 +286,41 @@ MB2_HD float skelGradModelParameter(const SkeletonTables& S, const float* gjp, i
   return s;
 }
 
+// ---- Points fixed in joints' frames (pymomentum jointParametersToPositions, tensor_joint_parameters_to_positions.cpp:33-119) ----------
+// Point i on joint a (ps: a's world state): p_i = t_a + d_i with d_i = rot(q_a, s_a off_i), the position constraint's point
+// (transform.h:193-195). A point moves rigidly with its joint, so its backward is the skeleton-state backward seeded from the points
+// instead of a state gradient: joint a's own term is S_g = sum g_i, R = sum d_i x g_i, D = sum d_i . g_i, S_c = S_s = 0. d_i is the
+// rotated and scaled offset, never p_i - t_a, which cancels catastrophically for a rig far from the origin.
+MB2_HD F3 pointRelative(const float* ps, F3 off) { return qrot(ld4(ps + 3), ps[7] * off); }
+// dLoss / d off_i = s_a R_a^T g_i
+MB2_HD F3 pointOffsetGradient(const float* ps, F3 g) { return ps[7] * qrot(qconj(ld4(ps + 3)), g); }
+// joint a's seed in skelGradSeed's layout from its own points, in the order of P.pointIndex; off [N][3], g [N][3] dLoss / d p
+MB2_HD void pointGradSeed(const PointTables& P, const float* js, int a, const float* off, const float* g, float* acc) {
+  const float* ps = js + a * kJointStateStride;
+  F3 sg = f3(0.f, 0.f, 0.f), r = sg;
+  float d = 0.f;
+#pragma unroll 1
+  for (int k = P.pointStart[a]; k < P.pointStart[a + 1]; ++k) {
+    const int i = P.pointIndex[k];
+    const F3 di = pointRelative(ps, ld3(off + 3 * i)), gi = ld3(g + 3 * i);
+    sg = sg + gi;
+    r = r + cross(di, gi);
+    d = d + dot(di, gi);
+  }
+  float* A = acc + a * kSkelAccStride;
+  A[0] = sg.x; A[1] = sg.y; A[2] = sg.z;
+  A[3] = r.x; A[4] = r.y; A[5] = r.z; A[6] = d;
+  A[7] = 0.f; A[8] = 0.f; A[9] = 0.f; A[10] = 0.f;
+}
+// A gradient of an input shared by the batch (skin_points' rest points, the positions' offsets) is the batch sum of per-instance terms:
+// summed in instance order within chunks of this many instances, at most kBatchSumChunks of them, then chunk by chunk in order. The
+// chunking depends on the batch size only.
+constexpr int kBatchSumChunks = 128;
+MB2_HD int batchSumChunk(int batch) {
+  const int c = batch / kBatchSumChunks + (batch % kBatchSumChunks != 0);
+  return c > 8 ? c : 8;
+}
+
 // ---- Joint parameters <-> local and world skeleton states, one joint at a time (pymomentum tensor_skeleton_state.cpp:139-185, :346-498,
 // :589-668, tensor_transforms.cpp:86-164, tensor_quaternion.cpp:179-230) ----------------------------------------------------------------
 // The local state of joint j from its seven parameters is fkLocalFromParameters. Its backward, from the kDeriv local state ls (the DOF
@@ -554,15 +589,11 @@ MB2_HD void fkPasses(const Lanes& g, const CharacterTables& C, const float* src,
     for (int i = g.lane; i < 3 * C.numJoints; i += g.size) fkAxis(C, i / 3, i % 3, js);
 }
 
-// The skeleton-state backward of one instance, right after fkPasses<true> (fkAxis writes only the axes and the seed reads only t, q, s:
-// the seed shares the axes' barrier): every joint seeds its subtree sums from the upstream gradient grad [J][8], the levels from the
-// deepest up fold in their children, lanes = joint-parameter rows into gjp [7 J], lanes = model parameters into out [n] (out == nullptr:
-// stops after gjp). Ends without a barrier.
+// The tail of the skeleton-state backward of one instance, once every joint's seed is in acc and a barrier has passed: the levels from
+// the deepest up fold in their children, lanes = joint-parameter rows into gjp [7 J], lanes = model parameters into out [n]
+// (out == nullptr: stops after gjp). Ends without a barrier.
 template <class Lanes>
-MB2_HD void skelGradPasses(const Lanes& g, const CharacterTables& C, const SkeletonTables& S, const float* js, const float* grad, float* acc,
-                           float* gjp, float* out) {
-  for (int i = g.lane; i < C.numJoints; i += g.size) skelGradSeed(js, i, grad + 8 * i, acc);
-  g.sync();
+MB2_HD void skelGradTail(const Lanes& g, const CharacterTables& C, const SkeletonTables& S, const float* js, float* acc, float* gjp, float* out) {
   for (int lvl = C.numLevels - 2; lvl >= 0; --lvl) { // the deepest level has no children
     const int end = C.levelStart[lvl + 1];
     for (int k = C.levelStart[lvl] + g.lane; k < end; k += g.size) skelGradFold(S, js, C.levelJoints[k], acc);
@@ -572,6 +603,45 @@ MB2_HD void skelGradPasses(const Lanes& g, const CharacterTables& C, const Skele
   if (out == nullptr) return; // the joint-parameter gradient is the result (joint_parameters_to_skeleton_state)
   g.sync();
   for (int p = g.lane; p < C.numParams; p += g.size) out[p] = skelGradModelParameter(S, gjp, p);
+}
+
+// The skeleton-state backward of one instance, right after fkPasses<true> (fkAxis writes only the axes and the seed reads only t, q, s:
+// the seed shares the axes' barrier): every joint seeds its subtree sums from the upstream gradient grad [J][8], then skelGradTail.
+template <class Lanes>
+MB2_HD void skelGradPasses(const Lanes& g, const CharacterTables& C, const SkeletonTables& S, const float* js, const float* grad, float* acc,
+                           float* gjp, float* out) {
+  for (int i = g.lane; i < C.numJoints; i += g.size) skelGradSeed(js, i, grad + 8 * i, acc);
+  g.sync();
+  skelGradTail(g, C, S, js, acc, gjp, out);
+}
+
+// The positions [N][3] of one instance's points with offsets off [N][3], lanes = points, once fkPasses<false> has ended (with its
+// barrier). Ends without a barrier.
+template <class Lanes>
+MB2_HD void positionPasses(const Lanes& g, const PointTables& P, const float* js, const float* off, float* out) {
+  for (int i = g.lane; i < P.numPoints; i += g.size) {
+    const float* ps = js + P.parent[i] * kJointStateStride;
+    const F3 p = ld3(ps) + pointRelative(ps, ld3(off + 3 * i));
+    out[3 * i] = p.x; out[3 * i + 1] = p.y; out[3 * i + 2] = p.z;
+  }
+}
+
+// Their backward from grad [N][3], right after fkPasses<true>: lanes = points write dLoss / d off into gOff [N][3] (when set), and every
+// joint seeds its subtree sums from its points (when gjp is set), both reading only t, q, s, so they share the axes' barrier; then
+// skelGradTail into gjp and out. Ends without a barrier.
+template <class Lanes>
+MB2_HD void positionGradPasses(const Lanes& g, const CharacterTables& C, const SkeletonTables& S, const PointTables& P, const float* js,
+                               const float* off, const float* grad, float* acc, float* gjp, float* out, float* gOff) {
+  if (gOff != nullptr)
+#pragma unroll 1
+    for (int i = g.lane; i < P.numPoints; i += g.size) {
+      const F3 r = pointOffsetGradient(js + P.parent[i] * kJointStateStride, ld3(grad + 3 * i));
+      gOff[3 * i] = r.x; gOff[3 * i + 1] = r.y; gOff[3 * i + 2] = r.z;
+    }
+  if (gjp == nullptr) return;
+  for (int j = g.lane; j < C.numJoints; j += g.size) pointGradSeed(P, js, j, off, grad, acc);
+  g.sync();
+  skelGradTail(g, C, S, js, acc, gjp, out);
 }
 
 // The joint motions of one instance under the parameter direction v (js: world state and DOF axes, complete): every joint's own share,

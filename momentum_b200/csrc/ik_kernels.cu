@@ -261,10 +261,9 @@ size_t skeletonStateSmemPerInstance(const CharacterTables& C, bool backward, boo
   return sizeof(float) * skeletonStateSmemPerInstanceFloats(C.numJoints, C.numParams, backward, joint);
 }
 
-size_t skeletonStateTableBytes(const SkeletonStateArgs& a, bool backward, bool joint) {
-  const CharacterTables& C = a.T;
+size_t skeletonStateTableBytes(const CharacterTables& C, int numChildren, bool backward, bool joint) {
   size_t w = characterTableWords(C);
-  if (backward) w += tableWords(C.numJoints + 1, 4) + tableWords(a.numChildren, 4);
+  if (backward) w += tableWords(C.numJoints + 1, 4) + tableWords(numChildren, 4);
   if (backward && !joint) w += tableWords(C.numParams + 1, 4) + tableWords(C.ptNnz, 4) * 2;
   return w * 4;
 }
@@ -359,7 +358,7 @@ cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaS
       {{skeletonStateKernel<false, 1, true>, skeletonStateKernel<false, 2, true>, skeletonStateKernel<false, 4, true>, skeletonStateKernel<false, 8, true>},
        {skeletonStateKernel<true, 1, true>, skeletonStateKernel<true, 2, true>, skeletonStateKernel<true, 4, true>, skeletonStateKernel<true, 8, true>}}};
   const bool joint = a.fromJointParameters != 0;
-  return launchInstanceGroups(kernels[joint][backward], a, skeletonStateSmemPerInstance(a.T, backward, joint), skeletonStateTableBytes(a, backward, joint),
+  return launchInstanceGroups(kernels[joint][backward], a, skeletonStateSmemPerInstance(a.T, backward, joint), skeletonStateTableBytes(a.T, a.numChildren, backward, joint),
                               stream);
 }
 
@@ -425,7 +424,7 @@ cudaError_t forEachInstanceSlice(int batch, size_t perInstance, cudaStream_t str
 //   skinVertexKernel<kMode>  a persistent grid of work items (instances, vertex range): per instance the CTA writes the J skinning
 //                            transforms M_j = T_j o IBP_j to shared memory, then lanes = vertices blend. kMode 0: points [B][V][3];
 //                            1: rest-point gradient per instance; 2: rest-point gradient summed over a fixed chunk of instances, in
-//                            instance order, into one row of bounded scratch (the chunks are summed in order by skinChunkSumKernel).
+//                            instance order, into one row of bounded scratch (the chunks are summed in order by rowGroupSumKernel).
 //   skinStatePartialKernel   one warp per (instance, segment of a joint's influence list): lanes = influences, then a butterfly sum
 //                            of the 12 floats (a_j, E_j) to scratch.
 //   skinStateFinishKernel    lanes = (instance, joint): the joint's segments summed in order, then skinStateGradient.
@@ -434,7 +433,6 @@ cudaError_t forEachInstanceSlice(int batch, size_t perInstance, cudaStream_t str
 constexpr int kSkinThreads = 256;
 constexpr int kSkinVertsPerThread = 4;                              // kMode 2 keeps their sums in registers
 constexpr int kSkinChunkVerts = kSkinThreads * kSkinVertsPerThread; // vertex range of a kMode 2 work item
-constexpr int kSkinMaxBatchChunks = 128;                            // kMode 2 scratch: at most 128 x [V][3] floats
 
 template <int kMode>
 __global__ void __launch_bounds__(kSkinThreads) skinVertexKernel(const SkinArgs a, int perChunk, int numChunks, int vSplit, int vLen, float* out) {
@@ -488,13 +486,24 @@ __global__ void __launch_bounds__(kSkinThreads) skinVertexKernel(const SkinArgs 
   }
 }
 
-__global__ void skinChunkSumKernel(const float* partial, int numChunks, size_t n, float* out) {
-  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
-    float s = partial[i];
-    for (int c = 1; c < numChunks; ++c) s += partial[size_t(c) * n + i];
+// rows [numRows][n] summed over groups of rowsPerGroup consecutive rows, each group in row order, into out [groups][n]: the batch sums of
+// a shared input's gradient (batchSumChunk), per chunk and then over the chunks
+__global__ void rowGroupSumKernel(const float* rows, int numRows, int rowsPerGroup, size_t n, float* out) {
+  const size_t total = size_t((numRows + rowsPerGroup - 1) / rowsPerGroup) * n;
+  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += size_t(gridDim.x) * blockDim.x) {
+    const size_t r0 = i / n * rowsPerGroup, k = i % n, r1 = min(size_t(numRows), r0 + rowsPerGroup);
+    float s = rows[r0 * n + k];
+    for (size_t r = r0 + 1; r < r1; ++r) s += rows[r * n + k];
     out[i] = s;
   }
 }
+namespace {
+cudaError_t launchRowGroupSum(const float* rows, int numRows, int rowsPerGroup, size_t n, float* out, cudaStream_t stream) {
+  const size_t total = size_t((numRows + rowsPerGroup - 1) / rowsPerGroup) * n;
+  rowGroupSumKernel<<<unsigned(std::min<size_t>((total + kSkinThreads - 1) / kSkinThreads, 4096)), kSkinThreads, 0, stream>>>(rows, numRows, rowsPerGroup, n, out);
+  return cudaGetLastError();
+}
+} // namespace
 
 __global__ void __launch_bounds__(kSkinThreads) skinStatePartialKernel(const SkinArgs a, int b0, int nb, float* partial) {
   const SkinTables S = a.S;
@@ -584,7 +593,7 @@ cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream) {
   if (e != cudaSuccess || a.gradRest == nullptr) return e;
   if (a.restBatched) return launchSkinPerInstance<1>(a, a.gradRest, stream);
   // shared rest points: the batch sum over fixed chunks of instances (the chunking depends on the batch size only)
-  const int perChunk = std::max(8, (a.batch + kSkinMaxBatchChunks - 1) / kSkinMaxBatchChunks);
+  const int perChunk = batchSumChunk(a.batch);
   const int numChunks = (a.batch + perChunk - 1) / perChunk;
   const int vSplit = (V + kSkinChunkVerts - 1) / kSkinChunkVerts;
   const size_t n = size_t(V) * 3, smem = size_t(J) * kSkinIbpStride * sizeof(float);
@@ -601,9 +610,136 @@ cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream) {
   }
   if (numChunks > 1) {
     if (e == cudaSuccess) {
-      skinChunkSumKernel<<<unsigned(std::min<size_t>((n + kSkinThreads - 1) / kSkinThreads, 4096)), kSkinThreads, 0, stream>>>(partial, numChunks, n, a.gradRest);
-      e = cudaGetLastError();
+      e = launchRowGroupSum(partial, numChunks, numChunks, n, a.gradRest, stream);
     }
+    const cudaError_t f = cudaFreeAsync(partial, stream);
+    if (e == cudaSuccess) e = f;
+  }
+  return e;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Positions of points fixed in joints' frames (ik_device.cuh positionPasses / positionGradPasses), in the per-instance frame of
+// skeletonStateKernel: its shared memory per instance, its tables and its launch (launchInstanceGroups), then lanes = points. The point
+// tables (each point's joint; backward: the points by joint) follow the character tables in shared memory when staging them costs no
+// instance per CTA, else they are read from global memory.
+//   forward:   fkPasses, then lanes = points: p = t + rot(q, s off), [N][3] out
+//   backward:  fkPasses with the DOF axes, then lanes = points write the per-instance offset gradient s rot(conj(q), g), and lanes =
+//              joints seed their subtree sums from their own points in index order; then the tail of skelGradPasses.
+// Shared offsets: their gradient is the batch sum of the per-instance rows, per chunk of batchSumChunk(B) instances in order and then
+// over the chunks in order (rowGroupSumKernel). The rows of a slice of whole chunks go to bounded scratch. No atomics, and no result
+// depends on the slicing or the launch shape.
+// ------------------------------------------------------------------------------------------------
+size_t pointTableBytes(const PointTables& P, int J, bool backward) {
+  size_t w = tableWords(P.numPoints, 4);
+  if (backward) w += tableWords(size_t(J) + 1, 4) + tableWords(P.numPoints, 4);
+  return w * 4;
+}
+
+// kStagePoints: a template parameter rather than a run-time branch, so that the staged point tables are provably shared-memory addresses
+template <bool kBackward, int W, bool kJoint, bool kStagePoints>
+__global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) positionsKernel(const PositionArgs a) {
+  extern __shared__ __align__(16) float smem[];
+  CharacterTables T = a.T;
+  SkeletonTables S = a.S;
+  PointTables P = a.P;
+  const WarpLanes<W> g = WarpLanes<W>::of(threadIdx.x >> 5, threadIdx.x & 31);
+  const int groupsPerCta = (blockDim.x >> 5) / W;
+  const int J = T.numJoints, n = T.numParams, N = P.numPoints;
+  const int inN = kJoint ? J * kParametersPerJoint : n; // floats per instance of the input
+  const int thF = int(skelAligned(inN)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
+  const int accF = kBackward ? int(skelAligned(size_t(J) * kSkelAccStride)) : 0;
+  const int perGroup = int(skeletonStateSmemPerInstanceFloats(J, n, kBackward, kJoint));
+  float* th = smem + size_t(g.group) * perGroup;
+  float* js = th + thF;
+  float* acc = js + jsF;
+  float* gjp = acc + accF;
+  {
+    uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
+    stageCharacterTables(T, cursor);
+    if constexpr (kBackward) {
+      stageTable(S.childStart, size_t(J) + 1, cursor); stageTable(S.children, a.numChildren, cursor);
+      if constexpr (!kJoint) { stageTable(S.ptColStart, n + 1, cursor); stageTable(S.ptColRows, T.ptNnz, cursor); stageTable(S.ptColVals, T.ptNnz, cursor); }
+    }
+    if constexpr (kStagePoints) {
+      stageTable(P.parent, N, cursor);
+      if constexpr (kBackward) { stageTable(P.pointStart, size_t(J) + 1, cursor); stageTable(P.pointIndex, N, cursor); }
+    }
+    __syncthreads();
+  }
+  for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
+    const float* src = a.params + size_t(b) * inN;
+    for (int i = g.lane; i < inN; i += g.size) th[i] = src[i];
+    g.sync();
+    fkPasses<kBackward, kJoint>(g, T, th, js);
+    const float* off = a.offsets + (a.offsetsBatched ? size_t(b) * N * 3 : 0);
+    if constexpr (!kBackward) {
+      positionPasses(g, P, js, off, a.positions + size_t(b) * N * 3);
+    } else {
+      // the joint-parameter gradient is the result from joint parameters, else the model-parameter gradient's intermediate
+      float* gp = a.gradParams != nullptr ? a.gradParams + size_t(b) * inN : nullptr;
+      float* gOff = a.gradOffsets != nullptr ? a.gradOffsets + size_t(b) * N * 3 : nullptr;
+      positionGradPasses(g, T, S, P, js, off, a.gradPositions + size_t(b) * N * 3, acc, kJoint || gp == nullptr ? gp : gjp, kJoint ? nullptr : gp, gOff);
+    }
+    g.sync(); // the next instance overwrites th / js / gjp
+  }
+}
+
+namespace {
+cudaError_t launchPositionsKernel(const PositionArgs& a, bool backward, cudaStream_t stream) {
+  using K = void (*)(PositionArgs);
+#define MB2_POSITION_KERNELS(B, J, S) {positionsKernel<B, 1, J, S>, positionsKernel<B, 2, J, S>, positionsKernel<B, 4, J, S>, positionsKernel<B, 8, J, S>}
+  static const K kernels[2][2][2][4] = {
+      {{MB2_POSITION_KERNELS(false, false, false), MB2_POSITION_KERNELS(false, false, true)},
+       {MB2_POSITION_KERNELS(true, false, false), MB2_POSITION_KERNELS(true, false, true)}},
+      {{MB2_POSITION_KERNELS(false, true, false), MB2_POSITION_KERNELS(false, true, true)},
+       {MB2_POSITION_KERNELS(true, true, false), MB2_POSITION_KERNELS(true, true, true)}}};
+#undef MB2_POSITION_KERNELS
+  const bool joint = a.fromJointParameters != 0;
+  const size_t per = skeletonStateSmemPerInstance(a.T, backward, joint);
+  const size_t tables = skeletonStateTableBytes(a.T, a.numChildren, backward, joint), points = pointTableBytes(a.P, a.T.numJoints, backward);
+  // instance groups per CTA as launchInstanceGroups counts them
+  auto groups = [&](size_t t) { return t + 16 + per > size_t(g_maxSmemOptin) ? 0 : std::min<size_t>((g_maxSmemOptin - t - 16) / per, kSkelMaxWarps); };
+  const bool stage = groups(tables + points) >= groups(tables);
+  return launchInstanceGroups(kernels[joint][backward][stage], a, per, tables + (stage ? points : 0), stream);
+}
+} // namespace
+
+cudaError_t launchPositions(const PositionArgs& a, cudaStream_t stream) {
+  if (a.batch <= 0 || a.P.numPoints == 0) return cudaSuccess;
+  return launchPositionsKernel(a, false, stream);
+}
+
+cudaError_t launchPositionsBackward(const PositionArgs& a, cudaStream_t stream) {
+  if (a.batch <= 0) return cudaSuccess;
+  const size_t inN = a.fromJointParameters ? size_t(a.T.numJoints) * kParametersPerJoint : size_t(a.T.numParams);
+  const size_t n3 = size_t(a.P.numPoints) * 3;
+  if (n3 == 0) // no point: the parameter gradient is zero and the offset gradient empty
+    return a.gradParams != nullptr ? cudaMemsetAsync(a.gradParams, 0, size_t(a.batch) * inN * sizeof(float), stream) : cudaSuccess;
+  if (a.gradOffsets == nullptr || a.offsetsBatched) return launchPositionsKernel(a, true, stream);
+  const int perChunk = batchSumChunk(a.batch);
+  const int numChunks = (a.batch + perChunk - 1) / perChunk;
+  float* partial = a.gradOffsets;
+  cudaError_t e = cudaSuccess;
+  if (numChunks > 1) {
+    e = cudaMallocAsync(reinterpret_cast<void**>(&partial), n3 * numChunks * sizeof(float), stream);
+    if (e != cudaSuccess) return e;
+  }
+  // slices of whole chunks: the instances b0 .. b0 + nb write their offset-gradient rows to scratch, summed per chunk into partial
+  e = forEachInstanceSlice(numChunks, size_t(perChunk) * n3 * sizeof(float), stream, [&](float* rows, int, int c0, int nc) {
+    const int b0 = c0 * perChunk, nb = std::min(nc * perChunk, a.batch - b0);
+    PositionArgs s = a;
+    s.batch = nb;
+    s.params += size_t(b0) * inN;
+    s.gradPositions += size_t(b0) * n3;
+    if (s.gradParams != nullptr) s.gradParams += size_t(b0) * inN;
+    s.gradOffsets = rows;
+    cudaError_t r = launchPositionsKernel(s, true, stream);
+    if (r == cudaSuccess) r = launchRowGroupSum(rows, nb, perChunk, n3, partial + size_t(c0) * n3, stream);
+    return r;
+  });
+  if (numChunks > 1) {
+    if (e == cudaSuccess) e = launchRowGroupSum(partial, numChunks, numChunks, n3, a.gradOffsets, stream);
     const cudaError_t f = cudaFreeAsync(partial, stream);
     if (e == cudaSuccess) e = f;
   }

@@ -151,6 +151,27 @@ struct SkeletonStateArgs {
   int32_t fromJointParameters; // joint_parameters_to_skeleton_state: the FK from joint parameters, S.ptCol* unused
 };
 cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream);
+// positionsKernel<kBackward>: pymomentum's model_parameters_to_positions / joint_parameters_to_positions for a batch on the character
+// alone, and their backward
+struct PositionArgs {
+  CharacterTables T;
+  SkeletonTables S;          // backward only
+  PointTables P;             // device memory
+  int32_t numChildren;       // entries of S.children
+  int32_t batch;
+  const float* params;       // [B][n], or [B][7 J] joint parameters when fromJointParameters
+  const float* offsets;      // [N][3] shared by the batch, or [B][N][3] when offsetsBatched
+  int32_t offsetsBatched;
+  float* positions;          // forward: [B][N][3]
+  const float* gradPositions; // backward: [B][N][3] dLoss / d positions
+  float* gradParams;         // backward, optional: [B][n] ([B][7 J]), overwritten
+  float* gradOffsets;        // backward, optional: [N][3] (the batch sum) or [B][N][3], overwritten
+  int32_t fromJointParameters;
+};
+// Both enqueue on `stream`. The backward of shared offsets takes stream-ordered scratch (cudaMallocAsync) for the per-instance offset
+// gradients of a slice of instances (at most 256 MiB) and 128 x [N][3] floats for their chunk sums.
+cudaError_t launchPositions(const PositionArgs& a, cudaStream_t stream);
+cudaError_t launchPositionsBackward(const PositionArgs& a, cudaStream_t stream);
 // parameterTransformKernel ... worldToJointParametersBackwardKernel: the flat joint-parameter operations of ik_device.cuh jointOpElement
 // for a batch, forward or backward; arrays [B][...] dense, device memory
 struct JointOpArgs {

@@ -216,6 +216,24 @@ std::string makeMeshFaces(int32_t numVertices, int32_t numFaces, const int32_t* 
   return "";
 }
 
+std::string makePointTables(int32_t numJoints, int32_t numPoints, const int32_t* parents, std::vector<int32_t>& out) {
+  if (numPoints < 0) return "positions: the number of points must not be negative";
+  if (numPoints > 0 && parents == nullptr) return "positions: null parents";
+  for (int32_t i = 0; i < numPoints; ++i)
+    if (parents[i] < 0 || parents[i] >= numJoints) return "positions: a parent is outside [0, num_joints)";
+  const size_t N = size_t(numPoints), J = size_t(numJoints);
+  std::vector<int32_t> t(2 * N + J + 1, 0);
+  int32_t* start = t.data() + N;
+  int32_t* index = start + J + 1;
+  std::copy(parents, parents + N, t.begin());
+  for (size_t i = 0; i < N; ++i) ++start[parents[i] + 1];
+  for (size_t j = 0; j < J; ++j) start[j + 1] += start[j];
+  std::vector<int32_t> fill(start, start + J);
+  for (size_t i = 0; i < N; ++i) index[fill[parents[i]]++] = int32_t(i); // i ascending within a joint
+  out = std::move(t);
+  return "";
+}
+
 std::string makeMeshTree(const HostMeshFaces& faces, int32_t numVertices, const float* referencePositions, HostMeshTree& out) {
   if (faces.numFaces < 1) return "mesh tree: the mesh has no faces";
   if (numVertices != faces.numVertices) return "mesh tree: num_vertices differs from the mesh faces' num_vertices";

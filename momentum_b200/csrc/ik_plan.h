@@ -139,6 +139,14 @@ std::string makeBlendShape(int32_t numShapes, int32_t numVertices, const float* 
 // faces [F][3] over V vertices; V >= 1, F >= 0, 3 F within int32, every index in [0, V). Degenerate faces and faces that repeat an index
 // are accepted (they add a zero normal, and a repeated vertex counts once per corner).
 std::string makeMeshFaces(int32_t numVertices, int32_t numFaces, const int32_t* faces, HostMeshFaces& out);
+// The point tables of model / joint_parameters_to_positions for N points on the joints parents [N] (PointTables), in one array:
+// parents [N], then the points grouped by joint, pointStart [J+1] and pointIndex [N], point indices ascending within a joint. N >= 0;
+// a parent outside [0, J) is rejected (checkValidBoneIndex).
+std::string makePointTables(int32_t numJoints, int32_t numPoints, const int32_t* parents, std::vector<int32_t>& out);
+// PointTables over such an array (host or device memory)
+inline PointTables pointTablesAt(const int32_t* base, int32_t numJoints, int32_t numPoints) {
+  return PointTables{numPoints, base, base + numPoints, base + numPoints + numJoints + 1};
+}
 // The topology of a bounding-volume tree over `faces` (MeshTreeTables), built from the face centroids of referencePositions [V][3]: a
 // node's faces are ordered by (centroid along the longest axis of their centroid bounds, face index) and split at the median rounded
 // up to whole leaves (the first ceil(g / 2) kLeafFaces faces left, g = ceil(n / kLeafFaces)), until at most kLeafFaces are left, so

@@ -136,6 +136,15 @@ struct SkeletonTables {
   const float* ptColVals;    // [nnz]
 };
 
+// Points fixed in joints' frames (model / joint_parameters_to_positions), shared by the batch (makePointTables): each point's joint, and
+// the points grouped by joint (CSR), point indices ascending within a joint
+struct PointTables {
+  int32_t numPoints;
+  const int32_t* parent;     // [N] in [0, J)
+  const int32_t* pointStart; // [J+1] into pointIndex
+  const int32_t* pointIndex; // [N]
+};
+
 // The flat joint-parameter operations (ik_device.cuh jointOpElement), forward / backward:
 //   kJointOpParameterTransform  jp [7 J] = P theta + o (jointParameterRow)      /  g_theta [n] = P^T g_jp
 //   kJointOpLocalState          local states [J][8] of jp [J][7]                /  g_jp [J][7] of g_local [J][8]

@@ -104,6 +104,10 @@ CABI_SIGNATURES = {
     "mb2_character_local_skeleton_state_to_joint_parameters_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
     "mb2_character_skeleton_state_to_joint_parameters_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
     "mb2_character_skeleton_state_to_joint_parameters_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_model_parameters_to_positions_device": (_int, [_vp, _int32, _vp, _int32, _ip, _vp, _int32, _vp, _vp]),
+    "mb2_character_joint_parameters_to_positions_device": (_int, [_vp, _int32, _vp, _int32, _ip, _vp, _int32, _vp, _vp]),
+    "mb2_character_model_parameters_to_positions_backward_device": (_int, [_vp, _int32, _vp, _int32, _ip, _vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_joint_parameters_to_positions_backward_device": (_int, [_vp, _int32, _vp, _int32, _ip, _vp, _int32, _vp, _vp, _vp, _vp]),
     "mb2_character_set_skinning": (_int, [_vp, _int32, _fp, _ip, _fp, _fp]),
     "mb2_character_num_vertices": (_int32, [_vp]),
     "mb2_character_skin_points_device": (_int, [_vp, _int32, _vp, _vp, _int32, _vp, _vp]),
@@ -444,6 +448,27 @@ class DeviceCharacter(_Base):
         0 pointer is passed as null."""
         fn = getattr(self._L, JOINT_OPS[name][1 if backward else 0])
         self._check(fn(self._h, int(batch), *ptrs, stream))
+
+    def positions_device(self, joint: bool, batch: int, params_device_ptr: int, parents: np.ndarray, offsets_device_ptr: int, offsets_batched: bool,
+                         positions_device_ptr: int, stream: int = 0):
+        """World positions [B][N][3] of N points fixed in joints' frames from model parameters [B][n] (``joint``: joint parameters
+        [B][7 J]). ``parents``: an int32 host array [N] of joint indices; offsets [N][3], or [B][N][3] when ``offsets_batched``. float32
+        device memory on this character's device, enqueued on ``stream``."""
+        p = np.ascontiguousarray(parents, np.int32)
+        fn = self._L.mb2_character_joint_parameters_to_positions_device if joint else self._L.mb2_character_model_parameters_to_positions_device
+        self._check(fn(self._h, int(batch), params_device_ptr, int(p.size), p.ctypes.data_as(_ip), offsets_device_ptr, int(bool(offsets_batched)),
+                       positions_device_ptr, stream))
+
+    def positions_backward_device(self, joint: bool, batch: int, params_device_ptr: int, parents: np.ndarray, offsets_device_ptr: int,
+                                  offsets_batched: bool, grad_positions_device_ptr: int, grad_params_device_ptr: int, grad_offsets_device_ptr: int,
+                                  stream: int = 0):
+        """dLoss/d parameters and dLoss/d offsets (the offset layout; the batch sum when shared) from dLoss/d positions [B][N][3]. A 0
+        output pointer is skipped; not both."""
+        p = np.ascontiguousarray(parents, np.int32)
+        fn = (self._L.mb2_character_joint_parameters_to_positions_backward_device if joint
+              else self._L.mb2_character_model_parameters_to_positions_backward_device)
+        self._check(fn(self._h, int(batch), params_device_ptr, int(p.size), p.ctypes.data_as(_ip), offsets_device_ptr, int(bool(offsets_batched)),
+                       grad_positions_device_ptr, grad_params_device_ptr, grad_offsets_device_ptr, stream))
 
     def __del__(self):
         if getattr(self, "_h", None):

@@ -1,5 +1,6 @@
 """Differentiable forward kinematics on CUDA tensors: ``model_parameters_to_skeleton_state`` and the rest of pymomentum's skeleton-state
-family (``apply_parameter_transform``, joint parameters to world and local states, and back), then skinning, normals and closest points.
+family (``apply_parameter_transform``, joint parameters to world and local states, and back, and the positions of points fixed in
+joints' frames), then skinning, normals and closest points.
 
 Mirror of ``pymomentum.geometry.model_parameters_to_skeleton_state`` (pymomentum/tensor_momentum/tensor_skeleton_state.cpp:500-502:
 ``jointParametersToSkeletonState(applyParamTransform(theta))``) for the batched device path. The forward pass is the solver's own FK
@@ -184,6 +185,116 @@ def skeleton_state_to_joint_parameters(character, skel_state: torch.Tensor) -> t
 
 local_skeleton_state_to_joint_parameters.__doc__ += _EULER_NOTE
 skeleton_state_to_joint_parameters.__doc__ += _EULER_NOTE
+
+
+class _Positions(torch.autograd.Function):
+    """model_parameters_to_positions (joint False) and joint_parameters_to_positions (joint True) on float32 rows, forward and backward on
+    the device; ``parents`` is the checked int32 host array."""
+
+    @staticmethod
+    def forward(ctx, dc, joint, params, parents, offsets):
+        dev = params.device
+        N = parents.shape[0]
+        rows = params.detach().to(torch.float32).reshape(-1, params.shape[-1]).contiguous()
+        B = rows.shape[0]
+        off = offsets.detach().to(torch.float32).contiguous()
+        batched = off.dim() == 3
+        out = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
+        if B * N > 0:
+            dc.positions_device(joint, B, rows.data_ptr(), parents, off.data_ptr(), batched, out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        ctx.dc, ctx.joint, ctx.parents, ctx.batched = dc, joint, parents, batched
+        ctx.params_shape, ctx.params_dtype, ctx.offsets_dtype = params.shape, params.dtype, offsets.dtype
+        ctx.save_for_backward(rows, off)
+        return out.reshape(*params.shape[:-1], N, 3).to(params.dtype)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_positions):
+        rows, off = ctx.saved_tensors
+        B, N = rows.shape[0], ctx.parents.shape[0]
+        dev = rows.device
+        need_params, need_offsets = ctx.needs_input_grad[2], ctx.needs_input_grad[4]
+        gp = torch.zeros_like(rows) if need_params else None
+        go = torch.zeros_like(off) if need_offsets else None
+        if B * N > 0 and (need_params or need_offsets):  # else the gradients are zero
+            g = grad_positions.to(device=dev, dtype=torch.float32).reshape(B, N, 3).contiguous()
+            ctx.dc.positions_backward_device(ctx.joint, B, rows.data_ptr(), ctx.parents, off.data_ptr(), ctx.batched, g.data_ptr(),
+                                             0 if gp is None else gp.data_ptr(), 0 if go is None else go.data_ptr(),
+                                             torch.cuda.current_stream(dev).cuda_stream)
+        return (None, None, None if gp is None else gp.reshape(ctx.params_shape).to(ctx.params_dtype), None,
+                None if go is None else go.to(ctx.offsets_dtype))
+
+
+def _point_parents(name, parents, J):
+    """parents as a checked int32 host array [N]: a sequence, a numpy array or an integer tensor (a CUDA tensor is copied to the host)."""
+    if torch.is_tensor(parents):
+        if parents.dtype.is_floating_point or parents.dtype.is_complex or parents.dtype == torch.bool:
+            raise ValueError(f"{name}: parents must hold integer joint indices, got {parents.dtype}")
+        p = parents.detach().cpu().numpy()
+    else:
+        p = np.asarray(parents)
+        if p.size == 0:
+            p = p.astype(np.int32)
+        if not np.issubdtype(p.dtype, np.integer):
+            raise ValueError(f"{name}: parents must hold integer joint indices, got {p.dtype}")
+    if p.ndim != 1:
+        raise ValueError(f"{name}: parents must be [N], got {tuple(p.shape)}")
+    if p.size and (p.min() < 0 or p.max() >= J):
+        raise ValueError(f"{name}: every parent must be a joint index in [0, {J})")
+    return np.ascontiguousarray(p, np.int32)
+
+
+def _positions(name, joint, character, params, parents, offsets, what, width):
+    """Checks the arguments before any library call, then runs the operation."""
+    if not torch.is_tensor(params):
+        raise ValueError(f"{name}: {what} must be a tensor")
+    if params.dim() not in (1, 2) or params.shape[-1] != width:
+        raise ValueError(f"{name}: {what} must be [{width}] or [B, {width}], got {tuple(params.shape)}")
+    ch, _ = _resolve(character)
+    p = _point_parents(name, parents, ch.num_joints)
+    N = p.shape[0]
+    if not torch.is_tensor(offsets) or not offsets.dtype.is_floating_point:
+        raise ValueError(f"{name}: offsets must be a floating-point tensor")
+    B = params.shape[0] if params.dim() == 2 else None
+    if not (offsets.shape == (N, 3) or (B is not None and offsets.shape == (B, N, 3))):
+        raise ValueError(f"{name}: offsets must be [N, 3] or [B, N, 3] with N = {N} and the parameters' B, got {tuple(offsets.shape)}")
+    if not params.is_cuda or not offsets.is_cuda:
+        raise ValueError(f"{name} runs on CUDA tensors (there is no CPU fallback)")
+    if offsets.device != params.device:
+        raise ValueError(f"{name}: offsets must be on the parameters' device")
+    return _Positions.apply(_device_character(character, params.device), joint, params, p, offsets)
+
+
+_POSITIONS_NOTE = """
+    ``parents`` [N] holds joint indices in [0, J): a sequence, a numpy array or an integer tensor. A CUDA tensor is copied to the host
+    once per call, which synchronises with its device. ``offsets`` is [N, 3], shared by the batch (its gradient is the batch sum), or
+    [B, N, 3] with the parameters' B. Point i is at t_a + rot(q_a, s_a offsets_i) for the world state (t_a, q_a, s_a) of joint
+    a = parents[i]. Returns [N, 3] or [B, N, 3] in the parameters' dtype, computed in float32. N = 0 gives an empty result and zero
+    gradients. Differentiable once with respect to the parameters and the offsets, not ``parents``. The backward seeds the skeleton-state
+    backward's subtree sums from the points, so it costs O(J + N) per instance whatever the depth of the joints."""
+
+
+def model_parameters_to_positions(character, model_parameters: torch.Tensor, parents, offsets: torch.Tensor) -> torch.Tensor:
+    """World positions of points fixed in joints' frames (pymomentum ``model_parameters_to_positions``): markers, keypoints or locators
+    of ``model_parameters`` ([n] or [B, n], on a CUDA device), without the [B, J, 8] skeleton state in memory. ``character`` is a
+    ``momentum_b200.character.Character`` or a ``solver.DeviceCharacter`` on the tensor's device.
+    """
+    ch, _ = _resolve(character)
+    return _positions("model_parameters_to_positions", False, character, model_parameters, parents, offsets, f"model_parameters (n = {ch.num_params})",
+                      ch.num_params)
+
+
+def joint_parameters_to_positions(character, joint_parameters: torch.Tensor, parents, offsets: torch.Tensor) -> torch.Tensor:
+    """``model_parameters_to_positions`` from flat joint parameters (pymomentum ``joint_parameters_to_positions``): [7 J] or [B, 7 J] on a
+    CUDA device, the layout of ``joint_parameters_to_skeleton_state``.
+    """
+    ch, _ = _resolve(character)
+    J = ch.num_joints
+    return _positions("joint_parameters_to_positions", True, character, joint_parameters, parents, offsets, f"joint_parameters (7 J = {7 * J})", 7 * J)
+
+
+model_parameters_to_positions.__doc__ += _POSITIONS_NOTE
+joint_parameters_to_positions.__doc__ += _POSITIONS_NOTE
 
 
 class _SkinPoints(torch.autograd.Function):
