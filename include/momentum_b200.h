@@ -272,6 +272,16 @@ int mb2_character_apply_parameter_transform_device(const mb2_character* c, int32
                                                    float* joint_parameters_device, void* cuda_stream);
 int mb2_character_apply_parameter_transform_backward_device(const mb2_character* c, int32_t batch, const float* grad_joint_parameters_device,
                                                             float* grad_model_parameters_device, void* cuda_stream);
+/* pymomentum apply_inverse_parameter_transform (diff_transform_pybind.cpp:44-59, tensor_parameter_transform.cpp:378-466):
+ * [B][7 J] -> theta = W (jp - o) [B][n], the offsets subtracted first, with W = P^+ the Moore-Penrose pseudo-inverse of
+ * InverseParameterTransform (inverse_parameter_transform.cpp:18-38) under its rule of utility.cpp:423-435: a singular value > 1e-6
+ * (absolute) is inverted, any other is 0. W is built once per character, in float64 per connected component of P's sparsity pattern, and
+ * rounded to float entry by entry. The `offsets` half of InverseParameterTransform::apply is not returned. Its backward is W^T, so it
+ * reads no input. */
+int mb2_character_apply_inverse_parameter_transform_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                           float* model_parameters_device, void* cuda_stream);
+int mb2_character_apply_inverse_parameter_transform_backward_device(const mb2_character* c, int32_t batch, const float* grad_model_parameters_device,
+                                                                    float* grad_joint_parameters_device, void* cuda_stream);
 /* pymomentum joint_parameters_to_skeleton_state (tensor_skeleton_state.cpp:203-343, :488-491): the forward kinematics of
  * mb2_character_skeleton_state_device from joint parameters [B][7 J] -> [B][J][8] */
 int mb2_character_joint_parameters_to_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,

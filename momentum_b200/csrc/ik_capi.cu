@@ -124,6 +124,8 @@ struct mb2_character {
   DeviceBuffer<float> offset, prerot, ptVals, ptOffsets;
   DeviceBuffer<int32_t> childStart, children, ptColStart, ptColRows; // skeleton-state backward (HostCharacter::buildBackwardTables)
   DeviceBuffer<float> ptColVals;
+  DeviceBuffer<int32_t> invStart, invRows, invRowStart, invParams; // inverse ParameterTransform (HostCharacter::buildInverseTables)
+  DeviceBuffer<float> invVals, invRowVals;
   uint64_t limitsVersion{0};
   // linear-blend skinning (mb2_character_set_skinning): numVertices == 0 when there is none
   HostSkinning skin;
@@ -249,7 +251,9 @@ CharacterTables mb2_character::tables() const {
   return C;
 }
 
-SkeletonTables mb2_character::skeletonTables() const { return SkeletonTables{childStart.p, children.p, ptColStart.p, ptColRows.p, ptColVals.p}; }
+SkeletonTables mb2_character::skeletonTables() const {
+  return SkeletonTables{childStart.p, children.p, ptColStart.p, ptColRows.p, ptColVals.p, invStart.p, invRows.p, invVals.p, invRowStart.p, invParams.p, invRowVals.p};
+}
 
 SkinTables mb2_character::skinTables() const {
   const SkinBuffers& d = *skinDev;
@@ -601,6 +605,12 @@ int mb2_character_create(int device, int32_t J, const int32_t* parents, const fl
   MB2_CUDA(c->ptColStart.upload(h.ptColStart, nullptr));
   MB2_CUDA(c->ptColRows.upload(h.ptColRows, nullptr));
   MB2_CUDA(c->ptColVals.upload(h.ptColVals, nullptr));
+  MB2_CUDA(c->invStart.upload(h.invStart, nullptr));
+  MB2_CUDA(c->invRows.upload(h.invRows, nullptr));
+  MB2_CUDA(c->invVals.upload(h.invVals, nullptr));
+  MB2_CUDA(c->invRowStart.upload(h.invRowStart, nullptr));
+  MB2_CUDA(c->invParams.upload(h.invParams, nullptr));
+  MB2_CUDA(c->invRowVals.upload(h.invRowVals, nullptr));
   MB2_CUDA(cudaStreamSynchronize(nullptr));
   *out = c.release();
   return MB2_OK;
@@ -1060,14 +1070,14 @@ int skeletonStateDevice(const mb2_character* c, int32_t batch, const float* thet
   return MB2_OK;
 }
 
-// both directions of the flat joint-parameter operations (launchJointOp); `in` is optional only for the linear parameter transform's
-// backward, which does not read it
+// both directions of the flat joint-parameter operations (launchJointOp); `in` is optional only for the backward of the two linear
+// ParameterTransform ops, which do not read it
 int jointOpDevice(const mb2_character* c, int32_t batch, JointOp op, const char* name, const float* in, const float* grad, float* out, void* stream,
                   bool backward) {
   MB2_CHECK(c != nullptr, "null character");
   MB2_CHECK(batch >= 0, "batch must not be negative");
   if (batch == 0) return MB2_OK;
-  const bool needIn = !(backward && op == kJointOpParameterTransform);
+  const bool needIn = !(backward && (op == kJointOpParameterTransform || op == kJointOpInverseParameterTransform));
   MB2_CHECK((in != nullptr || !needIn) && out != nullptr && (!backward || grad != nullptr), "null argument");
   MB2_DEVICE_GUARD(c->device);
   MB2_CHECK(onDevice(c->device, {out}, {in, grad}), std::string(name) + ": every array must be device memory on the character's device");
@@ -1101,6 +1111,16 @@ int mb2_character_apply_parameter_transform_backward_device(const mb2_character*
                                                             float* grad_model_parameters_device, void* cuda_stream) {
   return jointOpDevice(c, batch, kJointOpParameterTransform, "applyParameterTransformBackward", nullptr, grad_joint_parameters_device, grad_model_parameters_device,
                        cuda_stream, true);
+}
+int mb2_character_apply_inverse_parameter_transform_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
+                                                           float* model_parameters_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpInverseParameterTransform, "applyInverseParameterTransform", joint_parameters_device, nullptr,
+                       model_parameters_device, cuda_stream, false);
+}
+int mb2_character_apply_inverse_parameter_transform_backward_device(const mb2_character* c, int32_t batch, const float* grad_model_parameters_device,
+                                                                    float* grad_joint_parameters_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpInverseParameterTransform, "applyInverseParameterTransformBackward", nullptr, grad_model_parameters_device,
+                       grad_joint_parameters_device, cuda_stream, true);
 }
 int mb2_character_joint_parameters_to_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
                                                             float* skeleton_state_device, void* cuda_stream) {

@@ -453,11 +453,30 @@ MB2_HD void worldStateGradient(const CharacterTables& T, const SkeletonTables& S
   }
 }
 
+// Model parameter p of the joint parameters jp [7 J] of one instance (InverseParameterTransform::apply,
+// inverse_parameter_transform.cpp:30-38): theta_p = sum_k W_pk (jp_k - o_k) over W's entries in table order, the offsets subtracted
+// before the product
+MB2_HD float inverseParameterRow(const CharacterTables& T, const SkeletonTables& S, int p, const float* jp) {
+  float s = 0.f;
+  for (int k = S.invStart[p]; k < S.invStart[p + 1]; ++k) {
+    const int r = S.invRows[k];
+    s += S.invVals[k] * (jp[r] - T.ptOffsets[r]);
+  }
+  return s;
+}
+// its backward for joint-parameter row r from dLoss / d theta [n]: (W^T g)_r over the row's entries, parameters ascending
+MB2_HD float inverseParameterGradient(const SkeletonTables& S, int r, const float* gTheta) {
+  float s = 0.f;
+  for (int k = S.invRowStart[r]; k < S.invRowStart[r + 1]; ++k) s += S.invRowVals[k] * gTheta[S.invParams[k]];
+  return s;
+}
+
 // The flat operations of a batch (JointOp), one element per thread: kOp's per-instance item count (rows, parameters or joints) and
 // element i of the batch, for input `in`, upstream gradient `grad` (backward) and output `out`, every array [B][...] dense.
 template <int kOp, bool kBackward>
 MB2_HD int jointOpItems(const CharacterTables& T) {
   if constexpr (kOp == kJointOpParameterTransform) return kBackward ? T.numParams : T.numJoints * kParametersPerJoint;
+  else if constexpr (kOp == kJointOpInverseParameterTransform) return kBackward ? T.numJoints * kParametersPerJoint : T.numParams;
   else return T.numJoints;
 }
 template <int kOp, bool kBackward>
@@ -468,6 +487,9 @@ MB2_HD void jointOpElement(const CharacterTables& T, const SkeletonTables& S, lo
   if constexpr (kOp == kJointOpParameterTransform) {
     if constexpr (kBackward) out[i] = skelGradModelParameter(S, grad + b * (7L * J), k);
     else out[i] = jointParameterRow(T, k, in + b * n);
+  } else if constexpr (kOp == kJointOpInverseParameterTransform) {
+    if constexpr (kBackward) out[i] = inverseParameterGradient(S, k, grad + b * n);
+    else out[i] = inverseParameterRow(T, S, k, in + b * (7L * J));
   } else if constexpr (kOp == kJointOpLocalState) {
     if constexpr (kBackward) {
       float ls[kJointStateStride];

@@ -384,14 +384,24 @@ __global__ void __launch_bounds__(kJointOpThreads) localToJointParametersKernel(
 __global__ void __launch_bounds__(kJointOpThreads) localToJointParametersBackwardKernel(const JointOpArgs a) { jointOpGrid<kJointOpFromLocal, true>(a); }
 __global__ void __launch_bounds__(kJointOpThreads) worldToJointParametersKernel(const JointOpArgs a) { jointOpGrid<kJointOpFromWorld, false>(a); }
 __global__ void __launch_bounds__(kJointOpThreads) worldToJointParametersBackwardKernel(const JointOpArgs a) { jointOpGrid<kJointOpFromWorld, true>(a); }
+__global__ void __launch_bounds__(kJointOpThreads) inverseParameterTransformKernel(const JointOpArgs a) {
+  jointOpGrid<kJointOpInverseParameterTransform, false>(a);
+}
+__global__ void __launch_bounds__(kJointOpThreads) inverseParameterTransformBackwardKernel(const JointOpArgs a) {
+  jointOpGrid<kJointOpInverseParameterTransform, true>(a);
+}
 
 cudaError_t launchJointOp(const JointOpArgs& a, JointOp op, bool backward, cudaStream_t stream) {
   using K = void (*)(JointOpArgs);
-  static const K kernels[4][2] = {{parameterTransformKernel, parameterTransformBackwardKernel}, {localStateKernel, localStateBackwardKernel},
+  static const K kernels[5][2] = {{parameterTransformKernel, parameterTransformBackwardKernel}, {localStateKernel, localStateBackwardKernel},
                                   {localToJointParametersKernel, localToJointParametersBackwardKernel},
-                                  {worldToJointParametersKernel, worldToJointParametersBackwardKernel}};
+                                  {worldToJointParametersKernel, worldToJointParametersBackwardKernel},
+                                  {inverseParameterTransformKernel, inverseParameterTransformBackwardKernel}};
   if (a.batch <= 0) return cudaSuccess;
-  const long per = op == kJointOpParameterTransform ? (backward ? a.T.numParams : long(a.T.numJoints) * kParametersPerJoint) : a.T.numJoints;
+  const long rows = long(a.T.numJoints) * kParametersPerJoint;
+  const long per = op == kJointOpParameterTransform          ? (backward ? a.T.numParams : rows)
+                   : op == kJointOpInverseParameterTransform ? (backward ? rows : a.T.numParams)
+                                                             : a.T.numJoints;
   const long items = long(a.batch) * per;
   if (items == 0) return cudaSuccess;
   const int grid = int(std::min<long>((items + kJointOpThreads - 1) / kJointOpThreads, long(std::max(g_numSms, 1)) * kJointOpCtasPerSm));

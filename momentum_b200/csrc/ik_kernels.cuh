@@ -172,13 +172,14 @@ struct PositionArgs {
 // gradients of a slice of instances (at most 256 MiB) and 128 x [N][3] floats for their chunk sums.
 cudaError_t launchPositions(const PositionArgs& a, cudaStream_t stream);
 cudaError_t launchPositionsBackward(const PositionArgs& a, cudaStream_t stream);
-// parameterTransformKernel ... worldToJointParametersBackwardKernel: the flat joint-parameter operations of ik_device.cuh jointOpElement
-// for a batch, forward or backward; arrays [B][...] dense, device memory
+// parameterTransformKernel ... inverseParameterTransformBackwardKernel: the flat joint-parameter operations of ik_device.cuh
+// jointOpElement for a batch, forward or backward; arrays [B][...] dense, device memory
 struct JointOpArgs {
   CharacterTables T;
-  SkeletonTables S;          // the backward of kJointOpParameterTransform (ptCol*) and of kJointOpFromWorld (children)
+  SkeletonTables S;          // the backward of kJointOpParameterTransform (ptCol*), of kJointOpFromWorld (children), and both directions
+                             // of kJointOpInverseParameterTransform (inv*)
   int32_t batch;
-  const float* in;           // the forward's input (backward: the forward's input, unused by the linear kJointOpParameterTransform)
+  const float* in;           // the forward's input (backward: the forward's input, unused by the two linear ParameterTransform ops)
   const float* grad;         // backward: dLoss / d the forward's output
   float* out;                // forward: the output; backward: dLoss / d in, overwritten
 };

@@ -5,6 +5,9 @@
 #include <cmath>
 #include <cstring>
 #include <map>
+#include <numeric>
+
+#include "ik_jacobi.cuh"
 
 namespace mb2 {
 
@@ -65,6 +68,149 @@ void HostCharacter::buildBackwardTables() {
     }
 }
 
+namespace {
+constexpr double kInverseSigmaTol = 1e-6;  // utility.cpp:423-435: a singular value is inverted when > 1e-6 (absolute), else 0
+constexpr int kInverseMaxSweeps = 64;      // cyclic Jacobi sweeps of one component's Gram matrix (it stops at the first sweep without a rotation)
+
+// W = A^+ [c][m] of the dense block A [m][c] (row-major), through the eigen-decomposition K = Q Lambda Q^T of the Gram matrix on A's
+// smaller side: c <= m: K = A^T A, W = Q Lambda^+ Q^T A^T; m < c: K = A A^T, W = A^T Q Lambda^+ Q^T. lambda = sigma^2 is inverted when
+// sigma > 1e-6, i.e. lambda > 1e-12. The rotations are ik_jacobi.cuh's (jacobiRotation, its skip floor), applied cyclically by rows.
+void blockPseudoInverse(const std::vector<double>& A, int m, int c, std::vector<double>& W) {
+  const bool colSide = c <= m;
+  const int k = colSide ? c : m;
+  std::vector<double> K(size_t(k) * k), Q(size_t(k) * k, 0.0);
+  for (int a = 0; a < k; ++a)
+    for (int b = a; b < k; ++b) {
+      double s = 0.0;
+      if (colSide)
+        for (int r = 0; r < m; ++r) s += A[size_t(r) * c + a] * A[size_t(r) * c + b];
+      else
+        for (int p = 0; p < c; ++p) s += A[size_t(a) * c + p] * A[size_t(b) * c + p];
+      K[size_t(a) * k + b] = K[size_t(b) * k + a] = s;
+    }
+  double maxDiagonal = 0.0;
+  for (int a = 0; a < k; ++a) {
+    Q[size_t(a) * k + a] = 1.0;
+    maxDiagonal = std::max(maxDiagonal, K[size_t(a) * k + a]);
+  }
+  const double floor = jacobiFloor(maxDiagonal);
+  for (int sweep = 0; sweep < kInverseMaxSweeps; ++sweep) {
+    bool rotated = false;
+    for (int p = 0; p < k; ++p)
+      for (int q = p + 1; q < k; ++q) {
+        double cs, sn, t;
+        if (!jacobiRotation(K[size_t(p) * k + p], K[size_t(q) * k + q], K[size_t(p) * k + q], floor, cs, sn, t)) continue;
+        rotated = true;
+        // K <- R^T K R (R_pp = R_qq = c, R_pq = s, R_qp = -s), Q <- Q R
+        const double apq = K[size_t(p) * k + q];
+        K[size_t(p) * k + p] -= t * apq;
+        K[size_t(q) * k + q] += t * apq;
+        K[size_t(p) * k + q] = K[size_t(q) * k + p] = 0.0;
+        for (int i = 0; i < k; ++i) {
+          if (i != p && i != q) {
+            const double kip = K[size_t(i) * k + p], kiq = K[size_t(i) * k + q];
+            K[size_t(i) * k + p] = K[size_t(p) * k + i] = cs * kip - sn * kiq;
+            K[size_t(i) * k + q] = K[size_t(q) * k + i] = sn * kip + cs * kiq;
+          }
+          const double qip = Q[size_t(i) * k + p], qiq = Q[size_t(i) * k + q];
+          Q[size_t(i) * k + p] = cs * qip - sn * qiq;
+          Q[size_t(i) * k + q] = sn * qip + cs * qiq;
+        }
+      }
+    if (!rotated) break;
+  }
+  // M = Q Lambda^+ Q^T [k][k]
+  std::vector<double> inv(k), M(size_t(k) * k, 0.0);
+  for (int a = 0; a < k; ++a) {
+    const double lambda = K[size_t(a) * k + a];
+    inv[a] = lambda > kInverseSigmaTol * kInverseSigmaTol ? 1.0 / lambda : 0.0;
+  }
+  for (int i = 0; i < k; ++i)
+    for (int j = 0; j < k; ++j) {
+      double s = 0.0;
+      for (int a = 0; a < k; ++a) s += Q[size_t(i) * k + a] * inv[a] * Q[size_t(j) * k + a];
+      M[size_t(i) * k + j] = s;
+    }
+  W.assign(size_t(c) * m, 0.0);
+  for (int p = 0; p < c; ++p)
+    for (int r = 0; r < m; ++r) {
+      double s = 0.0;
+      if (colSide)
+        for (int a = 0; a < c; ++a) s += M[size_t(p) * k + a] * A[size_t(r) * c + a]; // (M A^T)_pr
+      else
+        for (int a = 0; a < m; ++a) s += A[size_t(a) * c + p] * M[size_t(a) * k + r]; // (A^T M)_pr
+      W[size_t(p) * m + r] = s;
+    }
+}
+} // namespace
+
+// P is block-diagonal under the permutation that groups the connected components of its sparsity graph (joint-parameter rows and model
+// parameters, joined by every stored entry, stored zeros included). The pseudo-inverse of a block-diagonal matrix is the block-diagonal
+// matrix of the blocks' pseudo-inverses, and P's singular values are the union of the blocks', so the absolute 1e-6 rule truncates the
+// same values per block as for the whole matrix: W is the reference's matrix, computed per component. A parameter without entries is a
+// component of its own with an empty row of W. Entries that round to 0 are not stored.
+void HostCharacter::buildInverseTables() {
+  const int rows = numJoints * kParametersPerJoint, n = numParams;
+  std::vector<int32_t> root(size_t(rows) + n);
+  std::iota(root.begin(), root.end(), 0);
+  auto find = [&](int32_t x) {
+    while (root[x] != x) x = root[x] = root[root[x]];
+    return x;
+  };
+  for (int r = 0; r < rows; ++r)
+    for (int k = ptOuter[r]; k < ptOuter[r + 1]; ++k) {
+      const int32_t a = find(r), b = find(rows + ptInner[k]);
+      if (a != b) root[std::max(a, b)] = std::min(a, b);
+    }
+  // the rows and parameters of each component, both ascending
+  std::map<int32_t, std::pair<std::vector<int32_t>, std::vector<int32_t>>> comps;
+  for (int r = 0; r < rows; ++r) comps[find(r)].first.push_back(r);
+  for (int p = 0; p < n; ++p) comps[find(rows + p)].second.push_back(p);
+  std::vector<std::vector<std::pair<int32_t, float>>> byParam(n);
+  std::vector<double> A, W;
+  std::vector<int32_t> local(rows, -1);
+  for (const auto& kv : comps) {
+    const std::vector<int32_t>& cr = kv.second.first;
+    const std::vector<int32_t>& cp = kv.second.second;
+    const int m = int(cr.size()), c = int(cp.size());
+    if (m == 0 || c == 0) continue; // a parameter without entries, or rows no parameter drives
+    for (int i = 0; i < m; ++i) local[cr[i]] = i;
+    std::map<int32_t, int32_t> col;
+    for (int j = 0; j < c; ++j) col[cp[j]] = j;
+    A.assign(size_t(m) * c, 0.0);
+    for (int i = 0; i < m; ++i)
+      for (int k = ptOuter[cr[i]]; k < ptOuter[cr[i] + 1]; ++k) A[size_t(i) * c + col[ptInner[k]]] += double(ptVals[k]);
+    blockPseudoInverse(A, m, c, W);
+    for (int j = 0; j < c; ++j)
+      for (int i = 0; i < m; ++i) {
+        const float w = float(W[size_t(j) * m + i]);
+        if (w != 0.f) byParam[cp[j]].push_back({cr[i], w});
+      }
+  }
+  invStart.assign(n + 1, 0);
+  invRows.clear();
+  invVals.clear();
+  for (int p = 0; p < n; ++p) {
+    for (const auto& e : byParam[p]) {
+      invRows.push_back(e.first);
+      invVals.push_back(e.second);
+    }
+    invStart[p + 1] = int32_t(invRows.size());
+  }
+  invRowStart.assign(rows + 1, 0);
+  for (int32_t r : invRows) invRowStart[r + 1]++;
+  for (int r = 0; r < rows; ++r) invRowStart[r + 1] += invRowStart[r];
+  invParams.resize(invRows.size());
+  invRowVals.resize(invRows.size());
+  std::vector<int32_t> cursor(invRowStart.begin(), invRowStart.end() - 1);
+  for (int p = 0; p < n; ++p) // ascending parameters: each row's parameters in increasing order
+    for (int k = invStart[p]; k < invStart[p + 1]; ++k) {
+      const int at = cursor[invRows[k]]++;
+      invParams[at] = p;
+      invRowVals[at] = invVals[k];
+    }
+}
+
 std::vector<uint8_t> HostCharacter::computeActiveJointParams(const std::vector<uint8_t>& enabled) const {
   std::vector<uint8_t> r(size_t(numJoints) * kParametersPerJoint, 0);
   for (int row = 0; row < numJoints * kParametersPerJoint; ++row)
@@ -122,6 +268,7 @@ std::string makeCharacter(int32_t numJoints, const int32_t* parents, const float
   if (!err.empty()) return err;
   out.buildLevels();
   out.buildBackwardTables();
+  out.buildInverseTables();
   return "";
 }
 

@@ -38,9 +38,18 @@ struct HostCharacter {
   std::vector<int32_t> childStart, children;
   std::vector<int32_t> ptColStart, ptColRows;
   std::vector<float> ptColVals;
+  // the inverse ParameterTransform (buildInverseTables): the pseudo-inverse W = P^+ [n][7J], by model parameter (CSR, rows ascending
+  // within a parameter) and the same entries by joint-parameter row (CSR, parameters ascending within a row)
+  std::vector<int32_t> invStart, invRows;
+  std::vector<float> invVals;
+  std::vector<int32_t> invRowStart, invParams;
+  std::vector<float> invRowVals;
   std::string validate() const; // empty when fine (MT_CHECK-style message otherwise)
   void buildLevels();
   void buildBackwardTables();
+  // InverseParameterTransform's matrix (inverse_parameter_transform.cpp:18-38, utility.cpp:423-435), component by component of P's
+  // sparsity graph, in float64, each entry rounded to float once
+  void buildInverseTables();
   // ParameterTransformT::computeActiveJointParams (parameter_transform.cpp:97-107)
   std::vector<uint8_t> computeActiveJointParams(const std::vector<uint8_t>& enabled) const;
 };

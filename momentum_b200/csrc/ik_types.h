@@ -134,6 +134,14 @@ struct SkeletonTables {
   const int32_t* ptColStart; // [n+1] ParameterTransform as CSC
   const int32_t* ptColRows;  // [nnz] ascending within a column
   const float* ptColVals;    // [nnz]
+  // the inverse ParameterTransform W = P^+ (HostCharacter::buildInverseTables): by model parameter for its forward, by joint-parameter
+  // row for its backward
+  const int32_t* invStart;    // [n+1]
+  const int32_t* invRows;     // [nnz W] ascending within a parameter
+  const float* invVals;       // [nnz W]
+  const int32_t* invRowStart; // [7J+1]
+  const int32_t* invParams;   // [nnz W] ascending within a row
+  const float* invRowVals;    // [nnz W]
 };
 
 // Points fixed in joints' frames (model / joint_parameters_to_positions), shared by the batch (makePointTables): each point's joint, and
@@ -150,7 +158,14 @@ struct PointTables {
 //   kJointOpLocalState          local states [J][8] of jp [J][7]                /  g_jp [J][7] of g_local [J][8]
 //   kJointOpFromLocal           jp [J][7] of local states [J][8]                /  g_local [J][8] of g_jp [J][7]
 //   kJointOpFromWorld           jp [J][7] of world states [J][8]                /  g_world [J][8] of g_jp [J][7]
-enum JointOp : int32_t { kJointOpParameterTransform = 0, kJointOpLocalState = 1, kJointOpFromLocal = 2, kJointOpFromWorld = 3 };
+//   kJointOpInverseParameterTransform  theta [n] = W (jp - o), W = P^+          /  g_jp [7 J] = W^T g_theta
+enum JointOp : int32_t {
+  kJointOpParameterTransform = 0,
+  kJointOpLocalState = 1,
+  kJointOpFromLocal = 2,
+  kJointOpFromWorld = 3,
+  kJointOpInverseParameterTransform = 4,
+};
 
 // Linear-blend skinning tables (HostSkinning, makeSkinning), shared by the whole batch. The active influences of every vertex (the slots
 // before its first zero weight) are stored twice: by vertex for the blend, and by joint for the reductions of the backward, where each

@@ -96,6 +96,8 @@ CABI_SIGNATURES = {
     "mb2_character_skeleton_state_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
     "mb2_character_apply_parameter_transform_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
     "mb2_character_apply_parameter_transform_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_apply_inverse_parameter_transform_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_apply_inverse_parameter_transform_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
     "mb2_character_joint_parameters_to_skeleton_state_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
     "mb2_character_joint_parameters_to_skeleton_state_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
     "mb2_character_joint_parameters_to_local_skeleton_state_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
@@ -176,9 +178,11 @@ CABI_SYMBOLS = sorted(CABI_SIGNATURES)
 JOINT_OPS = {
     "model_parameters_to_skeleton_state": ("mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device"),
     **{name: (f"mb2_character_{name}_device", f"mb2_character_{name}_backward_device")
-       for name in ("apply_parameter_transform", "joint_parameters_to_skeleton_state", "joint_parameters_to_local_skeleton_state",
-                    "local_skeleton_state_to_joint_parameters", "skeleton_state_to_joint_parameters")},
+       for name in ("apply_parameter_transform", "apply_inverse_parameter_transform", "joint_parameters_to_skeleton_state",
+                    "joint_parameters_to_local_skeleton_state", "local_skeleton_state_to_joint_parameters", "skeleton_state_to_joint_parameters")},
 }
+# the operations whose backward does not read their input (P^T and W^T), so their backward takes no input pointer
+LINEAR_JOINT_OPS = frozenset({"apply_parameter_transform", "apply_inverse_parameter_transform"})
 
 _libs = {}
 
@@ -441,11 +445,11 @@ class DeviceCharacter(_Base):
 
     def joint_op_device(self, name: str, backward: bool, batch: int, *ptrs: int, stream: int = 0):
         """One direction of an operation of the skeleton-state family (``JOINT_OPS``: model_parameters_to_skeleton_state,
-        apply_parameter_transform, joint_parameters_to_skeleton_state, joint_parameters_to_local_skeleton_state,
-        local_skeleton_state_to_joint_parameters, skeleton_state_to_joint_parameters), float32 device memory on this character's device,
-        enqueued on ``stream`` (0: the legacy default stream). ``ptrs``: forward (input, output); backward (input, dLoss/d output,
-        dLoss/d input), except apply_parameter_transform's backward, which takes (dLoss/d joint parameters, dLoss/d model parameters). A
-        0 pointer is passed as null."""
+        apply_parameter_transform, apply_inverse_parameter_transform, joint_parameters_to_skeleton_state,
+        joint_parameters_to_local_skeleton_state, local_skeleton_state_to_joint_parameters, skeleton_state_to_joint_parameters), float32
+        device memory on this character's device, enqueued on ``stream`` (0: the legacy default stream). ``ptrs``: forward (input,
+        output); backward (input, dLoss/d output, dLoss/d input), except the backward of the two linear ops in ``LINEAR_JOINT_OPS``,
+        which takes (dLoss/d output, dLoss/d input). A 0 pointer is passed as null."""
         fn = getattr(self._L, JOINT_OPS[name][1 if backward else 0])
         self._check(fn(self._h, int(batch), *ptrs, stream))
 

@@ -1,6 +1,6 @@
 """Differentiable forward kinematics on CUDA tensors: ``model_parameters_to_skeleton_state`` and the rest of pymomentum's skeleton-state
-family (``apply_parameter_transform``, joint parameters to world and local states, and back, and the positions of points fixed in
-joints' frames), then skinning, normals and closest points.
+family (``apply_parameter_transform`` and its inverse, joint parameters to world and local states, and back, and the positions of
+points fixed in joints' frames), then skinning, normals and closest points.
 
 Mirror of ``pymomentum.geometry.model_parameters_to_skeleton_state`` (pymomentum/tensor_momentum/tensor_skeleton_state.cpp:500-502:
 ``jointParametersToSkeletonState(applyParamTransform(theta))``) for the batched device path. The forward pass is the solver's own FK
@@ -86,7 +86,7 @@ class _JointOp(torch.autograd.Function):
         g = grad_out.to(device=dev, dtype=torch.float32).reshape(B, ctx.out_numel).contiguous()
         gx = torch.empty_like(rows)
         ptrs = (g.data_ptr(), gx.data_ptr())
-        if ctx.name != "apply_parameter_transform":  # P^T: the only one that does not read its input
+        if ctx.name not in ms.LINEAR_JOINT_OPS:  # P^T and W^T do not read their input
             ptrs = (rows.data_ptr(),) + ptrs
         ctx.dc.joint_op_device(ctx.name, True, B, *ptrs, stream=torch.cuda.current_stream(dev).cuda_stream)
         return None, None, gx.reshape(ctx.in_shape).to(ctx.in_dtype), None
@@ -122,6 +122,19 @@ def apply_parameter_transform(character, model_parameters: torch.Tensor) -> torc
     ch, _ = _resolve(character)
     return _joint_op("apply_parameter_transform", character, model_parameters, f"model_parameters (n = {ch.num_params})", (ch.num_params,),
                      (7 * ch.num_joints,))
+
+
+def apply_inverse_parameter_transform(character, joint_parameters: torch.Tensor) -> torch.Tensor:
+    """Model parameters of flat ``joint_parameters`` (pymomentum ``apply_inverse_parameter_transform``): [7 J] or [B, 7 J] on a CUDA
+    device -> [n] or [B, n] in the input dtype, computed in float32: theta = P^+ (jp - o), the offsets o subtracted first. P^+ is the
+    Moore-Penrose pseudo-inverse of the ParameterTransform with pymomentum's truncation (a singular value above 1e-6, absolute, is
+    inverted, any other is 0), so theta is the minimum-norm least-squares solution of P theta + o = jp. It is built once per device
+    character, in float64 for each connected component of P's sparsity pattern, and rounded to float32 entry by entry: more accurate than
+    pymomentum's float SVD, so the two can differ by that SVD's error. ``character`` is a ``momentum_b200.character.Character`` or a
+    ``solver.DeviceCharacter`` on the tensor's device. Differentiable once; the gradient is (P^+)^T applied on the device."""
+    ch, _ = _resolve(character)
+    return _joint_op("apply_inverse_parameter_transform", character, joint_parameters, f"joint_parameters (7 J = {7 * ch.num_joints})",
+                     (7 * ch.num_joints,), (ch.num_params,))
 
 
 def joint_parameters_to_skeleton_state(character, joint_parameters: torch.Tensor) -> torch.Tensor:
