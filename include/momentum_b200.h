@@ -541,6 +541,17 @@ int mb2_solver_get_fused_profile(mb2_solver* s, int32_t* fused, int32_t* groups,
  * shared memory (the entry that launched it failed). The fused persistent kernel runs its own sweep and records nothing here.
  * No reference counterpart. */
 int mb2_solver_function_get_sweep_launch(mb2_solver_function* f, int32_t jacobian, int64_t out[5]);
+/* What the character operations' per-instance kernels would launch for `batch` instances, planned by the code that launches them and
+ * with nothing enqueued. op: 0 model_parameters_to_skeleton_state, 1 joint_parameters_to_skeleton_state, 2 model_parameters_to_positions,
+ * 3 joint_parameters_to_positions (num_points points); backward != 0: their backward. out: [0] warps per instance W (1, 2, 4 or 8),
+ * [1] instances per CTA, [2] threads per CTA, [3] CTAs, [4] dynamic shared memory per CTA in bytes, [5] 1 when the point tables are
+ * staged in shared memory. All zero when nothing runs (batch 0, positions with no point). An instance that does not fit in shared
+ * memory next to the tables is refused with MB2_ERR_CUDA, as the operation refuses it. The shared-offset positions backward launches
+ * per slice of the batch when its per-instance offset rows exceed 256 MiB of scratch: this reports one launch of `batch` instances.
+ * No reference counterpart. */
+int mb2_character_get_instance_launch(const mb2_character* c, int32_t op, int32_t backward, int32_t batch, int32_t num_points, int64_t out[6]);
+/* The same record for mb2_solver_function_input_gradients_device over the function's batch ([5] is 0). No reference counterpart. */
+int mb2_solver_function_get_input_gradient_launch(mb2_solver_function* f, int64_t out[6]);
 /* The linear-solve path the solver's last solve ran, as one host function chose it (the CPU emulator of the tests runs the same
  * choice): [0] kind (1 JtJ + dense Eigen-structured Cholesky, 2 JtJ + tile-scheduled Cholesky, 3 tile-sparse Gram + tile Cholesky
  * in two launches, 4 Gram + Cholesky in one launch, 5 the persistent kernel, 6 QR, 7 trust-region QR), [1] plan mode (1 compact

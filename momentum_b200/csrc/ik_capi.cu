@@ -2040,6 +2040,56 @@ int mb2_solver_function_get_sweep_launch(mb2_solver_function* f, int32_t jacobia
   return MB2_OK;
 }
 
+namespace {
+void instanceLaunchWords(const InstanceLaunchQuery& q, int64_t out[6]) {
+  out[0] = q.launch.warpsPerInstance;
+  out[1] = q.launch.groupsPerCta;
+  out[2] = q.launch.threads;
+  out[3] = q.grid;
+  out[4] = q.launch.smemBytes;
+  out[5] = q.launch.stagedPoints;
+}
+} // namespace
+
+int mb2_character_get_instance_launch(const mb2_character* c, int32_t op, int32_t backward, int32_t batch, int32_t num_points, int64_t out[6]) {
+  MB2_CHECK(c != nullptr && out != nullptr, "null argument");
+  MB2_CHECK(op >= kInstanceOpModelSkeletonState && op <= kInstanceOpJointPositions, "instance launch: op must be 0, 1, 2 or 3");
+  MB2_CHECK(batch >= 0 && num_points >= 0, "instance launch: batch and num_points must not be negative");
+  MB2_DEVICE_GUARD(c->device);
+  InstanceLaunchQuery q;
+  const bool joint = op == kInstanceOpJointSkeletonState || op == kInstanceOpJointPositions;
+  if (op == kInstanceOpModelSkeletonState || op == kInstanceOpJointSkeletonState) {
+    SkeletonStateArgs a{};
+    a.T = c->tables();
+    a.numChildren = int(c->host.children.size());
+    a.batch = batch;
+    a.fromJointParameters = joint;
+    MB2_CUDA(launchSkeletonState(a, backward != 0, nullptr, &q));
+  } else {
+    PositionArgs a{};
+    a.T = c->tables();
+    a.numChildren = int(c->host.children.size());
+    a.batch = batch;
+    a.P.numPoints = num_points;
+    a.fromJointParameters = joint;
+    MB2_CUDA(queryPositionsLaunch(a, backward != 0, &q));
+  }
+  instanceLaunchWords(q, out);
+  return MB2_OK;
+}
+
+int mb2_solver_function_get_input_gradient_launch(mb2_solver_function* f, int64_t out[6]) {
+  MB2_CHECK(f != nullptr && out != nullptr, "null argument");
+  MB2_DEVICE_GUARD(f->ch->device);
+  InputGradientArgs a{};
+  a.T = f->tables();
+  a.batch = f->B;
+  InstanceLaunchQuery q;
+  MB2_CUDA(launchInputGradients(a, nullptr, &q));
+  instanceLaunchWords(q, out);
+  return MB2_OK;
+}
+
 int mb2_solver_get_solve_path(mb2_solver* s, int64_t out[15]) {
   MB2_CHECK(s != nullptr && out != nullptr, "null argument");
   solvePathWords(s->path, out);

@@ -237,7 +237,7 @@ MB2_HD F3 pointDerivative(const CharacterTables& T, const float* js, int a, int 
 //   [7..9] S_c = sum 1/2 (w_i g_v + v_i x g_v - g_w v_i)        [10] S_s = sum s_i g_s
 // R and D are kept relative to the joint's own origin and shifted once per child edge: the form sum t_i x g - t_a x sum g cancels
 // catastrophically for a rig far from the origin.
-constexpr int kSkelAccStride = 11; // odd: conflict-free with lanes = joints
+// (kSkelAccStride, ik_types.h: the 11 floats above per joint)
 
 // the joint's own term (its subtree before any child is folded in); g: the joint's 8 upstream gradient floats
 MB2_HD void skelGradSeed(const float* js, int i, const float* g, float* acc) {
@@ -520,7 +520,7 @@ MB2_HD void jointOpElement(const CharacterTables& T, const SkeletonTables& S, lo
 //   tdot_j = tdot_pi + w_pi x (t_j - t_pi) + sigma_pi (t_j - t_pi) + sum_k u[7j+k] B_jk
 // (A = rotationAxisCol, B = translationAxisCol; zero motion above a root). A point p attached to j moves at
 // pdot = tdot_j + w_j x (p - t_j) + sigma_j (p - t_j) = J_c v. t_j - t_pi stays relative (no cancellation for a rig far from the origin).
-constexpr int kTangentStride = 7; // w(3) sigma tdot(3); odd: conflict-free with lanes = joints
+// (kTangentStride, ik_types.h: w(3) sigma tdot(3) per joint)
 
 // u[row] = (P v)[row] without ptOffsets (jointParameterRow adds them)
 MB2_HD float tangentJointParameter(const CharacterTables& T, int row, const float* v) {

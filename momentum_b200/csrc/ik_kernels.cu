@@ -43,18 +43,10 @@ size_t sweepSmemPerInstance(const FunctionTables& T, int warpsPerInstance) {
 
 // The read-only tables (character + plan) are walked by dependent loads (cell -> unit -> contributions -> joint);
 // from L2 each hop costs several hundred cycles, so a persistent CTA copies them into shared memory once.
-MB2_HD size_t tableWords(size_t count, size_t elemBytes) { return (count * elemBytes + 15) / 16 * 4; }
+// (tableWords, characterTableWords: ik_instance_launch.h)
 // mode 1: every table; mode 2: everything except the two big ones, cells and contributions (large rigs: those are streamed through
 // L1 / L2, one sequential record per lane and iteration, while the tables walked by dependent loads - character, units, error functions -
 // still sit in shared memory)
-// the character tables, staged first by every kernel that stages tables (stageCharacterTables)
-size_t characterTableWords(const CharacterTables& C) {
-  const size_t J = C.numJoints;
-  size_t w = tableWords(J, 4) + tableWords(3 * J, 4) + tableWords(4 * J, 4);                 // parent, offset, prerot
-  w += tableWords(7 * J + 1, 4) + tableWords(C.ptNnz, 4) * 2 + tableWords(7 * J, 4);         // ptOuter, ptInner, ptVals, ptOffsets
-  w += tableWords(C.numLevels + 1, 4) + tableWords(J, 4);                                    // levelStart, levelJoints
-  return w;
-}
 size_t sweepTableBytes(const FunctionTables& T, int mode) {
   if (mode == 0) return 0;
   size_t w = characterTableWords(T);
@@ -246,27 +238,8 @@ cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream,
 // kJoint (joint_parameters_to_skeleton_state): the input is the joint parameters [7 J], staged where theta is staged otherwise; the
 // backward writes the joint-parameter gradient straight out and stops before the ParameterTransform.
 // Every output element is written by one lane in a fixed order: no atomics, the result does not depend on the launch shape.
+// Shared memory per instance and per CTA, and the choice of W: ik_instance_launch.h.
 // ------------------------------------------------------------------------------------------------
-constexpr int kSkelMaxWarps = 16;
-MB2_HD size_t skelAligned(size_t floats) { return (floats + 3) & ~size_t(3); } // 16-byte aligned regions
-
-// per instance: the input (theta [n], or the joint parameters [7 J]), joint states [J][17], backward: subtree sums [J][11] and, from
-// theta, the joint-parameter gradient [7 J]
-MB2_HD size_t skeletonStateSmemPerInstanceFloats(int J, int n, bool backward, bool joint) {
-  size_t f = skelAligned(joint ? size_t(J) * kParametersPerJoint : size_t(n)) + skelAligned(size_t(J) * kJointStateStride);
-  if (backward) f += skelAligned(size_t(J) * kSkelAccStride) + (joint ? 0 : skelAligned(size_t(J) * kParametersPerJoint));
-  return f;
-}
-size_t skeletonStateSmemPerInstance(const CharacterTables& C, bool backward, bool joint) {
-  return sizeof(float) * skeletonStateSmemPerInstanceFloats(C.numJoints, C.numParams, backward, joint);
-}
-
-size_t skeletonStateTableBytes(const CharacterTables& C, int numChildren, bool backward, bool joint) {
-  size_t w = characterTableWords(C);
-  if (backward) w += tableWords(C.numJoints + 1, 4) + tableWords(numChildren, 4);
-  if (backward && !joint) w += tableWords(C.numParams + 1, 4) + tableWords(C.ptNnz, 4) * 2;
-  return w * 4;
-}
 
 template <bool kBackward, int W, bool kJoint>
 __global__ void __launch_bounds__(32 * kSkelMaxWarps) skeletonStateKernel(const SkeletonStateArgs a) {
@@ -324,33 +297,30 @@ cudaError_t persistentGrid(K kernel, int threads, size_t smem, long work, int* g
   return cudaSuccess;
 }
 
-// A persistent kernel with one group of W warps per instance and the tables staged once per CTA (skeletonStateKernel,
-// inputGradientKernel). As many instances per CTA as shared memory holds next to the tables, one warp each up to kSkelMaxWarps. When
-// fewer than eight fit (large rigs), several warps share an instance. A batch smaller than one instance group per SM is spread over the
-// SMs. kernels[0..3]: the instantiations for W = 1, 2, 4, 8.
+// A persistent kernel with one group of W warps per instance and the tables staged once per CTA (skeletonStateKernel, positionsKernel,
+// inputGradientKernel), launched as planInstanceOp planned it (ik_instance_launch.cpp). kernels[0..3]: the instantiations for W = 1, 2,
+// 4, 8. With `query`, the launch is reported there and nothing is enqueued.
 template <class Args>
-cudaError_t launchInstanceGroups(void (*const kernels[4])(Args), const Args& a, size_t perInstance, size_t tableBytes, cudaStream_t stream) {
+cudaError_t launchInstanceGroups(void (*const kernels[4])(Args), const Args& a, int numChildren, int op, bool backward, int numPoints, cudaStream_t stream,
+                                 InstanceLaunchQuery* query) {
+  if (query) *query = InstanceLaunchQuery{};
   if (a.batch <= 0) return cudaSuccess;
-  const size_t budget = size_t(g_maxSmemOptin);
-  tableBytes += 16;
-  if (tableBytes + perInstance > budget) return cudaErrorInvalidConfiguration;
-  const int fit = int((budget - tableBytes) / perInstance);
-  int W = 1, w = 0, groups = std::min(fit, kSkelMaxWarps);
-  if (fit < 8)
-    while (W < 8 && groups * W * 2 <= kSkelMaxWarps) { W *= 2; ++w; } // named barriers 1..groups
-  const int sms = std::max(g_numSms, 1);
-  if (a.batch < sms * groups) groups = std::max(1, (a.batch + sms - 1) / sms);
-  const size_t smem = perInstance * groups + tableBytes;
-  const int threads = groups * W * 32;
+  const InstanceLaunch l = planInstanceOp(a.T, numChildren, op, backward, numPoints, a.batch, size_t(g_maxSmemOptin), g_numSms);
+  if (l.warpsPerInstance == 0) return cudaErrorInvalidConfiguration; // not even one instance fits next to the tables
+  const int w = l.warpsPerInstance == 1 ? 0 : l.warpsPerInstance == 2 ? 1 : l.warpsPerInstance == 4 ? 2 : 3;
   int grid = 0;
-  const cudaError_t e = persistentGrid(kernels[w], threads, smem, (long(a.batch) + groups - 1) / groups, &grid);
+  const cudaError_t e = persistentGrid(kernels[w], l.threads, size_t(l.smemBytes), (long(a.batch) + l.groupsPerCta - 1) / l.groupsPerCta, &grid);
   if (e != cudaSuccess) return e;
-  kernels[w]<<<grid, threads, smem, stream>>>(a);
+  if (query) {
+    *query = InstanceLaunchQuery{l, grid};
+    return cudaSuccess;
+  }
+  kernels[w]<<<grid, l.threads, size_t(l.smemBytes), stream>>>(a);
   return cudaGetLastError();
 }
 } // namespace
 
-cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream) {
+cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query) {
   using K = void (*)(SkeletonStateArgs);
   static const K kernels[2][2][4] = {
       {{skeletonStateKernel<false, 1, false>, skeletonStateKernel<false, 2, false>, skeletonStateKernel<false, 4, false>, skeletonStateKernel<false, 8, false>},
@@ -358,8 +328,8 @@ cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaS
       {{skeletonStateKernel<false, 1, true>, skeletonStateKernel<false, 2, true>, skeletonStateKernel<false, 4, true>, skeletonStateKernel<false, 8, true>},
        {skeletonStateKernel<true, 1, true>, skeletonStateKernel<true, 2, true>, skeletonStateKernel<true, 4, true>, skeletonStateKernel<true, 8, true>}}};
   const bool joint = a.fromJointParameters != 0;
-  return launchInstanceGroups(kernels[joint][backward], a, skeletonStateSmemPerInstance(a.T, backward, joint), skeletonStateTableBytes(a.T, a.numChildren, backward, joint),
-                              stream);
+  return launchInstanceGroups(kernels[joint][backward], a, a.numChildren, joint ? kInstanceOpJointSkeletonState : kInstanceOpModelSkeletonState, backward, 0, stream,
+                              query);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -640,12 +610,6 @@ cudaError_t launchSkinPointsBackward(const SkinArgs& a, cudaStream_t stream) {
 // over the chunks in order (rowGroupSumKernel). The rows of a slice of whole chunks go to bounded scratch. No atomics, and no result
 // depends on the slicing or the launch shape.
 // ------------------------------------------------------------------------------------------------
-size_t pointTableBytes(const PointTables& P, int J, bool backward) {
-  size_t w = tableWords(P.numPoints, 4);
-  if (backward) w += tableWords(size_t(J) + 1, 4) + tableWords(P.numPoints, 4);
-  return w * 4;
-}
-
 // kStagePoints: a template parameter rather than a run-time branch, so that the staged point tables are provably shared-memory addresses
 template <bool kBackward, int W, bool kJoint, bool kStagePoints>
 __global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) positionsKernel(const PositionArgs a) {
@@ -696,7 +660,8 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) positionsKernel(const P
 }
 
 namespace {
-cudaError_t launchPositionsKernel(const PositionArgs& a, bool backward, cudaStream_t stream) {
+// kernels[joint][backward][kStagePoints]; planInstanceOp decides the staging
+cudaError_t launchPositionsKernel(const PositionArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query = nullptr) {
   using K = void (*)(PositionArgs);
 #define MB2_POSITION_KERNELS(B, J, S) {positionsKernel<B, 1, J, S>, positionsKernel<B, 2, J, S>, positionsKernel<B, 4, J, S>, positionsKernel<B, 8, J, S>}
   static const K kernels[2][2][2][4] = {
@@ -706,14 +671,17 @@ cudaError_t launchPositionsKernel(const PositionArgs& a, bool backward, cudaStre
        {MB2_POSITION_KERNELS(true, true, false), MB2_POSITION_KERNELS(true, true, true)}}};
 #undef MB2_POSITION_KERNELS
   const bool joint = a.fromJointParameters != 0;
-  const size_t per = skeletonStateSmemPerInstance(a.T, backward, joint);
-  const size_t tables = skeletonStateTableBytes(a.T, a.numChildren, backward, joint), points = pointTableBytes(a.P, a.T.numJoints, backward);
-  // instance groups per CTA as launchInstanceGroups counts them
-  auto groups = [&](size_t t) { return t + 16 + per > size_t(g_maxSmemOptin) ? 0 : std::min<size_t>((g_maxSmemOptin - t - 16) / per, kSkelMaxWarps); };
-  const bool stage = groups(tables + points) >= groups(tables);
-  return launchInstanceGroups(kernels[joint][backward][stage], a, per, tables + (stage ? points : 0), stream);
+  const int op = joint ? kInstanceOpJointPositions : kInstanceOpModelPositions;
+  const bool stage = planInstanceOp(a.T, a.numChildren, op, backward, a.P.numPoints, a.batch, size_t(g_maxSmemOptin), g_numSms).stagedPoints != 0;
+  return launchInstanceGroups(kernels[joint][backward][stage], a, a.numChildren, op, backward, a.P.numPoints, stream, query);
 }
 } // namespace
+
+cudaError_t queryPositionsLaunch(const PositionArgs& a, bool backward, InstanceLaunchQuery* query) {
+  *query = InstanceLaunchQuery{};
+  if (a.P.numPoints == 0) return cudaSuccess; // nothing runs (the backward clears the parameter gradient)
+  return launchPositionsKernel(a, backward, nullptr, query);
+}
 
 cudaError_t launchPositions(const PositionArgs& a, cudaStream_t stream) {
   if (a.batch <= 0 || a.P.numPoints == 0) return cudaSuccess;
@@ -1640,11 +1608,7 @@ cudaError_t launchClosestPointsOnCloud(const ClosestCloudArgs& a, cudaStream_t s
 //   then level by level the parent's motion added;  lanes = constraints of the block.
 // Every output element is written by one lane: no atomics, the result does not depend on the launch shape.
 // ------------------------------------------------------------------------------------------------
-// per instance: theta [n], v [n], joint states [J][17], joint motions [J][7]
-MB2_HD size_t inputGradientSmemPerInstanceFloats(int J, int n) {
-  return 2 * skelAligned(size_t(n)) + skelAligned(size_t(J) * kJointStateStride) + skelAligned(size_t(J) * kTangentStride);
-}
-
+// (shared memory per instance: inputGradientSmemPerInstanceFloats, ik_instance_launch.h)
 template <int W>
 __global__ void __launch_bounds__(32 * kSkelMaxWarps) inputGradientKernel(const InputGradientArgs a) {
   extern __shared__ __align__(16) float smem[];
@@ -1690,10 +1654,9 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps) inputGradientKernel(const 
   }
 }
 
-cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream) {
+cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream, InstanceLaunchQuery* query) {
   static void (*const kernels[4])(InputGradientArgs) = {inputGradientKernel<1>, inputGradientKernel<2>, inputGradientKernel<4>, inputGradientKernel<8>};
-  const size_t per = sizeof(float) * inputGradientSmemPerInstanceFloats(a.T.numJoints, a.T.numParams);
-  return launchInstanceGroups(kernels, a, per, characterTableWords(a.T) * 4, stream);
+  return launchInstanceGroups(kernels, a, 0, kInstanceOpInputGradients, false, 0, stream, query);
 }
 
 // ------------------------------------------------------------------------------------------------

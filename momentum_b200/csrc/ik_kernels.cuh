@@ -5,6 +5,7 @@
 
 #include "ik_chol_sched.cuh"
 #include "ik_chol_sched.h"
+#include "ik_instance_launch.h"
 #include "ik_solve_path.h"
 #include "ik_types.h"
 
@@ -150,7 +151,14 @@ struct SkeletonStateArgs {
   float* out;                // forward: [B][J][8] (t, q xyzw, s); backward: [B][n] dLoss / d theta ([B][7 J] d joint parameters), overwritten
   int32_t fromJointParameters; // joint_parameters_to_skeleton_state: the FK from joint parameters, S.ptCol* unused
 };
-cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream);
+// What a per-instance kernel of the character operations launches (mb2_character_get_instance_launch,
+// mb2_solver_function_get_input_gradient_launch): planInstanceOp's plan and the grid the device's occupancy gives it
+struct InstanceLaunchQuery {
+  InstanceLaunch launch;
+  int32_t grid{0};
+};
+// `query` (optional): the launch is planned and reported there and nothing is enqueued; all zero for an empty batch
+cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query = nullptr);
 // positionsKernel<kBackward>: pymomentum's model_parameters_to_positions / joint_parameters_to_positions for a batch on the character
 // alone, and their backward
 struct PositionArgs {
@@ -172,6 +180,9 @@ struct PositionArgs {
 // gradients of a slice of instances (at most 256 MiB) and 128 x [N][3] floats for their chunk sums.
 cudaError_t launchPositions(const PositionArgs& a, cudaStream_t stream);
 cudaError_t launchPositionsBackward(const PositionArgs& a, cudaStream_t stream);
+// the launch of positionsKernel over a.batch instances with a.P.numPoints points (a.P's arrays are not read); the shared-offset
+// backward launches it per slice of whole batch-sum chunks, which is the whole batch unless the offset rows exceed the scratch bound
+cudaError_t queryPositionsLaunch(const PositionArgs& a, bool backward, InstanceLaunchQuery* query);
 // parameterTransformKernel ... inverseParameterTransformBackwardKernel: the flat joint-parameter operations of ik_device.cuh
 // jointOpElement for a batch, forward or backward; arrays [B][...] dense, device memory
 struct JointOpArgs {
@@ -278,7 +289,7 @@ struct InputGradientArgs {
   float* gradOffsets;        // [B][nc][3|4] or null
   float* gradTargets;        // [B][nc][3|4] or null
 };
-cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream);
+cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream, InstanceLaunchQuery* query = nullptr);
 // implicitDirectionKernel: per instance v = (2 J_E^T J_E)^+ g (the reference's hessianInverseTimes, ik_jacobi.cuh), J v, the residual
 // and the gradient RMS, from the K-major Jacobian [B][n + 1][ldJ] of a mode-0 plan
 struct ImplicitDirectionArgs {

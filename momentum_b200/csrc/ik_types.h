@@ -20,6 +20,8 @@ namespace mb2 {
 
 constexpr int kParametersPerJoint = 7; // character/types.h:21
 constexpr int kJointStateStride = 17;  // t(3) q(4) s(1) rotationAxis(9); odd => bank-conflict-free per-joint access
+constexpr int kSkelAccStride = 11;     // subtree sums of the skeleton-state backward (ik_device.cuh); odd: conflict-free with lanes = joints
+constexpr int kTangentStride = 7;      // joint motion w(3) sigma tdot(3) of the input gradients (ik_device.cuh); odd: conflict-free with lanes = joints
 constexpr float kLn2 = 0.69314718055994530942f; // math/constants.h:40
 constexpr float kPi = 3.14159265358979323846f;
 

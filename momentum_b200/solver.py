@@ -143,6 +143,8 @@ CABI_SIGNATURES = {
     "mb2_solver_get_plan_stats": (_int, [_vp, _lp]),
     "mb2_solver_get_fused_profile": (_int, [_vp, _ip, _ip, _dp, _up]),
     "mb2_solver_function_get_sweep_launch": (_int, [_vp, _int32, _lp]),
+    "mb2_character_get_instance_launch": (_int, [_vp, _int32, _int32, _int32, _int32, _lp]),
+    "mb2_solver_function_get_input_gradient_launch": (_int, [_vp, _lp]),
     "mb2_solver_get_solve_path": (_int, [_vp, _lp]),
     "mb2_mixed_batch_last_error": (C.c_char_p, []),
     "mb2_mixed_batch_create": (_int, [_int, _int32, _out]),
@@ -279,6 +281,15 @@ class _Base:
     def _check(self, rc):
         if rc != 0:
             raise MomentumB200Error(self._L.mb2_last_error().decode())
+
+
+# the operations mb2_character_get_instance_launch reports on, by its op code
+INSTANCE_OPS = {"model_parameters_to_skeleton_state": 0, "joint_parameters_to_skeleton_state": 1, "model_parameters_to_positions": 2,
+                "joint_parameters_to_positions": 3}
+
+
+def _instance_launch(out) -> dict:
+    return dict(zip(("warps", "groups", "threads", "grid", "smem", "staged"), (int(v) for v in out)))
 
 
 class DeviceCharacter(_Base):
@@ -452,6 +463,14 @@ class DeviceCharacter(_Base):
         which takes (dLoss/d output, dLoss/d input). A 0 pointer is passed as null."""
         fn = getattr(self._L, JOINT_OPS[name][1 if backward else 0])
         self._check(fn(self._h, int(batch), *ptrs, stream))
+
+    def get_instance_launch(self, op: str, backward: bool, batch: int, num_points: int = 0) -> dict:
+        """What the per-instance kernel of ``op`` (a key of ``INSTANCE_OPS``) would launch for ``batch`` instances (and ``num_points``
+        points): warps per instance, instances per CTA, threads per CTA, CTAs, dynamic shared memory bytes and whether the point tables
+        are staged. All zero when nothing runs; raises when one instance does not fit in shared memory."""
+        out = (C.c_int64 * 6)()
+        self._check(self._L.mb2_character_get_instance_launch(self._h, INSTANCE_OPS[op], int(bool(backward)), int(batch), int(num_points), out))
+        return _instance_launch(out)
 
     def positions_device(self, joint: bool, batch: int, params_device_ptr: int, parents: np.ndarray, offsets_device_ptr: int, offsets_batched: bool,
                          positions_device_ptr: int, stream: int = 0):
@@ -641,6 +660,12 @@ class SkeletonSolverFunction(_Base):
         out = (C.c_int64 * 5)()
         self._check(self._L.mb2_solver_function_get_sweep_launch(self._h, int(bool(jacobian)), out))
         return dict(zip(("stage", "warps", "groups", "grid", "smem"), (int(v) for v in out)))
+
+    def get_input_gradient_launch(self) -> dict:
+        """What ``input_gradients_device`` launches over this handle's batch, as ``DeviceCharacter.get_instance_launch`` reports it."""
+        out = (C.c_int64 * 6)()
+        self._check(self._L.mb2_solver_function_get_input_gradient_launch(self._h, out))
+        return _instance_launch(out)
 
 
 class GaussNewtonSolver(_Base):

@@ -11,7 +11,7 @@ import numpy as np
 EMU_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emu")
 EMU_LIB = os.path.join(EMU_DIR, "libmb2_emu.so")
 
-_i32, _f32, _p = ctypes.c_int32, ctypes.c_float, ctypes.c_void_p
+_i32, _i64, _f32, _p = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p
 _CHARACTER = [_i32, _p, _p, _p, _i32, _p, _p, _p, _p]  # mb2_character_create's arguments
 _SKINNING = _CHARACTER + [_i32, _p, _p, _p, _p]  # V, rest vertices, skin index, skin weight, inverse bind poses
 _BLEND = _SKINNING + [_i32, _i32, _p, _p]  # K, V, base shape, shape vectors
@@ -31,6 +31,8 @@ _SIGNATURES = {
     "emu_mesh_tree": [_i32, _i32, _p, _i32, _p, _p, _p, _p, _p, _p],
     "emu_mesh_tree_boxes": [_i32, _i32, _p, _p, _p, _p],
     "emu_closest_points": [_i32, _i32, _p, _p, _i32, _i32, _p, _p, _f32, _i32, _p, _p, _p, _p],
+    "emu_plan_instance_groups": [_i64] * 4 + [_i32, _p],
+    "emu_instance_launch": _CHARACTER + [_i32, _i32, _i64, _i32, _i64, _i32, _p],
 }
 
 

@@ -25,6 +25,8 @@ def test_header_symbols_exported(lib):
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in momentum_b200.h but not exported"
     assert sorted(ms.CABI_SYMBOLS) == declared
+    # the launch reports of the per-instance character kernels (tests/test_instance_launch_variants.py)
+    assert {"mb2_character_get_instance_launch", "mb2_solver_function_get_input_gradient_launch"} <= set(declared)
     # every binding takes as many arguments as its prototype declares (comments dropped: some hold commas or calls)
     prototypes = dict(re.findall(r"\b(mb2_[a-z0-9_]+)\s*\(([^)]*)\)", re.sub(r"/\*.*?\*/", "", header, flags=re.S)))
     for name, (_, argtypes) in ms.CABI_SIGNATURES.items():
