@@ -32,6 +32,7 @@ import torch
 
 from . import character as mc
 from . import solver as ms
+from . import torch_skeleton as tsk
 
 GRADIENT_RMSE_THRESHOLD = 0.01  # tensor_ik.cpp:46
 
@@ -67,26 +68,20 @@ class SolverOptions:
     verbose: bool = False
 
 
-_handles = {}
-
-
-def _f32c(t, device):
-    return t.detach().to(device=device, dtype=torch.float32).contiguous()
-
-
-def _build(character: mc.Character, B, device_index, pos_parents, pos_offsets, ori_parents, ori_offsets, motion_weights, use_limit, active):
-    """One cached solver function per (character, batch, constraint topology): the plan is built once. ``pos_offsets`` /
-    ``ori_offsets`` None with parents given select the instanced block (offsets per element, in the target records): the key then
-    holds the parents only, so new offset values reuse the handle."""
+def _build(character: mc.Character, B, device, pos_parents, pos_offsets, ori_parents, ori_offsets, motion_weights, use_limit, active):
+    """One cached solver function per (character, device, batch, constraint topology), on the character's DeviceCharacter and in its
+    registry entry (``torch_skeleton._handle``): the plan is built once. ``pos_offsets`` / ``ori_offsets`` None with parents given select
+    the instanced block (offsets per element, in the target records): the key then holds the parents only, so new values reuse it."""
     def key_of(a):
         return None if a is None else a.tobytes()
 
-    key = (id(character), B, device_index, key_of(pos_parents), "instanced" if pos_parents is not None and pos_offsets is None else key_of(pos_offsets),
+    handle = tsk._handle(character, device)
+    key = (B, key_of(pos_parents), "instanced" if pos_parents is not None and pos_offsets is None else key_of(pos_offsets),
            key_of(ori_parents), "instanced" if ori_parents is not None and ori_offsets is None else key_of(ori_offsets),
            key_of(motion_weights), use_limit, active.tobytes())
-    if key in _handles:
-        return _handles[key]
-    fn = ms.SkeletonSolverFunction(character, B, device=device_index)
+    if key in handle.solver_functions:
+        return handle.solver_functions[key]
+    fn = ms.SkeletonSolverFunction(handle.dc, B)
     blocks = {}
     n = character.num_params
     if pos_parents is not None:
@@ -107,8 +102,8 @@ def _build(character: mc.Character, B, device_index, pos_parents, pos_offsets, o
     if motion_weights is not None:
         blocks["motion"] = fn.add_error_function(mc.ModelParametersErrorFunction(motion_weights, np.zeros((B, n), np.float32), weight=1.0))
     fn.set_enabled_parameters(active)
-    _handles[key] = (fn, blocks)
-    return _handles[key]
+    handle.solver_functions[key] = (fn, blocks)
+    return fn, blocks
 
 
 def _normalization_backward(g, q):
@@ -118,18 +113,12 @@ def _normalization_backward(g, q):
     return (g - qh * (qh * g).sum(dim=-1, keepdim=True)) / nrm
 
 
-def _reduce_to(g, like):
-    """A per-element gradient [B, ...] for an input shared by the batch ([...]): the sum over the batch."""
-    return g.sum(dim=0) if like.dim() == g.dim() - 1 else g
-
-
 class _SolveIK(torch.autograd.Function):
     @staticmethod
     def forward(ctx, cfg, theta0, efw, pos_targets, pos_weights, pos_offsets, ori_targets, ori_weights, ori_offsets, motion_targets, motion_weights):
         fn, blocks, opts, kinds = cfg["fn"], cfg["blocks"], cfg["options"], cfg["kinds"]
         dev = theta0.device
-        B = theta0.shape[0]
-        efw32 = _f32c(efw, dev)
+        efw32 = tsk._float32(efw, device=dev)
         saved = {}  # device copies of everything the handle was given: the backward sends them again before it reads the handle
         # per-element error-function weights (buildMomentumErrorFunctions, tensor_ik_utility.cpp:149-181): folded into the per-instance
         # constraint weights for Position / Orientation; Limit and Motion carry one weight for the whole batch on the device
@@ -137,26 +126,25 @@ class _SolveIK(torch.autograd.Function):
             if name not in blocks:
                 continue
             k = kinds.index(ErrorFunctionType.Position if name == "position" else ErrorFunctionType.Orientation)
-            rec = _f32c(tgt, dev)
+            rec = tsk._float32(tgt, device=dev)
             if off is not None:  # instanced block: the record is target, then offset, per constraint
-                rec = torch.cat([rec, _f32c(off, dev).expand(rec.shape)], dim=-1).contiguous()
+                rec = torch.cat([rec, tsk._float32(off, device=dev).expand(rec.shape)], dim=-1).contiguous()
             saved[name + "_record"] = rec
-            saved[name + "_weights"] = (_f32c(w, dev) * efw32[:, k:k + 1]).contiguous()
+            saved[name + "_weights"] = (tsk._float32(w, device=dev) * efw32[:, k:k + 1]).contiguous()
         if "motion" in blocks:
-            saved["motion_targets"] = _f32c(motion_targets, dev)
+            saved["motion_targets"] = tsk._float32(motion_targets, device=dev)
         for name, kind in (("limit", ErrorFunctionType.Limit), ("motion", ErrorFunctionType.Motion)):
             if name not in blocks:
                 continue
             col = efw32[:, kinds.index(kind)]
             if not bool(torch.all(col == col[0])):
                 raise ValueError(f"{name} error-function weights must be the same for every batch element on the device path")
-        _SolveIK._send(cfg, efw32, saved, torch.cuda.current_stream(dev).cuda_stream)
+        _SolveIK._send(cfg, efw32, saved, tsk._stream(dev))
         solver = ms.GaussNewtonSolver(opts, fn)
-        theta = _f32c(theta0, dev).clone()
-        solver.solve_device(theta.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        theta = tsk._float32(theta0, device=dev).clone()
+        solver.solve_device(theta.data_ptr(), tsk._stream(dev))
         res = solver.get_results()  # synchronises; the NaN / Inf guard (tensor_ik.cpp:168-173) already ran on the device
         ctx.cfg = cfg
-        ctx.status = res["status"]
         ctx.names = list(saved)
         raw = [t.detach() if t is not None else None for t in (ori_targets, ori_offsets, pos_offsets, motion_weights)]
         ctx.raw_present = [t is not None for t in raw]
@@ -193,14 +181,14 @@ class _SolveIK(torch.autograd.Function):
         ori_targets_raw, ori_offsets_raw, pos_offsets_raw, motion_weights_raw = [next(rest) if p else None for p in ctx.raw_present]
         dev = theta.device
         B, n = theta.shape
-        stream = torch.cuda.current_stream(dev).cuda_stream
+        stream = tsk._stream(dev)
         # another solve on the same cached handle may have run since this forward: give it this forward's inputs again
         _SolveIK._send(cfg, efw32, saved, stream)
         # v = (2 J^T J)^+ g (fully_differentiable_body_ik.cpp:78-109), J v, the residual and the gradient RMS, all on the device: the
         # Jacobian sweep and a float64 Jacobi eigen-solve of the Gram matrix of the enabled columns, on this stream
         rows = sum(cfg["block_rows"].values())
         stride = fn.jacobian_rows
-        g32 = grad_theta.to(device=dev, dtype=torch.float32).contiguous()
+        g32 = tsk._float32(grad_theta, device=dev)
         v32 = torch.empty(B, n, device=dev)
         jv32, r32 = torch.empty(B, stride, device=dev), torch.empty(B, stride, device=dev)
         rms32 = torch.empty(B, device=dev)
@@ -238,7 +226,7 @@ class _SolveIK(torch.autograd.Function):
                 if need["pos_offsets"] and pos_offsets_raw is not None:
                     go = torch.empty(B, nc, 3, device=dev)
                     fn.input_gradients_device(blocks["position"], theta.data_ptr(), v_ok32.data_ptr(), grad_offsets_ptr=go.data_ptr(), stream=stream)
-                    grads["pos_offsets"] = _reduce_to(-go.double(), pos_offsets_raw)
+                    grads["pos_offsets"] = tsk._batch_sum(-go.double(), pos_offsets_raw.shape)
             elif name == "orientation":
                 nc = nr // 9
                 if not (need["ori_targets"] or need["ori_weights"] or need["ori_offsets"]):
@@ -247,13 +235,12 @@ class _SolveIK(torch.autograd.Function):
                 gw = torch.empty(B, nc, device=dev)
                 gt = torch.empty(B, nc, 4, device=dev)
                 go = torch.empty(B, nc, 4, device=dev) if ori_offsets_raw is not None else None
-                fn.input_gradients_device(blocks["orientation"], theta.data_ptr(), v_ok32.data_ptr(), gw.data_ptr(), 0 if go is None else go.data_ptr(),
-                                          gt.data_ptr(), stream)
+                fn.input_gradients_device(blocks["orientation"], theta.data_ptr(), v_ok32.data_ptr(), gw.data_ptr(), tsk._ptr(go), gt.data_ptr(), stream)
                 grads["ori_weights"] = -gw.double() * wk[:, None]   # the device weight is constraint weight x error-function weight
                 grads["ori_targets"] = _normalization_backward(-gt.double(), ori_targets_raw.to(dev).double())
                 if go is not None:
                     off = ori_offsets_raw.to(dev).double().expand(B, nc, 4)
-                    grads["ori_offsets"] = _reduce_to(_normalization_backward(-go.double(), off), ori_offsets_raw)
+                    grads["ori_offsets"] = tsk._batch_sum(_normalization_backward(-go.double(), off), ori_offsets_raw.shape)
             elif name == "motion":
                 # E = efw 0.1 sum_i w_i^2 (theta_i - t_i)^2 over the enabled parameters with w_i > 0 (model_parameters_error_function.cpp,
                 # kMotionWeight = 0.1): d/dt_i [grad E . v] = -2 s w_i^2 v_i,  d/dw_i = 4 s w_i (theta_i - t_i) v_i
@@ -334,7 +321,7 @@ def solve_ik(character: mc.Character, active_parameters, model_parameters_init: 
     if use_motion:
         mwt = motion_weights if motion_weights is not None else torch.ones(n)
         mw = np_or_none(mwt[0] if (torch.is_tensor(mwt) and mwt.dim() == 2) else mwt, np.float32)
-    fn, blocks = _build(character, B, dev.index or 0, pp, po, op, oo, mw, ErrorFunctionType.Limit in kinds, active)
+    fn, blocks = _build(character, B, dev, pp, po, op, oo, mw, ErrorFunctionType.Limit in kinds, active)
     order = [name for name in ("position", "orientation", "limit", "motion") if name in blocks]
     block_rows = {}
     for name in order:

@@ -11,6 +11,8 @@ positions or rotations after ``torch_ik.solve_ik`` back-propagates to the solver
 """
 from __future__ import annotations
 
+from collections import namedtuple
+
 import numpy as np
 import torch
 from torch.autograd.function import once_differentiable
@@ -18,28 +20,57 @@ from torch.autograd.function import once_differentiable
 from . import character as mc
 from . import solver as ms
 
+# The registry entry of one (character, device): the character, kept alive so that its id stays unique; the (skinning, faces, blend
+# shape) its DeviceCharacter ``dc`` was made with; and the solver functions ``torch_ik._build`` made on ``dc``.
+_Handle = namedtuple("_Handle", "character mesh dc solver_functions")
 _handles = {}
 
 
+def _device_index(device: torch.device) -> int:
+    return device.index if device.index is not None else torch.cuda.current_device()
+
+
+def _handle(character: mc.Character, device: torch.device) -> _Handle:
+    """The torch layer's one entry per (character, device). When ``skinning``, its ``faces`` or ``blend_shape`` is replaced, a new entry
+    with a new DeviceCharacter is made instead of uploading into the old one: a graph recorded before keeps its handle (``ctx.dc``) and
+    tables, and no kernel in flight on another stream reads tables being replaced. The old entry's solver functions go with it."""
+    index = _device_index(device)
+    entry = _handles.get((id(character), index))
+    mesh = (character.skinning, None if character.skinning is None else character.skinning.faces, character.blend_shape)
+    if entry is None or any(a is not b for a, b in zip(entry.mesh, mesh)):
+        entry = _handles[id(character), index] = _Handle(character, mesh, ms.DeviceCharacter(character, index), {})
+    return entry
+
+
 def _device_character(character, device: torch.device) -> ms.DeviceCharacter:
-    """The handle every operation here runs on: a DeviceCharacter as given, or for a Character the one DeviceCharacter per (character,
-    device) holding ``character.skinning`` (with its ``faces``) and ``character.blend_shape``. When any of them is replaced, a new handle
-    is made instead of uploading into the old one: a graph recorded with the old skinning keeps its handle (``ctx.dc``) and its tables,
-    and no kernel in flight on another stream reads tables that are being replaced. An old handle is freed with the last graph that uses
-    it."""
-    index = device.index if device.index is not None else torch.cuda.current_device()
-    if isinstance(character, ms.DeviceCharacter):
-        if character.device != index:
-            raise ValueError(f"model parameters are on cuda:{index} but the device character lives on cuda:{character.device}")
-        return character
-    key = (id(character), index)
-    entry = _handles.get(key)
-    faces = None if character.skinning is None else character.skinning.faces
-    if entry is None or entry[1] is not character.skinning or entry[2] is not character.blend_shape or entry[3] is not faces:
-        # the character is kept alive so that its id stays unique
-        entry = (character, character.skinning, character.blend_shape, faces, ms.DeviceCharacter(character, index))
-        _handles[key] = entry
-    return entry[4]
+    """The handle every operation here runs on: a DeviceCharacter as given, or for a Character its registry entry's (``_handle``)."""
+    if not isinstance(character, ms.DeviceCharacter):
+        return _handle(character, device).dc
+    if character.device != _device_index(device):
+        raise ValueError(f"model parameters are on cuda:{_device_index(device)} but the device character lives on cuda:{character.device}")
+    return character
+
+
+def _stream(device: torch.device) -> int:
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+def _float32(t: torch.Tensor, *shape, device=None) -> torch.Tensor:
+    """``t`` detached, as contiguous float32 on ``device`` (default: its own), reshaped to ``shape`` when one is given."""
+    return t.detach().to(device=device, dtype=torch.float32).reshape(shape or t.shape).contiguous()
+
+
+def _restore(t, shape, dtype):
+    return None if t is None else t.reshape(shape).to(dtype)
+
+
+def _ptr(t) -> int:
+    return 0 if t is None else t.data_ptr()
+
+
+def _batch_sum(g, shape):
+    """A per-element gradient [B, ...] of an input of ``shape``: the sum over the batch when the input is shared by it ([...])."""
+    return g.sum(dim=0) if g is not None and g.dim() == len(shape) + 1 else g
 
 
 def _resolve(character, need=None):
@@ -66,30 +97,28 @@ class _JointOp(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, dc, name, x, out_trailing):
-        dev = x.device
         lead = x.shape[:-2] if name.endswith("to_joint_parameters") else x.shape[:-1]
-        rows = x.detach().to(torch.float32).reshape(-1, int(np.prod(x.shape[len(lead):]))).contiguous()
+        rows = _float32(x, -1, int(np.prod(x.shape[len(lead):])))
         B = rows.shape[0]
-        out = torch.empty(B, int(np.prod(out_trailing)), device=dev, dtype=torch.float32)
-        dc.joint_op_device(name, False, B, rows.data_ptr(), out.data_ptr(), stream=torch.cuda.current_stream(dev).cuda_stream)
+        out = torch.empty(B, int(np.prod(out_trailing)), device=x.device, dtype=torch.float32)
+        dc.joint_op_device(name, False, B, rows.data_ptr(), out.data_ptr(), stream=_stream(x.device))
         ctx.dc, ctx.name, ctx.out_numel = dc, name, out.shape[1]
         ctx.in_shape, ctx.in_dtype = x.shape, x.dtype
         ctx.save_for_backward(rows)
-        return out.reshape(*lead, *out_trailing).to(x.dtype)
+        return _restore(out, (*lead, *out_trailing), x.dtype)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, grad_out):
         (rows,) = ctx.saved_tensors
         B = rows.shape[0]
-        dev = rows.device
-        g = grad_out.to(device=dev, dtype=torch.float32).reshape(B, ctx.out_numel).contiguous()
+        g = _float32(grad_out, B, ctx.out_numel)
         gx = torch.empty_like(rows)
         ptrs = (g.data_ptr(), gx.data_ptr())
         if ctx.name not in ms.LINEAR_JOINT_OPS:  # P^T and W^T do not read their input
             ptrs = (rows.data_ptr(),) + ptrs
-        ctx.dc.joint_op_device(ctx.name, True, B, *ptrs, stream=torch.cuda.current_stream(dev).cuda_stream)
-        return None, None, gx.reshape(ctx.in_shape).to(ctx.in_dtype), None
+        ctx.dc.joint_op_device(ctx.name, True, B, *ptrs, stream=_stream(rows.device))
+        return None, None, _restore(gx, ctx.in_shape, ctx.in_dtype), None
 
 
 def _joint_op(name, character, x, what, trailing, out_trailing):
@@ -206,36 +235,32 @@ class _Positions(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, dc, joint, params, parents, offsets):
-        dev = params.device
         N = parents.shape[0]
-        rows = params.detach().to(torch.float32).reshape(-1, params.shape[-1]).contiguous()
+        rows = _float32(params, -1, params.shape[-1])
         B = rows.shape[0]
-        off = offsets.detach().to(torch.float32).contiguous()
+        off = _float32(offsets)
         batched = off.dim() == 3
-        out = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
+        out = torch.empty(B, N, 3, device=params.device, dtype=torch.float32)
         if B * N > 0:
-            dc.positions_device(joint, B, rows.data_ptr(), parents, off.data_ptr(), batched, out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+            dc.positions_device(joint, B, rows.data_ptr(), parents, off.data_ptr(), batched, out.data_ptr(), _stream(params.device))
         ctx.dc, ctx.joint, ctx.parents, ctx.batched = dc, joint, parents, batched
         ctx.params_shape, ctx.params_dtype, ctx.offsets_dtype = params.shape, params.dtype, offsets.dtype
         ctx.save_for_backward(rows, off)
-        return out.reshape(*params.shape[:-1], N, 3).to(params.dtype)
+        return _restore(out, (*params.shape[:-1], N, 3), params.dtype)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, grad_positions):
         rows, off = ctx.saved_tensors
         B, N = rows.shape[0], ctx.parents.shape[0]
-        dev = rows.device
         need_params, need_offsets = ctx.needs_input_grad[2], ctx.needs_input_grad[4]
         gp = torch.zeros_like(rows) if need_params else None
         go = torch.zeros_like(off) if need_offsets else None
         if B * N > 0 and (need_params or need_offsets):  # else the gradients are zero
-            g = grad_positions.to(device=dev, dtype=torch.float32).reshape(B, N, 3).contiguous()
-            ctx.dc.positions_backward_device(ctx.joint, B, rows.data_ptr(), ctx.parents, off.data_ptr(), ctx.batched, g.data_ptr(),
-                                             0 if gp is None else gp.data_ptr(), 0 if go is None else go.data_ptr(),
-                                             torch.cuda.current_stream(dev).cuda_stream)
-        return (None, None, None if gp is None else gp.reshape(ctx.params_shape).to(ctx.params_dtype), None,
-                None if go is None else go.to(ctx.offsets_dtype))
+            g = _float32(grad_positions, B, N, 3)
+            ctx.dc.positions_backward_device(ctx.joint, B, rows.data_ptr(), ctx.parents, off.data_ptr(), ctx.batched, g.data_ptr(), _ptr(gp),
+                                             _ptr(go), _stream(rows.device))
+        return None, None, _restore(gp, ctx.params_shape, ctx.params_dtype), None, _restore(go, off.shape, ctx.offsets_dtype)
 
 
 def _point_parents(name, parents, J):
@@ -314,18 +339,17 @@ class _SkinPoints(torch.autograd.Function):
     @staticmethod
     def forward(ctx, dc, skel_state, rest_points):
         J, V = dc.character.num_joints, dc.skinning.num_vertices
-        dev = skel_state.device
-        st = skel_state.detach().to(torch.float32).reshape(-1, J, 8).contiguous()
+        st = _float32(skel_state, -1, J, 8)
         B = st.shape[0]
-        rest = None if rest_points is None else rest_points.detach().to(device=dev, dtype=torch.float32).contiguous()
+        rest = None if rest_points is None else _float32(rest_points)
         batched = rest is not None and rest.dim() == 3
-        out = torch.empty(B, V, 3, device=dev, dtype=torch.float32)
-        dc.skin_points_device(B, st.data_ptr(), 0 if rest is None else rest.data_ptr(), batched, out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-        ctx.dc, ctx.skinning, ctx.V, ctx.batched, ctx.has_rest = dc, dc.skinning, V, batched, rest is not None
+        out = st.new_empty(B, V, 3)
+        dc.skin_points_device(B, st.data_ptr(), _ptr(rest), batched, out.data_ptr(), _stream(st.device))
+        ctx.dc, ctx.skinning, ctx.V, ctx.batched = dc, dc.skinning, V, batched
         ctx.state_shape, ctx.state_dtype = skel_state.shape, skel_state.dtype
         ctx.rest_dtype = None if rest_points is None else rest_points.dtype
-        ctx.save_for_backward(st, rest if rest is not None else st.new_empty(0))
-        return out.reshape(*skel_state.shape[:-2], V, 3).to(skel_state.dtype)
+        ctx.save_for_backward(st, rest)
+        return _restore(out, (*skel_state.shape[:-2], V, 3), skel_state.dtype)
 
     @staticmethod
     @once_differentiable
@@ -336,16 +360,12 @@ class _SkinPoints(torch.autograd.Function):
             raise RuntimeError("skin_points backward: the DeviceCharacter's skinning was replaced (set_skinning) after the forward; "
                                "keep one DeviceCharacter per skinning, or pass the Character and replace character.skinning instead")
         B, J, _ = st.shape
-        dev = st.device
-        g = grad_points.to(device=dev, dtype=torch.float32).reshape(B, ctx.V, 3).contiguous()
-        need_state, need_rest = ctx.needs_input_grad[1], ctx.needs_input_grad[2] and ctx.has_rest
-        gs = torch.empty(B, J, 8, device=dev, dtype=torch.float32) if need_state else None
+        g = _float32(grad_points, B, ctx.V, 3)
+        need_state, need_rest = ctx.needs_input_grad[1:]  # no gradient is asked of rest_points None
+        gs = st.new_empty(B, J, 8) if need_state else None
         gr = torch.empty_like(rest) if need_rest else None
-        dc.skin_points_backward_device(B, st.data_ptr(), rest.data_ptr() if ctx.has_rest else 0, ctx.batched, g.data_ptr(),
-                                       gs.data_ptr() if gs is not None else 0, gr.data_ptr() if gr is not None else 0,
-                                       torch.cuda.current_stream(dev).cuda_stream)
-        return (None, None if gs is None else gs.reshape(ctx.state_shape).to(ctx.state_dtype),
-                None if gr is None else gr.to(ctx.rest_dtype))
+        dc.skin_points_backward_device(B, st.data_ptr(), _ptr(rest), ctx.batched, g.data_ptr(), _ptr(gs), _ptr(gr), _stream(st.device))
+        return None, _restore(gs, ctx.state_shape, ctx.state_dtype), None if gr is None else gr.to(ctx.rest_dtype)
 
 
 def skin_points(character, skel_state: torch.Tensor, rest_points=None) -> torch.Tensor:
@@ -379,17 +399,16 @@ class _SkinWithBlendShapes(torch.autograd.Function):
     @staticmethod
     def forward(ctx, dc, skel_state, blend_weights):
         J, V = dc.character.num_joints, dc.skinning.num_vertices
-        dev = skel_state.device
-        st = skel_state.detach().to(torch.float32).reshape(-1, J, 8).contiguous()
+        st = _float32(skel_state, -1, J, 8)
         B, K = st.shape[0], blend_weights.shape[-1]
-        w = blend_weights.detach().to(device=dev, dtype=torch.float32).expand(B, K).contiguous()
-        out = torch.empty(B, V, 3, device=dev, dtype=torch.float32)
-        dc.skin_with_blend_shapes_device(B, st.data_ptr(), w.data_ptr(), K, out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        w = _float32(blend_weights.expand(B, K))
+        out = st.new_empty(B, V, 3)
+        dc.skin_with_blend_shapes_device(B, st.data_ptr(), w.data_ptr(), K, out.data_ptr(), _stream(st.device))
         ctx.dc, ctx.skinning, ctx.blend_shape, ctx.V = dc, dc.skinning, dc.blend_shape, V
         ctx.state_shape, ctx.state_dtype = skel_state.shape, skel_state.dtype
         ctx.weights_shape, ctx.weights_dtype = blend_weights.shape, blend_weights.dtype
         ctx.save_for_backward(st, w)
-        return out.reshape(*skel_state.shape[:-2], V, 3).to(skel_state.dtype)
+        return _restore(out, (*skel_state.shape[:-2], V, 3), skel_state.dtype)
 
     @staticmethod
     @once_differentiable
@@ -401,18 +420,12 @@ class _SkinWithBlendShapes(torch.autograd.Function):
                                "set_blend_shape) after the forward; keep one DeviceCharacter per mesh, or pass the Character and replace "
                                "its attributes instead")
         B, J, _ = st.shape
-        K = w.shape[1]
-        dev = st.device
-        g = grad_points.to(device=dev, dtype=torch.float32).reshape(B, ctx.V, 3).contiguous()
-        need_state, need_weights = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-        gs = torch.empty(B, J, 8, device=dev, dtype=torch.float32) if need_state else None
-        gw = torch.empty(B, K, device=dev, dtype=torch.float32) if need_weights else None
-        dc.skin_with_blend_shapes_backward_device(B, st.data_ptr(), w.data_ptr(), K, g.data_ptr(), gs.data_ptr() if gs is not None else 0,
-                                                  gw.data_ptr() if gw is not None else 0, torch.cuda.current_stream(dev).cuda_stream)
-        if gw is not None and len(ctx.weights_shape) == 1:
-            gw = gw.sum(0)  # weights shared by the batch
-        return (None, None if gs is None else gs.reshape(ctx.state_shape).to(ctx.state_dtype),
-                None if gw is None else gw.to(ctx.weights_dtype))
+        g = _float32(grad_points, B, ctx.V, 3)
+        need_state, need_weights = ctx.needs_input_grad[1:]
+        gs = st.new_empty(B, J, 8) if need_state else None
+        gw = torch.empty_like(w) if need_weights else None
+        dc.skin_with_blend_shapes_backward_device(B, st.data_ptr(), w.data_ptr(), w.shape[1], g.data_ptr(), _ptr(gs), _ptr(gw), _stream(st.device))
+        return None, _restore(gs, ctx.state_shape, ctx.state_dtype), _restore(_batch_sum(gw, ctx.weights_shape), ctx.weights_shape, ctx.weights_dtype)
 
 
 def skin_with_blend_shapes(character, skel_state: torch.Tensor, blend_weights: torch.Tensor) -> torch.Tensor:
@@ -452,16 +465,13 @@ def skin_with_blend_shapes(character, skel_state: torch.Tensor, blend_weights: t
 class _VertexNormals(torch.autograd.Function):
     @staticmethod
     def forward(ctx, dc, vertex_positions):
-        V = dc.skinning.num_vertices
-        dev = vertex_positions.device
-        x = vertex_positions.detach().to(torch.float32).reshape(-1, V, 3).contiguous()
-        B = x.shape[0]
-        out = torch.empty(B, V, 3, device=dev, dtype=torch.float32)
-        dc.vertex_normals_device(B, x.data_ptr(), out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        x = _float32(vertex_positions, -1, dc.skinning.num_vertices, 3)
+        out = torch.empty_like(x)
+        dc.vertex_normals_device(x.shape[0], x.data_ptr(), out.data_ptr(), _stream(x.device))
         ctx.dc, ctx.skinning, ctx.faces = dc, dc.skinning, dc.faces
         ctx.in_shape, ctx.in_dtype = vertex_positions.shape, vertex_positions.dtype
         ctx.save_for_backward(x)
-        return out.reshape(vertex_positions.shape).to(vertex_positions.dtype)
+        return _restore(out, ctx.in_shape, ctx.in_dtype)
 
     @staticmethod
     @once_differentiable
@@ -471,12 +481,10 @@ class _VertexNormals(torch.autograd.Function):
         if dc.skinning is not ctx.skinning or dc.faces is not ctx.faces:
             raise RuntimeError("compute_vertex_normals backward: the DeviceCharacter's skinning was replaced (set_skinning) after the forward; "
                                "keep one DeviceCharacter per mesh, or pass the Character and replace character.skinning instead")
-        B, V, _ = x.shape
-        dev = x.device
-        g = grad_normals.to(device=dev, dtype=torch.float32).reshape(B, V, 3).contiguous()
+        g = _float32(grad_normals, *x.shape)
         gx = torch.empty_like(x)
-        dc.vertex_normals_backward_device(B, x.data_ptr(), g.data_ptr(), gx.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-        return None, gx.reshape(ctx.in_shape).to(ctx.in_dtype)
+        dc.vertex_normals_backward_device(x.shape[0], x.data_ptr(), g.data_ptr(), gx.data_ptr(), _stream(x.device))
+        return None, _restore(gx, ctx.in_shape, ctx.in_dtype)
 
 
 def compute_vertex_normals(character, vertex_positions: torch.Tensor) -> torch.Tensor:
@@ -556,13 +564,12 @@ def find_closest_points_on_mesh(character, points_source: torch.Tensor, vertices
     N = points_source.shape[-2]
     dtype = torch.promote_types(points_source.dtype, vertices_target.dtype)
     with torch.no_grad():
-        p = points_source.detach().to(torch.float32).expand(B, N, 3).contiguous()
-        x = vertices_target.detach().to(torch.float32).expand(B, V, 3).contiguous()
+        p = _float32(points_source.expand(B, N, 3))
+        x = _float32(vertices_target.expand(B, V, 3))
         q = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
         face = torch.empty(B, N, device=dev, dtype=torch.int32)
         bary = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
-        dc.closest_points_on_mesh_device(B, N, x.data_ptr(), p.data_ptr(), max_dist, q.data_ptr(), face.data_ptr(), bary.data_ptr(),
-                                         torch.cuda.current_stream(dev).cuda_stream)
+        dc.closest_points_on_mesh_device(B, N, x.data_ptr(), p.data_ptr(), max_dist, q.data_ptr(), face.data_ptr(), bary.data_ptr(), _stream(dev))
         valid = face >= 0
         q, bary = q.to(dtype), bary.to(dtype)
     if not batched:
@@ -660,7 +667,7 @@ def find_closest_points(*args, **kwargs):
         t = t if t.dim() == 3 else t.unsqueeze(0)
         return (t if shared else t.expand(B, rows, 3)).contiguous()
 
-    index = dev.index if dev.index is not None else torch.cuda.current_device()
+    index = _device_index(dev)
     with torch.no_grad(), torch.cuda.device(index):
         p = prep(src, N, False)
         x = prep(tgt, M, not target_batched)
@@ -672,7 +679,7 @@ def find_closest_points(*args, **kwargs):
         ptr = lambda t: 0 if t is None or t.numel() == 0 else t.data_ptr()  # noqa: E731
         if B * N > 0:
             ms.closest_points_device(index, B, N, M, target_batched, ptr(p), ptr(pn), ptr(x), ptr(xn), max_dist, max_normal_dot, ptr(q),
-                                     ptr(qn), ptr(idx), torch.cuda.current_stream(dev).cuda_stream)
+                                     ptr(qn), ptr(idx), _stream(dev))
         valid = idx >= 0
         q = q[..., :D].to(dtype)
         qn = qn.to(dtype) if normals else None

@@ -31,6 +31,7 @@ for p in (ROOT, os.path.join(ROOT, "scripts")):
 from momentum_b200 import character as mc  # noqa: E402
 from momentum_b200 import solver as ms  # noqa: E402
 from momentum_b200 import torch_ik as ti  # noqa: E402
+from momentum_b200 import torch_skeleton as tsk  # noqa: E402
 from momentum_b200.problems import add_test_limits, bodyhands_problem, humanoid_problem  # noqa: E402
 from skeleton_state_bench import TorchFK, card, timed  # noqa: E402
 
@@ -128,8 +129,7 @@ def backward_case(args, dev, name, B, svd_column):
     for _ in range(2):
         total()
     t_total = float(np.median([total() for _ in range(args.reps)]))
-    key = [k for k in ti._handles if k[0] == id(ch) and k[1] == B]
-    fn, blocks = ti._handles[key[-1]]
+    [(fn, blocks)] = tsk._handle(ch, dev).solver_functions.values()  # the one solver function the solves above built
     theta = torch.from_numpy(theta_star.astype(np.float32)).to(dev)
     v = torch.from_numpy(np.random.default_rng(2).normal(size=(B, n)).astype(np.float32)).to(dev)
     stream = torch.cuda.current_stream(dev).cuda_stream

@@ -538,8 +538,9 @@ def test_solve_ik_backward_matches_finite_differences_for_offsets_orientations_a
 
 
 @pytest.mark.gpu
-def test_shared_offsets_cache_and_an_interleaved_forward():
+def test_shared_offsets_cache_in_the_registry_and_an_interleaved_forward():
     from momentum_b200 import torch_ik as ti
+    from momentum_b200 import torch_skeleton as tsk
 
     B = 3
     Pr = _ik_problem(B, 13, reachable=False)
@@ -554,11 +555,12 @@ def test_shared_offsets_cache_and_an_interleaved_forward():
         (_solve(Pr, kinds, opts, po=off).double() * gout).sum().backward()
     assert torch.allclose(shared.grad, batched.grad.sum(0), rtol=1e-12, atol=0.0)
     # new offset values reuse the cached handle
-    count = len(ti._handles)
+    solver_functions = tsk._handle(Pr["ch"], dev).solver_functions
+    count = len(solver_functions)
     for k in range(3):
         off = (shared.detach() + 0.01 * k).requires_grad_(True)
         (_solve(Pr, kinds, opts, po=off).double() * gout).sum().backward()
-    assert len(ti._handles) == count
+    assert tsk._handle(Pr["ch"], dev).solver_functions is solver_functions and len(solver_functions) == count
     # a forward on the same handle between a forward and its backward does not change that backward
 
     def grads(interleave):
