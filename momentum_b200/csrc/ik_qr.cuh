@@ -6,8 +6,10 @@
 // when a block does not fit beside R — by Householder reflectors, column by column (math/online_householder_qr.cpp:171-221):
 //     [beta, mu] from (R(i,i), A(:,i));  every remaining column j (and the right-hand side): s = beta (R(i,j) + v . A(:,j)),
 //     R(i,j) -= s, A(:,j) -= s v      with v = A(:,i) / v1, v_1 = 1 implicit.
-// Thread j owns column j of the chunk for the whole sweep: its dot product, its update and the squared norm of the updated column
-// (the next reflector's sigma) are thread-local, so a column step costs ONE block barrier. A column that is still structurally
+// At step i, thread t takes the columns i + 1 + t, i + 1 + t + 256, ... (and the right-hand side when it falls on one of them): their
+// dot products, updates and the squared norms of the updated columns (the next reflectors' sigma). Which thread holds a column moves by
+// one at every step, so nothing carries over in a thread: what step i + 1 reads (the norms and the updated chunk columns) was written
+// by other threads at step i and is ordered by the ONE block barrier that ends each step. A column that is still structurally
 // zero in this chunk with R(i,j) = 0 is skipped (the reference's beta == 0 / exact-zero cases). Then R x = y by one warp, g = R^T y
 // (= J^T r, for the line search), theta -= delta and the SolverT bookkeeping through the same tail as the Cholesky kernels.
 // R^T R = J^T J + lambda I, so the step equals the Cholesky path's up to rounding — without squaring the condition number.

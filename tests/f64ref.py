@@ -50,7 +50,10 @@ SOLVE_K = {
     "tiles": 0.06,           # tile-scheduled kernel (FUSED_OFF) worst measured k 0.0148 (bodyhands300, 3xTF32 JtJ)
     "gram_cholesky": 0.004,  # Gram + Cholesky in one launch     worst measured k 0.00101 (humanoid72)
     "persistent": 0.0045,    # persistent whole-solve kernel     worst measured k 0.00113 (humanoid72 with a disabled subset)
-    "qr": 0.006,             # QR step                           worst measured k 0.00154 (humanoid72, split block)
+    "qr": 0.006,             # QR step                           worst measured k 0.00154 (humanoid72, split block); over the cases
+                             # of tests/test_qr_bounds.py 0.00018 (n = 257), 0.00098 with lambda = 0, and for the trust-region
+                             # step, held to F times this limit after F Householder folds (J and each damping block), 0.00126
+                             # per fold (five folds, a step taken after a rejection); H100 80GB HBM3, 700 W power limit
 }
 
 
