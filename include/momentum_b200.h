@@ -282,6 +282,31 @@ int mb2_character_apply_inverse_parameter_transform_device(const mb2_character* 
                                                            float* model_parameters_device, void* cuda_stream);
 int mb2_character_apply_inverse_parameter_transform_backward_device(const mb2_character* c, int32_t batch, const float* grad_model_parameters_device,
                                                                     float* grad_joint_parameters_device, void* cuda_stream);
+/* Parameter limits as character operations. The limit tables are built when the limits are set (mb2_character_set_parameter_limits),
+ * which keeps accepting limits whose indices are out of range: these entries then return MB2_ERR_INVALID_ARGUMENT with the reason, naming
+ * the limit, in mb2_last_error, as the solver's LimitErrorFunction blocks reject them when planned.
+ * mb2_character_num_limit_residuals: R, the rows of LimitErrorFunction over the limits: one per limit in list order, none for
+ * MinMaxJointPassive, three for an Ellipsoid. */
+int mb2_character_num_limit_residuals(const mb2_character* c, int32_t* out);
+/* The residual [B][R] of LimitErrorFunction at weight 1 with the L2 loss (limit_error_function.cpp:992-1121) for model parameters [B][n]:
+ * the rows getJacobian returns, sqrt(kLimitWeight w) (Ellipsoid: sqrt(kLimitWeight kLimitPositionWeight w)) times the limit's residual, 0
+ * for an inactive limit; the sum of squares is getError. Joint-space limits read P theta + o, Ellipsoids the skeleton state of theta. Its
+ * backward writes dLoss / d theta [B][n] from dLoss / d residual [B][R]: the exact derivative of the rows, an Ellipsoid's projection onto
+ * the ellipsoid and its ellipsoid parent's motion included (not computeEllipsoidJacobian's truncated chain). Fixed summation order, no
+ * atomics, no scratch. R == 0 is valid (the residual arrays may then be NULL; the gradient is zero). The argument rules of
+ * mb2_character_skeleton_state_device. */
+int mb2_character_parameter_limits_residual_device(const mb2_character* c, int32_t batch, const float* model_parameters_device, float* residual_device,
+                                                   void* cuda_stream);
+int mb2_character_parameter_limits_residual_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                            const float* grad_residual_device, float* grad_model_parameters_device, void* cuda_stream);
+/* pymomentum apply_model_param_limits (tensor_parameter_transform.cpp:638-697): [B][n] -> [B][n], each parameter a MinMax limit names
+ * clamped to [min, max] as torch.clamp does it (NaN stays NaN), every other parameter passed through; other limit types are ignored.
+ * When several MinMax limits name one parameter, the last in list order decides. Its backward passes dLoss / d out where
+ * min <= theta <= max (every unlimited parameter) and writes 0 elsewhere; it reads the input. */
+int mb2_character_apply_model_parameter_limits_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                      float* clamped_model_parameters_device, void* cuda_stream);
+int mb2_character_apply_model_parameter_limits_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                               const float* grad_clamped_device, float* grad_model_parameters_device, void* cuda_stream);
 /* pymomentum joint_parameters_to_skeleton_state (tensor_skeleton_state.cpp:203-343, :488-491): the forward kinematics of
  * mb2_character_skeleton_state_device from joint parameters [B][7 J] -> [B][J][8] */
 int mb2_character_joint_parameters_to_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
@@ -543,9 +568,10 @@ int mb2_solver_get_fused_profile(mb2_solver* s, int32_t* fused, int32_t* groups,
 int mb2_solver_function_get_sweep_launch(mb2_solver_function* f, int32_t jacobian, int64_t out[5]);
 /* What the character operations' per-instance kernels would launch for `batch` instances, planned by the code that launches them and
  * with nothing enqueued. op: 0 model_parameters_to_skeleton_state, 1 joint_parameters_to_skeleton_state, 2 model_parameters_to_positions,
- * 3 joint_parameters_to_positions (num_points points); backward != 0: their backward. out: [0] warps per instance W (1, 2, 4 or 8),
+ * 3 joint_parameters_to_positions (num_points points), 5 parameter_limits_residual (num_points is ignored; the kernel runs the FK when the
+ * character has an Ellipsoid limit); backward != 0: their backward. out: [0] warps per instance W (1, 2, 4 or 8),
  * [1] instances per CTA, [2] threads per CTA, [3] CTAs, [4] dynamic shared memory per CTA in bytes, [5] 1 when the point tables are
- * staged in shared memory. All zero when nothing runs (batch 0, positions with no point). An instance that does not fit in shared
+ * staged in shared memory. All zero when nothing runs (batch 0, positions with no point, limits with no residual row). An instance that does not fit in shared
  * memory next to the tables is refused with MB2_ERR_CUDA, as the operation refuses it. The shared-offset positions backward launches
  * per slice of the batch when its per-instance offset rows exceed 256 MiB of scratch: this reports one launch of `batch` instances.
  * No reference counterpart. */

@@ -718,6 +718,84 @@ def synthetic_blend_shape(ch: Character, skinning: Skinning, num_shapes: int, se
     return BlendShape(x.astype(np.float32), S.astype(np.float32))
 
 
+def synthetic_limits(ch: Character, seed: int = 0) -> List[ParameterLimit]:
+    """A seeded, realistic ParameterLimits set for any rig, in list order:
+
+    * MinMax on every model parameter, sized by what it drives (rotation +-0.4..1.5 rad, translation +-0.5..2 bone lengths, scale
+      +-0.05..0.3), and a second, tighter MinMax on every fifth parameter;
+    * MinMaxJoint on a rotation row of every third joint, and a MinMaxJointPassive on every seventh;
+    * Linear between pairs of parameters, LinearJoint between a joint's rotation row and its parent's, each with the (0, 0) range
+      (everywhere) or a finite one;
+    * HalfPlane on pairs of parameters with a random unit normal;
+    * one Ellipsoid per limb: for each leaf joint at depth 2 or more, the leaf's point (an offset of up to 0.2 bone lengths) against an
+      ellipsoid in its grandparent's frame around the point's rest position, with axes of 0.3 to 1 times the distance.
+
+    The rig's own ``limits`` are not changed: assign the result to use it."""
+    rng = np.random.default_rng(seed)
+    J, n = ch.num_joints, ch.num_params
+    parents = np.asarray(ch.parents)
+    t, q, s = forward_kinematics(ch, np.zeros((1, n)))
+    t, q, s = t[0], q[0], s[0]
+    length = np.where(parents >= 0, np.linalg.norm(t - t[np.maximum(parents, 0)], axis=-1), 0.0)
+    length = np.where(length > 0, length, max(float(length.max()), 1.0))
+    # the joint-parameter rows each model parameter drives
+    rows_of = [[] for _ in range(n)]
+    for r in range(7 * J):
+        for k in range(ch.pt_outer[r], ch.pt_outer[r + 1]):
+            rows_of[int(ch.pt_inner[k])].append(r)
+    driven = [r for r in range(7 * J) if ch.pt_outer[r + 1] > ch.pt_outer[r]]
+    U = lambda a, b: float(rng.uniform(a, b))
+    L = []
+    for p in range(n):
+        r = rows_of[p][0] if rows_of[p] else 3
+        d = r % 7
+        half = U(0.4, 1.5) if 3 <= d < 6 else (U(0.5, 2.0) * length[r // 7] if d < 3 else U(0.05, 0.3))
+        L.append(ParameterLimit(LIMIT_MINMAX, U(0.5, 2.0), (p,), (-half * U(0.6, 1.0), half)))
+    for p in range(0, n, 5):
+        lo, hi = L[p].f
+        L.append(ParameterLimit(LIMIT_MINMAX, U(0.5, 2.0), (p,), (0.7 * lo, 0.7 * hi)))
+    rot_rows = [r for r in driven if 3 <= r % 7 < 6]
+    for j in range(0, J, 3):
+        rows = [r for r in rot_rows if r // 7 == j]
+        if rows:
+            h = U(0.3, 1.0)
+            L.append(ParameterLimit(LIMIT_MINMAX_JOINT, U(0.5, 2.0), (j, int(rng.choice(rows)) % 7), (-h, h)))
+    for j in range(0, J, 7):
+        L.append(ParameterLimit(LIMIT_MINMAX_JOINT_PASSIVE, 1.0, (j, 3), (-0.5, 0.5)))
+    rot_params = [p for p in range(n) if rows_of[p] and 3 <= rows_of[p][0] % 7 < 6]
+    for k in range(max(2, len(rot_params) // 8)):
+        ref, tgt = (int(x) for x in rng.choice(rot_params, 2, replace=False))
+        rmin, rmax = (0.0, 0.0) if k % 2 == 0 else (-U(0.2, 1.0), U(0.2, 1.0))
+        L.append(ParameterLimit(LIMIT_LINEAR, U(0.5, 2.0), (ref, tgt), (U(0.3, 1.0), U(-0.1, 0.1), rmin, rmax)))
+    for k, r in enumerate(rot_rows[1::max(1, len(rot_rows) // 10)]):
+        j = r // 7
+        prows = [x for x in rot_rows if x // 7 == parents[j]] if parents[j] >= 0 else []
+        if not prows:
+            continue
+        ref = int(rng.choice(prows))
+        rmin, rmax = (0.0, 0.0) if k % 2 == 0 else (-U(0.2, 1.0), U(0.2, 1.0))
+        L.append(ParameterLimit(LIMIT_LINEAR_JOINT, U(0.5, 2.0), (ref // 7, ref % 7, j, r % 7), (U(0.3, 1.0), U(-0.1, 0.1), rmin, rmax)))
+    for _ in range(max(2, len(rot_params) // 10)):
+        p1, p2 = (int(x) for x in rng.choice(rot_params, 2, replace=False))
+        a = U(0, 2 * np.pi)
+        L.append(ParameterLimit(LIMIT_HALFPLANE, U(0.5, 2.0), (p1, p2), (float(np.cos(a)), float(np.sin(a)), U(-0.5, 0.2))))
+    depth = ch.depth()
+    leaves = [j for j in range(J) if j not in set(int(p) for p in parents) and depth[j] >= 2]
+    for leaf in leaves:
+        e = int(parents[parents[leaf]])
+        off = rng.uniform(-0.2, 0.2, 3) * length[leaf]
+        x = t[leaf] + s[leaf] * _qrot(q[leaf], off)
+        local = _qrot(q[e] * np.array([-1, -1, -1, 1]), x - t[e]) / s[e]
+        dist = max(float(np.linalg.norm(local)), 1e-3)
+        A = np.linalg.qr(rng.normal(size=(3, 3)))[0] @ np.diag(rng.uniform(0.3, 1.0, 3) * dist)
+        c = local + rng.uniform(-0.1, 0.1, 3) * dist
+        M = np.concatenate([A, c[:, None]], 1)
+        Ai = np.linalg.inv(A)
+        Mi = np.concatenate([Ai, (-Ai @ c)[:, None]], 1)
+        L.append(ParameterLimit(LIMIT_ELLIPSOID, U(0.5, 2.0), (e, leaf), tuple(M.reshape(-1)) + tuple(Mi.reshape(-1)) + tuple(off)))
+    return L
+
+
 def skin_with_blend_shapes(ch: Character, skel_state, blend_weights):
     """skinWithBlendShapes in float64 (blend_shape_skinning.cpp:50-140): the rest mesh base_shape + sum_k w_k shape_vectors[k] over the
     first K' = len(w) shape vectors, skinned by ``skin_points``. skel_state [B,J,8] or [J,8]; blend_weights [K'] (shared) or [B,K']."""

@@ -116,6 +116,12 @@ struct MeshFaceBuffers {
 struct MeshTreeBuffers {
   DeviceBuffer<int32_t> nodeStart, nodeCount, leafFaces, levelStart;
 };
+// the device copy of a HostLimitTables (LimitTables, SkeletonTables::paramClamp)
+struct LimitBuffers {
+  DeviceBuffer<LimitDesc> limits;
+  DeviceBuffer<float> ellipsoidData, rowCoef, paramCoef, paramClamp;
+  DeviceBuffer<int32_t> jointStart, jointEntry, rowStart, rowLimit, paramStart, paramLimit;
+};
 
 struct mb2_character {
   int device{0};
@@ -127,6 +133,9 @@ struct mb2_character {
   DeviceBuffer<int32_t> invStart, invRows, invRowStart, invParams; // inverse ParameterTransform (HostCharacter::buildInverseTables)
   DeviceBuffer<float> invVals, invRowVals;
   uint64_t limitsVersion{0};
+  // the limits as parameter_limits_residual and apply_model_param_limits read them, built and uploaded whenever the limits are set
+  HostLimitTables limits;
+  std::unique_ptr<LimitBuffers> limitsDev; // replaced whole by installLimitTables
   // linear-blend skinning (mb2_character_set_skinning): numVertices == 0 when there is none
   HostSkinning skin;
   std::unique_ptr<SkinBuffers> skinDev; // replaced whole by mb2_character_set_skinning, never rewritten in place
@@ -146,6 +155,7 @@ struct mb2_character {
   BlendShapeTables blendShapeTables() const;
   MeshFaceTables meshFaceTables() const;
   MeshTreeTables meshTreeTables() const;
+  LimitTables limitTables() const;
 };
 
 struct DeviceSchedule {
@@ -252,7 +262,14 @@ CharacterTables mb2_character::tables() const {
 }
 
 SkeletonTables mb2_character::skeletonTables() const {
-  return SkeletonTables{childStart.p, children.p, ptColStart.p, ptColRows.p, ptColVals.p, invStart.p, invRows.p, invVals.p, invRowStart.p, invParams.p, invRowVals.p};
+  return SkeletonTables{childStart.p, children.p,  ptColStart.p, ptColRows.p, ptColVals.p, invStart.p,
+                        invRows.p,    invVals.p,   invRowStart.p, invParams.p, invRowVals.p, limitsDev ? limitsDev->paramClamp.p : nullptr};
+}
+
+LimitTables mb2_character::limitTables() const {
+  const LimitBuffers& d = *limitsDev;
+  return LimitTables{int32_t(limits.limits.size()), limits.numRows, limits.ellipsoid ? 1 : 0, d.limits.p, d.ellipsoidData.p, d.jointStart.p,
+                     d.jointEntry.p, d.rowStart.p, d.rowLimit.p, d.rowCoef.p, d.paramStart.p, d.paramLimit.p, d.paramCoef.p};
 }
 
 SkinTables mb2_character::skinTables() const {
@@ -300,6 +317,24 @@ int installMeshTree(mb2_character* c, HostMeshTree&& t) {
     MB2_CUDA(d.levelStart.upload(t.levelStart, nullptr));
     return MB2_OK;
   }, present);
+}
+
+// builds the limit tables of c's limits and installs them (rejected limits install empty tables and keep the reason)
+int installLimitTables(mb2_character* c) {
+  return installTables(c->device, c->limitsDev, c->limits, makeLimitTables(c->host), [](LimitBuffers& d, const HostLimitTables& t) -> int {
+    MB2_CUDA(d.limits.upload(t.limits, nullptr));
+    MB2_CUDA(d.ellipsoidData.upload(t.ellipsoidData, nullptr));
+    MB2_CUDA(d.jointStart.upload(t.jointStart, nullptr));
+    MB2_CUDA(d.jointEntry.upload(t.jointEntry, nullptr));
+    MB2_CUDA(d.rowStart.upload(t.rowStart, nullptr));
+    MB2_CUDA(d.rowLimit.upload(t.rowLimit, nullptr));
+    MB2_CUDA(d.rowCoef.upload(t.rowCoef, nullptr));
+    MB2_CUDA(d.paramStart.upload(t.paramStart, nullptr));
+    MB2_CUDA(d.paramLimit.upload(t.paramLimit, nullptr));
+    MB2_CUDA(d.paramCoef.upload(t.paramCoef, nullptr));
+    MB2_CUDA(d.paramClamp.upload(t.paramClamp, nullptr));
+    return MB2_OK;
+  });
 }
 } // namespace
 
@@ -612,6 +647,8 @@ int mb2_character_create(int device, int32_t J, const int32_t* parents, const fl
   MB2_CUDA(c->invParams.upload(h.invParams, nullptr));
   MB2_CUDA(c->invRowVals.upload(h.invRowVals, nullptr));
   MB2_CUDA(cudaStreamSynchronize(nullptr));
+  rc = installLimitTables(c.get()); // no limits yet: empty tables and a pass-through clamp
+  if (rc != MB2_OK) return rc;
   *out = c.release();
   return MB2_OK;
 }
@@ -621,7 +658,7 @@ int mb2_character_set_parameter_limits(mb2_character* c, int32_t count, const mb
   const std::string err = setParameterLimits(c->host, count, limits);
   if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
   c->limitsVersion++;
-  return MB2_OK;
+  return installLimitTables(c);
 }
 
 void mb2_character_destroy(mb2_character* c) { delete c; }
@@ -658,6 +695,8 @@ int mb2_character_clone(const mb2_character* c, int device, mb2_character** out)
   if (rc != MB2_OK) return rc;
   copy->host.limits = h.limits;
   copy->limitsVersion = 1;
+  rc = installLimitTables(copy);
+  if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
   const HostSkinning& s = c->skin;
   if (s.numVertices > 0) { // back to [V][8] slots: the active ones, then zero weights
     std::vector<int32_t> index(size_t(s.numVertices) * kSkinMaxInfluences, 0);
@@ -1079,6 +1118,7 @@ int jointOpDevice(const mb2_character* c, int32_t batch, JointOp op, const char*
   if (batch == 0) return MB2_OK;
   const bool needIn = !(backward && (op == kJointOpParameterTransform || op == kJointOpInverseParameterTransform));
   MB2_CHECK((in != nullptr || !needIn) && out != nullptr && (!backward || grad != nullptr), "null argument");
+  MB2_CHECK(op != kJointOpClampParameters || c->limits.rejected.empty(), c->limits.rejected);
   MB2_DEVICE_GUARD(c->device);
   MB2_CHECK(onDevice(c->device, {out}, {in, grad}), std::string(name) + ": every array must be device memory on the character's device");
   NvtxRange range(name);
@@ -1122,6 +1162,61 @@ int mb2_character_apply_inverse_parameter_transform_backward_device(const mb2_ch
   return jointOpDevice(c, batch, kJointOpInverseParameterTransform, "applyInverseParameterTransformBackward", nullptr, grad_model_parameters_device,
                        grad_joint_parameters_device, cuda_stream, true);
 }
+int mb2_character_apply_model_parameter_limits_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                      float* clamped_model_parameters_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpClampParameters, "applyModelParameterLimits", model_parameters_device, nullptr, clamped_model_parameters_device,
+                       cuda_stream, false);
+}
+int mb2_character_apply_model_parameter_limits_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                               const float* grad_clamped_device, float* grad_model_parameters_device, void* cuda_stream) {
+  return jointOpDevice(c, batch, kJointOpClampParameters, "applyModelParameterLimitsBackward", model_parameters_device, grad_clamped_device,
+                       grad_model_parameters_device, cuda_stream, true);
+}
+
+int mb2_character_num_limit_residuals(const mb2_character* c, int32_t* out) {
+  MB2_CHECK(c != nullptr && out != nullptr, "null argument");
+  MB2_CHECK(c->limits.rejected.empty(), c->limits.rejected);
+  *out = c->limits.numRows;
+  return MB2_OK;
+}
+
+namespace {
+// both directions of mb2_character_parameter_limits_residual*_device: residual is the forward's output, gradResidual the backward's input
+int parameterLimitsDevice(const mb2_character* c, int32_t batch, const float* theta, float* residual, const float* gradResidual, float* gradTheta,
+                          void* stream, bool backward) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(batch >= 0, "batch must not be negative");
+  MB2_CHECK(c->limits.rejected.empty(), c->limits.rejected);
+  if (batch == 0) return MB2_OK;
+  const bool rows = c->limits.numRows > 0;
+  MB2_CHECK(theta != nullptr && (backward ? gradTheta != nullptr && (gradResidual != nullptr || !rows) : residual != nullptr || !rows), "null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(onDevice(c->device, {theta}, {residual, gradResidual, gradTheta}), "parameter limits: every array must be device memory on the character's device");
+  NvtxRange range(backward ? "parameterLimitsResidualBackward" : "parameterLimitsResidual");
+  ParameterLimitArgs a{};
+  a.T = c->tables();
+  a.S = c->skeletonTables();
+  a.L = c->limitTables();
+  a.numChildren = int(c->host.children.size());
+  a.batch = batch;
+  a.theta = theta;
+  a.residual = residual;
+  a.gradResidual = gradResidual;
+  a.gradTheta = gradTheta;
+  MB2_CUDA(launchParameterLimits(a, backward, (cudaStream_t)stream));
+  return MB2_OK;
+}
+} // namespace
+
+int mb2_character_parameter_limits_residual_device(const mb2_character* c, int32_t batch, const float* model_parameters_device, float* residual_device,
+                                                   void* cuda_stream) {
+  return parameterLimitsDevice(c, batch, model_parameters_device, residual_device, nullptr, nullptr, cuda_stream, false);
+}
+int mb2_character_parameter_limits_residual_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
+                                                            const float* grad_residual_device, float* grad_model_parameters_device, void* cuda_stream) {
+  return parameterLimitsDevice(c, batch, model_parameters_device, nullptr, grad_residual_device, grad_model_parameters_device, cuda_stream, true);
+}
+
 int mb2_character_joint_parameters_to_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
                                                             float* skeleton_state_device, void* cuda_stream) {
   return skeletonStateDevice(c, batch, joint_parameters_device, nullptr, skeleton_state_device, cuda_stream, false, true);
@@ -2053,12 +2148,21 @@ void instanceLaunchWords(const InstanceLaunchQuery& q, int64_t out[6]) {
 
 int mb2_character_get_instance_launch(const mb2_character* c, int32_t op, int32_t backward, int32_t batch, int32_t num_points, int64_t out[6]) {
   MB2_CHECK(c != nullptr && out != nullptr, "null argument");
-  MB2_CHECK(op >= kInstanceOpModelSkeletonState && op <= kInstanceOpJointPositions, "instance launch: op must be 0, 1, 2 or 3");
+  MB2_CHECK((op >= kInstanceOpModelSkeletonState && op <= kInstanceOpJointPositions) || op == kInstanceOpParameterLimits,
+            "instance launch: op must be 0, 1, 2, 3 or 5");
   MB2_CHECK(batch >= 0 && num_points >= 0, "instance launch: batch and num_points must not be negative");
+  MB2_CHECK(op != kInstanceOpParameterLimits || c->limits.rejected.empty(), c->limits.rejected);
   MB2_DEVICE_GUARD(c->device);
   InstanceLaunchQuery q;
   const bool joint = op == kInstanceOpJointSkeletonState || op == kInstanceOpJointPositions;
-  if (op == kInstanceOpModelSkeletonState || op == kInstanceOpJointSkeletonState) {
+  if (op == kInstanceOpParameterLimits) {
+    ParameterLimitArgs a{};
+    a.T = c->tables();
+    a.L = c->limitTables();
+    a.numChildren = int(c->host.children.size());
+    a.batch = batch;
+    MB2_CUDA(launchParameterLimits(a, backward != 0, nullptr, &q));
+  } else if (op == kInstanceOpModelSkeletonState || op == kInstanceOpJointSkeletonState) {
     SkeletonStateArgs a{};
     a.T = c->tables();
     a.numChildren = int(c->host.children.size());

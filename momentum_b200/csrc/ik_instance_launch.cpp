@@ -27,10 +27,13 @@ InstanceLaunch planInstanceGroups(size_t perInstance, size_t tableBytes, long ba
 }
 
 InstanceLaunch planInstanceOp(const CharacterTables& C, int numChildren, int op, bool backward, int numPoints, long batch, size_t smemBudget,
-                              int numSms) {
+                              int numSms, bool limitsFk) {
   if (op == kInstanceOpInputGradients)
     return planInstanceGroups(sizeof(float) * inputGradientSmemPerInstanceFloats(C.numJoints, C.numParams), characterTableWords(C) * 4, batch,
                               smemBudget, numSms);
+  if (op == kInstanceOpParameterLimits)
+    return planInstanceGroups(sizeof(float) * parameterLimitsSmemPerInstanceFloats(C.numJoints, C.numParams, backward, limitsFk),
+                              parameterLimitsTableBytes(C, numChildren, backward, limitsFk), batch, smemBudget, numSms);
   const bool joint = op == kInstanceOpJointSkeletonState || op == kInstanceOpJointPositions;
   const size_t per = sizeof(float) * skeletonStateSmemPerInstanceFloats(C.numJoints, C.numParams, backward, joint);
   const size_t tables = skeletonStateTableBytes(C, numChildren, backward, joint);

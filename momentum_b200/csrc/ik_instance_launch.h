@@ -1,5 +1,6 @@
-// The launch of the per-instance kernels of the character operations (skeletonStateKernel, positionsKernel, inputGradientKernel): their
-// shared memory per instance and per CTA, and the one rule that picks the warps per instance W and the instance groups per CTA from it.
+// The launch of the per-instance kernels of the character operations (skeletonStateKernel, positionsKernel, inputGradientKernel,
+// parameterLimitsKernel): their shared memory per instance and per CTA, and the one rule that picks the warps per instance W and the
+// instance groups per CTA from it.
 // Host code shared by the library (ik_kernels.cu) and the CPU emulator (tests/emu), so that the launch a test sizes a rig for is the
 // launch that runs.
 #pragma once
@@ -45,6 +46,22 @@ inline size_t pointTableBytes(int numPoints, int J, bool backward) {
   if (backward) w += tableWords(size_t(J) + 1, 4) + tableWords(size_t(numPoints), 4);
   return w * 4;
 }
+// parameterLimitsKernel, per instance: theta [n], the joint parameters [7 J], with the FK (an Ellipsoid among the limits) the joint
+// states [J][17]; backward: the joint-parameter gradient [7 J] and, with the FK, the subtree sums [J][11]
+MB2_HD size_t parameterLimitsSmemPerInstanceFloats(int J, int n, bool backward, bool fk) {
+  size_t f = skelAligned(size_t(n)) + skelAligned(size_t(J) * kParametersPerJoint);
+  if (fk) f += skelAligned(size_t(J) * kJointStateStride);
+  if (backward) f += skelAligned(size_t(J) * kParametersPerJoint) + (fk ? skelAligned(size_t(J) * kSkelAccStride) : 0);
+  return f;
+}
+// its tables: the character's; backward: with the FK the children in CSR, and the ParameterTransform in CSC. The limit tables are read
+// from global memory.
+inline size_t parameterLimitsTableBytes(const CharacterTables& C, int numChildren, bool backward, bool fk) {
+  size_t w = characterTableWords(C);
+  if (backward && fk) w += tableWords(size_t(C.numJoints) + 1, 4) + tableWords(size_t(numChildren), 4);
+  if (backward) w += tableWords(size_t(C.numParams) + 1, 4) + tableWords(size_t(C.ptNnz), 4) * 2;
+  return w * 4;
+}
 // inputGradientKernel, per instance: theta [n], v [n], joint states [J][17], joint motions [J][7]; its tables are the character's
 MB2_HD size_t inputGradientSmemPerInstanceFloats(int J, int n) {
   return 2 * skelAligned(size_t(n)) + skelAligned(size_t(J) * kJointStateStride) + skelAligned(size_t(J) * kTangentStride);
@@ -72,10 +89,12 @@ enum InstanceOp : int32_t { // the operations whose kernels run in this frame (m
   kInstanceOpModelPositions = 2,     // positionsKernel<kBackward, W, false, kStagePoints>
   kInstanceOpJointPositions = 3,     // positionsKernel<kBackward, W, true, kStagePoints>
   kInstanceOpInputGradients = 4,     // inputGradientKernel<W> (forward only)
+  kInstanceOpParameterLimits = 5,    // parameterLimitsKernel<kBackward, W, kEllipsoid>
 };
 // The launch of one operation over `batch` instances of the character C (numChildren: entries of its children table), with numPoints
-// points for the positions, whose tables are staged when that costs no instance per CTA.
+// points for the positions, whose tables are staged when that costs no instance per CTA. limitsFk: for the parameter limits, that the
+// character has an Ellipsoid limit, so the kernel runs the FK passes (LimitTables::ellipsoid).
 InstanceLaunch planInstanceOp(const CharacterTables& C, int numChildren, int op, bool backward, int numPoints, long batch, size_t smemBudget,
-                              int numSms);
+                              int numSms, bool limitsFk = false);
 
 } // namespace mb2

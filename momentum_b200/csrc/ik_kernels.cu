@@ -302,10 +302,10 @@ cudaError_t persistentGrid(K kernel, int threads, size_t smem, long work, int* g
 // 4, 8. With `query`, the launch is reported there and nothing is enqueued.
 template <class Args>
 cudaError_t launchInstanceGroups(void (*const kernels[4])(Args), const Args& a, int numChildren, int op, bool backward, int numPoints, cudaStream_t stream,
-                                 InstanceLaunchQuery* query) {
+                                 InstanceLaunchQuery* query, bool limitsFk = false) {
   if (query) *query = InstanceLaunchQuery{};
   if (a.batch <= 0) return cudaSuccess;
-  const InstanceLaunch l = planInstanceOp(a.T, numChildren, op, backward, numPoints, a.batch, size_t(g_maxSmemOptin), g_numSms);
+  const InstanceLaunch l = planInstanceOp(a.T, numChildren, op, backward, numPoints, a.batch, size_t(g_maxSmemOptin), g_numSms, limitsFk);
   if (l.warpsPerInstance == 0) return cudaErrorInvalidConfiguration; // not even one instance fits next to the tables
   const int w = l.warpsPerInstance == 1 ? 0 : l.warpsPerInstance == 2 ? 1 : l.warpsPerInstance == 4 ? 2 : 3;
   int grid = 0;
@@ -360,17 +360,21 @@ __global__ void __launch_bounds__(kJointOpThreads) inverseParameterTransformKern
 __global__ void __launch_bounds__(kJointOpThreads) inverseParameterTransformBackwardKernel(const JointOpArgs a) {
   jointOpGrid<kJointOpInverseParameterTransform, true>(a);
 }
+__global__ void __launch_bounds__(kJointOpThreads) clampParametersKernel(const JointOpArgs a) { jointOpGrid<kJointOpClampParameters, false>(a); }
+__global__ void __launch_bounds__(kJointOpThreads) clampParametersBackwardKernel(const JointOpArgs a) { jointOpGrid<kJointOpClampParameters, true>(a); }
 
 cudaError_t launchJointOp(const JointOpArgs& a, JointOp op, bool backward, cudaStream_t stream) {
   using K = void (*)(JointOpArgs);
-  static const K kernels[5][2] = {{parameterTransformKernel, parameterTransformBackwardKernel}, {localStateKernel, localStateBackwardKernel},
+  static const K kernels[6][2] = {{parameterTransformKernel, parameterTransformBackwardKernel}, {localStateKernel, localStateBackwardKernel},
                                   {localToJointParametersKernel, localToJointParametersBackwardKernel},
                                   {worldToJointParametersKernel, worldToJointParametersBackwardKernel},
-                                  {inverseParameterTransformKernel, inverseParameterTransformBackwardKernel}};
+                                  {inverseParameterTransformKernel, inverseParameterTransformBackwardKernel},
+                                  {clampParametersKernel, clampParametersBackwardKernel}};
   if (a.batch <= 0) return cudaSuccess;
   const long rows = long(a.T.numJoints) * kParametersPerJoint;
   const long per = op == kJointOpParameterTransform          ? (backward ? a.T.numParams : rows)
                    : op == kJointOpInverseParameterTransform ? (backward ? rows : a.T.numParams)
+                   : op == kJointOpClampParameters           ? a.T.numParams
                                                              : a.T.numJoints;
   const long items = long(a.batch) * per;
   if (items == 0) return cudaSuccess;
@@ -722,6 +726,65 @@ cudaError_t launchPositionsBackward(const PositionArgs& a, cudaStream_t stream) 
     if (e == cudaSuccess) e = f;
   }
   return e;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Parameter-limit residuals (ik_device.cuh limitPasses / limitGradPasses), in the per-instance frame of skeletonStateKernel: theta and the
+// joint parameters P theta + o in shared memory, then lanes = limits write their rows. kEllipsoid (the character has an Ellipsoid limit,
+// a fact of its limit tables): the FK passes from the joint parameters run before, with the DOF axes in the backward.
+//   backward:  Ellipsoid seeds by joint (skelGradSeed's layout) and skelGradTail's fold when kEllipsoid; the joint-space terms added to
+//              the joint-parameter gradient by row; P^T plus the parameter-space terms by model parameter. Each a host-planned CSR in
+//              limit-list order: no atomics, and no result depends on the launch shape.
+// The limit tables are read from global memory; they are small and shared by the batch.
+// ------------------------------------------------------------------------------------------------
+template <bool kBackward, int W, bool kEllipsoid>
+__global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) parameterLimitsKernel(const ParameterLimitArgs a) {
+  extern __shared__ __align__(16) float smem[];
+  CharacterTables T = a.T;
+  SkeletonTables S = a.S;
+  const LimitTables L = a.L;
+  const WarpLanes<W> g = WarpLanes<W>::of(threadIdx.x >> 5, threadIdx.x & 31);
+  const int groupsPerCta = (blockDim.x >> 5) / W;
+  const int J = T.numJoints, n = T.numParams, R = L.numRows;
+  const int perGroup = int(parameterLimitsSmemPerInstanceFloats(J, n, kBackward, kEllipsoid));
+  float* th = smem + size_t(g.group) * perGroup;
+  float* jp = th + skelAligned(size_t(n));
+  float* js = jp + skelAligned(size_t(J) * kParametersPerJoint);
+  float* gjp = js + (kEllipsoid ? skelAligned(size_t(J) * kJointStateStride) : 0);
+  float* acc = gjp + (kBackward ? skelAligned(size_t(J) * kParametersPerJoint) : 0);
+  {
+    uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
+    stageCharacterTables(T, cursor);
+    if constexpr (kBackward) {
+      if constexpr (kEllipsoid) { stageTable(S.childStart, size_t(J) + 1, cursor); stageTable(S.children, a.numChildren, cursor); }
+      stageTable(S.ptColStart, n + 1, cursor); stageTable(S.ptColRows, T.ptNnz, cursor); stageTable(S.ptColVals, T.ptNnz, cursor);
+    }
+    __syncthreads();
+  }
+  for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
+    const float* src = a.theta + size_t(b) * n;
+    for (int i = g.lane; i < n; i += g.size) th[i] = src[i];
+    g.sync();
+    if constexpr (!kBackward) limitPasses<kEllipsoid>(g, T, L, th, jp, js, a.residual + size_t(b) * R);
+    else limitGradPasses<kEllipsoid>(g, T, S, L, th, jp, js, acc, gjp, a.gradResidual + size_t(b) * R, a.gradTheta + size_t(b) * n);
+    g.sync(); // the next instance overwrites th / jp / js / gjp
+  }
+}
+
+cudaError_t launchParameterLimits(const ParameterLimitArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query) {
+  using K = void (*)(ParameterLimitArgs);
+#define MB2_LIMIT_KERNELS(B, E) {parameterLimitsKernel<B, 1, E>, parameterLimitsKernel<B, 2, E>, parameterLimitsKernel<B, 4, E>, parameterLimitsKernel<B, 8, E>}
+  static const K kernels[2][2][4] = {{MB2_LIMIT_KERNELS(false, false), MB2_LIMIT_KERNELS(false, true)},
+                                     {MB2_LIMIT_KERNELS(true, false), MB2_LIMIT_KERNELS(true, true)}};
+#undef MB2_LIMIT_KERNELS
+  if (query) *query = InstanceLaunchQuery{};
+  if (a.batch <= 0) return cudaSuccess;
+  if (a.L.numRows == 0) { // no live limit: nothing to write, and the gradient is zero
+    if (query) return cudaSuccess;
+    return backward ? cudaMemsetAsync(a.gradTheta, 0, size_t(a.batch) * a.T.numParams * sizeof(float), stream) : cudaSuccess;
+  }
+  const bool fk = a.L.ellipsoid != 0;
+  return launchInstanceGroups(kernels[backward][fk], a, a.numChildren, kInstanceOpParameterLimits, backward, 0, stream, query, fk);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -183,12 +183,28 @@ cudaError_t launchPositionsBackward(const PositionArgs& a, cudaStream_t stream);
 // the launch of positionsKernel over a.batch instances with a.P.numPoints points (a.P's arrays are not read); the shared-offset
 // backward launches it per slice of whole batch-sum chunks, which is the whole batch unless the offset rows exceed the scratch bound
 cudaError_t queryPositionsLaunch(const PositionArgs& a, bool backward, InstanceLaunchQuery* query);
-// parameterTransformKernel ... inverseParameterTransformBackwardKernel: the flat joint-parameter operations of ik_device.cuh
-// jointOpElement for a batch, forward or backward; arrays [B][...] dense, device memory
+// parameterLimitsKernel<kBackward>: the rows of the character's limits (LimitErrorFunction at weight 1, L2 loss) for a batch of model
+// parameters, and their backward
+struct ParameterLimitArgs {
+  CharacterTables T;
+  SkeletonTables S;           // backward only
+  LimitTables L;              // device memory
+  int32_t numChildren;        // entries of S.children
+  int32_t batch;
+  const float* theta;         // [B][n]
+  float* residual;            // forward: [B][R]
+  const float* gradResidual;  // backward: [B][R] dLoss / d residual
+  float* gradTheta;           // backward: [B][n], overwritten
+};
+// Both enqueue on `stream` and take no scratch. R == 0: the forward writes nothing and the backward zeroes gradTheta. With `query`,
+// the launch is reported there and nothing is enqueued.
+cudaError_t launchParameterLimits(const ParameterLimitArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query = nullptr);
+// parameterTransformKernel ... clampParametersBackwardKernel: the flat joint-parameter operations of ik_device.cuh jointOpElement for a
+// batch, forward or backward; arrays [B][...] dense, device memory
 struct JointOpArgs {
   CharacterTables T;
-  SkeletonTables S;          // the backward of kJointOpParameterTransform (ptCol*), of kJointOpFromWorld (children), and both directions
-                             // of kJointOpInverseParameterTransform (inv*)
+  SkeletonTables S;          // the backward of kJointOpParameterTransform (ptCol*), of kJointOpFromWorld (children), both directions
+                             // of kJointOpInverseParameterTransform (inv*) and of kJointOpClampParameters (paramClamp)
   int32_t batch;
   const float* in;           // the forward's input (backward: the forward's input, unused by the two linear ParameterTransform ops)
   const float* grad;         // backward: dLoss / d the forward's output

@@ -1,6 +1,7 @@
 #include "ik_plan.h"
 
 #include <algorithm>
+#include <array>
 #include <cfloat>
 #include <cmath>
 #include <cstring>
@@ -476,6 +477,111 @@ std::string setParameterLimits(HostCharacter& ch, int32_t count, const mb2_param
     ch.limits.push_back(l);
   }
   return "";
+}
+
+namespace {
+const char* limitTypeName(int type) {
+  static const char* names[] = {"MinMax", "MinMaxJoint", "MinMaxJointPassive", "Linear", "LinearJoint", "Ellipsoid", "HalfPlane"};
+  return type >= 0 && type <= 6 ? names[type] : "unknown";
+}
+// CSR of (key, limit, coef) triples: keys in [0, count), the triples of a key in the order given
+void limitCsr(int count, const std::vector<std::array<double, 3>>& t, std::vector<int32_t>& start, std::vector<int32_t>& limit,
+              std::vector<float>* coef) {
+  start.assign(size_t(count) + 1, 0);
+  for (const auto& e : t) ++start[size_t(e[0]) + 1];
+  for (int k = 0; k < count; ++k) start[k + 1] += start[k];
+  std::vector<int32_t> fill(start.begin(), start.end() - 1);
+  limit.assign(t.size(), 0);
+  if (coef) coef->assign(t.size(), 0.f);
+  for (const auto& e : t) { // stable: the triples of one key keep their order
+    const int32_t at = fill[size_t(e[0])]++;
+    limit[at] = int32_t(e[1]);
+    if (coef) (*coef)[at] = float(e[2]);
+  }
+}
+} // namespace
+
+HostLimitTables makeLimitTables(const HostCharacter& ch) {
+  HostLimitTables t;
+  const int J = ch.numJoints, n = ch.numParams, rows = J * kParametersPerJoint;
+  std::vector<std::array<double, 3>> byJoint, byRow, byParam;
+  t.paramClamp.assign(size_t(n) * 3, 0.f);
+  for (size_t k = 0; k < ch.limits.size(); ++k) {
+    const HostLimit& l = ch.limits[k];
+    if (l.type == kLimitMinMaxJointPassive) continue; // no rows (limit_error_function.cpp:1051-1052)
+    const std::string name = "parameter limits: limit " + std::to_string(k) + " (" + limitTypeName(l.type) + ")";
+    auto param = [&](int p) { return p >= 0 && p < n; };
+    auto joint = [&](int j) { return j >= 0 && j < J; };
+    auto jointRow = [&](int j, int d) { return joint(j) && d >= 0 && d < kParametersPerJoint; };
+    LimitDesc D{};
+    D.type = l.type;
+    D.row = t.numRows;
+    D.data = -1;
+    const int l32 = int(t.limits.size());
+    const double w = std::sqrt(10.0 * double(l.weight)); // kLimitWeight
+    D.w = float(w);
+    for (int i = 0; i < 4; ++i) D.f[i] = l.f[i];
+    switch (l.type) {
+      case kLimitMinMax:
+        if (!param(l.i[0])) { t = HostLimitTables{}; t.rejected = name + ": parameter index " + std::to_string(l.i[0]) + " is outside [0, n)"; return t; }
+        D.i0 = l.i[0];
+        byParam.push_back({double(D.i0), double(l32), w});
+        t.paramClamp[3 * D.i0] = l.f[0];
+        t.paramClamp[3 * D.i0 + 1] = l.f[1];
+        t.paramClamp[3 * D.i0 + 2] = 1.f;
+        break;
+      case kLimitMinMaxJoint:
+        if (!jointRow(l.i[0], l.i[1])) { t = HostLimitTables{}; t.rejected = name + ": joint " + std::to_string(l.i[0]) + " parameter " + std::to_string(l.i[1]) + " is out of range"; return t; }
+        D.i0 = l.i[0] * kParametersPerJoint + l.i[1];
+        byRow.push_back({double(D.i0), double(l32), w});
+        break;
+      case kLimitLinear:
+        if (!param(l.i[0]) || !param(l.i[1])) { t = HostLimitTables{}; t.rejected = name + ": a parameter index is outside [0, n)"; return t; }
+        D.i0 = l.i[0];
+        D.i1 = l.i[1];
+        byParam.push_back({double(D.i1), double(l32), w * double(l.f[0])});
+        byParam.push_back({double(D.i0), double(l32), -w});
+        break;
+      case kLimitLinearJoint:
+        if (!jointRow(l.i[0], l.i[1]) || !jointRow(l.i[2], l.i[3])) { t = HostLimitTables{}; t.rejected = name + ": a joint or joint parameter is out of range"; return t; }
+        D.i0 = l.i[0] * kParametersPerJoint + l.i[1];
+        D.i1 = l.i[2] * kParametersPerJoint + l.i[3];
+        byRow.push_back({double(D.i1), double(l32), w * double(l.f[0])});
+        byRow.push_back({double(D.i0), double(l32), -w});
+        break;
+      case kLimitHalfPlane:
+        if (!param(l.i[0]) || !param(l.i[1])) { t = HostLimitTables{}; t.rejected = name + ": a parameter index is outside [0, n)"; return t; }
+        D.i0 = l.i[0];
+        D.i1 = l.i[1];
+        byParam.push_back({double(D.i0), double(l32), w * double(l.f[0])});
+        byParam.push_back({double(D.i1), double(l32), w * double(l.f[1])});
+        break;
+      case kLimitEllipsoid:
+        if (!joint(l.i[0]) || !joint(l.i[1])) { t = HostLimitTables{}; t.rejected = name + ": a joint index is outside [0, J)"; return t; }
+        D.i0 = l.i[0];
+        D.i1 = l.i[1];
+        D.w = float(std::sqrt(10.0 * 1e-4 * double(l.weight))); // kLimitWeight kLimitPositionWeight
+        D.data = int32_t(t.ellipsoidData.size());
+        t.ellipsoidData.insert(t.ellipsoidData.end(), l.f, l.f + 27);
+        byJoint.push_back({double(D.i1), double(2 * l32), 0.0});
+        byJoint.push_back({double(D.i0), double(2 * l32 + 1), 0.0});
+        t.ellipsoid = true;
+        break;
+      default: t = HostLimitTables{}; t.rejected = name + ": unknown limit type"; return t;
+    }
+    t.numRows += l.type == kLimitEllipsoid ? 3 : 1;
+    t.limits.push_back(D);
+  }
+  limitCsr(J, byJoint, t.jointStart, t.jointEntry, nullptr);
+  limitCsr(rows, byRow, t.rowStart, t.rowLimit, &t.rowCoef);
+  limitCsr(n, byParam, t.paramStart, t.paramLimit, &t.paramCoef);
+  return t;
+}
+
+LimitTables hostLimitTables(const HostLimitTables& t) {
+  return LimitTables{int32_t(t.limits.size()), t.numRows, t.ellipsoid ? 1 : 0, t.limits.data(), t.ellipsoidData.data(), t.jointStart.data(),
+                     t.jointEntry.data(), t.rowStart.data(), t.rowLimit.data(), t.rowCoef.data(), t.paramStart.data(), t.paramLimit.data(),
+                     t.paramCoef.data()};
 }
 
 // What Position, Plane and Orientation blocks share: the generalized loss, and the parent joint and weight of each constraint.

@@ -54,6 +54,24 @@ struct HostCharacter {
   std::vector<uint8_t> computeActiveJointParams(const std::vector<uint8_t>& enabled) const;
 };
 
+// The character's limits as parameter_limits_residual and apply_model_param_limits read them (LimitTables, SkeletonTables::paramClamp).
+// Built by makeLimitTables only, whenever the limits are set.
+struct HostLimitTables {
+  // why the limits cannot be evaluated (an index out of range, naming the limit), empty when they can; the tables are then empty. The
+  // solver's own limit blocks keep their rule: they reject such limits when a LimitErrorFunction is planned.
+  std::string rejected;
+  int32_t numRows{0};
+  bool ellipsoid{false};
+  std::vector<LimitDesc> limits;
+  std::vector<float> ellipsoidData;
+  std::vector<int32_t> jointStart, jointEntry, rowStart, rowLimit, paramStart, paramLimit;
+  std::vector<float> rowCoef, paramCoef;
+  std::vector<float> paramClamp; // [n][3]
+};
+HostLimitTables makeLimitTables(const HostCharacter& ch);
+// LimitTables over the host vectors of t
+LimitTables hostLimitTables(const HostLimitTables& t);
+
 // Linear-blend skinning of a character (SkinWeights + Character::inverseBindPose, skin_weights.h:19-40, character.h), flattened into
 // the tables of SkinTables (ik_types.h). Built and validated by makeSkinning only.
 struct HostSkinning {

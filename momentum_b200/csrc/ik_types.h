@@ -144,6 +144,57 @@ struct SkeletonTables {
   const int32_t* invRowStart; // [7J+1]
   const int32_t* invParams;   // [nnz W] ascending within a row
   const float* invRowVals;    // [nnz W]
+  // apply_model_param_limits (makeLimitTables): per model parameter min, max and 1 when a MinMax limit names it (the last such limit in
+  // list order), else 0, 0, 0
+  const float* paramClamp;    // [n][3]
+};
+
+// character/parameter_limits.h:20-33 LimitType
+enum LimitType : int32_t {
+  kLimitMinMax = 0,
+  kLimitMinMaxJoint = 1,
+  kLimitMinMaxJointPassive = 2,
+  kLimitLinear = 3,
+  kLimitLinearJoint = 4,
+  kLimitEllipsoid = 5,
+  kLimitHalfPlane = 6,
+};
+
+// One live limit of parameter_limits_residual (makeLimitTables): its rows are the LimitErrorFunction rows at weight 1 and L2 loss.
+//   MinMax       i0 parameter,            f0 f1 min max
+//   MinMaxJoint  i0 joint-parameter row,  f0 f1 min max
+//   Linear       i0 reference, i1 target parameter,   f0 scale, f1 offset, f2 f3 range
+//   LinearJoint  i0 reference, i1 target row,         f0 .. f3 as Linear
+//   HalfPlane    i0 i1 parameters, f0 f1 normal, f2 offset
+//   Ellipsoid    i0 ellipsoidParent, i1 parent joint; its 27 floats (ellipsoid, ellipsoidInv, offset) at `data` in the ellipsoid array
+struct LimitDesc {
+  int32_t type;   // LimitType, never kLimitMinMaxJointPassive
+  int32_t row;    // its first residual row
+  int32_t i0, i1;
+  float f[4];
+  float w;        // the row scale sqrt(kLimitWeight weight), Ellipsoid sqrt(kLimitWeight kLimitPositionWeight weight), rounded once from double
+  int32_t data;   // Ellipsoid: float offset into LimitTables::ellipsoidData; -1 otherwise
+};
+
+// The character's limits as parameter_limits_residual reads them (makeLimitTables), shared by the batch. The backward's gradient terms
+// are grouped three ways, each a CSR in limit-list order within a group, so that every output is one lane's fixed-order sum:
+//   by joint                Ellipsoid seeds: entry 2 l + role, role 0 the parent joint (the constrained point), 1 the ellipsoid parent
+//   by joint-parameter row  MinMaxJoint and LinearJoint terms (target before reference), added before P^T
+//   by model parameter      MinMax, Linear and HalfPlane terms (target / param1 first), added after P^T
+struct LimitTables {
+  int32_t numLimits;     // live limits (every type but MinMaxJointPassive)
+  int32_t numRows;       // R
+  int32_t ellipsoid;     // an Ellipsoid is among them: the operation runs the FK passes
+  const LimitDesc* limits;       // [numLimits] in list order
+  const float* ellipsoidData;    // [Ellipsoids][27]
+  const int32_t* jointStart;     // [J+1]
+  const int32_t* jointEntry;
+  const int32_t* rowStart;       // [7J+1]
+  const int32_t* rowLimit;
+  const float* rowCoef;
+  const int32_t* paramStart;     // [n+1]
+  const int32_t* paramLimit;
+  const float* paramCoef;
 };
 
 // Points fixed in joints' frames (model / joint_parameters_to_positions), shared by the batch (makePointTables): each point's joint, and
@@ -161,12 +212,14 @@ struct PointTables {
 //   kJointOpFromLocal           jp [J][7] of local states [J][8]                /  g_local [J][8] of g_jp [J][7]
 //   kJointOpFromWorld           jp [J][7] of world states [J][8]                /  g_world [J][8] of g_jp [J][7]
 //   kJointOpInverseParameterTransform  theta [n] = W (jp - o), W = P^+          /  g_jp [7 J] = W^T g_theta
+//   kJointOpClampParameters     theta [n] clamped by the MinMax limits          /  g_theta where min <= theta <= max, else 0
 enum JointOp : int32_t {
   kJointOpParameterTransform = 0,
   kJointOpLocalState = 1,
   kJointOpFromLocal = 2,
   kJointOpFromWorld = 3,
   kJointOpInverseParameterTransform = 4,
+  kJointOpClampParameters = 5,
 };
 
 // Linear-blend skinning tables (HostSkinning, makeSkinning), shared by the whole batch. The active influences of every vertex (the slots

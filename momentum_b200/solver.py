@@ -144,6 +144,11 @@ CABI_SIGNATURES = {
     "mb2_solver_get_fused_profile": (_int, [_vp, _ip, _ip, _dp, _up]),
     "mb2_solver_function_get_sweep_launch": (_int, [_vp, _int32, _lp]),
     "mb2_character_get_instance_launch": (_int, [_vp, _int32, _int32, _int32, _int32, _lp]),
+    "mb2_character_num_limit_residuals": (_int, [_vp, _ip]),
+    "mb2_character_parameter_limits_residual_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_parameter_limits_residual_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
+    "mb2_character_apply_model_parameter_limits_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_apply_model_parameter_limits_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
     "mb2_solver_function_get_input_gradient_launch": (_int, [_vp, _lp]),
     "mb2_solver_get_solve_path": (_int, [_vp, _lp]),
     "mb2_mixed_batch_last_error": (C.c_char_p, []),
@@ -181,7 +186,8 @@ JOINT_OPS = {
     "model_parameters_to_skeleton_state": ("mb2_character_skeleton_state_device", "mb2_character_skeleton_state_backward_device"),
     **{name: (f"mb2_character_{name}_device", f"mb2_character_{name}_backward_device")
        for name in ("apply_parameter_transform", "apply_inverse_parameter_transform", "joint_parameters_to_skeleton_state",
-                    "joint_parameters_to_local_skeleton_state", "local_skeleton_state_to_joint_parameters", "skeleton_state_to_joint_parameters")},
+                    "joint_parameters_to_local_skeleton_state", "local_skeleton_state_to_joint_parameters", "skeleton_state_to_joint_parameters",
+                    "apply_model_parameter_limits")},
 }
 # the operations whose backward does not read their input (P^T and W^T), so their backward takes no input pointer
 LINEAR_JOINT_OPS = frozenset({"apply_parameter_transform", "apply_inverse_parameter_transform"})
@@ -283,9 +289,11 @@ class _Base:
             raise MomentumB200Error(self._L.mb2_last_error().decode())
 
 
-# the operations mb2_character_get_instance_launch reports on, by its op code
+# the skeleton-state and positions operations mb2_character_get_instance_launch reports on, by its op code
 INSTANCE_OPS = {"model_parameters_to_skeleton_state": 0, "joint_parameters_to_skeleton_state": 1, "model_parameters_to_positions": 2,
                 "joint_parameters_to_positions": 3}
+# its op code of parameter_limits_residual, whose launch depends on the character's limits rather than on a rig alone
+PARAMETER_LIMITS_INSTANCE_OP = 5
 
 
 def _instance_launch(out) -> dict:
@@ -465,12 +473,31 @@ class DeviceCharacter(_Base):
         self._check(fn(self._h, int(batch), *ptrs, stream))
 
     def get_instance_launch(self, op: str, backward: bool, batch: int, num_points: int = 0) -> dict:
-        """What the per-instance kernel of ``op`` (a key of ``INSTANCE_OPS``) would launch for ``batch`` instances (and ``num_points``
-        points): warps per instance, instances per CTA, threads per CTA, CTAs, dynamic shared memory bytes and whether the point tables
-        are staged. All zero when nothing runs; raises when one instance does not fit in shared memory."""
+        """What the per-instance kernel of ``op`` (a key of ``INSTANCE_OPS``, or "parameter_limits_residual") would launch for ``batch``
+        instances (and ``num_points`` points): warps per instance, instances per CTA, threads per CTA, CTAs, dynamic shared memory bytes
+        and whether the point tables are staged. All zero when nothing runs; raises when one instance does not fit in shared memory."""
+        code = PARAMETER_LIMITS_INSTANCE_OP if op == "parameter_limits_residual" else INSTANCE_OPS[op]
         out = (C.c_int64 * 6)()
-        self._check(self._L.mb2_character_get_instance_launch(self._h, INSTANCE_OPS[op], int(bool(backward)), int(batch), int(num_points), out))
+        self._check(self._L.mb2_character_get_instance_launch(self._h, code, int(bool(backward)), int(batch), int(num_points), out))
         return _instance_launch(out)
+
+    def num_limit_residuals(self) -> int:
+        """R, the rows of parameter_limits_residual for the limits this handle was made with (one per limit, none for
+        MinMaxJointPassive, three for an Ellipsoid). Raises with the reason when a limit's index is out of range."""
+        out = C.c_int32(0)
+        self._check(self._L.mb2_character_num_limit_residuals(self._h, C.byref(out)))
+        return int(out.value)
+
+    def parameter_limits_residual_device(self, batch: int, theta_device_ptr: int, residual_device_ptr: int, stream: int = 0):
+        """The LimitErrorFunction rows [B][R] (weight 1, L2 loss) of model parameters [B][n]; float32 device memory on this character's
+        device, enqueued on ``stream``."""
+        self._check(self._L.mb2_character_parameter_limits_residual_device(self._h, int(batch), theta_device_ptr, residual_device_ptr, stream))
+
+    def parameter_limits_residual_backward_device(self, batch: int, theta_device_ptr: int, grad_residual_device_ptr: int,
+                                                  grad_theta_device_ptr: int, stream: int = 0):
+        """dLoss/d model parameters [B][n] from dLoss/d residual [B][R], overwritten."""
+        self._check(self._L.mb2_character_parameter_limits_residual_backward_device(self._h, int(batch), theta_device_ptr, grad_residual_device_ptr,
+                                                                                  grad_theta_device_ptr, stream))
 
     def positions_device(self, joint: bool, batch: int, params_device_ptr: int, parents: np.ndarray, offsets_device_ptr: int, offsets_batched: bool,
                          positions_device_ptr: int, stream: int = 0):

@@ -335,6 +335,85 @@ model_parameters_to_positions.__doc__ += _POSITIONS_NOTE
 joint_parameters_to_positions.__doc__ += _POSITIONS_NOTE
 
 
+class _ParameterLimits(torch.autograd.Function):
+    """parameter_limits_residual on [B, n] float32 rows, forward and backward on the device."""
+
+    @staticmethod
+    def forward(ctx, dc, R, theta):
+        rows = _float32(theta, -1, theta.shape[-1])
+        B = rows.shape[0]
+        out = torch.empty(B, R, device=theta.device, dtype=torch.float32)
+        if B * R > 0:
+            dc.parameter_limits_residual_device(B, rows.data_ptr(), out.data_ptr(), _stream(theta.device))
+        ctx.dc, ctx.R, ctx.shape, ctx.dtype = dc, R, theta.shape, theta.dtype
+        ctx.save_for_backward(rows)
+        return _restore(out, (*theta.shape[:-1], R), theta.dtype)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_residual):
+        (rows,) = ctx.saved_tensors
+        B = rows.shape[0]
+        gt = torch.zeros_like(rows)
+        if B * ctx.R > 0:  # else the gradient is zero
+            g = _float32(grad_residual, B, ctx.R)
+            ctx.dc.parameter_limits_residual_backward_device(B, rows.data_ptr(), g.data_ptr(), gt.data_ptr(), _stream(rows.device))
+        return None, None, _restore(gt, ctx.shape, ctx.dtype)
+
+
+_LIMITS_NOTE = """
+    The limits are those of the device handle: for a ``Character``, ``character.limits`` as they were when the torch layer first made
+    its handle for it on that device (``solve_ik`` reads them at the same moment). A changed limit list needs a new ``Character`` or
+    ``DeviceCharacter``. A limit whose index is out of range raises ``MomentumB200Error`` naming it; ``solve_ik`` only rejects it when its
+    objective has a limit block."""
+
+
+def parameter_limits_residual(character, model_parameters: torch.Tensor) -> torch.Tensor:
+    """The residual of momentum's ``LimitErrorFunction`` over the character's ParameterLimits, at weight 1 with the L2 loss, for
+    ``model_parameters`` ([n] or [B, n], on a CUDA device): [R] or [B, R] in the input dtype, computed in float32, so that
+    ``residual.square().sum(-1)`` is ``LimitErrorFunction::getError``. The rows are those its ``getJacobian`` returns: one per limit in
+    ``character.limits`` order, none for MinMaxJointPassive, three for an Ellipsoid; sqrt(10 w) times the limit's residual
+    (Ellipsoid: sqrt(10 * 1e-4 w)); 0 for an inactive limit. MinMax gives theta - min below the minimum and theta - max above the
+    maximum; Linear and LinearJoint apply only where the target is in [rangeMin, rangeMax), (0, 0) meaning everywhere; HalfPlane only
+    where its value is negative. Joint-space limits read P theta + o, Ellipsoids the skeleton state of theta. A character without live
+    limits gives [B, 0].
+
+    Against pymomentum's torch module ``pymomentum.torch.parameter_limits.ParameterLimits``: the module groups its rows by limit type,
+    its MinMax rows below the minimum have the opposite sign (min - theta), and it lacks the (0, 0) rule of Linear and LinearJoint
+    ranges. Where that rule does not apply, the sum of squares is the same.
+
+    Differentiable once with respect to ``model_parameters``. The gradient is the exact derivative of these rows: for an Ellipsoid it
+    includes the projection onto the ellipsoid and the motion of the ellipsoid's parent joint, where momentum's
+    ``computeEllipsoidJacobian`` walks only the joints from the parent up to the ellipsoid parent and holds the projected point fixed.
+    It costs O(J + limits) per instance."""
+    name = "parameter_limits_residual"
+    ch, _ = _resolve(character)
+    n = ch.num_params
+    if not torch.is_tensor(model_parameters):
+        raise ValueError(f"{name}: model_parameters must be a tensor")
+    if model_parameters.dim() not in (1, 2) or model_parameters.shape[-1] != n:
+        raise ValueError(f"{name}: model_parameters must be [{n}] or [B, {n}], got {tuple(model_parameters.shape)}")
+    if not model_parameters.is_cuda:
+        raise ValueError(f"{name} runs on CUDA tensors (there is no CPU fallback)")
+    dc = _device_character(character, model_parameters.device)
+    return _ParameterLimits.apply(dc, dc.num_limit_residuals(), model_parameters)
+
+
+def apply_model_param_limits(character, model_parameters: torch.Tensor) -> torch.Tensor:
+    """pymomentum ``apply_model_param_limits``: ``model_parameters`` ([n] or [B, n], on a CUDA device) with every parameter that a MinMax
+    limit names clamped to [min, max] as ``torch.clamp`` does it (NaN stays NaN), every other parameter passed through, in the input
+    dtype, computed in float32. Other limit types are ignored. When several MinMax limits name one parameter, the last in list order
+    decides both the value and the gradient, as a sequential ``index_copy`` would. Differentiable once: the gradient is ``torch.clamp``'s,
+    the upstream gradient where min <= theta <= max and 0 elsewhere."""
+    ch, _ = _resolve(character)
+    return _joint_op("apply_model_parameter_limits", character, model_parameters, f"model_parameters (n = {ch.num_params})", (ch.num_params,),
+                     (ch.num_params,))
+
+
+parameter_limits_residual.__doc__ += _LIMITS_NOTE
+apply_model_param_limits.__doc__ += _LIMITS_NOTE
+
+
 class _SkinPoints(torch.autograd.Function):
     @staticmethod
     def forward(ctx, dc, skel_state, rest_points):
