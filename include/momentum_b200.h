@@ -76,6 +76,18 @@ typedef struct mb2_parameter_limit {
   float f[27];
 } mb2_parameter_limit;
 
+/* character/collision_geometry.h TaperedCapsuleT: the local transformation (translation, rotation xyzw, scale) in the parent joint's
+ * frame (parent -1: world-fixed), the radii at the two ends and the length along the local x axis. The rotation is normalised when the
+ * geometry is set; the reference composes a non-unit rotation as it is, so the two differ for one. */
+typedef struct mb2_tapered_capsule {
+  int32_t parent;
+  float translation[3];
+  float rotation[4];
+  float scale;
+  float radius[2];
+  float length;
+} mb2_tapered_capsule;
+
 /* state_error_function.h:17-32 RotationErrorType */
 typedef enum mb2_rotation_error_type {
   MB2_ROTATION_MATRIX_DIFFERENCE = 0,
@@ -307,6 +319,27 @@ int mb2_character_apply_model_parameter_limits_device(const mb2_character* c, in
                                                       float* clamped_model_parameters_device, void* cuda_stream);
 int mb2_character_apply_model_parameter_limits_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
                                                                const float* grad_clamped_device, float* grad_model_parameters_device, void* cuda_stream);
+/* Self-collision of the character's tapered capsules (CollisionErrorFunction, collision_error_function.cpp) as a character operation.
+ * mb2_character_set_collision_geometry replaces the geometry (count == 0: an empty one) and plans the valid pairs then: for i < j in
+ * ascending order, both world-fixed: dropped; exactly one: kept; same or parent-child joints: dropped; otherwise kept unless the two
+ * capsules overlap at the rest pose (model parameters zero through the ParameterTransform, offsets included; updateCollisionPairs with
+ * filterRestPoseOverlaps), evaluated in double where the reference's float build evaluates it in float. A parent outside [-1, J), a
+ * negative radius or length, a non-finite value, a zero rotation or a direction (scale times length) that overflows float is
+ * MB2_ERR_INVALID_ARGUMENT naming the capsule, and leaves the earlier geometry in place. mb2_character_clone copies the geometry. Until a geometry is set the collision entries return MB2_ERR_INVALID_ARGUMENT.
+ * mb2_character_get_collision_pairs writes the planned pairs, int32 [P][2]. */
+int mb2_character_set_collision_geometry(mb2_character* c, int32_t count, const mb2_tapered_capsule* capsules);
+int mb2_character_num_collision_pairs(const mb2_character* c, int32_t* out);
+int mb2_character_get_collision_pairs(const mb2_character* c, int32_t* pairs);
+/* The rows [B][P] of the valid pairs for skeleton states [B][J][8] (t, q xyzw, s; q normalised): sqrt(kCollisionWeight) times the
+ * overlap where the reference's overlaps() reports a contact, else 0, so that the sum of squares is CollisionErrorFunction::getError at
+ * weight 1. The narrow phase is closestPointsOnSegments branch for branch in float. Its backward writes dLoss / d state [B][J][8] from
+ * dLoss / d rows [B][P]: the exact derivative of the rows, the motion of the closest-point parameters included (getJacobian holds them
+ * fixed). Fixed summation order, no atomics, no scratch. P == 0 is valid (the row arrays may then be NULL; the gradient is zero). The
+ * argument rules of mb2_character_skeleton_state_device. */
+int mb2_character_collision_residual_device(const mb2_character* c, int32_t batch, const float* skel_state_device, float* residual_device,
+                                            void* cuda_stream);
+int mb2_character_collision_residual_backward_device(const mb2_character* c, int32_t batch, const float* skel_state_device,
+                                                     const float* grad_residual_device, float* grad_skel_state_device, void* cuda_stream);
 /* pymomentum joint_parameters_to_skeleton_state (tensor_skeleton_state.cpp:203-343, :488-491): the forward kinematics of
  * mb2_character_skeleton_state_device from joint parameters [B][7 J] -> [B][J][8] */
 int mb2_character_joint_parameters_to_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
@@ -569,9 +602,9 @@ int mb2_solver_function_get_sweep_launch(mb2_solver_function* f, int32_t jacobia
 /* What the character operations' per-instance kernels would launch for `batch` instances, planned by the code that launches them and
  * with nothing enqueued. op: 0 model_parameters_to_skeleton_state, 1 joint_parameters_to_skeleton_state, 2 model_parameters_to_positions,
  * 3 joint_parameters_to_positions (num_points points), 5 parameter_limits_residual (num_points is ignored; the kernel runs the FK when the
- * character has an Ellipsoid limit); backward != 0: their backward. out: [0] warps per instance W (1, 2, 4 or 8),
+ * character has an Ellipsoid limit), 6 collision_residual (num_points is ignored); backward != 0: their backward. out: [0] warps per instance W (1, 2, 4 or 8),
  * [1] instances per CTA, [2] threads per CTA, [3] CTAs, [4] dynamic shared memory per CTA in bytes, [5] 1 when the point tables are
- * staged in shared memory. All zero when nothing runs (batch 0, positions with no point, limits with no residual row). An instance that does not fit in shared
+ * staged in shared memory. All zero when nothing runs (batch 0, positions with no point, limits with no residual row, collision with no pair). An instance that does not fit in shared
  * memory next to the tables is refused with MB2_ERR_CUDA, as the operation refuses it. The shared-offset positions backward launches
  * per slice of the batch when its per-instance offset rows exceed 256 MiB of scratch: this reports one launch of `batch` instances.
  * No reference counterpart. */

@@ -68,6 +68,33 @@ MAX_SKIN_JOINTS = 8  # kMaxSkinJoints, skin_weights.h:19
 
 
 @dataclass
+class TaperedCapsule:
+    """One ``TaperedCapsuleT`` (character/collision_geometry.h): the local ``transformation`` (translation, rotation xyzw, scale) in the
+    ``parent`` joint's frame, -1 for a world-fixed capsule; the radii at its two ends and its length along the local x axis. The rotation is
+    normalised when the geometry is uploaded (momentum composes a non-unit rotation as it is, so the two differ for one)."""
+
+    parent: int = -1
+    translation: Sequence[float] = (0.0, 0.0, 0.0)
+    rotation: Sequence[float] = (0.0, 0.0, 0.0, 1.0)
+    scale: float = 1.0
+    radius: Sequence[float] = (0.0, 0.0)
+    length: float = 0.0
+
+
+# mb2_tapered_capsule, 48 bytes
+CAPSULE_DTYPE = np.dtype([("parent", "<i4"), ("translation", "<f4", 3), ("rotation", "<f4", 4), ("scale", "<f4"), ("radius", "<f4", 2),
+                          ("length", "<f4")])
+
+
+def capsule_array(capsules: Sequence[TaperedCapsule]) -> np.ndarray:
+    """The capsules as a contiguous mb2_tapered_capsule array."""
+    a = np.zeros(len(capsules), CAPSULE_DTYPE)
+    for k, c in enumerate(capsules):
+        a[k] = (int(c.parent), tuple(c.translation), tuple(c.rotation), float(c.scale), tuple(c.radius), float(c.length))
+    return a
+
+
+@dataclass
 class Skinning:
     """Linear-blend skinning of a character: ``SkinWeights`` (skin_weights.h:19-40) and ``Character::inverseBindPose``. A vertex's
     influences end at its first zero weight (linear_skinning.cpp:76-80); the slots after it are ignored."""
@@ -114,6 +141,7 @@ class Character:
     name: str = "character"
     skinning: Optional[Skinning] = None
     blend_shape: Optional["BlendShape"] = None
+    collision: Optional[List[TaperedCapsule]] = None
 
     @property
     def num_joints(self) -> int:
@@ -810,3 +838,207 @@ def world_rotations(ch: Character, theta, parents, offsets_q):
     _, q, _ = forward_kinematics(ch, theta)
     parents = np.asarray(parents)
     return _qmul(q[:, parents], np.broadcast_to(np.asarray(offsets_q, np.float64)[None], (q.shape[0], len(parents), 4)))
+
+
+# ---- Self-collision of tapered capsules (CollisionErrorFunction) in float64 ----------------------------------------------------------
+COLLISION_WEIGHT = 5e-3  # kCollisionWeight, collision_error_function.h:139
+SEG_CONST, SEG_INTERIOR, SEG_EDGE0, SEG_EDGE1 = range(4)  # which closed form a closest-point parameter came from (ik_device.cuh SegmentForm)
+
+
+def _capsule_locals(capsules: Sequence[TaperedCapsule]):
+    """[C] parents and [C, 8] local geometry in float64: origin, direction R(q^) e_x scale length (rotation normalised), r0, r1."""
+    par = np.array([int(c.parent) for c in capsules], np.int64)
+    L = np.zeros((len(capsules), 8))
+    for k, c in enumerate(capsules):
+        q = np.asarray(c.rotation, np.float64)
+        q = q / np.linalg.norm(q)
+        L[k, :3] = c.translation
+        L[k, 3:6] = _qrot(q, np.array([float(c.scale) * float(c.length), 0.0, 0.0]))
+        L[k, 6:] = c.radius
+    return par, L
+
+
+def capsule_world(capsules: Sequence[TaperedCapsule], skel_state) -> np.ndarray:
+    """CollisionGeometryStateT::updatePrimitive in float64 for skeleton states [B, J, 8] (t, q xyzw, s; q normalised): [B, C, 8] world
+    origin, direction, r0, r1. A world-fixed capsule keeps its local geometry."""
+    st = np.asarray(skel_state, np.float64)
+    par, L = _capsule_locals(capsules)
+    B = st.shape[0]
+    W = np.broadcast_to(L, (B,) + L.shape).copy()
+    att = par >= 0
+    if att.any():
+        ps = st[:, par[att]]
+        q = ps[..., 3:7] / np.linalg.norm(ps[..., 3:7], axis=-1, keepdims=True)
+        s = ps[..., 7:8]
+        W[:, att, :3] = ps[..., :3] + _qrot(q, s * L[att, :3])
+        W[:, att, 3:6] = _qrot(q, s * L[att, 3:6])
+        W[:, att, 6:] = L[att, 6:] * s
+    return W
+
+
+def capsule_contact(A, B, dist_eps: float = 1e-8, margins=None):
+    """overlaps() over closestPointsOnSegments (collision_geometry_state.h:120-157, math/utility.cpp:443-552) branch for branch, in the
+    precision of A and B [8]: (hit, s, t, dist, overlap, sForm, tForm). dist_eps is Eps (1e-8 in float, 1e-17 in double). ``margins``, a
+    list, receives (what, relative margin) for every decision taken: "far" for the early-outs, "overlap" and "dist" for the contact
+    test, "branch" for the rest, so that a caller can tell a sample within rounding of a branch boundary."""
+    A = np.asarray(A)
+    B = np.asarray(B)
+    T = A.dtype.type
+    m = margins if margins is not None else []
+
+    def lt(x, y, what="branch"):
+        m.append((what, abs(float(x) - float(y)) / (abs(float(x)) + abs(float(y)) + 1e-30)))
+        return x < y
+
+    miss = (False, T(0), T(0), T(0), T(0), SEG_CONST, SEG_CONST)
+    maxA = A[7] if A[6] < A[7] else A[6]
+    maxB = B[7] if B[6] < B[7] else B[6]
+    maxDist = T(maxA + maxB)
+    maxSq = T(maxDist * maxDist)
+    d1, d2 = A[3:6], B[3:6]
+    w = A[:3] - B[:3]
+    dot = lambda x, y: T(x[0] * y[0] + x[1] * y[1] + x[2] * y[2])
+    a, b, c, d, e = dot(d1, d1), dot(d1, d2), dot(d2, d2), dot(d1, w), dot(d2, w)
+    D = T(a * c - b * b)
+    sD, tD = D, D
+    if lt(D, T(1e-7)):
+        sN, sD, tN, tD = T(0), T(1), e, c
+        sF, tF = SEG_CONST, SEG_EDGE0
+        if lt(maxSq, dot(w, w), "far"):
+            return miss
+    else:
+        sN, tN = T(b * e - c * d), T(a * e - b * d)
+        sF = tF = SEG_INTERIOR
+        q = w + d1 * sN / D - d2 * tN / D
+        if lt(maxSq, dot(q, q), "far"):
+            return miss
+        if lt(sN, T(0)):
+            sN, tN, tD, sF, tF = T(0), e, c, SEG_CONST, SEG_EDGE0
+        elif lt(sD, sN):
+            sN, tN, tD, sF, tF = sD, T(e + b), c, SEG_CONST, SEG_EDGE1
+    if lt(tN, T(0)):
+        tN, tF = T(0), SEG_CONST
+        if lt(-d, T(0)):
+            sN, sF = T(0), SEG_CONST
+        elif lt(a, -d):
+            sN, sF = sD, SEG_CONST
+        else:
+            sN, sD, sF = -d, a, SEG_EDGE0
+    elif lt(tD, tN):
+        tN, tF = tD, SEG_CONST
+        if lt(T(-d + b), T(0)):
+            sN, sF = T(0), SEG_CONST
+        elif lt(a, T(-d + b)):
+            sN, sF = sD, SEG_CONST
+        else:
+            sN, sD, sF = T(-d + b), a, SEG_EDGE1
+    s_snap = lt(abs(sN), T(1e-7)) or lt(abs(sD), T(1e-7))
+    t_snap = lt(abs(tN), T(1e-7)) or lt(abs(tD), T(1e-7))
+    s = T(0) if s_snap else T(sN / sD)
+    t = T(0) if t_snap else T(tN / tD)
+    dP = w + d1 * s - d2 * t
+    distSq = dot(dP, dP)
+    if lt(maxSq, distSq, "far"):
+        return miss
+    dist = T(np.sqrt(distSq))
+    overlap = T(A[6] + s * (A[7] - A[6]) + B[6] + t * (B[7] - B[6]) - dist)
+    m.append(("overlap", abs(float(overlap)) / (float(A[6] + B[6]) + abs(float(A[7] - A[6])) + abs(float(B[7] - B[6])) + 1e-30)))
+    m.append(("dist", float(dist) / (float(maxDist) + 1e-30)))
+    hit = overlap > 0 and not dist < T(dist_eps)
+    return (bool(hit), s, t, dist, overlap, SEG_CONST if s_snap else sF, SEG_CONST if t_snap else tF)
+
+
+def collision_pairs(ch: Character, capsules: Sequence[TaperedCapsule]) -> np.ndarray:
+    """updateCollisionPairs with isValidCollisionPair and filterRestPoseOverlaps (collision_geometry_state.h:526-557), the rest pose
+    (model parameters zero) in float64: int64 [P, 2], i < j ascending."""
+    t, q, s = forward_kinematics(ch, np.zeros((1, ch.num_params)))
+    rest = capsule_world(capsules, np.concatenate([t, q, s[..., None]], -1))[0]
+    parents = np.asarray(ch.parents)
+    out = []
+    for i in range(len(capsules)):
+        for j in range(i + 1, len(capsules)):
+            p0, p1 = int(capsules[i].parent), int(capsules[j].parent)
+            if p0 < 0 or p1 < 0:
+                ok = p0 != p1
+            elif p0 == p1 or parents[p0] == p1 or parents[p1] == p0:
+                ok = False
+            else:
+                ok = not capsule_contact(rest[i], rest[j], 1e-17)[0]
+            if ok:
+                out.append((i, j))
+    return np.array(out, np.int64).reshape(-1, 2)
+
+
+def collision_rows(capsules: Sequence[TaperedCapsule], pairs, skel_state) -> np.ndarray:
+    """The rows of collision_residual in float64 for skeleton states [B, J, 8]: [B, P], sqrt(kCollisionWeight) overlap at a contact of
+    capsule_contact (with float's thresholds), else 0."""
+    geo = capsule_world(capsules, skel_state)
+    pairs = np.asarray(pairs).reshape(-1, 2)
+    out = np.zeros((geo.shape[0], len(pairs)))
+    wgt = np.sqrt(COLLISION_WEIGHT)
+    for b in range(geo.shape[0]):
+        for k, (i, j) in enumerate(pairs):
+            c = capsule_contact(geo[b, i], geo[b, j])
+            out[b, k] = wgt * c[4] if c[0] else 0.0
+    return out
+
+
+def synthetic_collision(ch: Character, seed: int = 0) -> List[TaperedCapsule]:
+    """A seeded tapered-capsule set for any rig: on every joint with a child (the spine and the limbs), one capsule along the bone to its
+    first child, with radii of 0.2 to 0.45 bone lengths, tapered (r1 = 0.55 to 0.9 r0) on two capsules in three and untapered on the
+    third; then two world-fixed capsules across the rest pose's bounding box. Radii this large put many pairs in contact under random
+    poses. At the rest pose every pair that isValidCollisionPair tests is clearly overlapping (and so filtered out of the valid pairs) or clearly apart: the radii of a
+    capsule whose rest-pose overlap with another lies within 1e-3 of their radii are shrunk by 3 % until none does.
+
+    The rig's own ``collision`` is not changed: assign the result to use it."""
+    rng = np.random.default_rng(seed)
+    J = ch.num_joints
+    parents = np.asarray(ch.parents)
+    t, q, s = forward_kinematics(ch, np.zeros((1, ch.num_params)))
+    rest = np.concatenate([t, q, s[..., None]], -1)
+    jp0 = np.asarray(ch.pt_offsets, np.float64).reshape(J, 7)
+    caps = []
+    for j in range(J):
+        kids = np.nonzero(parents == j)[0]
+        if kids.size == 0:
+            continue
+        bone = np.asarray(ch.offsets[kids[0]], np.float64) + jp0[kids[0], :3]  # the child's origin in j's frame
+        length = float(np.linalg.norm(bone))
+        if length < 1e-6:
+            continue
+        x = bone / length
+        axis = np.cross([1.0, 0.0, 0.0], x)
+        sin, cos = np.linalg.norm(axis), x[0]
+        if sin < 1e-9:
+            rot = (0.0, 0.0, 0.0, 1.0) if cos > 0 else (0.0, 0.0, 1.0, 0.0)
+        else:
+            half = 0.5 * np.arctan2(sin, cos)
+            rot = tuple(np.append(axis / sin * np.sin(half), np.cos(half)))
+        r0 = float(rng.uniform(0.2, 0.45)) * length
+        r1 = r0 if len(caps) % 3 == 2 else r0 * float(rng.uniform(0.55, 0.9))
+        caps.append(TaperedCapsule(j, (0.0, 0.0, 0.0), rot, 1.0, (r0, r1), length))
+    lo, hi = t[0].min(0), t[0].max(0)
+    size = float(np.linalg.norm(hi - lo))
+    for k in range(2):
+        o = lo + rng.uniform(0.2, 0.8, 3) * (hi - lo) + rng.normal(size=3) * 0.05 * size  # off any line the rig lies on
+        r = float(rng.uniform(0.04, 0.08)) * size
+        rot = np.append(rng.normal(size=3) * 0.5, 1.0)
+        caps.append(TaperedCapsule(-1, tuple(o), tuple(rot / np.linalg.norm(rot)), 1.0, (r, r * 0.7), 0.3 * size))
+    for _ in range(200):  # clear every rest-pose pair of its boundary
+        geo = capsule_world(caps, rest)[0]
+        bad = set()
+        for i in range(len(caps)):
+            for j in range(i + 1, len(caps)):
+                p0, p1 = caps[i].parent, caps[j].parent
+                if (p0 < 0 and p1 < 0) or (p0 >= 0 and p1 >= 0 and (p0 == p1 or parents[p0] == p1 or parents[p1] == p0)):
+                    continue  # never evaluated: not a valid pair whatever the pose
+                margins = []
+                capsule_contact(geo[i], geo[j], 1e-17, margins)
+                if min(v for what, v in margins if what != "branch") < 1e-3:
+                    bad.add(j)
+        if not bad:
+            return caps
+        for j in bad:
+            c = caps[j]
+            caps[j] = dataclasses.replace(c, radius=(c.radius[0] * 0.97, c.radius[1] * 0.97))
+    raise RuntimeError("synthetic_collision: could not clear the rest-pose pairs of their boundaries")

@@ -123,6 +123,12 @@ struct LimitBuffers {
   DeviceBuffer<int32_t> jointStart, jointEntry, rowStart, rowLimit, paramStart, paramLimit;
 };
 
+// the device copy of a HostCollision (CollisionTables)
+struct CollisionBuffers {
+  DeviceBuffer<CapsuleDesc> capsules;
+  DeviceBuffer<int32_t> pairs, capsuleStart, capsulePair, jointStart, jointCapsule;
+};
+
 struct mb2_character {
   int device{0};
   HostCharacter host;
@@ -136,6 +142,9 @@ struct mb2_character {
   // the limits as parameter_limits_residual and apply_model_param_limits read them, built and uploaded whenever the limits are set
   HostLimitTables limits;
   std::unique_ptr<LimitBuffers> limitsDev; // replaced whole by installLimitTables
+  // the tapered capsules and their valid pairs (mb2_character_set_collision_geometry); collisionDev is null until a geometry is set
+  HostCollision collision;
+  std::unique_ptr<CollisionBuffers> collisionDev;
   // linear-blend skinning (mb2_character_set_skinning): numVertices == 0 when there is none
   HostSkinning skin;
   std::unique_ptr<SkinBuffers> skinDev; // replaced whole by mb2_character_set_skinning, never rewritten in place
@@ -156,6 +165,7 @@ struct mb2_character {
   MeshFaceTables meshFaceTables() const;
   MeshTreeTables meshTreeTables() const;
   LimitTables limitTables() const;
+  CollisionTables collisionTables() const;
 };
 
 struct DeviceSchedule {
@@ -272,6 +282,12 @@ LimitTables mb2_character::limitTables() const {
                      d.jointEntry.p, d.rowStart.p, d.rowLimit.p, d.rowCoef.p, d.paramStart.p, d.paramLimit.p, d.paramCoef.p};
 }
 
+CollisionTables mb2_character::collisionTables() const {
+  const CollisionBuffers& d = *collisionDev;
+  return CollisionTables{int32_t(collision.capsules.size()), collision.numPairs(), d.capsules.p, d.pairs.p, d.capsuleStart.p, d.capsulePair.p,
+                         d.jointStart.p, d.jointCapsule.p};
+}
+
 SkinTables mb2_character::skinTables() const {
   const SkinBuffers& d = *skinDev;
   return SkinTables{skin.numVertices, skin.numSegments(), d.rest.p, d.vertStart.p, d.vertJoint.p, d.vertWeight.p,
@@ -317,6 +333,19 @@ int installMeshTree(mb2_character* c, HostMeshTree&& t) {
     MB2_CUDA(d.levelStart.upload(t.levelStart, nullptr));
     return MB2_OK;
   }, present);
+}
+
+// installs the collision geometry h
+int installCollision(mb2_character* c, HostCollision&& h) {
+  return installTables(c->device, c->collisionDev, c->collision, std::move(h), [](CollisionBuffers& d, const HostCollision& h) -> int {
+    MB2_CUDA(d.capsules.upload(h.capsules, nullptr));
+    MB2_CUDA(d.pairs.upload(h.pairs, nullptr));
+    MB2_CUDA(d.capsuleStart.upload(h.capsuleStart, nullptr));
+    MB2_CUDA(d.capsulePair.upload(h.capsulePair, nullptr));
+    MB2_CUDA(d.jointStart.upload(h.jointStart, nullptr));
+    MB2_CUDA(d.jointCapsule.upload(h.jointCapsule, nullptr));
+    return MB2_OK;
+  });
 }
 
 // builds the limit tables of c's limits and installs them (rejected limits install empty tables and keep the reason)
@@ -721,6 +750,10 @@ int mb2_character_clone(const mb2_character* c, int device, mb2_character** out)
   }
   if (c->tree.numNodes > 0) {
     rc = installMeshTree(copy, HostMeshTree(c->tree));
+    if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
+  }
+  if (c->collisionDev) {
+    rc = installCollision(copy, HostCollision(c->collision));
     if (rc != MB2_OK) { mb2_character_destroy(copy); return rc; }
   }
   *out = copy;
@@ -1215,6 +1248,64 @@ int mb2_character_parameter_limits_residual_device(const mb2_character* c, int32
 int mb2_character_parameter_limits_residual_backward_device(const mb2_character* c, int32_t batch, const float* model_parameters_device,
                                                             const float* grad_residual_device, float* grad_model_parameters_device, void* cuda_stream) {
   return parameterLimitsDevice(c, batch, model_parameters_device, nullptr, grad_residual_device, grad_model_parameters_device, cuda_stream, true);
+}
+
+int mb2_character_set_collision_geometry(mb2_character* c, int32_t count, const mb2_tapered_capsule* capsules) {
+  MB2_CHECK(c != nullptr, "null character");
+  HostCollision h;
+  const std::string err = makeCollision(c->host, count, capsules, h);
+  if (!err.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, err);
+  return installCollision(c, std::move(h));
+}
+
+int mb2_character_num_collision_pairs(const mb2_character* c, int32_t* out) {
+  MB2_CHECK(c != nullptr && out != nullptr, "null argument");
+  MB2_CHECK(c->collisionDev != nullptr, "collision: the character has no collision geometry");
+  *out = c->collision.numPairs();
+  return MB2_OK;
+}
+
+int mb2_character_get_collision_pairs(const mb2_character* c, int32_t* pairs) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(c->collisionDev != nullptr, "collision: the character has no collision geometry");
+  MB2_CHECK(pairs != nullptr || c->collision.pairs.empty(), "null argument");
+  std::copy(c->collision.pairs.begin(), c->collision.pairs.end(), pairs);
+  return MB2_OK;
+}
+
+namespace {
+// both directions of mb2_character_collision_residual*_device: residual is the forward's output, gradResidual the backward's input
+int collisionDevice(const mb2_character* c, int32_t batch, const float* state, float* residual, const float* gradResidual, float* gradState,
+                    void* stream, bool backward) {
+  MB2_CHECK(c != nullptr, "null character");
+  MB2_CHECK(batch >= 0, "batch must not be negative");
+  MB2_CHECK(c->collisionDev != nullptr, "collision: the character has no collision geometry");
+  if (batch == 0) return MB2_OK;
+  const bool rows = c->collision.numPairs() > 0;
+  MB2_CHECK(state != nullptr && (backward ? gradState != nullptr && (gradResidual != nullptr || !rows) : residual != nullptr || !rows), "null argument");
+  MB2_DEVICE_GUARD(c->device);
+  MB2_CHECK(onDevice(c->device, {state}, {residual, gradResidual, gradState}), "collision: every array must be device memory on the character's device");
+  NvtxRange range(backward ? "collisionResidualBackward" : "collisionResidual");
+  CollisionArgs a{};
+  a.T = c->tables();
+  a.L = c->collisionTables();
+  a.batch = batch;
+  a.state = state;
+  a.residual = residual;
+  a.gradResidual = gradResidual;
+  a.gradState = gradState;
+  MB2_CUDA(launchCollision(a, backward, (cudaStream_t)stream));
+  return MB2_OK;
+}
+} // namespace
+
+int mb2_character_collision_residual_device(const mb2_character* c, int32_t batch, const float* skel_state_device, float* residual_device,
+                                            void* cuda_stream) {
+  return collisionDevice(c, batch, skel_state_device, residual_device, nullptr, nullptr, cuda_stream, false);
+}
+int mb2_character_collision_residual_backward_device(const mb2_character* c, int32_t batch, const float* skel_state_device,
+                                                     const float* grad_residual_device, float* grad_skel_state_device, void* cuda_stream) {
+  return collisionDevice(c, batch, skel_state_device, nullptr, grad_residual_device, grad_skel_state_device, cuda_stream, true);
 }
 
 int mb2_character_joint_parameters_to_skeleton_state_device(const mb2_character* c, int32_t batch, const float* joint_parameters_device,
@@ -2148,14 +2239,21 @@ void instanceLaunchWords(const InstanceLaunchQuery& q, int64_t out[6]) {
 
 int mb2_character_get_instance_launch(const mb2_character* c, int32_t op, int32_t backward, int32_t batch, int32_t num_points, int64_t out[6]) {
   MB2_CHECK(c != nullptr && out != nullptr, "null argument");
-  MB2_CHECK((op >= kInstanceOpModelSkeletonState && op <= kInstanceOpJointPositions) || op == kInstanceOpParameterLimits,
-            "instance launch: op must be 0, 1, 2, 3 or 5");
+  MB2_CHECK((op >= kInstanceOpModelSkeletonState && op <= kInstanceOpJointPositions) || op == kInstanceOpParameterLimits || op == kInstanceOpCollision,
+            "instance launch: op must be 0, 1, 2, 3, 5 or 6");
+  MB2_CHECK(op != kInstanceOpCollision || c->collisionDev != nullptr, "collision: the character has no collision geometry");
   MB2_CHECK(batch >= 0 && num_points >= 0, "instance launch: batch and num_points must not be negative");
   MB2_CHECK(op != kInstanceOpParameterLimits || c->limits.rejected.empty(), c->limits.rejected);
   MB2_DEVICE_GUARD(c->device);
   InstanceLaunchQuery q;
   const bool joint = op == kInstanceOpJointSkeletonState || op == kInstanceOpJointPositions;
-  if (op == kInstanceOpParameterLimits) {
+  if (op == kInstanceOpCollision) {
+    CollisionArgs a{};
+    a.T = c->tables();
+    a.L = c->collisionTables();
+    a.batch = batch;
+    MB2_CUDA(launchCollision(a, backward != 0, nullptr, &q));
+  } else if (op == kInstanceOpParameterLimits) {
     ParameterLimitArgs a{};
     a.T = c->tables();
     a.L = c->limitTables();

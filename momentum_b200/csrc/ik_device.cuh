@@ -993,6 +993,219 @@ MB2_HD void limitGradPasses(const Lanes& g, const CharacterTables& C, const Skel
     out[p] = skelGradModelParameter(S, gjp, p) + limitTermSum(L, L.paramStart, L.paramLimit, L.paramCoef, p, th, jp, grad);
 }
 
+// ---- Self-collision of tapered capsules as a character operation (collision_residual) ---------------------------------------------
+// The world capsule (CollisionGeometryStateT::updatePrimitive, collision_geometry_state.cpp:28-48), the narrow phase of overlaps
+// (collision_geometry_state.h:120-157) over closestPointsOnSegments (math/utility.cpp:443-552), branch for branch in the reference's
+// operation order, and the exact derivative of the overlap. A capsule's world geometry is 8 values: origin, direction (its length is the
+// segment's), r0, r1; delta = r1 - r0.
+constexpr int kCapsuleFloats = 8;
+MB2_HD void skinStateGradient(const float* acc, const float* state, float* out); // below, with the skinning
+// sqrt(kCollisionWeight) at weight 1 (collision_error_function.h:139, collision_error_function.cpp getJacobian's wgt), in float
+MB2_HD float collisionRowWeight() { return sqrtf(5e-3f); }
+
+// capsule c's world geometry out [8] from its parent's skeleton state ps [8] (t, q, s; q normalised), nullptr for a world-fixed capsule:
+// origin t + rot(q^, s o), direction rot(q^, s d), radii s r
+MB2_HD void capsuleWorld(const CapsuleDesc& c, const float* ps, float* out) {
+  F3 o = ld3(c.origin), d = ld3(c.dir);
+  float r0 = c.r0, r1 = c.r1;
+  if (ps != nullptr) {
+    const Q4 u = qnormalized(ld4(ps + 3));
+    const float s = ps[7];
+    o = ld3(ps) + qrot(u, s * o);
+    d = qrot(u, s * d);
+    r0 = r0 * s;
+    r1 = r1 * s;
+  }
+  out[0] = o.x; out[1] = o.y; out[2] = o.z;
+  out[3] = d.x; out[4] = d.y; out[5] = d.z;
+  out[6] = r0; out[7] = r1;
+}
+
+// Which closed form a segment parameter of a contact came from: a constant (a clamp, or the 1e-7 snap), the interior solution
+// s = (b e - c d) / D, t = (a e - b d) / D, or the projection onto an edge of the other segment.
+enum SegmentForm : int {
+  kSegConst = 0,
+  kSegInterior = 1,
+  kSegEdge0 = 2, // s on the t = 0 edge: -d / a;        t on the s = 0 edge (and the parallel branch): e / c
+  kSegEdge1 = 3, // s on the t = 1 edge: (b - d) / a;   t on the s = 1 edge: (e + b) / c
+};
+template <class T>
+struct CapsuleContact {
+  bool hit;     // overlaps(): overlap > 0 and dist >= Eps
+  T s, t;       // the closest-point parameters
+  T dist, overlap;
+  int sForm, tForm;
+};
+template <class T>
+MB2_HD T segDot(const T* a, const T* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+
+// overlaps(A, B) of two world capsules A, B [8] (T = float: the reference's float build; the planner's rest pose runs it in double, with
+// double's Eps as the reference's double build has it). A non-finite input fails every comparison that would report a contact.
+template <class T>
+MB2_HD CapsuleContact<T> capsuleContact(const T* A, const T* B) {
+  CapsuleContact<T> r;
+  r.hit = false;
+  r.s = r.t = r.dist = r.overlap = T(0);
+  r.sForm = r.tForm = kSegConst;
+  const T maxA = A[6] < A[7] ? A[7] : A[6], maxB = B[6] < B[7] ? B[7] : B[6]; // Vector2::maxCoeff
+  const T maxDist = maxA + maxB;
+  const T maxSq = maxDist * maxDist;
+  const T* d1 = A + 3;
+  const T* d2 = B + 3;
+  const T w[3] = {A[0] - B[0], A[1] - B[1], A[2] - B[2]};
+  const T a = segDot(d1, d1), b = segDot(d1, d2), c = segDot(d2, d2), d = segDot(d1, w), e = segDot(d2, w);
+  const T D = a * c - b * b;
+  T sN, sD = D, tN, tD = D;
+  int sF, tF;
+  if (D < T(1e-7)) { // parallel: s = 0, t along d2; too far when the origins are (the reference's early-out)
+    sN = T(0); sD = T(1); tN = e; tD = c;
+    sF = kSegConst; tF = kSegEdge0;
+    if (segDot(w, w) > maxSq) return r;
+  } else {
+    sN = b * e - c * d;
+    tN = a * e - b * d;
+    sF = tF = kSegInterior;
+    const T q[3] = {w[0] + d1[0] * sN / D - d2[0] * tN / D, w[1] + d1[1] * sN / D - d2[1] * tN / D, w[2] + d1[2] * sN / D - d2[2] * tN / D};
+    if (segDot(q, q) > maxSq) return r; // the infinite lines are too far
+    if (sN < T(0)) { sN = T(0); tN = e; tD = c; sF = kSegConst; tF = kSegEdge0; }
+    else if (sN > sD) { sN = sD; tN = e + b; tD = c; sF = kSegConst; tF = kSegEdge1; }
+  }
+  if (tN < T(0)) {
+    tN = T(0); tF = kSegConst;
+    if (-d < T(0)) { sN = T(0); sF = kSegConst; }
+    else if (-d > a) { sN = sD; sF = kSegConst; }
+    else { sN = -d; sD = a; sF = kSegEdge0; }
+  } else if (tN > tD) {
+    tN = tD; tF = kSegConst;
+    if ((-d + b) < T(0)) { sN = T(0); sF = kSegConst; }
+    else if ((-d + b) > a) { sN = sD; sF = kSegConst; }
+    else { sN = (-d + b); sD = a; sF = kSegEdge1; }
+  }
+  using std::fabs;
+  using std::sqrt;
+  const bool sSnap = fabs(sN) < T(1e-7) || fabs(sD) < T(1e-7), tSnap = fabs(tN) < T(1e-7) || fabs(tD) < T(1e-7);
+  const T s = sSnap ? T(0) : sN / sD, t = tSnap ? T(0) : tN / tD;
+  const T dP[3] = {w[0] + d1[0] * s - d2[0] * t, w[1] + d1[1] * s - d2[1] * t, w[2] + d1[2] * s - d2[2] * t};
+  const T distSq = segDot(dP, dP);
+  if (distSq > maxSq) return r;
+  const T dist = sqrt(distSq);
+  const T overlap = A[6] + s * (A[7] - A[6]) + B[6] + t * (B[7] - B[6]) - dist;
+  r.s = s; r.t = t; r.dist = dist; r.overlap = overlap;
+  r.sForm = sSnap ? int(kSegConst) : sF;
+  r.tForm = tSnap ? int(kSegConst) : tF;
+  r.hit = overlap > T(0) && dist >= (sizeof(T) == 4 ? T(1e-8) : T(1e-17));
+  return r;
+}
+
+// The exact derivative of a contact's overlap with respect to A [8] and B [8], times gw, added to gA and gB (either may be nullptr):
+// at fixed (s, t), d overlap = -n . d(dP) + ds (r1 - r0)_A ... with n = dP / dist; s and t move through the closed form of their branch
+// (sForm, tForm) with g_s = delta_A - n . dA, g_t = delta_B + n . dB, by way of a = dA.dA, b = dA.dB, c = dB.dB, d = dA.w, e = dB.w.
+// Constants (clamps, snaps) do not move. Unlike CollisionErrorFunction::getJacobian, which holds (s, t) fixed, this keeps delta ds.
+template <class T>
+MB2_HD void capsuleContactGrad(const T* A, const T* B, const CapsuleContact<T>& k, T gw, T* gA, T* gB) {
+  const T* d1 = A + 3;
+  const T* d2 = B + 3;
+  const T w[3] = {A[0] - B[0], A[1] - B[1], A[2] - B[2]};
+  const T a = segDot(d1, d1), b = segDot(d1, d2), c = segDot(d2, d2), d = segDot(d1, w), e = segDot(d2, w);
+  const T D = a * c - b * b;
+  const T s = k.s, t = k.t;
+  const T n[3] = {(w[0] + d1[0] * s - d2[0] * t) / k.dist, (w[1] + d1[1] * s - d2[1] * t) / k.dist, (w[2] + d1[2] * s - d2[2] * t) / k.dist};
+  const T gs = (A[7] - A[6]) - segDot(n, d1), gt = (B[7] - B[6]) + segDot(n, d2);
+  T ga = T(0), gb = T(0), gc = T(0), gd = T(0), ge = T(0);
+  if (k.sForm == kSegInterior) {
+    ga += gs * (-s * c) / D; gb += gs * (e + T(2) * b * s) / D; gc += gs * (-d - s * a) / D; gd += gs * (-c) / D; ge += gs * b / D;
+  } else if (k.sForm == kSegEdge0) {
+    gd += -gs / a; ga += -gs * s / a;
+  } else if (k.sForm == kSegEdge1) {
+    gb += gs / a; gd += -gs / a; ga += -gs * s / a;
+  }
+  if (k.tForm == kSegInterior) {
+    ga += gt * (e - t * c) / D; gb += gt * (-d + T(2) * b * t) / D; gc += gt * (-t * a) / D; gd += gt * (-b) / D; ge += gt * a / D;
+  } else if (k.tForm == kSegEdge0) {
+    ge += gt / c; gc += -gt * t / c;
+  } else if (k.tForm == kSegEdge1) {
+    ge += gt / c; gb += gt / c; gc += -gt * t / c;
+  }
+  for (int i = 0; i < 3; ++i) {
+    const T gW = -n[i] + gd * d1[i] + ge * d2[i];
+    if (gA != nullptr) {
+      gA[i] += gw * gW;
+      gA[3 + i] += gw * (-s * n[i] + T(2) * ga * d1[i] + gb * d2[i] + gd * w[i]);
+    }
+    if (gB != nullptr) {
+      gB[i] += gw * -gW;
+      gB[3 + i] += gw * (t * n[i] + gb * d1[i] + T(2) * gc * d2[i] + ge * w[i]);
+    }
+  }
+  if (gA != nullptr) { gA[6] += gw * (T(1) - s); gA[7] += gw * s; }
+  if (gB != nullptr) { gB[6] += gw * (T(1) - t); gB[7] += gw * t; }
+}
+
+// lanes = capsules: the world geometry geo [C][8] of one instance's states st [J][8]. Ends with a barrier.
+template <class Lanes>
+MB2_HD void collisionGeometryPasses(const Lanes& g, const CollisionTables& L, const float* st, float* geo) {
+  for (int k = g.lane; k < L.numCapsules; k += g.size) {
+    const CapsuleDesc& c = L.capsules[k];
+    capsuleWorld(c, c.parent >= 0 ? st + size_t(c.parent) * 8 : nullptr, geo + size_t(k) * kCapsuleFloats);
+  }
+  g.sync();
+}
+
+// The rows out [P] of one instance, lanes = pairs: sqrt(kCollisionWeight) overlap at a contact, else 0. Ends without a barrier.
+template <class Lanes>
+MB2_HD void collisionPasses(const Lanes& g, const CollisionTables& L, const float* st, float* geo, float* out) {
+  collisionGeometryPasses(g, L, st, geo);
+  const float wgt = collisionRowWeight();
+  for (int k = g.lane; k < L.numPairs; k += g.size) {
+    const CapsuleContact<float> c = capsuleContact(geo + size_t(L.pairs[2 * k]) * kCapsuleFloats, geo + size_t(L.pairs[2 * k + 1]) * kCapsuleFloats);
+    out[k] = c.hit ? wgt * c.overlap : 0.f;
+  }
+}
+
+// Its backward from grad [P] into out [J][8]: lanes = capsules walk their own pairs in ascending order, recompute each contact and sum
+// their own side's gradient into cg [C][8]; lanes = joints then take their capsules in order: the origin and the end point are fixed in the
+// parent's frame (a = sum g_o, E = sum g_o o^T + g_d d^T, skinStateGradient's (a, E) with q normalised) and the radii scale with s, so
+// ds gains sum (r0 g_r0 + r1 g_r1). Joints without a capsule get 0. Ends without a barrier.
+template <class Lanes>
+MB2_HD void collisionGradPasses(const Lanes& g, const CollisionTables& L, int numJoints, const float* st, float* geo, float* cg, const float* grad,
+                                float* out) {
+  collisionGeometryPasses(g, L, st, geo);
+  const float wgt = collisionRowWeight();
+  for (int k = g.lane; k < L.numCapsules; k += g.size) {
+    float acc[kCapsuleFloats] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int e = L.capsuleStart[k]; e < L.capsuleStart[k + 1]; ++e) {
+      const int p = L.capsulePair[e], i = L.pairs[2 * p], j = L.pairs[2 * p + 1];
+      const float* A = geo + size_t(i) * kCapsuleFloats;
+      const float* B = geo + size_t(j) * kCapsuleFloats;
+      const CapsuleContact<float> c = capsuleContact(A, B);
+      if (c.hit) capsuleContactGrad(A, B, c, wgt * grad[p], i == k ? acc : nullptr, i == k ? nullptr : acc);
+    }
+    for (int i = 0; i < kCapsuleFloats; ++i) cg[size_t(k) * kCapsuleFloats + i] = acc[i];
+  }
+  g.sync();
+  for (int j = g.lane; j < numJoints; j += g.size) {
+    float* o = out + size_t(j) * 8;
+    if (L.jointStart[j] == L.jointStart[j + 1]) {
+      for (int i = 0; i < 8; ++i) o[i] = 0.f;
+      continue;
+    }
+    float acc[12] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}; // skinAccumulate's (a, E)
+    float dsr = 0.f;
+    for (int e = L.jointStart[j]; e < L.jointStart[j + 1]; ++e) {
+      const int k = L.jointCapsule[e];
+      const CapsuleDesc& c = L.capsules[k];
+      const float* gk = cg + size_t(k) * kCapsuleFloats;
+      for (int r = 0; r < 3; ++r) {
+        acc[r] += gk[r];
+        for (int col = 0; col < 3; ++col) acc[3 + 3 * r + col] += gk[r] * c.origin[col] + gk[3 + r] * c.dir[col];
+      }
+      dsr += c.r0 * gk[6] + c.r1 * gk[7];
+    }
+    skinStateGradient(acc, st + size_t(j) * 8, o);
+    o[7] += dsr;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Evaluate one unit: residual rows, error contribution, and the evaluation record consumed by its
 // Jacobian cells. kJacobian=false is the getError() path (joint_error_function-inl.h:35-54 etc.):

@@ -34,6 +34,8 @@ InstanceLaunch planInstanceOp(const CharacterTables& C, int numChildren, int op,
   if (op == kInstanceOpParameterLimits)
     return planInstanceGroups(sizeof(float) * parameterLimitsSmemPerInstanceFloats(C.numJoints, C.numParams, backward, limitsFk),
                               parameterLimitsTableBytes(C, numChildren, backward, limitsFk), batch, smemBudget, numSms);
+  if (op == kInstanceOpCollision)
+    return planInstanceGroups(sizeof(float) * collisionSmemPerInstanceFloats(numPoints, backward), 0, batch, smemBudget, numSms);
   const bool joint = op == kInstanceOpJointSkeletonState || op == kInstanceOpJointPositions;
   const size_t per = sizeof(float) * skeletonStateSmemPerInstanceFloats(C.numJoints, C.numParams, backward, joint);
   const size_t tables = skeletonStateTableBytes(C, numChildren, backward, joint);

@@ -1,5 +1,5 @@
 // The launch of the per-instance kernels of the character operations (skeletonStateKernel, positionsKernel, inputGradientKernel,
-// parameterLimitsKernel): their shared memory per instance and per CTA, and the one rule that picks the warps per instance W and the
+// parameterLimitsKernel, collisionKernel): their shared memory per instance and per CTA, and the one rule that picks the warps per instance W and the
 // instance groups per CTA from it.
 // Host code shared by the library (ik_kernels.cu) and the CPU emulator (tests/emu), so that the launch a test sizes a rig for is the
 // launch that runs.
@@ -62,6 +62,11 @@ inline size_t parameterLimitsTableBytes(const CharacterTables& C, int numChildre
   if (backward) w += tableWords(size_t(C.numParams) + 1, 4) + tableWords(size_t(C.ptNnz), 4) * 2;
   return w * 4;
 }
+// collisionKernel, per instance: the world capsules [C][8]; backward: their gradients [C][8]. The skeleton states are read from global
+// memory where a capsule needs its parent's, and the collision tables are read from global memory: no staged tables.
+MB2_HD size_t collisionSmemPerInstanceFloats(int numCapsules, bool backward) {
+  return skelAligned(size_t(numCapsules) * 8) * (backward ? 2 : 1);
+}
 // inputGradientKernel, per instance: theta [n], v [n], joint states [J][17], joint motions [J][7]; its tables are the character's
 MB2_HD size_t inputGradientSmemPerInstanceFloats(int J, int n) {
   return 2 * skelAligned(size_t(n)) + skelAligned(size_t(J) * kJointStateStride) + skelAligned(size_t(J) * kTangentStride);
@@ -90,9 +95,10 @@ enum InstanceOp : int32_t { // the operations whose kernels run in this frame (m
   kInstanceOpJointPositions = 3,     // positionsKernel<kBackward, W, true, kStagePoints>
   kInstanceOpInputGradients = 4,     // inputGradientKernel<W> (forward only)
   kInstanceOpParameterLimits = 5,    // parameterLimitsKernel<kBackward, W, kEllipsoid>
+  kInstanceOpCollision = 6,          // collisionKernel<kBackward, W>
 };
 // The launch of one operation over `batch` instances of the character C (numChildren: entries of its children table), with numPoints
-// points for the positions, whose tables are staged when that costs no instance per CTA. limitsFk: for the parameter limits, that the
+// points for the positions (for the collision: numPoints capsules), whose tables are staged when that costs no instance per CTA. limitsFk: for the parameter limits, that the
 // character has an Ellipsoid limit, so the kernel runs the FK passes (LimitTables::ellipsoid).
 InstanceLaunch planInstanceOp(const CharacterTables& C, int numChildren, int op, bool backward, int numPoints, long batch, size_t smemBudget,
                               int numSms, bool limitsFk = false);

@@ -788,6 +788,46 @@ cudaError_t launchParameterLimits(const ParameterLimitArgs& a, bool backward, cu
 }
 
 // ------------------------------------------------------------------------------------------------
+// Self-collision rows of tapered capsules (ik_device.cuh collisionPasses / collisionGradPasses), in the per-instance frame of
+// skeletonStateKernel: lanes = capsules build the world capsules in shared memory from their parents' states, then
+//   forward:   lanes = pairs write the rows;
+//   backward:  lanes = capsules walk their own pairs (a host-planned CSR, pairs ascending), recompute each contact and sum their own
+//              side's gradient in shared memory; lanes = joints sum their capsules in CSR order into dLoss / d state.
+// No atomics and no global scratch: every output is one lane's fixed-order sum, so no result depends on the launch shape. The collision
+// tables are read from global memory; the states are read where a capsule or a joint with capsules needs them.
+// ------------------------------------------------------------------------------------------------
+template <bool kBackward, int W>
+__global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) collisionKernel(const CollisionArgs a) {
+  extern __shared__ __align__(16) float smem[];
+  const CollisionTables L = a.L;
+  const WarpLanes<W> g = WarpLanes<W>::of(threadIdx.x >> 5, threadIdx.x & 31);
+  const int groupsPerCta = (blockDim.x >> 5) / W;
+  const int J = a.T.numJoints, P = L.numPairs;
+  const int perGroup = int(collisionSmemPerInstanceFloats(L.numCapsules, kBackward));
+  float* geo = smem + size_t(g.group) * perGroup;
+  float* cg = geo + skelAligned(size_t(L.numCapsules) * kCapsuleFloats);
+  for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
+    const float* st = a.state + size_t(b) * J * 8;
+    if constexpr (!kBackward) collisionPasses(g, L, st, geo, a.residual + size_t(b) * P);
+    else collisionGradPasses(g, L, J, st, geo, cg, a.gradResidual + size_t(b) * P, a.gradState + size_t(b) * J * 8);
+    g.sync(); // the next instance overwrites geo / cg
+  }
+}
+
+cudaError_t launchCollision(const CollisionArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query) {
+  using K = void (*)(CollisionArgs);
+  static const K kernels[2][4] = {{collisionKernel<false, 1>, collisionKernel<false, 2>, collisionKernel<false, 4>, collisionKernel<false, 8>},
+                                  {collisionKernel<true, 1>, collisionKernel<true, 2>, collisionKernel<true, 4>, collisionKernel<true, 8>}};
+  if (query) *query = InstanceLaunchQuery{};
+  if (a.batch <= 0) return cudaSuccess;
+  if (a.L.numPairs == 0) { // no pair: nothing to write, and the gradient is zero
+    if (query) return cudaSuccess;
+    return backward ? cudaMemsetAsync(a.gradState, 0, size_t(a.batch) * a.T.numJoints * 8 * sizeof(float), stream) : cudaSuccess;
+  }
+  return launchInstanceGroups(kernels[backward], a, 0, kInstanceOpCollision, backward, a.L.numCapsules, stream, query);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Skinning with an identity blend shape (ik_device.cuh blendShapeRest / blendWeightAccumulate), on the skinning's building blocks.
 // A work item is (a tile of T instances, a block of kSkinThreads vertices, one per thread).
 //   blendSkinKernel<T, kRestOnly>   the tile's weights [K'][T] in shared memory; each thread forms its vertex's rest points for the T

@@ -199,6 +199,20 @@ struct ParameterLimitArgs {
 // Both enqueue on `stream` and take no scratch. R == 0: the forward writes nothing and the backward zeroes gradTheta. With `query`,
 // the launch is reported there and nothing is enqueued.
 cudaError_t launchParameterLimits(const ParameterLimitArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query = nullptr);
+// collisionKernel<kBackward>: the self-collision rows of the character's tapered capsules for a batch of skeleton states, and their
+// backward
+struct CollisionArgs {
+  CharacterTables T;          // numJoints only
+  CollisionTables L;          // device memory
+  int32_t batch;
+  const float* state;         // [B][J][8]
+  float* residual;            // forward: [B][P]
+  const float* gradResidual;  // backward: [B][P] dLoss / d residual
+  float* gradState;           // backward: [B][J][8], overwritten
+};
+// Both enqueue on `stream` and take no scratch. P == 0: the forward writes nothing and the backward zeroes gradState. With `query`, the
+// launch is reported there and nothing is enqueued.
+cudaError_t launchCollision(const CollisionArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query = nullptr);
 // parameterTransformKernel ... clampParametersBackwardKernel: the flat joint-parameter operations of ik_device.cuh jointOpElement for a
 // batch, forward or backward; arrays [B][...] dense, device memory
 struct JointOpArgs {

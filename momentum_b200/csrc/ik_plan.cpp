@@ -1,5 +1,7 @@
 #include "ik_plan.h"
 
+#include "ik_device.cuh" // capsuleContact, shared with the kernels
+
 #include <algorithm>
 #include <array>
 #include <cfloat>
@@ -582,6 +584,138 @@ LimitTables hostLimitTables(const HostLimitTables& t) {
   return LimitTables{int32_t(t.limits.size()), t.numRows, t.ellipsoid ? 1 : 0, t.limits.data(), t.ellipsoidData.data(), t.jointStart.data(),
                      t.jointEntry.data(), t.rowStart.data(), t.rowLimit.data(), t.rowCoef.data(), t.paramStart.data(), t.paramLimit.data(),
                      t.paramCoef.data()};
+}
+
+namespace {
+// Eigen QuaternionBase::_transformVector in double
+void rotateDouble(const double* q, const double* v, double* r) {
+  const double uv[3] = {2.0 * (q[1] * v[2] - q[2] * v[1]), 2.0 * (q[2] * v[0] - q[0] * v[2]), 2.0 * (q[0] * v[1] - q[1] * v[0])};
+  const double c[3] = {q[1] * uv[2] - q[2] * uv[1], q[2] * uv[0] - q[0] * uv[2], q[0] * uv[1] - q[1] * uv[0]};
+  for (int i = 0; i < 3; ++i) r[i] = v[i] + q[3] * uv[i] + c[i];
+}
+// JointStateT::set of every joint at model parameters zero (joint parameters = the ParameterTransform's offsets), in double:
+// t [J][3], q [J][4] (x, y, z, w), s [J]
+void restPoseDouble(const HostCharacter& ch, std::vector<double>& t, std::vector<double>& q, std::vector<double>& s) {
+  const int J = ch.numJoints;
+  t.assign(size_t(J) * 3, 0.0);
+  q.assign(size_t(J) * 4, 0.0);
+  s.assign(size_t(J), 0.0);
+  auto mul = [](const double* a, const double* b, double* r) {
+    const double x = a[3] * b[0] + a[0] * b[3] + a[1] * b[2] - a[2] * b[1], y = a[3] * b[1] + a[1] * b[3] + a[2] * b[0] - a[0] * b[2];
+    const double z = a[3] * b[2] + a[2] * b[3] + a[0] * b[1] - a[1] * b[0], w = a[3] * b[3] - a[0] * b[0] - a[1] * b[1] - a[2] * b[2];
+    r[0] = x; r[1] = y; r[2] = z; r[3] = w;
+  };
+  for (int j = 0; j < J; ++j) {
+    const float* p = ch.ptOffsets.data() + size_t(j) * kParametersPerJoint;
+    double ql[4] = {ch.prerot[4 * j], ch.prerot[4 * j + 1], ch.prerot[4 * j + 2], ch.prerot[4 * j + 3]};
+    for (int k = 2; k >= 0; --k) { // preRot Rz Ry Rx (joint_state.cpp:44-62)
+      double r[4] = {0.0, 0.0, 0.0, std::cos(0.5 * double(p[3 + k]))};
+      r[k] = std::sin(0.5 * double(p[3 + k]));
+      mul(ql, r, ql);
+    }
+    const double tl[3] = {double(ch.offset[3 * j]) + p[0], double(ch.offset[3 * j + 1]) + p[1], double(ch.offset[3 * j + 2]) + p[2]};
+    const double sl = std::exp2(double(p[6]));
+    const int par = ch.parent[j];
+    if (par < 0) {
+      for (int i = 0; i < 3; ++i) t[3 * j + i] = tl[i];
+      for (int i = 0; i < 4; ++i) q[4 * j + i] = ql[i];
+      s[j] = sl;
+      continue;
+    }
+    const double* qp = &q[4 * par];
+    const double v[3] = {s[par] * tl[0], s[par] * tl[1], s[par] * tl[2]};
+    double rv[3];
+    rotateDouble(qp, v, rv);
+    for (int i = 0; i < 3; ++i) t[3 * j + i] = t[3 * par + i] + rv[i];
+    mul(qp, ql, &q[4 * j]);
+    s[j] = s[par] * sl;
+  }
+}
+} // namespace
+
+std::string makeCollision(const HostCharacter& ch, int32_t count, const mb2_tapered_capsule* capsules, HostCollision& out) {
+  if (count < 0 || (count > 0 && capsules == nullptr)) return "collision geometry: count must not be negative and capsules must not be null";
+  const int J = ch.numJoints;
+  HostCollision h;
+  h.capsules.resize(size_t(count));
+  std::vector<double> local(size_t(count) * 8); // origin, dir, r0, r1 in double
+  for (int k = 0; k < count; ++k) {
+    const mb2_tapered_capsule& c = capsules[k];
+    const std::string name = "collision geometry: capsule " + std::to_string(k);
+    if (c.parent < -1 || c.parent >= J) return name + ": parent " + std::to_string(c.parent) + " is outside [-1, J)";
+    const float* values[] = {c.translation, c.translation + 1, c.translation + 2, c.rotation, c.rotation + 1, c.rotation + 2, c.rotation + 3,
+                             &c.scale, c.radius, c.radius + 1, &c.length};
+    for (const float* v : values)
+      if (!std::isfinite(*v)) return name + ": every value must be finite";
+    if (c.radius[0] < 0.f || c.radius[1] < 0.f) return name + ": a radius is negative";
+    if (c.length < 0.f) return name + ": the length is negative";
+    double qn = 0.0;
+    for (int i = 0; i < 4; ++i) qn += double(c.rotation[i]) * c.rotation[i];
+    if (!(qn > 0.0)) return name + ": the rotation is zero";
+    qn = std::sqrt(qn);
+    const double q[4] = {c.rotation[0] / qn, c.rotation[1] / qn, c.rotation[2] / qn, c.rotation[3] / qn};
+    const double ex[3] = {double(c.scale) * c.length, 0.0, 0.0};
+    double* L = &local[size_t(k) * 8];
+    rotateDouble(q, ex, L + 3);
+    for (int i = 0; i < 3; ++i) L[i] = c.translation[i];
+    L[6] = c.radius[0];
+    L[7] = c.radius[1];
+    CapsuleDesc& d = h.capsules[k];
+    d.parent = c.parent;
+    for (int i = 0; i < 3; ++i) { d.origin[i] = float(L[i]); d.dir[i] = float(L[3 + i]); }
+    for (int i = 0; i < 3; ++i) // scale times length can overflow float although both are finite
+      if (!std::isfinite(d.dir[i])) return name + ": its direction (scale times length) overflows float";
+    d.r0 = c.radius[0];
+    d.r1 = c.radius[1];
+  }
+  // the rest pose's world capsules (updatePrimitive), in double
+  std::vector<double> t, q, s, world(size_t(count) * 8);
+  restPoseDouble(ch, t, q, s);
+  for (int k = 0; k < count; ++k) {
+    const double* L = &local[size_t(k) * 8];
+    double* W = &world[size_t(k) * 8];
+    const int p = h.capsules[k].parent;
+    if (p < 0) { std::copy(L, L + 8, W); continue; }
+    const double so[3] = {s[p] * L[0], s[p] * L[1], s[p] * L[2]}, sd[3] = {s[p] * L[3], s[p] * L[4], s[p] * L[5]};
+    rotateDouble(&q[4 * p], so, W);
+    for (int i = 0; i < 3; ++i) W[i] += t[3 * p + i];
+    rotateDouble(&q[4 * p], sd, W + 3);
+    W[6] = L[6] * s[p];
+    W[7] = L[7] * s[p];
+  }
+  // updateCollisionPairs / isValidCollisionPair (collision_geometry_state.h:526-557), i < j ascending
+  for (int i = 0; i < count; ++i)
+    for (int j = i + 1; j < count; ++j) {
+      const int p0 = h.capsules[i].parent, p1 = h.capsules[j].parent;
+      bool valid;
+      if (p0 < 0 || p1 < 0) valid = p0 != p1;
+      else if (p0 == p1 || ch.parent[p0] == p1 || ch.parent[p1] == p0) valid = false;
+      else valid = !capsuleContact<double>(&world[size_t(i) * 8], &world[size_t(j) * 8]).hit;
+      if (valid) { h.pairs.push_back(i); h.pairs.push_back(j); }
+    }
+  const int P = h.numPairs();
+  h.capsuleStart.assign(size_t(count) + 1, 0);
+  for (int k = 0; k < 2 * P; ++k) ++h.capsuleStart[size_t(h.pairs[k]) + 1];
+  for (int k = 0; k < count; ++k) h.capsuleStart[k + 1] += h.capsuleStart[k];
+  h.capsulePair.assign(size_t(2) * P, 0);
+  std::vector<int32_t> fill(h.capsuleStart.begin(), h.capsuleStart.end() - 1);
+  for (int p = 0; p < P; ++p) // pairs ascending within a capsule
+    for (int side = 0; side < 2; ++side) h.capsulePair[fill[size_t(h.pairs[2 * p + side])]++] = p;
+  h.jointStart.assign(size_t(J) + 1, 0);
+  for (const CapsuleDesc& c : h.capsules)
+    if (c.parent >= 0) ++h.jointStart[size_t(c.parent) + 1];
+  for (int j = 0; j < J; ++j) h.jointStart[j + 1] += h.jointStart[j];
+  h.jointCapsule.assign(size_t(h.jointStart[J]), 0);
+  fill.assign(h.jointStart.begin(), h.jointStart.end() - 1);
+  for (int k = 0; k < count; ++k)
+    if (h.capsules[k].parent >= 0) h.jointCapsule[fill[size_t(h.capsules[k].parent)]++] = k;
+  out = std::move(h);
+  return "";
+}
+
+CollisionTables hostCollisionTables(const HostCollision& c) {
+  return CollisionTables{int32_t(c.capsules.size()), c.numPairs(), c.capsules.data(), c.pairs.data(), c.capsuleStart.data(),
+                         c.capsulePair.data(), c.jointStart.data(), c.jointCapsule.data()};
 }
 
 // What Position, Plane and Orientation blocks share: the generalized loss, and the parent joint and weight of each constraint.

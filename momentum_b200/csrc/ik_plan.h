@@ -72,6 +72,19 @@ HostLimitTables makeLimitTables(const HostCharacter& ch);
 // LimitTables over the host vectors of t
 LimitTables hostLimitTables(const HostLimitTables& t);
 
+// The character's tapered capsules as collision_residual reads them (CollisionTables), built by makeCollision only, when the geometry is
+// set: the capsules in their parents' frames, the valid pairs of updateCollisionPairs / isValidCollisionPair with filterRestPoseOverlaps
+// (the rest pose, model parameters zero through the ParameterTransform, evaluated in double), and the two CSRs of the backward.
+struct HostCollision {
+  std::vector<CapsuleDesc> capsules;
+  std::vector<int32_t> pairs; // [P][2]
+  std::vector<int32_t> capsuleStart, capsulePair, jointStart, jointCapsule;
+  int32_t numPairs() const { return int32_t(pairs.size() / 2); }
+};
+// count capsules as mb2_tapered_capsule; an empty string when they are valid, else the reason, naming the capsule
+std::string makeCollision(const HostCharacter& ch, int32_t count, const mb2_tapered_capsule* capsules, HostCollision& out);
+CollisionTables hostCollisionTables(const HostCollision& c);
+
 // Linear-blend skinning of a character (SkinWeights + Character::inverseBindPose, skin_weights.h:19-40, character.h), flattened into
 // the tables of SkinTables (ik_types.h). Built and validated by makeSkinning only.
 struct HostSkinning {

@@ -206,6 +206,29 @@ struct PointTables {
   const int32_t* pointIndex; // [N]
 };
 
+// One tapered capsule of collision_residual (makeCollision), in its parent joint's frame: the world origin is T_parent(origin), the world
+// direction s_parent R_parent dir and the world radii r0, r1 times s_parent, with T_parent the identity for a world-fixed capsule
+// (CollisionGeometryStateT::updatePrimitive). origin and dir fold the capsule's local transformation and length, rounded once from double.
+struct CapsuleDesc {
+  int32_t parent;  // joint, or -1: world-fixed
+  float origin[3]; // translation
+  float dir[3];    // R(rotation) e_x scale length
+  float r0, r1;    // radius
+};
+
+// The character's collision geometry as collision_residual reads it (makeCollision), shared by the batch: the capsules, the valid pairs
+// (updateCollisionPairs, ascending), each capsule's pairs (CSR, pair indices ascending) and each joint's capsules (CSR, ascending).
+struct CollisionTables {
+  int32_t numCapsules;
+  int32_t numPairs;
+  const CapsuleDesc* capsules;   // [C]
+  const int32_t* pairs;          // [P][2], i < j
+  const int32_t* capsuleStart;   // [C+1] into capsulePair
+  const int32_t* capsulePair;
+  const int32_t* jointStart;     // [J+1] into jointCapsule
+  const int32_t* jointCapsule;
+};
+
 // The flat joint-parameter operations (ik_device.cuh jointOpElement), forward / backward:
 //   kJointOpParameterTransform  jp [7 J] = P theta + o (jointParameterRow)      /  g_theta [n] = P^T g_jp
 //   kJointOpLocalState          local states [J][8] of jp [J][7]                /  g_jp [J][7] of g_local [J][8]

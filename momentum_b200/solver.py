@@ -144,6 +144,11 @@ CABI_SIGNATURES = {
     "mb2_solver_get_fused_profile": (_int, [_vp, _ip, _ip, _dp, _up]),
     "mb2_solver_function_get_sweep_launch": (_int, [_vp, _int32, _lp]),
     "mb2_character_get_instance_launch": (_int, [_vp, _int32, _int32, _int32, _int32, _lp]),
+    "mb2_character_set_collision_geometry": (_int, [_vp, _int32, _vp]),
+    "mb2_character_num_collision_pairs": (_int, [_vp, _ip]),
+    "mb2_character_get_collision_pairs": (_int, [_vp, _vp]),
+    "mb2_character_collision_residual_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
+    "mb2_character_collision_residual_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
     "mb2_character_num_limit_residuals": (_int, [_vp, _ip]),
     "mb2_character_parameter_limits_residual_device": (_int, [_vp, _int32, _vp, _vp, _vp]),
     "mb2_character_parameter_limits_residual_backward_device": (_int, [_vp, _int32, _vp, _vp, _vp, _vp]),
@@ -294,6 +299,8 @@ INSTANCE_OPS = {"model_parameters_to_skeleton_state": 0, "joint_parameters_to_sk
                 "joint_parameters_to_positions": 3}
 # its op code of parameter_limits_residual, whose launch depends on the character's limits rather than on a rig alone
 PARAMETER_LIMITS_INSTANCE_OP = 5
+# and of collision_residual, whose launch depends on the character's capsules
+COLLISION_INSTANCE_OP = 6
 
 
 def _instance_launch(out) -> dict:
@@ -328,6 +335,13 @@ class DeviceCharacter(_Base):
                 for j in range(27):
                     arr[k].f[j] = float(ff[j])
             self._check(self._L.mb2_character_set_parameter_limits(self._h, len(character.limits), arr))
+        # Capsules the library rejects are reported by the collision calls, as a rejected blend shape is: nothing else depends on them.
+        self.collision, self.collision_error = None, None
+        if character.collision is not None:
+            try:
+                self.set_collision_geometry(character.collision)
+            except (MomentumB200Error, ValueError) as e:
+                self.collision_error = str(e)
         self.skinning, self.faces, self.faces_error, self.mesh_tree_error = None, None, None, None
         if character.skinning is not None:
             self.set_skinning(character.skinning)
@@ -473,13 +487,44 @@ class DeviceCharacter(_Base):
         self._check(fn(self._h, int(batch), *ptrs, stream))
 
     def get_instance_launch(self, op: str, backward: bool, batch: int, num_points: int = 0) -> dict:
-        """What the per-instance kernel of ``op`` (a key of ``INSTANCE_OPS``, or "parameter_limits_residual") would launch for ``batch``
+        """What the per-instance kernel of ``op`` (a key of ``INSTANCE_OPS``, "parameter_limits_residual" or "collision_residual") would launch for ``batch``
         instances (and ``num_points`` points): warps per instance, instances per CTA, threads per CTA, CTAs, dynamic shared memory bytes
         and whether the point tables are staged. All zero when nothing runs; raises when one instance does not fit in shared memory."""
-        code = PARAMETER_LIMITS_INSTANCE_OP if op == "parameter_limits_residual" else INSTANCE_OPS[op]
+        code = {"parameter_limits_residual": PARAMETER_LIMITS_INSTANCE_OP, "collision_residual": COLLISION_INSTANCE_OP}.get(op)
+        code = INSTANCE_OPS[op] if code is None else code
         out = (C.c_int64 * 6)()
         self._check(self._L.mb2_character_get_instance_launch(self._h, code, int(bool(backward)), int(batch), int(num_points), out))
         return _instance_launch(out)
+
+    def set_collision_geometry(self, capsules):
+        """Uploads the tapered capsules (a list of ``character.TaperedCapsule``, replacing any earlier geometry; empty is valid) and plans
+        their valid pairs; ``self.collision`` is the list uploaded and ``self.num_collision_pairs`` P. Raises naming the capsule when one is rejected, and keeps the earlier
+        geometry then."""
+        arr = mc.capsule_array(capsules)
+        self._check(self._L.mb2_character_set_collision_geometry(self._h, len(arr), arr.ctypes.data if len(arr) else None))
+        self.collision, self.collision_error = list(capsules), None
+        n = C.c_int32(0)
+        self._check(self._L.mb2_character_num_collision_pairs(self._h, C.byref(n)))
+        self.num_collision_pairs = int(n.value)
+
+    def collision_pairs(self) -> np.ndarray:
+        """The planned pairs of the uploaded geometry: int32 [P, 2], i < j ascending."""
+        n = C.c_int32(0)
+        self._check(self._L.mb2_character_num_collision_pairs(self._h, C.byref(n)))
+        out = np.zeros((int(n.value), 2), np.int32)
+        self._check(self._L.mb2_character_get_collision_pairs(self._h, out.ctypes.data if out.size else None))
+        return out
+
+    def collision_residual_device(self, batch: int, state_device_ptr: int, residual_device_ptr: int, stream: int = 0):
+        """The collision rows [B][P] of skeleton states [B][J][8]; float32 device memory on this character's device, enqueued on
+        ``stream``."""
+        self._check(self._L.mb2_character_collision_residual_device(self._h, int(batch), state_device_ptr, residual_device_ptr, stream))
+
+    def collision_residual_backward_device(self, batch: int, state_device_ptr: int, grad_residual_device_ptr: int, grad_state_device_ptr: int,
+                                           stream: int = 0):
+        """dLoss/d skeleton states [B][J][8] from dLoss/d rows [B][P], overwritten."""
+        self._check(self._L.mb2_character_collision_residual_backward_device(self._h, int(batch), state_device_ptr, grad_residual_device_ptr,
+                                                                           grad_state_device_ptr, stream))
 
     def num_limit_residuals(self) -> int:
         """R, the rows of parameter_limits_residual for the limits this handle was made with (one per limit, none for

@@ -21,7 +21,7 @@ from . import character as mc
 from . import solver as ms
 
 # The registry entry of one (character, device): the character, kept alive so that its id stays unique; the (skinning, faces, blend
-# shape) its DeviceCharacter ``dc`` was made with; and the solver functions ``torch_ik._build`` made on ``dc``.
+# shape, collision) its DeviceCharacter ``dc`` was made with; and the solver functions ``torch_ik._build`` made on ``dc``.
 _Handle = namedtuple("_Handle", "character mesh dc solver_functions")
 _handles = {}
 
@@ -31,12 +31,12 @@ def _device_index(device: torch.device) -> int:
 
 
 def _handle(character: mc.Character, device: torch.device) -> _Handle:
-    """The torch layer's one entry per (character, device). When ``skinning``, its ``faces`` or ``blend_shape`` is replaced, a new entry
+    """The torch layer's one entry per (character, device). When ``skinning``, its ``faces``, ``blend_shape`` or ``collision`` is replaced, a new entry
     with a new DeviceCharacter is made instead of uploading into the old one: a graph recorded before keeps its handle (``ctx.dc``) and
     tables, and no kernel in flight on another stream reads tables being replaced. The old entry's solver functions go with it."""
     index = _device_index(device)
     entry = _handles.get((id(character), index))
-    mesh = (character.skinning, None if character.skinning is None else character.skinning.faces, character.blend_shape)
+    mesh = (character.skinning, None if character.skinning is None else character.skinning.faces, character.blend_shape, character.collision)
     if entry is None or any(a is not b for a, b in zip(entry.mesh, mesh)):
         entry = _handles[id(character), index] = _Handle(character, mesh, ms.DeviceCharacter(character, index), {})
     return entry
@@ -412,6 +412,94 @@ def apply_model_param_limits(character, model_parameters: torch.Tensor) -> torch
 
 parameter_limits_residual.__doc__ += _LIMITS_NOTE
 apply_model_param_limits.__doc__ += _LIMITS_NOTE
+
+
+class _Collision(torch.autograd.Function):
+    """collision_residual on [B, J, 8] float32 states, forward and backward on the device."""
+
+    @staticmethod
+    def forward(ctx, dc, P, skel_state):
+        J = dc.character.num_joints
+        st = _float32(skel_state, -1, J, 8)
+        B = st.shape[0]
+        out = torch.empty(B, P, device=st.device, dtype=torch.float32)
+        if B * P > 0:
+            dc.collision_residual_device(B, st.data_ptr(), out.data_ptr(), _stream(st.device))
+        ctx.dc, ctx.P, ctx.shape, ctx.dtype = dc, P, skel_state.shape, skel_state.dtype
+        ctx.save_for_backward(st)
+        return _restore(out, (*skel_state.shape[:-2], P), skel_state.dtype)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_residual):
+        (st,) = ctx.saved_tensors
+        B = st.shape[0]
+        gs = torch.zeros_like(st)
+        if B * ctx.P > 0:  # else the gradient is zero
+            g = _float32(grad_residual, B, ctx.P)
+            ctx.dc.collision_residual_backward_device(B, st.data_ptr(), g.data_ptr(), gs.data_ptr(), _stream(st.device))
+        return None, None, _restore(gs, ctx.shape, ctx.dtype)
+
+
+def _collision_handle(character, device):
+    """The handle of ``character`` with its collision geometry uploaded, or ValueError."""
+    ch, _ = _resolve(character)
+    if isinstance(character, ms.DeviceCharacter):
+        dc = _device_character(character, device)
+    else:
+        if ch.collision is None:
+            raise ValueError("the character has no collision geometry (character.collision is None)")
+        dc = _device_character(character, device)
+    if dc.collision is None:
+        rejected = dc.collision_error
+        raise ValueError("the character has no collision geometry" + (f" (its upload was rejected: {rejected})" if rejected else ""))
+    return dc
+
+
+def collision_residual(character, skel_state: torch.Tensor) -> torch.Tensor:
+    """Self-collision of the character's tapered capsules, the residual of momentum's ``CollisionErrorFunction`` at weight 1:
+    ``skel_state`` [J, 8] or [B, J, 8] (t, q xyzw, s; q is normalised) on a CUDA device -> [P] or [B, P] in the input dtype, computed
+    in float32. Row k belongs to valid pair k (``collision_pairs``): sqrt(5e-3) times the pair's overlap where the reference's
+    ``overlaps`` reports a contact, 0 otherwise, so that ``residual.square().sum(-1)`` is ``CollisionErrorFunction::getError`` and the
+    nonzero rows, in order, are the compacted residual of its ``getJacobian``. The narrow phase is ``closestPointsOnSegments`` branch for
+    branch in float, its quirks included: two nearly parallel capsules (D < 1e-7) whose origins are farther apart than the sum of their
+    largest radii have no contact even when their sides touch. A world capsule is T_parent o T_local: origin T.t, direction R(T.q) e_x
+    T.s length, radii radius times the parent's scale only. A capsule's local rotation is normalised when the geometry is uploaded; the
+    reference composes a non-unit rotation as it is, so the two differ for one (a zero rotation is rejected).
+
+    The valid pairs are planned when the geometry is uploaded: a pair of world-fixed capsules is dropped, a pair with exactly one is
+    kept, capsules on the same or parent-child joints are dropped, and the rest are kept unless they overlap at the rest pose (model
+    parameters zero), which is evaluated in double where the reference's float build evaluates it in float. An empty geometry gives
+    [B, 0]; ``character.collision`` None raises ValueError.
+
+    Differentiable once with respect to ``skel_state``. The gradient is the exact derivative of these rows, including the motion of
+    the closest-point parameters (s, t) through the closed form of the branch taken; a clamped or snapped parameter is constant. Momentum's
+    ``getJacobian`` holds (s, t) fixed and so drops delta ds/dtheta: it agrees with this gradient for untapered capsules (r0 = r1) and
+    differs for tapered ones. Compose with ``model_parameters_to_skeleton_state`` for a loss in model parameters.
+
+    ``character`` is a ``momentum_b200.character.Character``, whose ``collision`` list is read when the torch layer makes its handle:
+    replacing the attribute makes a new handle, as replacing ``skinning`` does (changing the list in place does not). Or it is a
+    ``solver.DeviceCharacter``, with what was uploaded to it."""
+    if not torch.is_tensor(skel_state) or not skel_state.is_cuda:
+        raise ValueError("collision_residual runs on CUDA tensors (there is no CPU fallback)")
+    ch, _ = _resolve(character)
+    J = ch.num_joints
+    if skel_state.dim() not in (2, 3) or skel_state.shape[-2:] != (J, 8):
+        raise ValueError(f"skel_state must be [J, 8] or [B, J, 8] with J = {J}, got {tuple(skel_state.shape)}")
+    dc = _collision_handle(character, skel_state.device)
+    return _Collision.apply(dc, dc.num_collision_pairs, skel_state)
+
+
+def collision_pairs(character, device=None) -> torch.Tensor:
+    """The valid pairs of ``collision_residual``'s rows: a CPU int64 tensor [P, 2], capsule indices i < j, row k for pair k. ``device``
+    (a CUDA device, default the current one) is where a ``Character``'s handle lives. The pairs are planned on the host, but reading them
+    makes (or reuses) that device handle, so this needs a CUDA device; ``character.collision_pairs`` restates the same rules in float64
+    without one."""
+    if isinstance(character, ms.DeviceCharacter):
+        dc = _collision_handle(character, torch.device("cuda", character.device))
+    else:
+        dc = _collision_handle(character, torch.device("cuda") if device is None else torch.device(device))
+    return torch.from_numpy(dc.collision_pairs().astype(np.int64))
 
 
 class _SkinPoints(torch.autograd.Function):
