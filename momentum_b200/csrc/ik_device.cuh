@@ -997,8 +997,7 @@ MB2_HD void limitGradPasses(const Lanes& g, const CharacterTables& C, const Skel
 // The world capsule (CollisionGeometryStateT::updatePrimitive, collision_geometry_state.cpp:28-48), the narrow phase of overlaps
 // (collision_geometry_state.h:120-157) over closestPointsOnSegments (math/utility.cpp:443-552), branch for branch in the reference's
 // operation order, and the exact derivative of the overlap. A capsule's world geometry is 8 values: origin, direction (its length is the
-// segment's), r0, r1; delta = r1 - r0.
-constexpr int kCapsuleFloats = 8;
+// segment's), r0, r1; delta = r1 - r0 (kCapsuleFloats, ik_types.h).
 MB2_HD void skinStateGradient(const float* acc, const float* state, float* out); // below, with the skinning
 // sqrt(kCollisionWeight) at weight 1 (collision_error_function.h:139, collision_error_function.cpp getJacobian's wgt), in float
 MB2_HD float collisionRowWeight() { return sqrtf(5e-3f); }

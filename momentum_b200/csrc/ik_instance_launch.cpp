@@ -28,21 +28,21 @@ InstanceLaunch planInstanceGroups(size_t perInstance, size_t tableBytes, long ba
 
 InstanceLaunch planInstanceOp(const CharacterTables& C, int numChildren, int op, bool backward, int numPoints, long batch, size_t smemBudget,
                               int numSms, bool limitsFk) {
-  if (op == kInstanceOpInputGradients)
-    return planInstanceGroups(sizeof(float) * inputGradientSmemPerInstanceFloats(C.numJoints, C.numParams), characterTableWords(C) * 4, batch,
-                              smemBudget, numSms);
-  if (op == kInstanceOpParameterLimits)
-    return planInstanceGroups(sizeof(float) * parameterLimitsSmemPerInstanceFloats(C.numJoints, C.numParams, backward, limitsFk),
-                              parameterLimitsTableBytes(C, numChildren, backward, limitsFk), batch, smemBudget, numSms);
-  if (op == kInstanceOpCollision)
-    return planInstanceGroups(sizeof(float) * collisionSmemPerInstanceFloats(numPoints, backward), 0, batch, smemBudget, numSms);
+  const int J = C.numJoints, n = C.numParams;
+  const SkeletonTables S{}; // the lists read only the counts
+  const PointTables P{numPoints};
   const bool joint = op == kInstanceOpJointSkeletonState || op == kInstanceOpJointPositions;
-  const size_t per = sizeof(float) * skeletonStateSmemPerInstanceFloats(C.numJoints, C.numParams, backward, joint);
-  const size_t tables = skeletonStateTableBytes(C, numChildren, backward, joint);
-  if (op != kInstanceOpModelPositions && op != kInstanceOpJointPositions) return planInstanceGroups(per, tables, batch, smemBudget, numSms);
-  const size_t points = pointTableBytes(numPoints, C.numJoints, backward);
-  const bool stage = instanceGroupsFit(per, tables + points, smemBudget) >= instanceGroupsFit(per, tables, smemBudget);
-  InstanceLaunch l = planInstanceGroups(per, tables + (stage ? points : 0), batch, smemBudget, numSms);
+  size_t per = 0; // floats, then bytes per instance
+  TableBytes tables, points;
+  if (op == kInstanceOpInputGradients) { per = inputGradientFrame(J, n).floats; characterTableList(tables, C); }
+  else if (op == kInstanceOpCollision) per = collisionFrame(numPoints, backward).floats;
+  else if (op != kInstanceOpParameterLimits) { per = skeletonStateFrame(J, n, backward, joint).floats; skeletonTableList(tables, C, S, numChildren, backward, backward && !joint); }
+  else { per = parameterLimitsFrame(J, n, backward, limitsFk).floats; skeletonTableList(tables, C, S, numChildren, backward && limitsFk, backward); }
+  per *= sizeof(float);
+  if (op != kInstanceOpModelPositions && op != kInstanceOpJointPositions) return planInstanceGroups(per, tables.bytes, batch, smemBudget, numSms);
+  pointTableList(points, P, J, backward);
+  const bool stage = instanceGroupsFit(per, tables.bytes + points.bytes, smemBudget) >= instanceGroupsFit(per, tables.bytes, smemBudget);
+  InstanceLaunch l = planInstanceGroups(per, tables.bytes + (stage ? points.bytes : 0), batch, smemBudget, numSms);
   if (l.warpsPerInstance != 0) l.stagedPoints = stage;
   return l;
 }

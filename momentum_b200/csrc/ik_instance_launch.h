@@ -1,8 +1,8 @@
-// The launch of the per-instance kernels of the character operations (skeletonStateKernel, positionsKernel, inputGradientKernel,
-// parameterLimitsKernel, collisionKernel): their shared memory per instance and per CTA, and the one rule that picks the warps per instance W and the
-// instance groups per CTA from it.
-// Host code shared by the library (ik_kernels.cu) and the CPU emulator (tests/emu), so that the launch a test sizes a rig for is the
-// launch that runs.
+// The frame of the per-instance kernels of the character operations (skeletonStateKernel, positionsKernel, inputGradientKernel,
+// parameterLimitsKernel, collisionKernel): the regions of an instance's shared memory, the tables each kernel stages, and the one rule
+// that picks the warps per instance W and the instance groups per CTA from them.
+// Shared by the library's kernels and launch planning (ik_kernels.cu, ik_instance_launch.cpp) and the CPU emulator (tests/emu), so that
+// the frame and tables a kernel takes are those its launch was sized for and those the emulated passes run in.
 #pragma once
 
 #include <cstddef>
@@ -14,62 +14,98 @@ namespace mb2 {
 
 constexpr int kSkelMaxWarps = 16; // warps per CTA, and instance groups per CTA (named barriers 1..groups when W > 1)
 
-// words (4 bytes) of a table of `count` elements staged in shared memory: every table starts on a 16-byte boundary
-MB2_HD size_t tableWords(size_t count, size_t elemBytes) { return (count * elemBytes + 15) / 16 * 4; }
-// the character tables, staged first by every kernel that stages tables (stageCharacterTables)
-inline size_t characterTableWords(const CharacterTables& C) {
-  const size_t J = C.numJoints;
-  size_t w = tableWords(J, 4) + tableWords(3 * J, 4) + tableWords(4 * J, 4);                 // parent, offset, prerot
-  w += tableWords(7 * J + 1, 4) + tableWords(C.ptNnz, 4) * 2 + tableWords(7 * J, 4);         // ptOuter, ptInner, ptVals, ptOffsets
-  w += tableWords(C.numLevels + 1, 4) + tableWords(J, 4);                                    // levelStart, levelJoints
-  return w;
+// ---- The regions of one instance group, in floats from the group's base: every region starts on a 16-byte boundary and an empty one
+// takes no space. `floats` is the group's total; the CTA holds groupsPerCta of them, then the staged tables. The kernels size their groups
+// with `floats`, whose sum keeps the grouping they have always compiled with: a regrouped sum moves ptxas's register allocation.
+MB2_HD size_t skelAligned(size_t floats) { return (floats + 3) & ~size_t(3); }
+// skeletonStateKernel and positionsKernel: the input (theta [n], or the joint parameters [7 J]), joint states [J][17]; backward: subtree
+// sums [J][11] and, from theta, the joint-parameter gradient [7 J]
+struct SkeletonStateFrame { size_t in, js, acc, gjp, floats; };
+MB2_HD SkeletonStateFrame skeletonStateFrame(int J, int n, bool backward, bool joint) {
+  const size_t in = skelAligned(joint ? size_t(J) * kParametersPerJoint : size_t(n)), js = skelAligned(size_t(J) * kJointStateStride);
+  const size_t acc = backward ? skelAligned(size_t(J) * kSkelAccStride) : 0, gjp = backward && !joint ? skelAligned(size_t(J) * kParametersPerJoint) : 0;
+  return {0, in, in + js, in + js + acc, in + js + (acc + gjp)};
+}
+// parameterLimitsKernel: theta [n], the joint parameters [7 J], with the FK (an Ellipsoid among the limits) the joint states [J][17];
+// backward: the joint-parameter gradient [7 J] and, with the FK, the subtree sums [J][11]
+struct ParameterLimitsFrame { size_t th, jp, js, gjp, acc, floats; };
+MB2_HD ParameterLimitsFrame parameterLimitsFrame(int J, int n, bool backward, bool fk) {
+  const size_t th = skelAligned(size_t(n)), jp = skelAligned(size_t(J) * kParametersPerJoint), js = fk ? skelAligned(size_t(J) * kJointStateStride) : 0;
+  ParameterLimitsFrame f{0, th, th + jp, th + jp + js, th + jp + js + (backward ? jp : 0), th + jp};
+  if (fk) f.floats += skelAligned(size_t(J) * kJointStateStride);
+  if (backward) f.floats += skelAligned(size_t(J) * kParametersPerJoint) + (fk ? skelAligned(size_t(J) * kSkelAccStride) : 0);
+  return f;
+}
+// collisionKernel: the world capsules [C][8]; backward: their gradients [C][8]. The skeleton states are read from global memory where a
+// capsule needs its parent's.
+struct CollisionFrame { size_t geo, cg, floats; };
+MB2_HD CollisionFrame collisionFrame(int numCapsules, bool backward) {
+  const size_t geo = skelAligned(size_t(numCapsules) * kCapsuleFloats);
+  return {0, geo, geo * (backward ? 2 : 1)};
+}
+// inputGradientKernel: theta [n], v [n], joint states [J][17], joint motions [J][7]
+struct InputGradientFrame { size_t th, vs, js, tan, floats; };
+MB2_HD InputGradientFrame inputGradientFrame(int J, int n) {
+  const size_t th = skelAligned(size_t(n)), js = skelAligned(size_t(J) * kJointStateStride), tan = skelAligned(size_t(J) * kTangentStride);
+  return {0, th, 2 * th, 2 * th + js, 2 * th + js + tan};
 }
 
-MB2_HD size_t skelAligned(size_t floats) { return (floats + 3) & ~size_t(3); } // 16-byte aligned regions
-// skeletonStateKernel and positionsKernel, per instance: the input (theta [n], or the joint parameters [7 J]), joint states [J][17],
-// backward: subtree sums [J][11] and, from theta, the joint-parameter gradient [7 J]
-MB2_HD size_t skeletonStateSmemPerInstanceFloats(int J, int n, bool backward, bool joint) {
-  size_t f = skelAligned(joint ? size_t(J) * kParametersPerJoint : size_t(n)) + skelAligned(size_t(J) * kJointStateStride);
-  if (backward) f += skelAligned(size_t(J) * kSkelAccStride) + (joint ? 0 : skelAligned(size_t(J) * kParametersPerJoint));
-  return f;
+// ---- The tables a kernel stages in shared memory once per CTA, as lists walked by a visitor v(table, count): on the device
+// TableStager copies each table and points it at the copy, on the host TableBytes adds up the bytes the copies take. Every table
+// starts on a 16-byte boundary.
+MB2_HD size_t tableWords(size_t count, size_t elemBytes) { return (count * elemBytes + 15) / 16 * 4; }
+struct TableBytes {
+  size_t bytes = 0;
+  template <class E> MB2_HD void operator()(const E*, size_t count) { bytes += 4 * tableWords(count, sizeof(E)); }
+};
+#if defined(__CUDACC__)
+// The CTA's threads copy each table to `cursor` word by word and move the table's pointer there; the caller syncs the CTA before the
+// copies are read.
+struct TableStager {
+  uint32_t* cursor;
+  template <class E> __device__ __forceinline__ void operator()(const E*& table, size_t count) {
+    static_assert(sizeof(E) % 4 == 0, "tables are staged word by word");
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(table);
+    const size_t words = count * (sizeof(E) / 4);
+    // eight loads in flight per thread (a word-by-word loop is a chain of global-load latencies: 23 of them for the 40 KB of cfg3)
+    const int nt = int(blockDim.x);
+    size_t i = threadIdx.x;
+    for (; i + 7 * size_t(nt) < words; i += 8 * size_t(nt)) {
+      uint32_t v[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) v[k] = src[i + size_t(k) * nt];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) cursor[i + size_t(k) * nt] = v[k];
+    }
+    for (; i < words; i += nt) cursor[i] = src[i];
+    table = reinterpret_cast<const E*>(cursor);
+    cursor += tableWords(count, sizeof(E));
+  }
+};
+#endif
+
+// The character's tables, first in every kernel that stages tables (C: CharacterTables or FunctionTables)
+template <class V, class C>
+MB2_HD void characterTableList(V& v, C& T) {
+  const size_t J = T.numJoints;
+  v(T.parent, J); v(T.offset, 3 * J); v(T.prerot, 4 * J);
+  v(T.ptOuter, 7 * J + 1); v(T.ptInner, T.ptNnz); v(T.ptVals, T.ptNnz); v(T.ptOffsets, 7 * J);
+  v(T.levelStart, T.numLevels + 1); v(T.levelJoints, J);
 }
-// their tables: the character's; backward: the children in CSR and, from theta, the ParameterTransform in CSC
-inline size_t skeletonStateTableBytes(const CharacterTables& C, int numChildren, bool backward, bool joint) {
-  size_t w = characterTableWords(C);
-  if (backward) w += tableWords(size_t(C.numJoints) + 1, 4) + tableWords(size_t(numChildren), 4);
-  if (backward && !joint) w += tableWords(size_t(C.numParams) + 1, 4) + tableWords(size_t(C.ptNnz), 4) * 2;
-  return w * 4;
+// skeletonStateKernel, positionsKernel and parameterLimitsKernel: the character's; then for a backward the children in CSR where it
+// folds subtree sums (`children`), and the ParameterTransform in CSC where it ends in model parameters (`csc`)
+template <class V, class C, class S>
+MB2_HD void skeletonTableList(V& v, C& T, S& Sk, int numChildren, bool children, bool csc) {
+  const int J = T.numJoints, n = T.numParams;
+  characterTableList(v, T);
+  if (children) { v(Sk.childStart, size_t(J) + 1); v(Sk.children, numChildren); }
+  if (csc) { v(Sk.ptColStart, n + 1); v(Sk.ptColRows, T.ptNnz); v(Sk.ptColVals, T.ptNnz); }
 }
-// positionsKernel's point tables: each point's joint; backward: the points by joint
-inline size_t pointTableBytes(int numPoints, int J, bool backward) {
-  size_t w = tableWords(size_t(numPoints), 4);
-  if (backward) w += tableWords(size_t(J) + 1, 4) + tableWords(size_t(numPoints), 4);
-  return w * 4;
-}
-// parameterLimitsKernel, per instance: theta [n], the joint parameters [7 J], with the FK (an Ellipsoid among the limits) the joint
-// states [J][17]; backward: the joint-parameter gradient [7 J] and, with the FK, the subtree sums [J][11]
-MB2_HD size_t parameterLimitsSmemPerInstanceFloats(int J, int n, bool backward, bool fk) {
-  size_t f = skelAligned(size_t(n)) + skelAligned(size_t(J) * kParametersPerJoint);
-  if (fk) f += skelAligned(size_t(J) * kJointStateStride);
-  if (backward) f += skelAligned(size_t(J) * kParametersPerJoint) + (fk ? skelAligned(size_t(J) * kSkelAccStride) : 0);
-  return f;
-}
-// its tables: the character's; backward: with the FK the children in CSR, and the ParameterTransform in CSC. The limit tables are read
-// from global memory.
-inline size_t parameterLimitsTableBytes(const CharacterTables& C, int numChildren, bool backward, bool fk) {
-  size_t w = characterTableWords(C);
-  if (backward && fk) w += tableWords(size_t(C.numJoints) + 1, 4) + tableWords(size_t(numChildren), 4);
-  if (backward) w += tableWords(size_t(C.numParams) + 1, 4) + tableWords(size_t(C.ptNnz), 4) * 2;
-  return w * 4;
-}
-// collisionKernel, per instance: the world capsules [C][8]; backward: their gradients [C][8]. The skeleton states are read from global
-// memory where a capsule needs its parent's, and the collision tables are read from global memory: no staged tables.
-MB2_HD size_t collisionSmemPerInstanceFloats(int numCapsules, bool backward) {
-  return skelAligned(size_t(numCapsules) * 8) * (backward ? 2 : 1);
-}
-// inputGradientKernel, per instance: theta [n], v [n], joint states [J][17], joint motions [J][7]; its tables are the character's
-MB2_HD size_t inputGradientSmemPerInstanceFloats(int J, int n) {
-  return 2 * skelAligned(size_t(n)) + skelAligned(size_t(J) * kJointStateStride) + skelAligned(size_t(J) * kTangentStride);
+// positionsKernel's point tables, after skeletonTableList's when staged: each point's joint; backward: the points by joint
+template <class V, class P>
+MB2_HD void pointTableList(V& v, P& Pt, int J, bool backward) {
+  v(Pt.parent, Pt.numPoints);
+  if (backward) { v(Pt.pointStart, size_t(J) + 1); v(Pt.pointIndex, Pt.numPoints); }
 }
 
 // What a per-instance kernel runs with; all zero when one instance does not fit next to the tables.

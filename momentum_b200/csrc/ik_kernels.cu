@@ -42,45 +42,22 @@ size_t sweepSmemPerInstance(const FunctionTables& T, int warpsPerInstance) {
 }
 
 // The read-only tables (character + plan) are walked by dependent loads (cell -> unit -> contributions -> joint);
-// from L2 each hop costs several hundred cycles, so a persistent CTA copies them into shared memory once.
-// (tableWords, characterTableWords: ik_instance_launch.h)
+// from L2 each hop costs several hundred cycles, so a persistent CTA copies them into shared memory once (the lists and their visitors:
+// ik_instance_launch.h).
 // mode 1: every table; mode 2: everything except the two big ones, cells and contributions (large rigs: those are streamed through
 // L1 / L2, one sequential record per lane and iteration, while the tables walked by dependent loads - character, units, error functions -
 // still sit in shared memory)
+template <class V, class F>
+MB2_HD void sweepTableList(V& v, F& T, int mode) {
+  characterTableList(v, T);
+  v(T.efs, T.numEf); v(T.units, T.numUnits); v(T.limitData, T.numLimitData);
+  if (mode == 1) { v(T.cells, T.numCells); v(T.contribs, T.numContribs); }
+}
 size_t sweepTableBytes(const FunctionTables& T, int mode) {
   if (mode == 0) return 0;
-  size_t w = characterTableWords(T);
-  w += tableWords(T.numEf, sizeof(EfDesc)) + tableWords(T.numUnits, sizeof(UnitDesc)) + tableWords(T.numLimitData, 4);
-  if (mode == 1) w += tableWords(T.numCells, sizeof(CellDesc)) + tableWords(T.numContribs, sizeof(ContribDesc));
-  return w * 4;
-}
-
-template <class E>
-__device__ __forceinline__ void stageTable(const E*& table, size_t count, uint32_t*& cursor) {
-  static_assert(sizeof(E) % 4 == 0, "tables are staged word by word");
-  const uint32_t* src = reinterpret_cast<const uint32_t*>(table);
-  const size_t words = count * (sizeof(E) / 4);
-  // eight loads in flight per thread (a word-by-word loop is a chain of global-load latencies: 23 of them for the 40 KB of cfg3)
-  const int nt = int(blockDim.x);
-  size_t i = threadIdx.x;
-  for (; i + 7 * size_t(nt) < words; i += 8 * size_t(nt)) {
-    uint32_t v[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) v[k] = src[i + size_t(k) * nt];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) cursor[i + size_t(k) * nt] = v[k];
-  }
-  for (; i < words; i += nt) cursor[i] = src[i];
-  table = reinterpret_cast<const E*>(cursor);
-  cursor += tableWords(count, sizeof(E));
-}
-// C's pointers move to the copies at cursor (characterTableWords(C) words); the caller syncs the CTA before they are read
-__device__ __forceinline__ void stageCharacterTables(CharacterTables& C, uint32_t*& cursor) {
-  const size_t J = C.numJoints;
-  stageTable(C.parent, J, cursor); stageTable(C.offset, 3 * J, cursor); stageTable(C.prerot, 4 * J, cursor);
-  stageTable(C.ptOuter, 7 * J + 1, cursor); stageTable(C.ptInner, C.ptNnz, cursor); stageTable(C.ptVals, C.ptNnz, cursor);
-  stageTable(C.ptOffsets, 7 * J, cursor);
-  stageTable(C.levelStart, C.numLevels + 1, cursor); stageTable(C.levelJoints, J, cursor);
+  TableBytes tables;
+  sweepTableList(tables, T, mode);
+  return tables.bytes;
 }
 
 // kStage (1 all tables, 2 all but cells / contributions, 0 none): the tables live in shared memory for the whole kernel. A template parameter rather than a run-time branch so that every
@@ -105,10 +82,8 @@ __global__ void __launch_bounds__(32 * kSweepMaxWarps) sweepKernel(const SweepAr
   float* rec = js + ((T.numJoints * kJointStateStride + 1) & ~1);
   double* errSlots = reinterpret_cast<double*>(rec + ((T.recStride + 1) & ~1)); // W partial sums (8-byte aligned: every preceding size is even)
   if constexpr (kStage != 0) {
-    uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + ((size_t(groupsPerCta) * perGroup + 3) & ~size_t(3)));
-    stageCharacterTables(T, cursor);
-    stageTable(T.efs, T.numEf, cursor); stageTable(T.units, T.numUnits, cursor); stageTable(T.limitData, T.numLimitData, cursor);
-    if constexpr (kStage == 1) { stageTable(T.cells, T.numCells, cursor); stageTable(T.contribs, T.numContribs, cursor); }
+    TableStager stager{reinterpret_cast<uint32_t*>(smem + ((size_t(groupsPerCta) * perGroup + 3) & ~size_t(3)))};
+    sweepTableList(stager, T, kStage);
     __syncthreads();
   }
 
@@ -229,16 +204,17 @@ cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream,
 
 // ------------------------------------------------------------------------------------------------
 // Skeleton state of a batch of model parameters, and its backward (ik_device.cuh skelGrad*).
-// The per-instance frame, shared with inputGradientKernel: a persistent grid sized by launchInstanceGroups, one group of W warps per
-// instance (WarpLanes<W>), the character tables staged in shared memory once per CTA (stageCharacterTables, kernel-specific tables after
-// them), then per instance the pass functions of ik_device.cuh, which the CPU emulators run too.
+// The per-instance frame, shared with the positions, limits, collision and input-gradient kernels: a persistent grid sized by
+// launchInstanceGroups, one group of W warps per instance (WarpLanes<W>) with skeletonStateFrame's floats of shared memory, the kernel's
+// table list staged once per CTA after the groups (TableStager), then per instance the pass functions of ik_device.cuh, which the CPU
+// emulators run too.
 //   forward:   fkPasses from theta, [J][8] out
 //   backward:  fkPasses with the DOF axes, then skelGradPasses: lanes = joints seed their 11 subtree sums from G, levels from the
 //              deepest up fold in their children, lanes = joint-parameter rows, lanes = model parameters over the CSC ParameterTransform.
 // kJoint (joint_parameters_to_skeleton_state): the input is the joint parameters [7 J], staged where theta is staged otherwise; the
 // backward writes the joint-parameter gradient straight out and stops before the ParameterTransform.
 // Every output element is written by one lane in a fixed order: no atomics, the result does not depend on the launch shape.
-// Shared memory per instance and per CTA, and the choice of W: ik_instance_launch.h.
+// The frame's size, the staged tables and the choice of W: ik_instance_launch.h.
 // ------------------------------------------------------------------------------------------------
 
 template <bool kBackward, int W, bool kJoint>
@@ -252,18 +228,14 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps) skeletonStateKernel(const 
   const int inN = kJoint ? J * kParametersPerJoint : n; // floats per instance of the input
   const int thF = int(skelAligned(inN)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
   const int accF = kBackward ? int(skelAligned(size_t(J) * kSkelAccStride)) : 0;
-  const int perGroup = int(skeletonStateSmemPerInstanceFloats(J, n, kBackward, kJoint));
+  const int perGroup = int(skeletonStateFrame(J, n, kBackward, kJoint).floats);
   float* th = smem + size_t(g.group) * perGroup;
   float* js = th + thF;
   float* acc = js + jsF;
   float* gjp = acc + accF;
   {
-    uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
-    stageCharacterTables(T, cursor);
-    if constexpr (kBackward) {
-      stageTable(S.childStart, size_t(J) + 1, cursor); stageTable(S.children, a.numChildren, cursor);
-      if constexpr (!kJoint) { stageTable(S.ptColStart, n + 1, cursor); stageTable(S.ptColRows, T.ptNnz, cursor); stageTable(S.ptColVals, T.ptNnz, cursor); }
-    }
+    TableStager stager{reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup)};
+    skeletonTableList(stager, T, S, a.numChildren, kBackward, kBackward && !kJoint);
     __syncthreads();
   }
   for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
@@ -297,39 +269,41 @@ cudaError_t persistentGrid(K kernel, int threads, size_t smem, long work, int* g
   return cudaSuccess;
 }
 
-// A persistent kernel with one group of W warps per instance and the tables staged once per CTA (skeletonStateKernel, positionsKernel,
-// inputGradientKernel), launched as planInstanceOp planned it (ik_instance_launch.cpp). kernels[0..3]: the instantiations for W = 1, 2,
-// 4, 8. With `query`, the launch is reported there and nothing is enqueued.
-template <class Args>
-cudaError_t launchInstanceGroups(void (*const kernels[4])(Args), const Args& a, int numChildren, int op, bool backward, int numPoints, cudaStream_t stream,
-                                 InstanceLaunchQuery* query, bool limitsFk = false) {
+// f(std::true_type) or f(std::false_type): a run-time flag as a template argument
+template <class F>
+auto withFlag(bool flag, F&& f) { return flag ? f(std::true_type{}) : f(std::false_type{}); }
+
+// A kernel in the per-instance frame, launched as planInstanceOp plans it (ik_instance_launch.cpp): kernelFor(W, plan) is its
+// instantiation for the planned W (std::integral_constant<int, W>) and the plan's other choices. With `query`, the launch is reported
+// there and nothing is enqueued.
+template <class Args, class KernelFor>
+cudaError_t launchInstanceGroups(const Args& a, int numChildren, int op, bool backward, int numPoints, cudaStream_t stream, InstanceLaunchQuery* query,
+                                 bool limitsFk, KernelFor&& kernelFor) {
   if (query) *query = InstanceLaunchQuery{};
   if (a.batch <= 0) return cudaSuccess;
   const InstanceLaunch l = planInstanceOp(a.T, numChildren, op, backward, numPoints, a.batch, size_t(g_maxSmemOptin), g_numSms, limitsFk);
   if (l.warpsPerInstance == 0) return cudaErrorInvalidConfiguration; // not even one instance fits next to the tables
-  const int w = l.warpsPerInstance == 1 ? 0 : l.warpsPerInstance == 2 ? 1 : l.warpsPerInstance == 4 ? 2 : 3;
+  const int W = l.warpsPerInstance;
+  void (*const kernel)(Args) = W == 1 ? kernelFor(std::integral_constant<int, 1>{}, l) : W == 2 ? kernelFor(std::integral_constant<int, 2>{}, l)
+                             : W == 4 ? kernelFor(std::integral_constant<int, 4>{}, l) : kernelFor(std::integral_constant<int, 8>{}, l);
   int grid = 0;
-  const cudaError_t e = persistentGrid(kernels[w], l.threads, size_t(l.smemBytes), (long(a.batch) + l.groupsPerCta - 1) / l.groupsPerCta, &grid);
+  const cudaError_t e = persistentGrid(kernel, l.threads, size_t(l.smemBytes), (long(a.batch) + l.groupsPerCta - 1) / l.groupsPerCta, &grid);
   if (e != cudaSuccess) return e;
   if (query) {
     *query = InstanceLaunchQuery{l, grid};
     return cudaSuccess;
   }
-  kernels[w]<<<grid, l.threads, size_t(l.smemBytes), stream>>>(a);
+  kernel<<<grid, l.threads, size_t(l.smemBytes), stream>>>(a);
   return cudaGetLastError();
 }
 } // namespace
 
 cudaError_t launchSkeletonState(const SkeletonStateArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query) {
-  using K = void (*)(SkeletonStateArgs);
-  static const K kernels[2][2][4] = {
-      {{skeletonStateKernel<false, 1, false>, skeletonStateKernel<false, 2, false>, skeletonStateKernel<false, 4, false>, skeletonStateKernel<false, 8, false>},
-       {skeletonStateKernel<true, 1, false>, skeletonStateKernel<true, 2, false>, skeletonStateKernel<true, 4, false>, skeletonStateKernel<true, 8, false>}},
-      {{skeletonStateKernel<false, 1, true>, skeletonStateKernel<false, 2, true>, skeletonStateKernel<false, 4, true>, skeletonStateKernel<false, 8, true>},
-       {skeletonStateKernel<true, 1, true>, skeletonStateKernel<true, 2, true>, skeletonStateKernel<true, 4, true>, skeletonStateKernel<true, 8, true>}}};
   const bool joint = a.fromJointParameters != 0;
-  return launchInstanceGroups(kernels[joint][backward], a, a.numChildren, joint ? kInstanceOpJointSkeletonState : kInstanceOpModelSkeletonState, backward, 0, stream,
-                              query);
+  const int op = joint ? kInstanceOpJointSkeletonState : kInstanceOpModelSkeletonState;
+  return launchInstanceGroups(a, a.numChildren, op, backward, 0, stream, query, false, [&](auto W, const InstanceLaunch&) {
+    return withFlag(backward, [&](auto kB) { return withFlag(joint, [&](auto kJ) { return skeletonStateKernel<kB, W, kJ>; }); });
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -627,22 +601,21 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) positionsKernel(const P
   const int inN = kJoint ? J * kParametersPerJoint : n; // floats per instance of the input
   const int thF = int(skelAligned(inN)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
   const int accF = kBackward ? int(skelAligned(size_t(J) * kSkelAccStride)) : 0;
-  const int perGroup = int(skeletonStateSmemPerInstanceFloats(J, n, kBackward, kJoint));
+  const int perGroup = int(skeletonStateFrame(J, n, kBackward, kJoint).floats);
   float* th = smem + size_t(g.group) * perGroup;
   float* js = th + thF;
   float* acc = js + jsF;
   float* gjp = acc + accF;
   {
-    uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
-    stageCharacterTables(T, cursor);
+    TableStager stager{reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup)};
+    // skeletonTableList(stager, T, S, a.numChildren, kBackward, kBackward && !kJoint) spelled out: through the list ptxas allocates
+    // positionsKernel<true, 2, false, false> two more registers
+    characterTableList(stager, T);
     if constexpr (kBackward) {
-      stageTable(S.childStart, size_t(J) + 1, cursor); stageTable(S.children, a.numChildren, cursor);
-      if constexpr (!kJoint) { stageTable(S.ptColStart, n + 1, cursor); stageTable(S.ptColRows, T.ptNnz, cursor); stageTable(S.ptColVals, T.ptNnz, cursor); }
+      stager(S.childStart, size_t(J) + 1); stager(S.children, a.numChildren);
+      if constexpr (!kJoint) { stager(S.ptColStart, n + 1); stager(S.ptColRows, T.ptNnz); stager(S.ptColVals, T.ptNnz); }
     }
-    if constexpr (kStagePoints) {
-      stageTable(P.parent, N, cursor);
-      if constexpr (kBackward) { stageTable(P.pointStart, size_t(J) + 1, cursor); stageTable(P.pointIndex, N, cursor); }
-    }
+    if constexpr (kStagePoints) pointTableList(stager, P, J, kBackward);
     __syncthreads();
   }
   for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
@@ -664,20 +637,15 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) positionsKernel(const P
 }
 
 namespace {
-// kernels[joint][backward][kStagePoints]; planInstanceOp decides the staging
+// planInstanceOp decides the staging of the point tables
 cudaError_t launchPositionsKernel(const PositionArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query = nullptr) {
-  using K = void (*)(PositionArgs);
-#define MB2_POSITION_KERNELS(B, J, S) {positionsKernel<B, 1, J, S>, positionsKernel<B, 2, J, S>, positionsKernel<B, 4, J, S>, positionsKernel<B, 8, J, S>}
-  static const K kernels[2][2][2][4] = {
-      {{MB2_POSITION_KERNELS(false, false, false), MB2_POSITION_KERNELS(false, false, true)},
-       {MB2_POSITION_KERNELS(true, false, false), MB2_POSITION_KERNELS(true, false, true)}},
-      {{MB2_POSITION_KERNELS(false, true, false), MB2_POSITION_KERNELS(false, true, true)},
-       {MB2_POSITION_KERNELS(true, true, false), MB2_POSITION_KERNELS(true, true, true)}}};
-#undef MB2_POSITION_KERNELS
   const bool joint = a.fromJointParameters != 0;
   const int op = joint ? kInstanceOpJointPositions : kInstanceOpModelPositions;
-  const bool stage = planInstanceOp(a.T, a.numChildren, op, backward, a.P.numPoints, a.batch, size_t(g_maxSmemOptin), g_numSms).stagedPoints != 0;
-  return launchInstanceGroups(kernels[joint][backward][stage], a, a.numChildren, op, backward, a.P.numPoints, stream, query);
+  return launchInstanceGroups(a, a.numChildren, op, backward, a.P.numPoints, stream, query, false, [&](auto W, const InstanceLaunch& l) {
+    return withFlag(backward, [&](auto kB) {
+      return withFlag(joint, [&](auto kJ) { return withFlag(l.stagedPoints != 0, [&](auto kS) { return positionsKernel<kB, W, kJ, kS>; }); });
+    });
+  });
 }
 } // namespace
 
@@ -746,19 +714,15 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) parameterLimitsKernel(c
   const WarpLanes<W> g = WarpLanes<W>::of(threadIdx.x >> 5, threadIdx.x & 31);
   const int groupsPerCta = (blockDim.x >> 5) / W;
   const int J = T.numJoints, n = T.numParams, R = L.numRows;
-  const int perGroup = int(parameterLimitsSmemPerInstanceFloats(J, n, kBackward, kEllipsoid));
+  const int perGroup = int(parameterLimitsFrame(J, n, kBackward, kEllipsoid).floats);
   float* th = smem + size_t(g.group) * perGroup;
   float* jp = th + skelAligned(size_t(n));
   float* js = jp + skelAligned(size_t(J) * kParametersPerJoint);
   float* gjp = js + (kEllipsoid ? skelAligned(size_t(J) * kJointStateStride) : 0);
   float* acc = gjp + (kBackward ? skelAligned(size_t(J) * kParametersPerJoint) : 0);
   {
-    uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
-    stageCharacterTables(T, cursor);
-    if constexpr (kBackward) {
-      if constexpr (kEllipsoid) { stageTable(S.childStart, size_t(J) + 1, cursor); stageTable(S.children, a.numChildren, cursor); }
-      stageTable(S.ptColStart, n + 1, cursor); stageTable(S.ptColRows, T.ptNnz, cursor); stageTable(S.ptColVals, T.ptNnz, cursor);
-    }
+    TableStager stager{reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup)};
+    skeletonTableList(stager, T, S, a.numChildren, kBackward && kEllipsoid, kBackward);
     __syncthreads();
   }
   for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
@@ -772,11 +736,6 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) parameterLimitsKernel(c
 }
 
 cudaError_t launchParameterLimits(const ParameterLimitArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query) {
-  using K = void (*)(ParameterLimitArgs);
-#define MB2_LIMIT_KERNELS(B, E) {parameterLimitsKernel<B, 1, E>, parameterLimitsKernel<B, 2, E>, parameterLimitsKernel<B, 4, E>, parameterLimitsKernel<B, 8, E>}
-  static const K kernels[2][2][4] = {{MB2_LIMIT_KERNELS(false, false), MB2_LIMIT_KERNELS(false, true)},
-                                     {MB2_LIMIT_KERNELS(true, false), MB2_LIMIT_KERNELS(true, true)}};
-#undef MB2_LIMIT_KERNELS
   if (query) *query = InstanceLaunchQuery{};
   if (a.batch <= 0) return cudaSuccess;
   if (a.L.numRows == 0) { // no live limit: nothing to write, and the gradient is zero
@@ -784,7 +743,9 @@ cudaError_t launchParameterLimits(const ParameterLimitArgs& a, bool backward, cu
     return backward ? cudaMemsetAsync(a.gradTheta, 0, size_t(a.batch) * a.T.numParams * sizeof(float), stream) : cudaSuccess;
   }
   const bool fk = a.L.ellipsoid != 0;
-  return launchInstanceGroups(kernels[backward][fk], a, a.numChildren, kInstanceOpParameterLimits, backward, 0, stream, query, fk);
+  return launchInstanceGroups(a, a.numChildren, kInstanceOpParameterLimits, backward, 0, stream, query, fk, [&](auto W, const InstanceLaunch&) {
+    return withFlag(backward, [&](auto kB) { return withFlag(fk, [&](auto kE) { return parameterLimitsKernel<kB, W, kE>; }); });
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -803,7 +764,7 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) collisionKernel(const C
   const WarpLanes<W> g = WarpLanes<W>::of(threadIdx.x >> 5, threadIdx.x & 31);
   const int groupsPerCta = (blockDim.x >> 5) / W;
   const int J = a.T.numJoints, P = L.numPairs;
-  const int perGroup = int(collisionSmemPerInstanceFloats(L.numCapsules, kBackward));
+  const int perGroup = int(collisionFrame(L.numCapsules, kBackward).floats);
   float* geo = smem + size_t(g.group) * perGroup;
   float* cg = geo + skelAligned(size_t(L.numCapsules) * kCapsuleFloats);
   for (int b = blockIdx.x * groupsPerCta + g.group; b < a.batch; b += gridDim.x * groupsPerCta) {
@@ -815,16 +776,15 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps, 1) collisionKernel(const C
 }
 
 cudaError_t launchCollision(const CollisionArgs& a, bool backward, cudaStream_t stream, InstanceLaunchQuery* query) {
-  using K = void (*)(CollisionArgs);
-  static const K kernels[2][4] = {{collisionKernel<false, 1>, collisionKernel<false, 2>, collisionKernel<false, 4>, collisionKernel<false, 8>},
-                                  {collisionKernel<true, 1>, collisionKernel<true, 2>, collisionKernel<true, 4>, collisionKernel<true, 8>}};
   if (query) *query = InstanceLaunchQuery{};
   if (a.batch <= 0) return cudaSuccess;
   if (a.L.numPairs == 0) { // no pair: nothing to write, and the gradient is zero
     if (query) return cudaSuccess;
     return backward ? cudaMemsetAsync(a.gradState, 0, size_t(a.batch) * a.T.numJoints * 8 * sizeof(float), stream) : cudaSuccess;
   }
-  return launchInstanceGroups(kernels[backward], a, 0, kInstanceOpCollision, backward, a.L.numCapsules, stream, query);
+  return launchInstanceGroups(a, 0, kInstanceOpCollision, backward, a.L.numCapsules, stream, query, false, [&](auto W, const InstanceLaunch&) {
+    return withFlag(backward, [&](auto kB) { return collisionKernel<kB, W>; });
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1711,7 +1671,6 @@ cudaError_t launchClosestPointsOnCloud(const ClosestCloudArgs& a, cudaStream_t s
 //   then level by level the parent's motion added;  lanes = constraints of the block.
 // Every output element is written by one lane: no atomics, the result does not depend on the launch shape.
 // ------------------------------------------------------------------------------------------------
-// (shared memory per instance: inputGradientSmemPerInstanceFloats, ik_instance_launch.h)
 template <int W>
 __global__ void __launch_bounds__(32 * kSkelMaxWarps) inputGradientKernel(const InputGradientArgs a) {
   extern __shared__ __align__(16) float smem[];
@@ -1720,14 +1679,14 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps) inputGradientKernel(const 
   const int groupsPerCta = (blockDim.x >> 5) / W;
   const int J = T.numJoints, n = T.numParams, nc = a.numConstraints;
   const int thF = int(skelAligned(n)), jsF = int(skelAligned(size_t(J) * kJointStateStride));
-  const int perGroup = int(inputGradientSmemPerInstanceFloats(J, n));
+  const int perGroup = int(inputGradientFrame(J, n).floats);
   float* th = smem + size_t(g.group) * perGroup;
   float* vs = th + thF;
   float* js = vs + thF;
   float* tan = js + jsF;
   {
-    uint32_t* cursor = reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup);
-    stageCharacterTables(T, cursor);
+    TableStager stager{reinterpret_cast<uint32_t*>(smem + size_t(groupsPerCta) * perGroup)};
+    characterTableList(stager, T);
     __syncthreads();
   }
   const EfDesc e = T.efs[T.units[a.unitBegin].ef];
@@ -1758,8 +1717,8 @@ __global__ void __launch_bounds__(32 * kSkelMaxWarps) inputGradientKernel(const 
 }
 
 cudaError_t launchInputGradients(const InputGradientArgs& a, cudaStream_t stream, InstanceLaunchQuery* query) {
-  static void (*const kernels[4])(InputGradientArgs) = {inputGradientKernel<1>, inputGradientKernel<2>, inputGradientKernel<4>, inputGradientKernel<8>};
-  return launchInstanceGroups(kernels, a, 0, kInstanceOpInputGradients, false, 0, stream, query);
+  return launchInstanceGroups(a, 0, kInstanceOpInputGradients, false, 0, stream, query, false,
+                              [](auto W, const InstanceLaunch&) { return inputGradientKernel<W>; });
 }
 
 // ------------------------------------------------------------------------------------------------

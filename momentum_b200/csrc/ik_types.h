@@ -215,6 +215,7 @@ struct CapsuleDesc {
   float dir[3];    // R(rotation) e_x scale length
   float r0, r1;    // radius
 };
+constexpr int kCapsuleFloats = 8; // a world capsule (ik_device.cuh): origin, direction, r0, r1
 
 // The character's collision geometry as collision_residual reads it (makeCollision), shared by the batch: the capsules, the valid pairs
 // (updateCollisionPairs, ascending), each capsule's pairs (CSR, pair indices ascending) and each joint's capsules (CSR, ascending).

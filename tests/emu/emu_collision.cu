@@ -4,13 +4,12 @@
 // of ik_device.cuh (collisionPasses, collisionGradPasses) then run with HostLanes, the lanes of each pass in sequence. The launch is
 // planned by the library's planInstanceOp. It is not part of the product library and nothing in momentum_b200/ loads it.
 #include <cstdint>
-#include <vector>
 
 #include "../../include/momentum_b200.h"
 #include "../../momentum_b200/csrc/ik_device.cuh"
-#include "../../momentum_b200/csrc/ik_instance_launch.h"
 #include "../../momentum_b200/csrc/ik_plan.h"
 #include "emu_error.h"
+#include "emu_frame.h"
 
 using namespace mb2;
 
@@ -50,18 +49,19 @@ extern "C" int emu_collision_pairs(MB2_EMU_CHARACTER, int32_t* numPairs, int32_t
 extern "C" int emu_collision(MB2_EMU_CHARACTER, int32_t backward, int32_t batch, const float* state, const float* grad, float* out) {
   Emulated e;
   if (MB2_EMU_SETUP(e) != MB2_OK) return MB2_ERR_INVALID_ARGUMENT;
-  const int J = e.h.numJoints, P = e.c.numPairs(), C = int(e.c.capsules.size());
-  std::vector<float> geo(size_t(C) * kCapsuleFloats + 1), cg(geo.size());
+  const int J = e.h.numJoints, P = e.c.numPairs();
+  const auto f = collisionFrame(int(e.c.capsules.size()), backward != 0);
+  EmuFrame fr{f.floats};
   for (int b = 0; b < batch; ++b) {
     const float* st = state + size_t(b) * J * 8;
     if (P == 0) { // the library's launcher: nothing to write, a zero gradient
       if (backward) for (int i = 0; i < J * 8; ++i) out[size_t(b) * J * 8 + i] = 0.f;
       continue;
     }
-    if (!backward) collisionPasses(HostLanes{}, e.L, st, geo.data(), out + size_t(b) * P);
-    else collisionGradPasses(HostLanes{}, e.L, J, st, geo.data(), cg.data(), grad + size_t(b) * P, out + size_t(b) * J * 8);
+    if (!backward) collisionPasses(HostLanes{}, e.L, st, fr.at(f.geo), out + size_t(b) * P);
+    else collisionGradPasses(HostLanes{}, e.L, J, st, fr.at(f.geo), fr.at(f.cg), grad + size_t(b) * P, out + size_t(b) * J * 8);
   }
-  return MB2_OK;
+  return fr.check("collisionKernel");
 }
 
 // One pair of world capsules A, B [8] (origin, direction, r0, r1) through capsuleContact<float>: out = [hit, s, t, dist, overlap, sForm,
@@ -81,10 +81,6 @@ extern "C" int emu_collision_launch(MB2_EMU_CHARACTER, int32_t backward, int64_t
   if (MB2_EMU_SETUP(e) != MB2_OK) return MB2_ERR_INVALID_ARGUMENT;
   const InstanceLaunch l = planInstanceOp(hostCharacterTables(e.h), int(e.h.children.size()), kInstanceOpCollision, backward != 0,
                                           int(e.c.capsules.size()), long(batch), size_t(smemBudget), numSms);
-  out[0] = l.warpsPerInstance;
-  out[1] = l.groupsPerCta;
-  out[2] = l.threads;
-  out[3] = l.smemBytes;
-  out[4] = l.stagedPoints;
+  launchWords(l, out);
   return MB2_OK;
 }

@@ -12,6 +12,7 @@
 #include "../../momentum_b200/csrc/ik_device.cuh"
 #include "../../momentum_b200/csrc/ik_plan.h"
 #include "emu_error.h"
+#include "emu_frame.h"
 
 using namespace mb2;
 
@@ -52,14 +53,15 @@ extern "C" int emu_input_gradients(int32_t numJoints, const int32_t* parents, co
   T.efs = plan.efs.data(); T.units = plan.units.data();
   T.targetStride = stride;
   T.weightsPerInstance = 1; T.numWeights = nc;
-  const int J = T.numJoints, n = T.numParams;
-  std::vector<float> vs(n), js(size_t(J) * kJointStateStride), tan(size_t(J) * kTangentStride);
+  const int n = T.numParams;
+  const auto f = inputGradientFrame(T.numJoints, n);
+  EmuFrame fr{f.floats};
+  float *th = fr.at(f.th), *vs = fr.at(f.vs), *js = fr.at(f.js), *tan = fr.at(f.tan);
   for (int b = 0; b < batch; ++b) {
-    const float* th = theta + size_t(b) * n;
-    for (int i = 0; i < n; ++i) vs[i] = 0.f;
+    for (int i = 0; i < n; ++i) { th[i] = theta[size_t(b) * n + i]; vs[i] = 0.f; }
     for (int p : plan.enabledList) vs[p] = direction[size_t(b) * n + p];
-    fkPasses<true, false>(HostLanes{}, T, th, js.data());
-    tangentPasses(HostLanes{}, T, js.data(), vs.data(), tan.data());
+    fkPasses<true, false>(HostLanes{}, T, th, js);
+    tangentPasses(HostLanes{}, T, js, vs, tan);
     const float* tg = rec.data() + size_t(b) * stride;
     const float* cw = cweights + size_t(b) * nc;
     for (int c = 0; c < nc; ++c) {
@@ -68,9 +70,9 @@ extern "C" int emu_input_gradients(int32_t numJoints, const int32_t* parents, co
       float* gW = gradWeights ? gradWeights + o : nullptr;
       float* gO = gradOffsets ? gradOffsets + o * per : nullptr;
       float* gT = gradTargets ? gradTargets + o * per : nullptr;
-      if (kind == 0) positionInputGradient(u, T.efs[u.ef], js.data(), tan.data(), tg + u.targetOff, cw[u.weightIdx], gW, gO, gT);
-      else orientationInputGradient(u, T.efs[u.ef], js.data(), tan.data(), tg + u.targetOff, cw[u.weightIdx], gW, gO, gT);
+      if (kind == 0) positionInputGradient(u, T.efs[u.ef], js, tan, tg + u.targetOff, cw[u.weightIdx], gW, gO, gT);
+      else orientationInputGradient(u, T.efs[u.ef], js, tan, tg + u.targetOff, cw[u.weightIdx], gW, gO, gT);
     }
   }
-  return MB2_OK;
+  return fr.check("inputGradientKernel");
 }

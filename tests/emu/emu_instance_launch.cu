@@ -4,26 +4,16 @@
 #include <cstdint>
 
 #include "../../include/momentum_b200.h"
-#include "../../momentum_b200/csrc/ik_instance_launch.h"
 #include "../../momentum_b200/csrc/ik_plan.h"
 #include "emu_error.h"
+#include "emu_frame.h"
 
 using namespace mb2;
-
-namespace {
-void words(const InstanceLaunch& l, int64_t out[5]) {
-  out[0] = l.warpsPerInstance;
-  out[1] = l.groupsPerCta;
-  out[2] = l.threads;
-  out[3] = l.smemBytes;
-  out[4] = l.stagedPoints;
-}
-} // namespace
 
 // planInstanceGroups: out = [W, groups per CTA, threads, smem bytes, 0], all zero when refused
 extern "C" int emu_plan_instance_groups(int64_t perInstance, int64_t tableBytes, int64_t batch, int64_t smemBudget, int32_t numSms, int64_t out[5]) {
   if (perInstance < 0 || tableBytes < 0 || smemBudget < 0 || out == nullptr) { g_emuErr = "bad argument"; return MB2_ERR_INVALID_ARGUMENT; }
-  words(planInstanceGroups(size_t(perInstance), size_t(tableBytes), long(batch), size_t(smemBudget), numSms), out);
+  launchWords(planInstanceGroups(size_t(perInstance), size_t(tableBytes), long(batch), size_t(smemBudget), numSms), out);
   return MB2_OK;
 }
 
@@ -36,6 +26,6 @@ extern "C" int emu_instance_launch(int32_t numJoints, const int32_t* parents, co
   g_emuErr = makeCharacter(numJoints, parents, offsets, prerot, numParams, outer, inner, vals, ptOffsets, h);
   if (!g_emuErr.empty()) return MB2_ERR_INVALID_ARGUMENT;
   if (op < 0 || op > kInstanceOpInputGradients || numPoints < 0 || smemBudget < 0 || out == nullptr) { g_emuErr = "bad argument"; return MB2_ERR_INVALID_ARGUMENT; }
-  words(planInstanceOp(hostCharacterTables(h), int(h.children.size()), op, backward != 0, numPoints, long(batch), size_t(smemBudget), numSms), out);
+  launchWords(planInstanceOp(hostCharacterTables(h), int(h.children.size()), op, backward != 0, numPoints, long(batch), size_t(smemBudget), numSms), out);
   return MB2_OK;
 }

@@ -6,12 +6,12 @@
 // skelGradPasses, jointOpElement) then run with HostLanes or element by element in order. It is not part of the product library and
 // nothing in momentum_b200/ loads it.
 #include <cstdint>
-#include <vector>
 
 #include "../../include/momentum_b200.h"
 #include "../../momentum_b200/csrc/ik_device.cuh"
 #include "../../momentum_b200/csrc/ik_plan.h"
 #include "emu_error.h"
+#include "emu_frame.h"
 
 using namespace mb2;
 
@@ -38,18 +38,21 @@ extern "C" int emu_joint_parameters(int32_t numJoints, const int32_t* parents, c
   const SkeletonTables S{h.childStart.data(), h.children.data(), h.ptColStart.data(), h.ptColRows.data(), h.ptColVals.data()};
   const int J = C.numJoints;
   if (op == 4) {
-    std::vector<float> js(size_t(J) * kJointStateStride), acc(size_t(J) * kSkelAccStride);
+    const size_t inN = size_t(J) * kParametersPerJoint;
+    const auto f = skeletonStateFrame(J, C.numParams, backward != 0, true);
+    EmuFrame fr{f.floats};
+    float* js = fr.at(f.js);
     for (int b = 0; b < batch; ++b) {
-      const float* jp = in + size_t(b) * J * kParametersPerJoint;
+      const float* jp = fr.load(f.in, in + size_t(b) * inN, inN);
       if (backward) {
-        fkPasses<true, true>(HostLanes{}, C, jp, js.data());
-        skelGradPasses(HostLanes{}, C, S, js.data(), grad + size_t(b) * J * 8, acc.data(), out + size_t(b) * J * kParametersPerJoint, nullptr);
+        fkPasses<true, true>(HostLanes{}, C, jp, js);
+        skelGradPasses(HostLanes{}, C, S, js, grad + size_t(b) * J * 8, fr.at(f.acc), out + size_t(b) * inN, nullptr);
       } else {
-        fkPasses<false, true>(HostLanes{}, C, jp, js.data());
+        fkPasses<false, true>(HostLanes{}, C, jp, js);
         for (int i = 0; i < J * 8; ++i) out[size_t(b) * J * 8 + i] = js[(i >> 3) * kJointStateStride + (i & 7)];
       }
     }
-    return MB2_OK;
+    return fr.check("skeletonStateKernel");
   }
   switch (op * 2 + (backward ? 1 : 0)) {
     case 0: runElements<kJointOpParameterTransform, false>(C, S, batch, in, grad, out); break;

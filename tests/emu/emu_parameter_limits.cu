@@ -10,9 +10,9 @@
 
 #include "../../include/momentum_b200.h"
 #include "../../momentum_b200/csrc/ik_device.cuh"
-#include "../../momentum_b200/csrc/ik_instance_launch.h"
 #include "../../momentum_b200/csrc/ik_plan.h"
 #include "emu_error.h"
+#include "emu_frame.h"
 
 using namespace mb2;
 
@@ -69,24 +69,26 @@ extern "C" int emu_parameter_limits_tables(MB2_EMU_CHARACTER, int32_t* rows, int
 extern "C" int emu_parameter_limits(MB2_EMU_CHARACTER, int32_t backward, int32_t batch, const float* theta, const float* grad, float* out) {
   Emulated e;
   if (MB2_EMU_SETUP(e) != MB2_OK) return MB2_ERR_INVALID_ARGUMENT;
-  const int J = e.C.numJoints, n = e.C.numParams, R = e.t.numRows;
-  std::vector<float> jp(size_t(J) * kParametersPerJoint), js(size_t(J) * kJointStateStride), acc(size_t(J) * kSkelAccStride), gjp(jp.size());
+  const int n = e.C.numParams, R = e.t.numRows;
+  const auto f = parameterLimitsFrame(e.C.numJoints, n, backward != 0, e.t.ellipsoid != 0);
+  EmuFrame fr{f.floats};
+  float *jp = fr.at(f.jp), *js = fr.at(f.js), *gjp = fr.at(f.gjp), *acc = fr.at(f.acc);
   for (int b = 0; b < batch; ++b) {
-    const float* th = theta + size_t(b) * n;
     if (R == 0) { // the library's launcher: nothing to write, a zero gradient
       if (backward) for (int p = 0; p < n; ++p) out[size_t(b) * n + p] = 0.f;
       continue;
     }
+    const float* th = fr.load(f.th, theta + size_t(b) * n, n);
     if (!backward) {
-      if (e.t.ellipsoid) limitPasses<true>(HostLanes{}, e.C, e.L, th, jp.data(), js.data(), out + size_t(b) * R);
-      else limitPasses<false>(HostLanes{}, e.C, e.L, th, jp.data(), js.data(), out + size_t(b) * R);
+      if (e.t.ellipsoid) limitPasses<true>(HostLanes{}, e.C, e.L, th, jp, js, out + size_t(b) * R);
+      else limitPasses<false>(HostLanes{}, e.C, e.L, th, jp, js, out + size_t(b) * R);
     } else if (e.t.ellipsoid) {
-      limitGradPasses<true>(HostLanes{}, e.C, e.S, e.L, th, jp.data(), js.data(), acc.data(), gjp.data(), grad + size_t(b) * R, out + size_t(b) * n);
+      limitGradPasses<true>(HostLanes{}, e.C, e.S, e.L, th, jp, js, acc, gjp, grad + size_t(b) * R, out + size_t(b) * n);
     } else {
-      limitGradPasses<false>(HostLanes{}, e.C, e.S, e.L, th, jp.data(), js.data(), acc.data(), gjp.data(), grad + size_t(b) * R, out + size_t(b) * n);
+      limitGradPasses<false>(HostLanes{}, e.C, e.S, e.L, th, jp, js, acc, gjp, grad + size_t(b) * R, out + size_t(b) * n);
     }
   }
-  return MB2_OK;
+  return fr.check("parameterLimitsKernel");
 }
 
 // apply_model_param_limits: forward out [B][n] = the clamp of theta; backward out [B][n] from grad [B][n]
@@ -107,10 +109,6 @@ extern "C" int emu_parameter_limits_launch(MB2_EMU_CHARACTER, int32_t backward, 
   if (MB2_EMU_SETUP(e) != MB2_OK) return MB2_ERR_INVALID_ARGUMENT;
   const InstanceLaunch l = planInstanceOp(e.C, int(e.h.children.size()), kInstanceOpParameterLimits, backward != 0, 0, long(batch),
                                           size_t(smemBudget), numSms, e.t.ellipsoid);
-  out[0] = l.warpsPerInstance;
-  out[1] = l.groupsPerCta;
-  out[2] = l.threads;
-  out[3] = l.smemBytes;
-  out[4] = l.stagedPoints;
+  launchWords(l, out);
   return MB2_OK;
 }

@@ -13,6 +13,7 @@
 #include "../../momentum_b200/csrc/ik_device.cuh"
 #include "../../momentum_b200/csrc/ik_plan.h"
 #include "emu_error.h"
+#include "emu_frame.h"
 
 using namespace mb2;
 
@@ -48,14 +49,16 @@ extern "C" int emu_positions(int32_t numJoints, const int32_t* parents, const fl
   if (setUp(numJoints, parents, offsets, prerot, numParams, outer, inner, vals, ptOffsets, joint, numPoints, pointParents, e) != MB2_OK)
     return MB2_ERR_INVALID_ARGUMENT;
   const size_t n3 = size_t(numPoints) * 3;
-  std::vector<float> js(size_t(e.C.numJoints) * kJointStateStride);
+  const auto f = skeletonStateFrame(e.C.numJoints, e.C.numParams, false, joint != 0);
+  EmuFrame fr{f.floats};
+  float* js = fr.at(f.js);
   for (int b = 0; b < batch; ++b) {
-    const float* p = params + size_t(b) * e.inN;
-    if (joint) fkPasses<false, true>(HostLanes{}, e.C, p, js.data());
-    else fkPasses<false, false>(HostLanes{}, e.C, p, js.data());
-    positionPasses(HostLanes{}, e.P, js.data(), pointOffsets + (offsetsBatched ? size_t(b) * n3 : 0), positions + size_t(b) * n3);
+    const float* in = fr.load(f.in, params + size_t(b) * e.inN, e.inN);
+    if (joint) fkPasses<false, true>(HostLanes{}, e.C, in, js);
+    else fkPasses<false, false>(HostLanes{}, e.C, in, js);
+    positionPasses(HostLanes{}, e.P, js, pointOffsets + (offsetsBatched ? size_t(b) * n3 : 0), positions + size_t(b) * n3);
   }
-  return MB2_OK;
+  return fr.check("positionsKernel");
 }
 
 // its backward from gradPositions [B][N][3]: gradParams [B][n] ([B][7 J]) and gradOffsets ([N][3] the batch sum when shared, else
@@ -69,17 +72,20 @@ extern "C" int emu_positions_backward(int32_t numJoints, const int32_t* parents,
     return MB2_ERR_INVALID_ARGUMENT;
   const int J = e.C.numJoints;
   const size_t n3 = size_t(numPoints) * 3;
-  std::vector<float> js(size_t(J) * kJointStateStride), acc(size_t(J) * kSkelAccStride), gjp(size_t(J) * kParametersPerJoint);
+  const auto f = skeletonStateFrame(J, e.C.numParams, true, joint != 0);
+  EmuFrame fr{f.floats};
+  float* js = fr.at(f.js);
   std::vector<float> rows(gradOffsets != nullptr && !offsetsBatched ? size_t(batch) * n3 : 0);
   for (int b = 0; b < batch; ++b) {
-    const float* p = params + size_t(b) * e.inN;
-    if (joint) fkPasses<true, true>(HostLanes{}, e.C, p, js.data());
-    else fkPasses<true, false>(HostLanes{}, e.C, p, js.data());
+    const float* in = fr.load(f.in, params + size_t(b) * e.inN, e.inN);
+    if (joint) fkPasses<true, true>(HostLanes{}, e.C, in, js);
+    else fkPasses<true, false>(HostLanes{}, e.C, in, js);
     float* gp = gradParams != nullptr ? gradParams + size_t(b) * e.inN : nullptr;
     float* gOff = gradOffsets == nullptr ? nullptr : (offsetsBatched ? gradOffsets + size_t(b) * n3 : rows.data() + size_t(b) * n3);
-    positionGradPasses(HostLanes{}, e.C, e.S, e.P, js.data(), pointOffsets + (offsetsBatched ? size_t(b) * n3 : 0), gradPositions + size_t(b) * n3,
-                       acc.data(), joint || gp == nullptr ? gp : gjp.data(), joint ? nullptr : gp, gOff);
+    positionGradPasses(HostLanes{}, e.C, e.S, e.P, js, pointOffsets + (offsetsBatched ? size_t(b) * n3 : 0), gradPositions + size_t(b) * n3,
+                       fr.at(f.acc), joint || gp == nullptr ? gp : fr.at(f.gjp), joint ? nullptr : gp, gOff);
   }
+  if (const int rc = fr.check("positionsKernel")) return rc;
   if (gradOffsets != nullptr && !offsetsBatched) {
     const int perChunk = batchSumChunk(batch);
     for (size_t k = 0; k < n3; ++k) {

@@ -6,6 +6,8 @@ g passes when ||g - g64||_inf <= K * max(||g64||_inf, 1) per instance. K is pinn
 the fixtures below (emulator and H100); the self-checks show that the bound rejects a backward that drops the quaternion term or swaps
 two rotation DOFs.
 """
+import ctypes
+
 import numpy as np
 import pytest
 import torch
@@ -160,6 +162,24 @@ def _emu_backward(L, ch, theta, G):
     assert rc == 0, L.emu_last_error().decode()
     return out
 
+
+
+def test_emulated_frame_catches_an_overrun(emu):
+    """The emulator runs the backward in skeletonStateFrame's floats followed by a canary: in the kernel's frame it passes, and in a
+    frame one aligned block short, where the last region (the joint-parameter gradient) overruns, it fails instead of returning."""
+    ch = FIXTURES["humanoid72"]()
+    theta, G = _inputs(ch, 2, 3)
+    theta, G = np.ascontiguousarray(theta, np.float32), np.ascontiguousarray(G, np.float32)
+    emu.emu_skeleton_state_backward_frame.argtypes = emu_lib._CHARACTER + [ctypes.c_int32] + [ctypes.c_void_p] * 3 + [ctypes.c_int32]
+    results = []
+    for short in (0, 4):
+        keep, out = [], np.zeros(theta.shape, np.float32)
+        rc = emu.emu_skeleton_state_backward_frame(*emu_lib.character_args(ch, keep), theta.shape[0], theta.ctypes.data, G.ctypes.data,
+                                                   out.ctypes.data, short)
+        results.append((rc, emu.emu_last_error().decode() if rc else "", out))
+    assert results[0][0] == 0, results[0][1]
+    np.testing.assert_array_equal(results[0][2], _emu_backward(emu, ch, theta, G))
+    assert results[1][0] != 0 and "wrote past the instance's shared-memory frame" in results[1][1], results[1]
 
 def test_fk64_restates_forward_kinematics():
     for name, make in FIXTURES.items():
