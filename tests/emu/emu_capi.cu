@@ -631,6 +631,76 @@ extern "C" int emu_store_invariants(mb2_solver_function* f, int64_t out[6]) {
   return MB2_OK;
 }
 
+// The tile plan of the solver function (cholesky mode 2: dense pattern, 3: sparse pattern; strips always planned) as a sequence of int32
+// sections, each [length, values...], in this order:
+//   header {n (device columns), nPad, numTileCols, numTiles, numLevels, nParams, numRows, numStrips, strip stride, residOff, parkTiles,
+//           16-bit tables valid, then the 12 section offsets of GramCholLayout};
+//   perm, pos, deviceCols (device column -> model parameter, -1 = gap), tileRow, tileCol, tileIdTable, diagTile,
+//   levelColStart, levelCols, levelPanelStart, panelTile, panelDiag, panelRow, levelTaskStart, taskDst, taskPairStart, pairA, pairB,
+//   levelVTaskStart, vtaskRow, vtaskSrcStart, vsrcTile, vsrcCol, colPanelStart, colPanelTile, colPanelRow,
+//   levelOrderStart8, taskOrder8, levelOrderStart16, taskOrder16,
+//   Gram plan: stripCoord, tilePairStart, pairA, pairB, tileOrder, tileQuadStart, quad, colStripStart, colStrip, cellStripOff, cellQuadStride,
+//   GramCholTables::tab (undecoded), cells [numCells][5] {first row, row count, device column, unit, unit kind}.
+// Called with out = nullptr it only returns the word count in *words; with a buffer of *words ints it fills it.
+extern "C" int emu_tile_plan(mb2_solver_function* f, int32_t cholMode, int32_t* out, int64_t* words) {
+  CholSchedule s;
+  GramPlan g;
+  const std::string e = planTiles(f, cholMode, true, s, g);
+  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
+  GramCholTables gc;
+  const bool valid = makeGramCholTables(g, s, gc).empty();
+  const Plan& p = f->plan;
+  std::vector<int32_t> blob;
+  auto add = [&](auto first, auto last) { blob.push_back(int32_t(last - first)); for (auto it = first; it != last; ++it) blob.push_back(int32_t(*it)); };
+  auto sec = [&](const auto& v) { add(v.begin(), v.end()); };
+  const GramCholLayout& L = gc.L;
+  const std::vector<int32_t> header = {s.n, s.nPad, s.numTileCols, s.numTiles, s.numLevels, s.nParams, p.numRows, g.numStrips, g.stride, g.residOff,
+                                       gc.parkTiles, valid ? 1 : 0, L.gram, L.quad, L.col, L.colEnt, L.level, L.diag, L.panel, L.order, L.pair, L.vtask,
+                                       L.vsrc, L.colPanel};
+  sec(header);
+  sec(s.perm); sec(s.pos); sec(p.deviceCols); sec(s.tileRow); sec(s.tileCol); sec(s.tileIdTable); sec(s.diagTile);
+  sec(s.levelColStart); sec(s.levelCols); sec(s.levelPanelStart); sec(s.panelTile); sec(s.panelDiag); sec(s.panelRow);
+  sec(s.levelTaskStart); sec(s.taskDst); sec(s.taskPairStart); sec(s.pairA); sec(s.pairB);
+  sec(s.levelVTaskStart); sec(s.vtaskRow); sec(s.vtaskSrcStart); sec(s.vsrcTile); sec(s.vsrcCol);
+  sec(s.colPanelStart); sec(s.colPanelTile); sec(s.colPanelRow);
+  sec(s.levelOrderStart8); sec(s.taskOrder8); sec(s.levelOrderStart16); sec(s.taskOrder16);
+  sec(g.stripCoord); sec(g.tilePairStart); sec(g.pairA); sec(g.pairB); sec(g.tileOrder); sec(g.tileQuadStart); sec(g.quad);
+  sec(g.colStripStart); sec(g.colStrip); sec(g.cellStripOff); sec(g.cellQuadStride);
+  sec(gc.tab);
+  std::vector<int32_t> cells;
+  for (const CellDesc& c : p.cells) {
+    const UnitDesc& u = p.units[c.unit];
+    cells.insert(cells.end(), {int32_t(u.row0), int32_t(u.numRows), int32_t(c.col), int32_t(c.unit), int32_t(u.kind)});
+  }
+  sec(cells);
+  if (out != nullptr) {
+    if (*words < int64_t(blob.size())) return fail(MB2_ERR_INVALID_ARGUMENT, "emu_tile_plan: buffer too small");
+    std::copy(blob.begin(), blob.end(), out);
+  }
+  *words = int64_t(blob.size());
+  return MB2_OK;
+}
+
+// The normal equations the tile-sparse Gram computes for instance b at params (the instance's theta, [numParams] floats), without
+// damping: out = [numTiles][256] tiles in the fragment layout (tileIdx; padded rows / columns hold the identity extension) followed
+// by J^T r in slot order [nPad]. *floats gets the count; out = nullptr only returns it.
+extern "C" int emu_gram_system(mb2_solver_function* f, int32_t cholMode, int32_t b, const float* params, float* out, int64_t* floats) {
+  TilePlan tp;
+  const std::string e = planTiles(f, cholMode, true, tp.sched, tp.gram);
+  if (!e.empty()) return fail(MB2_ERR_INVALID_ARGUMENT, e);
+  const int64_t count = int64_t(tp.sched.numTiles) * 256 + tp.sched.nPad;
+  if (out != nullptr) {
+    if (*floats < count) return fail(MB2_ERR_INVALID_ARGUMENT, "emu_gram_system: buffer too small");
+    makeScheduleBlob(tp.sched, tp.blob, tp.S);
+    const FunctionTables T = tables(f);
+    double err;
+    sweepOne<true>(f, T, b, params, &err, nullptr);
+    gramOne(f, b, tp.gram, tp.S, 0.f, out);
+  }
+  *floats = count;
+  return MB2_OK;
+}
+
 // The device the solve path is chosen for (SM count, opt-in shared memory per block, shared memory per SM).
 extern "C" void emu_set_device_limits(int32_t numSms, int32_t smemOptin, int32_t smemPerSm) { g_limits = DeviceLimits{numSms, smemOptin, smemPerSm}; }
 
