@@ -618,9 +618,10 @@ int mb2_solver_function_get_input_gradient_launch(mb2_solver_function* f, int64_
  * size NB, [6] its matrix in shared memory, [7] / [8] threads of the Gram / tile Cholesky kernels (256 or 512), [9] Jacobian rows
  * the QR kernels fold at once (the limit), [10] QR row chunks, [11] rows of the widest chunk, [12] floats of the trust-region R kept
  * per instance, [13] instance groups per CTA of the persistent kernel (any plan with strips), [14] its dynamic shared memory in
- * bytes. All zero before the first solve and after a refused solve (by its options, or no resident Gram + Cholesky CTA); a CUDA error
+ * bytes, [15] instance slices whose iteration chains ran concurrently on streams of their own (2 on the Gram + Cholesky path, without
+ * line search, from four waves of its resident CTAs on; 1 otherwise, and in a profiling solve). All zero before the first solve and after a refused solve (by its options, or no resident Gram + Cholesky CTA); a CUDA error
  * later in a solve leaves the path it had chosen. No reference counterpart. */
-int mb2_solver_get_solve_path(mb2_solver* s, int64_t out[15]);
+int mb2_solver_get_solve_path(mb2_solver* s, int64_t out[16]);
 
 /* ---- Mixed-rig batches (BASELINE.json configs[4]): heterogeneous instances -> buckets sharing one plan -> batched solves --------
  * The reference treats a batch element by element (pymomentum/tensor_ik/tensor_ik.cpp:127-177 builds error functions, solver function

@@ -153,10 +153,11 @@ cudaError_t launchSweep(const SweepArgs& a0, bool jacobian, cudaStream_t stream,
     // this device (rounds x warps x SMs closest above the batch); more warps than kSweepMaxWarps spill registers.
     const int sms = std::max(g_numSms, 1);
     const int maxG = std::min(groupsOneWarp, kSweepMaxWarps), minG = std::min(12, maxG);
+    const int planned = a.planBatch > 0 ? a.planBatch : a.batch;
     long best = -1;
-    if (a.batch < sms * minG) { groups = std::max(1, (a.batch + sms - 1) / sms); best = 0; } // a small batch: spread it over the SMs
+    if (planned < sms * minG) { groups = std::max(1, (planned + sms - 1) / sms); best = 0; } // a small batch: spread it over the SMs
     for (int gcand = maxG; gcand >= minG && best != 0; --gcand) {
-      const long rounds = (a.batch + long(sms) * gcand - 1) / (long(sms) * gcand);
+      const long rounds = (planned + long(sms) * gcand - 1) / (long(sms) * gcand);
       if (best < 0 || rounds * gcand < best) { best = rounds * gcand; groups = gcand; }
     }
   } else {
@@ -2343,7 +2344,7 @@ __device__ int acquireParkSlot(uint32_t* words, int numWords, int start) {
 // The per-instance critical path is a chain of dependent phases no wider than a few warps: instances in flight per SM are what
 // buys throughput. The per-tile arithmetic is that of gramTilesKernel + choleskyScheduledKernel (the same device functions).
 template <bool kProfile, class Tables>
-__global__ void __launch_bounds__(kGramThreads, 4) gramCholeskyKernel(const GramCholArgs a, const CholSchedDev S, const __grid_constant__ Tables P) {
+__global__ void __launch_bounds__(kGramThreads, kGramCholCtasPerSm) gramCholeskyKernel(const GramCholArgs a, const CholSchedDev S, const __grid_constant__ Tables P) {
   extern __shared__ __align__(16) float gcSmem[];
   const GramArgs& g = a.g;
   const CholArgs& c = a.c;

@@ -22,6 +22,7 @@ struct SweepArgs {           // K1 (FK + residual + Jacobian) and K4 (FK + error
   double* errors;            // [B]
   const int32_t* active;     // optional per-instance mask
   float* stateOut;           // optional [B][J][8]
+  int32_t planBatch;         // instances launchSweep plans the variant for (0: batch): the whole batch when this launch is one slice of it
   int32_t stageTables;       // set by launchSweep: 1 every read-only table in shared memory, 2 all but cells / contributions, 0 none
   int32_t warpsPerInstance;  // set by launchSweep: 1, 2, 4 or 8 warps share one instance (large rigs: few instances fit in shared memory)
 };
@@ -112,7 +113,10 @@ struct GramCholGlobalTables {
   GramCholLayout L;
   const uint16_t* tab;
 };
-// scratch slots for the parked tiles: resident CTAs of the launch on this device, rounded up to whole 32-bit words of parkSlots
+// scratch slots for the parked tiles: resident CTAs of the launch on this device, rounded up to whole 32-bit words of parkSlots.
+// The instance slices of a solve (SolvePath::slices) run concurrent gramCholeskyKernel grids on one bitmap: correct while the slots are
+// at least all resident CTAs of every concurrent grid, which holds because the occupancy an SM allows this kernel bounds the CTAs of
+// all its grids together.
 int gramCholeskyParkSlots(const GramCholArgs& a, const CholSchedDev& sched, bool paramTables);
 // tables: exactly one of inParams (non-null) or inGlobal is used
 cudaError_t launchGramCholesky(const GramCholArgs& a, const CholSchedDev& sched, const GramCholParamTables* inParams, const GramCholGlobalTables& inGlobal, bool profile,

@@ -117,6 +117,7 @@ int tileThreads(size_t smem, const DeviceLimits& lim) { return 2 * (smem + 1024)
 int chooseSolvePath(const mb2_gauss_newton_options& o, int batch, const HostCharacter& ch, const HostFunction& fn, const PlanFiguresFn& plan,
                     const DeviceLimits& lim, SolvePath& P, std::string& msg) {
   P = SolvePath{};
+  P.slices = 1;
   auto refuse = [&](int code, const char* m) { msg = m; return code; };
   PlanFigures F;
   auto request = [&](int mode, bool schedDense, bool strips) {
@@ -204,6 +205,11 @@ int chooseSolvePath(const mb2_gauss_newton_options& o, int batch, const HostChar
     P.kind = useTr ? kSolveTrustRegionQr : kSolveQr;
   } else if (useGramChol) {
     P.kind = kSolveGramCholesky;
+    // resident gramCholeskyKernel CTAs on the device (1 KB of shared memory is reserved per CTA); the line search's launches run on
+    // the whole batch, so only the plain iteration chain is sliced
+    const size_t perCta = gramCholeskySmemBytes(size_t(F.stripStride), ns, F.nPad, F.numTiles) + 1024;
+    const int resident = lim.numSms * std::min<int>(kGramCholCtasPerSm, int(size_t(lim.smemPerSm) / perCta));
+    if (o.do_line_search == 0 && resident > 0 && batch >= kSliceMinWaves * resident) P.slices = kSolveSlices;
   } else if (useSchedule) {
     P.kind = useGram ? kSolveTiles : kSolveTilesKMajor;
     P.cholThreads = tileThreads(choleskyScheduledSmemBytes(ns, F.nPad, F.numTiles, F.schedBlobInts), lim);
@@ -220,7 +226,7 @@ int chooseSolvePath(const mb2_gauss_newton_options& o, int batch, const HostChar
 void solvePathWords(const SolvePath& p, int64_t out[kSolvePathWords]) {
   const int64_t w[kSolvePathWords] = {p.kind, p.planMode, p.schedDense, p.strips, p.jtjMode, p.denseNb, p.denseInSmem, p.gramThreads, p.cholThreads,
                                       p.qrMaxChunkRows, p.qrChunkStarts.empty() ? 0 : int64_t(p.qrChunkStarts.size()) - 1, p.qrWidestChunk,
-                                      int64_t(p.trRSavedFloats), p.fused.groups, int64_t(p.fused.smemBytes)};
+                                      int64_t(p.trRSavedFloats), p.fused.groups, int64_t(p.fused.smemBytes), p.slices};
   std::copy(w, w + kSolvePathWords, out);
 }
 

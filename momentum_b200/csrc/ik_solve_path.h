@@ -91,14 +91,23 @@ struct SolvePath {
   int32_t qrWidestChunk{0};
   size_t trRSavedFloats{0};           // trust-region QR: floats of the saved R per instance
   FusedConfig fused;                  // persistent kernel: instance groups per CTA next to the staged plan (every plan with strips it requested)
+  int32_t slices{0};                  // concurrent instance slices of the iteration chain (kSolveSlices or 1; 0 before a path is chosen)
 };
+
+// gramCholeskyKernel's resident CTAs per SM: its launch bound (shared memory may allow fewer)
+constexpr int kGramCholCtasPerSm = 4;
+// A batch of at least kSliceMinWaves waves of resident gramCholeskyKernel CTAs (no line search) runs as kSolveSlices instance slices,
+// each with its own chain of sweep + gramCholeskyKernel launches on its own stream: instances do not interact inside a solve, so the
+// tail and drain of one slice's launch are filled by the other slice's next launch instead of idling the GPU at every kernel boundary.
+constexpr int kSolveSlices = 2;
+constexpr int kSliceMinWaves = 4;
 
 // The path of one solve of `batch` instances with options `o`. Every refusal returns its error code with `msg` set; plan builds go
 // through `plan`, in the order the fallbacks need them.
 int chooseSolvePath(const mb2_gauss_newton_options& o, int batch, const HostCharacter& ch, const HostFunction& fn, const PlanFiguresFn& plan,
                     const DeviceLimits& lim, SolvePath& out, std::string& msg);
 
-constexpr int kSolvePathWords = 15;
+constexpr int kSolvePathWords = 16;
 // the record as mb2_solver_get_solve_path reports it (include/momentum_b200.h)
 void solvePathWords(const SolvePath& p, int64_t out[kSolvePathWords]);
 

@@ -835,12 +835,12 @@ class GaussNewtonSolver(_Base):
 
     SOLVE_PATH_KINDS = {0: None, 1: "dense", 2: "tiles_kmajor", 3: "tiles", 4: "gram_cholesky", 5: "persistent", 6: "qr", 7: "trust_region_qr"}
     SOLVE_PATH_KEYS = ["kind", "plan_mode", "sched_dense", "strips", "jtj_mode", "dense_nb", "dense_in_smem", "gram_threads", "chol_threads",
-                       "qr_max_chunk_rows", "qr_chunks", "qr_widest_chunk", "tr_r_floats", "fused_groups", "fused_smem"]
+                       "qr_max_chunk_rows", "qr_chunks", "qr_widest_chunk", "tr_r_floats", "fused_groups", "fused_smem", "slices"]
 
     def get_solve_path(self) -> dict:
         """The linear-solve path of the last solve (mb2_solver_get_solve_path): kind as a name (None before the first solve), the
-        plan request, the resolved JtJ mode and the launch variants of the kernels it runs."""
-        out = (C.c_int64 * 15)()
+        plan request, the resolved JtJ mode, the launch variants of the kernels it runs and the instance slices it ran as."""
+        out = (C.c_int64 * 16)()
         self._check(self._L.mb2_solver_get_solve_path(self._h, out))
         d = dict(zip(self.SOLVE_PATH_KEYS, (int(v) for v in out)))
         d["kind"] = self.SOLVE_PATH_KINDS[d["kind"]]
