@@ -577,14 +577,14 @@ void recordPhaseStop(mb2_solver* s, cudaStream_t st) {
   cudaEventRecord(s->events.back().stop, st);
 }
 
-__global__ void initSolveStateKernel(int batch, int32_t* active, int32_t* iterations, int32_t* status, double* lastErrors, double* errors) {
+__global__ void initSolveStateKernel(int batch, const SolveState s) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= batch) return;
-  active[b] = 1;
-  iterations[b] = 0;
-  status[b] = 0;
-  lastErrors[b] = DBL_MAX; // solver.cpp:83-84
-  errors[b] = DBL_MAX;
+  s.active[b] = 1;
+  s.iterations[b] = 0;
+  s.status[b] = 0;
+  s.lastErrors[b] = DBL_MAX; // solver.cpp:83-84
+  s.errors[b] = DBL_MAX;
 }
 __global__ void initLineSearchKernel(int batch, const int32_t* active, int32_t* searching, float* scale) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1824,6 +1824,15 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
     MB2_CUDA(cudaMemsetAsync(s->dHistory.p, 0, size_t(B) * std::max(maxIt, 1) * sizeof(double), st));
     s->historyStride = size_t(std::max(maxIt, 1));
   }
+  // the per-instance state every launch takes (lastErrors, active, activeCount: below; the persistent kernel keeps them in shared memory)
+  SolveState state{};
+  state.errors = f->dErrors.p;
+  state.iterations = s->dIterations.p;
+  state.status = s->dStatus.p;
+  state.history = o.store_error_history ? s->dHistory.p : nullptr;
+  state.minIterations = minIt;
+  state.maxIterations = maxIt;
+  state.threshold = o.threshold;
   for (auto& e : s->events) { cudaEventDestroy(e.start); cudaEventDestroy(e.stop); }
   s->events.clear();
   if (s->profiling && (P.kind == kSolvePersistent || P.kind == kSolveGramCholesky)) {
@@ -1847,17 +1856,11 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
     fa.residOff = ds.gram.residOff;
     fa.numOrder = int32_t(ds.gram.tileOrder.size());
     fa.regularization = o.regularization;
-    fa.threshold = o.threshold;
-    fa.minIterations = minIt;
-    fa.maxIterations = maxIt;
     fa.theta = theta;
     fa.ldTheta = n;
     fa.targets = f->dTargets.p;
     fa.cweights = f->dWeights.p;
-    fa.errors = f->dErrors.p;
-    fa.iterations = s->dIterations.p;
-    fa.status = s->dStatus.p;
-    fa.history = o.store_error_history ? s->dHistory.p : nullptr;
+    fa.state = state;
     fa.workCounter = s->dWorkCounter.p;
     fa.phaseCycles = s->inKernelProfile ? s->dPhaseCycles.p : nullptr;
     if (s->profiling) {
@@ -1891,6 +1894,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   MB2_CUDA(s->dLastErrors.resize(B));
   MB2_CUDA(s->dActive.resize(B));
   MB2_CUDA(s->dActiveCount.resize(size_t(P.slices)));
+  state.lastErrors = s->dLastErrors.p; state.active = s->dActive.p; state.activeCount = s->dActiveCount.p;
   const bool lineSearch = o.do_line_search != 0 && P.kind != kSolveTrustRegionQr; // (TrustRegionQRT has no line search: steps are accepted or rejected by rho)
   if (lineSearch) {
     MB2_CUDA(s->dThetaOrig.resize(size_t(B) * n));
@@ -1899,7 +1903,6 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
     MB2_CUDA(s->dSearching.resize(B));
     MB2_CUDA(s->dGradDotDelta.resize(B));
   }
-  double* history = o.store_error_history ? s->dHistory.p : nullptr;
 
   // ---- kernel arguments: only the iteration changes from one iteration to the next ----
   const SweepArgs sweep = sweepArgs(f, theta, s->dActive.p);
@@ -1936,16 +1939,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   c.ldTheta = n;
   c.delta = s->dDelta.p;
   c.applyUpdate = lineSearch ? 0 : 1;
-  c.errors = f->dErrors.p;
-  c.lastErrors = s->dLastErrors.p;
-  c.active = s->dActive.p;
-  c.iterations = s->dIterations.p;
-  c.status = s->dStatus.p;
-  c.history = history;
-  c.minIterations = minIt;
-  c.maxIterations = maxIt;
-  c.threshold = o.threshold;
-  c.activeCount = s->dActiveCount.p;
+  c.state = state;
   c.bookkeeping = lineSearch ? 0 : 1;
   c.gradDotDelta = lineSearch ? s->dGradDotDelta.p : nullptr;
   c.g = s->dGrad.p;
@@ -1997,57 +1991,19 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   SweepArgs trial = sweepArgs(f, theta, s->dSearching.p);
   trial.errors = s->dTrialErrors.p;
   LineSearchArgs la{};
-  la.batch = B; la.ns = ns; la.numParams = n; la.ldTheta = n;
+  la.batch = B;
   la.errors = f->dErrors.p;
   la.trialErrors = s->dTrialErrors.p;
   la.gradDotDelta = s->dGradDotDelta.p;
   la.scale = s->dScale.p;
   la.searching = s->dSearching.p;
   la.subsetVariant = o.subset_line_search;
-  la.active = s->dActive.p;
-  BookkeepingArgs ba{};
-  ba.batch = B;
-  ba.errors = f->dErrors.p; ba.lastErrors = s->dLastErrors.p; ba.active = s->dActive.p; ba.iterations = s->dIterations.p;
-  ba.status = s->dStatus.p; ba.history = history;
-  ba.theta = theta; ba.ldTheta = n; ba.numParams = n;
-  ba.minIterations = minIt; ba.maxIterations = maxIt; ba.threshold = o.threshold; ba.activeCount = s->dActiveCount.p;
 
   // ---- instance slices (SolvePath::slices): slice k holds instances [B k / S, B (k + 1) / S) with its own active counter, and runs its
-  // iteration chain on its own stream (slice 0 on the caller's). Every per-instance pointer of its launches is offset to its first instance.
+  // iteration chain on its own stream (slice 0 on the caller's). The arguments' slice functions offset its per-instance pointers.
   const int S = P.slices;
   auto sliceBegin = [&](int k) { return int(int64_t(B) * k / S); };
   auto sliceStream = [&](int k) { return k == 0 ? st : s->sliceStreams[k - 1]; };
-  auto sliceSweep = [&](int k) {
-    const int b0 = sliceBegin(k);
-    SweepArgs a = sweep;
-    a.batch = sliceBegin(k + 1) - b0;
-    a.planBatch = B; // the variant the whole batch gets
-    a.theta += size_t(b0) * a.ldTheta;
-    a.targets += size_t(b0) * a.T.targetStride;
-    if (a.T.weightsPerInstance) a.cweights += size_t(b0) * a.T.numWeights;
-    a.jacobian += size_t(b0) * a.T.jacobianStride;
-    a.errors += b0;
-    if (a.active) a.active += b0;
-    return a;
-  };
-  auto sliceGramCholesky = [&](int k) {
-    const int b0 = sliceBegin(k);
-    GramCholArgs a = gc;
-    a.g.batch = a.c.batch = sliceBegin(k + 1) - b0;
-    a.g.strips += size_t(b0) * a.g.stripStride;
-    a.g.active += b0;
-    CholArgs& c = a.c;
-    c.theta += size_t(b0) * c.ldTheta;
-    c.delta += size_t(b0) * c.ns;
-    c.errors += b0;
-    c.lastErrors += b0;
-    c.active += b0;
-    c.iterations += b0;
-    c.status += b0;
-    if (c.history) c.history += size_t(b0) * c.maxIterations;
-    c.activeCount += k;
-    return a; // (H, g, tilesIn and the line search's gradDotDelta are not read on this path)
-  };
   if (S > 1 && !s->forkEvent) {
     MB2_CUDA(cudaEventCreateWithFlags(&s->forkEvent, cudaEventDisableTiming));
     for (int i = 0; i < kSolveSlices - 1; ++i) {
@@ -2070,7 +2026,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   };
 
   s->kernelLaunches = 0;
-  initSolveStateKernel<<<(B + 127) / 128, 128, 0, st>>>(B, s->dActive.p, s->dIterations.p, s->dStatus.p, s->dLastErrors.p, f->dErrors.p);
+  initSolveStateKernel<<<(B + 127) / 128, 128, 0, st>>>(B, state);
   MB2_CUDA(cudaGetLastError());
   MB2_CUDA(cudaMemcpyAsync(s->dTheta0.p, theta, size_t(B) * n * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if ((rc = fork()) != MB2_OK) return rc;
@@ -2078,15 +2034,16 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
   static const bool cholProfile = getenv("MB2_CHOL_PROFILE") != nullptr;
   constexpr int kPollEvery = 4; // iterations between two reads of the device-side active counter (each read blocks the host on `st`)
   for (int it = 0; it < maxIt; ++it) {
-    step.iteration = it;
+    step.state.iteration = it;
     step.profile = (it == 0 && cholProfile) ? 1 : 0;
     // S > 1 only on the Gram + Cholesky path without line search: every other path runs the whole batch as slice 0
     for (int k = 0; k < S; ++k) {
       const cudaStream_t sk = sliceStream(k);
+      const int b0 = sliceBegin(k), count = sliceBegin(k + 1) - b0;
       MB2_CUDA(cudaMemsetAsync(s->dActiveCount.p + k, 0, sizeof(int), sk));
       // --- doIteration (gauss_newton_solver.cpp:224-280) ---
       recordPhaseStart(s, 0, sk);
-      MB2_CUDA(launchSweep(sliceSweep(k), true, sk, &f->lastSweep[1]));
+      MB2_CUDA(launchSweep(sweep.slice(b0, count), true, sk, &f->lastSweep[1]));
       recordPhaseStop(s, sk);
       switch (P.kind) {
         case kSolveDense:
@@ -2102,7 +2059,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
           break;
         case kSolveGramCholesky:
           recordPhaseStart(s, 2, sk);
-          MB2_CUDA(launchGramCholesky(sliceGramCholesky(k), f->sched->dev, f->sched->gcParams.get(), gt, s->inKernelProfile, sk));
+          MB2_CUDA(launchGramCholesky(gc.slice(k, b0, count), f->sched->dev, f->sched->gcParams.get(), gt, s->inKernelProfile, sk));
           break;
         case kSolveQr: // the QR kernels read the Jacobian directly
           recordPhaseStart(s, 2, sk);
@@ -2127,8 +2084,7 @@ int mb2_solver_solve_device(mb2_solver* s, float* theta, void* cudaStream) {
         MB2_CUDA(launchLineSearchStep(la, st));
         s->kernelLaunches += 2;
       }
-      ba.iteration = it;
-      MB2_CUDA(launchBookkeeping(ba, st));
+      MB2_CUDA(launchBookkeeping(B, step.state, st));
       s->kernelLaunches += 1;
     }
     // Instances can only stop once iteration >= minIterations (solver.cpp:113): poll the device counter from then on (every

@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
     if (gt == 0) { errSlots[8] = DBL_MAX; errSlots[9] = DBL_MAX; flags[0] = 0; flags[1] = 0; flags[3] = 0; } // solver.cpp:83-84
     int iterations = 0;
     MB2_PH(kPhFetch)
-    for (int it = 0; it < a.maxIterations; ++it) {
+    for (int it = 0; it < a.state.maxIterations; ++it) {
       // ---- ParameterTransform::apply + zero background of the strips (ResizeableMatrix::resizeAndSetZero, solver_function.cpp:96) ----
       g.sync(); // theta (first iteration: the loads above; later: the update) is visible; the previous iteration is done with the tiles
       for (int row = gt; row < numJointParams; row += kFusedGroupThreads) jp[row] = jointParameterRow(T, row, th);
@@ -213,9 +213,8 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
       iterations = it + 1;
       if (gt == 0) {
         const double error = errSlots[8], last = errSlots[9];
-        if (a.history != nullptr) a.history[size_t(b) * a.maxIterations + it] = error;
-        const bool converged = fabs(last - error) / (fabs(error) + (double)FLT_MIN) <= (double)(a.threshold * FLT_EPSILON);
-        const bool stop = (it >= a.minIterations && converged) || it + 1 >= a.maxIterations;
+        if (a.state.history != nullptr) a.state.history[size_t(b) * a.state.maxIterations + it] = error;
+        const bool stop = solveStops(error, last, it, a.state.minIterations, a.state.maxIterations, a.state.threshold);
         if (!stop) errSlots[9] = error;
         flags[1] = stop ? 1 : 0;
       }
@@ -232,9 +231,9 @@ __global__ void __launch_bounds__(kFusedGroupThreads* kGroups, 1) fusedSolveKern
     if (!nonFinite)
       for (int i = gt; i < T.numParams; i += kFusedGroupThreads) thetaG[i] = th[i];
     if (gt == 0) {
-      a.errors[b] = errSlots[8];
-      a.iterations[b] = iterations;
-      a.status[b] = nonFinite ? 2 : (flags[0] != 0 ? 1 : 0);
+      a.state.errors[b] = errSlots[8];
+      a.state.iterations[b] = iterations;
+      a.state.status[b] = nonFinite ? 2 : (flags[0] != 0 ? 1 : 0);
     }
     MB2_PH(kPhFinish)
   }

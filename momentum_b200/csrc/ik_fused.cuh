@@ -33,16 +33,12 @@ struct FusedArgs {
   const int32_t* schedGlobal;  // = S.blob
   int32_t gramOff[8];          // makeGramBlob offsets
   int32_t numStrips, stripStride, residOff, numOrder; // GramPlan (numOrder: entries of the tile-order table)
-  float regularization, threshold;
-  int32_t minIterations, maxIterations;
+  float regularization;
   float* theta;                // [B][ldTheta] in/out
   int32_t ldTheta;
   const float* targets;        // [B][T.targetStride]
   const float* cweights;       // [numWeights] or [B][numWeights]
-  double* errors;              // [B] objective before the last update (what SolverT::solve returns)
-  int32_t* iterations;         // [B]
-  int32_t* status;             // [B] mb2_instance_status
-  double* history;             // optional [B][maxIterations]
+  SolveState state;            // errors (what SolverT::solve returns), iterations, status, history, options; the rest is in shared memory
   int32_t* workCounter;        // zeroed before the launch
   unsigned long long* phaseCycles; // optional [16]: per-phase cycles of the first group of CTA 0 (profiling instantiation)
   int32_t groups;              // instance groups per CTA (1..3)

@@ -1946,6 +1946,16 @@ cudaError_t launchJtJSimt(const JtJArgs& a, cudaStream_t stream) {
 // is factored in place with Eigen's LLT structure (ik_chol.cuh); the appended row turns into
 // y = L^-1 g for free; back substitution gives delta.
 // ------------------------------------------------------------------------------------------------
+// The SolverT bookkeeping of instance b after iteration s.iteration (solver.cpp:92-122), by one thread
+__device__ __forceinline__ void finishIteration(const SolveState& s, int b) {
+  const double error = s.errors[b], last = s.lastErrors[b];
+  if (s.history != nullptr) s.history[size_t(b) * s.maxIterations + s.iteration] = error;
+  const bool stop = solveStops(error, last, s.iteration, s.minIterations, s.maxIterations, s.threshold);
+  s.iterations[b] = s.iteration + 1;
+  if (stop) s.active[b] = 0;
+  else { s.lastErrors[b] = error; atomicAdd(s.activeCount, 1); }
+}
+
 // Common tail of both Cholesky kernels: delta, parameter update (skeleton_solver_function.cpp:153-159),
 // g.delta for the subset line search, status and the SolverT bookkeeping (solver.cpp:92-122).
 // dsub / gsub are indexed by subset position. Every thread of the CTA must call it.
@@ -1973,15 +1983,8 @@ __device__ void cholFinish(const CholArgs& a, int b, int n, const float* dsub, c
     }
   }
   if (tid == 0) {
-    if (failed && a.status[b] == 0) a.status[b] = 1; // MB2_INSTANCE_CHOLESKY_BREAKDOWN
-    if (a.bookkeeping) {
-      const double error = a.errors[b], last = a.lastErrors[b];
-      if (a.history != nullptr) a.history[size_t(b) * a.maxIterations + a.iteration] = error;
-      const bool converged = fabs(last - error) / (fabs(error) + (double)FLT_MIN) <= (double)(a.threshold * FLT_EPSILON);
-      a.iterations[b] = a.iteration + 1;
-      if ((a.iteration >= a.minIterations && converged) || a.iteration + 1 >= a.maxIterations) a.active[b] = 0;
-      else { a.lastErrors[b] = error; atomicAdd(a.activeCount, 1); }
-    }
+    if (failed && a.state.status[b] == 0) a.state.status[b] = 1; // MB2_INSTANCE_CHOLESKY_BREAKDOWN
+    if (a.bookkeeping) finishIteration(a.state, b);
   }
 }
 
@@ -1989,7 +1992,7 @@ template <int NB>
 __global__ void __launch_bounds__(kCholThreads) choleskyKernel(const CholArgs a, const int useSmemMatrix) {
   extern __shared__ float smem[];
   const int b = blockIdx.x;
-  if (a.active[b] == 0) return;
+  if (a.state.active[b] == 0) return;
   const int n = a.ns;
   const int tid = threadIdx.x;
   float* Hg = a.H + size_t(b) * a.hStride;
@@ -2173,7 +2176,7 @@ template <int kSchedThreads, bool kProfile>
 __global__ void __launch_bounds__(kSchedThreads, kSchedThreads == 256 ? 3 : 1) choleskyScheduledKernel(const __grid_constant__ CUtensorMap hmap, const CholArgs a, const CholSchedDev Sg) {
   extern __shared__ __align__(16) float smemRaw[];
   const int b = blockIdx.x;
-  if (a.active[b] == 0) return;
+  if (a.state.active[b] == 0) return;
   const int n = a.ns, tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31, hw = tid >> 4, hl = tid & 15;
   const unsigned hmask = 0xFFFFu << (16 * ((tid >> 4) & 1));
@@ -2349,7 +2352,7 @@ __global__ void __launch_bounds__(kGramThreads, kGramCholCtasPerSm) gramCholesky
   const GramArgs& g = a.g;
   const CholArgs& c = a.c;
   const int b = blockIdx.x;
-  if (c.active[b] == 0) return;
+  if (c.state.active[b] == 0) return;
   const int n = c.ns, tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31, hw = tid >> 4, hl = tid & 15;
   constexpr int kWarps = kGramThreads / 32;
@@ -2549,16 +2552,8 @@ cudaError_t launchTrialUpdate(int batch, const float* thetaOrig, int ldTheta, co
 __global__ void lineSearchStepKernel(const LineSearchArgs a) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= a.batch || a.searching[b] == 0) return;
-  const double error = a.errors[b], errorNew = a.trialErrors[b];
   const float scale = a.scale[b];
-  bool accept;
-  if (!a.subsetVariant) {
-    const float scaledError = 1e-3f * (float)error; // kC1 * error_ in T
-    accept = (error - errorNew) >= (double)(scale * scaledError);
-  } else {
-    accept = (error - errorNew) >= (double)(1e-4f * scale) * (double)a.gradDotDelta[b];
-  }
-  if (accept || a.step >= 9) a.searching[b] = 0;
+  if (lineSearchStops(a.errors[b], a.trialErrors[b], scale, a.subsetVariant, a.gradDotDelta + b, a.step)) a.searching[b] = 0;
   else a.scale[b] = scale * 0.5f;
 }
 cudaError_t launchLineSearchStep(const LineSearchArgs& a, cudaStream_t stream) {
@@ -2566,28 +2561,13 @@ cudaError_t launchLineSearchStep(const LineSearchArgs& a, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
-__global__ void commitTrialKernel(int batch, int numParams, int ldTheta, const float* thetaTrial, float* theta, const int32_t* active) {
-  const int b = blockIdx.x;
-  if (active[b] == 0) return;
-  for (int i = threadIdx.x; i < numParams; i += blockDim.x) theta[size_t(b) * ldTheta + i] = thetaTrial[size_t(b) * ldTheta + i];
-}
-cudaError_t launchCommitTrial(int batch, int numParams, int ldTheta, const float* thetaTrial, float* theta, const int32_t* active, cudaStream_t stream) {
-  commitTrialKernel<<<batch, 128, 0, stream>>>(batch, numParams, ldTheta, thetaTrial, theta, active);
-  return cudaGetLastError();
-}
-
-__global__ void bookkeepingKernel(const BookkeepingArgs a) {
+__global__ void bookkeepingKernel(int batch, const SolveState s) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= a.batch || a.active[b] == 0) return;
-  const double error = a.errors[b], last = a.lastErrors[b];
-  if (a.history != nullptr) a.history[size_t(b) * a.maxIterations + a.iteration] = error;
-  const bool converged = fabs(last - error) / (fabs(error) + (double)FLT_MIN) <= (double)(a.threshold * FLT_EPSILON);
-  a.iterations[b] = a.iteration + 1;
-  if ((a.iteration >= a.minIterations && converged) || a.iteration + 1 >= a.maxIterations) a.active[b] = 0;
-  else { a.lastErrors[b] = error; atomicAdd(a.activeCount, 1); }
+  if (b >= batch || s.active[b] == 0) return;
+  finishIteration(s, b);
 }
-cudaError_t launchBookkeeping(const BookkeepingArgs& a, cudaStream_t stream) {
-  bookkeepingKernel<<<(a.batch + 127) / 128, 128, 0, stream>>>(a);
+cudaError_t launchBookkeeping(int batch, const SolveState& s, cudaStream_t stream) {
+  bookkeepingKernel<<<(batch + 127) / 128, 128, 0, stream>>>(batch, s);
   return cudaGetLastError();
 }
 

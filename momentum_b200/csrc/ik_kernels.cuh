@@ -25,6 +25,20 @@ struct SweepArgs {           // K1 (FK + residual + Jacobian) and K4 (FK + error
   int32_t planBatch;         // instances launchSweep plans the variant for (0: batch): the whole batch when this launch is one slice of it
   int32_t stageTables;       // set by launchSweep: 1 every read-only table in shared memory, 2 all but cells / contributions, 0 none
   int32_t warpsPerInstance;  // set by launchSweep: 1, 2, 4 or 8 warps share one instance (large rigs: few instances fit in shared memory)
+  // the launch over instances b0 .. b0 + count - 1, with the variant planned for the whole batch
+  SweepArgs slice(int b0, int count) const {
+    SweepArgs a = *this;
+    a.batch = count;
+    a.planBatch = planBatch > 0 ? planBatch : batch;
+    a.theta += size_t(b0) * ldTheta;
+    a.targets += size_t(b0) * T.targetStride;
+    if (T.weightsPerInstance) a.cweights += size_t(b0) * T.numWeights;
+    if (jacobian != nullptr) a.jacobian += size_t(b0) * T.jacobianStride;
+    a.errors += b0;
+    if (active != nullptr) a.active += b0;
+    if (stateOut != nullptr) a.stateOut += size_t(b0) * T.numJoints * 8;
+    return a;
+  }
 };
 
 struct JtJArgs {             // K2
@@ -52,15 +66,7 @@ struct CholArgs {            // K3: damped Cholesky + solve + update + SolverT b
   int32_t ldTheta;
   float* delta;              // [B][ns] (always written)
   int32_t applyUpdate;       // 1: theta -= delta here
-  const double* errors;      // [B] error of this iteration (from K1)
-  double* lastErrors;        // [B]
-  int32_t* active;           // [B] in/out
-  int32_t* iterations;       // [B]
-  int32_t* status;           // [B]
-  double* history;           // optional [B][maxIterations]
-  int32_t iteration, minIterations, maxIterations;
-  float threshold;
-  int32_t* activeCount;      // device counter (atomicAdd of instances still active)
+  SolveState state;          // the error of this iteration (from K1) and the SolverT bookkeeping
   int32_t bookkeeping;       // 1: run the SolverT convergence test here (no line search)
   float* gradDotDelta;       // optional [B]: Jtr . delta (SubsetGaussNewtonSolverT line search)
   const float* g;            // scheduled kernel: [B][ldG] J^T r as a contiguous vector (ldG = ns rounded up to 4)
@@ -68,6 +74,19 @@ struct CholArgs {            // K3: damped Cholesky + solve + update + SolverT b
   const float* tilesIn;      // scheduled kernel, optional: [B][tilesStride] tiles + slot-ordered J^T r from the Gram kernel (H, g unused)
   size_t tilesStride;
   int32_t profile;           // MB2_CHOL_PROFILE=1: block 0 prints per-phase cycles (debug aid)
+  // the launch over instances b0 .. b0 + count - 1, which belong to instance slice k
+  CholArgs slice(int k, int b0, int count) const {
+    CholArgs a = *this;
+    a.batch = count;
+    if (H != nullptr) a.H += size_t(b0) * hStride;
+    a.theta += size_t(b0) * ldTheta;
+    a.delta += size_t(b0) * ns;
+    a.state = state.slice(k, b0);
+    if (gradDotDelta != nullptr) a.gradDotDelta += b0;
+    if (g != nullptr) a.g += size_t(b0) * ldG;
+    if (tilesIn != nullptr) a.tilesIn += size_t(b0) * tilesStride;
+    return a;
+  }
 };
 
 struct GramArgs {            // K2s: stored tiles of J^T J + lambda I and J^T r from the non-zero strips of the Jacobian (GramPlan)
@@ -85,6 +104,15 @@ struct GramArgs {            // K2s: stored tiles of J^T J + lambda I and J^T r 
   float regularization;
   float* out;                // [B][outStride]: numTiles x 256 floats in tile storage order, then the slot-ordered J^T r [nPad]
   size_t outStride;
+  // the launch over instances b0 .. b0 + count - 1
+  GramArgs slice(int b0, int count) const {
+    GramArgs a = *this;
+    a.batch = count;
+    a.strips += size_t(b0) * stripStride;
+    if (active != nullptr) a.active += b0;
+    if (out != nullptr) a.out += size_t(b0) * outStride;
+    return a;
+  }
 };
 // threads: SolvePath::gramThreads
 cudaError_t launchGramTiles(const GramArgs& a, int threads, cudaStream_t stream);
@@ -101,6 +129,8 @@ struct GramCholArgs {
   float* park;
   uint32_t* parkSlots;
   int32_t parkSlotWords, parkTiles;
+  // the launch over instances b0 .. b0 + count - 1, which belong to instance slice k
+  GramCholArgs slice(int k, int b0, int count) const { GramCholArgs a = *this; a.g = g.slice(b0, count); a.c = c.slice(k, b0, count); return a; }
 };
 // gramCholeskyKernel's flattened tables (GramCholTables): in the kernel's parameter block (read through the constant cache) when
 // they fit, else in global memory
@@ -377,7 +407,7 @@ DeviceLimits deviceLimits(); // of the device initKernelAttributes last read
 cudaError_t launchTrialUpdate(int batch, const float* thetaOrig, int ldTheta, const float* delta, int ns, const int32_t* cols, const float* scale /*[B]*/,
                               float* thetaTrial, const int32_t* active, cudaStream_t stream);
 struct LineSearchArgs {
-  int32_t batch, ns, numParams, ldTheta;
+  int32_t batch;
   const double* errors;      // error_ at theta (from the Jacobian pass)
   const double* trialErrors; // getError(theta - scale*delta)
   const float* gradDotDelta; // [B] (subset variant) or nullptr
@@ -385,17 +415,10 @@ struct LineSearchArgs {
   int32_t* searching;        // [B] 1 while the instance is still halving
   int32_t step;              // 0..9
   int32_t subsetVariant;
-  const int32_t* active;
 };
 cudaError_t launchLineSearchStep(const LineSearchArgs& a, cudaStream_t stream);
-cudaError_t launchCommitTrial(int batch, int numParams, int ldTheta, const float* thetaTrial, float* theta, const int32_t* active, cudaStream_t stream);
-struct BookkeepingArgs {
-  int32_t batch;
-  const double* errors; double* lastErrors; int32_t* active; int32_t* iterations; int32_t* status; double* history;
-  const float* theta; int32_t ldTheta, numParams;
-  int32_t iteration, minIterations, maxIterations; float threshold; int32_t* activeCount;
-};
-cudaError_t launchBookkeeping(const BookkeepingArgs& a, cudaStream_t stream);
+// the SolverT bookkeeping of s.iteration for the active instances of a batch (after a line search)
+cudaError_t launchBookkeeping(int batch, const SolveState& s, cudaStream_t stream);
 cudaError_t launchScatterTargets(const float* packed, float* dst, int size, int strideFloats, int batch, cudaStream_t stream);
 cudaError_t launchNormalizeQuats(float* base, int count, int strideFloats, int quatsPerRecord, int batch, cudaStream_t stream);
 

@@ -102,7 +102,7 @@ __global__ void __launch_bounds__(kQrThreads, 1) qrSolveKernel(const QrArgs a) {
   extern __shared__ __align__(16) float qrSmem[];
   const CholArgs& c = a.c;
   const int b = blockIdx.x;
-  if (c.active[b] == 0) return;
+  if (c.state.active[b] == 0) return;
   const int n = c.ns, tid = threadIdx.x, lane = tid & 31;
   float* R = qrSmem;                                  // packed upper triangle, row-major
   float* y = R + (size_t(n) * (n + 1) / 2 + 3 & ~size_t(3));

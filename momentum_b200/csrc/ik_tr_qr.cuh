@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(kQrThreads, 1) trustRegionQrKernel(const TrQrA
   extern __shared__ __align__(16) float trSmem[];
   const CholArgs& c = a.q.c;
   const int b = blockIdx.x;
-  if (c.active[b] == 0) return;
+  if (c.state.active[b] == 0) return;
   const FunctionTables& T = a.T;
   const int n = c.ns, tid = threadIdx.x, lane = tid & 31;
   const size_t packed = (size_t(n) * (n + 1) / 2 + 3) & ~size_t(3);
@@ -133,7 +133,7 @@ __global__ void __launch_bounds__(kQrThreads, 1) trustRegionQrKernel(const TrQrA
   float* Rsaved = a.rSaved + size_t(b) * packed; // Rmatrix_ (:119)
   for (size_t idx = tid; idx < size_t(n) * (n + 1) / 2; idx += kQrThreads) Rsaved[idx] = R[idx];
   __syncthreads();
-  const double error = c.errors[b];
+  const double error = c.state.errors[b];
   const float* targets = a.targets + size_t(b) * T.targetStride;
   const float* cw = a.cweights + (T.weightsPerInstance ? size_t(b) * T.numWeights : 0);
   float radius = a.radius[b], lambda = 1e-10f;

@@ -8,6 +8,8 @@
 // into it, joint_error_function-inl.h:229-294).
 #pragma once
 
+#include <cfloat>
+#include <cmath>
 #include <cstdint>
 
 #if defined(__CUDACC__)
@@ -128,6 +130,52 @@ struct FunctionTables : CharacterTables {
   int32_t stripMode, residOff;
   size_t jacobianStride;     // floats per instance in the Jacobian buffer
 };
+
+// The per-instance state of SolverT::solve (solver.cpp:50-128) on the device, and the options of its stopping rule. The arrays are
+// device memory: [B] for the whole batch, or from an instance slice's first instance on (slice).
+struct SolveState {
+  double* errors;        // [B] error of the iteration (written by the sweep)
+  double* lastErrors;    // [B] error of the previous iteration (solver.cpp:83-84: DBL_MAX before the first)
+  int32_t* active;       // [B] 1 while the instance iterates
+  int32_t* iterations;   // [B]
+  int32_t* status;       // [B] mb2_instance_status
+  double* history;       // optional [B][maxIterations]
+  int32_t* activeCount;  // the slice's counter: atomicAdd of the instances still active after the iteration
+  int32_t minIterations, maxIterations, iteration;
+  float threshold;
+
+  // the record of the instances from b0 on, which belong to slice k: the one place its pointers are offset
+  MB2_HD SolveState slice(int k, int b0) const {
+    SolveState s = *this;
+    s.errors += b0;
+    s.lastErrors += b0;
+    s.active += b0;
+    s.iterations += b0;
+    s.status += b0;
+    if (history != nullptr) s.history += size_t(b0) * maxIterations;
+    s.activeCount += k;
+    return s;
+  }
+};
+
+// SolverT::solve's stopping rule (solver.cpp:98-113) after `iteration`: converged (error against `last`) past minIterations, or the last one
+MB2_HD bool solveStops(double error, double last, int iteration, int minIterations, int maxIterations, float threshold) {
+  const bool converged = fabs(last - error) / (fabs(error) + (double)FLT_MIN) <= (double)(threshold * FLT_EPSILON);
+  return (iteration >= minIterations && converged) || iteration + 1 >= maxIterations;
+}
+
+// The line search (gauss_newton_solver.cpp:283-313; subsetVariant: subset_gauss_newton_solver.cpp:119-141, reads *gradDotDelta = J^T r . delta)
+// stops at step `step` (0..9), whose trial theta - scale delta has the error trialError, when the trial is accepted or at the tenth step
+MB2_HD bool lineSearchStops(double error, double trialError, float scale, bool subsetVariant, const float* gradDotDelta, int step) {
+  bool accept;
+  if (!subsetVariant) {
+    const float scaledError = 1e-3f * (float)error; // kC1 * error_ in T
+    accept = (error - trialError) >= (double)(scale * scaledError);
+  } else {
+    accept = (error - trialError) >= (double)(1e-4f * scale) * (double)*gradDotDelta;
+  }
+  return accept || step >= 9;
+}
 
 // What the skeleton-state backward walks besides CharacterTables (HostCharacter::buildBackwardTables)
 struct SkeletonTables {

@@ -532,17 +532,13 @@ int mb2_solver_solve(mb2_solver* s, float* params, double* errors, int32_t* iter
           for (int a = 0; a < ns; ++a) { const int c = f->plan.deviceCols[a]; if (c >= 0) theta[c] = orig[c] - scale * delta[a]; }
           double en;
           sweepOne<false>(f, T, b, theta, &en, nullptr);
-          bool accept;
-          if (!o.subset_line_search) accept = (error - en) >= (double)(scale * (1e-3f * (float)error));
-          else accept = (error - en) >= (double)(1e-4f * scale) * (double)gdd;
-          if (accept || step >= 9) break;
+          if (lineSearchStops(error, en, scale, o.subset_line_search != 0, &gdd, step)) break;
           scale *= 0.5f;
         }
       }
       s->history[size_t(b) * std::max(maxIt, 1) + it] = error;
       s->iterations[b] = it + 1;
-      const bool converged = std::fabs(last - error) / (std::fabs(error) + (double)FLT_MIN) <= (double)(o.threshold * FLT_EPSILON);
-      if (it >= minIt && converged) break;
+      if (solveStops(error, last, it, minIt, maxIt, o.threshold)) break;
       last = error;
     }
     bool bad = false;
@@ -565,7 +561,7 @@ int mb2_solver_get_counters(mb2_solver* s, uint64_t* totalIterations, uint64_t* 
   if (kernelLaunches) *kernelLaunches = 0;
   return MB2_OK;
 }
-int mb2_solver_get_solve_path(mb2_solver* s, int64_t out[15]) {
+int mb2_solver_get_solve_path(mb2_solver* s, int64_t out[kSolvePathWords]) {
   solvePathWords(s->path, out);
   return MB2_OK;
 }
